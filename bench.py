@@ -14,8 +14,11 @@ point: every timed step is an iteration the reference's loop would execute, neve
 
 Workload: N = 1 -> BASELINE.json configs[1] (BAL ladybug problem-1723-156502, float32); N > 1 -> configs[3] (BAL venice
 problem-1778-993923, float32, landmarks sharded over the N GPUs); --workload final-13682 = configs[4].  Synthetic
-stand-ins of the same shape (no BAL file exists on the box; SURVEY.md section 8d).  A line measured at N > 1 also
-carries the N = 1 time of the SAME workload (rank 0 alone, same run), because the driver's own N = 1 line is configs[1].
+stand-ins of the same shape (SURVEY.md section 8d).  A line measured at N > 1 also carries the N = 1 time of the SAME
+workload (rank 0 alone, same run), because the default N = 1 line is configs[1].
+
+--dump-outputs DIR writes what the timed device-resident run computed in its last step (cameras, landmarks, LM record)
+as DIR/<name>.npy, so that two builds can be compared output for output on identical, seeded inputs.
 """
 from __future__ import annotations
 
@@ -33,7 +36,7 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
-METRIC = "ms/LM-iter (linearize+QR+PCG) on BAL at 1/2/4/8 B200 vs CPU ref"
+METRIC = "ms/LM-iter (linearize+QR+PCG) on BAL at 1/2/4/8 H100 vs CPU ref"
 
 
 # ----------------------------------------------------------------------------------------------
@@ -233,7 +236,7 @@ class OracleBackend:
 
 # ----------------------------------------------------------------------------------------------
 class ClockSampler(threading.Thread):
-    """samples nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)"""
+    """samples nvidia-smi clocks / throttle reasons during the timed region"""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -289,7 +292,7 @@ def hbm_peak():
     try:
         return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
+        return 3350.0, "H100 SXM data sheet (HBM3)"
 
 
 def make_problem(args):
@@ -394,6 +397,43 @@ def trajectory_fields(st) -> dict:
             "final_cost": next((r.get("cost") for r in reversed(st.log) if r.get("cost") is not None and r.get("cost") == r.get("cost")), None)}
 
 
+DUMP_LIMIT_BYTES = 64 << 20
+LM_LOG_COLUMNS = ("lambda", "cost", "l_diff", "relative_decrease", "cg_iterations", "cg_termination", "accepted", "terminated")
+
+
+def gather_state(lin, world, dist):
+    """cameras and landmarks on the device, downloaded; with N > 1 every rank holds its own landmark shard, which are
+    summed into rank 0's copy (the other ranks' rows are zero)"""
+    lin.download_state()
+    cams, lms = lin.bal_problem.cams.copy(), lin.bal_problem.lms.copy()
+    if world > 1:
+        import torch
+        s = lin.stats()
+        mine = np.zeros_like(lms)
+        mine[s["landmark_begin"]:s["landmark_end"]] = lms[s["landmark_begin"]:s["landmark_end"]]
+        t = torch.from_numpy(mine).cuda()
+        dist.all_reduce(t)
+        lms = t.cpu().numpy()
+    return cams, lms
+
+
+def dump_outputs(out_dir, cams, lms, log, seed):
+    """What the timed path computed, as .npy in the solver's float type: the cameras and landmarks after the last timed
+    step and the per-step LM record.  Landmarks beyond the size limit are a fixed sample (seeded), with its row indices."""
+    os.makedirs(out_dir, exist_ok=True)
+    out = {"cameras": cams, "lm_log": np.array([[float(r[k]) for k in LM_LOG_COLUMNS] for r in log], dtype=np.float64).reshape(-1, len(LM_LOG_COLUMNS))}
+    room = DUMP_LIMIT_BYTES - sum(a.nbytes for a in out.values()) - 4096  # 4096: the .npy headers
+    row_bytes = lms.shape[1] * lms.itemsize + 8  # + the float64 row index when sampled
+    if lms.nbytes <= room:
+        out["landmarks"] = lms
+    else:
+        idx = np.sort(np.random.default_rng(seed).choice(lms.shape[0], room // row_bytes, replace=False))
+        out["landmarks"] = lms[idx]
+        out["landmarks_index"] = idx.astype(np.float64)
+    for name, a in out.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), a)
+
+
 def bench_reference(args):
     """the reference's algorithm (CPU restatement, oracle/) on the host cores; rank 0 only"""
     rank = int(os.environ.get("RANK", "0"))
@@ -485,10 +525,11 @@ def bench_ours(args):
     PH = ("stage1_time", "stage2_time", "compute_preconditioner_time", "solve_reduced_system_time",
           "back_substitution_time", "update_cameras_time", "residual_evaluation_time")
 
-    def timed_run(lin, sync=barrier):
+    def timed_run(lin, sync=barrier, on_last_step=None):
         """device-resident run: returns (device seconds for K steps, wall, log holder, phases, per-step device ms, launches).
         The LM loop runs natively (rba_lm_run: optimize_lm_ours in the library, one host synchronisation per iteration, no
-        interpreter between iterations); a solve that ends is followed by a new solve from the initial point."""
+        interpreter between iterations); a solve that ends is followed by a new solve from the initial point.
+        `on_last_step` is called once the last timed step is done, before that reset."""
         be = GpuBackend(lin)
         phase = {k: 0.0 for k in PH}
         step_ms, log = [], []
@@ -505,6 +546,8 @@ def bench_ours(args):
                     step_ms.extend(1e3 * i["device_seconds"] for i in its)
                     for k in PH:
                         phase[k] += tot[k]
+                    if left <= 0 and on_last_step:
+                        on_last_step()
                 if term or left > 0:
                     be.reset()  # a new solve from the initial point
 
@@ -530,7 +573,14 @@ def bench_ours(args):
     if rank == 0:
         sampler.start()
     lin = make_linearizor()
-    dev_s, wall_s, st, phase, step_ms, launches = timed_run(lin)
+    # --dump-outputs: the state after the last timed step is parked in the device backup (a device-to-device copy, no
+    # host synchronisation) before the reset to the initial point, and downloaded after the timed window
+    dev_s, wall_s, st, phase, step_ms, launches = timed_run(lin, on_last_step=lin._backup if args.dump_outputs else None)
+    if args.dump_outputs:
+        lin._restore()
+        cams, lms = gather_state(lin, world, dist)
+        if rank == 0:
+            dump_outputs(args.dump_outputs, cams, lms, st.log, args.seed)
     secs = torch.tensor([dev_s], dtype=torch.float64, device="cuda")
     if world > 1:
         dist.all_reduce(secs, op=dist.ReduceOp.MAX)
@@ -549,13 +599,6 @@ def bench_ours(args):
         dist.all_reduce(mv_t, op=dist.ReduceOp.MAX)
         dist.all_reduce(mv_bytes, op=dist.ReduceOp.SUM)
     peak, peak_src = hbm_peak()
-    traffic = None
-    try:  # DRAM bytes of the dominant kernel from the committed ncu --set full capture (same workload), per launch
-        tj = json.load(open(os.path.join(ROOT, "profiles", "r2_matvec_traffic.json")))
-        if args.workload == tj.get("workload") and args.scale == 1.0 and args.dtype == "f32" and world == 1 and args.operator == "dense":
-            traffic = tj["traffic_bytes_per_launch"]
-    except Exception:
-        pass
     achieved = float(mv_bytes.item()) / float(mv_t.item()) / 1e9 / world  # per GPU
     traj = trajectory_fields(st)
     lin.close()
@@ -605,7 +648,7 @@ def bench_ours(args):
     if rank == 0:
         cfg = workload_config(args, arrays)
         cfg.update(parallelism=f"landmark-shard x{world}",
-                   l2="inputs larger than L2 (Q2 panels %.0f MB per GPU vs 126 MB L2)" % (stats["panel_scalars"] * sz / 1e6))
+                   l2="inputs larger than L2 (Q2 panels %.0f MB per GPU vs 50 MB L2)" % (stats["panel_scalars"] * sz / 1e6))
         if args.operator == "implicit":
             cfg["solver"] += ", operator_form=IMPLICIT (opt-in)"
         out = {
@@ -617,7 +660,7 @@ def bench_ours(args):
             "clocks": {"sm_mhz": clocks.get("sm_mhz"), "sm_max_mhz": clocks.get("sm_max_mhz"), "reasons": clocks.get("reasons", [])},
             "roofline": {"bound": "hbm", "kernel": "rcs_matvec (k_matvec_implicit + camera reduction), bytes of the implicit form" if args.operator == "implicit"
                          else "rcs_matvec (k_matvec_small_tma + camera reduction)", "achieved": achieved, "peak": peak,
-                         "unit": "GB/s", "frac": achieved / peak, "traffic": traffic, "peak_source": peak_src,
+                         "unit": "GB/s", "frac": achieved / peak, "peak_source": peak_src,
                          "algorithmic_bytes_per_launch": float(mv_bytes.item()) / world, "us_per_launch": 1e6 * float(mv_t.item())},
             "cpu_baseline": cpu,
             "phases_ms_per_step": {k: 1e3 * v / args.steps for k, v in phase.items()},
@@ -653,7 +696,12 @@ def main():
     ap.add_argument("--cpu-budget-s", type=float, default=150.0, help="reference arm: wall-time budget of the timed steps")
     ap.add_argument("--operator", default="dense", choices=["dense", "implicit"],
                     help="PCG operator form: dense = the reference's Q2-panel product (default, contract kernel); implicit = opt-in")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the cameras, landmarks and LM record of the last timed step as DIR/<name>.npy "
+                         "(at most 64 MB; a seeded sample of the landmarks beyond that)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     if args.workload is None:
         args.workload = default_workload(args.gpus)
     if args.impl == "reference":

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Solve a BAL (or Bundler) problem with the square-root solver on one B200 and write the reference's ba_log.json.
+"""Solve a BAL (or Bundler) problem with the square-root solver on one H100 and write the reference's ba_log.json.
 
     python examples/solve_bal.py problem-49-7776-pre.txt [--float] [--max-num-iterations 20] [--operator-form DENSE|IMPLICIT]
 

@@ -1,5 +1,5 @@
 /*
- * rootba_b200.h -- C ABI of the B200-native square-root bundle-adjustment inner loop.
+ * rootba_b200.h -- C ABI of the H100-native square-root bundle-adjustment inner loop.
  *
  * This is the drop-in boundary for the ONE hot path of NikolausDemmel/rootba that this
  * repository accelerates: the QR (square-root) Levenberg-Marquardt inner loop.  The

@@ -28,7 +28,7 @@
 //   LLT), Sophus@d0b7315a (SO3::exp, SE3), basalt-headers@91293fa4
 //   (BalCamera::project).
 //
-// All "ref:" citations are relative to /root/reference/src/rootba/.
+// All "ref:" citations are relative to src/rootba/ of the reference (NikolausDemmel/rootba @ d3900037).
 // ===========================================================================
 #pragma once
 

@@ -1,4 +1,4 @@
-"""rootba_b200 -- B200-native square-root bundle-adjustment inner loop (drop-in for rootba's LinearizorQR path).
+"""rootba_b200 -- H100-native square-root bundle-adjustment inner loop (drop-in for rootba's LinearizorQR path).
 
 The compute path is the CUDA library rootba_b200/librootba_b200.so (C ABI: include/rootba_b200.h).
 Python here is only the host-side mirror of the reference interface and the synthetic-data generator.

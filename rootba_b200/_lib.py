@@ -94,7 +94,7 @@ def struct_to_dict(s: C.Structure) -> dict:
 
 
 def build(force: bool = False) -> str:
-    """Compile the CUDA extension in-tree for sm_100a (nvcc cross-compiles without a GPU)."""
+    """Compile the CUDA extension in-tree for sm_90a (nvcc cross-compiles without a GPU)."""
     src_dir = os.path.join(_HERE, "csrc")
     if force and os.path.exists(LIB_PATH):
         os.remove(LIB_PATH)

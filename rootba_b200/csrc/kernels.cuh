@@ -1,6 +1,6 @@
-// Hand-written sm_100a kernels of the square-root BA inner loop.  See DESIGN.md for the data layout,
+// Hand-written sm_90a kernels of the square-root BA inner loop.  See DESIGN.md for the data layout,
 // the algorithmic bytes of every kernel and the reference function each one replaces.
-// "ref:" citations are relative to /root/reference/src/rootba/.
+// "ref:" citations are relative to src/rootba/ of the reference (NikolausDemmel/rootba @ d3900037).
 #pragma once
 
 #include <cooperative_groups.h>
@@ -2237,8 +2237,10 @@ __device__ __forceinline__ void pcg_publish_progress(int* prog, int iter, int do
 }
 
 
+// One CTA per SM (the grid is one cluster): the minimum of 1 block lets ptxas use up to 128 registers, where its sm_90
+// default caps the kernel at 64 and spills the register-resident vectors.
 template <class S>
-__global__ void __launch_bounds__(VEC_THREADS) k_pcg_vec(DevPtrs<S> D, PcgState* st, S lambda, int i, int mode,
+__global__ void __launch_bounds__(VEC_THREADS, 1) k_pcg_vec(DevPtrs<S> D, PcgState* st, S lambda, int i, int mode,
                                                          double eta, int min_it, int is_last, int pdl, PeerComm pc, int seq,
                                                          const int* __restrict__ cam_item_ptr, int* prog) {
   __shared__ S sr[VEC_THREADS * VEC_EPT + 16];

@@ -1,6 +1,6 @@
-// Host orchestration + C ABI (include/rootba_b200.h) of the B200-native square-root BA inner loop.
+// Host orchestration + C ABI (include/rootba_b200.h) of the H100-native square-root BA inner loop.
 // One rba_handle = one landmark shard on one GPU; everything is enqueued on one CUDA stream.
-// "ref:" citations are relative to /root/reference/src/rootba/.
+// "ref:" citations are relative to src/rootba/ of the reference (NikolausDemmel/rootba @ d3900037).
 #include <cuda_runtime.h>
 #include <dlfcn.h>
 
@@ -84,7 +84,7 @@ struct Solver : rba_handle {
   Layout L;
   int nc = 0, nl_total = 0;
   int device = 0;
-  int sm_count = 148;
+  int sm_count = 132;
   cudaStream_t stream = nullptr;
   std::vector<void*> allocs;
   size_t device_bytes = 0;
@@ -454,7 +454,7 @@ struct Solver : rba_handle {
   static constexpr int K2_CAP = 3072;   // stage 2 needs 3 * W * CS + 9 * W * n + 20 W + 8 (<= 3048 for the standard tiles)
   Scratch<S> k1_sc{}, k2_sc{};
   size_t k1_smem = 0, k2_smem = 0;
-  int k1_bps = 2, k2_bps = 2, k1_max_blocks = 296, k2_max_blocks = 296;
+  int k1_bps = 2, k2_bps = 2, k1_max_blocks = 264, k2_max_blocks = 264;
   size_t k4_smem_small = 0, k4_smem_tma = 0;
   bool use_tma = true;
   int k4_tma_blocks_per_sm = 2;

@@ -1,9 +1,9 @@
 // Microbenchmark (diagnostic, not product): what read bandwidth can per-warp cp.async.bulk rings reach on this GPU, as a
 // function of stage size, ring depth and resident warps?  The dense PCG operator (k_matvec_small_tma) streams its panels
-// with exactly this structure and stays at 5.0 TB/s even with the arithmetic compiled out (DESIGN.md section 11.1);
-// this sweep separates "structure of the stream" from "everything else".
+// with exactly this structure (DESIGN.md section 11.1); this sweep separates "structure of the stream" from "everything
+// else".
 //
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -o tma_stream tma_stream.cu && ./tma_stream [GiB]
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -o tma_stream tma_stream.cu && ./tma_stream [GiB]
 //
 // Prints one line per configuration: GB/s read.  Baselines: grid-stride 16-byte loads, cudaMemcpy device-to-device.
 #include <cuda_runtime.h>

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""Per-kernel SASS instruction mnemonics of the built library (no GPU needed): evidence that the sm_100a code uses
+"""Per-kernel SASS instruction mnemonics of the built library (no GPU needed): evidence that the sm_90a code uses
 TMA bulk copies, mbarriers, cluster barriers and programmatic dependent launch.
-   python scripts/sass_mnemonics.py > profiles/r1_sass_mnemonics.txt"""
+   python scripts/sass_mnemonics.py"""
 import collections, os, re, subprocess, sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -9,7 +9,7 @@ lib = os.path.join(ROOT, "rootba_b200", "librootba_b200.so")
 sass = subprocess.run(["cuobjdump", "-sass", lib], capture_output=True, text=True, check=True).stdout
 names = subprocess.run(["c++filt"], input="\n".join(re.findall(r"Function : (\S+)", sass)), capture_output=True, text=True).stdout.split("\n")
 INTEREST = re.compile(r"^(UBLKCP|SYNCS|UCGABAR|ACQBULK|SHFL|[DF]FMA|LDG|STG|LDS|STS|ATOMG|REDG|REDUX|MEMBAR|ERRBAR|CCTL|BAR|HMMA|UTC|MUFU)")
-print("SASS evidence (cuobjdump -sass rootba_b200/librootba_b200.so, sm_100a) -- instruction mnemonics per kernel")
+print("SASS evidence (cuobjdump -sass rootba_b200/librootba_b200.so, sm_90a) -- instruction mnemonics per kernel")
 print("UBLKCP = cp.async.bulk (TMA 1-D bulk copy); SYNCS.* = mbarrier arrive.expect_tx / try_wait; UCGABAR_* = barrier.cluster;")
 print("ACQBULK = griddepcontrol.wait (programmatic dependent launch); SHFL = warp shuffles; no HMMA / UTC*MMA by design (DESIGN.md section 4).")
 print()

@@ -5,7 +5,7 @@ Tolerances (relative norm ||a-b||/(||a||+||b||), reference testing/eigen_utils.h
   SCHUR_JACOBI inverse blocks:      f32 1e-4 (explicit inverse of a 9x9 block: round-off x its condition number), f64 1e-8
   after a PCG solve (inc, l_diff):  f32 1e-4, f64 1e-8   (error growth through PCG; CG iteration count +-2)
   indices / counts:                 bit-exact
-Measured on B200 (profiles/r2_f32_trajectory_diag.txt): GPU-f32 vs oracle-f32 inc 3e-6 .. 1e-5, while BOTH are 2e-5 .. 4e-5 from the
+Measured on an H100 (scripts/diag_f32.py): GPU-f32 vs oracle-f32 inc 3e-6 .. 1e-5, while BOTH are 2e-5 .. 4e-5 from the
 float64 oracle (b 4e-5, H x 2e-4, inverse blocks 1e-4 .. 3e-4): the float32 linearisation itself is the noise floor.
 
 Order: the cheap single-solve checks of every option branch come first, the LM-trajectory tests last, so that one
@@ -429,7 +429,7 @@ def test_lm_trajectory(small_problem, dtype, kw):
     float64 pins the trajectory: same number of logged iterations, every accept/reject decision, cost at 1e-9, PCG
     iterations +-2.  In float32 the function-tolerance stop (|dcost| <= 1e-6 cost, bal_bundle_adjustment.cpp:174-201) sits
     at the round-off level of the cost itself -- the float32 ORACLE needs 5, 6 or 9 logged iterations on these problems where
-    the float64 oracle needs 6 (profiles/r2_f32_trajectory_diag.txt), and GPU-f32 / oracle-f32 / oracle-f64 costs agree to
+    the float64 oracle needs 6 (scripts/diag_f32.py), and GPU-f32 / oracle-f32 / oracle-f64 costs agree to
     1e-6 .. 3e-6 on every iteration they share.  So float32 compares what is above that noise: the cost of every shared
     iteration at 1e-5 (SURVEY 8c allows 1e-4), decisions and PCG counts while the step still lowers the cost by more than
     1e-5 relative, and the final cost at 1e-5; the number of noise-level iterations at the end is not compared."""
