@@ -2,6 +2,7 @@
 """Solve a BAL (or Bundler) problem with the square-root solver on one H100 and write the reference's ba_log.json.
 
     python examples/solve_bal.py problem-49-7776-pre.txt [--float] [--max-num-iterations 20] [--operator-form DENSE|IMPLICIT]
+        [--fix-intrinsics] [--fix-cameras I,J,...]
 
 Mirrors what `bal_qr --input ...` of the reference does (src/app/bal_qr.cpp): load + normalise (bal_problem.cpp:773-852),
 optimize_lm_ours with the QR linearizor (solver/bal_bundle_adjustment.cpp:249-544), log (bal/ba_log.hpp)."""
@@ -25,13 +26,28 @@ def main():
     ap.add_argument("--operator-form", default="DENSE", choices=["DENSE", "IMPLICIT"])
     ap.add_argument("--init-depth-threshold", type=float, default=0.0)
     ap.add_argument("--log-path", default="ba_log.json")
+    ap.add_argument("--fix-intrinsics", action="store_true", help="hold f, k1, k2 of every camera constant")
+    ap.add_argument("--fix-cameras", default="", metavar="I,J,...",
+                    help="hold every parameter of the listed cameras constant; indices refer to the loaded problem "
+                         "(a Bundler file's cameras with focal length 0 are dropped by the loader first)")
     args = ap.parse_args()
+    try:
+        fix_cameras = [int(v) for v in args.fix_cameras.split(",")] if args.fix_cameras else []
+    except ValueError:
+        ap.error(f"--fix-cameras expects a comma-separated list of camera indices, got {args.fix_cameras!r}")
 
     t0 = time.perf_counter()
     dtype = np.float32 if args.float else np.float64
     problem = rb.BalProblem.load_bal(args.input, dtype, normalize=True, init_depth_threshold=args.init_depth_threshold)
     t_load = time.perf_counter() - t0
     print(f"Loaded {problem.num_cameras()} cams, {problem.num_landmarks()} lms, {problem.num_observations()} obs in {t_load:.2f}s")
+    if args.fix_intrinsics or fix_cameras:
+        bad = [c for c in fix_cameras if not 0 <= c < problem.num_cameras()]
+        if bad:
+            ap.error(f"--fix-cameras: {bad} out of range (the loaded problem has {problem.num_cameras()} cameras)")
+        flags = np.full(problem.num_cameras(), rb.FIX_INTRINSICS if args.fix_intrinsics else 0, np.uint8)
+        flags[fix_cameras] = rb.FIX_ALL
+        problem.camera_fixed = flags
     options = rb.SolverOptions(max_num_iterations=args.max_num_iterations, preconditioner_type=args.preconditioner_type,
                                operator_form=args.operator_form, use_double=not args.float)
     summary = rb.bundle_adjust_manual(problem, options, verbose=True)

@@ -217,6 +217,29 @@ int32_t rba_get_state(rba_handle* h, void* cams, void* lms);
 int32_t rba_backup(rba_handle* h);
 int32_t rba_restore(rba_handle* h);
 
+/* ---- camera parameters held constant ---------------------------------------------------- */
+
+/* One byte of flags per camera.  Bit order follows the 9-entry increment of a camera
+ * (tx,ty,tz, rx,ry,rz, f, k1, k2).  The pose is one group: the increment is a left-multiplied SE(3)
+ * exponential, so a free rotation would move a "fixed" translation. */
+#define RBA_FIX_POSE 1u       /* increment entries 0..5; camera parameters qx,qy,qz,qw, tx,ty,tz */
+#define RBA_FIX_F 2u          /* entry 6; f  */
+#define RBA_FIX_K1 4u         /* entry 7; k1 */
+#define RBA_FIX_K2 8u         /* entry 8; k2 */
+#define RBA_FIX_INTRINSICS 14u
+#define RBA_FIX_ALL 15u
+
+/* Not in the reference (its fix_pose_gauge is unimplemented, bal/solver_options.hpp:106-108).
+ * flags [num_cameras of the full problem]: RBA_FIX_* bits per camera; NULL = every parameter free (the default).
+ * Every rank of a sharded problem passes the same array.  Takes effect at the next rba_solve; the device-resident
+ * increment of an earlier solve is discarded (rba_apply(h, NULL) then returns RBA_ERR_STATE until the next solve).
+ * A solve then gives the LM step with the flagged parameters held constant: their increment entries are exactly 0, the
+ * free entries solve H_ff x_f = -b_f (the reduced camera system restricted to the free rows and columns), and the flagged
+ * camera parameters stay bit-identical through rba_apply / rba_lm_step / rba_lm_run, also when rba_apply is given a host
+ * increment with non-zero entries there (they are zeroed before the back-substitution).  Landmarks are all free.
+ * A flag with a bit above 3 set -> RBA_ERR_INVALID_ARGUMENT, and the previous flags stay in force. */
+int32_t rba_set_camera_fixed(rba_handle* h, const uint8_t* flags);
+
 /* ---- Linearizor interface (solver/linearizor.hpp:56-82) ---------------------------------- */
 
 /* LinearizorBase::compute_error (linearizor_base.cpp:59-67) -> BalBundleAdjustmentHelper::compute_error
@@ -287,13 +310,15 @@ int32_t rba_get_timings(const rba_handle* h, rba_stage_timings* out);
 /* pose_jacobian_scaling_ (linearizor_qr.cpp:130-132) [9*Nc] and the squared column norms
  * LinearizationQR::get_stage1 returns (linearization_qr.hpp:634-712) */
 int32_t rba_get_jacobian_scaling(rba_handle* h, void* scaling_out, void* diag2_out);
-/* RHS b of the reduced camera system after the last rba_solve (get_stage2, linearization_qr.hpp:716-815) */
+/* RHS b of the reduced camera system after the last rba_solve (get_stage2, linearization_qr.hpp:716-815);
+ * the entries of parameters held by rba_set_camera_fixed are 0 */
 int32_t rba_get_rhs(rba_handle* h, void* b_out);
 /* explicit inverse of the block-Jacobi preconditioner (cg/preconditioner.hpp:79-120) [81*Nc] and the
- * blocks it was built from (damping already added) [81*Nc] */
+ * blocks it was built from (damping already added) [81*Nc].  For a camera with rba_set_camera_fixed flags the inverse is
+ * that of the free sub-block, embedded in the 9x9 slot with zero fixed rows and columns; the blocks are not masked. */
 int32_t rba_get_preconditioner(rba_handle* h, void* inv_out, void* blocks_out);
 /* LinearizationQR::right_multiply (linearization_qr.hpp:823-825): y = (Q2^T Jp)^T (Q2^T Jp) x + lambda x
- * with the damping of the last rba_solve */
+ * with the damping of the last rba_solve.  A debug accessor of the full operator: it ignores rba_set_camera_fixed. */
 int32_t rba_right_multiply(rba_handle* h, const void* x, void* y);
 /* LinearizationQR::back_substitute (linearization_qr.hpp:165-179) without the camera update */
 int32_t rba_back_substitute_f32(rba_handle* h, const float* pose_inc, float* l_diff_out);

@@ -18,6 +18,14 @@ HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "rootba_b200.h")
 RBA_OK = 0
 RBA_NUMERICAL_FAILURE = 1
 
+# camera parameters held constant, one byte of bits per camera (RBA_FIX_*, rba_set_camera_fixed)
+FIX_POSE = 1        # rotation and translation (increment entries 0..5)
+FIX_F = 2           # focal length (entry 6)
+FIX_K1 = 4          # entry 7
+FIX_K2 = 8          # entry 8
+FIX_INTRINSICS = FIX_F | FIX_K1 | FIX_K2
+FIX_ALL = FIX_POSE | FIX_INTRINSICS
+
 
 class RbaError(RuntimeError):
     def __init__(self, code: int, msg: str):

@@ -89,7 +89,13 @@ struct DevPtrs {
   S* partial;    // [max items][9]
   S* pblk;       // [csr_obs items][48] partial preconditioner blocks (45 used)
   int nc;
+  const uint8_t* cam_fixed;  // [nc] RBA_FIX_* bits per camera (rba_set_camera_fixed), nullptr = every parameter free
 };
+
+// increment entries (tx,ty,tz, rx,ry,rz, f,k1,k2) held by a camera's RBA_FIX_* bits, as a 9-bit mask
+__host__ __device__ __forceinline__ unsigned fixed_entry_mask(unsigned flags) {
+  return ((flags & 1u) ? 0x3fu : 0u) | ((flags & 14u) << 5);
+}
 
 // ------------------------------------------------------------------------------------------------
 // device math (same formulas and operation order as the oracle / reference)
@@ -1452,11 +1458,17 @@ __global__ void __launch_bounds__(128) k_panel_grad_blocks(DevPtrs<S> D, int wan
 
 // K3b  (blocks + lambda I) -> explicit inverse via Cholesky (ref: cg/preconditioner.hpp:79-120; pose damping
 //      linearization_qr.hpp:796-802 / linearizor_qr.cpp:228-232).  thread per camera.
+//      Camera with fixed parameters (cam_fixed): the fixed rows and columns of the damped block become the identity before
+//      the Cholesky and are zeroed in the inverse, and the fixed entries of b (final here) are zeroed.  The result is the
+//      inverse of the free sub-block: z = M^-1 r then has exactly zero fixed entries whatever r holds there, which keeps PCG
+//      and the power series on the restricted system (DESIGN.md, "Fixed camera parameters").
 template <class S>
 __global__ void __launch_bounds__(64) k_precond_invert(const S* __restrict__ src, S lambda, int nc,
-                                                        S* __restrict__ blocks_out, S* __restrict__ inv) {
+                                                        S* __restrict__ blocks_out, S* __restrict__ inv,
+                                                        const uint8_t* __restrict__ cam_fixed, S* __restrict__ b) {
   const int cam = blockIdx.x * blockDim.x + threadIdx.x;
   if (cam >= nc) return;
+  const unsigned fm = cam_fixed ? fixed_entry_mask(cam_fixed[cam]) : 0u;
   // everything is fully unrolled so that the 9x9 block lives in registers (no local-memory round trips)
   S A[9][9];
 #pragma unroll
@@ -1470,6 +1482,16 @@ __global__ void __launch_bounds__(64) k_precond_invert(const S* __restrict__ src
     for (int r = 0; r < 9; ++r)
 #pragma unroll
       for (int c = 0; c < 9; ++c) blocks_out[81 * (size_t)cam + 9 * r + c] = A[r][c];
+  if (fm) {
+#pragma unroll
+    for (int r = 0; r < 9; ++r)
+#pragma unroll
+      for (int c = 0; c < 9; ++c)
+        if (((fm >> r) | (fm >> c)) & 1u) A[r][c] = (r == c) ? S(1) : S(0);
+#pragma unroll
+    for (int d = 0; d < 9; ++d)
+      if ((fm >> d) & 1u) b[9 * (size_t)cam + d] = S(0);
+  }
   // in-place Cholesky of the upper-stored symmetric block: lower factor L in A[i][j], i >= j
   // (selfadjointView<Upper>().llt(), ref: cg/preconditioner.hpp:107-113)
 #pragma unroll
@@ -1502,6 +1524,13 @@ __global__ void __launch_bounds__(64) k_precond_invert(const S* __restrict__ src
       }
     }
   }
+  // A fixed entry d has an identity row and column in the block, so column d of Li is the unit vector e_d and row d of Li
+  // is zero off the diagonal.  Zeroing Li[d][d] therefore zeroes row and column d of the inverse exactly and leaves the free
+  // entries (the inverse of the free sub-block) unchanged.
+  if (fm)
+#pragma unroll
+    for (int d = 0; d < 9; ++d)
+      if ((fm >> d) & 1u) Li[d][d] = S(0);
   // inverse = Li^T Li
   S* out = inv + 81 * (size_t)cam;
 #pragma unroll
@@ -2675,11 +2704,27 @@ __global__ void k_camera_update(DevPtrs<S> D, const S* __restrict__ inc) {
 #pragma unroll
     for (int k = 0; k < 4; ++k) rq[k] *= sc;
   }
-  cm[0] = rq[0]; cm[1] = rq[1]; cm[2] = rq[2]; cm[3] = rq[3];
-  cm[4] = Re[0] * t0 + Re[1] * t1 + Re[2] * t2 + v[0];
-  cm[5] = Re[3] * t0 + Re[4] * t1 + Re[5] * t2 + v[1];
-  cm[6] = Re[6] * t0 + Re[7] * t1 + Re[8] * t2 + v[2];
-  cm[7] += v[6]; cm[8] += v[7]; cm[9] += v[8];
+  // fixed parameters are not written: the quaternion product with exp(0) renormalises when |q|^2 != 1 and could change
+  // the last bit, so a zero increment alone would not keep them constant
+  const unsigned f = D.cam_fixed ? D.cam_fixed[cam] : 0u;
+  if (!(f & 1u)) {
+    cm[0] = rq[0]; cm[1] = rq[1]; cm[2] = rq[2]; cm[3] = rq[3];
+    cm[4] = Re[0] * t0 + Re[1] * t1 + Re[2] * t2 + v[0];
+    cm[5] = Re[3] * t0 + Re[4] * t1 + Re[5] * t2 + v[1];
+    cm[6] = Re[6] * t0 + Re[7] * t1 + Re[8] * t2 + v[2];
+  }
+  if (!(f & 2u)) cm[7] += v[6];
+  if (!(f & 4u)) cm[8] += v[7];
+  if (!(f & 8u)) cm[9] += v[8];
+}
+
+// zero the increment entries of fixed camera parameters (a host increment given to rba_apply / rba_back_substitute), so that
+// the back-substitution and l_diff see the increment the cameras receive.  Thread per entry.
+template <class S>
+__global__ void k_mask_fixed_inc(S* __restrict__ inc, const uint8_t* __restrict__ cam_fixed, int nc) {
+  const int e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= 9 * nc) return;
+  if ((fixed_entry_mask(cam_fixed[e / 9]) >> (e % 9)) & 1u) inc[e] = S(0);
 }
 
 }  // namespace rba

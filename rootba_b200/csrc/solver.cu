@@ -48,6 +48,7 @@ struct rba_handle {
   virtual int get_state(void* cams, void* lms) = 0;
   virtual int backup() = 0;
   virtual int restore() = 0;
+  virtual int set_camera_fixed(const uint8_t* flags) = 0;
   virtual int compute_error(rba_residual_info* out) = 0;
   virtual int linearize() = 0;
   virtual int solve(double lambda, void* inc_out, rba_cg_summary* cg) = 0;
@@ -128,6 +129,8 @@ struct Solver : rba_handle {
   bool have_inc = false;
   S last_lambda = 0;
   bool damping_valid = false;
+  uint8_t* d_cam_fixed = nullptr;  // [nc] flags of rba_set_camera_fixed; D.cam_fixed points here while any flag is set
+  bool all_cams_fixed = false;     // no free camera parameter: the reduced system is empty and its solve is skipped
   rba_stage_timings tm{};
   EventPair ev_stage1, ev_stage2, ev_precond, ev_pcg, ev_backsub, ev_update, ev_error, ev_mv, ev_user;
   long long launches = 0;
@@ -563,6 +566,29 @@ struct Solver : rba_handle {
     CU(cudaMemcpyAsync(D.lms, lms_bk, (size_t)3 * L.nl_local * sizeof(S), cudaMemcpyDeviceToDevice, stream));
     return RBA_OK;
   }
+  // Held parameters restrict the reduced camera system to its free rows and columns; the masking happens once per solve
+  // in k_precond_invert (see there) and in the camera update.  No flag set = the unmodified path (D.cam_fixed == nullptr).
+  int set_camera_fixed(const uint8_t* flags) override {
+    bool any = false, all = flags != nullptr;
+    if (flags)
+      for (int c = 0; c < nc; ++c) {
+        if (flags[c] & ~RBA_FIX_ALL) {
+          g_err = "rba_set_camera_fixed: camera " + std::to_string(c) + " has flags " + std::to_string(flags[c]) + ", only bits 0..3 (RBA_FIX_ALL = 15) are defined";
+          return RBA_ERR_INVALID_ARGUMENT;
+        }
+        any = any || flags[c] != 0;
+        all = all && flags[c] == RBA_FIX_ALL;
+      }
+    if (any) {
+      if (!d_cam_fixed) { int rc = dalloc(&d_cam_fixed, (size_t)nc, false); if (rc) return rc; }
+      CU(cudaMemcpyAsync(d_cam_fixed, flags, (size_t)nc, cudaMemcpyHostToDevice, stream));
+      CU(cudaStreamSynchronize(stream));
+    }
+    D.cam_fixed = any ? d_cam_fixed : nullptr;
+    all_cams_fixed = all;
+    have_inc = false;  // the device-resident increment was solved under the previous flags
+    return RBA_OK;
+  }
 
   // launch with optional programmatic dependent launch (the kernel may start before its predecessor in the stream has
   // finished and orders itself with griddepcontrol.wait) and optional thread-block-cluster dimension
@@ -891,11 +917,27 @@ struct Solver : rba_handle {
     rc = stop(ev_stage2); if (rc) return rc;
     rc = start(ev_precond); if (rc) return rc;
     // pose damping lambda*I added to the blocks, then explicit inverse (ref: linearization_qr.hpp:796-802, linearizor_qr.cpp:228-237)
-    k_precond_invert<S><<<(nc + 63) / 64, 64, 0, stream>>>(schur ? D.blocks : D.jblocks, lambda, nc, schur ? D.blocks : nullptr, D.inv);
+    // (+ the masking of the held camera parameters, D.cam_fixed)
+    k_precond_invert<S><<<(nc + 63) / 64, 64, 0, stream>>>(schur ? D.blocks : D.jblocks, lambda, nc, schur ? D.blocks : nullptr, D.inv,
+                                                           D.cam_fixed, D.b);
     ++launches;
     rc = stop(ev_precond); if (rc) return rc;
     last_lambda = lambda;
     damping_valid = true;
+    if (all_cams_fixed) {
+      // no free camera parameter: inc = 0 without PCG / power series (whose stopping tests would divide 0 by 0); stage 2
+      // above still ran for the damped landmark factors of the back-substitution.  Every rank skips alike.
+      rc = start(ev_pcg); if (rc) return rc;
+      CU(cudaMemsetAsync(D.inc, 0, (size_t)9 * nc * sizeof(S), stream));
+      if (inc_out) CU(cudaMemcpyAsync(inc_out, D.inc, (size_t)9 * nc * sizeof(S), cudaMemcpyDeviceToHost, stream));
+      rc = stop(ev_pcg); if (rc) return rc;
+      // no copy into h_state is in flight: every entry point synchronises the stream before it returns
+      h_state[0] = PcgState{};
+      h_state[0].done = 1; h_state[0].term = 1; h_state[0].reason = 2;  // SUCCESS, |b_f| = 0, 0 iterations
+      have_inc = true;
+      new_linearization_point = false;
+      return RBA_OK;
+    }
     if (power) return power_enqueue(inc_out);
     // PCG (ref: cg/conjugate_gradient.hpp:113-298 ; linearizor_base.cpp:81-103)
     rc = start(ev_pcg); if (rc) return rc;
@@ -990,8 +1032,13 @@ struct Solver : rba_handle {
     if (!linearized || !damping_valid) { g_err = "rba_apply / rba_back_substitute need rba_linearize + rba_solve first"; return RBA_ERR_STATE; }
     apply_l0 = launches;
     ++state_version;
-    if (inc_host) CU(cudaMemcpyAsync(D.inc, inc_host, (size_t)9 * nc * sizeof(S), cudaMemcpyHostToDevice, stream));
-    else if (!have_inc) { g_err = "no device-resident increment"; return RBA_ERR_STATE; }
+    if (inc_host) {
+      CU(cudaMemcpyAsync(D.inc, inc_host, (size_t)9 * nc * sizeof(S), cudaMemcpyHostToDevice, stream));
+      if (D.cam_fixed) {  // the back-substitution must see the increment the cameras receive
+        k_mask_fixed_inc<S><<<(9 * nc + 255) / 256, 256, 0, stream>>>(D.inc, D.cam_fixed, nc);
+        ++launches;
+      }
+    } else if (!have_inc) { g_err = "no device-resident increment (none solved since rba_linearize or rba_set_camera_fixed)"; return RBA_ERR_STATE; }
     int rc = start(ev_backsub); if (rc) return rc;
     CU(cudaMemsetAsync(d_flags, 0, 4 * sizeof(int), stream));
     const int grid = std::min(tile_grid(sm_count * 4), EBLOCKS);
@@ -1443,6 +1490,7 @@ int32_t rba_set_state(rba_handle* h, const void* cams, const void* lms) { return
 int32_t rba_get_state(rba_handle* h, void* cams, void* lms) { return h->get_state(cams, lms); }
 int32_t rba_backup(rba_handle* h) { return h->backup(); }
 int32_t rba_restore(rba_handle* h) { return h->restore(); }
+int32_t rba_set_camera_fixed(rba_handle* h, const uint8_t* flags) { return h->set_camera_fixed(flags); }
 int32_t rba_compute_error(rba_handle* h, rba_residual_info* out) { return h->compute_error(out); }
 int32_t rba_linearize(rba_handle* h) { return h->linearize(); }
 

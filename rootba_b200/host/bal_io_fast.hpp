@@ -140,6 +140,7 @@ class BalProblemSoA {
   std::vector<int64_t> lm_off;    // [nl + 1]
   std::vector<int32_t> obs_cam;   // ascending inside a landmark
   std::vector<Scalar> obs_xy;     // [nobs][2]
+  std::vector<uint8_t> camera_fixed;  // [nc] RBA_FIX_* bits (rba_set_camera_fixed), forwarded by LinearizorQR::create; empty = all free
 
   int num_cameras() const { return nc; }
   int num_landmarks() const { return nl; }

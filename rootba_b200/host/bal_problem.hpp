@@ -220,6 +220,10 @@ class BalProblem {
     for (size_t i = 0; i < landmarks_.size(); ++i) std::copy(lms.begin() + 3 * i, lms.begin() + 3 * (i + 1), landmarks_[i].p_w.begin());
   }
 
+  // RBA_FIX_* bits per camera (rba_set_camera_fixed), forwarded by LinearizorQR::create; empty = every parameter free.
+  // Not in the reference.
+  std::vector<uint8_t> camera_fixed;
+
  private:
   static void fail(FILE* f, const std::string& path) { std::fclose(f); throw std::runtime_error("Failed to parse '" + path + "'"); }
   static Scalar median_destructive(std::vector<Scalar>& d) {  // bal_problem.cpp:116-122

@@ -2,6 +2,7 @@
 //   bal_qr --input <bal file> [--no-use-double] [--max-num-iterations N] [--preconditioner-type JACOBI|SCHUR_JACOBI]
 //          [--residual-robust-norm NONE|HUBER] [--residual-huber-parameter X] [--no-normalize] [--dump-problem out.bin]
 //          [--loader parallel|map] [--num-threads T] [--operator-form dense|implicit] [--init-depth-threshold Z]
+//          [--fix-intrinsics] [--fix-cameras I,J,...]
 //   --loader parallel (default): mmap + multi-threaded parse into flat arrays (bal_io_fast.hpp);
 //   --loader map: the reference-style fscanf + std::map loader (bal_problem.hpp).  Both give identical problems.
 #include <chrono>
@@ -18,26 +19,56 @@ static double seconds_since(std::chrono::steady_clock::time_point t0) {
   return std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
 }
 
+// camera parameters held constant (rba_set_camera_fixed): --fix-intrinsics, --fix-cameras I,J,...
+struct FixOptions {
+  bool intrinsics = false;
+  std::vector<long long> cameras;  // indices into the loaded problem
+};
+
+// "I,J,..." -> indices; false on an empty or malformed list
+static bool parse_camera_list(const std::string& v, std::vector<long long>& out) {
+  size_t pos = 0;
+  while (true) {
+    const size_t end = v.find(',', pos);
+    const std::string tok = v.substr(pos, end == std::string::npos ? std::string::npos : end - pos);
+    if (tok.empty() || tok.find_first_not_of("0123456789") != std::string::npos || tok.size() > 12) return false;
+    out.push_back(std::stoll(tok));
+    if (end == std::string::npos) return true;
+    pos = end + 1;
+  }
+}
+
 template <class S, class Problem>
-int solve_and_log(Problem& problem, const SolverOptions& o, const std::string& log_path, const std::string& input, double load_time);
+int solve_and_log(Problem& problem, const SolverOptions& o, const FixOptions& fix, const std::string& log_path, const std::string& input, double load_time);
 
 template <class S>
-int run(const std::string& input, bool normalize, const SolverOptions& o, const std::string& log_path, bool parallel_loader, int num_threads, double depth_thr) {
+int run(const std::string& input, bool normalize, const SolverOptions& o, const FixOptions& fix, const std::string& log_path, bool parallel_loader, int num_threads,
+        double depth_thr) {
   const auto t0 = std::chrono::steady_clock::now();
   if (parallel_loader) {
     auto problem = load_normalized_bal_problem_parallel<S>(input, normalize, 100.0, num_threads, depth_thr);
     std::printf("Loaded BAL problem (%d cams, %d lms, %lld obs) from '%s' in %.3fs (parallel loader)\n", problem.num_cameras(),
                 problem.num_landmarks(), (long long)problem.num_observations(), input.c_str(), seconds_since(t0));
-    return solve_and_log<S>(problem, o, log_path, input, seconds_since(t0));
+    return solve_and_log<S>(problem, o, fix, log_path, input, seconds_since(t0));
   }
   auto problem = load_normalized_bal_problem<S>(input, normalize, 100.0, depth_thr);
   std::printf("Loaded BAL problem (%d cams, %d lms, %lld obs) from '%s' in %.3fs (map loader)\n", problem.num_cameras(),
               problem.num_landmarks(), (long long)problem.num_observations(), input.c_str(), seconds_since(t0));
-  return solve_and_log<S>(problem, o, log_path, input, seconds_since(t0));
+  return solve_and_log<S>(problem, o, fix, log_path, input, seconds_since(t0));
 }
 
 template <class S, class Problem>
-int solve_and_log(Problem& problem, const SolverOptions& o, const std::string& log_path, const std::string& input, double load_time) {
+int solve_and_log(Problem& problem, const SolverOptions& o, const FixOptions& fix, const std::string& log_path, const std::string& input, double load_time) {
+  if (fix.intrinsics || !fix.cameras.empty()) {
+    problem.camera_fixed.assign((size_t)problem.num_cameras(), fix.intrinsics ? (uint8_t)RBA_FIX_INTRINSICS : (uint8_t)0);
+    for (long long c : fix.cameras) {
+      if (c >= problem.num_cameras()) {
+        std::cerr << "--fix-cameras: camera " << c << " out of range (the loaded problem has " << problem.num_cameras() << " cameras)\n";
+        return 2;
+      }
+      problem.camera_fixed[(size_t)c] = (uint8_t)RBA_FIX_ALL;
+    }
+  }
   const DatasetSummary ds = summarize_problem<S>(problem, input);
   SolverSummary summary;
   bundle_adjust_manual<S>(problem, o, &summary);
@@ -91,6 +122,7 @@ int main(int argc, char** argv) {
   int num_threads = 0;
   double depth_thr = 0.0;  // BalDatasetOptions::init_depth_threshold (bal_dataset_options.hpp:82)
   SolverOptions o;
+  FixOptions fix;
   for (int i = 1; i < argc; ++i) {
     const std::string a = argv[i];
     auto next = [&]() -> std::string { if (i + 1 >= argc) { std::cerr << "missing value for " << a << "\n"; std::exit(2); } return argv[++i]; };
@@ -114,8 +146,19 @@ int main(int argc, char** argv) {
     else if (a == "--num-threads") num_threads = std::stoi(next());
     else if (a == "--init-depth-threshold") depth_thr = std::stod(next());
     else if (a == "--dump-problem") dump = next();
+    else if (a == "--fix-intrinsics") fix.intrinsics = true;
+    else if (a == "--fix-cameras") {
+      const std::string v = next();
+      if (!parse_camera_list(v, fix.cameras)) { std::cerr << "--fix-cameras expects a comma-separated list of camera indices, got '" << v << "'\n"; return 2; }
+    }
     else if (a == "--selftest-log") return selftest_log(next());
-    else if (a == "--help" || a == "-h") { std::cout << "usage: bal_qr --input <bal file> [--no-use-double] [--max-num-iterations N] [--preconditioner-type JACOBI|SCHUR_JACOBI] ...\n"; return 0; }
+    else if (a == "--help" || a == "-h") {
+      std::cout << "usage: bal_qr --input <bal file> [--no-use-double] [--max-num-iterations N] [--preconditioner-type JACOBI|SCHUR_JACOBI] ...\n"
+                   "  --fix-intrinsics      hold f, k1, k2 of every camera constant\n"
+                   "  --fix-cameras I,J,... hold every parameter of the listed cameras constant; indices refer to the loaded problem\n"
+                   "                        (a Bundler file's cameras with focal length 0 are dropped by the loader first)\n";
+      return 0;
+    }
     else { std::cerr << "unknown option " << a << "\n"; return 2; }
   }
   if (input.empty()) { std::cerr << "--input is required\n"; return 2; }
@@ -141,7 +184,8 @@ int main(int argc, char** argv) {
       return 0;
     }
     o.use_double = use_double;
-    return use_double ? run<double>(input, normalize, o, log_path, parallel_loader, num_threads, depth_thr) : run<float>(input, normalize, o, log_path, parallel_loader, num_threads, depth_thr);
+    return use_double ? run<double>(input, normalize, o, fix, log_path, parallel_loader, num_threads, depth_thr)
+                      : run<float>(input, normalize, o, fix, log_path, parallel_loader, num_threads, depth_thr);
   } catch (const std::exception& e) {
     std::cerr << "FATAL: " << e.what() << "\n";
     return 1;

@@ -174,6 +174,10 @@ class LinearizorQR {
     std::vector<Scalar> c, l;
     bp.export_state(c, l);
     check(rba_set_state(h_, c.data(), l.data()));
+    if (!bp.camera_fixed.empty()) {
+      if ((int)bp.camera_fixed.size() != bp.num_cameras()) throw std::runtime_error("camera_fixed must have one entry per camera");
+      check(rba_set_camera_fixed(h_, bp.camera_fixed.data()));
+    }
   }
   Problem& bal_problem_;
   SolverSummary* summary_ = nullptr;

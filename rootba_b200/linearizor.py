@@ -20,7 +20,7 @@ import time
 import numpy as np
 
 from . import _lib
-from ._lib import (CgSummary, LmIteration, LmOpts, LmStepResult, ProblemView, RbaError, ResidualInfo, SolverOpts, StageTimings, WorkloadStats,
+from ._lib import (FIX_ALL, CgSummary, LmIteration, LmOpts, LmStepResult, ProblemView, RbaError, ResidualInfo, SolverOpts, StageTimings, WorkloadStats,
                    check, struct_to_dict)
 
 
@@ -65,9 +65,22 @@ class SolverOptions:  # bal/solver_options.hpp (QR-relevant subset, reference de
         return self.optimized_cost != "ERROR"
 
 
+def _camera_fixed_array(flags, num_cameras: int):
+    """None, or a validated uint8 copy of one FIX_* bit set per camera"""
+    if flags is None:
+        return None
+    a = np.asarray(flags)
+    if a.shape != (num_cameras,):
+        raise ValueError(f"camera_fixed must have one entry per camera ({num_cameras}), got shape {a.shape}")
+    if a.dtype.kind not in "iu" or np.any(a < 0) or np.any(a > FIX_ALL):
+        raise ValueError(f"camera_fixed entries must be integers combining FIX_* bits (0..{FIX_ALL})")
+    return np.ascontiguousarray(a, dtype=np.uint8).copy()
+
+
 class BalProblem:
     """SoA BalProblem: cameras [nc,10] (quat xyzw, t, f,k1,k2), landmarks [nl,3], observations in
-    CSR-by-landmark order with ascending camera index."""
+    CSR-by-landmark order with ascending camera index.  `camera_fixed` (not in the reference): None or one uint8 of FIX_*
+    bits per camera, held constant by the solver; forwarded to an attached LinearizorQR on assignment."""
 
     def __init__(self, cams, lms, lm_off, obs_cam, obs_xy, dtype=np.float64):
         self.dtype = np.dtype(dtype)
@@ -80,6 +93,17 @@ class BalProblem:
         self._cams_backup = self.cams.copy()
         self._lms_backup = self.lms.copy()
         self._linearizor = None
+        self._camera_fixed = None
+
+    @property
+    def camera_fixed(self):
+        return self._camera_fixed
+
+    @camera_fixed.setter
+    def camera_fixed(self, flags):
+        self._camera_fixed = _camera_fixed_array(flags, self.num_cameras())
+        if self._linearizor is not None:
+            self._linearizor._upload_camera_fixed()
 
     @classmethod
     def from_arrays(cls, arrays, dtype=np.float64) -> "BalProblem":
@@ -180,6 +204,8 @@ class LinearizorQR:
         self.upload_state()
         bal_problem._linearizor = self
         self.last_cg = CgSummary()
+        if bal_problem.camera_fixed is not None:
+            self._upload_camera_fixed()
 
     # factory like Linearizor::create (linearizor.cpp:47-65)
     @staticmethod
@@ -205,6 +231,15 @@ class LinearizorQR:
 
     def download_state(self):
         check(_lib.lib().rba_get_state(self.h, _p(self.bal_problem.cams), _p(self.bal_problem.lms)))
+
+    def set_camera_fixed(self, flags):
+        """hold camera parameters constant (rba_set_camera_fixed): None, or one uint8 of FIX_* bits per camera.  Takes effect
+        at the next solve; the flags are stored on the BalProblem."""
+        self.bal_problem.camera_fixed = flags  # validates and forwards to _upload_camera_fixed
+
+    def _upload_camera_fixed(self):
+        f = self.bal_problem.camera_fixed
+        check(_lib.lib().rba_set_camera_fixed(self.h, None if f is None else _p(f)))
 
     def _backup(self):
         check(_lib.lib().rba_backup(self.h))
