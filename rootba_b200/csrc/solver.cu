@@ -816,13 +816,17 @@ struct Solver : rba_handle {
     return launch_ex(k_pcg_vec<S>, pcg_cluster, VEC_THREADS, 0, pdl && use_pdl, pcg_cluster, D, d_state, lambda, i, mode, (double)opt.eta,
                      (int)opt.min_linear_solver_iterations, is_last, (int)(pdl && use_pdl), c, ar_seq, from_partials ? op_item_ptr : (const int*)nullptr, d_prog);
   }
+  // The hand-over through per-segment sums is taken when a cluster CTA's share of the cameras fits the vector kernel's
+  // register-resident layout (9 ceil(nc / cluster) <= VEC_THREADS VEC_EPT: <= 1808 cameras with a 16-CTA cluster, <= 904
+  // with 8); larger camera counts on one GPU (Final-13682) keep the arrival-counter reduction into D.y, the combination that
+  // was measured at that size.
+  bool pcg_from_partials() const {
+    const bool vec_cached = 9 * ((nc + pcg_cluster - 1) / pcg_cluster) <= VEC_THREADS * VEC_EPT;
+    return opt.nranks == 1 && pcg_partials && vec_cached;
+  }
   // finish one operator application inside PCG (H v for v = p in mode 0/1, x in mode 2) and do the vector step
   int pcg_apply(int i, int mode, int is_last, S lambda) {
-    // The hand-over through per-segment sums is taken when a cluster CTA's share of the cameras fits the vector kernel's
-    // register-resident layout (<= 1820 cameras with a 16-CTA cluster); larger camera counts on one GPU (Final-13682)
-    // keep the arrival-counter reduction below, the combination that was measured at that size.
-    const bool vec_cached = 9 * ((nc + pcg_cluster - 1) / pcg_cluster) <= VEC_THREADS * VEC_EPT;
-    if (opt.nranks == 1 && pcg_partials && vec_cached) {
+    if (pcg_from_partials()) {
       // one GPU: the vector kernel adds the per-segment sums itself (same order as k_cam_reduce_final's last arriver:
       // bit-identical) -- no arrival counters, fences or second pass in the reduction
       int rc = launch_ex(k_cam_reduce<S>, grid_for(n_op_items, 8, 8), 256, 0, use_pdl, 1, (const S*)D.yobs, op_slots, op_items, n_op_items, D.partial,
@@ -938,6 +942,11 @@ struct Solver : rba_handle {
       new_linearization_point = false;
       return RBA_OK;
     }
+    // k_cam_reduce_final writes D.y only for cameras with observations, and an earlier call may have left other values in
+    // the remaining entries (rba_right_multiply stores lambda x there for every camera).  The one-GPU consumers that read
+    // D.y (k_power_vec, and k_pcg_vec without the per-segment hand-over) need the operator's 0 for a camera without
+    // observations: cleared once per solve, outside the iteration.
+    if (opt.nranks == 1 && (power || !pcg_from_partials())) CU(cudaMemsetAsync(D.y, 0, (size_t)9 * nc * sizeof(S), stream));
     if (power) return power_enqueue(inc_out);
     // PCG (ref: cg/conjugate_gradient.hpp:113-298 ; linearizor_base.cpp:81-103)
     rc = start(ev_pcg); if (rc) return rc;

@@ -173,12 +173,23 @@ def _sample_tracks(rng: np.random.Generator, nc: int, n: np.ndarray) -> np.ndarr
 
 
 def synth_bal(nc: int, nl: int, mean_n: float, seed: int = 38401, *, max_track: int = 400, max_tan: float = 1.0,
-              locality: float = 0.0,
+              locality: float = 0.0, track_lengths=None, lm_spread: float = 3.0,
               obs_noise: float = 0.5, perturb_lm: float = 0.05, perturb_rot: float = 0.002,
               perturb_trans: float = 0.01, normalize_scale: float | None = 100.0) -> BalArrays:
     """Generate a synthetic BAL problem (already in the loaded convention), optionally normalised
     like the reference's default pipeline (bal/bal_problem.cpp:428-469, scale 100) and with a
-    perturbed initial state so that LM has real work to do."""
+    perturbed initial state so that LM has real work to do.
+
+    `track_lengths` (one entry per landmark, each in [2, nc]) replaces the geometric draw of the track lengths: landmark l
+    gets exactly track_lengths[l] observations (`nl` must equal its length, `mean_n` and `max_track` are not used).  Pair it
+    with a small `lm_spread` (standard deviation of the landmark positions; the cameras stand at distance ~10) so that every
+    landmark lies inside every camera's field of view and no observation is filtered; a filtered one raises ValueError."""
+    if track_lengths is not None:
+        want = np.asarray(track_lengths, dtype=np.int64).ravel()
+        if want.shape[0] != nl:
+            raise ValueError(f"track_lengths has {want.shape[0]} entries for nl = {nl} landmarks")
+        if want.size and (want.min() < 2 or want.max() > nc):
+            raise ValueError(f"track lengths must lie in [2, nc = {nc}]")
     rng = np.random.default_rng(seed)
     # cameras on a ring of radius 10 looking at the origin
     ang = rng.uniform(0.0, 2 * np.pi, nc)
@@ -201,10 +212,13 @@ def synth_bal(nc: int, nl: int, mean_n: float, seed: int = 38401, *, max_track: 
     cams[:, 8] = rng.normal(0, 1e-7, nc)
     cams[:, 9] = rng.normal(0, 1e-13, nc)
     # landmarks and track lengths
-    lms = rng.normal(0, 3.0, (nl, 3))
-    p = 1.0 / (mean_n - 1.0)
-    n = 2 + (rng.geometric(p, nl) - 1)
-    n = np.minimum(n, min(nc, max_track)).astype(np.int64)
+    lms = rng.normal(0, lm_spread, (nl, 3))
+    if track_lengths is None:
+        p = 1.0 / (mean_n - 1.0)
+        n = 2 + (rng.geometric(p, nl) - 1)
+        n = np.minimum(n, min(nc, max_track)).astype(np.int64)
+    else:
+        n = want
     obs_cam = _sample_tracks_local(rng, nc, n, locality) if locality > 0 else _sample_tracks(rng, nc, n)
     lm_of_obs = np.repeat(np.arange(nl), n)
     xy, z, tan = project(cams[obs_cam], lms[lm_of_obs], return_tan=True)
@@ -222,6 +236,9 @@ def synth_bal(nc: int, nl: int, mean_n: float, seed: int = 38401, *, max_track: 
     counts = np.bincount(lm_of_obs, minlength=nl2)
     lm_off = np.concatenate([[0], np.cumsum(counts)]).astype(np.int64)
     prob = BalArrays(cams, lms, lm_off, obs_cam.astype(np.int32), xy)
+    if track_lengths is not None and not np.array_equal(prob.track_lengths(), want):
+        raise ValueError(f"{int(want.sum()) - prob.nobs} observations fell outside the field of view or behind a camera; "
+                         "use a smaller lm_spread")
     if normalize_scale:
         normalize(prob, normalize_scale)
     # perturb the initial state (relative to the normalised scale)

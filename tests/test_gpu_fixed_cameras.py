@@ -27,10 +27,10 @@ def fixed_params(flags):
     return out
 
 
-def _dense_case():
+def _dense_case(nc=7, nl=90):
     from rootba_b200.synthetic import synth_bal
     from test_oracle_dense_numpy import _dense_system, _reduced
-    prob = synth_bal(7, 90, 3.6, seed=21)
+    prob = synth_bal(nc, nl, 3.6, seed=21)
     Jp, Jl, r = _dense_system(prob)
     lam = 1e-3
     return prob, lam, r, _reduced(Jp, Jl, r, lam, prob.nl, float(np.sqrt(1e-10)))
@@ -42,15 +42,30 @@ CONFIGS += [dict(solver_type="SCHUR_COMPLEMENT"), dict(solver_type="POWER_SCHUR_
 
 
 @pytest.mark.parametrize("cfg", CONFIGS, ids=lambda c: "-".join(str(v) for v in c.values()))
-def test_f64_against_restricted_dense_system(cfg):
+def test_f64_against_restricted_dense_system(cfg, monkeypatch):
+    _check_restricted(cfg, 7, 90, {}, monkeypatch)
+
+
+@pytest.mark.parametrize("cfg", CONFIGS, ids=lambda c: "-".join(str(v) for v in c.values()))
+def test_f64_uncached_vector_step_against_restricted_dense_system(cfg, monkeypatch):
+    """120 cameras with a one-CTA PCG vector kernel (RBA_PCG_CLUSTER=1): from 114 cameras on, its share of the vectors is no
+    longer register-resident and it reads the camera-reduced operator output (DESIGN.md section 13)"""
+    _check_restricted(cfg, 120, 500, {"RBA_PCG_CLUSTER": "1"}, monkeypatch)
+
+
+def _check_restricted(cfg, nc, nl, env, monkeypatch):
     import rootba_b200 as rb
-    prob, lam, r, (D, sl, Jps, Jls, Minv, H, b) = _dense_case()
-    fixed = fixed_entries(MASK)
+    prob, lam, r, (D, sl, Jps, Jls, Minv, H, b) = _dense_case(nc, nl)
+    mask = np.resize(MASK, nc)
+    fixed = fixed_entries(mask)
     free = ~fixed
     bp = rb.BalProblem.from_arrays(prob, np.float64)
-    bp.camera_fixed = MASK
+    bp.camera_fixed = mask
     so = rb.SolverOptions(eta=1e-13, **cfg)
-    lin = rb.LinearizorQR.create(bp, so)
+    with monkeypatch.context() as m:
+        for k, v in env.items():
+            m.setenv(k, v)
+        lin = rb.LinearizorQR.create(bp, so)
     cams0 = bp.cams.copy()
     lin.compute_error()
     lin.linearize()
@@ -80,7 +95,7 @@ def test_f64_against_restricted_dense_system(cfg):
     assert abs(l_diff - want_l) <= 1e-8 * abs(want_l)
     lin.download_state()
     assert rel_err(bp.lms, prob.lms + (sl * dl_s).reshape(-1, 3)) < 1e-10
-    fp = fixed_params(MASK)
+    fp = fixed_params(mask)
     assert np.array_equal(bp.cams[fp], cams0[fp])
     assert not np.array_equal(bp.cams[~fp], cams0[~fp])
     lin.close()

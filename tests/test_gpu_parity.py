@@ -234,34 +234,6 @@ def test_implicit_operator_form(small_problem, mixed_problem, dtype, which):
     lin.close()
 
 
-def test_long_tracks_generic_path():
-    """track lengths beyond the register-resident classes (KP > 16) take the shared-memory matvec variant"""
-    from rootba_b200.synthetic import synth_bal
-    arrays = synth_bal(300, 120, 60.0, seed=4, max_track=300)
-    assert arrays.track_lengths().max() > 113
-    for dtype, hh in ((np.float32, True), (np.float64, True), (np.float64, False)):
-        bp, lin, o, _ = make_pair(arrays, dtype, use_householder_marginalization=hh)
-        lin.linearize(); assert o.linearize()
-        inc_g = lin.solve(0.01)
-        inc_c, _ = o.solve(0.01)
-        x = np.random.default_rng(0).uniform(-1, 1, 9 * lin.nc).astype(dtype)
-        assert rel_err(lin.right_multiply(x), o.right_multiply(x)) < TOL1[dtype] * 4
-        assert rel_err(inc_g, inc_c) < TOLS[dtype]
-        lin.close()
-
-
-def test_minimal_tracks_and_ragged_tiles():
-    """n = 2 only, landmark count not a multiple of the tile width"""
-    from rootba_b200.synthetic import synth_bal
-    arrays = synth_bal(9, 77, 2.0001, seed=2)
-    assert arrays.track_lengths().max() <= 3
-    bp, lin, o, _ = make_pair(arrays, np.float64)
-    lin.linearize(); assert o.linearize()
-    inc_g = lin.solve(1e-3); inc_c, _ = o.solve(1e-3)
-    assert rel_err(inc_g, inc_c) < 1e-8
-    lin.close()
-
-
 def test_rejects_bad_input(small_problem):
     import rootba_b200 as rb
     a = small_problem
