@@ -175,7 +175,8 @@ def _sample_tracks(rng: np.random.Generator, nc: int, n: np.ndarray) -> np.ndarr
 def synth_bal(nc: int, nl: int, mean_n: float, seed: int = 38401, *, max_track: int = 400, max_tan: float = 1.0,
               locality: float = 0.0, track_lengths=None, lm_spread: float = 3.0,
               obs_noise: float = 0.5, perturb_lm: float = 0.05, perturb_rot: float = 0.002,
-              perturb_trans: float = 0.01, normalize_scale: float | None = 100.0) -> BalArrays:
+              perturb_trans: float = 0.01, normalize_scale: float | None = 100.0, k1_sigma: float = 1e-7,
+              k2_sigma: float = 1e-13, tracks=None) -> BalArrays:
     """Generate a synthetic BAL problem (already in the loaded convention), optionally normalised
     like the reference's default pipeline (bal/bal_problem.cpp:428-469, scale 100) and with a
     perturbed initial state so that LM has real work to do.
@@ -183,7 +184,17 @@ def synth_bal(nc: int, nl: int, mean_n: float, seed: int = 38401, *, max_track: 
     `track_lengths` (one entry per landmark, each in [2, nc]) replaces the geometric draw of the track lengths: landmark l
     gets exactly track_lengths[l] observations (`nl` must equal its length, `mean_n` and `max_track` are not used).  Pair it
     with a small `lm_spread` (standard deviation of the landmark positions; the cameras stand at distance ~10) so that every
-    landmark lies inside every camera's field of view and no observation is filtered; a filtered one raises ValueError."""
+    landmark lies inside every camera's field of view and no observation is filtered; a filtered one raises ValueError.
+
+    `tracks` (one sequence of distinct camera indices per landmark) goes one step further and names the cameras of every
+    landmark; it implies the track lengths and the same no-filtering rule.  `k1_sigma` / `k2_sigma` are the standard
+    deviations of the radial distortion coefficients (the defaults make distortion negligible, as in the spec above; real
+    photo-collection cameras have |k1| up to ~0.5).  With the defaults of every option the output is unchanged."""
+    if tracks is not None:
+        tracks = [np.unique(np.asarray(t, dtype=np.int64)) for t in tracks]
+        track_lengths = [len(t) for t in tracks]
+        if any(t.size and (t[0] < 0 or t[-1] >= nc) for t in tracks):
+            raise ValueError(f"camera indices of tracks must lie in [0, nc = {nc})")
     if track_lengths is not None:
         want = np.asarray(track_lengths, dtype=np.int64).ravel()
         if want.shape[0] != nl:
@@ -209,8 +220,8 @@ def synth_bal(nc: int, nl: int, mean_n: float, seed: int = 38401, *, max_track: 
     cams[:, :4] = rot_to_quat(R)
     cams[:, 4:7] = t
     cams[:, 7] = rng.uniform(500, 2000, nc)
-    cams[:, 8] = rng.normal(0, 1e-7, nc)
-    cams[:, 9] = rng.normal(0, 1e-13, nc)
+    cams[:, 8] = rng.normal(0, k1_sigma, nc)
+    cams[:, 9] = rng.normal(0, k2_sigma, nc)
     # landmarks and track lengths
     lms = rng.normal(0, lm_spread, (nl, 3))
     if track_lengths is None:
@@ -219,7 +230,10 @@ def synth_bal(nc: int, nl: int, mean_n: float, seed: int = 38401, *, max_track: 
         n = np.minimum(n, min(nc, max_track)).astype(np.int64)
     else:
         n = want
-    obs_cam = _sample_tracks_local(rng, nc, n, locality) if locality > 0 else _sample_tracks(rng, nc, n)
+    if tracks is not None:
+        obs_cam = np.concatenate(tracks).astype(np.int32) if tracks else np.empty(0, np.int32)
+    else:
+        obs_cam = _sample_tracks_local(rng, nc, n, locality) if locality > 0 else _sample_tracks(rng, nc, n)
     lm_of_obs = np.repeat(np.arange(nl), n)
     xy, z, tan = project(cams[obs_cam], lms[lm_of_obs], return_tan=True)
     xy = xy + rng.normal(0, obs_noise, xy.shape)
@@ -254,6 +268,19 @@ def synth_bal(nc: int, nl: int, mean_n: float, seed: int = 38401, *, max_track: 
         prob.cams[:, :4] = rot_to_quat(Rn)
         prob.cams[:, 4:7] = -np.einsum("mij,mj->mi", Rn, ctr)
     return prob
+
+
+def turn_cameras_around(prob: BalArrays, cams) -> BalArrays:
+    """A copy of `prob` in which the chosen cameras are turned by 180 degrees about their own y axis (pc -> (-x, y, -z)):
+    every landmark they saw in front of them now lies behind them, at the same distance, so their observations become
+    invalid projections while the observed pixel values stay as they were."""
+    idx = np.atleast_1d(np.asarray(cams, dtype=np.int64))
+    flip = np.diag([-1.0, 1.0, -1.0])
+    out = BalArrays(prob.cams.copy(), prob.lms.copy(), prob.lm_off.copy(), prob.obs_cam.copy(), prob.obs_xy.copy())
+    R = np.einsum("ij,mjk->mik", flip, quat_to_rot(prob.cams[idx, :4]))
+    out.cams[idx, :4] = rot_to_quat(R)
+    out.cams[idx, 4:7] = prob.cams[idx, 4:7] @ flip.T
+    return out
 
 
 def synth_config(name: str, seed: int = 38401, scale: float = 1.0, **kw) -> BalArrays:

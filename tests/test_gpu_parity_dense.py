@@ -1,5 +1,5 @@
 """Oracle-independent GPU parity check: the CUDA path (through the C ABI) against dense float64 numpy algebra built from
-the per-observation Jacobians only.  tests/test_oracle_dense_numpy.py states the algebra and holds the oracle to the same bar."""
+the Jacobians of the independent camera model (tests/camera_model.py) only.  tests/test_oracle_dense_numpy.py states the algebra and holds the oracle to the same bar."""
 import numpy as np
 import pytest
 
@@ -11,12 +11,21 @@ pytestmark = pytest.mark.gpu
 @pytest.mark.parametrize("use_householder", [True, False])
 def test_f64_against_dense_normal_equations(use_householder):
     """Oracle-independent check of the CUDA path: b, H x, the converged PCG solution, the model cost change and the landmark
-    update against dense float64 numpy algebra built from the per-observation Jacobians only
+    update against dense float64 numpy algebra built from the Jacobians of the independent camera model only
     (tests/test_oracle_dense_numpy.py states the algebra and holds the oracle to the same bar)."""
+    _check_against_dense_normal_equations(use_householder, "benign")
+
+
+@pytest.mark.parametrize("use_householder", [True, False])
+def test_f64_against_dense_normal_equations_with_distortion(use_householder):
+    """the same check on a problem with real lens distortion (|k1| ~ 0.1, |x/z| <= 1.4)"""
+    _check_against_dense_normal_equations(use_householder, "distorted")
+
+
+def _check_against_dense_normal_equations(use_householder, kind):
     import rootba_b200 as rb
-    from rootba_b200.synthetic import synth_bal
-    from test_oracle_dense_numpy import _dense_system, _reduced
-    prob = synth_bal(7, 90, 3.6, seed=21)
+    from test_oracle_dense_numpy import _dense_system, _problem, _reduced
+    prob = _problem(kind)
     Jp, Jl, r = _dense_system(prob)
     lam = 1e-3
     D, sl, Jps, Jls, Minv, H, b = _reduced(Jp, Jl, r, lam, prob.nl, float(np.sqrt(1e-10)))

@@ -2,7 +2,8 @@
 
 The reference cannot be built here and ships no golden vectors ("parity unpinned", DESIGN.md section 6). What can be
 done without it: derive, from the per-observation Jacobians alone, what LinearizorQR must produce using nothing but
-dense textbook algebra in float64 numpy (no QR, no landmark blocks, no PCG), and require the oracle's
+dense textbook algebra in float64 numpy (no QR, no landmark blocks, no PCG), with the per-observation Jacobians from the
+independent camera model of tests/camera_model.py (on the benign stand-in and once with real lens distortion), and require the oracle's
 stage 1 / stage 2 / PCG / back-substitution pipeline (Householder and Givens, both preconditioners, staged and
 un-staged) to reproduce it.  The algebra (Demmel et al., "Square Root Bundle Adjustment", eq. 9-17; reference
 qr/impl/landmark_block_base.ipp):
@@ -19,25 +20,32 @@ qr/impl/landmark_block_base.ipp):
 import numpy as np
 import pytest
 
+import camera_model as cm
 from conftest import rel_err
 from oracle import oracle_py as orc
 
 
 def _dense_system(prob):
-    """dense weighted Jacobians (float64) of the whole problem from the per-observation linearisation"""
+    """dense Jacobians and residual (float64) of the whole problem from the independent camera model (tests/camera_model.py),
+    so that neither side of the comparison takes its linearisation from the oracle"""
     nobs, nc, nl = prob.nobs, prob.nc, prob.nl
+    jp, jl, res, _ = cm.weighted(prob)
     Jp = np.zeros((2 * nobs, 9 * nc))
     Jl = np.zeros((2 * nobs, 3 * nl))
-    r = np.zeros(2 * nobs)
-    for l in range(nl):
-        for k in range(int(prob.lm_off[l]), int(prob.lm_off[l + 1])):
-            c = int(prob.obs_cam[k])
-            res, jp, ji, jl, _ = orc.linearize_point(prob.obs_xy[k], prob.lms[l], prob.cams[c])
-            Jp[2 * k:2 * k + 2, 9 * c:9 * c + 6] = jp
-            Jp[2 * k:2 * k + 2, 9 * c + 6:9 * c + 9] = ji
-            Jl[2 * k:2 * k + 2, 3 * l:3 * l + 3] = jl
-            r[2 * k:2 * k + 2] = res
-    return Jp, Jl, r
+    lm_of_obs = np.repeat(np.arange(nl), np.diff(prob.lm_off))
+    for k in range(nobs):
+        c, l = int(prob.obs_cam[k]), int(lm_of_obs[k])
+        Jp[2 * k:2 * k + 2, 9 * c:9 * c + 9] = jp[k]
+        Jl[2 * k:2 * k + 2, 3 * l:3 * l + 3] = jl[k]
+    return Jp, Jl, res.ravel()
+
+
+def _problem(kind):
+    """the benign stand-in, or the same shape with real lens distortion and a wide field of view"""
+    from rootba_b200.synthetic import synth_bal
+    if kind == "distorted":
+        return synth_bal(7, 90, 3.6, seed=21, k1_sigma=0.1, k2_sigma=0.02, max_tan=1.4)
+    return synth_bal(7, 90, 3.6, seed=21)
 
 
 def _reduced(Jp, Jl, r, lam, nl, eps):
@@ -56,8 +64,13 @@ def _reduced(Jp, Jl, r, lam, nl, eps):
 
 @pytest.fixture(scope="module")
 def dense_case():
-    from rootba_b200.synthetic import synth_bal
-    prob = synth_bal(7, 90, 3.6, seed=21)
+    prob = _problem("benign")
+    return prob, _dense_system(prob)
+
+
+@pytest.fixture(scope="module")
+def distorted_case():
+    prob = _problem("distorted")
     return prob, _dense_system(prob)
 
 
@@ -65,7 +78,19 @@ def dense_case():
 @pytest.mark.parametrize("precond", [1, 0])
 @pytest.mark.parametrize("staged", [1, 0])
 def test_lm_inner_step_matches_dense_normal_equations(dense_case, use_householder, precond, staged):
-    prob, (Jp, Jl, r) = dense_case
+    _check_lm_inner_step(dense_case, use_householder, precond, staged)
+
+
+@pytest.mark.parametrize("use_householder", [1, 0])
+@pytest.mark.parametrize("precond", [1, 0])
+@pytest.mark.parametrize("staged", [1, 0])
+def test_lm_inner_step_matches_dense_normal_equations_with_distortion(distorted_case, use_householder, precond, staged):
+    """the same derivation on a problem with real lens distortion (|k1| ~ 0.1, |x/z| <= 1.4)"""
+    _check_lm_inner_step(distorted_case, use_householder, precond, staged)
+
+
+def _check_lm_inner_step(case, use_householder, precond, staged):
+    prob, (Jp, Jl, r) = case
     lam = 1e-3
     eps = float(np.sqrt(1e-10))  # Sophus::Constants<double>::epsilonSqrt(), linearizor_base.cpp:72-79
     D, sl, Jps, Jls, Minv, H, b = _reduced(Jp, Jl, r, lam, prob.nl, eps)
@@ -104,7 +129,15 @@ def test_lm_inner_step_matches_dense_normal_equations(dense_case, use_householde
 def test_first_order_model_predicts_the_true_cost_change(dense_case):
     """ties the linear algebra to the nonlinear problem: for a small step the model decrease l_diff (ipp:255-262) must
     match the true decrease of the cost (bal_bundle_adjustment.cpp:430-446: step_quality = f_diff / l_diff -> 1)"""
-    prob, _ = dense_case
+    _check_first_order_model(dense_case)
+
+
+def test_first_order_model_predicts_the_true_cost_change_with_distortion(distorted_case):
+    _check_first_order_model(distorted_case)
+
+
+def _check_first_order_model(case):
+    prob, _ = case
     o = orc.Oracle(prob, np.float64, orc.default_options(num_threads=1))
     e0 = o.compute_error()["all"]["error"]
     assert o.linearize()
@@ -116,6 +149,14 @@ def test_first_order_model_predicts_the_true_cost_change(dense_case):
 
 
 def test_sc_and_power_sc_linearizors_match_dense_normal_equations(dense_case):
+    _check_sc_and_power_sc(dense_case)
+
+
+def test_sc_and_power_sc_linearizors_match_dense_normal_equations_with_distortion(distorted_case):
+    _check_sc_and_power_sc(distorted_case)
+
+
+def _check_sc_and_power_sc(case):
     """the Schur-complement and Power-SC restatements (the checkers of tests/test_gpu_sc.py; reference
     solver/linearizor_sc.cpp, solver/linearizor_power_sc.cpp, sc/linearization_power_sc.hpp:92-160) against the same dense
     derivation:  H = Hpp + lambda I - E0,  Hpp = Jp_s^T Jp_s (block diagonal),  E0 = W M^-1 W^T,
@@ -123,7 +164,7 @@ def test_sc_and_power_sc_linearizors_match_dense_normal_equations(dense_case):
     These are the properties the reference's own tests check between its classes -- sc/linearization_power_sc.test.cpp:67-137
     (Hpp^-1 == inverted JACOBI blocks), :142-211 (b and the product of PowerSC == explicit SC), :214-300 (solve for m = 0 and
     m = 5 == the series written out), cg/preconditioner.test.cpp:59-136 -- here against dense numpy instead of against each other."""
-    prob, (Jp, Jl, r) = dense_case
+    prob, (Jp, Jl, r) = case
     lam = 1e-3
     eps = float(np.sqrt(1e-10))
     D, sl, Jps, Jls, Minv, H, b = _reduced(Jp, Jl, r, lam, prob.nl, eps)
