@@ -43,6 +43,7 @@ class SolverOptions:  # bal/solver_options.hpp (QR-relevant subset, reference de
     min_linear_solver_iterations: int = 0
     max_linear_solver_iterations: int = 500
     eta: float = 0.1
+    residual_reset_period: int = 10              # ConjugateGradientsSolver::Options (cg/conjugate_gradient.hpp:87): r = b - H x every this many iterations
     jacobi_scaling_epsilon: float = 0.0
     preconditioner_type: str = "SCHUR_JACOBI"     # JACOBI | SCHUR_JACOBI
     function_tolerance: float = 1e-6
@@ -188,6 +189,7 @@ class LinearizorQR:
         o.min_linear_solver_iterations = options.min_linear_solver_iterations
         o.max_linear_solver_iterations = options.max_linear_solver_iterations
         o.eta = options.eta
+        o.residual_reset_period = options.residual_reset_period
         o.device, o.rank, o.nranks = options.device, options.rank, options.nranks
         o.pcg_check_period = options.pcg_check_period
         o.operator_form = {"DENSE": 0, "IMPLICIT": 1}[options.operator_form]

@@ -2,7 +2,7 @@
 parameters") restated in float64 numpy, and bal_qr's argument checks.
 
 The device masks only the block-Jacobi inverse M^-1 (fixed rows and columns zero) and b (fixed entries zero), once per solve.
-The PCG recurrences of k_pcg_vec then never move a fixed entry of x, and the free entries follow PCG on the restricted
+The PCG recurrences of k_pcg_vec (tests/pcg_replay.py) then never move a fixed entry of x, and the free entries follow PCG on the restricted
 system H_ff x_f = -b_f iteration for iteration.  Same for the power series with the masked Hpp^-1."""
 import os
 import subprocess
@@ -11,6 +11,7 @@ import numpy as np
 import pytest
 
 from conftest import ROOT, rel_err
+from pcg_replay import pcg_replay
 
 FIX_POSE, FIX_F, FIX_K1, FIX_K2 = 1, 2, 4, 8
 # every bit, a combination of intrinsics, one fully fixed camera, free cameras
@@ -47,35 +48,6 @@ def block_apply(inv_blocks, v):
     return np.einsum("cij,cj->ci", inv_blocks, v.reshape(-1, 9)).ravel()
 
 
-def pcg_like_k_pcg_vec(H, b, apply_minv, eta, max_it, period=10):
-    """the recurrences of k_pcg_vec: mode 3 (x = 0, r = b, z = M^-1 r, p = z), mode 0 per iteration, every `period`-th
-    iteration mode 1 (x += alpha p) + mode 2 (r = b - H x), the zeta stopping rule; returns the iterates x_i"""
-    x = np.zeros_like(b)
-    r = b.copy()
-    z = apply_minv(r)
-    rho = r @ z
-    p = z.copy()
-    q0 = 0.0
-    xs = [x.copy()]
-    if np.linalg.norm(b) == 0:
-        return xs
-    for i in range(1, max_it + 1):
-        q = H @ p
-        alpha = rho / (p @ q)
-        x = x + alpha * p
-        r = b - H @ x if i % period == 0 else r - alpha * q
-        z = apply_minv(r)
-        rho_new = r @ z
-        q1 = -(x @ (b + r))
-        zeta = i * (q1 - q0) / q1
-        xs.append(x.copy())
-        if zeta < eta:
-            break
-        p = z + (rho_new / rho) * p
-        rho, q0 = rho_new, q1
-    return xs
-
-
 @pytest.fixture(scope="module")
 def system():
     from rootba_b200.synthetic import synth_bal
@@ -110,7 +82,7 @@ def test_pcg_with_masked_preconditioner_is_pcg_on_the_restricted_system(system):
     blocks = np.array([H[9 * c:9 * c + 9, 9 * c:9 * c + 9] for c in range(prob.nc)])
     inv = masked_block_inverse(blocks, fixed)
     bm = np.where(fixed, 0.0, b)
-    xs = pcg_like_k_pcg_vec(H, bm, lambda v: block_apply(inv, v), eta=1e-13, max_it=300)
+    xs = pcg_replay(lambda v: H @ v, bm, inv, eta=1e-13, max_it=300)["xs"]
     # restricted problem: fixed rows and columns deleted, block-Jacobi on the free sub-blocks
     Hff, bf = H[np.ix_(free, free)], b[free]
     sizes = [int(free[9 * c:9 * c + 9].sum()) for c in range(prob.nc)]
@@ -119,7 +91,7 @@ def test_pcg_with_masked_preconditioner_is_pcg_on_the_restricted_system(system):
 
     def minv_f(v):
         return np.concatenate([inv_f[c] @ v[starts[c]:starts[c + 1]] for c in range(prob.nc) if sizes[c]])
-    xs_f = pcg_like_k_pcg_vec(Hff, bf, minv_f, eta=1e-13, max_it=300)
+    xs_f = pcg_replay(lambda v: Hff @ v, bf, minv_f, eta=1e-13, max_it=300)["xs"]
     assert len(xs) == len(xs_f) > 10  # same iteration count: same zeta history
     for x, xf in zip(xs, xs_f):
         assert np.all(x[fixed] == 0)

@@ -76,6 +76,12 @@ def test_power_schur_complement_solver_against_oracle(small_problem, dtype):
         assert lin2.last_cg.termination_type == dbg["termination"]
         if lin2.last_cg.num_iterations == dbg["power_order"]:
             assert rel_err(inc_g, inc_c) < 10 * tol
+        else:  # a zeta within rounding of eta: the float64 replay of the series on the handle's own inputs
+            from pcg_replay import power_replay
+            from test_gpu_pcg_iterates import operator_of
+            rep = power_replay(operator_of(lin2, dtype), lin2.get_preconditioner()[0], lin2.get_rhs(), order=order, eta=eta)
+            assert (rep["iterations"], rep["termination"]) == (lin2.last_cg.num_iterations, lin2.last_cg.termination_type)
+            assert rel_err(inc_g, rep["sums"][-1]) < 10 * tol
         l_g, l_c = lin2.apply(inc_g), None
         assert np.isfinite(l_g) and l_g > 0
         lin2.close()
