@@ -240,6 +240,28 @@ int32_t rba_restore(rba_handle* h);
  * A flag with a bit above 3 set -> RBA_ERR_INVALID_ARGUMENT, and the previous flags stay in force. */
 int32_t rba_set_camera_fixed(rba_handle* h, const uint8_t* flags);
 
+/* ---- Gaussian priors on the cameras (DESIGN.md section 14) -------------------------------- */
+
+/* Not in the reference.  A soft prior on each camera's centre, orientation and intrinsics.
+ * mean [10*Nc] Scalar per camera: qx,qy,qz,qw (world->camera rotation R0, the state's convention), cx,cy,cz (camera
+ *   CENTRE c0 in the world frame, not t), f0, k1_0, k2_0.
+ * sqrt_info [81*Nc] Scalar: per camera a row-major 9x9 square-root information L_c.  Residual order
+ *   e = (c - c0 [3], Log(R R0^T) [3], f - f0, k1 - k1_0, k2 - k2_0),  c = -R^T t.
+ *   The prior cost is 1/2 |L_c e_c|^2, in the same convention as the reprojection terms (err = 1/2 r^2), not robustified.
+ *   An all-zero L_c means no prior on camera c.  Partial priors are rows of L (e.g. centre only).
+ * Both NULL: no priors, the default.  Every rank of a sharded problem passes the same arrays.
+ * The prior Jacobian is part of the linearisation: the Jacobi scaling is computed from the whole Jacobian (reprojection and
+ * prior columns), and rba_get_jacobian_scaling, rba_get_rhs, rba_get_preconditioner and rba_right_multiply include the
+ * prior terms.  After a call, rba_solve returns RBA_ERR_STATE until the next rba_linearize, the device-resident increment
+ * is discarded and the next rba_compute_error is evaluated afresh.
+ * rba_compute_error adds sum_c 1/2 |L_c e_c|^2 (accumulated in double) to all_error and valid_error; a non-finite prior
+ * cost clears is_numerically_valid; the observation counts and residual sums are unchanged.  So every optimized_cost,
+ * rba_lm_step, rba_lm_run and the host LM loops minimise the total (reprojection + prior) cost with no change of their own.
+ * With rba_set_camera_fixed the solve gives the restricted system of the total problem.
+ * Exactly one NULL pointer, a non-finite entry, or a mean quaternion whose norm is not within 1e-3 of 1 ->
+ * RBA_ERR_INVALID_ARGUMENT, and the previous priors stay in force.  A valid quaternion is normalised in double. */
+int32_t rba_set_camera_prior(rba_handle* h, const void* mean, const void* sqrt_info);
+
 /* ---- Linearizor interface (solver/linearizor.hpp:56-82) ---------------------------------- */
 
 /* LinearizorBase::compute_error (linearizor_base.cpp:59-67) -> BalBundleAdjustmentHelper::compute_error
@@ -308,17 +330,17 @@ int32_t rba_get_timings(const rba_handle* h, rba_stage_timings* out);
 /* ---- LinearizationQR-level access used by the parity tests -------------------------------- */
 
 /* pose_jacobian_scaling_ (linearizor_qr.cpp:130-132) [9*Nc] and the squared column norms
- * LinearizationQR::get_stage1 returns (linearization_qr.hpp:634-712) */
+ * LinearizationQR::get_stage1 returns (linearization_qr.hpp:634-712); with camera priors the prior columns are included */
 int32_t rba_get_jacobian_scaling(rba_handle* h, void* scaling_out, void* diag2_out);
 /* RHS b of the reduced camera system after the last rba_solve (get_stage2, linearization_qr.hpp:716-815);
- * the entries of parameters held by rba_set_camera_fixed are 0 */
+ * + A^T r of the camera priors; the entries of parameters held by rba_set_camera_fixed are 0 */
 int32_t rba_get_rhs(rba_handle* h, void* b_out);
 /* explicit inverse of the block-Jacobi preconditioner (cg/preconditioner.hpp:79-120) [81*Nc] and the
- * blocks it was built from (damping already added) [81*Nc].  For a camera with rba_set_camera_fixed flags the inverse is
+ * blocks it was built from (damping and the camera priors' A^T A already added; the blocks are written with SCHUR_JACOBI) [81*Nc].  For a camera with rba_set_camera_fixed flags the inverse is
  * that of the free sub-block, embedded in the 9x9 slot with zero fixed rows and columns; the blocks are not masked. */
 int32_t rba_get_preconditioner(rba_handle* h, void* inv_out, void* blocks_out);
-/* LinearizationQR::right_multiply (linearization_qr.hpp:823-825): y = (Q2^T Jp)^T (Q2^T Jp) x + lambda x
- * with the damping of the last rba_solve.  A debug accessor of the full operator: it ignores rba_set_camera_fixed. */
+/* LinearizationQR::right_multiply (linearization_qr.hpp:823-825): y = (Q2^T Jp)^T (Q2^T Jp) x + lambda x (+ A^T A x of the
+ * camera priors: the operator PCG applies) with the damping of the last rba_solve.  A debug accessor of the full operator: it ignores rba_set_camera_fixed. */
 int32_t rba_right_multiply(rba_handle* h, const void* x, void* y);
 /* LinearizationQR::back_substitute (linearization_qr.hpp:165-179) without the camera update */
 int32_t rba_back_substitute_f32(rba_handle* h, const float* pose_inc, float* l_diff_out);

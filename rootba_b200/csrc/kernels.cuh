@@ -90,6 +90,7 @@ struct DevPtrs {
   S* pblk;       // [csr_obs items][48] partial preconditioner blocks (45 used)
   int nc;
   const uint8_t* cam_fixed;  // [nc] RBA_FIX_* bits per camera (rba_set_camera_fixed), nullptr = every parameter free
+  const S* prior_H;          // [nc][81] A^T A of the scaled camera priors (rba_set_camera_prior), nullptr = no priors
 };
 
 // increment entries (tx,ty,tz, rx,ry,rz, f,k1,k2) held by a camera's RBA_FIX_* bits, as a 9-bit mask
@@ -1462,10 +1463,13 @@ __global__ void __launch_bounds__(128) k_panel_grad_blocks(DevPtrs<S> D, int wan
 //      the Cholesky and are zeroed in the inverse, and the fixed entries of b (final here) are zeroed.  The result is the
 //      inverse of the free sub-block: z = M^-1 r then has exactly zero fixed entries whatever r holds there, which keeps PCG
 //      and the power series on the restricted system (DESIGN.md, "Fixed camera parameters").
+//      Camera priors (DESIGN.md section 14): prior_H (the SCHUR_JACOBI blocks; the JACOBI blocks hold it since the
+//      linearisation) is added to the block and prior_g to b (already summed over the shards), both before the masking.
 template <class S>
 __global__ void __launch_bounds__(64) k_precond_invert(const S* __restrict__ src, S lambda, int nc,
                                                         S* __restrict__ blocks_out, S* __restrict__ inv,
-                                                        const uint8_t* __restrict__ cam_fixed, S* __restrict__ b) {
+                                                        const uint8_t* __restrict__ cam_fixed, S* __restrict__ b,
+                                                        const S* __restrict__ prior_H = nullptr, const S* __restrict__ prior_g = nullptr) {
   const int cam = blockIdx.x * blockDim.x + threadIdx.x;
   if (cam >= nc) return;
   const unsigned fm = cam_fixed ? fixed_entry_mask(cam_fixed[cam]) : 0u;
@@ -1475,6 +1479,14 @@ __global__ void __launch_bounds__(64) k_precond_invert(const S* __restrict__ src
   for (int r = 0; r < 9; ++r)
 #pragma unroll
     for (int c = 0; c < 9; ++c) A[r][c] = src[81 * (size_t)cam + 9 * r + c];
+  if (prior_H)
+#pragma unroll
+    for (int r = 0; r < 9; ++r)
+#pragma unroll
+      for (int c = 0; c < 9; ++c) A[r][c] += prior_H[81 * (size_t)cam + 9 * r + c];
+  if (prior_g)
+#pragma unroll
+    for (int d = 0; d < 9; ++d) b[9 * (size_t)cam + d] += prior_g[9 * (size_t)cam + d];
 #pragma unroll
   for (int d = 0; d < 9; ++d) A[d][d] += lambda;
   if (blocks_out)
@@ -2167,7 +2179,14 @@ __global__ void __launch_bounds__(128) k_pcg_q(DevPtrs<S> D, const PcgState* st,
 #pragma unroll
     for (int c = 0; c < 9; ++c) {
       const S pv = vec[9 * (size_t)cam + c];
-      const S qv = yv[c] + lambda * pv;
+      S qv = yv[c] + lambda * pv;
+      if (D.prior_H) {  // + A^T A v of the camera prior, in the order of k_pcg_vec<S, true>
+        const S* hr = D.prior_H + 81 * (size_t)cam + 9 * c;
+        S h = 0;
+#pragma unroll
+        for (int k = 0; k < 9; ++k) h += hr[k] * vec[9 * (size_t)cam + k];
+        qv += h;
+      }
       out[9 * (size_t)cam + c] = qv;
       pq += pv * qv;
     }
@@ -2268,7 +2287,10 @@ __device__ __forceinline__ void pcg_publish_progress(int* prog, int iter, int do
 
 // One CTA per SM (the grid is one cluster): the minimum of 1 block lets ptxas use up to 128 registers, where its sm_90
 // default caps the kernel at 64 and spills the register-resident vectors.
-template <class S>
+// PRIOR (D.prior_H set, DESIGN.md section 14): P1 adds the camera-prior term, q = y + lambda v + A^T A v.  The rows of A^T A
+// are fetched with the M^-1 rows, ahead of the grid dependency; the 9 entries of v of a camera are exchanged through shared
+// memory like r for z = M^-1 r.  PRIOR = false is the kernel without priors, unchanged.
+template <class S, bool PRIOR = false>
 __global__ void __launch_bounds__(VEC_THREADS, 1) k_pcg_vec(DevPtrs<S> D, PcgState* st, S lambda, int i, int mode,
                                                          double eta, int min_it, int is_last, int pdl, PeerComm pc, int seq,
                                                          const int* __restrict__ cam_item_ptr, int* prog) {
@@ -2286,6 +2308,7 @@ __global__ void __launch_bounds__(VEC_THREADS, 1) k_pcg_vec(DevPtrs<S> D, PcgSta
   if (*reinterpret_cast<const volatile int*>(&st->done)) return;  // monotonic flag, see k_matvec_small_tma
   // ---- prefetch of everything that does not depend on the previous kernel of this iteration ----
   S xv[VEC_EPT], rv[VEC_EPT], pv[VEC_EPT], bv[VEC_EPT], qv[VEC_EPT], zv[VEC_EPT], inv[VEC_EPT][9];
+  S hrow[PRIOR ? VEC_EPT : 1][9];  // rows of the camera prior's A^T A (PRIOR only)
   if (cached) {
 #pragma unroll
     for (int k = 0; k < VEC_EPT; ++k) {
@@ -2296,6 +2319,11 @@ __global__ void __launch_bounds__(VEC_THREADS, 1) k_pcg_vec(DevPtrs<S> D, PcgSta
       const S* row = D.inv + 9 * (size_t)e;  // inv[cam][a][:] = 9 consecutive scalars at 81 cam + 9 a = 9 e
 #pragma unroll
       for (int c = 0; c < 9; ++c) inv[k][c] = on ? row[c] : S(0);
+      if constexpr (PRIOR) {
+        const S* hr = D.prior_H + 9 * (size_t)e;  // same layout as inv
+#pragma unroll
+        for (int c = 0; c < 9; ++c) hrow[k][c] = on ? hr[c] : S(0);
+      }
       qv[k] = 0; zv[k] = 0;
     }
   }
@@ -2363,6 +2391,14 @@ __global__ void __launch_bounds__(VEC_THREADS, 1) k_pcg_vec(DevPtrs<S> D, PcgSta
     // ---- P1 ----
     double acc = 0;
     if (cached) {
+      if constexpr (PRIOR) {  // v of every camera of this CTA to shared memory (sr is free until P2a)
+#pragma unroll
+        for (int k = 0; k < VEC_EPT; ++k) {
+          const int l = tid + k * VEC_THREADS;
+          if (l < ne) sr[l] = (mode == 2) ? xv[k] : pv[k];
+        }
+        __syncthreads();
+      }
 #pragma unroll
       for (int k = 0; k < VEC_EPT; ++k) {
         const int l = tid + k * VEC_THREADS;
@@ -2375,6 +2411,13 @@ __global__ void __launch_bounds__(VEC_THREADS, 1) k_pcg_vec(DevPtrs<S> D, PcgSta
             for (int q = pi0[k]; q < pi1[k]; ++q) yk += __ldcg(D.partial + 9 * (size_t)q + c);
           } else yk = load_y(e0 + l);
           qv[k] = yk + lambda * vv;
+          if constexpr (PRIOR) {
+            const S* vc = sr + 9 * (l / 9);
+            S h = 0;
+#pragma unroll
+            for (int c = 0; c < 9; ++c) h += hrow[k][c] * vc[c];
+            qv[k] += h;
+          }
           acc += (double)(vv * qv[k]);
         }
       }
@@ -2382,7 +2425,15 @@ __global__ void __launch_bounds__(VEC_THREADS, 1) k_pcg_vec(DevPtrs<S> D, PcgSta
       const S* vec = (mode == 2) ? D.x : D.p;
       for (int l = tid; l < ne; l += VEC_THREADS) {
         const S vv = vec[e0 + l];
-        const S q = load_y(e0 + l) + lambda * vv;
+        S q = load_y(e0 + l) + lambda * vv;
+        if constexpr (PRIOR) {
+          const S* hr = D.prior_H + 9 * (size_t)(e0 + l);
+          const S* vc = vec + 9 * (size_t)((e0 + l) / 9);
+          S h = 0;
+#pragma unroll
+          for (int c = 0; c < 9; ++c) h += hr[c] * vc[c];
+          q += h;
+        }
         D.q[e0 + l] = q;
         acc += (double)(vv * q);
       }
@@ -2725,6 +2776,179 @@ __global__ void k_mask_fixed_inc(S* __restrict__ inc, const uint8_t* __restrict_
   const int e = blockIdx.x * blockDim.x + threadIdx.x;
   if (e >= 9 * nc) return;
   if ((fixed_entry_mask(cam_fixed[e / 9]) >> (e % 9)) & 1u) inc[e] = S(0);
+}
+
+// ------------------------------------------------------------------------------------------------
+// K8  Gaussian camera priors (rba_set_camera_prior, DESIGN.md section 14).  Per camera the residual
+//       e = (c - c0, Log(R R0^T), f - f0, k1 - k1_0, k2 - k2_0),   c = -R^T t the camera centre,
+//     the cost 1/2 |L e|^2 and, for the increment (v, w, df, dk1, dk2) of k_camera_update (R' = Exp(w) R, t' = Exp(w) t + v),
+//       de/dv = -R^T (rows 0..2),  dLog/dw = J_l^-1(Log(R R0^T)) (rows 3..5),  identity on the intrinsics (rows 6..8).
+//     mean [nc][10] (qx,qy,qz,qw of R0, c0, f0, k1_0, k2_0; unit quaternion), sqrt_info [nc][81] row-major L.
+// ------------------------------------------------------------------------------------------------
+// e of one camera; with JAC also J_l^-1 (row-major 3x3) and R (row-major 3x3)
+template <class S, bool JAC>
+__device__ __forceinline__ void prior_residual(const S* __restrict__ cam, const S* __restrict__ mean, S* e, S* Jinv, S* R) {
+  S Rl[9];
+  S* Rm = JAC ? R : Rl;
+  quat_to_rot(cam, Rm);
+  const S t0 = cam[4], t1 = cam[5], t2 = cam[6];
+#pragma unroll
+  for (int k = 0; k < 3; ++k) e[k] = -(Rm[k] * t0 + Rm[3 + k] * t1 + Rm[6 + k] * t2) - mean[4 + k];
+  // relative rotation q (x) conj(q0) (Hamilton product, xyzw); its Log with the angle in [0, pi]
+  const S a0 = cam[0], a1 = cam[1], a2 = cam[2], a3 = cam[3];
+  const S b0 = -mean[0], b1 = -mean[1], b2 = -mean[2], b3 = mean[3];
+  S w = a3 * b3 - a0 * b0 - a1 * b1 - a2 * b2;
+  S v0 = a3 * b0 + a0 * b3 + a1 * b2 - a2 * b1;
+  S v1 = a3 * b1 + a1 * b3 + a2 * b0 - a0 * b2;
+  S v2 = a3 * b2 + a2 * b3 + a0 * b1 - a1 * b0;
+  if (w < S(0)) { w = -w; v0 = -v0; v1 = -v1; v2 = -v2; }
+  const S n2 = v0 * v0 + v1 * v1 + v2 * v2;
+  const S n = sqrt(n2);
+  // theta / n with theta = 2 atan2(n, w); series 2/w (1 - n^2 / (3 w^2)) where n is tiny against w
+  const S fac = (n < ST<S>::eps_sqrt() * w) ? S(2) / w * (S(1) - n2 / (S(3) * w * w)) : S(2) * atan2(n, w) / n;
+  e[3] = fac * v0; e[4] = fac * v1; e[5] = fac * v2;
+  e[6] = cam[7] - mean[7]; e[7] = cam[8] - mean[8]; e[8] = cam[9] - mean[9];
+  if (JAC) {
+    // J_l^-1(phi) = I - 1/2 [phi]x + a [phi]x^2,  a = 1/th^2 - cot(th/2) / (2 th)  (series 1/12 + th^2/720 + th^4/30240)
+    const S p0 = e[3], p1 = e[4], p2 = e[5];
+    const S th2 = p0 * p0 + p1 * p1 + p2 * p2;
+    S a;
+    if (th2 < S(1e-4)) a = S(1.0 / 12.0) + th2 * (S(1.0 / 720.0) + th2 * S(1.0 / 30240.0));
+    else {
+      const S th = sqrt(th2), h = S(0.5) * th;
+      a = S(1) / th2 - cos(h) / (S(2) * th * sin(h));
+    }
+    // [phi]x^2 = phi phi^T - th^2 I
+    Jinv[0] = S(1) + a * (p0 * p0 - th2); Jinv[1] = S(0.5) * p2 + a * p0 * p1;       Jinv[2] = -S(0.5) * p1 + a * p0 * p2;
+    Jinv[3] = -S(0.5) * p2 + a * p1 * p0; Jinv[4] = S(1) + a * (p1 * p1 - th2);       Jinv[5] = S(0.5) * p0 + a * p1 * p2;
+    Jinv[6] = S(0.5) * p1 + a * p2 * p0;  Jinv[7] = -S(0.5) * p0 + a * p2 * p1;       Jinv[8] = S(1) + a * (p2 * p2 - th2);
+  }
+}
+
+// once per linearisation, after the cross-shard sum of diag2 and before k_scaling: the unscaled prior Jacobian
+// J = L de/d(inc) -> A [nc][81], r = L e -> pr [nc][9], and its squared column norms added to diag2 (the Jacobi scaling is
+// that of the whole Jacobian).  Thread per camera; identical on every shard (the prior data and the cameras are replicated).
+template <class S>
+__global__ void k_prior_linearize(const S* __restrict__ cams, const S* __restrict__ mean, const S* __restrict__ Lsq, int nc,
+                                  S* __restrict__ diag2, S* __restrict__ A, S* __restrict__ pr) {
+  const int cam = blockIdx.x * blockDim.x + threadIdx.x;
+  if (cam >= nc) return;
+  S e[9], Jinv[9], R[9];
+  prior_residual<S, true>(cams + 10 * (size_t)cam, mean + 10 * (size_t)cam, e, Jinv, R);
+  const S* Lc = Lsq + 81 * (size_t)cam;
+  S* Ac = A + 81 * (size_t)cam;
+  S cn[9];
+#pragma unroll
+  for (int j = 0; j < 9; ++j) cn[j] = 0;
+  for (int i = 0; i < 9; ++i) {
+    S l[9];
+#pragma unroll
+    for (int k = 0; k < 9; ++k) l[k] = Lc[9 * i + k];
+    S row[9], ri = 0;
+#pragma unroll
+    for (int k = 0; k < 9; ++k) ri += l[k] * e[k];
+#pragma unroll
+    for (int j = 0; j < 3; ++j) row[j] = -(l[0] * R[3 * j] + l[1] * R[3 * j + 1] + l[2] * R[3 * j + 2]);  // L (-R^T)
+#pragma unroll
+    for (int j = 0; j < 3; ++j) row[3 + j] = l[3] * Jinv[j] + l[4] * Jinv[3 + j] + l[5] * Jinv[6 + j];
+#pragma unroll
+    for (int j = 6; j < 9; ++j) row[j] = l[j];
+#pragma unroll
+    for (int j = 0; j < 9; ++j) { Ac[9 * i + j] = row[j]; cn[j] += row[j] * row[j]; }
+    pr[9 * (size_t)cam + i] = ri;
+  }
+#pragma unroll
+  for (int j = 0; j < 9; ++j) diag2[9 * (size_t)cam + j] += cn[j];
+}
+
+// after k_scaling (and after the JACOBI blocks are built): A <- J diag(s) in place, H = A^T A, g = A^T r, and H added to the
+// JACOBI blocks when they exist (jblocks != nullptr; they are the Hpp of Power-SC).  Thread per camera.
+template <class S>
+__global__ void k_prior_scale(S* __restrict__ A, const S* __restrict__ pr, const S* __restrict__ scaling, int nc,
+                              S* __restrict__ H, S* __restrict__ g, S* __restrict__ jblocks) {
+  const int cam = blockIdx.x * blockDim.x + threadIdx.x;
+  if (cam >= nc) return;
+  S s[9];
+#pragma unroll
+  for (int j = 0; j < 9; ++j) s[j] = scaling[9 * (size_t)cam + j];
+  S* Ac = A + 81 * (size_t)cam;
+  for (int i = 0; i < 9; ++i)
+#pragma unroll
+    for (int j = 0; j < 9; ++j) Ac[9 * i + j] *= s[j];
+  for (int a = 0; a < 9; ++a) {
+    S ga = 0;
+    for (int i = 0; i < 9; ++i) ga += Ac[9 * i + a] * pr[9 * (size_t)cam + i];
+    g[9 * (size_t)cam + a] = ga;
+    for (int b = 0; b < 9; ++b) {
+      S h = 0;
+      for (int i = 0; i < 9; ++i) h += Ac[9 * i + a] * Ac[9 * i + b];
+      H[81 * (size_t)cam + 9 * a + b] = h;
+      if (jblocks) jblocks[81 * (size_t)cam + 9 * a + b] += h;
+    }
+  }
+}
+
+// sum over the cameras of one double per camera, in a fixed order, added to out[0] (and out[1] when two are given).
+// One block: every entry point calls it after the cross-shard sum, so the prior term is added once and identically on every shard.
+__device__ __forceinline__ double prior_block_sum(double v) {
+  __shared__ double sh[32];
+  v = warp_sum(v);
+  if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = v;
+  __syncthreads();
+  double s = 0;
+  if (threadIdx.x == 0)
+    for (int w = 0; w < (int)(blockDim.x >> 5); ++w) s += sh[w];
+  return s;  // valid in thread 0
+}
+
+// prior cost sum_c 1/2 |L_c e_c|^2 at the current cameras, added to the all / valid errors (red[1], red[4]); a non-finite
+// sum sets the numerical-failure flag.  One block.
+template <class S>
+__global__ void k_prior_cost(const S* __restrict__ cams, const S* __restrict__ mean, const S* __restrict__ Lsq, int nc,
+                             double* red, int* bad_flag) {
+  double acc = 0;
+  for (int cam = threadIdx.x; cam < nc; cam += blockDim.x) {
+    S e[9];
+    prior_residual<S, false>(cams + 10 * (size_t)cam, mean + 10 * (size_t)cam, e, nullptr, nullptr);
+    const S* Lc = Lsq + 81 * (size_t)cam;
+    S c2 = 0;
+    for (int i = 0; i < 9; ++i) {
+      S ri = 0;
+#pragma unroll
+      for (int k = 0; k < 9; ++k) ri += Lc[9 * i + k] * e[k];
+      c2 += ri * ri;
+    }
+    acc += 0.5 * (double)c2;
+  }
+  const double s = prior_block_sum(acc);
+  if (threadIdx.x == 0) {
+    red[1] += s;
+    red[4] += s;
+    if (!isfinite(s)) *bad_flag = 1;
+  }
+}
+
+// prior part of the model cost change: l_diff -= sum_c (A d)^T (1/2 A d + r) for the (masked, scaled) increment d, added to
+// red[0] (the back-substitution's l_diff, already summed over the shards).  One block.
+template <class S>
+__global__ void k_prior_ldiff(const S* __restrict__ A, const S* __restrict__ pr, const S* __restrict__ inc, int nc, double* red) {
+  double acc = 0;
+  for (int cam = threadIdx.x; cam < nc; cam += blockDim.x) {
+    S d[9];
+#pragma unroll
+    for (int j = 0; j < 9; ++j) d[j] = inc[9 * (size_t)cam + j];
+    const S* Ac = A + 81 * (size_t)cam;
+    S lp = 0;
+    for (int i = 0; i < 9; ++i) {
+      S u = 0;
+#pragma unroll
+      for (int j = 0; j < 9; ++j) u += Ac[9 * i + j] * d[j];
+      lp += u * (S(0.5) * u + pr[9 * (size_t)cam + i]);
+    }
+    acc -= (double)lp;
+  }
+  const double s = prior_block_sum(acc);
+  if (threadIdx.x == 0) red[0] += s;
 }
 
 }  // namespace rba

@@ -49,6 +49,7 @@ struct rba_handle {
   virtual int backup() = 0;
   virtual int restore() = 0;
   virtual int set_camera_fixed(const uint8_t* flags) = 0;
+  virtual int set_camera_prior(const void* mean, const void* sqrt_info) = 0;
   virtual int compute_error(rba_residual_info* out) = 0;
   virtual int linearize() = 0;
   virtual int solve(double lambda, void* inc_out, rba_cg_summary* cg) = 0;
@@ -131,6 +132,13 @@ struct Solver : rba_handle {
   bool damping_valid = false;
   uint8_t* d_cam_fixed = nullptr;  // [nc] flags of rba_set_camera_fixed; D.cam_fixed points here while any flag is set
   bool all_cams_fixed = false;     // no free camera parameter: the reduced system is empty and its solve is skipped
+  // camera priors (rba_set_camera_prior, DESIGN.md section 14); D.prior_H points at d_prior_H while any L_c is non-zero
+  S* d_prior_mean = nullptr;       // [nc][10] mean, quaternion normalised
+  S* d_prior_L = nullptr;          // [nc][81] square-root information
+  S* d_prior_A = nullptr;          // [nc][81] L de/d(inc): unscaled after k_prior_linearize, scaled after k_prior_scale
+  S* d_prior_r = nullptr;          // [nc][9]  L e at the linearisation point
+  S* d_prior_H = nullptr;          // [nc][81] A^T A
+  S* d_prior_g = nullptr;          // [nc][9]  A^T r
   rba_stage_timings tm{};
   EventPair ev_stage1, ev_stage2, ev_precond, ev_pcg, ev_backsub, ev_update, ev_error, ev_mv, ev_user;
   long long launches = 0;
@@ -409,6 +417,7 @@ struct Solver : rba_handle {
     {
       // the PCG vector step runs on one thread-block cluster (16 CTAs if the device grants it, else 8)
       CU(cudaFuncSetAttribute(k_pcg_vec<S>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+      CU(cudaFuncSetAttribute((k_pcg_vec<S, true>), cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
       CU(cudaFuncSetAttribute(k_power_vec<S>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
       pcg_cluster = 16;
       if (const char* e = getenv("RBA_PDL")) use_pdl = atoi(e) != 0;
@@ -589,6 +598,66 @@ struct Solver : rba_handle {
     have_inc = false;  // the device-resident increment was solved under the previous flags
     return RBA_OK;
   }
+  // Gaussian priors on the camera parameters.  They are part of the linearisation (Jacobi scaling, A, r), so a change needs a
+  // new rba_linearize; the device-resident increment and the cost cache are discarded.  No prior (both NULL, or every L_c
+  // zero) = the unmodified path (D.prior_H == nullptr).
+  int set_camera_prior(const void* mean_v, const void* sqrt_info_v) override {
+    if ((mean_v == nullptr) != (sqrt_info_v == nullptr)) {
+      g_err = "rba_set_camera_prior: mean and sqrt_info must both be given or both be NULL";
+      return RBA_ERR_INVALID_ARGUMENT;
+    }
+    bool any = false;
+    std::vector<S> mean, Lsq;
+    if (mean_v) {
+      const S* m = (const S*)mean_v;
+      const S* Ls = (const S*)sqrt_info_v;
+      mean.assign(m, m + (size_t)10 * nc);
+      Lsq.assign(Ls, Ls + (size_t)81 * nc);
+      for (int c = 0; c < nc; ++c) {
+        for (int k = 0; k < 10; ++k)
+          if (!std::isfinite((double)mean[10 * (size_t)c + k])) {
+            g_err = "rba_set_camera_prior: camera " + std::to_string(c) + " has a non-finite mean";
+            return RBA_ERR_INVALID_ARGUMENT;
+          }
+        for (int k = 0; k < 81; ++k) {
+          const double v = (double)Lsq[81 * (size_t)c + k];
+          if (!std::isfinite(v)) {
+            g_err = "rba_set_camera_prior: camera " + std::to_string(c) + " has a non-finite sqrt_info";
+            return RBA_ERR_INVALID_ARGUMENT;
+          }
+          any = any || v != 0.0;
+        }
+        double q[4], n2 = 0;
+        for (int k = 0; k < 4; ++k) { q[k] = (double)mean[10 * (size_t)c + k]; n2 += q[k] * q[k]; }
+        const double n = std::sqrt(n2);
+        if (!(std::fabs(n - 1.0) <= 1e-3)) {
+          g_err = "rba_set_camera_prior: camera " + std::to_string(c) + " has a mean quaternion of norm " + std::to_string(n) + " (must be within 1e-3 of 1)";
+          return RBA_ERR_INVALID_ARGUMENT;
+        }
+        for (int k = 0; k < 4; ++k) mean[10 * (size_t)c + k] = (S)(q[k] / n);
+      }
+    }
+    if (any) {
+      if (!d_prior_mean) {
+        int rc;
+        if ((rc = dalloc(&d_prior_mean, (size_t)10 * nc, false))) return rc;
+        if ((rc = dalloc(&d_prior_L, (size_t)81 * nc, false))) return rc;
+        if ((rc = dalloc(&d_prior_A, (size_t)81 * nc, false))) return rc;
+        if ((rc = dalloc(&d_prior_r, (size_t)9 * nc, false))) return rc;
+        if ((rc = dalloc(&d_prior_H, (size_t)81 * nc, false))) return rc;
+        if ((rc = dalloc(&d_prior_g, (size_t)9 * nc, false))) return rc;
+      }
+      CU(cudaMemcpyAsync(d_prior_mean, mean.data(), mean.size() * sizeof(S), cudaMemcpyHostToDevice, stream));
+      CU(cudaMemcpyAsync(d_prior_L, Lsq.data(), Lsq.size() * sizeof(S), cudaMemcpyHostToDevice, stream));
+      CU(cudaStreamSynchronize(stream));
+    }
+    D.prior_H = any ? d_prior_H : nullptr;
+    linearized = false;  // the scaling, A and r of the last linearisation belong to the previous priors
+    damping_valid = false;
+    have_inc = false;
+    error_cache_valid = false;
+    return RBA_OK;
+  }
 
   // launch with optional programmatic dependent launch (the kernel may start before its predecessor in the stream has
   // finished and orders itself with griddepcontrol.wait) and optional thread-block-cluster dimension
@@ -672,6 +741,10 @@ struct Solver : rba_handle {
     k_sum_partials<6><<<1, 256, 0, stream>>>(d_epart, EBLOCKS, d_red);
     launches += 2;
     rc = allreduce_scalars(6); if (rc) return rc;
+    if (D.prior_H) {  // + sum of 1/2 |L e|^2, once, after the sum over the shards
+      k_prior_cost<S><<<1, 256, 0, stream>>>(D.cams, d_prior_mean, d_prior_L, nc, d_red, d_flags);
+      ++launches;
+    }
     CU(cudaMemcpyAsync(h_red, d_red, 6 * sizeof(double), cudaMemcpyDeviceToHost, stream));
     CU(cudaMemcpyAsync(h_flags, d_flags, 4 * sizeof(int), cudaMemcpyDeviceToHost, stream));
     rc = stop(ev_error); if (rc) return rc;
@@ -713,6 +786,10 @@ struct Solver : rba_handle {
     k_jp_norms<S><<<grid_for(L.nslots, 256, 8), 256, 0, stream>>>(D, ko, d_flags);
     ++launches;
     rc = camera_reduce(d_csr_obs_slots, d_csr_obs_items, n_obs_items, d_csr_obs_item_ptr, D.diag2, nullptr); if (rc) return rc;
+    if (D.prior_H) {  // prior Jacobian and its column norms (scaling from the whole Jacobian), after the sum over the shards
+      k_prior_linearize<S><<<(nc + 127) / 128, 128, 0, stream>>>(D.cams, d_prior_mean, d_prior_L, nc, D.diag2, d_prior_A, d_prior_r);
+      ++launches;
+    }
     k_scaling<S><<<(9 * nc + 255) / 256, 256, 0, stream>>>(D.diag2, D.scaling, 9 * nc, (S)ko.jacobi_eps);
     // pass B: linearize (scaled) + Jl scaling + Householder QR + panel write
     if (opt.use_householder_marginalization)
@@ -723,6 +800,11 @@ struct Solver : rba_handle {
     if (opt.preconditioner_type == 0 || opt.solver_type == 2) {
       // JACOBI: D (sum Jp^T Jp) D from the stored scaled Jacobians (Power-SC: these blocks are Hpp, sc/linearization_power_sc.hpp:92-128) (ref: ipp:554-569, block_sparse_matrix.hpp:89-100)
       rc = precond_blocks(0, D.jblocks, nullptr, true); if (rc) return rc;
+    }
+    if (D.prior_H) {  // scaled prior Jacobian, A^T A (+ into the JACOBI blocks), A^T r
+      const bool jac = opt.preconditioner_type == 0 || opt.solver_type == 2;
+      k_prior_scale<S><<<(nc + 127) / 128, 128, 0, stream>>>(d_prior_A, d_prior_r, D.scaling, nc, d_prior_H, d_prior_g, jac ? D.jblocks : nullptr);
+      ++launches;
     }
     if (panel_form) {
       // rows 3..2n-1 of the Q2 panels do not change with lambda: their part of the gradient (ipp:443-466) and of the
@@ -813,6 +895,9 @@ struct Solver : rba_handle {
   int pcg_vec(int i, int mode, bool pdl, int is_last, S lambda, bool fused_ar = false, bool from_partials = false) {
     PeerComm c = pc;
     if (!fused_ar) c.nranks = 1;
+    if (D.prior_H)
+      return launch_ex(k_pcg_vec<S, true>, pcg_cluster, VEC_THREADS, 0, pdl && use_pdl, pcg_cluster, D, d_state, lambda, i, mode, (double)opt.eta,
+                       (int)opt.min_linear_solver_iterations, is_last, (int)(pdl && use_pdl), c, ar_seq, from_partials ? op_item_ptr : (const int*)nullptr, d_prog);
     return launch_ex(k_pcg_vec<S>, pcg_cluster, VEC_THREADS, 0, pdl && use_pdl, pcg_cluster, D, d_state, lambda, i, mode, (double)opt.eta,
                      (int)opt.min_linear_solver_iterations, is_last, (int)(pdl && use_pdl), c, ar_seq, from_partials ? op_item_ptr : (const int*)nullptr, d_prog);
   }
@@ -921,9 +1006,11 @@ struct Solver : rba_handle {
     rc = stop(ev_stage2); if (rc) return rc;
     rc = start(ev_precond); if (rc) return rc;
     // pose damping lambda*I added to the blocks, then explicit inverse (ref: linearization_qr.hpp:796-802, linearizor_qr.cpp:228-237)
-    // (+ the masking of the held camera parameters, D.cam_fixed)
+    // (+ the masking of the held camera parameters, D.cam_fixed; + the camera priors: A^T A into the SCHUR_JACOBI blocks -- the
+    // JACOBI blocks hold it already -- and A^T r into b, both after the sum over the shards and before the masking)
     k_precond_invert<S><<<(nc + 63) / 64, 64, 0, stream>>>(schur ? D.blocks : D.jblocks, lambda, nc, schur ? D.blocks : nullptr, D.inv,
-                                                           D.cam_fixed, D.b);
+                                                           D.cam_fixed, D.b, schur ? (const S*)D.prior_H : nullptr,
+                                                           D.prior_H ? (const S*)d_prior_g : nullptr);
     ++launches;
     rc = stop(ev_precond); if (rc) return rc;
     last_lambda = lambda;
@@ -1055,6 +1142,10 @@ struct Solver : rba_handle {
     k_sum_partials<1><<<1, 256, 0, stream>>>(d_epart, grid, d_red);
     launches += 2;
     rc = allreduce_scalars(1); if (rc) return rc;
+    if (D.prior_H) {  // the prior part of the model cost change, once, after the sum over the shards
+      k_prior_ldiff<S><<<1, 256, 0, stream>>>(d_prior_A, d_prior_r, D.inc, nc, d_red);
+      ++launches;
+    }
     rc = stop(ev_backsub); if (rc) return rc;
     rc = start(ev_update); if (rc) return rc;
     if (update_cameras) {
@@ -1500,6 +1591,7 @@ int32_t rba_get_state(rba_handle* h, void* cams, void* lms) { return h->get_stat
 int32_t rba_backup(rba_handle* h) { return h->backup(); }
 int32_t rba_restore(rba_handle* h) { return h->restore(); }
 int32_t rba_set_camera_fixed(rba_handle* h, const uint8_t* flags) { return h->set_camera_fixed(flags); }
+int32_t rba_set_camera_prior(rba_handle* h, const void* mean, const void* sqrt_info) { return h->set_camera_prior(mean, sqrt_info); }
 int32_t rba_compute_error(rba_handle* h, rba_residual_info* out) { return h->compute_error(out); }
 int32_t rba_linearize(rba_handle* h) { return h->linearize(); }
 

@@ -141,6 +141,9 @@ class BalProblemSoA {
   std::vector<int32_t> obs_cam;   // ascending inside a landmark
   std::vector<Scalar> obs_xy;     // [nobs][2]
   std::vector<uint8_t> camera_fixed;  // [nc] RBA_FIX_* bits (rba_set_camera_fixed), forwarded by LinearizorQR::create; empty = all free
+  // Gaussian camera priors (rba_set_camera_prior), forwarded by LinearizorQR::create; empty = no priors.
+  std::vector<double> camera_prior_mean;       // [nc][10] qx,qy,qz,qw, centre, f, k1, k2
+  std::vector<double> camera_prior_sqrt_info;  // [nc][81] row-major L
 
   int num_cameras() const { return nc; }
   int num_landmarks() const { return nl; }

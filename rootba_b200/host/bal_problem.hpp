@@ -223,6 +223,9 @@ class BalProblem {
   // RBA_FIX_* bits per camera (rba_set_camera_fixed), forwarded by LinearizorQR::create; empty = every parameter free.
   // Not in the reference.
   std::vector<uint8_t> camera_fixed;
+  // Gaussian camera priors (rba_set_camera_prior), forwarded by LinearizorQR::create; empty = no priors.  Not in the reference.
+  std::vector<double> camera_prior_mean;       // [nc][10] qx,qy,qz,qw (R0), camera centre c0, f0, k1_0, k2_0
+  std::vector<double> camera_prior_sqrt_info;  // [nc][81] row-major square-root information L
 
  private:
   static void fail(FILE* f, const std::string& path) { std::fclose(f); throw std::runtime_error("Failed to parse '" + path + "'"); }

@@ -178,6 +178,13 @@ class LinearizorQR {
       if ((int)bp.camera_fixed.size() != bp.num_cameras()) throw std::runtime_error("camera_fixed must have one entry per camera");
       check(rba_set_camera_fixed(h_, bp.camera_fixed.data()));
     }
+    if (!bp.camera_prior_mean.empty() || !bp.camera_prior_sqrt_info.empty()) {
+      if (bp.camera_prior_mean.size() != (size_t)10 * bp.num_cameras() || bp.camera_prior_sqrt_info.size() != (size_t)81 * bp.num_cameras())
+        throw std::runtime_error("camera priors must have 10 mean and 81 sqrt_info entries per camera");
+      const VecX m(bp.camera_prior_mean.begin(), bp.camera_prior_mean.end());
+      const VecX L(bp.camera_prior_sqrt_info.begin(), bp.camera_prior_sqrt_info.end());
+      check(rba_set_camera_prior(h_, m.data(), L.data()));
+    }
   }
   Problem& bal_problem_;
   SolverSummary* summary_ = nullptr;

@@ -78,10 +78,32 @@ def _camera_fixed_array(flags, num_cameras: int):
     return np.ascontiguousarray(a, dtype=np.uint8).copy()
 
 
+def _camera_prior_arrays(prior, num_cameras: int, dtype):
+    """None, or validated contiguous copies (mean [nc,10], sqrt_info [nc,9,9]) of a camera prior in the problem's dtype"""
+    if prior is None:
+        return None
+    mean, sqrt_info = prior
+    mean = np.array(mean, dtype=dtype, order="C", copy=True)
+    sqrt_info = np.array(sqrt_info, dtype=dtype, order="C", copy=True)
+    if mean.shape != (num_cameras, 10):
+        raise ValueError(f"camera_prior mean must have shape ({num_cameras}, 10), got {mean.shape}")
+    if sqrt_info.shape != (num_cameras, 9, 9):
+        raise ValueError(f"camera_prior sqrt_info must have shape ({num_cameras}, 9, 9), got {sqrt_info.shape}")
+    if not (np.all(np.isfinite(mean)) and np.all(np.isfinite(sqrt_info))):
+        raise ValueError("camera_prior entries must be finite")
+    qn = np.linalg.norm(mean[:, :4].astype(np.float64), axis=1)
+    if np.any(np.abs(qn - 1.0) > 1e-3):
+        raise ValueError(f"camera_prior mean quaternions must have norm 1 (within 1e-3); camera {int(np.argmax(np.abs(qn - 1.0)))} has {qn.max():.6g}")
+    return mean, sqrt_info
+
+
 class BalProblem:
     """SoA BalProblem: cameras [nc,10] (quat xyzw, t, f,k1,k2), landmarks [nl,3], observations in
     CSR-by-landmark order with ascending camera index.  `camera_fixed` (not in the reference): None or one uint8 of FIX_*
-    bits per camera, held constant by the solver; forwarded to an attached LinearizorQR on assignment."""
+    bits per camera, held constant by the solver; forwarded to an attached LinearizorQR on assignment.
+    `camera_prior` (not in the reference): None or (mean [nc,10], sqrt_info [nc,9,9]), a Gaussian prior per camera with the
+    cost 1/2 |L e|^2, e = (centre - c0, Log(R R0^T), f - f0, k1 - k1_0, k2 - k2_0) (rba_set_camera_prior, DESIGN.md section 14);
+    mean rows are (qx,qy,qz,qw of R0, camera centre c0, f0, k1_0, k2_0).  Forwarded to an attached LinearizorQR on assignment."""
 
     def __init__(self, cams, lms, lm_off, obs_cam, obs_xy, dtype=np.float64):
         self.dtype = np.dtype(dtype)
@@ -95,6 +117,18 @@ class BalProblem:
         self._lms_backup = self.lms.copy()
         self._linearizor = None
         self._camera_fixed = None
+        self._camera_prior = None
+
+    @property
+    def camera_prior(self):
+        return self._camera_prior
+
+    @camera_prior.setter
+    def camera_prior(self, prior):
+        p = _camera_prior_arrays(prior, self.num_cameras(), self.dtype)
+        if self._linearizor is not None:
+            self._linearizor._upload_camera_prior(p)  # raises on rejection: the previous priors stay in force
+        self._camera_prior = p
 
     @property
     def camera_fixed(self):
@@ -208,6 +242,8 @@ class LinearizorQR:
         self.last_cg = CgSummary()
         if bal_problem.camera_fixed is not None:
             self._upload_camera_fixed()
+        if bal_problem.camera_prior is not None:
+            self._upload_camera_prior(bal_problem.camera_prior)
 
     # factory like Linearizor::create (linearizor.cpp:47-65)
     @staticmethod
@@ -242,6 +278,17 @@ class LinearizorQR:
     def _upload_camera_fixed(self):
         f = self.bal_problem.camera_fixed
         check(_lib.lib().rba_set_camera_fixed(self.h, None if f is None else _p(f)))
+
+    def set_camera_prior(self, prior):
+        """Gaussian camera priors (rba_set_camera_prior): None, or (mean [nc,10], sqrt_info [nc,9,9]).  Needs a new linearize
+        before the next solve; the priors are stored on the BalProblem."""
+        self.bal_problem.camera_prior = prior  # validates and forwards to _upload_camera_prior
+
+    def _upload_camera_prior(self, prior):
+        if prior is None:
+            check(_lib.lib().rba_set_camera_prior(self.h, None, None))
+        else:
+            check(_lib.lib().rba_set_camera_prior(self.h, _p(prior[0]), _p(prior[1])))
 
     def _backup(self):
         check(_lib.lib().rba_backup(self.h))
