@@ -435,10 +435,7 @@ __device__ __forceinline__ void cam_sum_staged(const S* __restrict__ src, const 
   const int s3 = lane / 9, c = lane - 9 * s3;
   const bool on = lane < 27;
   S acc = 0;
-#ifndef RBA_CAM_DEPTH
-#define RBA_CAM_DEPTH 16  /* value loads in flight per lane; 3 * depth slots per round */
-#endif
-  constexpr int DEPTH = RBA_CAM_DEPTH;
+  constexpr int DEPTH = 16;  // value loads in flight per lane; 3 * DEPTH slots per round
   for (int base = 0; base < cnt; base += 3 * DEPTH) {
     S v[DEPTH];
 #pragma unroll
@@ -536,18 +533,6 @@ __global__ void __launch_bounds__(256) k_cam_reduce_final(const S* __restrict__ 
       if (lane == 0) cam_cnt[I.cam] = 0;
     }
   }
-}
-
-// out[cam*9+c] = sum over the camera's items (fixed order)
-template <class S>
-__global__ void k_cam_final(const S* __restrict__ partial, const int* __restrict__ cam_item_ptr, int nc,
-                            S* __restrict__ out) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= 9 * nc) return;
-  const int cam = i / 9, c = i - 9 * cam;
-  S s = 0;
-  for (int it = cam_item_ptr[cam]; it < cam_item_ptr[cam + 1]; ++it) s += partial[9 * (size_t)it + c];
-  out[i] = s;
 }
 
 // ref: solver/linearizor_qr.cpp:130-132
@@ -1823,29 +1808,8 @@ __device__ __forceinline__ void matvec_item_tma(const DevPtrs<S>& D, const Matve
     mbar_wait(&bars[slot], (consumed / NS) & 1u);
     const int rows = min(RPS, rows_left);
     const V2* st = reinterpret_cast<const V2*>(ring + (size_t)slot * STAGE_BYTES) + lane;
-    int r = 0;
-#ifndef RBA_K4_PAIR
-#define RBA_K4_PAIR 0  /* 1: two rows per step (more ILP, 146 registers); 0: one row, 96 registers, 20 warps/SM -- measured equal or better */
-#endif
-    for (; RBA_K4_PAIR && r + 2 <= rows; r += 2) {  // two rows at a time: independent dependency chains
-      V2 va[KP], vb[KP];
-#pragma unroll
-      for (int k = 0; k < KP; ++k) { va[k] = st[(r * KP + k) * 32]; vb[k] = st[((r + 1) * KP + k) * 32]; }
-      S da0 = 0, da1 = 0, db0 = 0, db1 = 0;
-#pragma unroll
-      for (int k = 0; k < KP; ++k) {
-        da0 = fma(va[k].x, xv[k].x, da0); da1 = fma(va[k].y, xv[k].y, da1);
-        db0 = fma(vb[k].x, xv[k].x, db0); db1 = fma(vb[k].y, xv[k].y, db1);
-      }
-      S da = da0 + da1, db = db0 + db1;
-      da = group_sum_p(da, G); db = group_sum_p(db, G);
-#pragma unroll
-      for (int k = 0; k < KP; ++k) {
-        yv[k].x = fma(da, va[k].x, yv[k].x); yv[k].y = fma(da, va[k].y, yv[k].y);
-        yv[k].x = fma(db, vb[k].x, yv[k].x); yv[k].y = fma(db, vb[k].y, yv[k].y);
-      }
-    }
-    for (; r < rows; ++r) {
+    // one row per step: 96 registers and 20 warps per SM measured equal or better than two rows per step (146 registers)
+    for (int r = 0; r < rows; ++r) {
       V2 va[KP];
 #pragma unroll
       for (int k = 0; k < KP; ++k) va[k] = st[(r * KP + k) * 32];
@@ -1876,11 +1840,9 @@ __device__ __forceinline__ void matvec_item_tma(const DevPtrs<S>& D, const Matve
 // K4 (TMA variant): persistent warps, each streams the panels of its items through a private NS-stage
 // shared-memory ring (cp.async.bulk + mbarrier complete_tx), so the bytes in flight per SM are set by the
 // ring size (WARPS * NS * STAGE_BYTES) instead of by registers.
-#ifndef RBA_K4_MINB
-#define RBA_K4_MINB (sizeof(S) == 4 ? 5 : 2)
-#endif
+// Minimum resident CTAs: 5 for float32 (the shared-memory limit), 2 for float64 (register-limited).
 template <class S, int WARPS, int NS, int STAGE_BYTES>
-__global__ void __launch_bounds__(WARPS * 32, RBA_K4_MINB) k_matvec_small_tma(DevPtrs<S> D, const MatvecItem* __restrict__ items,
+__global__ void __launch_bounds__(WARPS * 32, sizeof(S) == 4 ? 5 : 2) k_matvec_small_tma(DevPtrs<S> D, const MatvecItem* __restrict__ items,
                                                                   int item_begin, int item_end, int scratch_per_warp,
                                                                   const S* __restrict__ xvec, const int* done, int pdl) {
   extern __shared__ __align__(128) unsigned char smem_tma[];
@@ -2109,29 +2071,6 @@ __global__ void __launch_bounds__(WARPS * 32) k_matvec_implicit_tma(DevPtrs<S> D
   }
 }
 
-template <class S, int WARPS>
-__global__ void __launch_bounds__(WARPS * 32) k_matvec_small(DevPtrs<S> D, const MatvecItem* __restrict__ items,
-                                                              int item_begin, int item_end, int scratch_per_warp,
-                                                              const S* __restrict__ xvec, const int* done) {
-  if (done && *done) return;
-  extern __shared__ __align__(16) unsigned char smem_raw[];
-  const int wib = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  S* xs = reinterpret_cast<S*>(smem_raw) + (size_t)wib * scratch_per_warp;
-  for (int q = item_begin + blockIdx.x * WARPS + wib; q < item_end; q += gridDim.x * WARPS) {
-    const MatvecItem it = items[q];
-    if (it.nrows == 0) continue;  // padding of the host's dealing for the TMA kernel
-    const TileInfo T = D.tiles[it.tile];
-    switch (T.KP) {
-      case 5: matvec_item<S, 5>(D, it, T, lane, xs, xvec); break;
-      case 6: matvec_item<S, 6>(D, it, T, lane, xs, xvec); break;
-      case 7: matvec_item<S, 7>(D, it, T, lane, xs, xvec); break;
-      case 8: matvec_item<S, 8>(D, it, T, lane, xs, xvec); break;
-      case 9: matvec_item<S, 9>(D, it, T, lane, xs, xvec); break;
-      default: break;
-    }
-  }
-}
-
 template <class S, int WARPS, int KPMAX>
 __global__ void __launch_bounds__(WARPS * 32) k_matvec_large(DevPtrs<S> D, const MatvecItem* __restrict__ items,
                                                               int item_begin, int item_end, int scratch_per_warp,
@@ -2156,26 +2095,14 @@ __global__ void __launch_bounds__(WARPS * 32) k_matvec_large(DevPtrs<S> D, const
 //   all launched with exactly NPART blocks of 128 threads; thread per camera (9-vectors);
 //   partial sums per block in double, combined in a fixed order by the consumer kernel.
 // ------------------------------------------------------------------------------------------------
-// q = (sum of camera partials | y) + lambda p ; partial pq.   src9 = y vector [9nc] (already reduced)
+// out = y + lambda v (+ A^T A v of the camera priors), y = the camera-reduced operator output [9 nc]; out may be y.
+// The operator of rba_right_multiply: the same order of operations as P1 of k_pcg_vec.
 template <class S>
-__global__ void __launch_bounds__(128) k_pcg_q(DevPtrs<S> D, const PcgState* st, const S* __restrict__ partial,
-                                               const int* __restrict__ cam_item_ptr, const S* __restrict__ yfull,
-                                               const S* __restrict__ vec, S* __restrict__ out, S lambda, double* part) {
-  if (st && st->done) return;
-  double acc[1] = {0};
+__global__ void __launch_bounds__(128) k_pcg_q(DevPtrs<S> D, const S* yfull, const S* __restrict__ vec, S* out, S lambda) {
   for (int cam = blockIdx.x * blockDim.x + threadIdx.x; cam < D.nc; cam += gridDim.x * blockDim.x) {
     S yv[9];
-    if (yfull) {
 #pragma unroll
-      for (int c = 0; c < 9; ++c) yv[c] = yfull[9 * (size_t)cam + c];
-    } else {
-#pragma unroll
-      for (int c = 0; c < 9; ++c) yv[c] = 0;
-      for (int it = cam_item_ptr[cam]; it < cam_item_ptr[cam + 1]; ++it)
-#pragma unroll
-        for (int c = 0; c < 9; ++c) yv[c] += partial[9 * (size_t)it + c];
-    }
-    S pq = 0;
+    for (int c = 0; c < 9; ++c) yv[c] = yfull[9 * (size_t)cam + c];
 #pragma unroll
     for (int c = 0; c < 9; ++c) {
       const S pv = vec[9 * (size_t)cam + c];
@@ -2188,18 +2115,14 @@ __global__ void __launch_bounds__(128) k_pcg_q(DevPtrs<S> D, const PcgState* st,
         qv += h;
       }
       out[9 * (size_t)cam + c] = qv;
-      pq += pv * qv;
     }
-    acc[0] += (double)pq;
   }
-  if (part) block_sum_store<1>(acc, part);
 }
 
-// y_local = sum of camera partials (multi-GPU: feeds the all-reduce)
+// out = per-camera sum of the segment partials (+ addend)
 template <class S>
 __global__ void k_cam_final9(const S* __restrict__ partial, const int* __restrict__ cam_item_ptr, int nc,
-                             S* __restrict__ out, const int* done, const S* __restrict__ addend = nullptr) {
-  if (done && *done) return;
+                             S* __restrict__ out, const S* __restrict__ addend = nullptr) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= 9 * nc) return;
   const int cam = i / 9, c = i - 9 * cam;

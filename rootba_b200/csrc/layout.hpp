@@ -11,6 +11,7 @@
 #include <cstdint>
 #include <numeric>
 #include <string>
+#include <utility>
 #include <vector>
 
 namespace rba {
@@ -76,16 +77,12 @@ struct Layout {
   bool csr_y_is_obs = true;
   std::vector<ReduceItem> pb_items;   // csr_obs slot list cut into segments of PB_SEG_LEN (preconditioner blocks)
   std::vector<int> pb_cam_item_ptr;   // [nc + 1]
-  int k1_scratch_per_warp = 0;     // scalars of shared memory per warp for the linearize+QR kernel
   int k4_scratch_per_warp = 0;     // scalars of shared memory per warp for the matvec kernel
 };
 
 constexpr int KP_SMALL_MAX = 9;    // classes with G <= 32 and <= 18 columns per lane
 constexpr int ROWS_PER_ITEM = 32;  // row chunk of long tracks
-#ifndef RBA_SEG_LEN
-#define RBA_SEG_LEN 96
-#endif
-constexpr int SEG_LEN = RBA_SEG_LEN;  // camera slot-list segment reduced by one warp
+constexpr int SEG_LEN = 96;        // camera slot-list segment reduced by one warp
 constexpr int PB_SEG_LEN = 16;     // observations per thread in the preconditioner-block kernel
 
 // group size for a track length (see DESIGN.md "track-length classes")
@@ -139,6 +136,33 @@ inline void build_csr(int nc, int nslots_total, const std::vector<int>& cam_of_s
       out.items.push_back({c, b, std::min(b + SEG_LEN, out.cam_ptr[c + 1])});
   }
   out.cam_item_ptr[nc] = (int)out.items.size();
+}
+
+// Longest-processing-time-first dealing of jobs with the given costs to nw persistent warps, where warp w takes the
+// positions w, w + nw, w + 2 nw, ... of the returned order: position k * nw + w holds the k-th job of warp w, and -1 pads
+// the lists that end early.  Jobs are dealt in order of decreasing cost (equal costs in index order), each to the warp
+// with the least load so far (equal loads: the lowest warp).
+inline std::vector<int> deal_lpt(const std::vector<long long>& cost, int nw) {
+  std::vector<int> idx(cost.size());
+  std::iota(idx.begin(), idx.end(), 0);
+  std::stable_sort(idx.begin(), idx.end(), [&](int a, int b) { return cost[a] > cost[b]; });
+  std::vector<std::vector<int>> lists(nw);
+  std::vector<std::pair<long long, int>> heap(nw);  // (load, warp), min-heap
+  for (int w = 0; w < nw; ++w) heap[w] = {0, w};
+  auto cmp = [](const std::pair<long long, int>& a, const std::pair<long long, int>& b) { return a > b; };
+  std::make_heap(heap.begin(), heap.end(), cmp);
+  for (int j : idx) {
+    std::pop_heap(heap.begin(), heap.end(), cmp);
+    heap.back().first += cost[j];
+    lists[heap.back().second].push_back(j);
+    std::push_heap(heap.begin(), heap.end(), cmp);
+  }
+  size_t maxlen = 0;
+  for (auto& l : lists) maxlen = std::max(maxlen, l.size());
+  std::vector<int> order(maxlen * nw, -1);
+  for (int w = 0; w < nw; ++w)
+    for (size_t k = 0; k < lists[w].size(); ++k) order[k * nw + w] = lists[w][k];
+  return order;
 }
 
 // Returns "" on success or an error message.
@@ -274,7 +298,6 @@ inline std::string build_layout(int nc, int nl, const int64_t* lm_off, const int
   // shared-memory scratch sizes (scalars per warp)
   for (const TileInfo& T : L.tiles) {
     const int W = 32 / T.G;
-    L.k1_scratch_per_warp = std::max(L.k1_scratch_per_warp, W * 32 * (int)T.n);
     const int CS = (2 * T.G * T.KP) | 1;
     L.k4_scratch_per_warp = std::max(L.k4_scratch_per_warp, T.KP > kp_max ? 2 * 64 * (int)T.KP : W * CS);
   }

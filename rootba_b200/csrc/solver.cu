@@ -30,6 +30,7 @@ thread_local std::string g_err;
       return RBA_ERR_CUDA;                                                                         \
     }                                                                                              \
   } while (0)
+#define TRY(x) do { int rc_ = (x); if (rc_) return rc_; } while (0)
 
 struct EventPair {
   cudaEvent_t a = nullptr, b = nullptr;
@@ -73,14 +74,27 @@ struct rba_handle {
   virtual int ipc_import(const void* all) = 0;
 };
 
-#ifndef RBA_IMP_NS
-#define RBA_IMP_NS 1
-#endif
-
 namespace rba {
 
 template <class S>
 struct Solver : rba_handle {
+  static constexpr int EBLOCKS = 592;
+  static constexpr int KPMAX = sizeof(S) == 4 ? 16 : 10;
+  // tile kernels (linearize+QR, stage 2, panel gradient)
+  static constexpr int TILE_WARPS = 4;
+  static constexpr int K1_CAP = 3904;   // scalars of shared memory per warp: linearize+QR needs 60 * W * n + 64 (= 3904 for the standard tiles)
+  static constexpr int K2_CAP = 3072;   // stage 2 needs 3 * W * CS + 9 * W * n + 20 W + 8 (<= 3048 for the standard tiles)
+  // dense operator (k_matvec_small_tma, k_matvec_large)
+  static constexpr int K4_WARPS = 4;
+  static constexpr int K4_NS = 2;        // TMA ring stages per warp
+  static constexpr int K4_STAGE = 4608;  // bytes per stage (2 rows of an f32 KP=9 tile)
+  static constexpr size_t K4_SMEM_TMA = (size_t)K4_WARPS * K4_NS * K4_STAGE;
+  // longest-first dealing of the small matvec items: cost = rows x KP (x 256 B) + this per-item constant (~12 KB-equivalent);
+  // 0 / 16 / 48 / 128 measured within 1 % of each other
+  static constexpr long long K4_ITEM_COST = 48;
+  // streamed implicit operator: warps per block, slots per stage, stages per warp
+  static constexpr int IMP_WARPS = 2, IMP_MAXSLOTS = 64, IMP_NS = 1;
+
   rba_solver_opts opt{};
   KOpts ko{};
   Layout L;
@@ -93,11 +107,9 @@ struct Solver : rba_handle {
   DevPtrs<S> D{};
   // device-only helpers
   S* cams_bk = nullptr; S* lms_bk = nullptr;
-  MatvecItem* d_items = nullptr;
-  std::vector<MatvecItem> dealt_items;  // L.items, the small-KP part dealt to the persistent warps (see init)
-  int n_dealt = 0, dealt_grid = 0, dealt_bps = 0;
   long long state_version = 0;     // bumped whenever cameras / landmarks change (set_state, apply, restore)
   rba_residual_info error_cache{}; long long error_cache_version = -1, error_enqueue_version = -1; bool error_cache_valid = false;
+  bool error_enqueued = false;
   int* d_csr_obs_slots = nullptr; ReduceItem* d_csr_obs_items = nullptr; int* d_csr_obs_item_ptr = nullptr;
   int* d_csr_y_slots = nullptr; ReduceItem* d_csr_y_items = nullptr; int* d_csr_y_item_ptr = nullptr;
   int n_obs_items = 0, n_y_items = 0;
@@ -105,24 +117,40 @@ struct Solver : rba_handle {
   // observation and row chunk) or the observation CSR of the implicit form
   const int* op_slots = nullptr; const ReduceItem* op_items = nullptr; const int* op_item_ptr = nullptr; int n_op_items = 0;
   bool implicit_op = false;
-  int e0_only_flag = 0;          // Power-SC: the implicit operator kernels return E_0 x = Q1d^T Q1d x alone
   bool panel_form = true;        // gradient and SCHUR_JACOBI blocks from the Q2 panels (reference form) instead of the identities
+  ReduceItem* d_pb_items = nullptr; int* d_pb_item_ptr = nullptr; int n_pb_items = 0;
+  // launch geometry and work orders of the persistent kernels (deal_work, setup_kernels)
+  Scratch<S> k1_sc{}, k2_sc{};
+  size_t k1_smem = 0, k2_smem = 0;
+  int k1_max_blocks = 264, k2_max_blocks = 264;
+  TileOrder order_k1{nullptr, 0}, order_kp{nullptr, 0};
+  MatvecItem* d_items = nullptr;   // L.items, the small-KP part dealt to the persistent warps of the TMA matvec
+  int n_dealt = 0, tma_grid = 1;
+  size_t k4_smem_small = 0;
   int imp_tile_split = 0;        // tiles [0, split) have <= IMP_MAXSLOTS slots and take the streamed kernel
   size_t imp_smem = 0; int imp_grid = 1;
-  ReduceItem* d_pb_items = nullptr; int* d_pb_item_ptr = nullptr; int n_pb_items = 0;
   int pcg_cluster = 16;
-  bool use_pdl = true;
+  // test hooks (read_test_hooks)
+  bool pcg_partials = true;      // one GPU: k_pcg_vec consumes the per-segment sums of k_cam_reduce
+  bool peer_ar = true;           // rba_ipc_import maps the peers' exchange regions
   int* h_prog = nullptr; int* d_prog = nullptr;  // PCG progress in host-mapped pinned memory: [0] last completed iteration, [1] solve ended
   int pcg_solve_id = 0;
-  bool pcg_partials = true;      // one GPU: k_pcg_vec consumes the per-segment sums of k_cam_reduce (RBA_PCG_PARTIALS=0: k_cam_reduce_final)
   double* d_epart = nullptr;     // [EBLOCKS][6]
   double* d_red = nullptr;       // [8] reduced doubles (error / l_diff)
-  int* d_flags = nullptr;        // [4] bad flags
+  int* d_flags = nullptr;        // [4] bad flags: [0] numerical failure, [1] peer-exchange time-out
   int* d_cam_cnt = nullptr;      // per-camera arrival counters of k_cam_reduce_final (zero between launches)
   PcgState* d_state = nullptr;
   PcgState* h_state = nullptr;   // pinned [2]
-  double* h_red = nullptr;       // pinned [8]
-  int* h_flags = nullptr;        // pinned [4]
+  // Pinned copies of d_red / d_flags, one slot per entry point, so that rba_lm_step can enqueue all of them and
+  // synchronise once
+  struct PinnedResults {
+    double error[6];             // compute_error
+    int error_flags[4];
+    int linearize_flags[4];      // linearize
+    double l_diff;               // apply
+    int apply_flags[4];
+  };
+  PinnedResults* h_res = nullptr;
   cudaEvent_t poll_ev[2] = {nullptr, nullptr};
   // status
   bool linearized = false;
@@ -142,6 +170,7 @@ struct Solver : rba_handle {
   rba_stage_timings tm{};
   EventPair ev_stage1, ev_stage2, ev_precond, ev_pcg, ev_backsub, ev_update, ev_error, ev_mv, ev_user;
   long long launches = 0;
+  long long lin_l0 = 0, solve_l0 = 0, apply_l0 = 0;  // `launches` at the start of the last linearize / solve / apply
   // NCCL
   NcclApi* nccl = nullptr;
   ncclComm_t comm = nullptr;
@@ -152,8 +181,6 @@ struct Solver : rba_handle {
   bool peer_ok = false;
   int ar_seq = 0, c_seq = 0, s_seq = 0;  // sequence numbers of the three flag families (operator output / vectors / scalars)
   std::vector<void*> ipc_opened;
-  static constexpr int EBLOCKS = 592;
-  static constexpr int KPMAX = sizeof(S) == 4 ? 16 : 10;
 
   ~Solver() override {
     if (comm && nccl) nccl->CommDestroy(comm);
@@ -161,8 +188,7 @@ struct Solver : rba_handle {
     for (void* p : allocs) cudaFree(p);
     if (h_prog) cudaFreeHost(h_prog);
     if (h_state) cudaFreeHost(h_state);
-    if (h_red) cudaFreeHost(h_red);
-    if (h_flags) cudaFreeHost(h_flags);
+    if (h_res) cudaFreeHost(h_res);
     for (EventPair* e : {&ev_stage1, &ev_stage2, &ev_precond, &ev_pcg, &ev_backsub, &ev_update, &ev_error, &ev_mv, &ev_user}) {
       if (e->a) cudaEventDestroy(e->a);
       if (e->b) cudaEventDestroy(e->b);
@@ -200,11 +226,10 @@ struct Solver : rba_handle {
   }
 
   // ------------------------------------------------------------------------------------------
+  // Set-up, in this order: the options, the layout, the dealing of the work to the persistent kernels, the device buffers,
+  // the tile scratch and the kernel attributes.
   int init(const rba_problem_view* pv, const rba_solver_opts* o) {
-    opt = *o;
-    if (opt.nranks < 1 || opt.rank < 0 || opt.rank >= opt.nranks) { g_err = "bad rank/nranks"; return RBA_ERR_INVALID_ARGUMENT; }
-    if (opt.pcg_check_period <= 0) opt.pcg_check_period = 4;
-    if (opt.residual_reset_period <= 0) opt.residual_reset_period = 10;
+    TRY(validate_options(*o));
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
       g_err = "no CUDA device: rootba_b200 has no CPU fallback";
@@ -221,13 +246,50 @@ struct Solver : rba_handle {
       CU(cudaEventCreate(&e->b));
     }
     for (auto& e : poll_ev) CU(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-    nc = pv->num_cameras;
-    nl_total = pv->num_landmarks;
+    read_test_hooks();
+    TRY(upload_layout(pv));
+    TRY(deal_work());
+    TRY(alloc_buffers());
+    TRY(setup_kernels());
+    CU(cudaStreamSynchronize(stream));
+    return RBA_OK;
+  }
+
+  int validate_options(const rba_solver_opts& o) {
+    opt = o;
+    if (opt.nranks < 1 || opt.rank < 0 || opt.rank >= opt.nranks) { g_err = "bad rank/nranks"; return RBA_ERR_INVALID_ARGUMENT; }
+    if (opt.operator_form != 0 && opt.operator_form != 1) { g_err = "operator_form must be 0 (dense) or 1 (implicit)"; return RBA_ERR_INVALID_ARGUMENT; }
+    if (opt.solver_type < 0 || opt.solver_type > 2) { g_err = "solver_type must be 0 (SQUARE_ROOT), 1 (SCHUR_COMPLEMENT) or 2 (POWER_SCHUR_COMPLEMENT)"; return RBA_ERR_INVALID_ARGUMENT; }
+    if (opt.solver_type == 2 && opt.nranks > 1) { g_err = "POWER_SCHUR_COMPLEMENT runs on one GPU (the power-series vector kernel has no peer exchange yet)"; return RBA_ERR_UNSUPPORTED; }
+    if (opt.stage2_form != 0 && opt.stage2_form != 1) { g_err = "stage2_form must be 0 (Q2 panel, reference) or 1 (orthogonality identity)"; return RBA_ERR_INVALID_ARGUMENT; }
+    if (opt.pcg_check_period <= 0) opt.pcg_check_period = 4;
+    if (opt.residual_reset_period <= 0) opt.residual_reset_period = 10;
+    if (opt.power_order <= 0) opt.power_order = 20;  // solver_options.hpp:270
+    // the Schur-complement solvers share the per-observation records and the implicit operator kernels (k_sc_stage2)
+    implicit_op = opt.operator_form == 1 || opt.solver_type != 0;
+    // gradient / SCHUR_JACOBI blocks from the stored Q2 panels like the reference, unless there are no panels (implicit operator)
+    panel_form = !implicit_op && opt.stage2_form == 0;
     ko.use_valid_projections_only = opt.use_valid_projections_only;
     ko.robust_norm = opt.robust_norm;
-    ko.write_panel = (opt.operator_form == 1 || opt.solver_type != 0) ? 0 : 1;
+    ko.write_panel = implicit_op ? 0 : 1;
     ko.huber = opt.huber_parameter;
     ko.jacobi_eps = opt.jacobi_scaling_epsilon > 0 ? opt.jacobi_scaling_epsilon : (double)ST<S>::eps_sqrt();  // ref: linearizor_base.cpp:72-79
+    return RBA_OK;
+  }
+
+  // Test hooks, not options: each forces at small size a path that the solver also takes on its own.
+  //   RBA_PCG_PARTIALS=0  PCG without the per-segment hand-over to the vector kernel (taken above 1808 cameras)
+  //   RBA_PCG_CLUSTER=k   a PCG vector cluster of at most k CTAs (taken when the device grants fewer than 16)
+  //   RBA_PEER_AR=0       NCCL for the reductions across shards (taken when the IPC mapping of a peer fails)
+  void read_test_hooks() {
+    if (const char* e = getenv("RBA_PCG_PARTIALS")) pcg_partials = atoi(e) != 0;
+    if (const char* e = getenv("RBA_PCG_CLUSTER")) pcg_cluster = std::max(1, std::min(atoi(e), 16));
+    if (const char* e = getenv("RBA_PEER_AR")) peer_ar = atoi(e) != 0;
+  }
+
+  int upload_layout(const rba_problem_view* pv) {
+    nc = pv->num_cameras;
+    nl_total = pv->num_landmarks;
     std::string msg = build_layout(nc, nl_total, pv->lm_obs_offset, pv->obs_cam_idx, opt.rank, opt.nranks, KPMAX, L);
     if (!msg.empty()) { g_err = msg; return RBA_ERR_INVALID_ARGUMENT; }
     // observation coordinates in slot order
@@ -235,66 +297,14 @@ struct Solver : rba_handle {
     const S* src = (const S*)pv->obs_xy;
     for (int s = 0; s < L.nslots; ++s)
       if (L.slot_obs[s] >= 0) { xy[2 * (size_t)s] = src[2 * L.slot_obs[s]]; xy[2 * (size_t)s + 1] = src[2 * L.slot_obs[s] + 1]; }
-    int rc;
     TileInfo* d_tiles; int* d_sorted; int* d_slot_cam; int* d_slot_lm; S* d_xy;
-#define TRY(x) do { rc = (x); if (rc) return rc; } while (0)
     TRY(upload(&d_tiles, L.tiles));
     TRY(upload(&d_sorted, L.sorted_lm));
     TRY(upload(&d_slot_cam, L.slot_cam));
     TRY(upload(&d_slot_lm, L.slot_lm));
     TRY(upload(&d_xy, xy));
-    // The persistent warps of the TMA matvec take the items q = first + k * (number of warps).  Dealing the items sorted by size
-    // round-robin leaves a warp with up to 1.6x the mean work on Ladybug-1723 (13 045 items for 2 960 warps: some get 5, some
-    // 4, and warp 0 the largest of every round); instead the small-KP items are dealt longest-processing-time-first on the host
-    // (greedy on bytes + a per-item constant) and laid out so that position k * W + w holds the k-th item of warp w, padded
-    // with empty items (nrows = 0 = end of a warp's list).  RBA_MATVEC_DEAL=rr keeps the round-robin order.
-    dealt_items = L.items;
-    n_dealt = (int)L.items.size();
-    {
-      const char* e = getenv("RBA_MATVEC_DEAL");
-      long long deal_ovh = 48;  // per-item constant (~12 KB-equivalent); 0 / 16 / 48 / 128 measured within 1 % of each other
-      if (const char* o2 = getenv("RBA_MATVEC_DEAL_OVH")) deal_ovh = atoll(o2);
-      const int nsmall = (int)L.items.size() - L.n_items_large;
-      // resident CTAs per SM of the TMA matvec (shared memory: 5; the float64 instance is register-limited to 2): the grid
-      // must be exactly the co-resident CTAs, or the longest-first lists of a later wave would start when the first is done
-      int tma_bps = std::max(1, (int)((220 * 1024) / ((size_t)K4_WARPS * K4_NS * K4_STAGE + 1024)));
-      {
-        const size_t smem = (size_t)K4_WARPS * K4_NS * K4_STAGE;
-        int occ = 0;
-        if (cudaFuncSetAttribute((k_matvec_small_tma<S, K4_WARPS, K4_NS, K4_STAGE>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) == cudaSuccess &&
-            cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, (k_matvec_small_tma<S, K4_WARPS, K4_NS, K4_STAGE>), K4_WARPS * 32, smem) == cudaSuccess && occ > 0)
-          tma_bps = std::min(tma_bps, occ);
-        else
-          cudaGetLastError();
-      }
-      dealt_bps = tma_bps;
-      const int W = grid_for(nsmall, K4_WARPS, tma_bps) * K4_WARPS;
-      if (!(e && std::string(e) == "rr") && nsmall > W && !implicit_op) {
-        std::vector<std::vector<int>> lists(W);
-        std::vector<std::pair<long long, int>> heap(W);  // (load, warp), min-heap on the load
-        for (int w = 0; w < W; ++w) heap[w] = {0, w};
-        auto cmp = [](const std::pair<long long, int>& a, const std::pair<long long, int>& b) { return a > b; };
-        std::make_heap(heap.begin(), heap.end(), cmp);
-        for (int q = L.n_items_large; q < (int)L.items.size(); ++q) {  // already sorted by decreasing work
-          std::pop_heap(heap.begin(), heap.end(), cmp);
-          auto& top = heap.back();
-          lists[top.second].push_back(q);
-          top.first += (long long)L.items[q].nrows * L.tiles[L.items[q].tile].KP + deal_ovh;  // rows x KP x 256 B, + a per-item constant
-          std::push_heap(heap.begin(), heap.end(), cmp);
-        }
-        size_t maxlen = 0;
-        for (auto& l : lists) maxlen = std::max(maxlen, l.size());
-        MatvecItem empty{}; empty.tile = 0; empty.row0 = 0; empty.nrows = 0; empty.yslot_base = 0; empty.pad = 0;
-        dealt_items.assign(L.items.begin(), L.items.begin() + L.n_items_large);
-        dealt_items.resize(L.n_items_large + maxlen * W, empty);
-        for (int w = 0; w < W; ++w)
-          for (size_t k = 0; k < lists[w].size(); ++k) dealt_items[L.n_items_large + k * W + w] = L.items[lists[w][k]];
-        n_dealt = (int)dealt_items.size();
-        dealt_grid = W / K4_WARPS;
-      }
-    }
-    TRY(upload(&d_items, dealt_items));
-
+    D.tiles = d_tiles; D.ntiles = (int)L.tiles.size(); D.sorted_lm = d_sorted;
+    D.slot_cam = d_slot_cam; D.slot_lm = d_slot_lm; D.slot_xy = d_xy; D.nslots = L.nslots; D.nc = nc;
     TRY(upload(&d_csr_obs_slots, L.csr_obs.slots));
     TRY(upload(&d_csr_obs_items, L.csr_obs.items));
     TRY(upload(&d_csr_obs_item_ptr, L.csr_obs.cam_item_ptr));
@@ -308,16 +318,16 @@ struct Solver : rba_handle {
       TRY(upload(&d_csr_y_item_ptr, L.csr_y.cam_item_ptr));
       n_y_items = (int)L.csr_y.items.size();
     }
-    implicit_op = opt.operator_form == 1 || opt.solver_type != 0;
-    if (opt.operator_form != 0 && opt.operator_form != 1) { g_err = "operator_form must be 0 (dense) or 1 (implicit)"; return RBA_ERR_INVALID_ARGUMENT; }
-    if (opt.solver_type < 0 || opt.solver_type > 2) { g_err = "solver_type must be 0 (SQUARE_ROOT), 1 (SCHUR_COMPLEMENT) or 2 (POWER_SCHUR_COMPLEMENT)"; return RBA_ERR_INVALID_ARGUMENT; }
-    if (opt.solver_type == 2 && opt.nranks > 1) { g_err = "POWER_SCHUR_COMPLEMENT runs on one GPU (the power-series vector kernel has no peer exchange yet)"; return RBA_ERR_UNSUPPORTED; }
-    if (opt.power_order <= 0) opt.power_order = 20;  // solver_options.hpp:270
-    // the Schur-complement solvers share the per-observation records and the implicit operator kernels (k_sc_stage2)
-    if (opt.solver_type != 0) implicit_op = true;
-    if (opt.stage2_form != 0 && opt.stage2_form != 1) { g_err = "stage2_form must be 0 (Q2 panel, reference) or 1 (orthogonality identity)"; return RBA_ERR_INVALID_ARGUMENT; }
-    // gradient / SCHUR_JACOBI blocks from the stored Q2 panels like the reference, unless there are no panels (implicit operator)
-    panel_form = !implicit_op && opt.stage2_form == 0;
+    if (implicit_op) { op_slots = d_csr_obs_slots; op_items = d_csr_obs_items; op_item_ptr = d_csr_obs_item_ptr; n_op_items = n_obs_items; }
+    else { op_slots = d_csr_y_slots; op_items = d_csr_y_items; op_item_ptr = d_csr_y_item_ptr; n_op_items = n_y_items; }
+    TRY(upload(&d_pb_items, L.pb_items));
+    TRY(upload(&d_pb_item_ptr, L.pb_cam_item_ptr));
+    n_pb_items = (int)L.pb_items.size();
+    return RBA_OK;
+  }
+
+  // The grids of the persistent kernels and the order in which their warps take the work.
+  int deal_work() {
     if (implicit_op) {
       while (imp_tile_split < (int)L.tiles.size() && (32 / L.tiles[imp_tile_split].G) * L.tiles[imp_tile_split].n <= IMP_MAXSLOTS) ++imp_tile_split;
       imp_smem = (size_t)IMP_WARPS * IMP_NS * (size_t)IMP_MAXSLOTS * 48 * sizeof(S);
@@ -325,14 +335,86 @@ struct Solver : rba_handle {
       int bps = 0;
       CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, (k_matvec_implicit_tma<S, IMP_WARPS, IMP_MAXSLOTS, IMP_NS>), IMP_WARPS * 32, imp_smem));
       imp_grid = std::max(1, std::min((imp_tile_split + IMP_WARPS - 1) / IMP_WARPS, sm_count * std::max(1, bps)));
+    } else {
+      TRY(deal_matvec_items());
     }
-    if (implicit_op) { op_slots = d_csr_obs_slots; op_items = d_csr_obs_items; op_item_ptr = d_csr_obs_item_ptr; n_op_items = n_obs_items; }
-    else { op_slots = d_csr_y_slots; op_items = d_csr_y_items; op_item_ptr = d_csr_y_item_ptr; n_op_items = n_y_items; }
-    TRY(upload(&d_pb_items, L.pb_items));
-    TRY(upload(&d_pb_item_ptr, L.pb_cam_item_ptr));
-    n_pb_items = (int)L.pb_items.size();
-    D.tiles = d_tiles; D.ntiles = (int)L.tiles.size(); D.sorted_lm = d_sorted;
-    D.slot_cam = d_slot_cam; D.slot_lm = d_slot_lm; D.slot_xy = d_xy; D.nslots = L.nslots; D.nc = nc;
+    // the tile kernels' scratch decides k_linearize_qr's grid
+    long long need1 = 0, need2 = 0;
+    for (const TileInfo& T : L.tiles) {
+      const int Wn = (32 / T.G) * T.n;
+      need1 = std::max<long long>(need1, (long long)Wn * 60 + 64);
+      need2 = std::max<long long>(need2, (long long)stage2_need(T.n, T.G, T.KP));
+    }
+    tile_scratch_geometry(k1_sc, K1_CAP, need1, k1_smem, k1_max_blocks);
+    tile_scratch_geometry(k2_sc, K2_CAP, need2, k2_smem, k2_max_blocks);
+    // tiles dealt to the persistent warps longest-first (the kernels' work per tile grows like n^2: panel rows x columns)
+    TRY(deal_tiles(tile_grid(k1_max_blocks) * TILE_WARPS, order_k1));
+    TRY(deal_tiles(tile_grid(sm_count * 8) * TILE_WARPS, order_kp));
+    return RBA_OK;
+  }
+
+  // The persistent warps of the TMA matvec take the items q = first + k * (number of warps).  Dealing the items sorted by
+  // size round-robin leaves a warp with up to 1.6x the mean work on Ladybug-1723 (13 045 items for 2 960 warps: some get 5,
+  // some 4, and warp 0 the largest of every round); instead the small-KP items are dealt longest-processing-time-first
+  // (deal_lpt), padded with empty items (nrows = 0 = end of a warp's list).  The grid must be exactly the co-resident CTAs
+  // (shared memory: 5 per SM; the float64 instance is register-limited to 2), or the longest-first lists of a later wave
+  // would start when the first is done.
+  int deal_matvec_items() {
+    CU(cudaFuncSetAttribute((k_matvec_small_tma<S, K4_WARPS, K4_NS, K4_STAGE>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)K4_SMEM_TMA));
+    int occ = 0;
+    CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, (k_matvec_small_tma<S, K4_WARPS, K4_NS, K4_STAGE>), K4_WARPS * 32, K4_SMEM_TMA));
+    int bps = std::max(1, (int)((220 * 1024) / (K4_SMEM_TMA + 1024)));
+    if (occ > 0) bps = std::min(bps, occ);
+    const int nsmall = (int)L.items.size() - L.n_items_large;
+    tma_grid = grid_for(nsmall, K4_WARPS, bps);
+    const int W = tma_grid * K4_WARPS;
+    std::vector<MatvecItem> items = L.items;
+    if (nsmall > W) {
+      std::vector<long long> cost(nsmall);
+      for (int q = 0; q < nsmall; ++q) {
+        const MatvecItem& it = L.items[L.n_items_large + q];
+        cost[q] = (long long)it.nrows * L.tiles[it.tile].KP + K4_ITEM_COST;
+      }
+      const MatvecItem empty{};
+      items.resize(L.n_items_large);
+      for (int q : deal_lpt(cost, W)) items.push_back(q >= 0 ? L.items[L.n_items_large + q] : empty);
+    }
+    n_dealt = (int)items.size();
+    return upload(&d_items, items);
+  }
+
+  // longest-first tile order for nw persistent warps of the tile kernels (none when every warp gets at most one tile)
+  int deal_tiles(int nw, TileOrder& out) {
+    const int nt = (int)L.tiles.size();
+    if (nt <= nw) return RBA_OK;
+    std::vector<long long> cost(nt);
+    for (int t = 0; t < nt; ++t) {
+      const TileInfo& T = L.tiles[t];
+      cost[t] = (long long)2 * T.n * T.KP + (long long)(32 / T.G) * T.n / 2 + 8;  // panel rows x column steps + per-observation work + constant
+    }
+    int* d = nullptr;
+    const std::vector<int> order = deal_lpt(cost, nw);
+    TRY(upload(&d, order));
+    out.order = d; out.count = (int)order.size();
+    return RBA_OK;
+  }
+
+  // tile kernels (linearize+QR, stage 2): scratch in shared memory when the tile fits in the kernel's cap (scalars per
+  // warp), else in a per-warp slice of a global buffer of at most 1 GiB (very long tracks; slow but general), which
+  // limits the grid
+  void tile_scratch_geometry(Scratch<S>& sc, int cap, long long need, size_t& smem, int& max_blocks) const {
+    sc.smem_cap = cap; sc.gbase = nullptr; sc.gstride = 0;
+    smem = (size_t)TILE_WARPS * cap * sizeof(S);
+    max_blocks = sm_count * std::max(1, (int)((220 * 1024) / (smem + 1024)));
+    if (need > cap) {
+      long long warps = (long long)max_blocks * TILE_WARPS;
+      while (warps > TILE_WARPS && warps * need * (long long)sizeof(S) > (1LL << 30)) warps /= 2;
+      max_blocks = (int)std::max<long long>(1, warps / TILE_WARPS);
+      sc.gstride = (need + 3) & ~3LL;
+    }
+  }
+
+  int alloc_buffers() {
     TRY(dalloc(&D.cams, (size_t)10 * nc)); TRY(dalloc(&cams_bk, (size_t)10 * nc));
     TRY(dalloc(&D.lms, (size_t)3 * L.nl_local)); TRY(dalloc(&lms_bk, (size_t)3 * L.nl_local));
     if (ko.write_panel) TRY(dalloc(&D.panel, (size_t)L.panel_scalars));  // the implicit operator never touches the panels
@@ -372,104 +454,37 @@ struct Solver : rba_handle {
     CU(cudaHostGetDevicePointer((void**)&d_prog, h_prog, 0));
     h_prog[0] = 0; h_prog[1] = 0;
     CU(cudaMallocHost((void**)&h_state, 2 * sizeof(PcgState)));
-    CU(cudaMallocHost((void**)&h_red, 24 * sizeof(double)));
-    CU(cudaMallocHost((void**)&h_flags, 12 * sizeof(int)));
-    // tile kernels (linearize+QR, stage 2): scratch in shared memory when the tile fits in the kernel's cap (scalars per
-    // warp), else in a per-warp slice of a global buffer (very long tracks; slow but general)
-    {
-      long long need1 = 0, need2 = 0;
-      for (const TileInfo& T : L.tiles) {
-        const int Wn = (32 / T.G) * T.n;
-        need1 = std::max<long long>(need1, (long long)Wn * 60 + 64);
-        need2 = std::max<long long>(need2, (long long)stage2_need(T.n, T.G, T.KP));
-      }
-      auto setup = [&](Scratch<S>& sc, int cap, long long need, size_t& smem, int& blocks_per_sm, int& max_blocks) -> int {
-        sc.smem_cap = cap; sc.gbase = nullptr; sc.gstride = 0;
-        smem = (size_t)TILE_WARPS * cap * sizeof(S);
-        blocks_per_sm = std::max(1, (int)((220 * 1024) / (smem + 1024)));
-        max_blocks = sm_count * blocks_per_sm;
-        if (need > cap) {
-          long long warps = (long long)max_blocks * TILE_WARPS;
-          while (warps > TILE_WARPS && warps * need * (long long)sizeof(S) > (1LL << 30)) warps /= 2;
-          max_blocks = (int)std::max<long long>(1, warps / TILE_WARPS);
-          sc.gstride = (need + 3) & ~3LL;
-          int rc2 = dalloc(&sc.gbase, (size_t)(max_blocks * TILE_WARPS) * sc.gstride, false);
-          if (rc2) return rc2;
-        }
-        return RBA_OK;
-      };
-      TRY(setup(k1_sc, K1_CAP, need1, k1_smem, k1_bps, k1_max_blocks));
-      TRY(setup(k2_sc, K2_CAP, need2, k2_smem, k2_bps, k2_max_blocks));
-      // tiles dealt to the persistent warps longest-first (the kernels' work per tile grows like n^2: panel rows x columns)
-      if (!(getenv("RBA_TILE_DEAL") && std::string(getenv("RBA_TILE_DEAL")) == "rr")) {
-        TRY(deal_tiles(tile_grid(k1_max_blocks) * TILE_WARPS, order_k1));
-        TRY(deal_tiles(tile_grid(sm_count * 8) * TILE_WARPS, order_kp));
-      }
-      CU(cudaFuncSetAttribute((k_linearize_qr<S, false>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)k1_smem));
-      CU(cudaFuncSetAttribute((k_linearize_qr<S, true>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)k1_smem));
-      CU(cudaFuncSetAttribute((k_stage2<S, true>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)k2_smem));
-      CU(cudaFuncSetAttribute((k_stage2<S, false>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)k2_smem));
-    }
-    k4_smem_small = (size_t)K4_WARPS * L.k4_scratch_per_warp * sizeof(S);
-    if (k4_smem_small > 200 * 1024) { g_err = "matvec scratch exceeds shared memory"; return RBA_ERR_UNSUPPORTED; }
-    CU(cudaFuncSetAttribute(k_matvec_small<S, K4_WARPS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(k4_smem_small, 1024)));
-    CU(cudaFuncSetAttribute((k_matvec_large<S, K4_WARPS, KPMAX>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(k4_smem_small, 1024)));
-    {
-      // the PCG vector step runs on one thread-block cluster (16 CTAs if the device grants it, else 8)
-      CU(cudaFuncSetAttribute(k_pcg_vec<S>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
-      CU(cudaFuncSetAttribute((k_pcg_vec<S, true>), cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
-      CU(cudaFuncSetAttribute(k_power_vec<S>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
-      pcg_cluster = 16;
-      if (const char* e = getenv("RBA_PDL")) use_pdl = atoi(e) != 0;
-      if (const char* e = getenv("RBA_PCG_PARTIALS")) pcg_partials = atoi(e) != 0;
-      if (const char* e = getenv("RBA_PCG_CLUSTER")) pcg_cluster = std::max(1, std::min(atoi(e), 16));
-      for (; pcg_cluster > 1; pcg_cluster >>= 1) {
-        cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3(pcg_cluster); cfg.blockDim = dim3(VEC_THREADS);
-        cudaLaunchAttribute at[1];
-        at[0].id = cudaLaunchAttributeClusterDimension;
-        at[0].val.clusterDim.x = pcg_cluster; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-        cfg.attrs = at; cfg.numAttrs = 1;
-        int ncl = 0;
-        if (cudaOccupancyMaxActiveClusters(&ncl, k_pcg_vec<S>, &cfg) == cudaSuccess && ncl >= 1) break;
-        cudaGetLastError();
-      }
-    }
-    {
-      const char* e = getenv("RBA_MATVEC");
-      use_tma = !(e && std::string(e) == "ldg");
-      k4_smem_tma = (size_t)K4_WARPS * K4_NS * K4_STAGE;
-      if (k4_smem_tma > 220 * 1024) use_tma = false;
-      if (use_tma) {
-        CU(cudaFuncSetAttribute((k_matvec_small_tma<S, K4_WARPS, K4_NS, K4_STAGE>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)k4_smem_tma));
-        k4_tma_blocks_per_sm = std::max(1, (int)((220 * 1024) / (k4_smem_tma + 1024)));
-        if (dealt_bps > 0) k4_tma_blocks_per_sm = dealt_bps;
-        if (const char* b = getenv("RBA_MATVEC_BLOCKS_PER_SM")) k4_tma_blocks_per_sm = std::max(1, atoi(b));
-      }
-    }
-#undef TRY
-    CU(cudaStreamSynchronize(stream));
+    CU(cudaMallocHost((void**)&h_res, sizeof(PinnedResults)));
     return RBA_OK;
   }
-  static constexpr int K4_WARPS = 4;
-  static constexpr int IMP_WARPS = 2, IMP_MAXSLOTS = 64, IMP_NS = RBA_IMP_NS;  // streamed implicit operator: warps per block, slots per stage, stages per warp
-#ifndef RBA_K4_NS
-#define RBA_K4_NS 2
-#endif
-#ifndef RBA_K4_STAGE
-#define RBA_K4_STAGE 4608
-#endif
-  static constexpr int K4_NS = RBA_K4_NS;        // TMA ring stages per warp
-  static constexpr int K4_STAGE = RBA_K4_STAGE;  // bytes per stage (2 rows of an f32 KP=9 tile)
-  static constexpr int TILE_WARPS = 4;
-  static constexpr int K1_CAP = 3904;   // scalars of shared memory per warp: linearize+QR needs 60 * W * n + 64 (= 3904 for the standard tiles)
-  static constexpr int K2_CAP = 3072;   // stage 2 needs 3 * W * CS + 9 * W * n + 20 W + 8 (<= 3048 for the standard tiles)
-  Scratch<S> k1_sc{}, k2_sc{};
-  size_t k1_smem = 0, k2_smem = 0;
-  int k1_bps = 2, k2_bps = 2, k1_max_blocks = 264, k2_max_blocks = 264;
-  size_t k4_smem_small = 0, k4_smem_tma = 0;
-  bool use_tma = true;
-  int k4_tma_blocks_per_sm = 2;
+
+  int setup_kernels() {
+    if (k1_sc.gstride) TRY(dalloc(&k1_sc.gbase, (size_t)(k1_max_blocks * TILE_WARPS) * k1_sc.gstride, false));
+    if (k2_sc.gstride) TRY(dalloc(&k2_sc.gbase, (size_t)(k2_max_blocks * TILE_WARPS) * k2_sc.gstride, false));
+    CU(cudaFuncSetAttribute((k_linearize_qr<S, false>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)k1_smem));
+    CU(cudaFuncSetAttribute((k_linearize_qr<S, true>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)k1_smem));
+    CU(cudaFuncSetAttribute((k_stage2<S, true>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)k2_smem));
+    CU(cudaFuncSetAttribute((k_stage2<S, false>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)k2_smem));
+    k4_smem_small = (size_t)K4_WARPS * L.k4_scratch_per_warp * sizeof(S);
+    if (k4_smem_small > 200 * 1024) { g_err = "matvec scratch exceeds shared memory"; return RBA_ERR_UNSUPPORTED; }
+    CU(cudaFuncSetAttribute((k_matvec_large<S, K4_WARPS, KPMAX>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(k4_smem_small, 1024)));
+    // the PCG vector step runs on one thread-block cluster (16 CTAs if the device grants it, else 8, ...)
+    CU(cudaFuncSetAttribute(k_pcg_vec<S>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+    CU(cudaFuncSetAttribute((k_pcg_vec<S, true>), cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+    CU(cudaFuncSetAttribute(k_power_vec<S>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+    for (; pcg_cluster > 1; pcg_cluster >>= 1) {
+      cudaLaunchConfig_t cfg = {};
+      cfg.gridDim = dim3(pcg_cluster); cfg.blockDim = dim3(VEC_THREADS);
+      cudaLaunchAttribute at[1];
+      at[0].id = cudaLaunchAttributeClusterDimension;
+      at[0].val.clusterDim.x = pcg_cluster; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
+      cfg.attrs = at; cfg.numAttrs = 1;
+      int ncl = 0;
+      if (cudaOccupancyMaxActiveClusters(&ncl, k_pcg_vec<S>, &cfg) == cudaSuccess && ncl >= 1) break;
+      cudaGetLastError();
+    }
+    return RBA_OK;
+  }
 
   // ------------------------------------------------------------------------------------------
   // sum over the shards, in place, on the solver stream: peer-memory push exchange when the ranks have mapped each other's
@@ -530,7 +545,7 @@ struct Solver : rba_handle {
   int ipc_import(const void* all) override {
     if (opt.nranks == 1) return RBA_OK;
     if (opt.nranks > MAX_PEERS) { g_err = "the peer-memory exchange supports at most 8 ranks"; return RBA_ERR_UNSUPPORTED; }
-    if (const char* e = getenv("RBA_PEER_AR")) if (atoi(e) == 0) return RBA_OK;
+    if (!peer_ar) return RBA_OK;  // test hook (read_test_hooks): NCCL
     CU(cudaSetDevice(device));
     for (int r = 0; r < opt.nranks; ++r) {
       if (r == opt.rank) continue;
@@ -674,41 +689,6 @@ struct Solver : rba_handle {
     ++launches;
     return RBA_OK;
   }
-  TileOrder order_k1{nullptr, 0}, order_kp{nullptr, 0};
-  // longest-processing-time-first lists of tiles for nw persistent warps, laid out so that position k * nw + w is the k-th
-  // tile of warp w (-1 = end of the warp's list)
-  int deal_tiles(int nw, TileOrder& out) {
-    const int nt = (int)L.tiles.size();
-    if (nt <= nw) return RBA_OK;  // at most one tile per warp: nothing to balance
-    std::vector<int> idx(nt);
-    std::vector<long long> cost(nt);
-    for (int t = 0; t < nt; ++t) {
-      idx[t] = t;
-      const TileInfo& T = L.tiles[t];
-      cost[t] = (long long)2 * T.n * T.KP + (long long)(32 / T.G) * T.n / 2 + 8;  // panel rows x column steps + per-observation work + constant
-    }
-    std::stable_sort(idx.begin(), idx.end(), [&](int a, int b) { return cost[a] > cost[b]; });
-    std::vector<std::vector<int>> lists(nw);
-    std::vector<std::pair<long long, int>> heap(nw);
-    for (int w = 0; w < nw; ++w) heap[w] = {0, w};
-    auto cmp = [](const std::pair<long long, int>& a, const std::pair<long long, int>& b) { return a > b; };
-    std::make_heap(heap.begin(), heap.end(), cmp);
-    for (int t : idx) {
-      std::pop_heap(heap.begin(), heap.end(), cmp);
-      heap.back().first += cost[t];
-      lists[heap.back().second].push_back(t);
-      std::push_heap(heap.begin(), heap.end(), cmp);
-    }
-    size_t maxlen = 0;
-    for (auto& l : lists) maxlen = std::max(maxlen, l.size());
-    std::vector<int> order(maxlen * nw, -1);
-    for (int w = 0; w < nw; ++w)
-      for (size_t k = 0; k < lists[w].size(); ++k) order[k * nw + w] = lists[w][k];
-    int* d = nullptr;
-    int rc = upload(&d, order); if (rc) return rc;
-    out.order = d; out.count = (int)order.size();
-    return RBA_OK;
-  }
   int tile_grid(int max_blocks) const { return std::max(1, std::min(max_blocks, (D.ntiles + TILE_WARPS - 1) / TILE_WARPS)); }
   int grid_for(long long work_items, int per_block, int blocks_per_sm) const {
     long long g = (work_items + per_block - 1) / per_block;
@@ -717,10 +697,10 @@ struct Solver : rba_handle {
   }
 
   // deterministic per-camera sum of yobs[slot][9] over a CSR -> dst[9 nc] (+ all-reduce across shards)
-  int camera_reduce(const int* slots, const ReduceItem* items, int nitems, const int* item_ptr, S* dst, const int* done,
+  int camera_reduce(const int* slots, const ReduceItem* items, int nitems, const int* item_ptr, S* dst,
                     const S* addend = nullptr, bool reduce_ranks = true) {
-    k_cam_reduce<S><<<grid_for(nitems, 8, 8), 256, 0, stream>>>(D.yobs, slots, items, nitems, D.partial, done, 0);
-    k_cam_final9<S><<<(9 * nc + 255) / 256, 256, 0, stream>>>(D.partial, item_ptr, nc, dst, done, addend);
+    k_cam_reduce<S><<<grid_for(nitems, 8, 8), 256, 0, stream>>>(D.yobs, slots, items, nitems, D.partial, nullptr, 0);
+    k_cam_final9<S><<<(9 * nc + 255) / 256, 256, 0, stream>>>(D.partial, item_ptr, nc, dst, addend);
     launches += 2;
     return reduce_ranks ? allreduce(dst, (size_t)9 * nc) : RBA_OK;
   }
@@ -730,8 +710,6 @@ struct Solver : rba_handle {
   // Every entry point is split into an enqueue half (kernels + asynchronous copies into its OWN pinned slot) and a finish
   // half (after a stream synchronisation): the public calls are enqueue + synchronise + finish, rba_lm_step strings the
   // enqueue halves of a whole LM inner iteration together and synchronises once.
-  // pinned slots: h_red + 8 * slot, h_flags + 4 * slot;  slot 0 compute_error, 1 linearize, 2 apply
-  bool error_enqueued = false;
   int compute_error_enqueue() {
     error_enqueued = false;
     if (error_cache_valid && error_cache_version == state_version) return RBA_OK;  // answered from the cache in finish
@@ -745,8 +723,8 @@ struct Solver : rba_handle {
       k_prior_cost<S><<<1, 256, 0, stream>>>(D.cams, d_prior_mean, d_prior_L, nc, d_red, d_flags);
       ++launches;
     }
-    CU(cudaMemcpyAsync(h_red, d_red, 6 * sizeof(double), cudaMemcpyDeviceToHost, stream));
-    CU(cudaMemcpyAsync(h_flags, d_flags, 4 * sizeof(int), cudaMemcpyDeviceToHost, stream));
+    CU(cudaMemcpyAsync(h_res->error, d_red, sizeof(h_res->error), cudaMemcpyDeviceToHost, stream));
+    CU(cudaMemcpyAsync(h_res->error_flags, d_flags, sizeof(h_res->error_flags), cudaMemcpyDeviceToHost, stream));
     rc = stop(ev_error); if (rc) return rc;
     error_enqueued = true;
     error_enqueue_version = state_version;
@@ -761,10 +739,11 @@ struct Solver : rba_handle {
       tm.residual_evaluation_time = 0.0;
       return RBA_OK;
     }
-    out->all_num_obs = (int64_t)llround(h_red[0]); out->all_error = h_red[1]; out->all_residual_sum = h_red[2];
-    out->valid_num_obs = (int64_t)llround(h_red[3]); out->valid_error = h_red[4]; out->valid_residual_sum = h_red[5];
-    if (h_flags[1]) { g_err = "a peer rank did not take part in a cross-shard reduction in time (peer-memory exchange timed out)"; return RBA_ERR_NCCL; }
-    out->is_numerically_valid = h_flags[0] ? 0 : 1;
+    const double* e = h_res->error;
+    out->all_num_obs = (int64_t)llround(e[0]); out->all_error = e[1]; out->all_residual_sum = e[2];
+    out->valid_num_obs = (int64_t)llround(e[3]); out->valid_error = e[4]; out->valid_residual_sum = e[5];
+    if (h_res->error_flags[1]) { g_err = "a peer rank did not take part in a cross-shard reduction in time (peer-memory exchange timed out)"; return RBA_ERR_NCCL; }
+    out->is_numerically_valid = h_res->error_flags[0] ? 0 : 1;
     out->pad_ = 0;
     tm.residual_evaluation_time = elapsed(ev_error);
     error_cache = *out; error_cache_version = error_enqueue_version; error_cache_valid = true;
@@ -777,7 +756,6 @@ struct Solver : rba_handle {
   }
 
   // ref: solver/linearizor_qr.cpp:78-138 (staged: LinearizationQR::get_stage1, linearization_qr.hpp:634-712)
-  long long lin_l0 = 0;
   int linearize_enqueue() {
     lin_l0 = launches;
     int rc = start(ev_stage1); if (rc) return rc;
@@ -785,7 +763,7 @@ struct Solver : rba_handle {
     // pass A: squared column norms of the weighted pose Jacobians -> pose_jacobian_scaling_
     k_jp_norms<S><<<grid_for(L.nslots, 256, 8), 256, 0, stream>>>(D, ko, d_flags);
     ++launches;
-    rc = camera_reduce(d_csr_obs_slots, d_csr_obs_items, n_obs_items, d_csr_obs_item_ptr, D.diag2, nullptr); if (rc) return rc;
+    rc = camera_reduce(d_csr_obs_slots, d_csr_obs_items, n_obs_items, d_csr_obs_item_ptr, D.diag2); if (rc) return rc;
     if (D.prior_H) {  // prior Jacobian and its column norms (scaling from the whole Jacobian), after the sum over the shards
       k_prior_linearize<S><<<(nc + 127) / 128, 128, 0, stream>>>(D.cams, d_prior_mean, d_prior_L, nc, D.diag2, d_prior_A, d_prior_r);
       ++launches;
@@ -813,11 +791,11 @@ struct Solver : rba_handle {
       const int want_blocks = opt.preconditioner_type == 1 ? 1 : 0;
       k_panel_grad_blocks<S><<<tile_grid(sm_count * 8), TILE_WARPS * 32, 0, stream>>>(D, want_blocks, order_kp);
       ++launches;
-      rc = camera_reduce(d_csr_obs_slots, d_csr_obs_items, n_obs_items, d_csr_obs_item_ptr, D.b0, nullptr, nullptr, false); if (rc) return rc;
+      rc = camera_reduce(d_csr_obs_slots, d_csr_obs_items, n_obs_items, d_csr_obs_item_ptr, D.b0, nullptr, false); if (rc) return rc;
       if (want_blocks) { rc = precond_blocks(3, D.blocks0, nullptr, false); if (rc) return rc; }
     }
     rc = allreduce_scalars(0); if (rc) return rc;
-    CU(cudaMemcpyAsync(h_flags + 4, d_flags, 4 * sizeof(int), cudaMemcpyDeviceToHost, stream));
+    CU(cudaMemcpyAsync(h_res->linearize_flags, d_flags, sizeof(h_res->linearize_flags), cudaMemcpyDeviceToHost, stream));
     rc = stop(ev_stage1); if (rc) return rc;
     linearized = true;  // provisional: linearize_finish withdraws it on a numerical failure
     new_linearization_point = true;
@@ -829,8 +807,8 @@ struct Solver : rba_handle {
     CU(cudaGetLastError());
     tm.stage1_time = elapsed(ev_stage1);
     tm.kernel_launches = launches - lin_l0;
-    if (h_flags[4 + 1]) { linearized = false; g_err = "a peer rank did not take part in a cross-shard reduction in time (peer-memory exchange timed out)"; return RBA_ERR_NCCL; }
-    if (h_flags[4 + 0]) { linearized = false; return RBA_NUMERICAL_FAILURE; }  // reference: CHECK abort (linearizor_qr.cpp:121-122)
+    if (h_res->linearize_flags[1]) { linearized = false; g_err = "a peer rank did not take part in a cross-shard reduction in time (peer-memory exchange timed out)"; return RBA_ERR_NCCL; }
+    if (h_res->linearize_flags[0]) { linearized = false; return RBA_NUMERICAL_FAILURE; }  // reference: CHECK abort (linearizor_qr.cpp:121-122)
     return RBA_OK;
   }
   int linearize() override {
@@ -853,53 +831,48 @@ struct Solver : rba_handle {
     return reduce_ranks ? allreduce(dst, (size_t)81 * nc) : RBA_OK;
   }
 
-  // operator part of one matvec: yobs = P^T P x_red for every landmark, then per-camera sums -> D.partial
   // one complete operator application outside PCG: y = sum over the landmarks of P^T P x_red (this shard), per camera in D.y
-  void matvec_launch(const S* xvec, const int* done) {
-    matvec_kernels(xvec, done);
-    k_cam_reduce_final<S, false><<<grid_for(n_op_items, 8, 8), 256, 0, stream>>>((const S*)D.yobs, op_slots, op_items, n_op_items, op_item_ptr, D.partial,
-                                                                               d_cam_cnt, D.y, done, 0, pc, 0, nc);
-    ++launches;
+  int matvec_launch(const S* xvec) {
+    matvec_kernels(xvec, nullptr, false);
+    return cam_reduce_final(false, 0, false);
   }
-  void matvec_kernels(const S* xvec, const int* done, bool pdl = false) {
+  // operator part of one matvec: yobs = P^T P x_red for every landmark (e0_only: the implicit operator's E_0 x alone)
+  void matvec_kernels(const S* xvec, const int* done, bool pdl, int e0_only = 0) {
     if (implicit_op) {
       const int ntl = (int)L.tiles.size();
-      const bool p = pdl && use_pdl && imp_tile_split == ntl;  // a single kernel between the PCG vector step and the reduction
-      if (imp_tile_split > 0 && use_tma)
-        launch_ex((k_matvec_implicit_tma<S, IMP_WARPS, IMP_MAXSLOTS, IMP_NS>), imp_grid, IMP_WARPS * 32, imp_smem, p, 1, D, imp_tile_split, xvec, done, (int)p, e0_only_flag);
-      const int tb = use_tma ? imp_tile_split : 0;
-      if (tb < ntl)
-        launch_ex(k_matvec_implicit<S>, (ntl - tb + TILE_WARPS - 1) / TILE_WARPS, TILE_WARPS * 32, 0, false, 1, D, tb, xvec, done, 0, e0_only_flag);
+      const bool p = pdl && imp_tile_split == ntl;  // a single kernel between the PCG vector step and the reduction
+      if (imp_tile_split > 0)
+        launch_ex((k_matvec_implicit_tma<S, IMP_WARPS, IMP_MAXSLOTS, IMP_NS>), imp_grid, IMP_WARPS * 32, imp_smem, p, 1, D, imp_tile_split, xvec, done, (int)p, e0_only);
+      if (imp_tile_split < ntl)
+        launch_ex(k_matvec_implicit<S>, (ntl - imp_tile_split + TILE_WARPS - 1) / TILE_WARPS, TILE_WARPS * 32, 0, false, 1, D, imp_tile_split, xvec, done, 0, e0_only);
       ++tm.matvec_launches;
       return;
     }
-    const int nitems = n_dealt;
     if (L.n_items_large > 0) {
       k_matvec_large<S, K4_WARPS, KPMAX><<<grid_for(L.n_items_large, K4_WARPS, 4), K4_WARPS * 32, k4_smem_small, stream>>>(
           D, d_items, 0, L.n_items_large, L.k4_scratch_per_warp, xvec, done);
       ++launches;
     }
-    if (nitems > L.n_items_large) {
-      if (use_tma) {
-        launch_ex(k_matvec_small_tma<S, K4_WARPS, K4_NS, K4_STAGE>, dealt_grid > 0 ? dealt_grid : grid_for(nitems - L.n_items_large, K4_WARPS, k4_tma_blocks_per_sm), K4_WARPS * 32,
-                  k4_smem_tma, pdl && use_pdl && L.n_items_large == 0, 1, D, (const MatvecItem*)d_items, L.n_items_large, nitems, L.k4_scratch_per_warp, xvec, done,
-                  (int)(pdl && use_pdl && L.n_items_large == 0));
-        --launches;
-      } else
-        k_matvec_small<S, K4_WARPS><<<grid_for(nitems - L.n_items_large, K4_WARPS, 5), K4_WARPS * 32, k4_smem_small, stream>>>(
-            D, d_items, L.n_items_large, nitems, L.k4_scratch_per_warp, xvec, done);
-      ++launches;
+    if (n_dealt > L.n_items_large) {
+      const bool p = pdl && L.n_items_large == 0;
+      launch_ex(k_matvec_small_tma<S, K4_WARPS, K4_NS, K4_STAGE>, tma_grid, K4_WARPS * 32, K4_SMEM_TMA, p, 1, D, (const MatvecItem*)d_items,
+                L.n_items_large, n_dealt, L.k4_scratch_per_warp, xvec, done, (int)p);
     }
     ++tm.matvec_launches;
+  }
+  // per-camera sums of the operator output into D.y (peers: into every rank's staging area of the peer exchange).  Inside a
+  // solve it is launched dependent on its predecessor and returns at once when the solve has ended.
+  int cam_reduce_final(bool peers, int seq, bool in_solve) {
+    auto kern = peers ? k_cam_reduce_final<S, true> : k_cam_reduce_final<S, false>;
+    return launch_ex(kern, grid_for(n_op_items, 8, 8), 256, 0, in_solve, 1, (const S*)D.yobs, op_slots, op_items, n_op_items, op_item_ptr,
+                     D.partial, d_cam_cnt, D.y, in_solve ? (const int*)&d_state->done : nullptr, (int)in_solve, pc, seq, nc);
   }
   int pcg_vec(int i, int mode, bool pdl, int is_last, S lambda, bool fused_ar = false, bool from_partials = false) {
     PeerComm c = pc;
     if (!fused_ar) c.nranks = 1;
-    if (D.prior_H)
-      return launch_ex(k_pcg_vec<S, true>, pcg_cluster, VEC_THREADS, 0, pdl && use_pdl, pcg_cluster, D, d_state, lambda, i, mode, (double)opt.eta,
-                       (int)opt.min_linear_solver_iterations, is_last, (int)(pdl && use_pdl), c, ar_seq, from_partials ? op_item_ptr : (const int*)nullptr, d_prog);
-    return launch_ex(k_pcg_vec<S>, pcg_cluster, VEC_THREADS, 0, pdl && use_pdl, pcg_cluster, D, d_state, lambda, i, mode, (double)opt.eta,
-                     (int)opt.min_linear_solver_iterations, is_last, (int)(pdl && use_pdl), c, ar_seq, from_partials ? op_item_ptr : (const int*)nullptr, d_prog);
+    auto kern = D.prior_H ? k_pcg_vec<S, true> : k_pcg_vec<S, false>;
+    return launch_ex(kern, pcg_cluster, VEC_THREADS, 0, pdl, pcg_cluster, D, d_state, lambda, i, mode, (double)opt.eta,
+                     (int)opt.min_linear_solver_iterations, is_last, (int)pdl, c, ar_seq, from_partials ? op_item_ptr : (const int*)nullptr, d_prog);
   }
   // The hand-over through per-segment sums is taken when a cluster CTA's share of the cameras fits the vector kernel's
   // register-resident layout (9 ceil(nc / cluster) <= VEC_THREADS VEC_EPT: <= 1808 cameras with a 16-CTA cluster, <= 904
@@ -914,9 +887,8 @@ struct Solver : rba_handle {
     if (pcg_from_partials()) {
       // one GPU: the vector kernel adds the per-segment sums itself (same order as k_cam_reduce_final's last arriver:
       // bit-identical) -- no arrival counters, fences or second pass in the reduction
-      int rc = launch_ex(k_cam_reduce<S>, grid_for(n_op_items, 8, 8), 256, 0, use_pdl, 1, (const S*)D.yobs, op_slots, op_items, n_op_items, D.partial,
-                         (const int*)&d_state->done, (int)use_pdl);
-      if (rc) return rc;
+      TRY(launch_ex(k_cam_reduce<S>, grid_for(n_op_items, 8, 8), 256, 0, true, 1, (const S*)D.yobs, op_slots, op_items, n_op_items, D.partial,
+                    (const int*)&d_state->done, 1));
       return pcg_vec(i, mode, true, is_last, lambda, false, true);
     }
     const bool fused = opt.nranks > 1 && peer_ok;
@@ -924,46 +896,21 @@ struct Solver : rba_handle {
     // NCCL path: k_cam_reduce_final writes y only for cameras that have observations in this shard; D.y is all-reduced IN
     // PLACE, so without this the other cameras would carry the previous iteration's global sum into the next all-reduce
     if (opt.nranks > 1 && !fused) CU(cudaMemsetAsync(D.y, 0, (size_t)9 * nc * sizeof(S), stream));
-    int rc = fused ? launch_ex((k_cam_reduce_final<S, true>), grid_for(n_op_items, 8, 8), 256, 0, use_pdl, 1, (const S*)D.yobs, op_slots,
-                               op_items, n_op_items, op_item_ptr, D.partial, d_cam_cnt, D.y, (const int*)&d_state->done, (int)use_pdl, pc, ar_seq, nc)
-                   : launch_ex((k_cam_reduce_final<S, false>), grid_for(n_op_items, 8, 8), 256, 0, use_pdl, 1, (const S*)D.yobs, op_slots,
-                               op_items, n_op_items, op_item_ptr, D.partial, d_cam_cnt, D.y, (const int*)&d_state->done, (int)use_pdl, pc, ar_seq, nc);
-    if (rc) return rc;
+    TRY(cam_reduce_final(fused, ar_seq, true));
     if (opt.nranks == 1) return pcg_vec(i, mode, true, is_last, lambda);
     if (fused) return pcg_vec(i, mode, true, is_last, lambda, true);
-    rc = allreduce(D.y, (size_t)9 * nc); if (rc) return rc;
+    TRY(allreduce(D.y, (size_t)9 * nc));
     return pcg_vec(i, mode, false, is_last, lambda);
   }
-  // q_out = H vec = sum + lambda vec ; optional partial p.q
-  int matvec_finish(const S* vec, S* out, S lambda, PcgState* st, double* part) {
-    int rc = allreduce(D.y, (size_t)9 * nc); if (rc) return rc;  // no-op on one GPU
-    k_pcg_q<S><<<NPART, 128, 0, stream>>>(D, st, nullptr, nullptr, D.y, vec, out, lambda, part);
-    ++launches;
-    return RBA_OK;
-  }
-
-  // ref: solver/linearizor_qr.cpp:140-265
-  // Power-series solve of the reduced camera system (ref: sc/linearization_power_sc.hpp:130-160, driven by
-  // solver/linearizor_power_sc.cpp:140-160 with q_tolerance = eta): per term one E_0 application (the implicit operator
-  // kernels with e0_only), the per-camera reduction and k_power_vec; the device convergence flag is polled like in PCG.
-  int power_enqueue(void* inc_out) {
-    int rc = start(ev_pcg); if (rc) return rc;
-    CU(cudaMemsetAsync(d_state, 0, sizeof(PcgState), stream));
-    const int order = opt.power_order, chk = opt.pcg_check_period;
-    rc = launch_ex(k_power_vec<S>, pcg_cluster, VEC_THREADS, 0, false, pcg_cluster, D, d_state, 0, (double)opt.eta, 0, 0); if (rc) return rc;
-    e0_only_flag = 1;
+  // Enqueue iterations 1..last in chunks of `chunk` (enqueue(i)); after each chunk the PcgState is copied into one of two
+  // pinned slots, and the host waits for the copy of the chunk before and stops once it shows the solve ended.
+  template <class F>
+  int enqueue_polled(int last, int chunk, F&& enqueue) {
     int i = 1, pending[2] = {0, 0}, slot = 0;
     bool finished = false;
-    while (i <= order && !finished) {
-      const int chunk_end = std::min(i + chk - 1, order);
-      for (; i <= chunk_end; ++i) {
-        matvec_kernels(D.p, &d_state->done, true);
-        rc = launch_ex((k_cam_reduce_final<S, false>), grid_for(n_op_items, 8, 8), 256, 0, use_pdl, 1, (const S*)D.yobs, op_slots, op_items,
-                       n_op_items, op_item_ptr, D.partial, d_cam_cnt, D.y, (const int*)&d_state->done, (int)use_pdl, pc, 0, nc);
-        if (rc) { e0_only_flag = 0; return rc; }
-        rc = launch_ex(k_power_vec<S>, pcg_cluster, VEC_THREADS, 0, use_pdl, pcg_cluster, D, d_state, i, (double)opt.eta, (int)(i == order), (int)use_pdl);
-        if (rc) { e0_only_flag = 0; return rc; }
-      }
+    while (i <= last && !finished) {
+      const int chunk_end = std::min(i + chunk - 1, last);
+      for (; i <= chunk_end; ++i) TRY(enqueue(i));
       CU(cudaMemcpyAsync(&h_state[slot], d_state, sizeof(PcgState), cudaMemcpyDeviceToHost, stream));
       CU(cudaEventRecord(poll_ev[slot], stream));
       pending[slot] = 1;
@@ -975,16 +922,31 @@ struct Solver : rba_handle {
       }
       slot = other;
     }
-    e0_only_flag = 0;
+    return RBA_OK;
+  }
+
+  // ref: solver/linearizor_qr.cpp:140-265
+  // Power-series solve of the reduced camera system (ref: sc/linearization_power_sc.hpp:130-160, driven by
+  // solver/linearizor_power_sc.cpp:140-160 with q_tolerance = eta): per term one E_0 application (the implicit operator
+  // kernels with e0_only), the per-camera reduction and k_power_vec; the device convergence flag is polled like in PCG.
+  int power_enqueue(void* inc_out) {
+    TRY(start(ev_pcg));
+    CU(cudaMemsetAsync(d_state, 0, sizeof(PcgState), stream));
+    const int order = opt.power_order;
+    TRY(launch_ex(k_power_vec<S>, pcg_cluster, VEC_THREADS, 0, false, pcg_cluster, D, d_state, 0, (double)opt.eta, 0, 0));
+    TRY(enqueue_polled(order, opt.pcg_check_period, [&](int i) -> int {
+      matvec_kernels(D.p, &d_state->done, true, 1);
+      TRY(cam_reduce_final(false, 0, true));
+      return launch_ex(k_power_vec<S>, pcg_cluster, VEC_THREADS, 0, true, pcg_cluster, D, d_state, i, (double)opt.eta, (int)(i == order), 1);
+    }));
     CU(cudaMemcpyAsync(&h_state[0], d_state, sizeof(PcgState), cudaMemcpyDeviceToHost, stream));
     if (inc_out) CU(cudaMemcpyAsync(inc_out, D.inc, (size_t)9 * nc * sizeof(S), cudaMemcpyDeviceToHost, stream));
-    rc = stop(ev_pcg); if (rc) return rc;
+    TRY(stop(ev_pcg));
     have_inc = true;
     new_linearization_point = false;
     return RBA_OK;
   }
 
-  long long solve_l0 = 0;
   int solve_enqueue(double lambda_d, void* inc_out) {
     if (!linearized) { g_err = "rba_solve called before a successful rba_linearize"; return RBA_ERR_STATE; }
     const S lambda = (S)lambda_d;
@@ -999,7 +961,7 @@ struct Solver : rba_handle {
     } else if (panel_form) k_stage2<S, true><<<tile_grid(k2_max_blocks), TILE_WARPS * 32, k2_smem, stream>>>(D, lambda, k2_sc, ko.write_panel);
     else k_stage2<S, false><<<tile_grid(k2_max_blocks), TILE_WARPS * 32, k2_smem, stream>>>(D, lambda, k2_sc, ko.write_panel);
     ++launches;
-    rc = camera_reduce(d_csr_obs_slots, d_csr_obs_items, n_obs_items, d_csr_obs_item_ptr, D.b, nullptr, panel_form ? D.b0 : nullptr); if (rc) return rc;
+    rc = camera_reduce(d_csr_obs_slots, d_csr_obs_items, n_obs_items, d_csr_obs_item_ptr, D.b, panel_form ? D.b0 : nullptr); if (rc) return rc;
     const bool power = opt.solver_type == 2;
     const bool schur = opt.preconditioner_type == 1 && !power;  // Power-SC inverts Hpp = sum Jp^T Jp + lambda I instead
     if (schur) { rc = panel_form ? precond_blocks(2, D.blocks, D.blocks0, true) : precond_blocks(1, D.blocks, nullptr, true); if (rc) return rc; }
@@ -1063,22 +1025,7 @@ struct Solver : rba_handle {
     if (opt.nranks > 1 && !peer_ok) {
       // NCCL exchange: every rank must enqueue the SAME number of all-reduces, so the decision to stop may depend only on
       // the iteration count -- the flag is polled once per chunk of `depth` iterations, one chunk behind
-      int i = 1, pending[2] = {0, 0}, slot = 0;
-      bool finished = false;
-      while (i <= max_it && !finished) {
-        const int chunk_end = std::min(i + depth - 1, max_it);
-        for (; i <= chunk_end; ++i) { rc = enqueue_iteration(i); if (rc) return rc; }
-        CU(cudaMemcpyAsync(&h_state[slot], d_state, sizeof(PcgState), cudaMemcpyDeviceToHost, stream));
-        CU(cudaEventRecord(poll_ev[slot], stream));
-        pending[slot] = 1;
-        const int other = slot ^ 1;
-        if (pending[other]) {
-          CU(cudaEventSynchronize(poll_ev[other]));
-          pending[other] = 0;
-          if (h_state[other].done) finished = true;
-        }
-        slot = other;
-      }
+      TRY(enqueue_polled(max_it, depth, enqueue_iteration));
     } else {
       volatile int* prog = h_prog;
       for (int i = 1; i <= max_it; ++i) {
@@ -1123,7 +1070,6 @@ struct Solver : rba_handle {
   }
 
   // ref: solver/linearizor_qr.cpp:267-291
-  long long apply_l0 = 0;
   int apply_enqueue(const void* inc_host, bool update_cameras) {
     if (!linearized || !damping_valid) { g_err = "rba_apply / rba_back_substitute need rba_linearize + rba_solve first"; return RBA_ERR_STATE; }
     apply_l0 = launches;
@@ -1155,8 +1101,8 @@ struct Solver : rba_handle {
       ++launches;
     }
     rc = stop(ev_update); if (rc) return rc;
-    CU(cudaMemcpyAsync(h_red + 16, d_red, sizeof(double), cudaMemcpyDeviceToHost, stream));
-    CU(cudaMemcpyAsync(h_flags + 8, d_flags, 4 * sizeof(int), cudaMemcpyDeviceToHost, stream));
+    CU(cudaMemcpyAsync(&h_res->l_diff, d_red, sizeof(double), cudaMemcpyDeviceToHost, stream));
+    CU(cudaMemcpyAsync(h_res->apply_flags, d_flags, sizeof(h_res->apply_flags), cudaMemcpyDeviceToHost, stream));
     return RBA_OK;
   }
   int apply_finish(void* l_diff_out) {
@@ -1164,10 +1110,10 @@ struct Solver : rba_handle {
     tm.back_substitution_time = elapsed(ev_backsub);
     tm.update_cameras_time = elapsed(ev_update);
     tm.kernel_launches = launches - apply_l0;
-    if (h_flags[8 + 1]) { g_err = "a peer rank did not take part in a cross-shard reduction in time (peer-memory exchange timed out)"; return RBA_ERR_NCCL; }
-    S l = (S)h_red[16];
+    if (h_res->apply_flags[1]) { g_err = "a peer rank did not take part in a cross-shard reduction in time (peer-memory exchange timed out)"; return RBA_ERR_NCCL; }
+    S l = (S)h_res->l_diff;
     int ret = RBA_OK;
-    if (h_flags[8 + 0] || !std::isfinite((double)l)) { l = std::numeric_limits<S>::quiet_NaN(); ret = RBA_NUMERICAL_FAILURE; }
+    if (h_res->apply_flags[0] || !std::isfinite((double)l)) { l = std::numeric_limits<S>::quiet_NaN(); ret = RBA_NUMERICAL_FAILURE; }
     *(S*)l_diff_out = l;
     return ret;
   }
@@ -1327,8 +1273,10 @@ struct Solver : rba_handle {
     if (!linearized || !damping_valid) { g_err = "rba_right_multiply needs rba_linearize + rba_solve first"; return RBA_ERR_STATE; }
     CU(cudaMemcpyAsync(D.z, x, (size_t)9 * nc * sizeof(S), cudaMemcpyHostToDevice, stream));
     CU(cudaMemsetAsync(D.y, 0, (size_t)9 * nc * sizeof(S), stream));  // cameras without observations in this shard are not written
-    matvec_launch(D.z, nullptr);
-    int rc = matvec_finish(D.z, D.y, last_lambda, nullptr, nullptr); if (rc) return rc;
+    TRY(matvec_launch(D.z));
+    TRY(allreduce(D.y, (size_t)9 * nc));  // no-op on one GPU
+    k_pcg_q<S><<<NPART, 128, 0, stream>>>(D, D.y, D.z, D.y, last_lambda);
+    ++launches;
     CU(cudaMemcpyAsync(y, D.y, (size_t)9 * nc * sizeof(S), cudaMemcpyDeviceToHost, stream));
     CU(cudaStreamSynchronize(stream));
     CU(cudaGetLastError());
@@ -1337,10 +1285,10 @@ struct Solver : rba_handle {
 
   int time_matvec(int reps, double* sec) override {
     if (!linearized || !damping_valid) { g_err = "rba_time_matvec needs rba_linearize + rba_solve first"; return RBA_ERR_STATE; }
-    matvec_launch(D.p, nullptr);  // warm-up
-    int rc = start(ev_mv); if (rc) return rc;
-    for (int r = 0; r < reps; ++r) matvec_launch(D.p, nullptr);
-    rc = stop(ev_mv); if (rc) return rc;
+    TRY(matvec_launch(D.p));  // warm-up
+    TRY(start(ev_mv));
+    for (int r = 0; r < reps; ++r) TRY(matvec_launch(D.p));
+    TRY(stop(ev_mv));
     CU(cudaStreamSynchronize(stream));
     CU(cudaGetLastError());
     *sec = elapsed(ev_mv) / std::max(reps, 1);
