@@ -1164,7 +1164,7 @@ __global__ void __launch_bounds__(128) k_stage2(DevPtrs<S> D, S lambda, Scratch<
 //   One warp per tile, G lanes per landmark, lane per observation.
 // ------------------------------------------------------------------------------------------------
 template <class S>
-__global__ void __launch_bounds__(128) k_sc_stage2(DevPtrs<S> D, S lambda, int* bad_flag) {
+__global__ void __launch_bounds__(128) k_sc_stage2(DevPtrs<S> D, S lambda) {
   const int wib = threadIdx.x >> 5, lane = threadIdx.x & 31;
   for (int t = blockIdx.x * (blockDim.x >> 5) + wib; t < D.ntiles; t += gridDim.x * (blockDim.x >> 5)) {
     const TileInfo T = D.tiles[t];
@@ -1188,7 +1188,9 @@ __global__ void __launch_bounds__(128) k_sc_stage2(DevPtrs<S> D, S lambda, int* 
 #pragma unroll
     for (int k = 0; k < 3; ++k) gv[k] = group_sum(gv[k], G);
     h[0] += lambda; h[3] += lambda; h[5] += lambda;  // landmark damping: Hll = Jl^T Jl + lambda I (sc/landmark_block.hpp:244-247)
-    // Cholesky Hll = R^T R
+    // Cholesky Hll = R^T R.  A block that is singular in working precision (one valid observation, lam below the resolution
+    // of its diagonal) gives a NaN pivot; it reaches b, PCG and the l_diff of rba_apply, which reports it (as the reference,
+    // whose Hll.inverse() feeds inf / NaN into CG), so no flag is raised here.
     const S r00 = sqrt(h[0]);
     const S r01 = h[1] / r00, r02 = h[2] / r00;
     const S r11 = sqrt(h[3] - r01 * r01);
@@ -1198,7 +1200,6 @@ __global__ void __launch_bounds__(128) k_sc_stage2(DevPtrs<S> D, S lambda, int* 
     const S rr1 = (gv[1] - r01 * rr0) / r11;
     const S rr2 = (gv[2] - r02 * rr0 - r12 * rr1) / r22;
     if (active && j == 0) {
-      if (!(finite_s(rr0) && finite_s(rr1) && finite_s(rr2) && r22 > S(0))) atomicOr(bad_flag, 1);
       S* lk = D.lmk + 24 * (size_t)(T.lm_base + g);
       lk[9] = r00; lk[10] = r01; lk[11] = r02; lk[12] = r11; lk[13] = r12; lk[14] = r22;
       lk[15] = rr0; lk[16] = rr1; lk[17] = rr2;

@@ -956,8 +956,7 @@ struct Solver : rba_handle {
     // stage 2: landmark damping + gradient (+ SCHUR_JACOBI blocks)
     if (opt.solver_type != 0) {
       // Schur-complement solvers: landmark eliminated through the normal equations (Cholesky of Jl^T Jl + lambda I)
-      CU(cudaMemsetAsync(d_flags, 0, 4 * sizeof(int), stream));
-      k_sc_stage2<S><<<tile_grid(sm_count * 8), TILE_WARPS * 32, 0, stream>>>(D, lambda, d_flags);
+      k_sc_stage2<S><<<tile_grid(sm_count * 8), TILE_WARPS * 32, 0, stream>>>(D, lambda);
     } else if (panel_form) k_stage2<S, true><<<tile_grid(k2_max_blocks), TILE_WARPS * 32, k2_smem, stream>>>(D, lambda, k2_sc, ko.write_panel);
     else k_stage2<S, false><<<tile_grid(k2_max_blocks), TILE_WARPS * 32, k2_smem, stream>>>(D, lambda, k2_sc, ko.write_panel);
     ++launches;
