@@ -2,7 +2,7 @@
 """Solve a BAL (or Bundler) problem with the square-root solver on one H100 and write the reference's ba_log.json.
 
     python examples/solve_bal.py problem-49-7776-pre.txt [--float] [--max-num-iterations 20] [--operator-form DENSE|IMPLICIT]
-        [--fix-intrinsics] [--fix-cameras I,J,...] [--camera-prior FILE.npz]
+        [--fix-intrinsics] [--fix-cameras I,J,...] [--camera-prior FILE.npz] [--camera-pair-prior FILE.npz]
 
 Mirrors what `bal_qr --input ...` of the reference does (src/app/bal_qr.cpp): load + normalise (bal_problem.cpp:773-852),
 optimize_lm_ours with the QR linearizor (solver/bal_bundle_adjustment.cpp:249-544), log (bal/ba_log.hpp)."""
@@ -33,6 +33,10 @@ def main():
     ap.add_argument("--camera-prior", default=None, metavar="FILE.npz",
                     help="Gaussian camera priors: arrays `mean` [nc, 10] (qx,qy,qz,qw, camera centre, f, k1, k2) and `sqrt_info` "
                          "[nc, 9, 9] in the coordinates of the loaded (normalised) problem (DESIGN.md section 14)")
+    ap.add_argument("--camera-pair-prior", default=None, metavar="FILE.npz",
+                    help="relative pose priors between pairs of cameras: arrays `pairs` [m, 2] (i, j), `mean` [m, 7] (qx,qy,qz,qw, t "
+                         "of T_i T_j^-1) and `sqrt_info` [m, 6, 6] in the coordinates of the loaded (normalised) problem "
+                         "(DESIGN.md section 15)")
     args = ap.parse_args()
     try:
         fix_cameras = [int(v) for v in args.fix_cameras.split(",")] if args.fix_cameras else []
@@ -59,6 +63,14 @@ def main():
                 problem.camera_prior = (f["mean"], f["sqrt_info"])
             except ValueError as e:
                 ap.error(f"--camera-prior: {e}")
+    if args.camera_pair_prior:
+        with np.load(args.camera_pair_prior) as f:
+            if "pairs" not in f or "mean" not in f or "sqrt_info" not in f:
+                ap.error(f"--camera-pair-prior: {args.camera_pair_prior} must hold the arrays `pairs`, `mean` and `sqrt_info`")
+            try:
+                problem.camera_pair_prior = (f["pairs"], f["mean"], f["sqrt_info"])
+            except ValueError as e:
+                ap.error(f"--camera-pair-prior: {e}")
     options = rb.SolverOptions(max_num_iterations=args.max_num_iterations, preconditioner_type=args.preconditioner_type,
                                operator_form=args.operator_form, use_double=not args.float)
     summary = rb.bundle_adjust_manual(problem, options, verbose=True)

@@ -90,7 +90,13 @@ struct DevPtrs {
   S* pblk;       // [csr_obs items][48] partial preconditioner blocks (45 used)
   int nc;
   const uint8_t* cam_fixed;  // [nc] RBA_FIX_* bits per camera (rba_set_camera_fixed), nullptr = every parameter free
-  const S* prior_H;          // [nc][81] A^T A of the scaled camera priors (rba_set_camera_prior), nullptr = no priors
+  const S* prior_H;          // [nc][81] A^T A of the scaled camera priors (rba_set_camera_prior) and the pair priors' diagonal
+                             //   blocks (rba_set_camera_pair_prior), nullptr = neither
+  // pair priors (DESIGN.md section 15): camera-major CSR of the directed edges i -> j; pair_ov == nullptr = no pair priors
+  const int* pair_ptr;       // [nc + 1]
+  const int* pair_nbr;       // [edges] j
+  const S* pair_O;           // [edges][36] O_ij = A_i^T A_j (pose 6x6, row-major), scaled
+  S* pair_ov;                // [9 nc] sum_j O_ij v_j of the vector the next PCG / power-series vector step consumes
 };
 
 // increment entries (tx,ty,tz, rx,ry,rz, f,k1,k2) held by a camera's RBA_FIX_* bits, as a 9-bit mask
@@ -2096,7 +2102,24 @@ __global__ void __launch_bounds__(WARPS * 32) k_matvec_large(DevPtrs<S> D, const
 //   all launched with exactly NPART blocks of 128 threads; thread per camera (9-vectors);
 //   partial sums per block in double, combined in a fixed order by the consumer kernel.
 // ------------------------------------------------------------------------------------------------
-// out = y + lambda v (+ A^T A v of the camera priors), y = the camera-reduced operator output [9 nc]; out may be y.
+// sum_j O_ij v_j of the pair priors (DESIGN.md section 15), entry e = 9 i + a of the camera vector (zero on the intrinsic
+// rows a >= 6), edges in list order
+template <class S>
+__device__ __forceinline__ S pair_ov_entry(const DevPtrs<S>& D, const S* __restrict__ v, int e) {
+  const int cam = e / 9, a = e - 9 * cam;
+  S s = 0;
+  if (a < 6)
+    for (int q = D.pair_ptr[cam], q1 = D.pair_ptr[cam + 1]; q < q1; ++q) {
+      const S* O = D.pair_O + 36 * (size_t)q + 6 * a;
+      const S* vj = v + 9 * (size_t)D.pair_nbr[q];
+#pragma unroll
+      for (int k = 0; k < 6; ++k) s += O[k] * vj[k];
+    }
+  return s;
+}
+
+// out = y + lambda v (+ A^T A v of the camera priors) (+ sum_j O_ij v_j of the pair priors), y = the camera-reduced
+// operator output [9 nc]; out may be y.
 // The operator of rba_right_multiply: the same order of operations as P1 of k_pcg_vec.
 template <class S>
 __global__ void __launch_bounds__(128) k_pcg_q(DevPtrs<S> D, const S* yfull, const S* __restrict__ vec, S* out, S lambda) {
@@ -2115,6 +2138,7 @@ __global__ void __launch_bounds__(128) k_pcg_q(DevPtrs<S> D, const S* yfull, con
         for (int k = 0; k < 9; ++k) h += hr[k] * vec[9 * (size_t)cam + k];
         qv += h;
       }
+      if (D.pair_ov) qv += pair_ov_entry(D, vec, 9 * cam + c);  // the value k_pair_ov gives k_pcg_vec<S, true, true>
       out[9 * (size_t)cam + c] = qv;
     }
   }
@@ -2214,10 +2238,13 @@ __device__ __forceinline__ void pcg_publish_progress(int* prog, int iter, int do
 // PRIOR (D.prior_H set, DESIGN.md section 14): P1 adds the camera-prior term, q = y + lambda v + A^T A v.  The rows of A^T A
 // are fetched with the M^-1 rows, ahead of the grid dependency; the 9 entries of v of a camera are exchanged through shared
 // memory like r for z = M^-1 r.  PRIOR = false is the kernel without priors, unchanged.
-template <class S, bool PRIOR = false>
+// PAIR (D.pair_ov set, DESIGN.md section 15; implies PRIOR, whose A^T A holds the pair priors' diagonal blocks): P1 also adds
+// sum_j O_ij v_j, which k_pair_ov, the kernel this one depends on, has written to D.pair_ov.
+template <class S, bool PRIOR = false, bool PAIR = false>
 __global__ void __launch_bounds__(VEC_THREADS, 1) k_pcg_vec(DevPtrs<S> D, PcgState* st, S lambda, int i, int mode,
                                                          double eta, int min_it, int is_last, int pdl, PeerComm pc, int seq,
                                                          const int* __restrict__ cam_item_ptr, int* prog) {
+  static_assert(PRIOR || !PAIR, "the pair priors' diagonal blocks are in prior_H");
   __shared__ S sr[VEC_THREADS * VEC_EPT + 16];
   __shared__ int peer_fail;
   __shared__ double cl_go;          // multi-GPU: CTA 0's verdict on the peer exchange (distributed shared memory)
@@ -2342,6 +2369,7 @@ __global__ void __launch_bounds__(VEC_THREADS, 1) k_pcg_vec(DevPtrs<S> D, PcgSta
             for (int c = 0; c < 9; ++c) h += hrow[k][c] * vc[c];
             qv[k] += h;
           }
+          if constexpr (PAIR) qv[k] += __ldcg(D.pair_ov + e0 + l);
           acc += (double)(vv * qv[k]);
         }
       }
@@ -2358,6 +2386,7 @@ __global__ void __launch_bounds__(VEC_THREADS, 1) k_pcg_vec(DevPtrs<S> D, PcgSta
           for (int c = 0; c < 9; ++c) h += hr[c] * vc[c];
           q += h;
         }
+        if constexpr (PAIR) q += __ldcg(D.pair_ov + e0 + l);
         D.q[e0 + l] = q;
         acc += (double)(vv * q);
       }
@@ -2505,8 +2534,10 @@ __global__ void __launch_bounds__(VEC_THREADS, 1) k_pcg_vec(DevPtrs<S> D, PcgSta
 //   One 16-CTA cluster like k_pcg_vec: i == 0 initialises, i >= 1 consumes y = E_0 p (camera-reduced by the previous
 //   kernel).  D.p = tmp, D.x = accum, D.inv = Hpp^-1 (block-diagonal, damped), D.inc = the result (already the increment:
 //   H inc = -b).  Norms are accumulated in double.
+//   PAIR (pair priors, DESIGN.md section 15): the series runs on Hpp^-1 (E_0 - O), tmp = Hpp^-1 ((E_0 - O) tmp), with
+//   O tmp = D.pair_ov written by k_pair_ov, the kernel this one depends on (Hpp holds the pairs' diagonal blocks).
 // ------------------------------------------------------------------------------------------------
-template <class S>
+template <class S, bool PAIR = false>
 __global__ void __launch_bounds__(VEC_THREADS) k_power_vec(DevPtrs<S> D, PcgState* st, int i, double eta, int is_last, int pdl) {
   __shared__ double cl[4][CL_MAX];
   const int tid = threadIdx.x;
@@ -2526,8 +2557,19 @@ __global__ void __launch_bounds__(VEC_THREADS) k_power_vec(DevPtrs<S> D, PcgStat
     const S* row = D.inv + 9 * (size_t)e;
     const S* v = (i == 0 ? D.b : D.y) + 9 * (size_t)cam;
     S z = 0;
+    if constexpr (PAIR) {
+      if (i != 0) {
+        const S* ov = D.pair_ov + 9 * (size_t)cam;
 #pragma unroll
-    for (int c = 0; c < 9; ++c) z += row[c] * __ldcg(v + c);
+        for (int c = 0; c < 9; ++c) z += row[c] * (__ldcg(v + c) - __ldcg(ov + c));
+      } else {
+#pragma unroll
+        for (int c = 0; c < 9; ++c) z += row[c] * __ldcg(v + c);
+      }
+    } else {
+#pragma unroll
+      for (int c = 0; c < 9; ++c) z += row[c] * __ldcg(v + c);
+    }
     if (i == 0) z = -z;
     const S acc = (i == 0) ? z : D.x[e] + z;
     D.x[e] = acc;
@@ -2709,18 +2751,12 @@ __global__ void k_mask_fixed_inc(S* __restrict__ inc, const uint8_t* __restrict_
 //       de/dv = -R^T (rows 0..2),  dLog/dw = J_l^-1(Log(R R0^T)) (rows 3..5),  identity on the intrinsics (rows 6..8).
 //     mean [nc][10] (qx,qy,qz,qw of R0, c0, f0, k1_0, k2_0; unit quaternion), sqrt_info [nc][81] row-major L.
 // ------------------------------------------------------------------------------------------------
-// e of one camera; with JAC also J_l^-1 (row-major 3x3) and R (row-major 3x3)
-template <class S, bool JAC>
-__device__ __forceinline__ void prior_residual(const S* __restrict__ cam, const S* __restrict__ mean, S* e, S* Jinv, S* R) {
-  S Rl[9];
-  S* Rm = JAC ? R : Rl;
-  quat_to_rot(cam, Rm);
-  const S t0 = cam[4], t1 = cam[5], t2 = cam[6];
-#pragma unroll
-  for (int k = 0; k < 3; ++k) e[k] = -(Rm[k] * t0 + Rm[3 + k] * t1 + Rm[6 + k] * t2) - mean[4 + k];
-  // relative rotation q (x) conj(q0) (Hamilton product, xyzw); its Log with the angle in [0, pi]
-  const S a0 = cam[0], a1 = cam[1], a2 = cam[2], a3 = cam[3];
-  const S b0 = -mean[0], b1 = -mean[1], b2 = -mean[2], b3 = mean[3];
+// SO(3) helpers of both prior kinds (absolute and pair priors).
+// phi = Log(a (x) conj(m)) for unit quaternions a, m (xyzw, Hamilton product), the angle in [0, pi] (the product is
+// flipped to w >= 0)
+template <class S>
+__device__ __forceinline__ void so3_log_rel(const S a0, const S a1, const S a2, const S a3, const S* __restrict__ m, S* phi) {
+  const S b0 = -m[0], b1 = -m[1], b2 = -m[2], b3 = m[3];
   S w = a3 * b3 - a0 * b0 - a1 * b1 - a2 * b2;
   S v0 = a3 * b0 + a0 * b3 + a1 * b2 - a2 * b1;
   S v1 = a3 * b1 + a1 * b3 + a2 * b0 - a0 * b2;
@@ -2730,23 +2766,37 @@ __device__ __forceinline__ void prior_residual(const S* __restrict__ cam, const 
   const S n = sqrt(n2);
   // theta / n with theta = 2 atan2(n, w); series 2/w (1 - n^2 / (3 w^2)) where n is tiny against w
   const S fac = (n < ST<S>::eps_sqrt() * w) ? S(2) / w * (S(1) - n2 / (S(3) * w * w)) : S(2) * atan2(n, w) / n;
-  e[3] = fac * v0; e[4] = fac * v1; e[5] = fac * v2;
-  e[6] = cam[7] - mean[7]; e[7] = cam[8] - mean[8]; e[8] = cam[9] - mean[9];
-  if (JAC) {
-    // J_l^-1(phi) = I - 1/2 [phi]x + a [phi]x^2,  a = 1/th^2 - cot(th/2) / (2 th)  (series 1/12 + th^2/720 + th^4/30240)
-    const S p0 = e[3], p1 = e[4], p2 = e[5];
-    const S th2 = p0 * p0 + p1 * p1 + p2 * p2;
-    S a;
-    if (th2 < S(1e-4)) a = S(1.0 / 12.0) + th2 * (S(1.0 / 720.0) + th2 * S(1.0 / 30240.0));
-    else {
-      const S th = sqrt(th2), h = S(0.5) * th;
-      a = S(1) / th2 - cos(h) / (S(2) * th * sin(h));
-    }
-    // [phi]x^2 = phi phi^T - th^2 I
-    Jinv[0] = S(1) + a * (p0 * p0 - th2); Jinv[1] = S(0.5) * p2 + a * p0 * p1;       Jinv[2] = -S(0.5) * p1 + a * p0 * p2;
-    Jinv[3] = -S(0.5) * p2 + a * p1 * p0; Jinv[4] = S(1) + a * (p1 * p1 - th2);       Jinv[5] = S(0.5) * p0 + a * p1 * p2;
-    Jinv[6] = S(0.5) * p1 + a * p2 * p0;  Jinv[7] = -S(0.5) * p0 + a * p2 * p1;       Jinv[8] = S(1) + a * (p2 * p2 - th2);
+  phi[0] = fac * v0; phi[1] = fac * v1; phi[2] = fac * v2;
+}
+// J_l^-1(phi) (row-major 3x3) = I - 1/2 [phi]x + a [phi]x^2,  a = 1/th^2 - cot(th/2) / (2 th)  (series 1/12 + th^2/720 + th^4/30240)
+template <class S>
+__device__ __forceinline__ void so3_jl_inv(const S* phi, S* Jinv) {
+  const S p0 = phi[0], p1 = phi[1], p2 = phi[2];
+  const S th2 = p0 * p0 + p1 * p1 + p2 * p2;
+  S a;
+  if (th2 < S(1e-4)) a = S(1.0 / 12.0) + th2 * (S(1.0 / 720.0) + th2 * S(1.0 / 30240.0));
+  else {
+    const S th = sqrt(th2), h = S(0.5) * th;
+    a = S(1) / th2 - cos(h) / (S(2) * th * sin(h));
   }
+  // [phi]x^2 = phi phi^T - th^2 I
+  Jinv[0] = S(1) + a * (p0 * p0 - th2); Jinv[1] = S(0.5) * p2 + a * p0 * p1;       Jinv[2] = -S(0.5) * p1 + a * p0 * p2;
+  Jinv[3] = -S(0.5) * p2 + a * p1 * p0; Jinv[4] = S(1) + a * (p1 * p1 - th2);       Jinv[5] = S(0.5) * p0 + a * p1 * p2;
+  Jinv[6] = S(0.5) * p1 + a * p2 * p0;  Jinv[7] = -S(0.5) * p0 + a * p2 * p1;       Jinv[8] = S(1) + a * (p2 * p2 - th2);
+}
+
+// e of one camera; with JAC also J_l^-1 (row-major 3x3) and R (row-major 3x3)
+template <class S, bool JAC>
+__device__ __forceinline__ void prior_residual(const S* __restrict__ cam, const S* __restrict__ mean, S* e, S* Jinv, S* R) {
+  S Rl[9];
+  S* Rm = JAC ? R : Rl;
+  quat_to_rot(cam, Rm);
+  const S t0 = cam[4], t1 = cam[5], t2 = cam[6];
+#pragma unroll
+  for (int k = 0; k < 3; ++k) e[k] = -(Rm[k] * t0 + Rm[3 + k] * t1 + Rm[6 + k] * t2) - mean[4 + k];
+  so3_log_rel(cam[0], cam[1], cam[2], cam[3], mean, e + 3);  // Log(R R0^T)
+  e[6] = cam[7] - mean[7]; e[7] = cam[8] - mean[8]; e[8] = cam[9] - mean[9];
+  if (JAC) so3_jl_inv(e + 3, Jinv);
 }
 
 // once per linearisation, after the cross-shard sum of diag2 and before k_scaling: the unscaled prior Jacobian
@@ -2868,6 +2918,226 @@ __global__ void k_prior_ldiff(const S* __restrict__ A, const S* __restrict__ pr,
 #pragma unroll
       for (int j = 0; j < 9; ++j) u += Ac[9 * i + j] * d[j];
       lp += u * (S(0.5) * u + pr[9 * (size_t)cam + i]);
+    }
+    acc -= (double)lp;
+  }
+  const double s = prior_block_sum(acc);
+  if (threadIdx.x == 0) red[0] += s;
+}
+
+// ------------------------------------------------------------------------------------------------
+// K9  Relative pose priors between two cameras (rba_set_camera_pair_prior, DESIGN.md section 15).  Pair p = (i, j) with the
+//     measured relative pose Z = (R0, t0) of T_i T_j^-1 and the 6x6 square-root information L:
+//       e_t = t_i - R_i R_j^T t_j - t0,   e_r = Log(R_i R_j^T R0^T),   cost 1/2 |L (e_t, e_r)|^2.
+//     For the increment of k_camera_update, with M = R_i R_j^T, t_rel = t_i - M t_j, phi = e_r:
+//       de_t/dv_i = I,  de_t/dw_i = -[t_rel]x,  de_t/dv_j = -M,  de_t/dw_j = 0,
+//       de_r/dw_i = J_l^-1(phi),  de_r/dw_j = -J_l^-1(phi) M,  de_r/dv = 0;  zero intrinsic columns.
+//     pairs [m][2], mean [m][7] (qx,qy,qz,qw of R0, t0; unit quaternion), sqrt_info [m][36] row-major L.
+//     A [m][2][36]: the pose blocks A_i, A_j (6x6, row-major) of L de/d(inc), unscaled after k_pair_linearize and scaled
+//     after k_pair_scale; pr [m][6] = L e.  Incident pair sides are listed camera-major (ptr [nc + 1], item = 2 p + side,
+//     ascending p within a camera), which is also the CSR of the directed edges i -> j of the off-diagonal blocks O_ij.
+// ------------------------------------------------------------------------------------------------
+// e [6] of one pair; M = R_i R_j^T and t_rel (needed by e); with JAC also J_l^-1(phi)
+template <class S, bool JAC>
+__device__ __forceinline__ void pair_residual(const S* __restrict__ ci, const S* __restrict__ cj, const S* __restrict__ mean,
+                                              S* e, S* M, S* tr, S* Jinv) {
+  S Ri[9], Rj[9];
+  quat_to_rot(ci, Ri);
+  quat_to_rot(cj, Rj);
+#pragma unroll
+  for (int a = 0; a < 3; ++a)
+#pragma unroll
+    for (int b = 0; b < 3; ++b) M[3 * a + b] = Ri[3 * a] * Rj[3 * b] + Ri[3 * a + 1] * Rj[3 * b + 1] + Ri[3 * a + 2] * Rj[3 * b + 2];
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    tr[a] = ci[4 + a] - (M[3 * a] * cj[4] + M[3 * a + 1] * cj[5] + M[3 * a + 2] * cj[6]);
+    e[a] = tr[a] - mean[4 + a];
+  }
+  // q_i (x) conj(q_j) is the quaternion of M; phi = Log(M R0^T)
+  const S a0 = ci[0], a1 = ci[1], a2 = ci[2], a3 = ci[3];
+  const S b0 = -cj[0], b1 = -cj[1], b2 = -cj[2], b3 = cj[3];
+  const S w = a3 * b3 - a0 * b0 - a1 * b1 - a2 * b2;
+  const S x = a3 * b0 + a0 * b3 + a1 * b2 - a2 * b1;
+  const S y = a3 * b1 + a1 * b3 + a2 * b0 - a0 * b2;
+  const S z = a3 * b2 + a2 * b3 + a0 * b1 - a1 * b0;
+  so3_log_rel(x, y, z, w, mean, e + 3);
+  if (JAC) so3_jl_inv(e + 3, Jinv);
+}
+
+// once per linearisation, after the cross-shard sum of diag2 (and the absolute priors) and before k_scaling: the unscaled
+// pose blocks A_i = L de/d(inc_i), A_j = L de/d(inc_j) and r = L e.  Thread per pair; identical on every shard.
+template <class S>
+__global__ void k_pair_linearize(const S* __restrict__ cams, const int* __restrict__ pairs, const S* __restrict__ mean,
+                                 const S* __restrict__ Lsq, int m, S* __restrict__ A, S* __restrict__ pr) {
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= m) return;
+  S e[6], M[9], tr[3], Jinv[9], JM[9];
+  pair_residual<S, true>(cams + 10 * (size_t)pairs[2 * p], cams + 10 * (size_t)pairs[2 * p + 1], mean + 7 * (size_t)p, e, M, tr, Jinv);
+#pragma unroll
+  for (int a = 0; a < 3; ++a)
+#pragma unroll
+    for (int b = 0; b < 3; ++b) JM[3 * a + b] = Jinv[3 * a] * M[b] + Jinv[3 * a + 1] * M[3 + b] + Jinv[3 * a + 2] * M[6 + b];
+  const S* Lp = Lsq + 36 * (size_t)p;
+  S* Ai = A + 72 * (size_t)p;
+  S* Aj = Ai + 36;
+  for (int i = 0; i < 6; ++i) {
+    S l[6];
+#pragma unroll
+    for (int k = 0; k < 6; ++k) l[k] = Lp[6 * i + k];
+    S ri = 0;
+#pragma unroll
+    for (int k = 0; k < 6; ++k) ri += l[k] * e[k];
+    pr[6 * (size_t)p + i] = ri;
+    // A_i row: (l_t, l_t (-[t_rel]x) + l_r J_l^-1);  A_j row: (-l_t M, -l_r J_l^-1 M)
+#pragma unroll
+    for (int j = 0; j < 3; ++j) Ai[6 * i + j] = l[j];
+    Ai[6 * i + 3] = -l[1] * tr[2] + l[2] * tr[1] + l[3] * Jinv[0] + l[4] * Jinv[3] + l[5] * Jinv[6];
+    Ai[6 * i + 4] = l[0] * tr[2] - l[2] * tr[0] + l[3] * Jinv[1] + l[4] * Jinv[4] + l[5] * Jinv[7];
+    Ai[6 * i + 5] = -l[0] * tr[1] + l[1] * tr[0] + l[3] * Jinv[2] + l[4] * Jinv[5] + l[5] * Jinv[8];
+#pragma unroll
+    for (int j = 0; j < 3; ++j) {
+      Aj[6 * i + j] = -(l[0] * M[j] + l[1] * M[3 + j] + l[2] * M[6 + j]);
+      Aj[6 * i + 3 + j] = -(l[3] * JM[j] + l[4] * JM[3 + j] + l[5] * JM[6 + j]);
+    }
+  }
+}
+
+// squared column norms of the incident pair blocks added to diag2 (the Jacobi scaling of the whole Jacobian).  Thread per
+// camera over its incident sides in list order: no atomics, bit-identical on every run and shard.
+template <class S>
+__global__ void k_pair_diag2(const S* __restrict__ A, const int* __restrict__ ptr, const int* __restrict__ item, int nc,
+                             S* __restrict__ diag2) {
+  const int cam = blockIdx.x * blockDim.x + threadIdx.x;
+  if (cam >= nc) return;
+  S cn[6];
+#pragma unroll
+  for (int j = 0; j < 6; ++j) cn[j] = 0;
+  for (int q = ptr[cam]; q < ptr[cam + 1]; ++q) {
+    const S* As = A + 36 * (size_t)item[q];
+    for (int i = 0; i < 6; ++i)
+#pragma unroll
+      for (int j = 0; j < 6; ++j) cn[j] += As[6 * i + j] * As[6 * i + j];
+  }
+#pragma unroll
+  for (int j = 0; j < 6; ++j) diag2[9 * (size_t)cam + j] += cn[j];
+}
+
+// after k_scaling: A_s <- A_s diag(s of its camera), in place.  Thread per pair.
+template <class S>
+__global__ void k_pair_scale(S* __restrict__ A, const int* __restrict__ pairs, const S* __restrict__ scaling, int m) {
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= m) return;
+  for (int s = 0; s < 2; ++s) {
+    const S* sc = scaling + 9 * (size_t)pairs[2 * p + s];
+    S* As = A + 72 * (size_t)p + 36 * s;
+    for (int i = 0; i < 6; ++i)
+#pragma unroll
+      for (int j = 0; j < 6; ++j) As[6 * i + j] *= sc[j];
+  }
+}
+
+// after k_pair_scale (and k_prior_scale): per camera the sum over its incident sides of A_s^T A_s into H [nc][81] and of
+// A_s^T r into g [9 nc] (added to the absolute priors' H, g when `accumulate`, else written with zero intrinsic rows and
+// columns), A_s^T A_s also into the JACOBI blocks when they exist, and O_ij = A_s^T A_other of every directed edge.
+// Thread per camera, sides in list order.
+template <class S>
+__global__ void k_pair_accum(const S* __restrict__ A, const S* __restrict__ pr, const int* __restrict__ ptr,
+                             const int* __restrict__ item, int nc, int accumulate, S* __restrict__ H, S* __restrict__ g,
+                             S* __restrict__ jblocks, S* __restrict__ O) {
+  const int cam = blockIdx.x * blockDim.x + threadIdx.x;
+  if (cam >= nc) return;
+  const int q0 = ptr[cam], q1 = ptr[cam + 1];
+  S* Hc = H + 81 * (size_t)cam;
+  for (int a = 0; a < 6; ++a) {
+    S hrow[6], ga = 0;
+#pragma unroll
+    for (int b = 0; b < 6; ++b) hrow[b] = 0;
+    for (int q = q0; q < q1; ++q) {
+      const int it = item[q];
+      const S* As = A + 36 * (size_t)it;
+      const S* Ao = A + 36 * (size_t)(it ^ 1);
+      const S* rp = pr + 6 * (size_t)(it >> 1);
+      S orow[6];
+#pragma unroll
+      for (int b = 0; b < 6; ++b) orow[b] = 0;
+      for (int i = 0; i < 6; ++i) {
+        const S ai = As[6 * i + a];
+        ga += ai * rp[i];
+#pragma unroll
+        for (int b = 0; b < 6; ++b) { hrow[b] += ai * As[6 * i + b]; orow[b] += ai * Ao[6 * i + b]; }
+      }
+#pragma unroll
+      for (int b = 0; b < 6; ++b) O[36 * (size_t)q + 6 * a + b] = orow[b];
+    }
+    g[9 * (size_t)cam + a] = (accumulate ? g[9 * (size_t)cam + a] : S(0)) + ga;
+#pragma unroll
+    for (int b = 0; b < 6; ++b) {
+      Hc[9 * a + b] = (accumulate ? Hc[9 * a + b] : S(0)) + hrow[b];
+      if (jblocks) jblocks[81 * (size_t)cam + 9 * a + b] += hrow[b];
+    }
+  }
+  if (!accumulate) {
+    for (int k = 0; k < 81; ++k)
+      if (k / 9 >= 6 || k % 9 >= 6) Hc[k] = 0;
+    for (int a = 6; a < 9; ++a) g[9 * (size_t)cam + a] = 0;
+  }
+}
+
+// Per PCG iteration (and power-series term), just ahead of the vector step: D.pair_ov = sum_j O_ij v_j for the vector v the
+// step is about to consume.  A kernel of its own: the vector step reads other cameras' v here, and computing the product in
+// a separate grid keeps it complete before any CTA of the vector step overwrites D.p or D.x.  Launched dependent on its
+// predecessor; its own wait keeps the dependency chain transitive for the vector step, which waits for this grid.
+template <class S>
+__global__ void __launch_bounds__(256) k_pair_ov(DevPtrs<S> D, const PcgState* st, const S* __restrict__ v) {
+  asm volatile("griddepcontrol.wait;" ::: "memory");
+  if (*reinterpret_cast<const volatile int*>(&st->done)) return;
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < 9 * D.nc; e += gridDim.x * blockDim.x) D.pair_ov[e] = pair_ov_entry(D, v, e);
+}
+
+// pair-prior cost sum_p 1/2 |L_p e_p|^2 at the current cameras, added like k_prior_cost.  One block.
+template <class S>
+__global__ void k_pair_cost(const S* __restrict__ cams, const int* __restrict__ pairs, const S* __restrict__ mean,
+                            const S* __restrict__ Lsq, int m, double* red, int* bad_flag) {
+  double acc = 0;
+  for (int p = threadIdx.x; p < m; p += blockDim.x) {
+    S e[6], M[9], tr[3];
+    pair_residual<S, false>(cams + 10 * (size_t)pairs[2 * p], cams + 10 * (size_t)pairs[2 * p + 1], mean + 7 * (size_t)p, e, M, tr, nullptr);
+    const S* Lp = Lsq + 36 * (size_t)p;
+    S c2 = 0;
+    for (int i = 0; i < 6; ++i) {
+      S ri = 0;
+#pragma unroll
+      for (int k = 0; k < 6; ++k) ri += Lp[6 * i + k] * e[k];
+      c2 += ri * ri;
+    }
+    acc += 0.5 * (double)c2;
+  }
+  const double s = prior_block_sum(acc);
+  if (threadIdx.x == 0) {
+    red[1] += s;
+    red[4] += s;
+    if (!isfinite(s)) *bad_flag = 1;
+  }
+}
+
+// pair part of the model cost change: l_diff -= sum_p (A d)^T (1/2 A d + r), A d = A_i d_i + A_j d_j for the (masked,
+// scaled) increment d, added to red[0] like k_prior_ldiff.  One block.
+template <class S>
+__global__ void k_pair_ldiff(const S* __restrict__ A, const S* __restrict__ pr, const int* __restrict__ pairs,
+                             const S* __restrict__ inc, int m, double* red) {
+  double acc = 0;
+  for (int p = threadIdx.x; p < m; p += blockDim.x) {
+    S di[6], dj[6];
+#pragma unroll
+    for (int j = 0; j < 6; ++j) { di[j] = inc[9 * (size_t)pairs[2 * p] + j]; dj[j] = inc[9 * (size_t)pairs[2 * p + 1] + j]; }
+    const S* Ai = A + 72 * (size_t)p;
+    S lp = 0;
+    for (int i = 0; i < 6; ++i) {
+      S u = 0;
+#pragma unroll
+      for (int j = 0; j < 6; ++j) u += Ai[6 * i + j] * di[j] + Ai[36 + 6 * i + j] * dj[j];
+      lp += u * (S(0.5) * u + pr[6 * (size_t)p + i]);
     }
     acc -= (double)lp;
   }

@@ -51,6 +51,7 @@ struct rba_handle {
   virtual int restore() = 0;
   virtual int set_camera_fixed(const uint8_t* flags) = 0;
   virtual int set_camera_prior(const void* mean, const void* sqrt_info) = 0;
+  virtual int set_camera_pair_prior(int32_t num_pairs, const int32_t* pairs, const void* mean, const void* sqrt_info) = 0;
   virtual int compute_error(rba_residual_info* out) = 0;
   virtual int linearize() = 0;
   virtual int solve(double lambda, void* inc_out, rba_cg_summary* cg) = 0;
@@ -160,13 +161,28 @@ struct Solver : rba_handle {
   bool damping_valid = false;
   uint8_t* d_cam_fixed = nullptr;  // [nc] flags of rba_set_camera_fixed; D.cam_fixed points here while any flag is set
   bool all_cams_fixed = false;     // no free camera parameter: the reduced system is empty and its solve is skipped
-  // camera priors (rba_set_camera_prior, DESIGN.md section 14); D.prior_H points at d_prior_H while any L_c is non-zero
+  // camera priors (rba_set_camera_prior, DESIGN.md section 14); has_abs_prior while any L_c is non-zero.  D.prior_H points at
+  // d_prior_H while there are absolute or pair priors.
+  bool has_abs_prior = false;
   S* d_prior_mean = nullptr;       // [nc][10] mean, quaternion normalised
   S* d_prior_L = nullptr;          // [nc][81] square-root information
   S* d_prior_A = nullptr;          // [nc][81] L de/d(inc): unscaled after k_prior_linearize, scaled after k_prior_scale
   S* d_prior_r = nullptr;          // [nc][9]  L e at the linearisation point
-  S* d_prior_H = nullptr;          // [nc][81] A^T A
-  S* d_prior_g = nullptr;          // [nc][9]  A^T r
+  S* d_prior_H = nullptr;          // [nc][81] A^T A (+ the pair priors' diagonal blocks)
+  S* d_prior_g = nullptr;          // [nc][9]  A^T r (+ the pair priors' A_s^T r)
+  // pair priors (rba_set_camera_pair_prior, DESIGN.md section 15): n_pairs pairs with a non-zero L, D.pair_ov set while
+  // n_pairs > 0.  Buffers are sized for pair_cap pairs.
+  int n_pairs = 0, pair_cap = 0;
+  int* d_pair_ij = nullptr;        // [m][2] cameras (i, j)
+  S* d_pair_mean = nullptr;        // [m][7] R0 quaternion (normalised), t0
+  S* d_pair_L = nullptr;           // [m][36] square-root information
+  S* d_pair_A = nullptr;           // [m][2][36] pose blocks A_i, A_j: unscaled after k_pair_linearize, scaled after k_pair_scale
+  S* d_pair_r = nullptr;           // [m][6] L e at the linearisation point
+  int* d_pair_item = nullptr;      // [2m] incident sides 2 p + side, camera-major (CSR d_pair_ptr)
+  int* d_pair_nbr = nullptr;       // [2m] the other camera of each side
+  S* d_pair_O = nullptr;           // [2m][36] O of each directed edge
+  int* d_pair_ptr = nullptr;       // [nc + 1]
+  S* d_pair_ov = nullptr;          // [9 nc]
   rba_stage_timings tm{};
   EventPair ev_stage1, ev_stage2, ev_precond, ev_pcg, ev_backsub, ev_update, ev_error, ev_mv, ev_user;
   long long launches = 0;
@@ -206,6 +222,13 @@ struct Solver : rba_handle {
     device_bytes += bytes;
     if (zero) CU(cudaMemsetAsync(q, 0, bytes, stream));
     *p = (T*)q;
+    return RBA_OK;
+  }
+  // frees a buffer of dalloc (nullptr: nothing to do); device_bytes keeps counting it (the most the handle has allocated)
+  int dfree(void* q) {
+    if (!q) return RBA_OK;
+    allocs.erase(std::find(allocs.begin(), allocs.end(), q));
+    CU(cudaFree(q));
     return RBA_OK;
   }
   template <class T>
@@ -471,7 +494,9 @@ struct Solver : rba_handle {
     // the PCG vector step runs on one thread-block cluster (16 CTAs if the device grants it, else 8, ...)
     CU(cudaFuncSetAttribute(k_pcg_vec<S>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
     CU(cudaFuncSetAttribute((k_pcg_vec<S, true>), cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+    CU(cudaFuncSetAttribute((k_pcg_vec<S, true, true>), cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
     CU(cudaFuncSetAttribute(k_power_vec<S>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+    CU(cudaFuncSetAttribute((k_power_vec<S, true>), cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
     for (; pcg_cluster > 1; pcg_cluster >>= 1) {
       cudaLaunchConfig_t cfg = {};
       cfg.gridDim = dim3(pcg_cluster); cfg.blockDim = dim3(VEC_THREADS);
@@ -654,24 +679,113 @@ struct Solver : rba_handle {
     }
     if (any) {
       if (!d_prior_mean) {
-        int rc;
-        if ((rc = dalloc(&d_prior_mean, (size_t)10 * nc, false))) return rc;
-        if ((rc = dalloc(&d_prior_L, (size_t)81 * nc, false))) return rc;
-        if ((rc = dalloc(&d_prior_A, (size_t)81 * nc, false))) return rc;
-        if ((rc = dalloc(&d_prior_r, (size_t)9 * nc, false))) return rc;
-        if ((rc = dalloc(&d_prior_H, (size_t)81 * nc, false))) return rc;
-        if ((rc = dalloc(&d_prior_g, (size_t)9 * nc, false))) return rc;
+        TRY(dalloc(&d_prior_mean, (size_t)10 * nc, false));
+        TRY(dalloc(&d_prior_L, (size_t)81 * nc, false));
+        TRY(dalloc(&d_prior_A, (size_t)81 * nc, false));
+        TRY(dalloc(&d_prior_r, (size_t)9 * nc, false));
       }
+      TRY(alloc_prior_diag());
       CU(cudaMemcpyAsync(d_prior_mean, mean.data(), mean.size() * sizeof(S), cudaMemcpyHostToDevice, stream));
       CU(cudaMemcpyAsync(d_prior_L, Lsq.data(), Lsq.size() * sizeof(S), cudaMemcpyHostToDevice, stream));
       CU(cudaStreamSynchronize(stream));
     }
-    D.prior_H = any ? d_prior_H : nullptr;
+    has_abs_prior = any;
+    return priors_changed();
+  }
+  int alloc_prior_diag() {
+    if (!d_prior_H) {
+      TRY(dalloc(&d_prior_H, (size_t)81 * nc, false));
+      TRY(dalloc(&d_prior_g, (size_t)9 * nc, false));
+    }
+    return RBA_OK;
+  }
+  int priors_changed() {
+    D.prior_H = (has_abs_prior || n_pairs > 0) ? d_prior_H : nullptr;
+    D.pair_ov = n_pairs > 0 ? d_pair_ov : nullptr;
     linearized = false;  // the scaling, A and r of the last linearisation belong to the previous priors
     damping_valid = false;
     have_inc = false;
     error_cache_valid = false;
     return RBA_OK;
+  }
+  // Relative pose priors between pairs of cameras (DESIGN.md section 15).  Like the absolute priors they are part of the
+  // linearisation.  Pairs with an all-zero L are dropped here; none left (num_pairs == 0 or every L zero) = the unmodified
+  // path (D.pair_ov == nullptr).  Every check runs before anything changes, so a rejected call leaves the previous pairs.
+  int set_camera_pair_prior(int32_t num_pairs, const int32_t* pairs, const void* mean_v, const void* sqrt_info_v) override {
+    auto bad = [&](const std::string& what) { g_err = "rba_set_camera_pair_prior: " + what; return RBA_ERR_INVALID_ARGUMENT; };
+    if (num_pairs < 0) return bad("num_pairs must be >= 0, got " + std::to_string(num_pairs));
+    if (num_pairs > 0 && (!pairs || !mean_v || !sqrt_info_v)) return bad("pairs, mean and sqrt_info must be given when num_pairs > 0");
+    const S* m = (const S*)mean_v;
+    const S* Ls = (const S*)sqrt_info_v;
+    std::vector<int> ij;
+    std::vector<S> mean, Lsq;
+    for (int p = 0; p < num_pairs; ++p) {
+      const int i = pairs[2 * p], j = pairs[2 * p + 1];
+      const std::string tag = "pair " + std::to_string(p);
+      if (i < 0 || i >= nc || j < 0 || j >= nc) return bad(tag + " has a camera index outside [0, " + std::to_string(nc) + ")");
+      if (i == j) return bad(tag + " joins camera " + std::to_string(i) + " to itself");
+      bool nonzero = false;
+      for (int k = 0; k < 7; ++k)
+        if (!std::isfinite((double)m[7 * (size_t)p + k])) return bad(tag + " has a non-finite mean");
+      for (int k = 0; k < 36; ++k) {
+        const double v = (double)Ls[36 * (size_t)p + k];
+        if (!std::isfinite(v)) return bad(tag + " has a non-finite sqrt_info");
+        nonzero = nonzero || v != 0.0;
+      }
+      double q[4], n2 = 0;
+      for (int k = 0; k < 4; ++k) { q[k] = (double)m[7 * (size_t)p + k]; n2 += q[k] * q[k]; }
+      const double n = std::sqrt(n2);
+      if (!(std::fabs(n - 1.0) <= 1e-3)) return bad(tag + " has a mean quaternion of norm " + std::to_string(n) + " (must be within 1e-3 of 1)");
+      if (!nonzero) continue;
+      ij.push_back(i); ij.push_back(j);
+      for (int k = 0; k < 4; ++k) mean.push_back((S)(q[k] / n));
+      for (int k = 4; k < 7; ++k) mean.push_back(m[7 * (size_t)p + k]);
+      Lsq.insert(Lsq.end(), Ls + 36 * (size_t)p, Ls + 36 * (size_t)(p + 1));
+    }
+    const int np = (int)(ij.size() / 2);
+    if (np > 0) {
+      // camera-major list of the incident sides, ascending pair within a camera (the fixed summation order of the kernels)
+      std::vector<int> ptr(nc + 1, 0), item(2 * (size_t)np), nbr(2 * (size_t)np);
+      for (int k = 0; k < 2 * np; ++k) ++ptr[ij[k] + 1];
+      for (int c = 0; c < nc; ++c) ptr[c + 1] += ptr[c];
+      std::vector<int> fill(ptr.begin(), ptr.end() - 1);
+      for (int k = 0; k < 2 * np; ++k) {
+        const int q = fill[ij[k]]++;
+        item[q] = k;            // 2 p + side
+        nbr[q] = ij[k ^ 1];
+      }
+      if (np > pair_cap) {
+        for (void* q : {(void*)d_pair_ij, (void*)d_pair_mean, (void*)d_pair_L, (void*)d_pair_A, (void*)d_pair_r, (void*)d_pair_item,
+                        (void*)d_pair_nbr, (void*)d_pair_O})
+          TRY(dfree(q));
+        TRY(dalloc(&d_pair_ij, 2 * (size_t)np, false));
+        TRY(dalloc(&d_pair_mean, 7 * (size_t)np, false));
+        TRY(dalloc(&d_pair_L, 36 * (size_t)np, false));
+        TRY(dalloc(&d_pair_A, 72 * (size_t)np, false));
+        TRY(dalloc(&d_pair_r, 6 * (size_t)np, false));
+        TRY(dalloc(&d_pair_item, 2 * (size_t)np, false));
+        TRY(dalloc(&d_pair_nbr, 2 * (size_t)np, false));
+        TRY(dalloc(&d_pair_O, 72 * (size_t)np, false));
+        pair_cap = np;
+      }
+      if (!d_pair_ptr) {
+        TRY(dalloc(&d_pair_ptr, (size_t)nc + 1, false));
+        TRY(dalloc(&d_pair_ov, 9 * (size_t)nc, false));
+      }
+      TRY(alloc_prior_diag());
+      CU(cudaMemcpyAsync(d_pair_ij, ij.data(), ij.size() * sizeof(int), cudaMemcpyHostToDevice, stream));
+      CU(cudaMemcpyAsync(d_pair_mean, mean.data(), mean.size() * sizeof(S), cudaMemcpyHostToDevice, stream));
+      CU(cudaMemcpyAsync(d_pair_L, Lsq.data(), Lsq.size() * sizeof(S), cudaMemcpyHostToDevice, stream));
+      CU(cudaMemcpyAsync(d_pair_item, item.data(), item.size() * sizeof(int), cudaMemcpyHostToDevice, stream));
+      CU(cudaMemcpyAsync(d_pair_nbr, nbr.data(), nbr.size() * sizeof(int), cudaMemcpyHostToDevice, stream));
+      CU(cudaMemcpyAsync(d_pair_ptr, ptr.data(), ptr.size() * sizeof(int), cudaMemcpyHostToDevice, stream));
+      CU(cudaStreamSynchronize(stream));
+    }
+    n_pairs = np;
+    D.pair_ptr = d_pair_ptr;
+    D.pair_nbr = d_pair_nbr;
+    D.pair_O = d_pair_O;
+    return priors_changed();
   }
 
   // launch with optional programmatic dependent launch (the kernel may start before its predecessor in the stream has
@@ -719,8 +833,12 @@ struct Solver : rba_handle {
     k_sum_partials<6><<<1, 256, 0, stream>>>(d_epart, EBLOCKS, d_red);
     launches += 2;
     rc = allreduce_scalars(6); if (rc) return rc;
-    if (D.prior_H) {  // + sum of 1/2 |L e|^2, once, after the sum over the shards
+    if (has_abs_prior) {  // + sum of 1/2 |L e|^2, once, after the sum over the shards
       k_prior_cost<S><<<1, 256, 0, stream>>>(D.cams, d_prior_mean, d_prior_L, nc, d_red, d_flags);
+      ++launches;
+    }
+    if (n_pairs > 0) {  // + the pair priors' 1/2 |L e|^2, likewise
+      k_pair_cost<S><<<1, 256, 0, stream>>>(D.cams, d_pair_ij, d_pair_mean, d_pair_L, n_pairs, d_red, d_flags);
       ++launches;
     }
     CU(cudaMemcpyAsync(h_res->error, d_red, sizeof(h_res->error), cudaMemcpyDeviceToHost, stream));
@@ -764,9 +882,14 @@ struct Solver : rba_handle {
     k_jp_norms<S><<<grid_for(L.nslots, 256, 8), 256, 0, stream>>>(D, ko, d_flags);
     ++launches;
     rc = camera_reduce(d_csr_obs_slots, d_csr_obs_items, n_obs_items, d_csr_obs_item_ptr, D.diag2); if (rc) return rc;
-    if (D.prior_H) {  // prior Jacobian and its column norms (scaling from the whole Jacobian), after the sum over the shards
+    if (has_abs_prior) {  // prior Jacobian and its column norms (scaling from the whole Jacobian), after the sum over the shards
       k_prior_linearize<S><<<(nc + 127) / 128, 128, 0, stream>>>(D.cams, d_prior_mean, d_prior_L, nc, D.diag2, d_prior_A, d_prior_r);
       ++launches;
+    }
+    if (n_pairs > 0) {  // pair-prior blocks and their column norms, likewise
+      k_pair_linearize<S><<<(n_pairs + 127) / 128, 128, 0, stream>>>(D.cams, d_pair_ij, d_pair_mean, d_pair_L, n_pairs, d_pair_A, d_pair_r);
+      k_pair_diag2<S><<<(nc + 127) / 128, 128, 0, stream>>>(d_pair_A, d_pair_ptr, d_pair_item, nc, D.diag2);
+      launches += 2;
     }
     k_scaling<S><<<(9 * nc + 255) / 256, 256, 0, stream>>>(D.diag2, D.scaling, 9 * nc, (S)ko.jacobi_eps);
     // pass B: linearize (scaled) + Jl scaling + Householder QR + panel write
@@ -779,10 +902,16 @@ struct Solver : rba_handle {
       // JACOBI: D (sum Jp^T Jp) D from the stored scaled Jacobians (Power-SC: these blocks are Hpp, sc/linearization_power_sc.hpp:92-128) (ref: ipp:554-569, block_sparse_matrix.hpp:89-100)
       rc = precond_blocks(0, D.jblocks, nullptr, true); if (rc) return rc;
     }
-    if (D.prior_H) {  // scaled prior Jacobian, A^T A (+ into the JACOBI blocks), A^T r
-      const bool jac = opt.preconditioner_type == 0 || opt.solver_type == 2;
+    const bool jac = opt.preconditioner_type == 0 || opt.solver_type == 2;
+    if (has_abs_prior) {  // scaled prior Jacobian, A^T A (+ into the JACOBI blocks), A^T r
       k_prior_scale<S><<<(nc + 127) / 128, 128, 0, stream>>>(d_prior_A, d_prior_r, D.scaling, nc, d_prior_H, d_prior_g, jac ? D.jblocks : nullptr);
       ++launches;
+    }
+    if (n_pairs > 0) {  // scaled pair blocks; their diagonal blocks and A^T r added to the absolute priors', the O_ij of every edge
+      k_pair_scale<S><<<(n_pairs + 127) / 128, 128, 0, stream>>>(d_pair_A, d_pair_ij, D.scaling, n_pairs);
+      k_pair_accum<S><<<(nc + 127) / 128, 128, 0, stream>>>(d_pair_A, d_pair_r, d_pair_ptr, d_pair_item, nc, (int)has_abs_prior,
+                                                            d_prior_H, d_prior_g, jac ? D.jblocks : nullptr, d_pair_O);
+      launches += 2;
     }
     if (panel_form) {
       // rows 3..2n-1 of the Q2 panels do not change with lambda: their part of the gradient (ipp:443-466) and of the
@@ -870,9 +999,18 @@ struct Solver : rba_handle {
   int pcg_vec(int i, int mode, bool pdl, int is_last, S lambda, bool fused_ar = false, bool from_partials = false) {
     PeerComm c = pc;
     if (!fused_ar) c.nranks = 1;
+    if (D.pair_ov) {  // pair priors: O v of the step's vector (v = x in the refresh's second half, else p) into D.pair_ov first
+      if (mode != 3) TRY(pair_ov(mode == 2 ? D.x : D.p, pdl));
+      return launch_ex(k_pcg_vec<S, true, true>, pcg_cluster, VEC_THREADS, 0, pdl, pcg_cluster, D, d_state, lambda, i, mode, (double)opt.eta,
+                       (int)opt.min_linear_solver_iterations, is_last, (int)pdl, c, ar_seq, from_partials ? op_item_ptr : (const int*)nullptr, d_prog);
+    }
     auto kern = D.prior_H ? k_pcg_vec<S, true> : k_pcg_vec<S, false>;
     return launch_ex(kern, pcg_cluster, VEC_THREADS, 0, pdl, pcg_cluster, D, d_state, lambda, i, mode, (double)opt.eta,
                      (int)opt.min_linear_solver_iterations, is_last, (int)pdl, c, ar_seq, from_partials ? op_item_ptr : (const int*)nullptr, d_prog);
+  }
+  // D.pair_ov = sum_j O_ij v_j (k_pair_ov), ahead of the vector step that consumes it
+  int pair_ov(const S* v, bool pdl) {
+    return launch_ex(k_pair_ov<S>, (9 * nc + 255) / 256, 256, 0, pdl, 1, D, (const PcgState*)d_state, v);
   }
   // The hand-over through per-segment sums is taken when a cluster CTA's share of the cameras fits the vector kernel's
   // register-resident layout (9 ceil(nc / cluster) <= VEC_THREADS VEC_EPT: <= 1808 cameras with a 16-CTA cluster, <= 904
@@ -933,11 +1071,14 @@ struct Solver : rba_handle {
     TRY(start(ev_pcg));
     CU(cudaMemsetAsync(d_state, 0, sizeof(PcgState), stream));
     const int order = opt.power_order;
-    TRY(launch_ex(k_power_vec<S>, pcg_cluster, VEC_THREADS, 0, false, pcg_cluster, D, d_state, 0, (double)opt.eta, 0, 0));
+    // pair priors: the series on Hpp^-1 (E_0 - O), O p from k_pair_ov ahead of each term (DESIGN.md section 15)
+    auto kern = D.pair_ov ? k_power_vec<S, true> : k_power_vec<S, false>;
+    TRY(launch_ex(kern, pcg_cluster, VEC_THREADS, 0, false, pcg_cluster, D, d_state, 0, (double)opt.eta, 0, 0));
     TRY(enqueue_polled(order, opt.pcg_check_period, [&](int i) -> int {
       matvec_kernels(D.p, &d_state->done, true, 1);
       TRY(cam_reduce_final(false, 0, true));
-      return launch_ex(k_power_vec<S>, pcg_cluster, VEC_THREADS, 0, true, pcg_cluster, D, d_state, i, (double)opt.eta, (int)(i == order), 1);
+      if (D.pair_ov) TRY(pair_ov(D.p, true));
+      return launch_ex(kern, pcg_cluster, VEC_THREADS, 0, true, pcg_cluster, D, d_state, i, (double)opt.eta, (int)(i == order), 1);
     }));
     CU(cudaMemcpyAsync(&h_state[0], d_state, sizeof(PcgState), cudaMemcpyDeviceToHost, stream));
     if (inc_out) CU(cudaMemcpyAsync(inc_out, D.inc, (size_t)9 * nc * sizeof(S), cudaMemcpyDeviceToHost, stream));
@@ -1087,8 +1228,12 @@ struct Solver : rba_handle {
     k_sum_partials<1><<<1, 256, 0, stream>>>(d_epart, grid, d_red);
     launches += 2;
     rc = allreduce_scalars(1); if (rc) return rc;
-    if (D.prior_H) {  // the prior part of the model cost change, once, after the sum over the shards
+    if (has_abs_prior) {  // the prior part of the model cost change, once, after the sum over the shards
       k_prior_ldiff<S><<<1, 256, 0, stream>>>(d_prior_A, d_prior_r, D.inc, nc, d_red);
+      ++launches;
+    }
+    if (n_pairs > 0) {  // the pair priors' part, likewise
+      k_pair_ldiff<S><<<1, 256, 0, stream>>>(d_pair_A, d_pair_r, d_pair_ij, D.inc, n_pairs, d_red);
       ++launches;
     }
     rc = stop(ev_backsub); if (rc) return rc;
@@ -1539,6 +1684,9 @@ int32_t rba_backup(rba_handle* h) { return h->backup(); }
 int32_t rba_restore(rba_handle* h) { return h->restore(); }
 int32_t rba_set_camera_fixed(rba_handle* h, const uint8_t* flags) { return h->set_camera_fixed(flags); }
 int32_t rba_set_camera_prior(rba_handle* h, const void* mean, const void* sqrt_info) { return h->set_camera_prior(mean, sqrt_info); }
+int32_t rba_set_camera_pair_prior(rba_handle* h, int32_t num_pairs, const int32_t* pairs, const void* mean, const void* sqrt_info) {
+  return h->set_camera_pair_prior(num_pairs, pairs, mean, sqrt_info);
+}
 int32_t rba_compute_error(rba_handle* h, rba_residual_info* out) { return h->compute_error(out); }
 int32_t rba_linearize(rba_handle* h) { return h->linearize(); }
 

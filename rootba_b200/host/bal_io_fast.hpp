@@ -144,6 +144,10 @@ class BalProblemSoA {
   // Gaussian camera priors (rba_set_camera_prior), forwarded by LinearizorQR::create; empty = no priors.
   std::vector<double> camera_prior_mean;       // [nc][10] qx,qy,qz,qw, centre, f, k1, k2
   std::vector<double> camera_prior_sqrt_info;  // [nc][81] row-major L
+  // Relative pose priors between pairs of cameras (rba_set_camera_pair_prior), forwarded by LinearizorQR::create; empty = none.
+  std::vector<int32_t> camera_pair_prior_pairs;    // [m][2] (i, j)
+  std::vector<double> camera_pair_prior_mean;      // [m][7] qx,qy,qz,qw, t0
+  std::vector<double> camera_pair_prior_sqrt_info; // [m][36] row-major L
 
   int num_cameras() const { return nc; }
   int num_landmarks() const { return nl; }

@@ -226,6 +226,11 @@ class BalProblem {
   // Gaussian camera priors (rba_set_camera_prior), forwarded by LinearizorQR::create; empty = no priors.  Not in the reference.
   std::vector<double> camera_prior_mean;       // [nc][10] qx,qy,qz,qw (R0), camera centre c0, f0, k1_0, k2_0
   std::vector<double> camera_prior_sqrt_info;  // [nc][81] row-major square-root information L
+  // Relative pose priors between pairs of cameras (rba_set_camera_pair_prior), forwarded by LinearizorQR::create; empty = none.
+  // Not in the reference.
+  std::vector<int32_t> camera_pair_prior_pairs;    // [m][2] cameras (i, j)
+  std::vector<double> camera_pair_prior_mean;      // [m][7] qx,qy,qz,qw (R0), t0 of T_i T_j^-1
+  std::vector<double> camera_pair_prior_sqrt_info; // [m][36] row-major square-root information L
 
  private:
   static void fail(FILE* f, const std::string& path) { std::fclose(f); throw std::runtime_error("Failed to parse '" + path + "'"); }

@@ -185,6 +185,15 @@ class LinearizorQR {
       const VecX L(bp.camera_prior_sqrt_info.begin(), bp.camera_prior_sqrt_info.end());
       check(rba_set_camera_prior(h_, m.data(), L.data()));
     }
+    if (!bp.camera_pair_prior_pairs.empty()) {
+      const size_t np = bp.camera_pair_prior_pairs.size() / 2;
+      if (bp.camera_pair_prior_pairs.size() != 2 * np || bp.camera_pair_prior_mean.size() != 7 * np ||
+          bp.camera_pair_prior_sqrt_info.size() != 36 * np)
+        throw std::runtime_error("pair priors must have 2 camera indices, 7 mean and 36 sqrt_info entries per pair");
+      const VecX m(bp.camera_pair_prior_mean.begin(), bp.camera_pair_prior_mean.end());
+      const VecX L(bp.camera_pair_prior_sqrt_info.begin(), bp.camera_pair_prior_sqrt_info.end());
+      check(rba_set_camera_pair_prior(h_, (int32_t)np, bp.camera_pair_prior_pairs.data(), m.data(), L.data()));
+    }
   }
   Problem& bal_problem_;
   SolverSummary* summary_ = nullptr;

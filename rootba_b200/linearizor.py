@@ -97,13 +97,42 @@ def _camera_prior_arrays(prior, num_cameras: int, dtype):
     return mean, sqrt_info
 
 
+def _camera_pair_prior_arrays(prior, num_cameras: int, dtype):
+    """None, or validated contiguous copies (pairs [m,2] int32, mean [m,7], sqrt_info [m,6,6]) of pair priors in the problem's
+    dtype"""
+    if prior is None:
+        return None
+    pairs, mean, sqrt_info = prior
+    pairs = np.array(pairs, dtype=np.int32, order="C", copy=True)
+    mean = np.array(mean, dtype=dtype, order="C", copy=True)
+    sqrt_info = np.array(sqrt_info, dtype=dtype, order="C", copy=True)
+    m = pairs.shape[0] if pairs.ndim == 2 else -1
+    if pairs.shape != (m, 2):
+        raise ValueError(f"camera_pair_prior pairs must have shape (m, 2), got {pairs.shape}")
+    if mean.shape != (m, 7):
+        raise ValueError(f"camera_pair_prior mean must have shape ({m}, 7), got {mean.shape}")
+    if sqrt_info.shape != (m, 6, 6):
+        raise ValueError(f"camera_pair_prior sqrt_info must have shape ({m}, 6, 6), got {sqrt_info.shape}")
+    if np.any(pairs < 0) or np.any(pairs >= num_cameras) or np.any(pairs[:, 0] == pairs[:, 1]):
+        raise ValueError(f"camera_pair_prior pairs must join two different cameras in [0, {num_cameras})")
+    if not (np.all(np.isfinite(mean)) and np.all(np.isfinite(sqrt_info))):
+        raise ValueError("camera_pair_prior entries must be finite")
+    qn = np.linalg.norm(mean[:, :4].astype(np.float64), axis=1)
+    if np.any(np.abs(qn - 1.0) > 1e-3):
+        raise ValueError(f"camera_pair_prior mean quaternions must have norm 1 (within 1e-3); pair {int(np.argmax(np.abs(qn - 1.0)))} has {qn.max():.6g}")
+    return pairs, mean, sqrt_info
+
+
 class BalProblem:
     """SoA BalProblem: cameras [nc,10] (quat xyzw, t, f,k1,k2), landmarks [nl,3], observations in
     CSR-by-landmark order with ascending camera index.  `camera_fixed` (not in the reference): None or one uint8 of FIX_*
     bits per camera, held constant by the solver; forwarded to an attached LinearizorQR on assignment.
     `camera_prior` (not in the reference): None or (mean [nc,10], sqrt_info [nc,9,9]), a Gaussian prior per camera with the
     cost 1/2 |L e|^2, e = (centre - c0, Log(R R0^T), f - f0, k1 - k1_0, k2 - k2_0) (rba_set_camera_prior, DESIGN.md section 14);
-    mean rows are (qx,qy,qz,qw of R0, camera centre c0, f0, k1_0, k2_0).  Forwarded to an attached LinearizorQR on assignment."""
+    mean rows are (qx,qy,qz,qw of R0, camera centre c0, f0, k1_0, k2_0).  Forwarded to an attached LinearizorQR on assignment.
+    `camera_pair_prior` (not in the reference): None or (pairs [m,2] int32, mean [m,7], sqrt_info [m,6,6]), relative pose priors
+    T_i T_j^-1 ~ (R0, t0) with the cost 1/2 |L e|^2, e = (t_i - R_i R_j^T t_j - t0, Log(R_i R_j^T R0^T))
+    (rba_set_camera_pair_prior, DESIGN.md section 15); mean rows are (qx,qy,qz,qw of R0, t0).  Forwarded likewise."""
 
     def __init__(self, cams, lms, lm_off, obs_cam, obs_xy, dtype=np.float64):
         self.dtype = np.dtype(dtype)
@@ -118,6 +147,18 @@ class BalProblem:
         self._linearizor = None
         self._camera_fixed = None
         self._camera_prior = None
+        self._camera_pair_prior = None
+
+    @property
+    def camera_pair_prior(self):
+        return self._camera_pair_prior
+
+    @camera_pair_prior.setter
+    def camera_pair_prior(self, prior):
+        p = _camera_pair_prior_arrays(prior, self.num_cameras(), self.dtype)
+        if self._linearizor is not None:
+            self._linearizor._upload_camera_pair_prior(p)  # raises on rejection: the previous pair priors stay in force
+        self._camera_pair_prior = p
 
     @property
     def camera_prior(self):
@@ -244,6 +285,8 @@ class LinearizorQR:
             self._upload_camera_fixed()
         if bal_problem.camera_prior is not None:
             self._upload_camera_prior(bal_problem.camera_prior)
+        if bal_problem.camera_pair_prior is not None:
+            self._upload_camera_pair_prior(bal_problem.camera_pair_prior)
 
     # factory like Linearizor::create (linearizor.cpp:47-65)
     @staticmethod
@@ -289,6 +332,17 @@ class LinearizorQR:
             check(_lib.lib().rba_set_camera_prior(self.h, None, None))
         else:
             check(_lib.lib().rba_set_camera_prior(self.h, _p(prior[0]), _p(prior[1])))
+
+    def set_camera_pair_prior(self, prior):
+        """relative pose priors (rba_set_camera_pair_prior): None, or (pairs [m,2], mean [m,7], sqrt_info [m,6,6]).  Needs a new
+        linearize before the next solve; the priors are stored on the BalProblem."""
+        self.bal_problem.camera_pair_prior = prior  # validates and forwards to _upload_camera_pair_prior
+
+    def _upload_camera_pair_prior(self, prior):
+        if prior is None:
+            check(_lib.lib().rba_set_camera_pair_prior(self.h, C.c_int32(0), None, None, None))
+        else:
+            check(_lib.lib().rba_set_camera_pair_prior(self.h, C.c_int32(len(prior[0])), _p(prior[0]), _p(prior[1]), _p(prior[2])))
 
     def _backup(self):
         check(_lib.lib().rba_backup(self.h))
