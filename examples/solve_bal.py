@@ -3,6 +3,7 @@
 
     python examples/solve_bal.py problem-49-7776-pre.txt [--float] [--max-num-iterations 20] [--operator-form DENSE|IMPLICIT]
         [--fix-intrinsics] [--fix-cameras I,J,...] [--camera-prior FILE.npz] [--camera-pair-prior FILE.npz]
+        [--covariance OUT.npz]
 
 Mirrors what `bal_qr --input ...` of the reference does (src/app/bal_qr.cpp): load + normalise (bal_problem.cpp:773-852),
 optimize_lm_ours with the QR linearizor (solver/bal_bundle_adjustment.cpp:249-544), log (bal/ba_log.hpp)."""
@@ -37,6 +38,10 @@ def main():
                     help="relative pose priors between pairs of cameras: arrays `pairs` [m, 2] (i, j), `mean` [m, 7] (qx,qy,qz,qw, t "
                          "of T_i T_j^-1) and `sqrt_info` [m, 6, 6] in the coordinates of the loaded (normalised) problem "
                          "(DESIGN.md section 15)")
+    ap.add_argument("--covariance", default=None, metavar="OUT.npz",
+                    help="after the solve, write the marginal covariances `cam` [nc, 9, 9] (tx,ty,tz, rx,ry,rz, f,k1,k2) and `lm` "
+                         "[nl, 3, 3] at the final state (DESIGN.md section 16); the gauge must be fixed by priors or held "
+                         "parameters")
     args = ap.parse_args()
     try:
         fix_cameras = [int(v) for v in args.fix_cameras.split(",")] if args.fix_cameras else []
@@ -77,6 +82,14 @@ def main():
     print(summary["termination_type"], summary["message"])
     rb.save_ba_log(args.log_path, summary, problem, args.input, {"load": t_load, "optimize": summary["total_time"]})
     print("wrote", args.log_path)
+    if args.covariance:
+        lin = rb.LinearizorQR.create(problem, options)  # at the final state, with the same priors and held parameters
+        try:
+            cam, lm = lin.covariance()
+        finally:
+            lin.close()
+        np.savez(args.covariance, cam=cam, lm=lm)
+        print("wrote", args.covariance)
 
 
 if __name__ == "__main__":

@@ -283,6 +283,26 @@ int32_t rba_set_camera_prior(rba_handle* h, const void* mean, const void* sqrt_i
 int32_t rba_set_camera_pair_prior(rba_handle* h, int32_t num_pairs, const int32_t* pairs, const void* mean,
                                   const void* sqrt_info);
 
+/* ---- Marginal covariances (DESIGN.md section 16) ------------------------------------------ */
+
+/* Not in the reference.  DESIGN.md section 16.  The covariance of the Gauss-Newton step of the total objective (reprojection
+ * terms + camera priors + pair priors) at lambda = 0 and the handle's current state: the inverse of H = J^T J, with J the rows
+ * rba_linearize would build (sqrt(w)-weighted by the robust norm, the rows use_valid_projections_only drops set to zero), and
+ * the parameters held by rba_set_camera_fixed as constants (their rows and columns are exactly 0).  Evaluated in float64 for
+ * either Scalar; unscaled (no Jacobi scaling); independent of solver_type, operator_form, stage2_form, preconditioner_type and
+ * the QR variant (bit-identical output within one Scalar).
+ *   cam_cov [81*Nc] double or NULL: per camera the 9x9 marginal block, row-major, in the order of the increment
+ *     (tx,ty,tz, rx,ry,rz, f,k1,k2) = (v, w, f, k1, k2) with R' = Exp(w) R, t' = Exp(w) t + v;
+ *   lm_cov [9*Nl] double or NULL: per landmark (problem order) its 3x3 marginal block; all NaN for a landmark whose Jl^T Jl has
+ *     rank < 3 (e.g. one valid observation) -- it is eliminated with the pseudo-inverse and the other outputs stay valid.
+ * No prior rba_linearize is needed, and nothing of the handle changes (state, linearisation, device-resident increment, error
+ * cache, timings); scratch device memory is allocated for the call and freed before it returns.
+ * RBA_NUMERICAL_FAILURE: a Cholesky pivot <= 1e-10 of the equilibrated reduced camera matrix (gauge not fixed, or a free camera
+ *   without observations and prior); the outputs are not written and rba_last_error names the camera and increment entry.
+ * RBA_ERR_UNSUPPORTED: nranks > 1, or the dense matrix and scratch do not fit in free device memory (the message gives the bytes).
+ * RBA_ERR_INVALID_ARGUMENT: both pointers NULL. */
+int32_t rba_compute_covariance(rba_handle* h, double* cam_cov, double* lm_cov);
+
 /* ---- Linearizor interface (solver/linearizor.hpp:56-82) ---------------------------------- */
 
 /* LinearizorBase::compute_error (linearizor_base.cpp:59-67) -> BalBundleAdjustmentHelper::compute_error

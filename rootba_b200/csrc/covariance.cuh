@@ -1,0 +1,524 @@
+// Marginal covariances of the cameras and landmarks (rba_compute_covariance, DESIGN.md section 16).
+//
+// Everything here is float64, also for a float32 handle (the state, observations and prior arrays are widened).  The
+// pipeline, on the solver stream:
+//   1. k_cov_landmark     per landmark: weighted Jp, Jl; Hll = Jl^T Jl = V Lambda V^T; K_i = Lambda+^-1/2 V+^T Jl_i^T Jp_i
+//   2. k_cov_assemble     lower triangle of the reduced camera matrix S = sum_l (delta_ij Jp_i^T Jp_i - K_i^T K_j), one
+//                         warp per co-visible camera pair over a host-built term list (fixed order, no atomics)
+//      k_cov_priors       + the absolute and pair priors' blocks, re-evaluated in double in the unscaled space
+//      k_cov_diag/_equil  held rows and columns -> identity, equilibration D S D with D = diag(S)^-1/2, padding -> identity
+//   3. dense SPD inverse in place: blocked potrf, trtri, lauum (LAPACK's potri) with the diagonal-tile kernels and one
+//      FP64 tensor-core GEMM (mma.sync m8n8k4 .f64) for every O(N^3) update
+//   4. k_cov_cam_out      9x9 diagonal blocks of D S^-1 D;  k_cov_lm_marginal  per landmark
+//                         W (I + sum_ab K_a S^-1_ab K_b^T) W^T,  W = V Lambda^-1/2
+// The dense matrix is column-major with a leading dimension padded to a multiple of COV_TB; only its lower triangle is
+// meaningful.
+#pragma once
+
+#include "kernels.cuh"
+
+namespace rba {
+
+constexpr int COV_TB = 64;               // diagonal tile of the blocked factorisation = GEMM block tile
+constexpr int COV_BK = 16;               // k slice of the GEMM held in shared memory
+constexpr int COV_LDS = COV_TB + 4;      // shared row stride: = 4 (mod 16) doubles, conflict-free fragment loads
+constexpr double COV_EIG_DROP = 1e-10;   // eigenvalues of Hll <= this * lambda_max are dropped (pseudo-inverse)
+constexpr double COV_PIVOT_TAU = 1e-10;  // a Cholesky pivot <= this of the equilibrated reduced matrix: singular (no gauge)
+
+// ------------------------------------------------------------------------------------------------
+// 1. per-landmark elimination
+// ------------------------------------------------------------------------------------------------
+// symmetric 3x3 eigendecomposition by cyclic Jacobi rotations: on return A holds the eigenvalues on its diagonal and the
+// columns of V (row-major) the eigenvectors.  Fixed number of sweeps: the same operations on every run.
+__device__ __forceinline__ void cov_sym3_eig(double (&A)[9], double (&V)[9]) {
+#pragma unroll
+  for (int k = 0; k < 9; ++k) V[k] = (k % 4 == 0) ? 1.0 : 0.0;
+  for (int sweep = 0; sweep < 8; ++sweep) {
+#pragma unroll
+    for (int pq = 0; pq < 3; ++pq) {
+      const int p = pq == 2 ? 1 : 0, q = pq == 0 ? 1 : 2;
+      const double apq = A[3 * p + q];
+      if (apq == 0.0) continue;
+      const double th = (A[3 * q + q] - A[3 * p + p]) / (2.0 * apq);
+      const double t = (th >= 0 ? 1.0 : -1.0) / (fabs(th) + sqrt(th * th + 1.0));
+      const double c = 1.0 / sqrt(t * t + 1.0), s = t * c;
+#pragma unroll
+      for (int k = 0; k < 3; ++k) {  // columns p, q
+        const double akp = A[3 * k + p], akq = A[3 * k + q];
+        A[3 * k + p] = c * akp - s * akq;
+        A[3 * k + q] = s * akp + c * akq;
+      }
+#pragma unroll
+      for (int k = 0; k < 3; ++k) {  // rows p, q
+        const double apk = A[3 * p + k], aqk = A[3 * q + k];
+        A[3 * p + k] = c * apk - s * aqk;
+        A[3 * q + k] = s * apk + c * aqk;
+      }
+#pragma unroll
+      for (int k = 0; k < 3; ++k) {
+        const double vkp = V[3 * k + p], vkq = V[3 * k + q];
+        V[3 * k + p] = c * vkp - s * vkq;
+        V[3 * k + q] = s * vkp + c * vkq;
+      }
+    }
+  }
+}
+
+// Warp per landmark (problem order).  Re-linearises every observation in double with the weights and validity rule of
+// rba_linearize (unscaled), then writes per slot jpw [18] = sqrt(w) Jp and kb [27] = K (3x9 row-major, rows of dropped
+// eigenvalues zero), and per landmark wl [9] = V Lambda^-1/2 (row-major; columns of dropped eigenvalues zero) and its rank.
+template <class S>
+__global__ void __launch_bounds__(128) k_cov_landmark(DevPtrs<S> D, KOpts o, const int* __restrict__ lm_slot0,
+                                                      const int* __restrict__ lm_n, int nl, double* __restrict__ jpw,
+                                                      double* __restrict__ kb, double* __restrict__ wl, int* __restrict__ rank) {
+  const int lane = threadIdx.x & 31;
+  const int warps = gridDim.x * (blockDim.x >> 5);
+  for (int lm = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); lm < nl; lm += warps) {
+    const int s0 = lm_slot0[lm], n = lm_n[lm];
+    const double pw[3] = {(double)D.lms[3 * lm], (double)D.lms[3 * lm + 1], (double)D.lms[3 * lm + 2]};
+    double h[6] = {0, 0, 0, 0, 0, 0};  // Hll: 00 01 02 11 12 22
+    for (int i = lane; i < n; i += 32) {
+      const int s = s0 + i;
+      const double obs[2] = {(double)D.slot_xy[2 * s], (double)D.slot_xy[2 * s + 1]};
+      double cam[10];
+      const S* cp = D.cams + 10 * (size_t)D.slot_cam[s];
+#pragma unroll
+      for (int k = 0; k < 10; ++k) cam[k] = (double)cp[k];
+      double res[2], Jp[18], Jl[6];
+      linearize_point<double, true>(obs, pw, cam, res, Jp, Jl);
+      bool keep = true;
+      if (o.use_valid_projections_only) {  // the handle's own validity threshold (that of its Scalar)
+        double R[9];
+        quat_to_rot(cam, R);
+        const double z = R[6] * pw[0] + R[7] * pw[1] + R[8] * pw[2] + cam[6];
+        keep = z >= (double)ST<S>::eps_sqrt();
+      }
+      double sw = 0.0;
+      if (keep) {
+        double err, w;
+        error_weight(o, res[0] * res[0] + res[1] * res[1], err, w);
+        sw = sqrt(w);
+      }
+#pragma unroll
+      for (int k = 0; k < 18; ++k) jpw[18 * (size_t)s + k] = sw * Jp[k];
+#pragma unroll
+      for (int k = 0; k < 6; ++k) { Jl[k] *= sw; kb[27 * (size_t)s + k] = Jl[k]; }  // Jl parked in kb until K replaces it
+      h[0] += Jl[0] * Jl[0] + Jl[3] * Jl[3];
+      h[1] += Jl[0] * Jl[1] + Jl[3] * Jl[4];
+      h[2] += Jl[0] * Jl[2] + Jl[3] * Jl[5];
+      h[3] += Jl[1] * Jl[1] + Jl[4] * Jl[4];
+      h[4] += Jl[1] * Jl[2] + Jl[4] * Jl[5];
+      h[5] += Jl[2] * Jl[2] + Jl[5] * Jl[5];
+    }
+#pragma unroll
+    for (int k = 0; k < 6; ++k) h[k] = warp_sum(h[k]);  // butterfly: the same sum in every lane
+    double A[9] = {h[0], h[1], h[2], h[1], h[3], h[4], h[2], h[4], h[5]}, V[9];
+    cov_sym3_eig(A, V);
+    const double lmax = fmax(A[0], fmax(A[4], A[8]));
+    double W[9];
+    int r = 0;
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+      const double ev = A[4 * k];
+      const bool kept = lmax > 0.0 && ev > COV_EIG_DROP * lmax;
+      r += kept ? 1 : 0;
+      const double f = kept ? 1.0 / sqrt(ev) : 0.0;
+#pragma unroll
+      for (int row = 0; row < 3; ++row) W[3 * row + k] = V[3 * row + k] * f;
+    }
+    if (lane == 0) {
+#pragma unroll
+      for (int k = 0; k < 9; ++k) wl[9 * (size_t)lm + k] = W[k];
+      rank[lm] = r;
+    }
+    for (int i = lane; i < n; i += 32) {
+      const int s = s0 + i;
+      double Jl[6], Jp[18];
+#pragma unroll
+      for (int k = 0; k < 6; ++k) Jl[k] = kb[27 * (size_t)s + k];
+#pragma unroll
+      for (int k = 0; k < 18; ++k) Jp[k] = jpw[18 * (size_t)s + k];
+      // K = W^T (Jl^T Jp)
+#pragma unroll
+      for (int k = 0; k < 3; ++k)
+#pragma unroll
+        for (int c = 0; c < 9; ++c) {
+          double v = 0.0;
+#pragma unroll
+          for (int a = 0; a < 3; ++a) v += W[3 * a + k] * (Jl[a] * Jp[c] + Jl[3 + a] * Jp[9 + c]);
+          kb[27 * (size_t)s + 9 * k + c] = v;
+        }
+    }
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
+// 2. assembly of the reduced camera matrix (unscaled), priors, held parameters, equilibration
+// ------------------------------------------------------------------------------------------------
+// Warp per co-visible camera pair (ca >= cb): block(ca, cb) = sum over its terms (sa, sb) of
+// [sa == sb] Jp_sa^T Jp_sa - K_sa^T K_sb, in the term order of the list.  Writes the lower triangle only.
+__global__ void __launch_bounds__(256) k_cov_assemble(const int2* __restrict__ blk_cam, const int* __restrict__ blk_ptr,
+                                                      const int2* __restrict__ terms, int nblk, const double* __restrict__ jpw,
+                                                      const double* __restrict__ kb, double* __restrict__ A, long long ld) {
+  const int lane = threadIdx.x & 31;
+  const int warps = gridDim.x * (blockDim.x >> 5);
+  for (int bi = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); bi < nblk; bi += warps) {
+    const int2 cc = blk_cam[bi];
+    const int t0 = blk_ptr[bi], t1 = blk_ptr[bi + 1];
+#pragma unroll
+    for (int u = 0; u < 3; ++u) {
+      const int e = lane + 32 * u, p = e / 9, q = e % 9;
+      if (e >= 81 || (cc.x == cc.y && p < q)) continue;
+      double acc = 0.0;
+      for (int t = t0; t < t1; ++t) {
+        const int2 st = terms[t];
+        const double* ka = kb + 27 * (size_t)st.x;
+        const double* kq = kb + 27 * (size_t)st.y;
+        double v = 0.0;
+        if (st.x == st.y) {
+          const double* j = jpw + 18 * (size_t)st.x;
+          v = j[p] * j[q] + j[9 + p] * j[9 + q];
+        }
+        v -= ka[p] * kq[q] + ka[9 + p] * kq[9 + q] + ka[18 + p] * kq[18 + q];
+        acc += v;
+      }
+      A[(9 * (long long)cc.x + p) + (9 * (long long)cc.y + q) * ld] = acc;
+    }
+  }
+}
+
+// Thread per camera c: adds to its block row (lower triangle) the absolute prior's A^T A and, over its incident pair sides
+// in list order, the pair blocks A_s^T A_s (diagonal) and A_s^T A_o (to the column block of the other camera o < c).
+// The blocks are those of k_prior_linearize / k_pair_linearize, unscaled, evaluated in double from the stored means and L.
+template <class S>
+__global__ void k_cov_priors(const S* __restrict__ cams, int nc, const S* __restrict__ pmean, const S* __restrict__ pL,
+                             const int* __restrict__ pairs, const S* __restrict__ qmean, const S* __restrict__ qL,
+                             const int* __restrict__ qptr, const int* __restrict__ qitem, const int* __restrict__ qnbr,
+                             double* __restrict__ A, long long ld) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= nc) return;
+  double* Acc = A + 9 * (long long)c + 9 * (long long)c * ld;  // diagonal block (c, c)
+  if (pmean) {
+    double cam[10], mean[10], e[9], Jinv[9], R[9];
+#pragma unroll
+    for (int k = 0; k < 10; ++k) { cam[k] = (double)cams[10 * (size_t)c + k]; mean[k] = (double)pmean[10 * (size_t)c + k]; }
+    prior_residual<double, true>(cam, mean, e, Jinv, R);
+    for (int i = 0; i < 9; ++i) {
+      double l[9], row[9];
+#pragma unroll
+      for (int k = 0; k < 9; ++k) l[k] = (double)pL[81 * (size_t)c + 9 * i + k];
+      // row i of L de/d(inc): de/dv = -R^T, dLog/dw = J_l^-1, identity on the intrinsics
+#pragma unroll
+      for (int j = 0; j < 3; ++j) row[j] = -(l[0] * R[3 * j] + l[1] * R[3 * j + 1] + l[2] * R[3 * j + 2]);
+#pragma unroll
+      for (int j = 0; j < 3; ++j) row[3 + j] = l[3] * Jinv[j] + l[4] * Jinv[3 + j] + l[5] * Jinv[6 + j];
+#pragma unroll
+      for (int j = 6; j < 9; ++j) row[j] = l[j];
+      for (int a = 0; a < 9; ++a)
+        for (int b = 0; b <= a; ++b) Acc[a + b * ld] += row[a] * row[b];
+    }
+  }
+  if (qptr) {
+    for (int q = qptr[c]; q < qptr[c + 1]; ++q) {
+      const int it = qitem[q], p = it >> 1, side = it & 1, o = qnbr[q];
+      double ci[10], cj[10], mean[7], e[6], M[9], tr[3], Jinv[9], JM[9];
+#pragma unroll
+      for (int k = 0; k < 10; ++k) {
+        ci[k] = (double)cams[10 * (size_t)pairs[2 * p] + k];
+        cj[k] = (double)cams[10 * (size_t)pairs[2 * p + 1] + k];
+      }
+#pragma unroll
+      for (int k = 0; k < 7; ++k) mean[k] = (double)qmean[7 * (size_t)p + k];
+      pair_residual<double, true>(ci, cj, mean, e, M, tr, Jinv);
+#pragma unroll
+      for (int a = 0; a < 3; ++a)
+#pragma unroll
+        for (int b = 0; b < 3; ++b) JM[3 * a + b] = Jinv[3 * a] * M[b] + Jinv[3 * a + 1] * M[3 + b] + Jinv[3 * a + 2] * M[6 + b];
+      double* Aco = A + 9 * (long long)c + 9 * (long long)o * ld;  // block (c, o), used when o < c
+      for (int i = 0; i < 6; ++i) {
+        double l[6], ri[6], rj[6];
+#pragma unroll
+        for (int k = 0; k < 6; ++k) l[k] = (double)qL[36 * (size_t)p + 6 * i + k];
+        // rows of A_i = (l_t, l_t (-[t_rel]x) + l_r J_l^-1) and A_j = (-l_t M, -l_r J_l^-1 M)
+#pragma unroll
+        for (int j = 0; j < 3; ++j) ri[j] = l[j];
+        ri[3] = -l[1] * tr[2] + l[2] * tr[1] + l[3] * Jinv[0] + l[4] * Jinv[3] + l[5] * Jinv[6];
+        ri[4] = l[0] * tr[2] - l[2] * tr[0] + l[3] * Jinv[1] + l[4] * Jinv[4] + l[5] * Jinv[7];
+        ri[5] = -l[0] * tr[1] + l[1] * tr[0] + l[3] * Jinv[2] + l[4] * Jinv[5] + l[5] * Jinv[8];
+#pragma unroll
+        for (int j = 0; j < 3; ++j) {
+          rj[j] = -(l[0] * M[j] + l[1] * M[3 + j] + l[2] * M[6 + j]);
+          rj[3 + j] = -(l[3] * JM[j] + l[4] * JM[3 + j] + l[5] * JM[6 + j]);
+        }
+        const double* own = side ? rj : ri;
+        const double* oth = side ? ri : rj;
+        for (int a = 0; a < 6; ++a) {
+          for (int b = 0; b <= a; ++b) Acc[a + b * ld] += own[a] * own[b];
+          if (o < c)
+            for (int b = 0; b < 6; ++b) Aco[a + b * ld] += own[a] * oth[b];
+        }
+      }
+    }
+  }
+}
+
+__device__ __forceinline__ bool cov_fixed(const uint8_t* __restrict__ cam_fixed, long long k) {
+  return cam_fixed && ((fixed_entry_mask(cam_fixed[k / 9]) >> (k % 9)) & 1u);
+}
+
+// d [np] = diag(S)^-1/2 (1 for held entries, the padding and a non-positive diagonal).  Thread per entry.
+__global__ void k_cov_diag(const double* __restrict__ A, long long ld, long long n, long long np,
+                           const uint8_t* __restrict__ cam_fixed, double* __restrict__ d) {
+  const long long k = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (k >= np) return;
+  double v = 1.0;
+  if (k < n && !cov_fixed(cam_fixed, k)) {
+    const double s = A[k + k * ld];
+    if (s > 0.0) v = 1.0 / sqrt(s);
+  }
+  d[k] = v;
+}
+
+// S <- D S D on the lower triangle; rows and columns of held entries and of the padding -> identity; upper triangle -> 0.
+// Thread per entry of a 32 x 8 patch, grid over the np x np matrix.
+__global__ void k_cov_equil(double* __restrict__ A, long long ld, long long n, long long np, const uint8_t* __restrict__ cam_fixed,
+                            const double* __restrict__ d) {
+  const long long r = blockIdx.x * 32LL + threadIdx.x;
+  const long long c = blockIdx.y * 8LL + threadIdx.y;
+  if (r >= np || c >= np) return;
+  double& a = A[r + c * ld];
+  if (r < c) { a = 0.0; return; }
+  if (r >= n || c >= n || cov_fixed(cam_fixed, r) || cov_fixed(cam_fixed, c)) { a = r == c ? 1.0 : 0.0; return; }
+  a = a * d[r] * d[c];
+}
+
+// ------------------------------------------------------------------------------------------------
+// 3. dense SPD inverse: diagonal-tile kernels (one CTA per COV_TB x COV_TB tile, in shared memory) and the DMMA GEMM
+// ------------------------------------------------------------------------------------------------
+// Cholesky of the lower triangle of tile (k0, k0), in place; upper part of the tile -> 0.  A pivot <= tau (or NaN) stores
+// the smallest such global index in *fail.
+__global__ void __launch_bounds__(256) k_cov_tile_potrf(double* __restrict__ A, long long ld, long long k0, double tau,
+                                                        int* __restrict__ fail) {
+  __shared__ double T[COV_TB][COV_TB + 1];
+  const int tid = threadIdx.x;
+  for (int e = tid; e < COV_TB * COV_TB; e += blockDim.x) T[e % COV_TB][e / COV_TB] = A[(k0 + e % COV_TB) + (k0 + e / COV_TB) * ld];
+  __syncthreads();
+  for (int j = 0; j < COV_TB; ++j) {
+    const double piv = T[j][j];
+    const double ljj = sqrt(piv);
+    if (tid == 0 && !(piv > tau)) atomicMin(fail, (int)(k0 + j));
+    __syncthreads();
+    if (tid == 0) T[j][j] = ljj;
+    for (int r = j + 1 + tid; r < COV_TB; r += blockDim.x) T[r][j] /= ljj;
+    __syncthreads();
+    const int m = COV_TB - 1 - j;
+    for (int e = tid; e < m * m; e += blockDim.x) {
+      const int r = j + 1 + e % m, c = j + 1 + e / m;
+      if (c <= r) T[r][c] -= T[r][j] * T[c][j];
+    }
+    __syncthreads();
+  }
+  for (int e = tid; e < COV_TB * COV_TB; e += blockDim.x) {
+    const int r = e % COV_TB, c = e / COV_TB;
+    A[(k0 + r) + (k0 + c) * ld] = r >= c ? T[r][c] : 0.0;
+  }
+}
+
+// Inverse of the lower-triangular tile (k0, k0) of A -> out (ldo), upper part 0.  Thread per column, forward substitution;
+// a thread reads back only the column it writes.
+__global__ void __launch_bounds__(COV_TB) k_cov_tile_trtri(const double* __restrict__ A, long long ld, long long k0,
+                                                           double* __restrict__ out, long long ldo) {
+  __shared__ double T[COV_TB][COV_TB + 1];
+  const int j = threadIdx.x;
+  for (int r = 0; r < COV_TB; ++r) T[r][j] = A[(k0 + r) + (k0 + j) * ld];
+  __syncthreads();
+  double* X = out + j * ldo;
+  for (int i = 0; i < COV_TB; ++i) {
+    double v = i == j ? 1.0 : 0.0;
+    for (int k = j; k < i; ++k) v -= T[i][k] * X[k];
+    X[i] = i >= j ? v / T[i][i] : 0.0;
+  }
+}
+
+// Tile (k0, k0) <- L^T L of its lower triangle L (LAPACK lauu2), lower triangle written, upper part 0.
+__global__ void __launch_bounds__(256) k_cov_tile_lauu2(double* __restrict__ A, long long ld, long long k0) {
+  __shared__ double T[COV_TB][COV_TB + 1];
+  const int tid = threadIdx.x;
+  for (int e = tid; e < COV_TB * COV_TB; e += blockDim.x) {
+    const int r = e % COV_TB, c = e / COV_TB;
+    T[r][c] = r >= c ? A[(k0 + r) + (k0 + c) * ld] : 0.0;
+  }
+  __syncthreads();
+  double out[COV_TB * COV_TB / 256];
+#pragma unroll
+  for (int u = 0; u < COV_TB * COV_TB / 256; ++u) {
+    const int e = tid + 256 * u, r = e % COV_TB, c = e / COV_TB;
+    double v = 0.0;
+    if (r >= c)
+      for (int k = r; k < COV_TB; ++k) v += T[k][r] * T[k][c];
+    out[u] = v;
+  }
+#pragma unroll
+  for (int u = 0; u < COV_TB * COV_TB / 256; ++u) {
+    const int e = tid + 256 * u;
+    A[(k0 + e % COV_TB) + (k0 + e / COV_TB) * ld] = out[u];
+  }
+}
+
+__device__ __forceinline__ void dmma_8x8x4(double& c0, double& c1, double a, double b) {
+  asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};"
+               : "+d"(c0), "+d"(c1) : "d"(a), "d"(b));
+}
+
+// C = alpha op(A) op(B) + beta C for column-major operands whose M, N, K are multiples of COV_TB; op(A)(i, k) = A(k, i) when
+// TA, op(B)(k, j) = B(j, k) when TB.  beta == 0 does not read C.  lower: only the tiles with row tile >= column tile.
+// ktri: op(A) is lower triangular by tiles (the k range of row tile i ends at (i + 1) COV_TB).
+// 256 threads = 8 warps as 2 (rows) x 4 (columns), a warp computes 32 x 16 of the 64 x 64 tile with 4 x 2 DMMA 8x8x4
+// fragments per k4 step; the next k slice is loaded into registers while the current one is multiplied.
+template <bool TA, bool TB>
+__global__ void __launch_bounds__(256) k_cov_dgemm(int M, int N, int K, double alpha, const double* __restrict__ A, long long lda,
+                                                   const double* __restrict__ B, long long ldb, double beta, double* __restrict__ C,
+                                                   long long ldc, int lower, int ktri) {
+  const int ti = blockIdx.x, tj = blockIdx.y;
+  if (lower && tj > ti) return;
+  __shared__ double As[COV_BK][COV_LDS];
+  __shared__ double Bs[COV_BK][COV_LDS];
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int gid = lane >> 2, tig = lane & 3;
+  const int wm = warp >> 2, wn = warp & 3;
+  const long long i0 = (long long)ti * COV_TB, j0 = (long long)tj * COV_TB;
+  const int kend = ktri ? min(K, (ti + 1) * COV_TB) : K;
+  constexpr int LD = COV_TB * COV_BK / 256;  // elements of each operand a thread loads per k slice
+  double ra[LD], rb[LD];
+  auto load = [&](int kt) {
+#pragma unroll
+    for (int u = 0; u < LD; ++u) {
+      const int e = tid + 256 * u;
+      if (!TA) ra[u] = A[(i0 + e % COV_TB) + (long long)(kt + e / COV_TB) * lda];
+      else ra[u] = A[(long long)(kt + e % COV_BK) + (i0 + e / COV_BK) * lda];
+      if (!TB) rb[u] = B[(long long)(kt + e % COV_BK) + (j0 + e / COV_BK) * ldb];
+      else rb[u] = B[(j0 + e % COV_TB) + (long long)(kt + e / COV_TB) * ldb];
+    }
+  };
+  auto stash = [&]() {
+#pragma unroll
+    for (int u = 0; u < LD; ++u) {
+      const int e = tid + 256 * u;
+      if (!TA) As[e / COV_TB][e % COV_TB] = ra[u];
+      else As[e % COV_BK][e / COV_BK] = ra[u];
+      if (!TB) Bs[e % COV_BK][e / COV_BK] = rb[u];
+      else Bs[e / COV_TB][e % COV_TB] = rb[u];
+    }
+  };
+  double acc[4][2][2];
+#pragma unroll
+  for (int mi = 0; mi < 4; ++mi)
+#pragma unroll
+    for (int ni = 0; ni < 2; ++ni) acc[mi][ni][0] = acc[mi][ni][1] = 0.0;
+  if (kend > 0) load(0);
+  for (int kt = 0; kt < kend; kt += COV_BK) {
+    __syncthreads();
+    stash();
+    __syncthreads();
+    if (kt + COV_BK < kend) load(kt + COV_BK);
+#pragma unroll
+    for (int ks = 0; ks < COV_BK / 4; ++ks) {
+      double a[4], b[2];
+#pragma unroll
+      for (int mi = 0; mi < 4; ++mi) a[mi] = As[4 * ks + tig][32 * wm + 8 * mi + gid];
+#pragma unroll
+      for (int ni = 0; ni < 2; ++ni) b[ni] = Bs[4 * ks + tig][16 * wn + 8 * ni + gid];
+#pragma unroll
+      for (int mi = 0; mi < 4; ++mi)
+#pragma unroll
+        for (int ni = 0; ni < 2; ++ni) dmma_8x8x4(acc[mi][ni][0], acc[mi][ni][1], a[mi], b[ni]);
+    }
+  }
+#pragma unroll
+  for (int mi = 0; mi < 4; ++mi)
+#pragma unroll
+    for (int ni = 0; ni < 2; ++ni)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const long long r = i0 + 32 * wm + 8 * mi + gid, c = j0 + 16 * wn + 8 * ni + 2 * tig + h;
+        double& out = C[r + c * ldc];
+        out = beta == 0.0 ? alpha * acc[mi][ni][h] : alpha * acc[mi][ni][h] + beta * out;
+      }
+}
+
+// ------------------------------------------------------------------------------------------------
+// 4. extraction
+// ------------------------------------------------------------------------------------------------
+// entry (r, c) of D S_eq^-1 D from the lower triangle; 0 in the rows and columns of held entries
+__device__ __forceinline__ double cov_sinv(const double* __restrict__ A, long long ld, const double* __restrict__ d,
+                                           const uint8_t* __restrict__ cam_fixed, long long r, long long c) {
+  if (cov_fixed(cam_fixed, r) || cov_fixed(cam_fixed, c)) return 0.0;
+  const double v = r >= c ? A[r + c * ld] : A[c + r * ld];
+  return v * d[r] * d[c];
+}
+
+// cam_cov [nc][81], thread per entry
+__global__ void k_cov_cam_out(const double* __restrict__ A, long long ld, const double* __restrict__ d,
+                              const uint8_t* __restrict__ cam_fixed, int nc, double* __restrict__ out) {
+  const long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (e >= 81LL * nc) return;
+  const long long c = e / 81;
+  const int p = (int)(e % 81) / 9, q = (int)(e % 9);
+  out[e] = cov_sinv(A, ld, d, cam_fixed, 9 * c + p, 9 * c + q);
+}
+
+// lm_cov [nl][9], warp per landmark: W (I + sum_ab K_a Sigma_ab K_b^T) W^T over the n^2 camera pairs of its track (lanes
+// over the pairs, fixed-order butterfly sum); all NaN when Hll has rank < 3.
+__global__ void __launch_bounds__(128) k_cov_lm_marginal(const double* __restrict__ A, long long ld, const double* __restrict__ d,
+                                                         const uint8_t* __restrict__ cam_fixed, const int* __restrict__ slot_cam,
+                                                         const int* __restrict__ lm_slot0, const int* __restrict__ lm_n, int nl,
+                                                         const double* __restrict__ kb, const double* __restrict__ wl,
+                                                         const int* __restrict__ rank, double* __restrict__ out) {
+  const int lane = threadIdx.x & 31;
+  const int warps = gridDim.x * (blockDim.x >> 5);
+  for (int lm = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); lm < nl; lm += warps) {
+    if (rank[lm] < 3) {
+      if (lane < 9) out[9 * (size_t)lm + lane] = __longlong_as_double(0x7ff8000000000000LL);
+      continue;
+    }
+    const int s0 = lm_slot0[lm], n = lm_n[lm];
+    double m[9];
+#pragma unroll
+    for (int k = 0; k < 9; ++k) m[k] = 0.0;
+    for (int t = lane; t < n * n; t += 32) {
+      const int a = t / n, b = t % n;
+      const long long ra = 9LL * slot_cam[s0 + a], rb = 9LL * slot_cam[s0 + b];
+      const double* ka = kb + 27 * (size_t)(s0 + a);
+      const double* kq = kb + 27 * (size_t)(s0 + b);
+      for (int p = 0; p < 9; ++p) {
+        double u[3] = {0.0, 0.0, 0.0};  // (Sigma_ab K_b^T) row p
+        for (int q = 0; q < 9; ++q) {
+          const double sv = cov_sinv(A, ld, d, cam_fixed, ra + p, rb + q);
+#pragma unroll
+          for (int l = 0; l < 3; ++l) u[l] += sv * kq[9 * l + q];
+        }
+#pragma unroll
+        for (int k = 0; k < 3; ++k)
+#pragma unroll
+          for (int l = 0; l < 3; ++l) m[3 * k + l] += ka[9 * k + p] * u[l];
+      }
+    }
+#pragma unroll
+    for (int k = 0; k < 9; ++k) m[k] = warp_sum(m[k]);
+    if (lane == 0) {
+      const double* W = wl + 9 * (size_t)lm;
+      double X[9];
+#pragma unroll
+      for (int k = 0; k < 9; ++k) X[k] = m[k] + (k % 4 == 0 ? 1.0 : 0.0);
+      for (int r = 0; r < 3; ++r)
+        for (int c = 0; c < 3; ++c) {
+          double v = 0.0;
+          for (int k = 0; k < 3; ++k)
+            for (int l = 0; l < 3; ++l) v += W[3 * r + k] * X[3 * k + l] * W[3 * c + l];
+          out[9 * (size_t)lm + 3 * r + c] = v;
+        }
+    }
+  }
+}
+
+}  // namespace rba

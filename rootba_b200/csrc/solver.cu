@@ -16,6 +16,7 @@
 #include "../../include/rootba_b200.h"
 #include "../host/bal_io_fast.hpp"
 #include "kernels.cuh"
+#include "covariance.cuh"
 #include "nccl_dyn.hpp"
 
 namespace rba {
@@ -65,6 +66,7 @@ struct rba_handle {
   virtual int get_precond(void* inv, void* blocks) = 0;
   virtual int right_multiply(const void* x, void* y) = 0;
   virtual int debug_get_block(int lm, void* out, int rows, int cols, void* jls) = 0;
+  virtual int compute_covariance(double* cam_cov, double* lm_cov) = 0;
   virtual int time_matvec(int reps, double* sec) = 0;
   virtual int timer_start() = 0;
   virtual int timer_stop(double* sec) = 0;
@@ -197,6 +199,12 @@ struct Solver : rba_handle {
   bool peer_ok = false;
   int ar_seq = 0, c_seq = 0, s_seq = 0;  // sequence numbers of the three flag families (operator output / vectors / scalars)
   std::vector<void*> ipc_opened;
+  // rba_compute_covariance (DESIGN.md section 16): the co-visible camera pairs and their (slot_a, slot_b) terms, and each
+  // landmark's first slot and track length, built at the first call
+  bool cov_ready = false;
+  int cov_nblk = 0;
+  int2* d_cov_blk_cam = nullptr; int* d_cov_blk_ptr = nullptr; int2* d_cov_terms = nullptr;
+  int* d_cov_lm_slot0 = nullptr; int* d_cov_lm_n = nullptr;
 
   ~Solver() override {
     if (comm && nccl) nccl->CommDestroy(comm);
@@ -1450,6 +1458,177 @@ struct Solver : rba_handle {
   void* stream_ptr() override { return (void*)stream; }
   int synchronize() override { CU(cudaStreamSynchronize(stream)); return RBA_OK; }
 
+  // ------------------------------------------------------------------------------------------
+  // Marginal covariances (DESIGN.md section 16).  Nothing of the handle changes: the scratch is allocated for the call and
+  // freed before it returns; the state, the linearisation, the increment, the error cache and the timings are not touched.
+  // The term lists built at the first call stay on the handle (not counted in device_bytes).
+  template <class T>
+  int cov_upload(T** p, const std::vector<T>& v) {
+    void* q = nullptr;
+    CU(cudaMalloc(&q, std::max<size_t>(v.size(), 1) * sizeof(T)));
+    allocs.push_back(q);
+    if (!v.empty()) CU(cudaMemcpy(q, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice));
+    *p = (T*)q;
+    return RBA_OK;
+  }
+  // Per landmark its first slot and track length; per co-visible camera pair (ca >= cb) the terms (slot_a, slot_b) of every
+  // landmark that sees both, landmarks in problem order and within a landmark in observation order: the fixed summation
+  // order of k_cov_assemble.
+  int cov_build_lists() {
+    if (cov_ready) return RBA_OK;
+    const int nl = L.nl_local;
+    std::vector<int> slot0(nl), nn(nl);
+    long long nt = 0;
+    for (int lm = 0; lm < nl; ++lm) {
+      const int sidx = L.sorted_of_lm[lm];
+      const TileInfo& T = L.tiles[L.tile_of_sorted[sidx]];
+      slot0[lm] = T.slot_base + (sidx - T.lm_base) * T.n;
+      nn[lm] = T.n;
+      nt += (long long)T.n * (T.n + 1) / 2;
+    }
+    if (nt > std::numeric_limits<int>::max()) { g_err = "rba_compute_covariance: more than 2^31 camera-pair terms"; return RBA_ERR_UNSUPPORTED; }
+    struct Term { long long key; int sa, sb; };
+    std::vector<Term> terms;
+    terms.reserve((size_t)nt);
+    for (int lm = 0; lm < nl; ++lm)
+      for (int a = 0; a < nn[lm]; ++a)
+        for (int b = 0; b <= a; ++b) {  // cameras ascend with the slot: camera(a) >= camera(b)
+          const int sa = slot0[lm] + a, sb = slot0[lm] + b;
+          terms.push_back({(long long)L.slot_cam[sa] * nc + L.slot_cam[sb], sa, sb});
+        }
+    std::stable_sort(terms.begin(), terms.end(), [](const Term& x, const Term& y) { return x.key < y.key; });
+    std::vector<int2> blk_cam, tl(terms.size());
+    std::vector<int> blk_ptr;
+    for (size_t t = 0; t < terms.size(); ++t) {
+      if (t == 0 || terms[t].key != terms[t - 1].key) {
+        blk_cam.push_back(make_int2((int)(terms[t].key / nc), (int)(terms[t].key % nc)));
+        blk_ptr.push_back((int)t);
+      }
+      tl[t] = make_int2(terms[t].sa, terms[t].sb);
+    }
+    blk_ptr.push_back((int)terms.size());
+    TRY(cov_upload(&d_cov_blk_cam, blk_cam));
+    TRY(cov_upload(&d_cov_blk_ptr, blk_ptr));
+    TRY(cov_upload(&d_cov_terms, tl));
+    TRY(cov_upload(&d_cov_lm_slot0, slot0));
+    TRY(cov_upload(&d_cov_lm_n, nn));
+    cov_nblk = (int)blk_cam.size();
+    cov_ready = true;
+    return RBA_OK;
+  }
+  template <bool TA, bool TB>
+  void cov_gemm(long long M, long long N, long long K, double alpha, const double* A, long long lda, const double* B, long long ldb,
+                double beta, double* C, long long ldc, int lower, int ktri) {
+    k_cov_dgemm<TA, TB><<<dim3((unsigned)(M / COV_TB), (unsigned)(N / COV_TB)), 256, 0, stream>>>((int)M, (int)N, (int)K, alpha, A, lda, B,
+                                                                                                   ldb, beta, C, ldc, lower, ktri);
+  }
+  // dst (rows x cols, column-major, ld dld) <- src (ld sld), on the stream
+  int cov_copy(double* dst, long long dld, const double* src, long long sld, long long rows, long long cols) {
+    CU(cudaMemcpy2DAsync(dst, dld * sizeof(double), src, sld * sizeof(double), rows * sizeof(double), cols, cudaMemcpyDeviceToDevice, stream));
+    return RBA_OK;
+  }
+  int compute_covariance(double* cam_cov, double* lm_cov) override {
+    if (!cam_cov && !lm_cov) { g_err = "rba_compute_covariance: cam_cov and lm_cov are both NULL"; return RBA_ERR_INVALID_ARGUMENT; }
+    if (opt.nranks > 1) {
+      g_err = "rba_compute_covariance: sharded handles (nranks > 1) are not supported: the reduced camera matrix would need a cross-rank sum";
+      return RBA_ERR_UNSUPPORTED;
+    }
+    TRY(cov_build_lists());
+    constexpr long long TB = COV_TB;
+    const long long n = 9LL * nc, np = (n + TB - 1) / TB * TB, ns = L.nslots;
+    const int nl = L.nl_local, nt = (int)(np / TB);
+    size_t total = 0;
+    auto carve = [&](size_t bytes) { const size_t o = total; total += (bytes + 255) & ~size_t(255); return o; };
+    const size_t o_A = carve((size_t)(np * np) * 8), o_W = carve((size_t)(np * TB) * 8), o_Y = carve((size_t)(np * TB) * 8),
+                 o_T = carve((size_t)(TB * TB) * 8), o_d = carve((size_t)np * 8), o_jp = carve((size_t)ns * 18 * 8),
+                 o_kb = carve((size_t)ns * 27 * 8), o_wl = carve((size_t)nl * 9 * 8), o_rk = carve((size_t)nl * 4), o_fail = carve(4),
+                 o_cam = carve((size_t)nc * 81 * 8), o_lm = carve(lm_cov ? (size_t)nl * 9 * 8 : 0);
+    size_t free_b = 0, total_b = 0;
+    CU(cudaMemGetInfo(&free_b, &total_b));
+    if (total > free_b) {
+      g_err = "rba_compute_covariance needs " + std::to_string(total) + " bytes of device memory (a dense " + std::to_string(n) + " x " +
+              std::to_string(n) + " float64 reduced camera matrix plus scratch); " + std::to_string(free_b) + " bytes are free";
+      return RBA_ERR_UNSUPPORTED;
+    }
+    char* base = nullptr;
+    CU(cudaMalloc(&base, total));
+    struct CovScratch { char* p; ~CovScratch() { cudaFree(p); } } scratch{base};  // cudaFree waits for the kernels
+    double* A = (double*)(base + o_A); double* W = (double*)(base + o_W); double* Y = (double*)(base + o_Y);
+    double* Tt = (double*)(base + o_T); double* d = (double*)(base + o_d); double* jp = (double*)(base + o_jp);
+    double* kb = (double*)(base + o_kb); double* wl = (double*)(base + o_wl); int* rk = (int*)(base + o_rk);
+    int* fail = (int*)(base + o_fail); double* cam_out = (double*)(base + o_cam); double* lm_out = (double*)(base + o_lm);
+    // 1.-2. elimination, assembly, priors, held parameters, equilibration
+    CU(cudaMemsetAsync(A, 0, (size_t)(np * np) * 8, stream));
+    CU(cudaMemsetAsync(fail, 0x7f, 4, stream));
+    const int wgrid = std::max(1, std::min((nl + 3) / 4, sm_count * 16));
+    k_cov_landmark<S><<<wgrid, 128, 0, stream>>>(D, ko, d_cov_lm_slot0, d_cov_lm_n, nl, jp, kb, wl, rk);
+    k_cov_assemble<<<std::max(1, std::min((cov_nblk + 7) / 8, sm_count * 8)), 256, 0, stream>>>(d_cov_blk_cam, d_cov_blk_ptr, d_cov_terms,
+                                                                                                  cov_nblk, jp, kb, A, np);
+    if (has_abs_prior || n_pairs > 0)
+      k_cov_priors<S><<<(nc + 127) / 128, 128, 0, stream>>>(D.cams, nc, has_abs_prior ? d_prior_mean : nullptr, d_prior_L, d_pair_ij,
+                                                            d_pair_mean, d_pair_L, n_pairs > 0 ? d_pair_ptr : nullptr, d_pair_item,
+                                                            d_pair_nbr, A, np);
+    k_cov_diag<<<(unsigned)((np + 255) / 256), 256, 0, stream>>>(A, np, n, np, D.cam_fixed, d);
+    k_cov_equil<<<dim3((unsigned)(np / 32), (unsigned)(np / 8)), dim3(32, 8), 0, stream>>>(A, np, n, np, D.cam_fixed, d);
+    // 3a. potrf, right-looking: factor the diagonal tile, panel <- panel L_kk^-T, trailing lower tiles -= panel panel^T
+    for (int k = 0; k < nt; ++k) {
+      const long long k0 = k * TB, m = np - k0 - TB;
+      k_cov_tile_potrf<<<1, 256, 0, stream>>>(A, np, k0, COV_PIVOT_TAU, fail);
+      if (m == 0) break;
+      k_cov_tile_trtri<<<1, COV_TB, 0, stream>>>(A, np, k0, Tt, TB);
+      double* P = A + (k0 + TB) + k0 * np;
+      TRY(cov_copy(W, m, P, np, m, TB));
+      cov_gemm<false, true>(m, TB, TB, 1.0, W, m, Tt, TB, 0.0, P, np, 0, 0);
+      cov_gemm<false, true>(m, m, TB, -1.0, P, np, P, np, 1.0, P + TB * np, np, 1, 0);
+    }
+    int h_fail = 0;
+    CU(cudaMemcpyAsync(&h_fail, fail, sizeof(int), cudaMemcpyDeviceToHost, stream));
+    CU(cudaStreamSynchronize(stream));
+    CU(cudaGetLastError());
+    if (h_fail < n) {
+      static const char* names[9] = {"tx", "ty", "tz", "rx", "ry", "rz", "f", "k1", "k2"};
+      g_err = "rba_compute_covariance: the reduced camera matrix is singular: Cholesky pivot <= " + std::to_string(COV_PIVOT_TAU) +
+              " of the equilibrated matrix at camera " + std::to_string(h_fail / 9) + ", increment entry " + std::to_string(h_fail % 9) +
+              " (" + names[h_fail % 9] + "). The gauge is not fixed, or a free camera has no observation and no prior: hold parameters "
+              "with rba_set_camera_fixed or add priors with rba_set_camera_prior";
+      return RBA_NUMERICAL_FAILURE;
+    }
+    // 3b. trtri, from the last tile: column panel <- -L22^-1 L21 L11^-1 with the already inverted trailing part
+    for (int j = nt - 1; j >= 0; --j) {
+      const long long j0 = j * TB, m = np - j0 - TB;
+      k_cov_tile_trtri<<<1, COV_TB, 0, stream>>>(A, np, j0, Tt, TB);
+      if (m > 0) {
+        double* P = A + (j0 + TB) + j0 * np;
+        TRY(cov_copy(W, m, P, np, m, TB));
+        cov_gemm<false, false>(m, TB, m, 1.0, P + TB * np, np, W, m, 0.0, Y, m, 0, 1);
+        cov_gemm<false, false>(m, TB, TB, -1.0, Y, m, Tt, TB, 0.0, P, np, 0, 0);
+      }
+      TRY(cov_copy(A + j0 + j0 * np, np, Tt, TB, TB, TB));
+    }
+    // 3c. lauum, by row tiles: row <- L_ii^T row, L_ii <- L_ii^T L_ii, row += (rows below)^T (rows below)
+    for (int i = 0; i < nt; ++i) {
+      const long long r0 = i * TB, kk = np - r0 - TB;
+      if (r0 > 0) {
+        TRY(cov_copy(W, TB, A + r0, np, TB, r0));
+        cov_gemm<true, false>(TB, r0, TB, 1.0, A + r0 + r0 * np, np, W, TB, 0.0, A + r0, np, 0, 0);
+      }
+      k_cov_tile_lauu2<<<1, 256, 0, stream>>>(A, np, r0);
+      if (kk > 0) cov_gemm<true, false>(TB, r0 + TB, kk, 1.0, A + (r0 + TB) + r0 * np, np, A + (r0 + TB), np, 1.0, A + r0, np, 0, 0);
+    }
+    // 4. extraction
+    if (cam_cov) {
+      k_cov_cam_out<<<(81 * nc + 255) / 256, 256, 0, stream>>>(A, np, d, D.cam_fixed, nc, cam_out);
+      CU(cudaMemcpyAsync(cam_cov, cam_out, (size_t)81 * nc * sizeof(double), cudaMemcpyDeviceToHost, stream));
+    }
+    if (lm_cov) {
+      k_cov_lm_marginal<<<wgrid, 128, 0, stream>>>(A, np, d, D.cam_fixed, D.slot_cam, d_cov_lm_slot0, d_cov_lm_n, nl, kb, wl, rk, lm_out);
+      CU(cudaMemcpyAsync(lm_cov, lm_out, (size_t)9 * nl * sizeof(double), cudaMemcpyDeviceToHost, stream));
+    }
+    CU(cudaGetLastError());
+    CU(cudaStreamSynchronize(stream));
+    return RBA_OK;
+  }
+
   // reference-layout view of one landmark block (see header)
   int debug_get_block(int lm, void* out, int rows, int cols, void* jls_out) override {
     if (lm < L.lm_begin || lm >= L.lm_end) { g_err = "landmark not in this shard"; return RBA_ERR_INVALID_ARGUMENT; }
@@ -1722,6 +1901,7 @@ int32_t rba_right_multiply(rba_handle* h, const void* x, void* y) { return h->ri
 int32_t rba_debug_get_block(rba_handle* h, int32_t lm, void* out, int32_t rows, int32_t cols, void* jls) {
   return h->debug_get_block(lm, out, rows, cols, jls);
 }
+int32_t rba_compute_covariance(rba_handle* h, double* cam_cov, double* lm_cov) { return h->compute_covariance(cam_cov, lm_cov); }
 int32_t rba_time_matvec(rba_handle* h, int32_t reps, double* sec) { return h->time_matvec(reps, sec); }
 int32_t rba_timer_start(rba_handle* h) { return h->timer_start(); }
 int32_t rba_timer_stop(rba_handle* h, double* sec) { return h->timer_stop(sec); }

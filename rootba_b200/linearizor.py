@@ -489,6 +489,15 @@ class LinearizorQR:
         check(_lib.lib().rba_debug_get_block(self.h, C.c_int32(lm), _p(out), rows, cols, _p(jls)))
         return out, 9 * n + pad, 9 * n + pad + 3, jls
 
+    def covariance(self, landmarks: bool = True):
+        """marginal covariances at the current state (rba_compute_covariance, DESIGN.md section 16): float64 arrays
+        (cam [nc, 9, 9] in the increment order tx,ty,tz, rx,ry,rz, f,k1,k2;  lm [nl, 3, 3], or None without landmarks).
+        Raises RbaError (code RBA_NUMERICAL_FAILURE) when the reduced camera matrix is singular (gauge not fixed)."""
+        cam = np.empty((self.nc, 9, 9), np.float64)
+        lm = np.empty((self.nl, 3, 3), np.float64) if landmarks else None
+        check(_lib.lib().rba_compute_covariance(self.h, cam.ctypes.data, None if lm is None else lm.ctypes.data))
+        return cam, lm
+
     def timer_start(self):
         check(_lib.lib().rba_timer_start(self.h))
 
