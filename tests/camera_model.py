@@ -26,10 +26,17 @@ EPS = {np.dtype(np.float32): np.float32(1e-5), np.dtype(np.float64): np.float64(
 EPS_SQRT = {np.dtype(np.float32): np.float32(0.0031622776601683794), np.dtype(np.float64): np.float64(1e-5)}
 
 
-def rotation(q):
-    """unit quaternions (x, y, z, w) [..., 4] -> rotation matrices: R = (w^2 - |v|^2) I + 2 v v^T + 2 w [v]x"""
+def rotation(q, device=False):
+    """unit quaternions (x, y, z, w) [..., 4] -> rotation matrices: R = (w^2 - |v|^2) I + 2 v v^T + 2 w [v]x.
+
+    device=True evaluates the form the kernels use (Eigen's Quaternion::toRotationMatrix), R = I + 2 w [v]x + 2 [v]x^2, on
+    the quaternion as stored: the two agree for a unit quaternion, and for a float32 quaternion whose norm is 1 + O(2^-24)
+    only the device form is the matrix the kernels actually apply."""
     q = np.asarray(q, dtype=np.float64)
     v, w = q[..., :3], q[..., 3]
+    if device:
+        K = hat(v)
+        return np.eye(3) + 2 * w[..., None, None] * K + 2 * K @ K
     R = (w * w - (v * v).sum(-1))[..., None, None] * np.eye(3) + 2 * v[..., :, None] * v[..., None, :]
     return R + 2 * w[..., None, None] * hat(v)
 
@@ -57,12 +64,13 @@ def project_pc(pc, intr):
     return (intr[:, 0] * rp)[:, None] * m
 
 
-def linearize(cams, p, obs, dtype=np.float64):
+def linearize(cams, p, obs, dtype=np.float64, device_rot=False):
     """per observation: residual [m, 2], Jp [m, 2, 6], Ji [m, 2, 3], Jl [m, 2, 3], pc [m, 3], valid [m] (z >= sqrt(eps) of
-    `dtype`).  Nothing is filtered: invalid observations get their (finite or not) values too."""
+    `dtype`).  Nothing is filtered: invalid observations get their (finite or not) values too.  device_rot: R as the kernels
+    build it (rotation(device=True))."""
     cams = np.asarray(cams, dtype=np.float64).reshape(-1, 10)
     obs = np.asarray(obs, dtype=np.float64).reshape(-1, 2)
-    R = rotation(cams[:, :4])
+    R = rotation(cams[:, :4], device=device_rot)
     pc = np.einsum("mij,mj->mi", R, np.asarray(p, dtype=np.float64).reshape(-1, 3)) + cams[:, 4:7]
     f, k1, k2 = cams[:, 7], cams[:, 8], cams[:, 9]
     z = pc[:, 2]
@@ -134,12 +142,13 @@ def condition(arrays, dtype=np.float64, threshold=None):
     return k
 
 
-def weighted(arrays, dtype=np.float64, threshold=None, valid_only=False, magnitude=False):
+def weighted(arrays, dtype=np.float64, threshold=None, valid_only=False, magnitude=False, device_rot=False):
     """per observation sqrt(w) Jp (2 x 9: pose then intrinsics), sqrt(w) Jl, sqrt(w) res and the row mask (0 for an
     observation that use_valid_projections_only drops) -- the unscaled rows of the landmark blocks.  magnitude=True appends
-    sqrt(w) (|proj| + |obs|), the scale of the rounding error of a residual computed as proj - obs."""
+    sqrt(w) (|proj| + |obs|), the scale of the rounding error of a residual computed as proj - obs.  device_rot: see
+    linearize."""
     cams, p, obs = observations(arrays)
-    L = linearize(cams, p, obs, dtype=dtype)
+    L = linearize(cams, p, obs, dtype=dtype, device_rot=device_rot)
     _, w = huber((L["res"] ** 2).sum(1), threshold)
     keep = L["valid"] if valid_only else np.ones(len(w), bool)
     sw = np.where(keep, np.sqrt(w), 0.0)[:, None]

@@ -33,17 +33,26 @@ def left_jacobian(phi):
     return np.eye(3) + (1 - np.cos(th)) / th ** 2 * K + (th - np.sin(th)) / th ** 3 * K @ K
 
 
-def residual(cam, mean):
-    """e [9] of one camera [10] against one prior mean [10]"""
+def _cam_rot(cam, device_rot):
+    """R of a camera: of its normalised quaternion, or (device_rot) as the kernels build it from the stored quaternion"""
+    q = np.asarray(cam[:4], np.float64)
+    return cm.rotation(q, device=True) if device_rot else cm.rotation(q / np.linalg.norm(q))
+
+
+def residual(cam, mean, device_rot=False):
+    """e [9] of one camera [10] against one prior mean [10].  device_rot: the centre -R^T t with R as the kernels build it;
+    the logarithm depends on the quaternions' directions only (the kernels' Log of a quaternion product is invariant to
+    their scale), so it is that of the normalised ones either way."""
     cam, mean = np.asarray(cam, np.float64), np.asarray(mean, np.float64)
     R, R0 = cm.rotation(cam[:4] / np.linalg.norm(cam[:4])), cm.rotation(mean[:4] / np.linalg.norm(mean[:4]))
-    return np.concatenate([-R.T @ cam[4:7] - mean[4:7], log_so3(R @ R0.T), cam[7:10] - mean[7:10]])
+    Rc = _cam_rot(cam, device_rot)
+    return np.concatenate([-Rc.T @ cam[4:7] - mean[4:7], log_so3(R @ R0.T), cam[7:10] - mean[7:10]])
 
 
-def jacobian(cam, mean):
+def jacobian(cam, mean, device_rot=False):
     """de/d(increment) [9, 9] at the camera"""
     cam = np.asarray(cam, np.float64)
-    R = cm.rotation(cam[:4] / np.linalg.norm(cam[:4]))
+    R = _cam_rot(cam, device_rot)
     phi = residual(cam, mean)[3:6]
     J = np.zeros((9, 9))
     J[0:3, 0:3] = -R.T
@@ -64,14 +73,14 @@ def apply_inc(cam, d):
     return out
 
 
-def rows(cams, mean, sqrt_info):
+def rows(cams, mean, sqrt_info, device_rot=False):
     """the prior rows of the whole problem, unscaled: A [nc, 9, 9] = L de/d(inc) and r [nc, 9] = L e"""
     nc = len(cams)
     A, r = np.zeros((nc, 9, 9)), np.zeros((nc, 9))
     for c in range(nc):
         L = np.asarray(sqrt_info[c], np.float64)
-        A[c] = L @ jacobian(cams[c], mean[c])
-        r[c] = L @ residual(cams[c], mean[c])
+        A[c] = L @ jacobian(cams[c], mean[c], device_rot)
+        r[c] = L @ residual(cams[c], mean[c], device_rot)
     return A, r
 
 
@@ -118,3 +127,71 @@ def dense_system_with_prior(prob, mean, sqrt_info):
     for c in range(nc):
         Jp_p[9 * c:9 * c + 9, 9 * c:9 * c + 9] = A[c]
     return np.vstack([Jp, Jp_p]), np.vstack([Jl, np.zeros((9 * nc, Jl.shape[1]))]), np.concatenate([r, rp.ravel()])
+
+
+# ------------------------------------------------------------------------------------------------
+# The kernels' SO(3) formulas (so3_log_rel, so3_jl_inv of rootba_b200/csrc/kernels.cuh), restated so that the CPU tests can
+# show that the device checks would reject a subtly wrong variant of them.  `fault` plants one such variant:
+#   "jl_identity"  J_l^-1 replaced by I;  "no_flip"  the product not flipped to w >= 0;  "series_everywhere"  the series of
+#   J_l^-1 used at every angle (its range is theta^2 < 1e-4).
+# ------------------------------------------------------------------------------------------------
+def log_quat_device(a, m, eps_sqrt=1e-5, fault=None):
+    """phi = Log(a (x) conj(m)) of two quaternions (x, y, z, w) as the kernels evaluate it: theta / n = 2 atan2(n, w) / n,
+    its series 2 / w (1 - n^2 / (3 w^2)) where n < eps_sqrt w, the product first flipped to w >= 0"""
+    a, m = np.asarray(a, np.float64), np.asarray(m, np.float64)
+    b = np.array([-m[0], -m[1], -m[2], m[3]])
+    w = a[3] * b[3] - a[0] * b[0] - a[1] * b[1] - a[2] * b[2]
+    v = np.array([a[3] * b[0] + a[0] * b[3] + a[1] * b[2] - a[2] * b[1],
+                  a[3] * b[1] + a[1] * b[3] + a[2] * b[0] - a[0] * b[2],
+                  a[3] * b[2] + a[2] * b[3] + a[0] * b[1] - a[1] * b[0]])
+    if w < 0 and fault != "no_flip":
+        w, v = -w, -v
+    n2 = float(v @ v)
+    n = np.sqrt(n2)
+    fac = 2 / w * (1 - n2 / (3 * w * w)) if n < eps_sqrt * w else 2 * np.arctan2(n, w) / n
+    return fac * v
+
+
+def jl_inv_device(phi, fault=None):
+    """J_l^-1(phi) = I - 1/2 [phi]x + a [phi]x^2, a = 1/th^2 - cot(th/2) / (2 th) (series 1/12 + th^2/720 + th^4/30240
+    below th^2 = 1e-4)"""
+    phi = np.asarray(phi, np.float64)
+    if fault == "jl_identity":
+        return np.eye(3)
+    th2 = float(phi @ phi)
+    if th2 < 1e-4 or fault == "series_everywhere":
+        a = 1 / 12 + th2 * (1 / 720 + th2 / 30240)
+    else:
+        th = np.sqrt(th2)
+        a = 1 / th2 - np.cos(th / 2) / (2 * th * np.sin(th / 2))
+    K = cm.hat(phi)
+    return np.eye(3) - 0.5 * K + a * K @ K
+
+
+def rows_device(cams, mean, sqrt_info, fault=None):
+    """rows() with the rotation rows by the kernels' formulas (and a planted fault): A [nc, 9, 9]"""
+    nc = len(cams)
+    A = np.zeros((nc, 9, 9))
+    for c in range(nc):
+        cam = np.asarray(cams[c], np.float64)
+        J = np.zeros((9, 9))
+        J[0:3, 0:3] = -cm.rotation(cam[:4], device=True).T
+        J[3:6, 3:6] = jl_inv_device(log_quat_device(cam[:4], mean[c][:4], fault=fault), fault=fault)
+        J[6:9, 6:9] = np.eye(3)
+        A[c] = np.asarray(sqrt_info[c], np.float64) @ J
+    return A
+
+
+# residual angles of the large-rotation tests: 0 exactly, both branches of the log's series and of the J_l^-1 series (its
+# switch is at theta = 0.01), and angles up to pi
+ROTATION_ANGLES = [0.0, 1e-9, 5e-4, 0.009, 0.011, 0.5, 2.0, 3.0, np.pi - 1e-3]
+
+
+def mean_at_angle(cam, theta, seed, negate=False):
+    """a quaternion R0 with Log(R R0^T) of angle theta about a random axis (R of the camera), or its negative"""
+    rng = np.random.default_rng(seed)
+    axis = rng.standard_normal(3)
+    axis /= np.linalg.norm(axis)
+    R = Rotation.from_quat(np.asarray(cam[:4], np.float64))
+    q0 = (Rotation.from_rotvec(-theta * axis) * R).as_quat()
+    return -q0 if negate else q0

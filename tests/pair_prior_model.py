@@ -18,23 +18,25 @@ import camera_model as cm
 import camera_prior_model as pm
 
 
-def _rot(cam):
+def _rot(cam, device_rot=False):
+    """R of a camera: of its normalised quaternion, or (device_rot) as the kernels build it from the stored quaternion"""
     cam = np.asarray(cam, np.float64)
-    return cm.rotation(cam[:4] / np.linalg.norm(cam[:4]))
+    return cm.rotation(cam[:4], device=True) if device_rot else cm.rotation(cam[:4] / np.linalg.norm(cam[:4]))
 
 
-def residual(ci, cj, mean):
-    """e [6] of one pair: cameras ci, cj [10], mean [7] (qx,qy,qz,qw of R0, t0)"""
+def residual(ci, cj, mean, device_rot=False):
+    """e [6] of one pair: cameras ci, cj [10], mean [7] (qx,qy,qz,qw of R0, t0).  device_rot: M = R_i R_j^T of the kernels'
+    rotation matrices in e_t; the logarithm is that of the normalised quaternions either way (camera_prior_model.residual)."""
     ci, cj, mean = (np.asarray(a, np.float64) for a in (ci, cj, mean))
     Ri, Rj, R0 = _rot(ci), _rot(cj), cm.rotation(mean[:4] / np.linalg.norm(mean[:4]))
-    M = Ri @ Rj.T
-    return np.concatenate([ci[4:7] - M @ cj[4:7] - mean[4:7], pm.log_so3(M @ R0.T)])
+    Md = _rot(ci, device_rot) @ _rot(cj, device_rot).T
+    return np.concatenate([ci[4:7] - Md @ cj[4:7] - mean[4:7], pm.log_so3(Ri @ Rj.T @ R0.T)])
 
 
-def jacobians(ci, cj, mean):
+def jacobians(ci, cj, mean, device_rot=False):
     """de/d(inc_i), de/d(inc_j) [6, 9] each at the cameras"""
     ci, cj = np.asarray(ci, np.float64), np.asarray(cj, np.float64)
-    M = _rot(ci) @ _rot(cj).T
+    M = _rot(ci, device_rot) @ _rot(cj, device_rot).T
     t_rel = ci[4:7] - M @ cj[4:7]
     Jinv = np.linalg.inv(pm.left_jacobian(residual(ci, cj, mean)[3:6]))
     Ji, Jj = np.zeros((6, 9)), np.zeros((6, 9))
@@ -69,16 +71,16 @@ def sqrt_info_kind(kind, rng, scale=1.0):
     return L
 
 
-def rows(cams, pairs, mean, sqrt_info):
+def rows(cams, pairs, mean, sqrt_info, device_rot=False):
     """the pair rows of the whole problem, unscaled: Jp [6 m, 9 nc] = L de/d(inc) and r [6 m] = L e"""
     nc, m = len(cams), len(pairs)
     J, r = np.zeros((6 * m, 9 * nc)), np.zeros(6 * m)
     for p, (i, j) in enumerate(pairs):
         L = np.asarray(sqrt_info[p], np.float64)
-        Ji, Jj = jacobians(cams[i], cams[j], mean[p])
+        Ji, Jj = jacobians(cams[i], cams[j], mean[p], device_rot)
         J[6 * p:6 * p + 6, 9 * i:9 * i + 9] += L @ Ji
         J[6 * p:6 * p + 6, 9 * j:9 * j + 9] += L @ Jj
-        r[6 * p:6 * p + 6] = L @ residual(cams[i], cams[j], mean[p])
+        r[6 * p:6 * p + 6] = L @ residual(cams[i], cams[j], mean[p], device_rot)
     return J, r
 
 

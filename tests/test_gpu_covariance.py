@@ -5,8 +5,10 @@ kernels at 500 cameras and below one tile, singular systems, and the absence of 
 
 Bars are c * kappa * u with u the float64 unit roundoff and kappa the condition number of the Jacobi-equilibrated matrix
 the test inverts; c = 8 * (number of unknowns) covers the rounding of the Cholesky-based inverse on both sides.  A float32
-handle is compared with the reference at its float32 state and prior arrays; the model normalises the quaternions the device
-uses as stored, which perturbs the rotation matrices by | |q|^2 - 1 |, amplified by at most kappa: that term is added."""
+handle is compared with the reference at its float32 state and prior arrays, the rotation matrices built from the stored
+quaternions as the kernels build them (camera_model.rotation(device=True)): the device widens those values to float64 and
+computes in float64, so the float32 bars are the float64 ones.  Larger shapes, long tracks, the benchmark size and large
+prior rotations are in test_gpu_covariance_shapes.py."""
 
 
 import numpy as np
@@ -25,38 +27,14 @@ pytestmark = pytest.mark.gpu
 U = 2.0 ** -53
 
 
-def _centre_priors(prob, seed=3):
-    rng = np.random.default_rng(seed)
-    mean = pm.mean_at(np.asarray(prob.cams, np.float64))
-    mean[:, 4:7] += rng.normal(0, 0.05, (len(mean), 3))
-    L = np.stack([pm.sqrt_info_kind("centre", rng) for _ in range(len(mean))])
-    return mean, L
+_centre_priors = cvm.centre_priors
 
 
-def _as_f32(prob, absp=None, pair=None):
-    """the problem and prior arrays as a float32 handle holds them, upcast (quaternions normalised, then rounded)"""
-    from rootba_b200.synthetic import BalArrays
-    r = lambda a: np.asarray(a, np.float32).astype(np.float64)
-    p32 = BalArrays(r(prob.cams), r(prob.lms), prob.lm_off, prob.obs_cam, r(prob.obs_xy))
-    qs = [np.asarray(prob.cams)[:, :4].astype(np.float32).astype(np.float64)]
-    if absp is not None:
-        m = np.array(absp[0], np.float64)
-        m[:, :4] /= np.linalg.norm(m[:, :4], axis=1, keepdims=True)
-        absp = (r(m), r(absp[1]))
-        qs.append(absp[0][:, :4])
-    if pair is not None:
-        m = np.array(pair[1], np.float64)
-        m[:, :4] /= np.linalg.norm(m[:, :4], axis=1, keepdims=True)
-        pair = (pair[0], r(m), r(pair[2]))
-        qs.append(pair[1][:, :4])
-    qdev = max(float(np.abs((q * q).sum(1) - 1).max()) for q in qs)
-    return p32, absp, pair, qdev
-
-
-def _dense(prob, absp=None, pair=None, threshold=None, valid_only=False):
-    """[Jp | Jl] of the total objective: weighted reprojection rows (camera_model), absolute and pair prior rows"""
+def _dense(prob, absp=None, pair=None, threshold=None, valid_only=False, dtype=np.float64):
+    """[Jp | Jl] of the total objective: weighted reprojection rows (camera_model), absolute and pair prior rows, rotations
+    as the kernels build them; `dtype` is the handle's (its validity threshold)"""
     nobs, nc, nl = len(prob.obs_cam), len(prob.cams), len(prob.lm_off) - 1
-    jp, jl, _, _ = cm.weighted(prob, threshold=threshold, valid_only=valid_only)
+    jp, jl, _, _ = cm.weighted(prob, dtype=dtype, threshold=threshold, valid_only=valid_only, device_rot=True)
     Jp, Jl = np.zeros((2 * nobs, 9 * nc)), np.zeros((2 * nobs, 3 * nl))
     lm_of_obs = np.repeat(np.arange(nl), np.diff(prob.lm_off))
     for k in range(nobs):
@@ -65,13 +43,13 @@ def _dense(prob, absp=None, pair=None, threshold=None, valid_only=False):
         Jl[2 * k:2 * k + 2, 3 * l:3 * l + 3] = jl[k]
     rows = [Jp]
     if absp is not None:
-        A, _ = pm.rows(np.asarray(prob.cams, np.float64), *absp)
+        A, _ = pm.rows(np.asarray(prob.cams, np.float64), *absp, device_rot=True)
         Ja = np.zeros((9 * nc, 9 * nc))
         for c in range(nc):
             Ja[9 * c:9 * c + 9, 9 * c:9 * c + 9] = A[c]
         rows.append(Ja)
     if pair is not None:
-        Jq, _ = qm.rows(np.asarray(prob.cams, np.float64), *pair)
+        Jq, _ = qm.rows(np.asarray(prob.cams, np.float64), *pair, device_rot=True)
         rows.append(Jq)
     Jp = np.vstack(rows)
     return Jp, np.vstack([Jl, np.zeros((Jp.shape[0] - Jl.shape[0], Jl.shape[1]))])
@@ -91,13 +69,11 @@ def _handle(prob, dtype, cfg=None, absp=None, pair=None, mask=None, **so_kw):
 
 def _check(cam, lm, prob, dtype, absp=None, pair=None, mask=None, threshold=None, valid_only=False):
     nc, nl = len(prob.cams), len(prob.lm_off) - 1
-    qdev = 0.0
-    if dtype == np.float32:
-        prob, absp, pair, qdev = _as_f32(prob, absp, pair)
-    Jp, Jl = _dense(prob, absp, pair, threshold, valid_only)
+    prob, absp, pair = cvm.as_stored(prob, dtype, absp, pair)
+    Jp, Jl = _dense(prob, absp, pair, threshold, valid_only, dtype)
     fixed = cvm.fixed_mask(mask, nc)
     cam_ref, lm_ref, kappa = cvm.dense_inverse(Jp, Jl, nc, nl, fixed)
-    bar = 8 * (int((~fixed).sum()) + 3 * nl) * kappa * U + 4 * kappa * qdev
+    bar = 8 * (int((~fixed).sum()) + 3 * nl) * kappa * U
     assert np.abs(cam - cam_ref).max() <= bar * np.abs(cam_ref).max(), (np.abs(cam - cam_ref).max() / np.abs(cam_ref).max(), bar)
     if lm is not None:
         assert np.abs(lm - lm_ref).max() <= bar * np.abs(lm_ref).max(), (np.abs(lm - lm_ref).max() / np.abs(lm_ref).max(), bar)
@@ -164,16 +140,24 @@ def test_gauge_fixed_by_two_held_poses():
 
 
 def test_huber_with_active_weights():
+    _huber_with_active_weights(np.float64)
+
+
+def test_huber_with_active_weights_float32():
+    _huber_with_active_weights(np.float32)
+
+
+def _huber_with_active_weights(dtype):
     prob, absp = _case(7, 90, 21)
     L = cm.linearize(*cm.observations(prob))
     rn = np.sqrt((L["res"] ** 2).sum(1))
     th = float(np.median(rn))
     assert (rn > th).sum() > 10
     from rootba_b200.linearizor import ResidualOptions
-    lin = _handle(prob, np.float64, absp=absp, residual=ResidualOptions("HUBER", th))
+    lin = _handle(prob, dtype, absp=absp, residual=ResidualOptions("HUBER", th))
     cam, lm = lin.covariance()
     lin.close()
-    _check(cam, lm, prob, np.float64, absp=absp, threshold=th)
+    _check(cam, lm, prob, dtype, absp=absp, threshold=th)
 
 
 def _turned():
@@ -185,21 +169,53 @@ def _turned():
     return turn_cameras_around(a, [0])
 
 
+def _with_shallow_observation(prob, depth=1e-3):
+    """prob + one landmark seen by camera 1 at `depth` in front of it (between float64's validity threshold sqrt(1e-10)
+    and float32's sqrt(1e-5)) and by every other camera 2..9 that has it at least 1 in front"""
+    from rootba_b200.synthetic import BalArrays
+    cams = np.asarray(prob.cams, np.float64)
+    R1 = cm.rotation(cams[1, :4])
+    p = R1.T @ (np.array([0.1, -0.1, 1.0]) * depth - cams[1, 4:7])
+    z = np.einsum("mij,j->mi", cm.rotation(cams[:, :4]), p)[:, 2] + cams[:, 6]
+    obs_cam = np.array([1] + [c for c in range(2, len(cams)) if z[c] >= 1.0], np.int32)
+    assert len(obs_cam) >= 3
+    proj = cm.linearize(cams[obs_cam], np.broadcast_to(p, (len(obs_cam), 3)), np.zeros((len(obs_cam), 2)))["res"]
+    xy = proj + np.random.default_rng(8).normal(0, 0.5, proj.shape)
+    return BalArrays(cams, np.vstack([prob.lms, p]), np.append(prob.lm_off, prob.lm_off[-1] + len(obs_cam)),
+                     np.concatenate([prob.obs_cam, obs_cam]), np.vstack([prob.obs_xy, xy]))
+
+
 def test_invalid_observations_dropped_and_rank2_landmark():
+    _invalid_observations_dropped_and_rank2_landmark(np.float64)
+
+
+def test_invalid_observations_dropped_and_rank2_landmark_float32():
+    _invalid_observations_dropped_and_rank2_landmark(np.float32)
+
+
+def _invalid_observations_dropped_and_rank2_landmark(dtype):
     """use_valid_projections_only (optimized_cost ERROR_VALID): camera 0's rows are zero, so it is held by its prior alone;
-    landmark 0 keeps one valid observation: NaN block, cameras against the pinv elimination"""
+    landmark 0 keeps one valid observation: NaN block, cameras against the pinv elimination.  The float32 handle also holds
+    an observation at depth 1e-3, which float32's validity threshold (the one the handle's own scalar uses) drops and
+    float64's would keep."""
     prob = _turned()
+    if dtype == np.float32:
+        prob = _with_shallow_observation(prob)
     absp = _centre_priors(prob, 4)
     absp[1][0] = pm.sqrt_info_kind("dense", np.random.default_rng(1))  # camera 0 has no valid observation
     nc, nl = len(prob.cams), len(prob.lm_off) - 1
-    lin = _handle(prob, np.float64, absp=absp, optimized_cost="ERROR_VALID")
+    lin = _handle(prob, dtype, absp=absp, optimized_cost="ERROR_VALID")
     cam, lm = lin.covariance()
     lin.close()
     assert np.isnan(lm[0]).all() and np.isfinite(lm[1:]).all()
-    jp, jl, _, keep = cm.weighted(prob, valid_only=True)
+    sprob, sabsp, _ = cvm.as_stored(prob, dtype, absp)
+    jp, jl, _, keep = cm.weighted(sprob, dtype=dtype, valid_only=True, device_rot=True)
     assert keep.sum() < len(keep) and keep[prob.lm_off[0]:prob.lm_off[1]].sum() == 1
+    if dtype == np.float32:
+        _, _, _, keep64 = cm.weighted(sprob, dtype=np.float64, valid_only=True, device_rot=True)
+        assert not keep[prob.lm_off[-2]] and keep64[prob.lm_off[-2]] and (keep64 != keep).sum() == 1
     S = cvm.schur_reduced(jp, jl, np.asarray(prob.obs_cam), np.asarray(prob.lm_off), nc)
-    A, _ = pm.rows(np.asarray(prob.cams, np.float64), *absp)
+    A, _ = pm.rows(np.asarray(sprob.cams, np.float64), *sabsp, device_rot=True)
     for c in range(nc):
         S[9 * c:9 * c + 9, 9 * c:9 * c + 9] += A[c].T @ A[c]
     d = 1 / np.sqrt(np.diag(S))
@@ -218,7 +234,8 @@ def test_invalid_observations_dropped_and_rank2_landmark():
 @pytest.mark.parametrize("nc, nl", [(500, 5000), (2, 40), (7, 90)], ids=["nc500", "nc2", "nc7"])
 def test_dense_kernels_against_schur_reduced(nc, nl):
     """N = 4500 (not a multiple of the 64 tile), N = 18 and N = 63 (below one tile).  One camera cannot hold a landmark (a
-    landmark needs two observations by distinct cameras), so two is the smallest problem."""
+    landmark needs two observations by distinct cameras), so two is the smallest problem.  Every camera and landmark block
+    is also compared componentwise with the vectorised reference (covariance_model.check)."""
     from rootba_b200.synthetic import synth_bal
     prob = synth_bal(nc, nl, 4.1 if nc > 2 else 2.0, seed=11)
     absp = _centre_priors(prob, 12)
@@ -240,6 +257,7 @@ def test_dense_kernels_against_schur_reduced(nc, nl):
     ref_cam = np.stack([ref[9 * c:9 * c + 9, 9 * c:9 * c + 9] for c in range(nc)])
     assert np.abs(cam - ref_cam).max() <= 8 * 9 * nc * kappa * U * np.abs(ref_cam).max()
     assert np.isfinite(lm2).all()
+    cvm.check(cam2, lm2, cvm.reference(prob, absp=absp), what=f"nc {nc}")
 
 
 @pytest.mark.parametrize("size", [(7, 90, 21), (120, 500, 5)], ids=["nc7", "nc120"])
