@@ -3,7 +3,7 @@
 
     python examples/solve_bal.py problem-49-7776-pre.txt [--float] [--max-num-iterations 20] [--operator-form DENSE|IMPLICIT]
         [--fix-intrinsics] [--fix-cameras I,J,...] [--camera-prior FILE.npz] [--camera-pair-prior FILE.npz]
-        [--covariance OUT.npz]
+        [--landmark-prior FILE.npz] [--covariance OUT.npz]
 
 Mirrors what `bal_qr --input ...` of the reference does (src/app/bal_qr.cpp): load + normalise (bal_problem.cpp:773-852),
 optimize_lm_ours with the QR linearizor (solver/bal_bundle_adjustment.cpp:249-544), log (bal/ba_log.hpp)."""
@@ -38,6 +38,9 @@ def main():
                     help="relative pose priors between pairs of cameras: arrays `pairs` [m, 2] (i, j), `mean` [m, 7] (qx,qy,qz,qw, t "
                          "of T_i T_j^-1) and `sqrt_info` [m, 6, 6] in the coordinates of the loaded (normalised) problem "
                          "(DESIGN.md section 15)")
+    ap.add_argument("--landmark-prior", default=None, metavar="FILE.npz",
+                    help="Gaussian priors on landmark positions (e.g. ground control points): arrays `idx` [m], `mean` [m, 3] and "
+                         "`sqrt_info` [m, 3, 3] in the coordinates of the loaded (normalised) problem (DESIGN.md section 17)")
     ap.add_argument("--covariance", default=None, metavar="OUT.npz",
                     help="after the solve, write the marginal covariances `cam` [nc, 9, 9] (tx,ty,tz, rx,ry,rz, f,k1,k2) and `lm` "
                          "[nl, 3, 3] at the final state (DESIGN.md section 16); the gauge must be fixed by priors or held "
@@ -76,6 +79,14 @@ def main():
                 problem.camera_pair_prior = (f["pairs"], f["mean"], f["sqrt_info"])
             except ValueError as e:
                 ap.error(f"--camera-pair-prior: {e}")
+    if args.landmark_prior:
+        with np.load(args.landmark_prior) as f:
+            if "idx" not in f or "mean" not in f or "sqrt_info" not in f:
+                ap.error(f"--landmark-prior: {args.landmark_prior} must hold the arrays `idx`, `mean` and `sqrt_info`")
+            try:
+                problem.landmark_prior = (f["idx"], f["mean"], f["sqrt_info"])
+            except ValueError as e:
+                ap.error(f"--landmark-prior: {e}")
     options = rb.SolverOptions(max_num_iterations=args.max_num_iterations, preconditioner_type=args.preconditioner_type,
                                operator_form=args.operator_form, use_double=not args.float)
     summary = rb.bundle_adjust_manual(problem, options, verbose=True)

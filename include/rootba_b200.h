@@ -283,6 +283,25 @@ int32_t rba_set_camera_prior(rba_handle* h, const void* mean, const void* sqrt_i
 int32_t rba_set_camera_pair_prior(rba_handle* h, int32_t num_pairs, const int32_t* pairs, const void* mean,
                                   const void* sqrt_info);
 
+/* ---- Gaussian priors on landmark positions (DESIGN.md section 17) ------------------------- */
+
+/* Not in the reference.  A soft prior on the world position of selected landmarks (surveyed ground control points, depth
+ * or LiDAR points, points of an earlier map).  Prior p is on landmark lm_idx[p] (problem order):
+ *   lm_idx [num] int32;  mean [3*num] Scalar, the prior position x0 (world frame);  sqrt_info [9*num] Scalar, row-major
+ *   3x3 L.  num == 0 (pointers ignored): no landmark priors, the default.  Residual e = x - x0, cost 1/2 |L e|^2, not
+ *   robustified.  L need not have full rank (a height-only prior is one non-zero row); an all-zero L is dropped.  Every
+ *   rank of a sharded problem passes the same full list and keeps the priors of its own landmark shard.
+ * The priors are part of the linearisation: the landmark Jacobi scaling is that of the whole Jacobian, and the solve, the
+ * back-substitution, l_diff of rba_apply, rba_compute_error and rba_compute_covariance include them (a prior can give a
+ * landmark with fewer than 2 valid observations a full-rank block, and priors on three non-collinear landmarks can fix the
+ * gauge).  They combine with the camera priors, the pair priors and rba_set_camera_fixed.  After a call rba_solve returns
+ * RBA_ERR_STATE until the next rba_linearize; the device-resident increment and the cached error are discarded.
+ * The 3 damping rows of a landmark with a prior (rba_debug_get_block's last 3 rows) are those of [C | 0 | c], the QR of the
+ * prior rows and the damping rows, after the 6 damping rotations, instead of those of [sqrt(lambda) I | 0 | 0].
+ * num < 0, a NULL array when num > 0, an index outside [0, Nl), a repeated index or a non-finite entry ->
+ * RBA_ERR_INVALID_ARGUMENT, and the previous landmark priors stay in force. */
+int32_t rba_set_landmark_prior(rba_handle* h, int32_t num, const int32_t* lm_idx, const void* mean, const void* sqrt_info);
+
 /* ---- Marginal covariances (DESIGN.md section 16) ------------------------------------------ */
 
 /* Not in the reference.  DESIGN.md section 16.  The covariance of the Gauss-Newton step of the total objective (reprojection

@@ -130,6 +130,7 @@ def lib():
         _lib.rba_last_error.restype = C.c_char_p
         _lib.rba_stream.restype = C.c_void_p
         _lib.rba_compute_covariance.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+        _lib.rba_set_landmark_prior.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
     return _lib
 
 

@@ -67,10 +67,13 @@ __device__ __forceinline__ void cov_sym3_eig(double (&A)[9], double (&V)[9]) {
 // Warp per landmark (problem order).  Re-linearises every observation in double with the weights and validity rule of
 // rba_linearize (unscaled), then writes per slot jpw [18] = sqrt(w) Jp and kb [27] = K (3x9 row-major, rows of dropped
 // eigenvalues zero), and per landmark wl [9] = V Lambda^-1/2 (row-major; columns of dropped eigenvalues zero) and its rank.
-template <class S>
+// LMP (landmark priors, DESIGN.md section 17): Hll += L^T L (unscaled, in double) for a landmark with prior slot
+// lmp_of_lm[lm] >= 0, so a landmark with fewer than 2 valid observations can be full rank.
+template <class S, bool LMP = false>
 __global__ void __launch_bounds__(128) k_cov_landmark(DevPtrs<S> D, KOpts o, const int* __restrict__ lm_slot0,
                                                       const int* __restrict__ lm_n, int nl, double* __restrict__ jpw,
-                                                      double* __restrict__ kb, double* __restrict__ wl, int* __restrict__ rank) {
+                                                      double* __restrict__ kb, double* __restrict__ wl, int* __restrict__ rank,
+                                                      const int* __restrict__ lmp_of_lm = nullptr) {
   const int lane = threadIdx.x & 31;
   const int warps = gridDim.x * (blockDim.x >> 5);
   for (int lm = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); lm < nl; lm += warps) {
@@ -112,6 +115,17 @@ __global__ void __launch_bounds__(128) k_cov_landmark(DevPtrs<S> D, KOpts o, con
     }
 #pragma unroll
     for (int k = 0; k < 6; ++k) h[k] = warp_sum(h[k]);  // butterfly: the same sum in every lane
+    if constexpr (LMP) {
+      const int lp = lmp_of_lm[lm];
+      if (lp >= 0) {
+        const S* Lp = D.lmp_L + 9 * (size_t)lp;
+#pragma unroll
+        for (int r = 0; r < 3; ++r) {
+          const double a0 = (double)Lp[3 * r], a1 = (double)Lp[3 * r + 1], a2 = (double)Lp[3 * r + 2];
+          h[0] += a0 * a0; h[1] += a0 * a1; h[2] += a0 * a2; h[3] += a1 * a1; h[4] += a1 * a2; h[5] += a2 * a2;
+        }
+      }
+    }
     double A[9] = {h[0], h[1], h[2], h[1], h[3], h[4], h[2], h[4], h[5]}, V[9];
     cov_sym3_eig(A, V);
     const double lmax = fmax(A[0], fmax(A[4], A[8]));

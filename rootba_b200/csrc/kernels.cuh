@@ -97,6 +97,12 @@ struct DevPtrs {
   const int* pair_nbr;       // [edges] j
   const S* pair_O;           // [edges][36] O_ij = A_i^T A_j (pose 6x6, row-major), scaled
   S* pair_ov;                // [9 nc] sum_j O_ij v_j of the vector the next PCG / power-series vector step consumes
+  // landmark priors (rba_set_landmark_prior, DESIGN.md section 17); lmp_slot == nullptr = none in this shard.  Only the
+  // kernels' LMP instances read them.
+  const int* lmp_slot;       // [nsorted] prior slot of each sorted landmark, -1 = no prior (and padding)
+  const S* lmp_mean;         // [m][3] x0
+  const S* lmp_L;            // [m][9] row-major square-root information L (unscaled)
+  S* lmp_Lg;                 // [m][12] L diag(jls) (9, row-major) and g = L (x - x0) (3) of the last linearisation
 };
 
 // increment entries (tx,ty,tz, rx,ry,rz, f,k1,k2) held by a camera's RBA_FIX_* bits, as a 9-bit mask
@@ -665,7 +671,9 @@ __device__ __forceinline__ void rot_apply(const Rot<S>& g, S& x, S& y) {
 //   block-diagonal Jp through their compact-WY form, one output element = 3 FMAs, written straight into
 //   the coalesced panel layout.
 // ------------------------------------------------------------------------------------------------
-template <class S, bool GIVENS>
+//   LMP (landmark priors, DESIGN.md section 17): the prior's squared column norms |L col c|^2 join the landmark's column
+//   norms behind jls (the scaling of the whole Jacobian), and lane 0 of the group writes L diag(jls) and g = L (x - x0).
+template <class S, bool GIVENS, bool LMP = false>
 __global__ void __launch_bounds__(128) k_linearize_qr(DevPtrs<S> D, KOpts o, Scratch<S> sc, int* bad_flag, TileOrder to) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   using V2 = typename ST<S>::V2;
@@ -744,9 +752,19 @@ __global__ void __launch_bounds__(128) k_linearize_qr(DevPtrs<S> D, KOpts o, Scr
       for (int c = 0; c < 3; ++c) cs[c] += e[c] * e[c] + e[3 + c] * e[3 + c];
     }
     S jls[3];
+    S lpn[3] = {0, 0, 0};
+    if constexpr (LMP) {
+      const int lp = active ? D.lmp_slot[sidx] : -1;
+      if (lp >= 0) {
+        const S* Lp = D.lmp_L + 9 * (size_t)lp;
+#pragma unroll
+        for (int c = 0; c < 3; ++c) lpn[c] = Lp[c] * Lp[c] + Lp[3 + c] * Lp[3 + c] + Lp[6 + c] * Lp[6 + c];
+      }
+    }
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
       cs[c] = group_sum(cs[c], G);
+      if constexpr (LMP) cs[c] += lpn[c];
       jls[c] = S(1) / (eps + sqrt(cs[c]));
     }
     for (int i = j; i < n; i += G) {
@@ -866,6 +884,22 @@ __global__ void __launch_bounds__(128) k_linearize_qr(DevPtrs<S> D, KOpts o, Scr
       lk[3] = A_AT(1, 1); lk[4] = A_AT(1, 2); lk[5] = A_AT(2, 2);
       lk[6] = A_AT(0, 3); lk[7] = A_AT(1, 3); lk[8] = A_AT(2, 3);
       lk[18] = jls[0]; lk[19] = jls[1]; lk[20] = jls[2];
+      if constexpr (LMP) {
+        const int lp = D.lmp_slot[sidx];  // (slot and position re-read here: keeping them live from stage a spills)
+        if (lp >= 0) {
+          const S* Lp = D.lmp_L + 9 * (size_t)lp;
+          const S* m = D.lmp_mean + 3 * (size_t)lp;
+          const S* x = D.lms + 3 * (size_t)D.sorted_lm[sidx];
+          const S e0 = x[0] - m[0], e1 = x[1] - m[1], e2 = x[2] - m[2];
+          S* out = D.lmp_Lg + 12 * (size_t)lp;
+#pragma unroll
+          for (int r = 0; r < 3; ++r) {
+#pragma unroll
+            for (int c = 0; c < 3; ++c) out[3 * r + c] = Lp[3 * r + c] * jls[c];
+            out[9 + r] = Lp[3 * r] * e0 + Lp[3 * r + 1] * e1 + Lp[3 * r + 2] * e2;
+          }
+        }
+      }
     }
     // Q^T r (rows 0..2 = Q1^T r, rows 3..2n-1 = Q2^T r: the residual column of the marginalised block, ipp:443-466)
     if (active)
@@ -1036,7 +1070,40 @@ __host__ __device__ inline int stage2_need(int n, int G, int KP) {
 // the three damping rows: yobs[slot] = sum_d D_d (Q^T r)_{damping row d}, and keeps the rows' 3x9 entries per slot (dmp)
 // for the block kernel.  PANEL = false (no panels stored: operator_form = implicit): the orthogonality identities
 //   P^T (Q2^T r) = Jp^T r - Q1d^T (Q1^T r)_d ,  B^T B = Jp^T Jp - Q1d^T Q1d   (they cancel: float64 recommended).
-template <class S, bool PANEL>
+// The landmark prior's 3 rows [L~ | 0 | g] and the 3 damping rows [sqrt(lambda) I | 0 | 0] have no camera columns, so a QR
+// of the 6x3 [L~; sqrt(lambda) I] with the residual [g; 0] compresses them into 3 rows [C | 0 | c], C upper triangular
+// (DESIGN.md section 17).  Givens rotations in Eigen's convention, as the damping rotations; a zero column (rank-deficient
+// L, and lambda = 0) only meets rotations with c = +-1, s = 0.  The residual left in rows 3..5 does not depend on the
+// step and is dropped.
+template <class S>
+__device__ __forceinline__ void lm_prior_compress(const S* __restrict__ Lg, S sl, S (&C)[3][3], S (&c)[3]) {
+  S M[6][4];
+#pragma unroll
+  for (int r = 0; r < 3; ++r) {
+#pragma unroll
+    for (int k = 0; k < 3; ++k) { M[r][k] = Lg[3 * r + k]; M[3 + r][k] = r == k ? sl : S(0); }
+    M[r][3] = Lg[9 + r];
+    M[3 + r][3] = 0;
+  }
+#pragma unroll
+  for (int k = 0; k < 3; ++k)
+#pragma unroll
+    for (int m = k + 1; m < 6; ++m) {
+      const Rot<S> gq = make_givens(M[k][k], M[m][k]);
+#pragma unroll
+      for (int cc = k; cc < 4; ++cc) rot_apply(gq, M[m][cc], M[k][cc]);
+    }
+#pragma unroll
+  for (int r = 0; r < 3; ++r) {
+#pragma unroll
+    for (int k = 0; k < 3; ++k) C[r][k] = k >= r ? M[r][k] : S(0);
+    c[r] = M[r][3];
+  }
+}
+
+// LMP (landmark priors): a landmark with a prior starts its 6 rotations from Dw = C, dr = c (lm_prior_compress) instead
+// of sqrt(lambda) I, 0, also at lambda = 0; every other landmark, and every per-observation step, is unchanged.
+template <class S, bool PANEL, bool LMP = false>
 __global__ void __launch_bounds__(128) k_stage2(DevPtrs<S> D, S lambda, Scratch<S> sc, int write_panel) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   using V2 = typename ST<S>::V2;
@@ -1060,12 +1127,15 @@ __global__ void __launch_bounds__(128) k_stage2(DevPtrs<S> D, S lambda, Scratch<
       S Dw[3][3] = {{0, 0, 0}, {0, 0, 0}, {0, 0, 0}};
       S rr[3] = {lk[6], lk[7], lk[8]}, dr[3] = {0, 0, 0};
       S* ro = sRot + 20 * lane;
-      if (lambda == S(0)) {
+      int lp = -1;
+      if constexpr (LMP) lp = D.lmp_slot[T.lm_base + lane];
+      if (lambda == S(0) && lp < 0) {
 #pragma unroll
         for (int q = 0; q < 6; ++q) { ro[2 * q] = 1; ro[2 * q + 1] = 0; }
       } else {
         const S sl = sqrt(lambda);
-        Dw[0][0] = sl; Dw[1][1] = sl; Dw[2][2] = sl;
+        if (LMP && lp >= 0) lm_prior_compress(D.lmp_Lg + 12 * (size_t)lp, sl, Dw, dr);
+        else { Dw[0][0] = sl; Dw[1][1] = sl; Dw[2][2] = sl; }
         int q = 0;
 #pragma unroll
         for (int nn = 0; nn < 3; ++nn)
@@ -1169,7 +1239,8 @@ __global__ void __launch_bounds__(128) k_stage2(DevPtrs<S> D, S lambda, Scratch<
 //   numerics: the condition number of the landmark block is squared, which is what the QR solver avoids.
 //   One warp per tile, G lanes per landmark, lane per observation.
 // ------------------------------------------------------------------------------------------------
-template <class S>
+//   LMP (landmark priors, DESIGN.md section 17): Hll += L~^T L~ and Jl^T r += L~^T g of the landmark's prior.
+template <class S, bool LMP = false>
 __global__ void __launch_bounds__(128) k_sc_stage2(DevPtrs<S> D, S lambda) {
   const int wib = threadIdx.x >> 5, lane = threadIdx.x & 31;
   for (int t = blockIdx.x * (blockDim.x >> 5) + wib; t < D.ntiles; t += gridDim.x * (blockDim.x >> 5)) {
@@ -1193,6 +1264,18 @@ __global__ void __launch_bounds__(128) k_sc_stage2(DevPtrs<S> D, S lambda) {
     for (int k = 0; k < 6; ++k) h[k] = group_sum(h[k], G);
 #pragma unroll
     for (int k = 0; k < 3; ++k) gv[k] = group_sum(gv[k], G);
+    if constexpr (LMP) {
+      const int lp = D.lmp_slot[T.lm_base + g];
+      if (lp >= 0) {
+        const S* pg = D.lmp_Lg + 12 * (size_t)lp;
+#pragma unroll
+        for (int r = 0; r < 3; ++r) {
+          const S a0 = pg[3 * r], a1 = pg[3 * r + 1], a2 = pg[3 * r + 2], gr = pg[9 + r];
+          h[0] += a0 * a0; h[1] += a0 * a1; h[2] += a0 * a2; h[3] += a1 * a1; h[4] += a1 * a2; h[5] += a2 * a2;
+          gv[0] += a0 * gr; gv[1] += a1 * gr; gv[2] += a2 * gr;
+        }
+      }
+    }
     h[0] += lambda; h[3] += lambda; h[5] += lambda;  // landmark damping: Hll = Jl^T Jl + lambda I (sc/landmark_block.hpp:244-247)
     // Cholesky Hll = R^T R.  A block that is singular in working precision (one valid observation, lam below the resolution
     // of its diagonal) gives a NaN pivot; it reaches b, PCG and the l_diff of rba_apply, which reports it (as the reference,
@@ -2603,7 +2686,9 @@ __global__ void __launch_bounds__(VEC_THREADS) k_power_vec(DevPtrs<S> D, PcgStat
 // ------------------------------------------------------------------------------------------------
 // One warp per tile, one lane per observation, no shared memory: every record is one or a few 16-byte loads.
 // Pass 1 (q1d, dp) gives s_m and the landmark increment, pass 2 (jp, jl, r, dp) the model cost change.
-template <class S>
+// LMP (landmark priors, DESIGN.md section 17): l_diff also loses (L~ d)^T (1/2 L~ d + g) of each prior landmark, into this
+// shard's partial (the term is landmark-owned: it is counted once by the sum over the shards).
+template <class S, bool LMP = false>
 __global__ void __launch_bounds__(128) k_back_substitute(DevPtrs<S> D, const S* __restrict__ pose_inc,
                                                           double* partials, int* bad_flag) {
   const int wib = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -2668,6 +2753,17 @@ __global__ void __launch_bounds__(128) k_back_substitute(DevPtrs<S> D, const S* 
     }
     lpart = group_sum(lpart, G);
     if (active && j == 0) {
+      if constexpr (LMP) {
+        const int lp = D.lmp_slot[sidx];
+        if (lp >= 0) {
+          const S* pg = D.lmp_Lg + 12 * (size_t)lp;
+#pragma unroll
+          for (int r = 0; r < 3; ++r) {
+            const S u = pg[3 * r] * inc[0] + pg[3 * r + 1] * inc[1] + pg[3 * r + 2] * inc[2];
+            lpart += u * (S(0.5) * u + pg[9 + r]);
+          }
+        }
+      }
       ld[0] -= (double)lpart;
       const int lm = D.sorted_lm[sidx];
       S* pw = D.lms + 3 * (size_t)lm;
@@ -2923,6 +3019,34 @@ __global__ void k_prior_ldiff(const S* __restrict__ A, const S* __restrict__ pr,
   }
   const double s = prior_block_sum(acc);
   if (threadIdx.x == 0) red[0] += s;
+}
+
+// landmark-prior cost sum_p 1/2 |L_p (x_p - x0_p)|^2 of this shard's m priors (lm = local landmark of each), added to the
+// shard's all / valid errors (red[1], red[4]) BEFORE the sum over the shards: the term is landmark-owned, so each shard adds
+// its own priors and the sum counts each once (DESIGN.md section 17).  A non-finite sum sets the flag.  One block.
+template <class S>
+__global__ void k_lm_prior_cost(const S* __restrict__ lms, const int* __restrict__ lm, const S* __restrict__ mean,
+                                const S* __restrict__ Lsq, int m, double* red, int* bad_flag) {
+  double acc = 0;
+  for (int p = threadIdx.x; p < m; p += blockDim.x) {
+    const S* x = lms + 3 * (size_t)lm[p];
+    const S* x0 = mean + 3 * (size_t)p;
+    const S e0 = x[0] - x0[0], e1 = x[1] - x0[1], e2 = x[2] - x0[2];
+    const S* Lp = Lsq + 9 * (size_t)p;
+    S c2 = 0;
+#pragma unroll
+    for (int r = 0; r < 3; ++r) {
+      const S v = Lp[3 * r] * e0 + Lp[3 * r + 1] * e1 + Lp[3 * r + 2] * e2;
+      c2 += v * v;
+    }
+    acc += 0.5 * (double)c2;
+  }
+  const double s = prior_block_sum(acc);
+  if (threadIdx.x == 0) {
+    red[1] += s;
+    red[4] += s;
+    if (!isfinite(s)) *bad_flag = 1;
+  }
 }
 
 // ------------------------------------------------------------------------------------------------

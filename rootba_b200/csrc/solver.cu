@@ -53,6 +53,7 @@ struct rba_handle {
   virtual int set_camera_fixed(const uint8_t* flags) = 0;
   virtual int set_camera_prior(const void* mean, const void* sqrt_info) = 0;
   virtual int set_camera_pair_prior(int32_t num_pairs, const int32_t* pairs, const void* mean, const void* sqrt_info) = 0;
+  virtual int set_landmark_prior(int32_t num, const int32_t* lm_idx, const void* mean, const void* sqrt_info) = 0;
   virtual int compute_error(rba_residual_info* out) = 0;
   virtual int linearize() = 0;
   virtual int solve(double lambda, void* inc_out, rba_cg_summary* cg) = 0;
@@ -185,6 +186,15 @@ struct Solver : rba_handle {
   S* d_pair_O = nullptr;           // [2m][36] O of each directed edge
   int* d_pair_ptr = nullptr;       // [nc + 1]
   S* d_pair_ov = nullptr;          // [9 nc]
+  // landmark priors (rba_set_landmark_prior, DESIGN.md section 17): the n_lmp priors of this shard with a non-zero L;
+  // D.lmp_slot set while n_lmp > 0.  Buffers are sized for lmp_cap priors.
+  int n_lmp = 0, lmp_cap = 0;
+  int* d_lmp_slot = nullptr;       // [nsorted] prior slot per sorted landmark, -1 = none
+  int* d_lmp_of_lm = nullptr;      // [nl_local] prior slot per local landmark, -1 = none (rba_compute_covariance)
+  int* d_lmp_lm = nullptr;         // [m] local landmark of each prior
+  S* d_lmp_mean = nullptr;         // [m][3]
+  S* d_lmp_L = nullptr;            // [m][9]
+  S* d_lmp_Lg = nullptr;           // [m][12]
   rba_stage_timings tm{};
   EventPair ev_stage1, ev_stage2, ev_precond, ev_pcg, ev_backsub, ev_update, ev_error, ev_mv, ev_user;
   long long launches = 0;
@@ -496,6 +506,11 @@ struct Solver : rba_handle {
     CU(cudaFuncSetAttribute((k_linearize_qr<S, true>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)k1_smem));
     CU(cudaFuncSetAttribute((k_stage2<S, true>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)k2_smem));
     CU(cudaFuncSetAttribute((k_stage2<S, false>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)k2_smem));
+    // the landmark-prior instances (DESIGN.md section 17)
+    CU(cudaFuncSetAttribute((k_linearize_qr<S, false, true>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)k1_smem));
+    CU(cudaFuncSetAttribute((k_linearize_qr<S, true, true>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)k1_smem));
+    CU(cudaFuncSetAttribute((k_stage2<S, true, true>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)k2_smem));
+    CU(cudaFuncSetAttribute((k_stage2<S, false, true>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)k2_smem));
     k4_smem_small = (size_t)K4_WARPS * L.k4_scratch_per_warp * sizeof(S);
     if (k4_smem_small > 200 * 1024) { g_err = "matvec scratch exceeds shared memory"; return RBA_ERR_UNSUPPORTED; }
     CU(cudaFuncSetAttribute((k_matvec_large<S, K4_WARPS, KPMAX>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(k4_smem_small, 1024)));
@@ -796,6 +811,70 @@ struct Solver : rba_handle {
     return priors_changed();
   }
 
+  // Gaussian priors on landmark positions (DESIGN.md section 17).  Part of the linearisation (Jacobi scaling, L~, g), like
+  // the camera priors.  Every rank receives the full list and keeps the priors of its own landmark shard.  Priors with an
+  // all-zero L are dropped; none left in this shard = the unmodified kernels (D.lmp_slot == nullptr).  Every check runs
+  // before anything changes, so a rejected call leaves the previous priors.
+  int set_landmark_prior(int32_t num, const int32_t* idx, const void* mean_v, const void* sqrt_info_v) override {
+    auto bad = [&](const std::string& what) { g_err = "rba_set_landmark_prior: " + what; return RBA_ERR_INVALID_ARGUMENT; };
+    if (num < 0) return bad("num must be >= 0, got " + std::to_string(num));
+    if (num > 0 && (!idx || !mean_v || !sqrt_info_v)) return bad("lm_idx, mean and sqrt_info must be given when num > 0");
+    const S* m = (const S*)mean_v;
+    const S* Ls = (const S*)sqrt_info_v;
+    std::vector<uint8_t> seen((size_t)nl_total, 0);
+    std::vector<int> slot(L.sorted_lm.size(), -1), of_lm((size_t)L.nl_local, -1), lm;
+    std::vector<S> mean, Lsq;
+    for (int p = 0; p < num; ++p) {
+      const int l = idx[p];
+      const std::string tag = "prior " + std::to_string(p);
+      if (l < 0 || l >= nl_total) return bad(tag + " has a landmark index outside [0, " + std::to_string(nl_total) + ")");
+      if (seen[l]) return bad(tag + " repeats landmark " + std::to_string(l));
+      seen[l] = 1;
+      bool nonzero = false;
+      for (int k = 0; k < 3; ++k)
+        if (!std::isfinite((double)m[3 * (size_t)p + k])) return bad(tag + " has a non-finite mean");
+      for (int k = 0; k < 9; ++k) {
+        const double v = (double)Ls[9 * (size_t)p + k];
+        if (!std::isfinite(v)) return bad(tag + " has a non-finite sqrt_info");
+        nonzero = nonzero || v != 0.0;
+      }
+      if (!nonzero || l < L.lm_begin || l >= L.lm_end) continue;
+      const int q = (int)lm.size();
+      lm.push_back(l - L.lm_begin);
+      slot[L.sorted_of_lm[l - L.lm_begin]] = q;
+      of_lm[l - L.lm_begin] = q;
+      mean.insert(mean.end(), m + 3 * (size_t)p, m + 3 * (size_t)(p + 1));
+      Lsq.insert(Lsq.end(), Ls + 9 * (size_t)p, Ls + 9 * (size_t)(p + 1));
+    }
+    const int np = (int)lm.size();
+    if (np > 0) {
+      if (np > lmp_cap) {
+        for (void* q : {(void*)d_lmp_lm, (void*)d_lmp_mean, (void*)d_lmp_L, (void*)d_lmp_Lg}) TRY(dfree(q));
+        TRY(dalloc(&d_lmp_lm, (size_t)np, false));
+        TRY(dalloc(&d_lmp_mean, 3 * (size_t)np, false));
+        TRY(dalloc(&d_lmp_L, 9 * (size_t)np, false));
+        TRY(dalloc(&d_lmp_Lg, 12 * (size_t)np, false));
+        lmp_cap = np;
+      }
+      if (!d_lmp_slot) {
+        TRY(dalloc(&d_lmp_slot, slot.size(), false));
+        TRY(dalloc(&d_lmp_of_lm, of_lm.size(), false));
+      }
+      CU(cudaMemcpyAsync(d_lmp_slot, slot.data(), slot.size() * sizeof(int), cudaMemcpyHostToDevice, stream));
+      CU(cudaMemcpyAsync(d_lmp_of_lm, of_lm.data(), of_lm.size() * sizeof(int), cudaMemcpyHostToDevice, stream));
+      CU(cudaMemcpyAsync(d_lmp_lm, lm.data(), lm.size() * sizeof(int), cudaMemcpyHostToDevice, stream));
+      CU(cudaMemcpyAsync(d_lmp_mean, mean.data(), mean.size() * sizeof(S), cudaMemcpyHostToDevice, stream));
+      CU(cudaMemcpyAsync(d_lmp_L, Lsq.data(), Lsq.size() * sizeof(S), cudaMemcpyHostToDevice, stream));
+      CU(cudaStreamSynchronize(stream));
+    }
+    n_lmp = np;
+    D.lmp_slot = np > 0 ? d_lmp_slot : nullptr;
+    D.lmp_mean = d_lmp_mean;
+    D.lmp_L = d_lmp_L;
+    D.lmp_Lg = d_lmp_Lg;
+    return priors_changed();
+  }
+
   // launch with optional programmatic dependent launch (the kernel may start before its predecessor in the stream has
   // finished and orders itself with griddepcontrol.wait) and optional thread-block-cluster dimension
   template <class... KArgs, class... Args>
@@ -840,6 +919,10 @@ struct Solver : rba_handle {
     k_error<S><<<EBLOCKS, 256, 0, stream>>>(D, ko, d_epart, d_flags);
     k_sum_partials<6><<<1, 256, 0, stream>>>(d_epart, EBLOCKS, d_red);
     launches += 2;
+    if (n_lmp > 0) {  // + this shard's landmark priors' 1/2 |L e|^2, BEFORE the sum over the shards (landmark-owned)
+      k_lm_prior_cost<S><<<1, 256, 0, stream>>>(D.lms, d_lmp_lm, d_lmp_mean, d_lmp_L, n_lmp, d_red, d_flags);
+      ++launches;
+    }
     rc = allreduce_scalars(6); if (rc) return rc;
     if (has_abs_prior) {  // + sum of 1/2 |L e|^2, once, after the sum over the shards
       k_prior_cost<S><<<1, 256, 0, stream>>>(D.cams, d_prior_mean, d_prior_L, nc, d_red, d_flags);
@@ -901,10 +984,11 @@ struct Solver : rba_handle {
     }
     k_scaling<S><<<(9 * nc + 255) / 256, 256, 0, stream>>>(D.diag2, D.scaling, 9 * nc, (S)ko.jacobi_eps);
     // pass B: linearize (scaled) + Jl scaling + Householder QR + panel write
-    if (opt.use_householder_marginalization)
-      k_linearize_qr<S, false><<<tile_grid(k1_max_blocks), TILE_WARPS * 32, k1_smem, stream>>>(D, ko, k1_sc, d_flags, order_k1);
-    else  // ref: ipp:149-163 selects perform_qr_givens
-      k_linearize_qr<S, true><<<tile_grid(k1_max_blocks), TILE_WARPS * 32, k1_smem, stream>>>(D, ko, k1_sc, d_flags, order_k1);
+    // (+ the landmark priors' column norms, L~ and g: the LMP instances)
+    const bool lmp = D.lmp_slot != nullptr;
+    auto k1 = opt.use_householder_marginalization ? (lmp ? k_linearize_qr<S, false, true> : k_linearize_qr<S, false>)
+                                                  : (lmp ? k_linearize_qr<S, true, true> : k_linearize_qr<S, true>);  // ref: ipp:149-163 selects perform_qr_givens
+    k1<<<tile_grid(k1_max_blocks), TILE_WARPS * 32, k1_smem, stream>>>(D, ko, k1_sc, d_flags, order_k1);
     launches += 2;
     if (opt.preconditioner_type == 0 || opt.solver_type == 2) {
       // JACOBI: D (sum Jp^T Jp) D from the stored scaled Jacobians (Power-SC: these blocks are Hpp, sc/linearization_power_sc.hpp:92-128) (ref: ipp:554-569, block_sparse_matrix.hpp:89-100)
@@ -1103,11 +1187,16 @@ struct Solver : rba_handle {
     tm.matvec_launches = 0;
     int rc = start(ev_stage2); if (rc) return rc;
     // stage 2: landmark damping + gradient (+ SCHUR_JACOBI blocks)
+    // (landmark priors: the LMP instances, DESIGN.md section 17)
+    const bool lmp = D.lmp_slot != nullptr;
     if (opt.solver_type != 0) {
       // Schur-complement solvers: landmark eliminated through the normal equations (Cholesky of Jl^T Jl + lambda I)
-      k_sc_stage2<S><<<tile_grid(sm_count * 8), TILE_WARPS * 32, 0, stream>>>(D, lambda);
-    } else if (panel_form) k_stage2<S, true><<<tile_grid(k2_max_blocks), TILE_WARPS * 32, k2_smem, stream>>>(D, lambda, k2_sc, ko.write_panel);
-    else k_stage2<S, false><<<tile_grid(k2_max_blocks), TILE_WARPS * 32, k2_smem, stream>>>(D, lambda, k2_sc, ko.write_panel);
+      auto k = lmp ? k_sc_stage2<S, true> : k_sc_stage2<S>;
+      k<<<tile_grid(sm_count * 8), TILE_WARPS * 32, 0, stream>>>(D, lambda);
+    } else {
+      auto k = panel_form ? (lmp ? k_stage2<S, true, true> : k_stage2<S, true>) : (lmp ? k_stage2<S, false, true> : k_stage2<S, false>);
+      k<<<tile_grid(k2_max_blocks), TILE_WARPS * 32, k2_smem, stream>>>(D, lambda, k2_sc, ko.write_panel);
+    }
     ++launches;
     rc = camera_reduce(d_csr_obs_slots, d_csr_obs_items, n_obs_items, d_csr_obs_item_ptr, D.b, panel_form ? D.b0 : nullptr); if (rc) return rc;
     const bool power = opt.solver_type == 2;
@@ -1232,7 +1321,8 @@ struct Solver : rba_handle {
     int rc = start(ev_backsub); if (rc) return rc;
     CU(cudaMemsetAsync(d_flags, 0, 4 * sizeof(int), stream));
     const int grid = std::min(tile_grid(sm_count * 4), EBLOCKS);
-    k_back_substitute<S><<<grid, TILE_WARPS * 32, 0, stream>>>(D, D.inc, d_epart, d_flags);
+    auto kb = D.lmp_slot ? k_back_substitute<S, true> : k_back_substitute<S>;  // + the landmark priors' part of l_diff
+    kb<<<grid, TILE_WARPS * 32, 0, stream>>>(D, D.inc, d_epart, d_flags);
     k_sum_partials<1><<<1, 256, 0, stream>>>(d_epart, grid, d_red);
     launches += 2;
     rc = allreduce_scalars(1); if (rc) return rc;
@@ -1561,7 +1651,10 @@ struct Solver : rba_handle {
     CU(cudaMemsetAsync(A, 0, (size_t)(np * np) * 8, stream));
     CU(cudaMemsetAsync(fail, 0x7f, 4, stream));
     const int wgrid = std::max(1, std::min((nl + 3) / 4, sm_count * 16));
-    k_cov_landmark<S><<<wgrid, 128, 0, stream>>>(D, ko, d_cov_lm_slot0, d_cov_lm_n, nl, jp, kb, wl, rk);
+    if (n_lmp > 0)  // + L^T L of the landmark priors in Hll
+      k_cov_landmark<S, true><<<wgrid, 128, 0, stream>>>(D, ko, d_cov_lm_slot0, d_cov_lm_n, nl, jp, kb, wl, rk, d_lmp_of_lm);
+    else
+      k_cov_landmark<S><<<wgrid, 128, 0, stream>>>(D, ko, d_cov_lm_slot0, d_cov_lm_n, nl, jp, kb, wl, rk);
     k_cov_assemble<<<std::max(1, std::min((cov_nblk + 7) / 8, sm_count * 8)), 256, 0, stream>>>(d_cov_blk_cam, d_cov_blk_ptr, d_cov_terms,
                                                                                                   cov_nblk, jp, kb, A, np);
     if (has_abs_prior || n_pairs > 0)
@@ -1865,6 +1958,9 @@ int32_t rba_set_camera_fixed(rba_handle* h, const uint8_t* flags) { return h->se
 int32_t rba_set_camera_prior(rba_handle* h, const void* mean, const void* sqrt_info) { return h->set_camera_prior(mean, sqrt_info); }
 int32_t rba_set_camera_pair_prior(rba_handle* h, int32_t num_pairs, const int32_t* pairs, const void* mean, const void* sqrt_info) {
   return h->set_camera_pair_prior(num_pairs, pairs, mean, sqrt_info);
+}
+int32_t rba_set_landmark_prior(rba_handle* h, int32_t num, const int32_t* lm_idx, const void* mean, const void* sqrt_info) {
+  return h->set_landmark_prior(num, lm_idx, mean, sqrt_info);
 }
 int32_t rba_compute_error(rba_handle* h, rba_residual_info* out) { return h->compute_error(out); }
 int32_t rba_linearize(rba_handle* h) { return h->linearize(); }

@@ -148,6 +148,10 @@ class BalProblemSoA {
   std::vector<int32_t> camera_pair_prior_pairs;    // [m][2] (i, j)
   std::vector<double> camera_pair_prior_mean;      // [m][7] qx,qy,qz,qw, t0
   std::vector<double> camera_pair_prior_sqrt_info; // [m][36] row-major L
+  // Gaussian priors on landmark positions (rba_set_landmark_prior), forwarded by LinearizorQR::create; empty = none.
+  std::vector<int32_t> landmark_prior_idx;         // [m]
+  std::vector<double> landmark_prior_mean;         // [m][3] x0
+  std::vector<double> landmark_prior_sqrt_info;    // [m][9] row-major L
 
   int num_cameras() const { return nc; }
   int num_landmarks() const { return nl; }

@@ -231,6 +231,11 @@ class BalProblem {
   std::vector<int32_t> camera_pair_prior_pairs;    // [m][2] cameras (i, j)
   std::vector<double> camera_pair_prior_mean;      // [m][7] qx,qy,qz,qw (R0), t0 of T_i T_j^-1
   std::vector<double> camera_pair_prior_sqrt_info; // [m][36] row-major square-root information L
+  // Gaussian priors on landmark positions (rba_set_landmark_prior), forwarded by LinearizorQR::create; empty = none.
+  // Not in the reference.
+  std::vector<int32_t> landmark_prior_idx;         // [m] landmark indices
+  std::vector<double> landmark_prior_mean;         // [m][3] prior position x0
+  std::vector<double> landmark_prior_sqrt_info;    // [m][9] row-major square-root information L
 
  private:
   static void fail(FILE* f, const std::string& path) { std::fclose(f); throw std::runtime_error("Failed to parse '" + path + "'"); }

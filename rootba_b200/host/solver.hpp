@@ -194,6 +194,14 @@ class LinearizorQR {
       const VecX L(bp.camera_pair_prior_sqrt_info.begin(), bp.camera_pair_prior_sqrt_info.end());
       check(rba_set_camera_pair_prior(h_, (int32_t)np, bp.camera_pair_prior_pairs.data(), m.data(), L.data()));
     }
+    if (!bp.landmark_prior_idx.empty()) {
+      const size_t np = bp.landmark_prior_idx.size();
+      if (bp.landmark_prior_mean.size() != 3 * np || bp.landmark_prior_sqrt_info.size() != 9 * np)
+        throw std::runtime_error("landmark priors must have 3 mean and 9 sqrt_info entries per prior");
+      const VecX m(bp.landmark_prior_mean.begin(), bp.landmark_prior_mean.end());
+      const VecX L(bp.landmark_prior_sqrt_info.begin(), bp.landmark_prior_sqrt_info.end());
+      check(rba_set_landmark_prior(h_, (int32_t)np, bp.landmark_prior_idx.data(), m.data(), L.data()));
+    }
   }
   Problem& bal_problem_;
   SolverSummary* summary_ = nullptr;

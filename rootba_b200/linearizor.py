@@ -123,6 +123,31 @@ def _camera_pair_prior_arrays(prior, num_cameras: int, dtype):
     return pairs, mean, sqrt_info
 
 
+def _landmark_prior_arrays(prior, num_landmarks: int, dtype):
+    """None, or validated contiguous copies (idx [m] int32, mean [m,3], sqrt_info [m,3,3]) of landmark priors in the
+    problem's dtype"""
+    if prior is None:
+        return None
+    idx, mean, sqrt_info = prior
+    idx = np.array(idx, dtype=np.int32, order="C", copy=True)
+    mean = np.array(mean, dtype=dtype, order="C", copy=True)
+    sqrt_info = np.array(sqrt_info, dtype=dtype, order="C", copy=True)
+    m = idx.shape[0] if idx.ndim == 1 else -1
+    if idx.shape != (m,):
+        raise ValueError(f"landmark_prior idx must have shape (m,), got {idx.shape}")
+    if mean.shape != (m, 3):
+        raise ValueError(f"landmark_prior mean must have shape ({m}, 3), got {mean.shape}")
+    if sqrt_info.shape != (m, 3, 3):
+        raise ValueError(f"landmark_prior sqrt_info must have shape ({m}, 3, 3), got {sqrt_info.shape}")
+    if np.any(idx < 0) or np.any(idx >= num_landmarks):
+        raise ValueError(f"landmark_prior idx must be landmark indices in [0, {num_landmarks})")
+    if len(np.unique(idx)) != m:
+        raise ValueError("landmark_prior idx must not repeat a landmark")
+    if not (np.all(np.isfinite(mean)) and np.all(np.isfinite(sqrt_info))):
+        raise ValueError("landmark_prior entries must be finite")
+    return idx, mean, sqrt_info
+
+
 class BalProblem:
     """SoA BalProblem: cameras [nc,10] (quat xyzw, t, f,k1,k2), landmarks [nl,3], observations in
     CSR-by-landmark order with ascending camera index.  `camera_fixed` (not in the reference): None or one uint8 of FIX_*
@@ -132,7 +157,9 @@ class BalProblem:
     mean rows are (qx,qy,qz,qw of R0, camera centre c0, f0, k1_0, k2_0).  Forwarded to an attached LinearizorQR on assignment.
     `camera_pair_prior` (not in the reference): None or (pairs [m,2] int32, mean [m,7], sqrt_info [m,6,6]), relative pose priors
     T_i T_j^-1 ~ (R0, t0) with the cost 1/2 |L e|^2, e = (t_i - R_i R_j^T t_j - t0, Log(R_i R_j^T R0^T))
-    (rba_set_camera_pair_prior, DESIGN.md section 15); mean rows are (qx,qy,qz,qw of R0, t0).  Forwarded likewise."""
+    (rba_set_camera_pair_prior, DESIGN.md section 15); mean rows are (qx,qy,qz,qw of R0, t0).  Forwarded likewise.
+    `landmark_prior` (not in the reference): None or (idx [m] int32, mean [m,3], sqrt_info [m,3,3]), Gaussian priors on
+    landmark positions with the cost 1/2 |L (x - x0)|^2 (rba_set_landmark_prior, DESIGN.md section 17).  Forwarded likewise."""
 
     def __init__(self, cams, lms, lm_off, obs_cam, obs_xy, dtype=np.float64):
         self.dtype = np.dtype(dtype)
@@ -148,6 +175,18 @@ class BalProblem:
         self._camera_fixed = None
         self._camera_prior = None
         self._camera_pair_prior = None
+        self._landmark_prior = None
+
+    @property
+    def landmark_prior(self):
+        return self._landmark_prior
+
+    @landmark_prior.setter
+    def landmark_prior(self, prior):
+        p = _landmark_prior_arrays(prior, self.num_landmarks(), self.dtype)
+        if self._linearizor is not None:
+            self._linearizor._upload_landmark_prior(p)  # raises on rejection: the previous landmark priors stay in force
+        self._landmark_prior = p
 
     @property
     def camera_pair_prior(self):
@@ -287,6 +326,8 @@ class LinearizorQR:
             self._upload_camera_prior(bal_problem.camera_prior)
         if bal_problem.camera_pair_prior is not None:
             self._upload_camera_pair_prior(bal_problem.camera_pair_prior)
+        if bal_problem.landmark_prior is not None:
+            self._upload_landmark_prior(bal_problem.landmark_prior)
 
     # factory like Linearizor::create (linearizor.cpp:47-65)
     @staticmethod
@@ -343,6 +384,17 @@ class LinearizorQR:
             check(_lib.lib().rba_set_camera_pair_prior(self.h, C.c_int32(0), None, None, None))
         else:
             check(_lib.lib().rba_set_camera_pair_prior(self.h, C.c_int32(len(prior[0])), _p(prior[0]), _p(prior[1]), _p(prior[2])))
+
+    def set_landmark_prior(self, prior):
+        """Gaussian landmark priors (rba_set_landmark_prior): None, or (idx [m], mean [m,3], sqrt_info [m,3,3]).  Needs a new
+        linearize before the next solve; the priors are stored on the BalProblem."""
+        self.bal_problem.landmark_prior = prior  # validates and forwards to _upload_landmark_prior
+
+    def _upload_landmark_prior(self, prior):
+        if prior is None:
+            check(_lib.lib().rba_set_landmark_prior(self.h, 0, None, None, None))
+        else:
+            check(_lib.lib().rba_set_landmark_prior(self.h, len(prior[0]), _p(prior[0]), _p(prior[1]), _p(prior[2])))
 
     def _backup(self):
         check(_lib.lib().rba_backup(self.h))
