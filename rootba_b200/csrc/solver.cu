@@ -17,6 +17,7 @@
 #include "../host/bal_io_fast.hpp"
 #include "kernels.cuh"
 #include "covariance.cuh"
+#include "assembled.cuh"
 #include "nccl_dyn.hpp"
 
 namespace rba {
@@ -137,6 +138,8 @@ struct Solver : rba_handle {
   // test hooks (read_test_hooks)
   bool pcg_partials = true;      // one GPU: k_pcg_vec consumes the per-segment sums of k_cam_reduce
   bool peer_ar = true;           // rba_ipc_import maps the peers' exchange regions
+  bool asm_hook = true;          // the assembled operator when it qualifies (setup_assembled)
+  int asm_at = 0;                // > 0: build S at this PCG iteration instead of the break-even one
   int* h_prog = nullptr; int* d_prog = nullptr;  // PCG progress in host-mapped pinned memory: [0] last completed iteration, [1] solve ended
   int pcg_solve_id = 0;
   double* d_epart = nullptr;     // [EBLOCKS][6]
@@ -215,6 +218,17 @@ struct Solver : rba_handle {
   int cov_nblk = 0;
   int2* d_cov_blk_cam = nullptr; int* d_cov_blk_ptr = nullptr; int2* d_cov_terms = nullptr;
   int* d_cov_lm_slot0 = nullptr; int* d_cov_lm_n = nullptr;
+  // assembled operator (setup_assembled, assembled.cuh): the terms as panel addresses in landmark-major order, the pair
+  // list (term ranges, landmark-major position of every term), per pair its positions (lower, upper or -1) in the full
+  // block-row CSR of S, the landmark ranges staged at a time, the staging buffer, S_u per pair and S
+  // asm_on: the structure exists; su_valid: S_u belongs to the current linearisation; s_valid: S = S_u + the damping part of
+  // the last solve's lambda, and that solve (and rba_right_multiply / rba_time_matvec after it) applies S
+  bool asm_on = false, su_valid = false, s_valid = false;
+  int asm_nblk = 0, asm_switch = 0; long long asm_nnzb = 0;
+  std::vector<long long> asm_ranges;
+  AsmTerm* d_asm_terms = nullptr; int* d_asm_wpos = nullptr; int* d_asm_blk_ptr = nullptr; int2* d_asm_pos = nullptr;
+  int* d_asm_row_ptr = nullptr; int* d_asm_col = nullptr;
+  S* d_asm_stage = nullptr; S* d_asm_Su = nullptr; S* d_asm_S = nullptr;
 
   ~Solver() override {
     if (comm && nccl) nccl->CommDestroy(comm);
@@ -291,6 +305,7 @@ struct Solver : rba_handle {
     TRY(upload_layout(pv));
     TRY(deal_work());
     TRY(alloc_buffers());
+    TRY(setup_assembled());
     TRY(setup_kernels());
     CU(cudaStreamSynchronize(stream));
     return RBA_OK;
@@ -322,10 +337,14 @@ struct Solver : rba_handle {
   //   RBA_PCG_PARTIALS=0  PCG without the per-segment hand-over to the vector kernel (taken above 1808 cameras)
   //   RBA_PCG_CLUSTER=k   a PCG vector cluster of at most k CTAs (taken when the device grants fewer than 16)
   //   RBA_PEER_AR=0       NCCL for the reductions across shards (taken when the IPC mapping of a peer fails)
+  //   RBA_ASSEMBLED_RCS=0 the panel product P^T (P x) instead of the assembled S x (taken when S does not qualify)
+  //   RBA_ASSEMBLED_AT=k  S built at PCG iteration k instead of the break-even iteration (taken by solves that run long)
   void read_test_hooks() {
     if (const char* e = getenv("RBA_PCG_PARTIALS")) pcg_partials = atoi(e) != 0;
     if (const char* e = getenv("RBA_PCG_CLUSTER")) pcg_cluster = std::max(1, std::min(atoi(e), 16));
     if (const char* e = getenv("RBA_PEER_AR")) peer_ar = atoi(e) != 0;
+    if (const char* e = getenv("RBA_ASSEMBLED_RCS")) asm_hook = atoi(e) != 0;
+    if (const char* e = getenv("RBA_ASSEMBLED_AT")) asm_at = std::max(0, atoi(e));
   }
 
   int upload_layout(const rba_problem_view* pv) {
@@ -1020,6 +1039,7 @@ struct Solver : rba_handle {
     rc = stop(ev_stage1); if (rc) return rc;
     linearized = true;  // provisional: linearize_finish withdraws it on a numerical failure
     new_linearization_point = true;
+    su_valid = s_valid = false;
     damping_valid = false;
     have_inc = false;
     return RBA_OK;
@@ -1055,10 +1075,17 @@ struct Solver : rba_handle {
   // one complete operator application outside PCG: y = sum over the landmarks of P^T P x_red (this shard), per camera in D.y
   int matvec_launch(const S* xvec) {
     matvec_kernels(xvec, nullptr, false);
-    return cam_reduce_final(false, 0, false);
+    return s_valid ? RBA_OK : cam_reduce_final(false, 0, false);
   }
-  // operator part of one matvec: yobs = P^T P x_red for every landmark (e0_only: the implicit operator's E_0 x alone)
+  // operator part of one matvec: yobs = P^T P x_red for every landmark (e0_only: the implicit operator's E_0 x alone);
+  // assembled operator: D.y = S x_red, complete
   void matvec_kernels(const S* xvec, const int* done, bool pdl, int e0_only = 0) {
+    if (s_valid) {
+      launch_ex(k_rcs_spmv<S>, nc, SPMV_WARPS * 32, 0, pdl, 1, (const int*)d_asm_row_ptr, (const int*)d_asm_col, (const S*)d_asm_S, xvec,
+                D.y, done, (int)pdl);
+      ++tm.matvec_launches;
+      return;
+    }
     if (implicit_op) {
       const int ntl = (int)L.tiles.size();
       const bool p = pdl && imp_tile_split == ntl;  // a single kernel between the PCG vector step and the reduction
@@ -1114,6 +1141,7 @@ struct Solver : rba_handle {
   }
   // finish one operator application inside PCG (H v for v = p in mode 0/1, x in mode 2) and do the vector step
   int pcg_apply(int i, int mode, int is_last, S lambda) {
+    if (s_valid) return pcg_vec(i, mode, true, is_last, lambda);  // k_rcs_spmv has written D.y
     if (pcg_from_partials()) {
       // one GPU: the vector kernel adds the per-segment sums itself (same order as k_cam_reduce_final's last arriver:
       // bit-identical) -- no arrival counters, fences or second pass in the reduction
@@ -1198,6 +1226,7 @@ struct Solver : rba_handle {
       k<<<tile_grid(k2_max_blocks), TILE_WARPS * 32, k2_smem, stream>>>(D, lambda, k2_sc, ko.write_panel);
     }
     ++launches;
+    s_valid = false;  // S of the previous lambda; rebuilt if this solve runs long enough (solve_enqueue)
     rc = camera_reduce(d_csr_obs_slots, d_csr_obs_items, n_obs_items, d_csr_obs_item_ptr, D.b, panel_form ? D.b0 : nullptr); if (rc) return rc;
     const bool power = opt.solver_type == 2;
     const bool schur = opt.preconditioner_type == 1 && !power;  // Power-SC inverts Hpp = sum Jp^T Jp + lambda I instead
@@ -1271,7 +1300,15 @@ struct Solver : rba_handle {
           // every 64k polls: has the stream run dry (a launch failed, or the kernels ended without publishing)?  Then do not wait.
           if ((++spins & 0xffffu) == 0 && cudaStreamQuery(stream) != cudaErrorNotReady) break;
         }
-        if (prog[1]) break;
+        // once the solve has ended (at iteration prog[0], final when prog[1] is seen), exactly `depth` no-op iterations
+        // follow it, whatever the host's pace: the enqueued work does not depend on timing
+        if (prog[1] && i - prog[0] > depth) break;
+        if (asm_on && i == asm_switch) {
+          // the solve has run asm_switch - 1 iterations: from here on S x (S_u once per linearisation, then S for lambda)
+          if (!su_valid) assemble(0);
+          assemble(1);
+          su_valid = s_valid = true;
+        }
         rc = enqueue_iteration(i); if (rc) return rc;
       }
     }
@@ -1486,7 +1523,9 @@ struct Solver : rba_handle {
     out->panel_scalars = L.panel_scalars;
     out->panel_scalars_algorithmic = 18 * L.sum_n2;
     out->device_bytes = (int64_t)device_bytes;
-    out->matvec_algorithmic_bytes = (18 * L.sum_n2 + 18 * L.nobs_local) * (int64_t)sizeof(S) + 4 * L.nobs_local;
+    // the operator the last solve ended with: the panels, or S (blocks, column indices, row pointers, x read and y written once)
+    out->matvec_algorithmic_bytes = s_valid ? (81 * asm_nnzb + 18 * (int64_t)nc) * (int64_t)sizeof(S) + 4 * (asm_nnzb + nc + 1)
+                                           : (18 * L.sum_n2 + 18 * L.nobs_local) * (int64_t)sizeof(S) + 4 * L.nobs_local;
     out->landmark_begin = L.lm_begin;
     out->landmark_end = L.lm_end;
     out->num_matvec_items = (int)L.items.size();
@@ -1549,6 +1588,155 @@ struct Solver : rba_handle {
   int synchronize() override { CU(cudaStreamSynchronize(stream)); return RBA_OK; }
 
   // ------------------------------------------------------------------------------------------
+  // Co-visible camera pairs, shared by the assembled operator and rba_compute_covariance.  Per landmark its first slot and
+  // track length; per co-visible camera pair (ca >= cb), ascending (ca, cb), the terms (slot_a, slot_b) of every landmark
+  // that sees both, landmarks in problem order and within a landmark in observation order: the fixed summation order of
+  // k_rcs_combine and k_cov_assemble.  wpos[t] = position of term t in the landmark-major enumeration (landmarks in
+  // problem order, then a = 0..n-1, b = 0..a), the order of k_rcs_terms.
+  struct PairTerms {
+    std::vector<int> slot0, nn;      // [nl_local]
+    std::vector<int2> blk_cam;       // [nblk] (ca, cb)
+    std::vector<int> blk_ptr;        // [nblk + 1] into terms
+    std::vector<int2> terms;         // (slot_a, slot_b)
+    std::vector<int> wpos;           // landmark-major position of each term
+  };
+  int pair_terms(PairTerms& P) {
+    const int nl = L.nl_local;
+    P.slot0.resize(nl); P.nn.resize(nl);
+    long long nt = 0;
+    for (int lm = 0; lm < nl; ++lm) {
+      const int sidx = L.sorted_of_lm[lm];
+      const TileInfo& T = L.tiles[L.tile_of_sorted[sidx]];
+      P.slot0[lm] = T.slot_base + (sidx - T.lm_base) * T.n;
+      P.nn[lm] = T.n;
+      nt += (long long)T.n * (T.n + 1) / 2;
+    }
+    if (nt > std::numeric_limits<int>::max()) { g_err = "more than 2^31 camera-pair terms"; return RBA_ERR_UNSUPPORTED; }
+    // landmark-major list, then two stable counting sorts of its positions (by cb, then by ca): ascending (ca, cb),
+    // landmark order kept
+    std::vector<int2> raw;
+    raw.reserve((size_t)nt);
+    for (int lm = 0; lm < nl; ++lm)
+      for (int a = 0; a < P.nn[lm]; ++a)
+        for (int b = 0; b <= a; ++b) raw.push_back(make_int2(P.slot0[lm] + a, P.slot0[lm] + b));  // camera(a) >= camera(b)
+    std::vector<int> idx(raw.size()), tmp(raw.size());
+    std::iota(idx.begin(), idx.end(), 0);
+    std::vector<long long> cnt((size_t)nc + 1);
+    auto pass = [&](const std::vector<int>& src, std::vector<int>& dst, bool by_a) {
+      std::fill(cnt.begin(), cnt.end(), 0LL);
+      for (int w : src) ++cnt[L.slot_cam[by_a ? raw[w].x : raw[w].y] + 1];
+      for (int c = 0; c < nc; ++c) cnt[c + 1] += cnt[c];
+      for (int w : src) dst[cnt[L.slot_cam[by_a ? raw[w].x : raw[w].y]]++] = w;
+    };
+    pass(idx, tmp, false);
+    pass(tmp, idx, true);
+    tmp.clear(); tmp.shrink_to_fit();
+    P.terms.resize(raw.size());
+    for (size_t t = 0; t < idx.size(); ++t) P.terms[t] = raw[idx[t]];
+    P.wpos.swap(idx);
+    P.blk_cam.clear(); P.blk_ptr.clear();
+    for (size_t t = 0; t < P.terms.size(); ++t) {
+      const int2 cc = make_int2(L.slot_cam[P.terms[t].x], L.slot_cam[P.terms[t].y]);
+      if (t == 0 || cc.x != P.blk_cam.back().x || cc.y != P.blk_cam.back().y) {
+        P.blk_cam.push_back(cc);
+        P.blk_ptr.push_back((int)t);
+      }
+    }
+    P.blk_ptr.push_back((int)P.terms.size());
+    return RBA_OK;
+  }
+
+  // The assembled operator (assembled.cuh, DESIGN.md section 4): taken with one GPU and the dense operator when S is at
+  // most a quarter of the panel bytes and its storage fits in the free device memory; else the panel product.  Built here,
+  // once: the terms as panel addresses in landmark-major order, the pair list, the full block-row CSR and the positions of
+  // every pair's blocks in it, and the landmark ranges whose terms fit in the staging buffer (at most 2 GB, or one
+  // landmark's terms if more).
+  int setup_assembled() {
+    if (!asm_hook || opt.nranks != 1 || implicit_op) return RBA_OK;
+    PairTerms P;
+    TRY(pair_terms(P));
+    const long long nblk = (long long)P.blk_cam.size(), nt = (long long)P.terms.size();
+    long long ndiag = 0;
+    for (const int2& c : P.blk_cam) ndiag += c.x == c.y;
+    const long long nnzb = 2 * nblk - ndiag;
+    const size_t s_bytes = (size_t)nnzb * 81 * sizeof(S);
+    if (4 * s_bytes > (size_t)L.panel_scalars * sizeof(S)) return RBA_OK;
+    const long long cap = std::max<long long>(1, ((long long)2 << 30) / (81 * (long long)sizeof(S)));
+    std::vector<long long> ranges{0};
+    long long w = 0, stage_terms = 0;
+    for (int lm = 0; lm < L.nl_local; ++lm) {
+      const long long k = (long long)P.nn[lm] * (P.nn[lm] + 1) / 2;
+      if (w + k - ranges.back() > cap && w > ranges.back()) ranges.push_back(w);
+      w += k;
+      stage_terms = std::max(stage_terms, w - ranges.back());
+    }
+    ranges.push_back(nt);
+    // range by range the combine searches every pair's terms once per range: measured slower than the panel product on
+    // Final-13682 (21 ranges); one range only
+    if (ranges.size() > 2) return RBA_OK;
+    const size_t need = s_bytes + (size_t)(nblk + stage_terms) * 81 * sizeof(S) + (size_t)nt * (sizeof(AsmTerm) + sizeof(int)) +
+                        (size_t)(nblk + nnzb + nc + 2) * sizeof(int) + (size_t)nblk * sizeof(int2);
+    size_t free_b = 0, total_b = 0;
+    CU(cudaMemGetInfo(&free_b, &total_b));
+    if (need + ((size_t)256 << 20) > free_b) return RBA_OK;  // keep 256 MB for the rest of the handle and the caller
+    // full CSR: row ca gets (ca, cb) and row cb the transpose; iterating the pairs in (ca, cb) order fills every row in
+    // ascending column order (lower blocks, the diagonal, then upper blocks)
+    std::vector<int> row_ptr((size_t)nc + 1, 0), colv((size_t)nnzb);
+    for (const int2& c : P.blk_cam) { ++row_ptr[c.x + 1]; if (c.x != c.y) ++row_ptr[c.y + 1]; }
+    for (int c = 0; c < nc; ++c) row_ptr[c + 1] += row_ptr[c];
+    std::vector<int> fill(row_ptr.begin(), row_ptr.end() - 1);
+    std::vector<int2> posv((size_t)nblk);
+    for (long long b = 0; b < nblk; ++b) {
+      const int2 c = P.blk_cam[b];
+      const int lo = fill[c.x]++;
+      colv[lo] = c.y;
+      int up = -1;
+      if (c.x != c.y) { up = fill[c.y]++; colv[up] = c.x; }
+      posv[b] = make_int2(lo, up);
+    }
+    std::vector<AsmTerm> at;
+    at.reserve((size_t)nt);
+    for (int lm = 0; lm < L.nl_local; ++lm) {
+      const int sidx = L.sorted_of_lm[lm];
+      const TileInfo& T = L.tiles[L.tile_of_sorted[sidx]];
+      const int g = sidx - T.lm_base;
+      for (int a = 0; a < T.n; ++a)
+        for (int b = 0; b <= a; ++b)
+          at.push_back({T.panel_off + 2LL * g * T.G, a | b << 16, T.n | (31 - __builtin_clz((unsigned)T.G)) << 15 | (int)T.KP << 18});
+    }
+    TRY(upload(&d_asm_terms, at));
+    TRY(upload(&d_asm_wpos, P.wpos));
+    TRY(upload(&d_asm_blk_ptr, P.blk_ptr));
+    TRY(upload(&d_asm_pos, posv));
+    TRY(upload(&d_asm_row_ptr, row_ptr));
+    TRY(upload(&d_asm_col, colv));
+    TRY(dalloc(&d_asm_stage, (size_t)stage_terms * 81, false));
+    TRY(dalloc(&d_asm_Su, (size_t)nblk * 81));
+    TRY(dalloc(&d_asm_S, (size_t)nnzb * 81));
+    asm_ranges = ranges;
+    asm_nblk = (int)nblk; asm_nnzb = nnzb;
+    // Switch point: building S costs about twice its staging traffic (stage 1 + stage 2, each written and read once) in
+    // units of operator time, and every iteration with S saves the panel bytes minus the bytes of S (measured on H100:
+    // Ladybug-1723 f32 breaks even after ~23 iterations, Trafalgar-257 f64 after ~24)
+    const double staged = 4.0 * (double)nt * 81 * sizeof(S), saved = (double)L.panel_scalars * sizeof(S) - (double)s_bytes;
+    asm_switch = asm_at > 0 ? asm_at : 1 + (int)std::ceil(2.0 * staged / std::max(saved, 1.0));
+    asm_on = true;
+    return RBA_OK;
+  }
+  // S_u (stage 1, damping = 0) or S = S_u + the damping rows' part (stage 2, damping = 1), one landmark range at a time
+  void assemble(int damping) {
+    for (size_t k = 0; k + 1 < asm_ranges.size(); ++k) {
+      const long long w0 = asm_ranges[k], w1 = asm_ranges[k + 1];
+      const int grid = (int)std::max<long long>(1, std::min<long long>((w1 - w0 + 23) / 24, (long long)sm_count * 16));
+      k_rcs_terms<S><<<grid, 256, 0, stream>>>(D.panel, d_asm_terms, w0, w1, damping, d_asm_stage);
+      k_rcs_combine<S><<<(unsigned)((81LL * asm_nblk + 255) / 256), 256, 0, stream>>>(
+          d_asm_blk_ptr, d_asm_wpos, asm_nblk, w0, w1, d_asm_stage, damping ? (const S*)d_asm_Su : nullptr,
+          damping ? (const int2*)d_asm_pos : nullptr, (int)(k == 0), damping ? d_asm_S : d_asm_Su);
+      launches += 2;
+    }
+  }
+
+  // ------------------------------------------------------------------------------------------
   // Marginal covariances (DESIGN.md section 16).  Nothing of the handle changes: the scratch is allocated for the call and
   // freed before it returns; the state, the linearisation, the increment, the error cache and the timings are not touched.
   // The term lists built at the first call stay on the handle (not counted in device_bytes).
@@ -1561,48 +1749,17 @@ struct Solver : rba_handle {
     *p = (T*)q;
     return RBA_OK;
   }
-  // Per landmark its first slot and track length; per co-visible camera pair (ca >= cb) the terms (slot_a, slot_b) of every
-  // landmark that sees both, landmarks in problem order and within a landmark in observation order: the fixed summation
-  // order of k_cov_assemble.
+  // The term lists of rba_compute_covariance (pair_terms), built at the first call.
   int cov_build_lists() {
     if (cov_ready) return RBA_OK;
-    const int nl = L.nl_local;
-    std::vector<int> slot0(nl), nn(nl);
-    long long nt = 0;
-    for (int lm = 0; lm < nl; ++lm) {
-      const int sidx = L.sorted_of_lm[lm];
-      const TileInfo& T = L.tiles[L.tile_of_sorted[sidx]];
-      slot0[lm] = T.slot_base + (sidx - T.lm_base) * T.n;
-      nn[lm] = T.n;
-      nt += (long long)T.n * (T.n + 1) / 2;
-    }
-    if (nt > std::numeric_limits<int>::max()) { g_err = "rba_compute_covariance: more than 2^31 camera-pair terms"; return RBA_ERR_UNSUPPORTED; }
-    struct Term { long long key; int sa, sb; };
-    std::vector<Term> terms;
-    terms.reserve((size_t)nt);
-    for (int lm = 0; lm < nl; ++lm)
-      for (int a = 0; a < nn[lm]; ++a)
-        for (int b = 0; b <= a; ++b) {  // cameras ascend with the slot: camera(a) >= camera(b)
-          const int sa = slot0[lm] + a, sb = slot0[lm] + b;
-          terms.push_back({(long long)L.slot_cam[sa] * nc + L.slot_cam[sb], sa, sb});
-        }
-    std::stable_sort(terms.begin(), terms.end(), [](const Term& x, const Term& y) { return x.key < y.key; });
-    std::vector<int2> blk_cam, tl(terms.size());
-    std::vector<int> blk_ptr;
-    for (size_t t = 0; t < terms.size(); ++t) {
-      if (t == 0 || terms[t].key != terms[t - 1].key) {
-        blk_cam.push_back(make_int2((int)(terms[t].key / nc), (int)(terms[t].key % nc)));
-        blk_ptr.push_back((int)t);
-      }
-      tl[t] = make_int2(terms[t].sa, terms[t].sb);
-    }
-    blk_ptr.push_back((int)terms.size());
-    TRY(cov_upload(&d_cov_blk_cam, blk_cam));
-    TRY(cov_upload(&d_cov_blk_ptr, blk_ptr));
-    TRY(cov_upload(&d_cov_terms, tl));
-    TRY(cov_upload(&d_cov_lm_slot0, slot0));
-    TRY(cov_upload(&d_cov_lm_n, nn));
-    cov_nblk = (int)blk_cam.size();
+    PairTerms P;
+    TRY(pair_terms(P));
+    TRY(cov_upload(&d_cov_blk_cam, P.blk_cam));
+    TRY(cov_upload(&d_cov_blk_ptr, P.blk_ptr));
+    TRY(cov_upload(&d_cov_terms, P.terms));
+    TRY(cov_upload(&d_cov_lm_slot0, P.slot0));
+    TRY(cov_upload(&d_cov_lm_n, P.nn));
+    cov_nblk = (int)P.blk_cam.size();
     cov_ready = true;
     return RBA_OK;
   }
