@@ -203,7 +203,8 @@ __global__ void __launch_bounds__(256) k_cov_assemble(const int2* __restrict__ b
 
 // Thread per camera c: adds to its block row (lower triangle) the absolute prior's A^T A and, over its incident pair sides
 // in list order, the pair blocks A_s^T A_s (diagonal) and A_s^T A_o (to the column block of the other camera o < c).
-// The blocks are those of k_prior_linearize / k_pair_linearize, unscaled, evaluated in double from the stored means and L.
+// The rows are those of k_prior_linearize / k_pair_linearize (prior_jac_row, pair_jac_rows), unscaled, evaluated in double
+// from the stored means and L.
 template <class S>
 __global__ void k_cov_priors(const S* __restrict__ cams, int nc, const S* __restrict__ pmean, const S* __restrict__ pL,
                              const int* __restrict__ pairs, const S* __restrict__ qmean, const S* __restrict__ qL,
@@ -221,13 +222,7 @@ __global__ void k_cov_priors(const S* __restrict__ cams, int nc, const S* __rest
       double l[9], row[9];
 #pragma unroll
       for (int k = 0; k < 9; ++k) l[k] = (double)pL[81 * (size_t)c + 9 * i + k];
-      // row i of L de/d(inc): de/dv = -R^T, dLog/dw = J_l^-1, identity on the intrinsics
-#pragma unroll
-      for (int j = 0; j < 3; ++j) row[j] = -(l[0] * R[3 * j] + l[1] * R[3 * j + 1] + l[2] * R[3 * j + 2]);
-#pragma unroll
-      for (int j = 0; j < 3; ++j) row[3 + j] = l[3] * Jinv[j] + l[4] * Jinv[3 + j] + l[5] * Jinv[6 + j];
-#pragma unroll
-      for (int j = 6; j < 9; ++j) row[j] = l[j];
+      prior_jac_row(l, R, Jinv, row);
       for (int a = 0; a < 9; ++a)
         for (int b = 0; b <= a; ++b) Acc[a + b * ld] += row[a] * row[b];
     }
@@ -243,27 +238,13 @@ __global__ void k_cov_priors(const S* __restrict__ cams, int nc, const S* __rest
       }
 #pragma unroll
       for (int k = 0; k < 7; ++k) mean[k] = (double)qmean[7 * (size_t)p + k];
-      pair_residual<double, true>(ci, cj, mean, e, M, tr, Jinv);
-#pragma unroll
-      for (int a = 0; a < 3; ++a)
-#pragma unroll
-        for (int b = 0; b < 3; ++b) JM[3 * a + b] = Jinv[3 * a] * M[b] + Jinv[3 * a + 1] * M[3 + b] + Jinv[3 * a + 2] * M[6 + b];
+      pair_residual<double, true>(ci, cj, mean, e, M, tr, Jinv, JM);
       double* Aco = A + 9 * (long long)c + 9 * (long long)o * ld;  // block (c, o), used when o < c
       for (int i = 0; i < 6; ++i) {
         double l[6], ri[6], rj[6];
 #pragma unroll
         for (int k = 0; k < 6; ++k) l[k] = (double)qL[36 * (size_t)p + 6 * i + k];
-        // rows of A_i = (l_t, l_t (-[t_rel]x) + l_r J_l^-1) and A_j = (-l_t M, -l_r J_l^-1 M)
-#pragma unroll
-        for (int j = 0; j < 3; ++j) ri[j] = l[j];
-        ri[3] = -l[1] * tr[2] + l[2] * tr[1] + l[3] * Jinv[0] + l[4] * Jinv[3] + l[5] * Jinv[6];
-        ri[4] = l[0] * tr[2] - l[2] * tr[0] + l[3] * Jinv[1] + l[4] * Jinv[4] + l[5] * Jinv[7];
-        ri[5] = -l[0] * tr[1] + l[1] * tr[0] + l[3] * Jinv[2] + l[4] * Jinv[5] + l[5] * Jinv[8];
-#pragma unroll
-        for (int j = 0; j < 3; ++j) {
-          rj[j] = -(l[0] * M[j] + l[1] * M[3 + j] + l[2] * M[6 + j]);
-          rj[3 + j] = -(l[3] * JM[j] + l[4] * JM[3 + j] + l[5] * JM[6 + j]);
-        }
+        pair_jac_rows(l, M, tr, Jinv, JM, ri, rj);
         const double* own = side ? rj : ri;
         const double* oth = side ? ri : rj;
         for (int a = 0; a < 6; ++a) {

@@ -2895,6 +2895,57 @@ __device__ __forceinline__ void prior_residual(const S* __restrict__ cam, const 
   if (JAC) so3_jl_inv(e + 3, Jinv);
 }
 
+// row of L de/d(inc) for the row l [9] of L: L (-R^T) on v, L J_l^-1 on w, L itself on the intrinsics
+template <class S>
+__device__ __forceinline__ void prior_jac_row(const S* l, const S* R, const S* Jinv, S* row) {
+#pragma unroll
+  for (int j = 0; j < 3; ++j) row[j] = -(l[0] * R[3 * j] + l[1] * R[3 * j + 1] + l[2] * R[3 * j + 2]);
+#pragma unroll
+  for (int j = 0; j < 3; ++j) row[3 + j] = l[3] * Jinv[j] + l[4] * Jinv[3 + j] + l[5] * Jinv[6 + j];
+#pragma unroll
+  for (int j = 6; j < 9; ++j) row[j] = l[j];
+}
+
+// The per-item terms of the one-block kernels k_prior_cost and k_prior_ldiff, one struct per prior kind (item = camera,
+// pair or landmark prior).  sq_norm(p) = |L e|^2 of item p, model_change(inc, p) = (A d)^T (1/2 A d + r) for its part d
+// of the increment; each kind keeps its own summation order.
+template <class S>
+struct CameraPrior {
+  using Scalar = S;
+  const S* cams;
+  const S* mean;  // [nc][10]
+  const S* L;     // [nc][81]
+  const S* A;     // [nc][81]
+  const S* r;     // [nc][9]
+  __device__ S sq_norm(int cam) const {
+    S e[9];
+    prior_residual<S, false>(cams + 10 * (size_t)cam, mean + 10 * (size_t)cam, e, nullptr, nullptr);
+    const S* Lc = L + 81 * (size_t)cam;
+    S c2 = 0;
+    for (int i = 0; i < 9; ++i) {
+      S ri = 0;
+#pragma unroll
+      for (int k = 0; k < 9; ++k) ri += Lc[9 * i + k] * e[k];
+      c2 += ri * ri;
+    }
+    return c2;
+  }
+  __device__ S model_change(const S* inc, int cam) const {
+    S d[9];
+#pragma unroll
+    for (int j = 0; j < 9; ++j) d[j] = inc[9 * (size_t)cam + j];
+    const S* Ac = A + 81 * (size_t)cam;
+    S lp = 0;
+    for (int i = 0; i < 9; ++i) {
+      S u = 0;
+#pragma unroll
+      for (int j = 0; j < 9; ++j) u += Ac[9 * i + j] * d[j];
+      lp += u * (S(0.5) * u + r[9 * (size_t)cam + i]);
+    }
+    return lp;
+  }
+};
+
 // once per linearisation, after the cross-shard sum of diag2 and before k_scaling: the unscaled prior Jacobian
 // J = L de/d(inc) -> A [nc][81], r = L e -> pr [nc][9], and its squared column norms added to diag2 (the Jacobi scaling is
 // that of the whole Jacobian).  Thread per camera; identical on every shard (the prior data and the cameras are replicated).
@@ -2917,12 +2968,7 @@ __global__ void k_prior_linearize(const S* __restrict__ cams, const S* __restric
     S row[9], ri = 0;
 #pragma unroll
     for (int k = 0; k < 9; ++k) ri += l[k] * e[k];
-#pragma unroll
-    for (int j = 0; j < 3; ++j) row[j] = -(l[0] * R[3 * j] + l[1] * R[3 * j + 1] + l[2] * R[3 * j + 2]);  // L (-R^T)
-#pragma unroll
-    for (int j = 0; j < 3; ++j) row[3 + j] = l[3] * Jinv[j] + l[4] * Jinv[3 + j] + l[5] * Jinv[6 + j];
-#pragma unroll
-    for (int j = 6; j < 9; ++j) row[j] = l[j];
+    prior_jac_row(l, R, Jinv, row);
 #pragma unroll
     for (int j = 0; j < 9; ++j) { Ac[9 * i + j] = row[j]; cn[j] += row[j] * row[j]; }
     pr[9 * (size_t)cam + i] = ri;
@@ -2971,25 +3017,12 @@ __device__ __forceinline__ double prior_block_sum(double v) {
   return s;  // valid in thread 0
 }
 
-// prior cost sum_c 1/2 |L_c e_c|^2 at the current cameras, added to the all / valid errors (red[1], red[4]); a non-finite
-// sum sets the numerical-failure flag.  One block.
-template <class S>
-__global__ void k_prior_cost(const S* __restrict__ cams, const S* __restrict__ mean, const S* __restrict__ Lsq, int nc,
-                             double* red, int* bad_flag) {
+// cost sum_p 1/2 |L_p e_p|^2 of the n items of one prior kind K at the current parameters, added to the all / valid errors
+// (red[1], red[4]); a non-finite sum sets the numerical-failure flag.  One block.
+template <class K>
+__global__ void k_prior_cost(K k, int n, double* red, int* bad_flag) {
   double acc = 0;
-  for (int cam = threadIdx.x; cam < nc; cam += blockDim.x) {
-    S e[9];
-    prior_residual<S, false>(cams + 10 * (size_t)cam, mean + 10 * (size_t)cam, e, nullptr, nullptr);
-    const S* Lc = Lsq + 81 * (size_t)cam;
-    S c2 = 0;
-    for (int i = 0; i < 9; ++i) {
-      S ri = 0;
-#pragma unroll
-      for (int k = 0; k < 9; ++k) ri += Lc[9 * i + k] * e[k];
-      c2 += ri * ri;
-    }
-    acc += 0.5 * (double)c2;
-  }
+  for (int p = threadIdx.x; p < n; p += blockDim.x) acc += 0.5 * (double)k.sq_norm(p);
   const double s = prior_block_sum(acc);
   if (threadIdx.x == 0) {
     red[1] += s;
@@ -2998,56 +3031,39 @@ __global__ void k_prior_cost(const S* __restrict__ cams, const S* __restrict__ m
   }
 }
 
-// prior part of the model cost change: l_diff -= sum_c (A d)^T (1/2 A d + r) for the (masked, scaled) increment d, added to
-// red[0] (the back-substitution's l_diff, already summed over the shards).  One block.
-template <class S>
-__global__ void k_prior_ldiff(const S* __restrict__ A, const S* __restrict__ pr, const S* __restrict__ inc, int nc, double* red) {
+// prior part of the model cost change: l_diff -= sum_p (A d)^T (1/2 A d + r) over the n items of one prior kind K for the
+// (masked, scaled) increment d, added to red[0] (the back-substitution's l_diff, already summed over the shards).  One block.
+template <class K>
+__global__ void k_prior_ldiff(K k, const typename K::Scalar* __restrict__ inc, int n, double* red) {
   double acc = 0;
-  for (int cam = threadIdx.x; cam < nc; cam += blockDim.x) {
-    S d[9];
-#pragma unroll
-    for (int j = 0; j < 9; ++j) d[j] = inc[9 * (size_t)cam + j];
-    const S* Ac = A + 81 * (size_t)cam;
-    S lp = 0;
-    for (int i = 0; i < 9; ++i) {
-      S u = 0;
-#pragma unroll
-      for (int j = 0; j < 9; ++j) u += Ac[9 * i + j] * d[j];
-      lp += u * (S(0.5) * u + pr[9 * (size_t)cam + i]);
-    }
-    acc -= (double)lp;
-  }
+  for (int p = threadIdx.x; p < n; p += blockDim.x) acc -= (double)k.model_change(inc, p);
   const double s = prior_block_sum(acc);
   if (threadIdx.x == 0) red[0] += s;
 }
 
-// landmark-prior cost sum_p 1/2 |L_p (x_p - x0_p)|^2 of this shard's m priors (lm = local landmark of each), added to the
-// shard's all / valid errors (red[1], red[4]) BEFORE the sum over the shards: the term is landmark-owned, so each shard adds
-// its own priors and the sum counts each once (DESIGN.md section 17).  A non-finite sum sets the flag.  One block.
+// Landmark priors (DESIGN.md section 17): e_p = x_p - x0_p of this shard's priors (lm = local landmark of each).  Their cost
+// is added BEFORE the sum over the shards: the term is landmark-owned, so each shard adds its own priors and the sum counts
+// each once.  Their share of l_diff is computed per landmark in k_back_substitute.
 template <class S>
-__global__ void k_lm_prior_cost(const S* __restrict__ lms, const int* __restrict__ lm, const S* __restrict__ mean,
-                                const S* __restrict__ Lsq, int m, double* red, int* bad_flag) {
-  double acc = 0;
-  for (int p = threadIdx.x; p < m; p += blockDim.x) {
+struct LandmarkPrior {
+  const S* lms;
+  const int* lm;   // [m]
+  const S* mean;   // [m][3]
+  const S* L;      // [m][9]
+  __device__ S sq_norm(int p) const {
     const S* x = lms + 3 * (size_t)lm[p];
     const S* x0 = mean + 3 * (size_t)p;
     const S e0 = x[0] - x0[0], e1 = x[1] - x0[1], e2 = x[2] - x0[2];
-    const S* Lp = Lsq + 9 * (size_t)p;
+    const S* Lp = L + 9 * (size_t)p;
     S c2 = 0;
 #pragma unroll
     for (int r = 0; r < 3; ++r) {
       const S v = Lp[3 * r] * e0 + Lp[3 * r + 1] * e1 + Lp[3 * r + 2] * e2;
       c2 += v * v;
     }
-    acc += 0.5 * (double)c2;
+    return c2;
   }
-  const double s = prior_block_sum(acc);
-  if (threadIdx.x == 0) {
-    red[1] += s;
-    red[4] += s;
-    if (!isfinite(s)) *bad_flag = 1;
-  }
-}
+};
 
 // ------------------------------------------------------------------------------------------------
 // K9  Relative pose priors between two cameras (rba_set_camera_pair_prior, DESIGN.md section 15).  Pair p = (i, j) with the
@@ -3061,10 +3077,10 @@ __global__ void k_lm_prior_cost(const S* __restrict__ lms, const int* __restrict
 //     after k_pair_scale; pr [m][6] = L e.  Incident pair sides are listed camera-major (ptr [nc + 1], item = 2 p + side,
 //     ascending p within a camera), which is also the CSR of the directed edges i -> j of the off-diagonal blocks O_ij.
 // ------------------------------------------------------------------------------------------------
-// e [6] of one pair; M = R_i R_j^T and t_rel (needed by e); with JAC also J_l^-1(phi)
+// e [6] of one pair; M = R_i R_j^T and t_rel (needed by e); with JAC also J_l^-1(phi) and JM = J_l^-1(phi) M
 template <class S, bool JAC>
 __device__ __forceinline__ void pair_residual(const S* __restrict__ ci, const S* __restrict__ cj, const S* __restrict__ mean,
-                                              S* e, S* M, S* tr, S* Jinv) {
+                                              S* e, S* M, S* tr, S* Jinv, S* JM) {
   S Ri[9], Rj[9];
   quat_to_rot(ci, Ri);
   quat_to_rot(cj, Rj);
@@ -3085,8 +3101,70 @@ __device__ __forceinline__ void pair_residual(const S* __restrict__ ci, const S*
   const S y = a3 * b1 + a1 * b3 + a2 * b0 - a0 * b2;
   const S z = a3 * b2 + a2 * b3 + a0 * b1 - a1 * b0;
   so3_log_rel(x, y, z, w, mean, e + 3);
-  if (JAC) so3_jl_inv(e + 3, Jinv);
+  if (JAC) {
+    so3_jl_inv(e + 3, Jinv);
+#pragma unroll
+    for (int a = 0; a < 3; ++a)
+#pragma unroll
+      for (int b = 0; b < 3; ++b) JM[3 * a + b] = Jinv[3 * a] * M[b] + Jinv[3 * a + 1] * M[3 + b] + Jinv[3 * a + 2] * M[6 + b];
+  }
 }
+
+// rows of A_i = L de/d(inc_i) and A_j = L de/d(inc_j) for the row l [6] of L:
+//   A_i row (l_t, l_t (-[t_rel]x) + l_r J_l^-1),  A_j row (-l_t M, -l_r J_l^-1 M)
+template <class S>
+__device__ __forceinline__ void pair_jac_rows(const S* l, const S* M, const S* tr, const S* Jinv, const S* JM, S* ri, S* rj) {
+#pragma unroll
+  for (int j = 0; j < 3; ++j) ri[j] = l[j];
+  ri[3] = -l[1] * tr[2] + l[2] * tr[1] + l[3] * Jinv[0] + l[4] * Jinv[3] + l[5] * Jinv[6];
+  ri[4] = l[0] * tr[2] - l[2] * tr[0] + l[3] * Jinv[1] + l[4] * Jinv[4] + l[5] * Jinv[7];
+  ri[5] = -l[0] * tr[1] + l[1] * tr[0] + l[3] * Jinv[2] + l[4] * Jinv[5] + l[5] * Jinv[8];
+#pragma unroll
+  for (int j = 0; j < 3; ++j) {
+    rj[j] = -(l[0] * M[j] + l[1] * M[3 + j] + l[2] * M[6 + j]);
+    rj[3 + j] = -(l[3] * JM[j] + l[4] * JM[3 + j] + l[5] * JM[6 + j]);
+  }
+}
+
+// the pair priors' terms of k_prior_cost and k_prior_ldiff (A d = A_i d_i + A_j d_j)
+template <class S>
+struct PairPrior {
+  using Scalar = S;
+  const S* cams;
+  const int* pairs;  // [m][2]
+  const S* mean;     // [m][7]
+  const S* L;        // [m][36]
+  const S* A;        // [m][2][36]
+  const S* r;        // [m][6]
+  __device__ S sq_norm(int p) const {
+    S e[6], M[9], tr[3];
+    pair_residual<S, false>(cams + 10 * (size_t)pairs[2 * p], cams + 10 * (size_t)pairs[2 * p + 1], mean + 7 * (size_t)p, e, M, tr,
+                            nullptr, nullptr);
+    const S* Lp = L + 36 * (size_t)p;
+    S c2 = 0;
+    for (int i = 0; i < 6; ++i) {
+      S ri = 0;
+#pragma unroll
+      for (int k = 0; k < 6; ++k) ri += Lp[6 * i + k] * e[k];
+      c2 += ri * ri;
+    }
+    return c2;
+  }
+  __device__ S model_change(const S* inc, int p) const {
+    S di[6], dj[6];
+#pragma unroll
+    for (int j = 0; j < 6; ++j) { di[j] = inc[9 * (size_t)pairs[2 * p] + j]; dj[j] = inc[9 * (size_t)pairs[2 * p + 1] + j]; }
+    const S* Ai = A + 72 * (size_t)p;
+    S lp = 0;
+    for (int i = 0; i < 6; ++i) {
+      S u = 0;
+#pragma unroll
+      for (int j = 0; j < 6; ++j) u += Ai[6 * i + j] * di[j] + Ai[36 + 6 * i + j] * dj[j];
+      lp += u * (S(0.5) * u + r[6 * (size_t)p + i]);
+    }
+    return lp;
+  }
+};
 
 // once per linearisation, after the cross-shard sum of diag2 (and the absolute priors) and before k_scaling: the unscaled
 // pose blocks A_i = L de/d(inc_i), A_j = L de/d(inc_j) and r = L e.  Thread per pair; identical on every shard.
@@ -3096,11 +3174,7 @@ __global__ void k_pair_linearize(const S* __restrict__ cams, const int* __restri
   const int p = blockIdx.x * blockDim.x + threadIdx.x;
   if (p >= m) return;
   S e[6], M[9], tr[3], Jinv[9], JM[9];
-  pair_residual<S, true>(cams + 10 * (size_t)pairs[2 * p], cams + 10 * (size_t)pairs[2 * p + 1], mean + 7 * (size_t)p, e, M, tr, Jinv);
-#pragma unroll
-  for (int a = 0; a < 3; ++a)
-#pragma unroll
-    for (int b = 0; b < 3; ++b) JM[3 * a + b] = Jinv[3 * a] * M[b] + Jinv[3 * a + 1] * M[3 + b] + Jinv[3 * a + 2] * M[6 + b];
+  pair_residual<S, true>(cams + 10 * (size_t)pairs[2 * p], cams + 10 * (size_t)pairs[2 * p + 1], mean + 7 * (size_t)p, e, M, tr, Jinv, JM);
   const S* Lp = Lsq + 36 * (size_t)p;
   S* Ai = A + 72 * (size_t)p;
   S* Aj = Ai + 36;
@@ -3112,17 +3186,7 @@ __global__ void k_pair_linearize(const S* __restrict__ cams, const int* __restri
 #pragma unroll
     for (int k = 0; k < 6; ++k) ri += l[k] * e[k];
     pr[6 * (size_t)p + i] = ri;
-    // A_i row: (l_t, l_t (-[t_rel]x) + l_r J_l^-1);  A_j row: (-l_t M, -l_r J_l^-1 M)
-#pragma unroll
-    for (int j = 0; j < 3; ++j) Ai[6 * i + j] = l[j];
-    Ai[6 * i + 3] = -l[1] * tr[2] + l[2] * tr[1] + l[3] * Jinv[0] + l[4] * Jinv[3] + l[5] * Jinv[6];
-    Ai[6 * i + 4] = l[0] * tr[2] - l[2] * tr[0] + l[3] * Jinv[1] + l[4] * Jinv[4] + l[5] * Jinv[7];
-    Ai[6 * i + 5] = -l[0] * tr[1] + l[1] * tr[0] + l[3] * Jinv[2] + l[4] * Jinv[5] + l[5] * Jinv[8];
-#pragma unroll
-    for (int j = 0; j < 3; ++j) {
-      Aj[6 * i + j] = -(l[0] * M[j] + l[1] * M[3 + j] + l[2] * M[6 + j]);
-      Aj[6 * i + 3 + j] = -(l[3] * JM[j] + l[4] * JM[3 + j] + l[5] * JM[6 + j]);
-    }
+    pair_jac_rows(l, M, tr, Jinv, JM, Ai + 6 * i, Aj + 6 * i);
   }
 }
 
@@ -3217,56 +3281,6 @@ __global__ void __launch_bounds__(256) k_pair_ov(DevPtrs<S> D, const PcgState* s
   if (*reinterpret_cast<const volatile int*>(&st->done)) return;
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < 9 * D.nc; e += gridDim.x * blockDim.x) D.pair_ov[e] = pair_ov_entry(D, v, e);
-}
-
-// pair-prior cost sum_p 1/2 |L_p e_p|^2 at the current cameras, added like k_prior_cost.  One block.
-template <class S>
-__global__ void k_pair_cost(const S* __restrict__ cams, const int* __restrict__ pairs, const S* __restrict__ mean,
-                            const S* __restrict__ Lsq, int m, double* red, int* bad_flag) {
-  double acc = 0;
-  for (int p = threadIdx.x; p < m; p += blockDim.x) {
-    S e[6], M[9], tr[3];
-    pair_residual<S, false>(cams + 10 * (size_t)pairs[2 * p], cams + 10 * (size_t)pairs[2 * p + 1], mean + 7 * (size_t)p, e, M, tr, nullptr);
-    const S* Lp = Lsq + 36 * (size_t)p;
-    S c2 = 0;
-    for (int i = 0; i < 6; ++i) {
-      S ri = 0;
-#pragma unroll
-      for (int k = 0; k < 6; ++k) ri += Lp[6 * i + k] * e[k];
-      c2 += ri * ri;
-    }
-    acc += 0.5 * (double)c2;
-  }
-  const double s = prior_block_sum(acc);
-  if (threadIdx.x == 0) {
-    red[1] += s;
-    red[4] += s;
-    if (!isfinite(s)) *bad_flag = 1;
-  }
-}
-
-// pair part of the model cost change: l_diff -= sum_p (A d)^T (1/2 A d + r), A d = A_i d_i + A_j d_j for the (masked,
-// scaled) increment d, added to red[0] like k_prior_ldiff.  One block.
-template <class S>
-__global__ void k_pair_ldiff(const S* __restrict__ A, const S* __restrict__ pr, const int* __restrict__ pairs,
-                             const S* __restrict__ inc, int m, double* red) {
-  double acc = 0;
-  for (int p = threadIdx.x; p < m; p += blockDim.x) {
-    S di[6], dj[6];
-#pragma unroll
-    for (int j = 0; j < 6; ++j) { di[j] = inc[9 * (size_t)pairs[2 * p] + j]; dj[j] = inc[9 * (size_t)pairs[2 * p + 1] + j]; }
-    const S* Ai = A + 72 * (size_t)p;
-    S lp = 0;
-    for (int i = 0; i < 6; ++i) {
-      S u = 0;
-#pragma unroll
-      for (int j = 0; j < 6; ++j) u += Ai[6 * i + j] * di[j] + Ai[36 + 6 * i + j] * dj[j];
-      lp += u * (S(0.5) * u + pr[6 * (size_t)p + i]);
-    }
-    acc -= (double)lp;
-  }
-  const double s = prior_block_sum(acc);
-  if (threadIdx.x == 0) red[0] += s;
 }
 
 }  // namespace rba

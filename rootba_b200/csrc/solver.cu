@@ -696,51 +696,69 @@ struct Solver : rba_handle {
       mean.assign(m, m + (size_t)10 * nc);
       Lsq.assign(Ls, Ls + (size_t)81 * nc);
       for (int c = 0; c < nc; ++c) {
-        for (int k = 0; k < 10; ++k)
-          if (!std::isfinite((double)mean[10 * (size_t)c + k])) {
-            g_err = "rba_set_camera_prior: camera " + std::to_string(c) + " has a non-finite mean";
-            return RBA_ERR_INVALID_ARGUMENT;
-          }
-        for (int k = 0; k < 81; ++k) {
-          const double v = (double)Lsq[81 * (size_t)c + k];
-          if (!std::isfinite(v)) {
-            g_err = "rba_set_camera_prior: camera " + std::to_string(c) + " has a non-finite sqrt_info";
-            return RBA_ERR_INVALID_ARGUMENT;
-          }
-          any = any || v != 0.0;
-        }
-        double q[4], n2 = 0;
-        for (int k = 0; k < 4; ++k) { q[k] = (double)mean[10 * (size_t)c + k]; n2 += q[k] * q[k]; }
-        const double n = std::sqrt(n2);
-        if (!(std::fabs(n - 1.0) <= 1e-3)) {
-          g_err = "rba_set_camera_prior: camera " + std::to_string(c) + " has a mean quaternion of norm " + std::to_string(n) + " (must be within 1e-3 of 1)";
+        bool nonzero;
+        const std::string why = check_prior(m + 10 * (size_t)c, 10, Ls + 81 * (size_t)c, 81, nonzero, mean.data() + 10 * (size_t)c);
+        if (!why.empty()) {
+          g_err = "rba_set_camera_prior: camera " + std::to_string(c) + " " + why;
           return RBA_ERR_INVALID_ARGUMENT;
         }
-        for (int k = 0; k < 4; ++k) mean[10 * (size_t)c + k] = (S)(q[k] / n);
+        any = any || nonzero;
       }
     }
     if (any) {
-      if (!d_prior_mean) {
-        TRY(dalloc(&d_prior_mean, (size_t)10 * nc, false));
-        TRY(dalloc(&d_prior_L, (size_t)81 * nc, false));
-        TRY(dalloc(&d_prior_A, (size_t)81 * nc, false));
-        TRY(dalloc(&d_prior_r, (size_t)9 * nc, false));
-      }
+      TRY(grow_upload(!d_prior_mean, dbuf(d_prior_mean, (size_t)10 * nc, &mean), dbuf(d_prior_L, (size_t)81 * nc, &Lsq),
+                      dbuf(d_prior_A, (size_t)81 * nc), dbuf(d_prior_r, (size_t)9 * nc)));
       TRY(alloc_prior_diag());
-      CU(cudaMemcpyAsync(d_prior_mean, mean.data(), mean.size() * sizeof(S), cudaMemcpyHostToDevice, stream));
-      CU(cudaMemcpyAsync(d_prior_L, Lsq.data(), Lsq.size() * sizeof(S), cudaMemcpyHostToDevice, stream));
       CU(cudaStreamSynchronize(stream));
     }
     has_abs_prior = any;
     return priors_changed();
   }
-  int alloc_prior_diag() {
-    if (!d_prior_H) {
-      TRY(dalloc(&d_prior_H, (size_t)81 * nc, false));
-      TRY(dalloc(&d_prior_g, (size_t)9 * nc, false));
+  // The checks of every prior setter on one prior, in this order: a finite mean (nm entries), a finite sqrt_info (nL
+  // entries) and, for the two camera kinds (q given), a mean quaternion within 1e-3 of unit norm, written normalised to q.
+  // Returns why the prior is rejected ("" = accepted); nonzero = L has a non-zero entry.
+  static std::string check_prior(const S* m, int nm, const S* Ls, int nL, bool& nonzero, S* q = nullptr) {
+    nonzero = false;
+    for (int k = 0; k < nm; ++k)
+      if (!std::isfinite((double)m[k])) return "has a non-finite mean";
+    for (int k = 0; k < nL; ++k) {
+      const double v = (double)Ls[k];
+      if (!std::isfinite(v)) return "has a non-finite sqrt_info";
+      nonzero = nonzero || v != 0.0;
     }
+    if (q) {
+      double n2 = 0;
+      for (int k = 0; k < 4; ++k) n2 += (double)m[k] * (double)m[k];
+      const double n = std::sqrt(n2);
+      if (!(std::fabs(n - 1.0) <= 1e-3)) return "has a mean quaternion of norm " + std::to_string(n) + " (must be within 1e-3 of 1)";
+      for (int k = 0; k < 4; ++k) q[k] = (S)((double)m[k] / n);
+    }
+    return "";
+  }
+  // One device buffer of a group: its entries when (re)allocated and, for an input, the host data copied into it.
+  template <class T>
+  struct DevBuf { T*& p; size_t count; const std::vector<T>* src; };
+  template <class T>
+  static DevBuf<T> dbuf(T*& p, size_t count, const std::vector<T>* src = nullptr) { return {p, count, src}; }
+  // Reallocates every buffer of the group when `grow` (contents not kept), then queues the copies of the inputs on the stream.
+  template <class... T>
+  int grow_upload(bool grow, DevBuf<T>... b) {
+    int rc = RBA_OK;
+    if (grow) {
+      ((rc = rc ? rc : dfree(b.p)), ...);
+      ((rc = rc ? rc : dalloc(&b.p, b.count, false)), ...);
+    }
+    ((rc = rc ? rc : copy_in(b.p, b.src)), ...);
+    return rc;
+  }
+  template <class T>
+  int copy_in(T* dst, const std::vector<T>* src) {
+    if (src) CU(cudaMemcpyAsync(dst, src->data(), src->size() * sizeof(T), cudaMemcpyHostToDevice, stream));
     return RBA_OK;
   }
+  int alloc_prior_diag() { return grow_upload(!d_prior_H, dbuf(d_prior_H, (size_t)81 * nc), dbuf(d_prior_g, (size_t)9 * nc)); }
+  CameraPrior<S> camera_prior() const { return {D.cams, d_prior_mean, d_prior_L, d_prior_A, d_prior_r}; }
+  PairPrior<S> pair_prior() const { return {D.cams, d_pair_ij, d_pair_mean, d_pair_L, d_pair_A, d_pair_r}; }
   int priors_changed() {
     D.prior_H = (has_abs_prior || n_pairs > 0) ? d_prior_H : nullptr;
     D.pair_ov = n_pairs > 0 ? d_pair_ov : nullptr;
@@ -766,22 +784,14 @@ struct Solver : rba_handle {
       const std::string tag = "pair " + std::to_string(p);
       if (i < 0 || i >= nc || j < 0 || j >= nc) return bad(tag + " has a camera index outside [0, " + std::to_string(nc) + ")");
       if (i == j) return bad(tag + " joins camera " + std::to_string(i) + " to itself");
-      bool nonzero = false;
-      for (int k = 0; k < 7; ++k)
-        if (!std::isfinite((double)m[7 * (size_t)p + k])) return bad(tag + " has a non-finite mean");
-      for (int k = 0; k < 36; ++k) {
-        const double v = (double)Ls[36 * (size_t)p + k];
-        if (!std::isfinite(v)) return bad(tag + " has a non-finite sqrt_info");
-        nonzero = nonzero || v != 0.0;
-      }
-      double q[4], n2 = 0;
-      for (int k = 0; k < 4; ++k) { q[k] = (double)m[7 * (size_t)p + k]; n2 += q[k] * q[k]; }
-      const double n = std::sqrt(n2);
-      if (!(std::fabs(n - 1.0) <= 1e-3)) return bad(tag + " has a mean quaternion of norm " + std::to_string(n) + " (must be within 1e-3 of 1)");
+      bool nonzero;
+      S q[4];
+      const std::string why = check_prior(m + 7 * (size_t)p, 7, Ls + 36 * (size_t)p, 36, nonzero, q);
+      if (!why.empty()) return bad(tag + " " + why);
       if (!nonzero) continue;
       ij.push_back(i); ij.push_back(j);
-      for (int k = 0; k < 4; ++k) mean.push_back((S)(q[k] / n));
-      for (int k = 4; k < 7; ++k) mean.push_back(m[7 * (size_t)p + k]);
+      mean.insert(mean.end(), q, q + 4);
+      mean.insert(mean.end(), m + 7 * (size_t)p + 4, m + 7 * (size_t)(p + 1));
       Lsq.insert(Lsq.end(), Ls + 36 * (size_t)p, Ls + 36 * (size_t)(p + 1));
     }
     const int np = (int)(ij.size() / 2);
@@ -796,31 +806,12 @@ struct Solver : rba_handle {
         item[q] = k;            // 2 p + side
         nbr[q] = ij[k ^ 1];
       }
-      if (np > pair_cap) {
-        for (void* q : {(void*)d_pair_ij, (void*)d_pair_mean, (void*)d_pair_L, (void*)d_pair_A, (void*)d_pair_r, (void*)d_pair_item,
-                        (void*)d_pair_nbr, (void*)d_pair_O})
-          TRY(dfree(q));
-        TRY(dalloc(&d_pair_ij, 2 * (size_t)np, false));
-        TRY(dalloc(&d_pair_mean, 7 * (size_t)np, false));
-        TRY(dalloc(&d_pair_L, 36 * (size_t)np, false));
-        TRY(dalloc(&d_pair_A, 72 * (size_t)np, false));
-        TRY(dalloc(&d_pair_r, 6 * (size_t)np, false));
-        TRY(dalloc(&d_pair_item, 2 * (size_t)np, false));
-        TRY(dalloc(&d_pair_nbr, 2 * (size_t)np, false));
-        TRY(dalloc(&d_pair_O, 72 * (size_t)np, false));
-        pair_cap = np;
-      }
-      if (!d_pair_ptr) {
-        TRY(dalloc(&d_pair_ptr, (size_t)nc + 1, false));
-        TRY(dalloc(&d_pair_ov, 9 * (size_t)nc, false));
-      }
+      TRY(grow_upload(np > pair_cap, dbuf(d_pair_ij, 2 * (size_t)np, &ij), dbuf(d_pair_mean, 7 * (size_t)np, &mean),
+                      dbuf(d_pair_L, 36 * (size_t)np, &Lsq), dbuf(d_pair_A, 72 * (size_t)np), dbuf(d_pair_r, 6 * (size_t)np),
+                      dbuf(d_pair_item, 2 * (size_t)np, &item), dbuf(d_pair_nbr, 2 * (size_t)np, &nbr), dbuf(d_pair_O, 72 * (size_t)np)));
+      pair_cap = std::max(pair_cap, np);
+      TRY(grow_upload(!d_pair_ptr, dbuf(d_pair_ptr, (size_t)nc + 1, &ptr), dbuf(d_pair_ov, 9 * (size_t)nc)));
       TRY(alloc_prior_diag());
-      CU(cudaMemcpyAsync(d_pair_ij, ij.data(), ij.size() * sizeof(int), cudaMemcpyHostToDevice, stream));
-      CU(cudaMemcpyAsync(d_pair_mean, mean.data(), mean.size() * sizeof(S), cudaMemcpyHostToDevice, stream));
-      CU(cudaMemcpyAsync(d_pair_L, Lsq.data(), Lsq.size() * sizeof(S), cudaMemcpyHostToDevice, stream));
-      CU(cudaMemcpyAsync(d_pair_item, item.data(), item.size() * sizeof(int), cudaMemcpyHostToDevice, stream));
-      CU(cudaMemcpyAsync(d_pair_nbr, nbr.data(), nbr.size() * sizeof(int), cudaMemcpyHostToDevice, stream));
-      CU(cudaMemcpyAsync(d_pair_ptr, ptr.data(), ptr.size() * sizeof(int), cudaMemcpyHostToDevice, stream));
       CU(cudaStreamSynchronize(stream));
     }
     n_pairs = np;
@@ -849,14 +840,9 @@ struct Solver : rba_handle {
       if (l < 0 || l >= nl_total) return bad(tag + " has a landmark index outside [0, " + std::to_string(nl_total) + ")");
       if (seen[l]) return bad(tag + " repeats landmark " + std::to_string(l));
       seen[l] = 1;
-      bool nonzero = false;
-      for (int k = 0; k < 3; ++k)
-        if (!std::isfinite((double)m[3 * (size_t)p + k])) return bad(tag + " has a non-finite mean");
-      for (int k = 0; k < 9; ++k) {
-        const double v = (double)Ls[9 * (size_t)p + k];
-        if (!std::isfinite(v)) return bad(tag + " has a non-finite sqrt_info");
-        nonzero = nonzero || v != 0.0;
-      }
+      bool nonzero;
+      const std::string why = check_prior(m + 3 * (size_t)p, 3, Ls + 9 * (size_t)p, 9, nonzero);
+      if (!why.empty()) return bad(tag + " " + why);
       if (!nonzero || l < L.lm_begin || l >= L.lm_end) continue;
       const int q = (int)lm.size();
       lm.push_back(l - L.lm_begin);
@@ -867,23 +853,10 @@ struct Solver : rba_handle {
     }
     const int np = (int)lm.size();
     if (np > 0) {
-      if (np > lmp_cap) {
-        for (void* q : {(void*)d_lmp_lm, (void*)d_lmp_mean, (void*)d_lmp_L, (void*)d_lmp_Lg}) TRY(dfree(q));
-        TRY(dalloc(&d_lmp_lm, (size_t)np, false));
-        TRY(dalloc(&d_lmp_mean, 3 * (size_t)np, false));
-        TRY(dalloc(&d_lmp_L, 9 * (size_t)np, false));
-        TRY(dalloc(&d_lmp_Lg, 12 * (size_t)np, false));
-        lmp_cap = np;
-      }
-      if (!d_lmp_slot) {
-        TRY(dalloc(&d_lmp_slot, slot.size(), false));
-        TRY(dalloc(&d_lmp_of_lm, of_lm.size(), false));
-      }
-      CU(cudaMemcpyAsync(d_lmp_slot, slot.data(), slot.size() * sizeof(int), cudaMemcpyHostToDevice, stream));
-      CU(cudaMemcpyAsync(d_lmp_of_lm, of_lm.data(), of_lm.size() * sizeof(int), cudaMemcpyHostToDevice, stream));
-      CU(cudaMemcpyAsync(d_lmp_lm, lm.data(), lm.size() * sizeof(int), cudaMemcpyHostToDevice, stream));
-      CU(cudaMemcpyAsync(d_lmp_mean, mean.data(), mean.size() * sizeof(S), cudaMemcpyHostToDevice, stream));
-      CU(cudaMemcpyAsync(d_lmp_L, Lsq.data(), Lsq.size() * sizeof(S), cudaMemcpyHostToDevice, stream));
+      TRY(grow_upload(np > lmp_cap, dbuf(d_lmp_lm, (size_t)np, &lm), dbuf(d_lmp_mean, 3 * (size_t)np, &mean),
+                      dbuf(d_lmp_L, 9 * (size_t)np, &Lsq), dbuf(d_lmp_Lg, 12 * (size_t)np)));
+      lmp_cap = std::max(lmp_cap, np);
+      TRY(grow_upload(!d_lmp_slot, dbuf(d_lmp_slot, slot.size(), &slot), dbuf(d_lmp_of_lm, of_lm.size(), &of_lm)));
       CU(cudaStreamSynchronize(stream));
     }
     n_lmp = np;
@@ -939,16 +912,16 @@ struct Solver : rba_handle {
     k_sum_partials<6><<<1, 256, 0, stream>>>(d_epart, EBLOCKS, d_red);
     launches += 2;
     if (n_lmp > 0) {  // + this shard's landmark priors' 1/2 |L e|^2, BEFORE the sum over the shards (landmark-owned)
-      k_lm_prior_cost<S><<<1, 256, 0, stream>>>(D.lms, d_lmp_lm, d_lmp_mean, d_lmp_L, n_lmp, d_red, d_flags);
+      k_prior_cost<<<1, 256, 0, stream>>>(LandmarkPrior<S>{D.lms, d_lmp_lm, d_lmp_mean, d_lmp_L}, n_lmp, d_red, d_flags);
       ++launches;
     }
     rc = allreduce_scalars(6); if (rc) return rc;
     if (has_abs_prior) {  // + sum of 1/2 |L e|^2, once, after the sum over the shards
-      k_prior_cost<S><<<1, 256, 0, stream>>>(D.cams, d_prior_mean, d_prior_L, nc, d_red, d_flags);
+      k_prior_cost<<<1, 256, 0, stream>>>(camera_prior(), nc, d_red, d_flags);
       ++launches;
     }
     if (n_pairs > 0) {  // + the pair priors' 1/2 |L e|^2, likewise
-      k_pair_cost<S><<<1, 256, 0, stream>>>(D.cams, d_pair_ij, d_pair_mean, d_pair_L, n_pairs, d_red, d_flags);
+      k_prior_cost<<<1, 256, 0, stream>>>(pair_prior(), n_pairs, d_red, d_flags);
       ++launches;
     }
     CU(cudaMemcpyAsync(h_res->error, d_red, sizeof(h_res->error), cudaMemcpyDeviceToHost, stream));
@@ -1364,11 +1337,11 @@ struct Solver : rba_handle {
     launches += 2;
     rc = allreduce_scalars(1); if (rc) return rc;
     if (has_abs_prior) {  // the prior part of the model cost change, once, after the sum over the shards
-      k_prior_ldiff<S><<<1, 256, 0, stream>>>(d_prior_A, d_prior_r, D.inc, nc, d_red);
+      k_prior_ldiff<<<1, 256, 0, stream>>>(camera_prior(), D.inc, nc, d_red);
       ++launches;
     }
     if (n_pairs > 0) {  // the pair priors' part, likewise
-      k_pair_ldiff<S><<<1, 256, 0, stream>>>(d_pair_A, d_pair_r, d_pair_ij, D.inc, n_pairs, d_red);
+      k_prior_ldiff<<<1, 256, 0, stream>>>(pair_prior(), D.inc, n_pairs, d_red);
       ++launches;
     }
     rc = stop(ev_backsub); if (rc) return rc;

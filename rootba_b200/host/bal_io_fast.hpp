@@ -128,9 +128,26 @@ struct FileBuffer {
 
 }  // namespace detail
 
+// Held cameras and priors of a problem (not in the reference), forwarded by LinearizorQR::create; an empty field = none.
+// Both problem classes (BalProblemSoA, BalProblem) carry them.
+struct ProblemPriors {
+  std::vector<uint8_t> camera_fixed;               // [nc] RBA_FIX_* bits (rba_set_camera_fixed)
+  // Gaussian camera priors (rba_set_camera_prior)
+  std::vector<double> camera_prior_mean;           // [nc][10] qx,qy,qz,qw (R0), camera centre c0, f0, k1_0, k2_0
+  std::vector<double> camera_prior_sqrt_info;      // [nc][81] row-major square-root information L
+  // Relative pose priors between pairs of cameras (rba_set_camera_pair_prior)
+  std::vector<int32_t> camera_pair_prior_pairs;    // [m][2] cameras (i, j)
+  std::vector<double> camera_pair_prior_mean;      // [m][7] qx,qy,qz,qw (R0), t0 of T_i T_j^-1
+  std::vector<double> camera_pair_prior_sqrt_info; // [m][36] row-major square-root information L
+  // Gaussian priors on landmark positions (rba_set_landmark_prior)
+  std::vector<int32_t> landmark_prior_idx;         // [m] landmark indices
+  std::vector<double> landmark_prior_mean;         // [m][3] prior position x0
+  std::vector<double> landmark_prior_sqrt_info;    // [m][9] row-major square-root information L
+};
+
 // Flat mirror of rootba::BalProblem<Scalar> with the member surface LinearizorQR / bundle_adjust_manual need.
 template <typename Scalar>
-class BalProblemSoA {
+class BalProblemSoA : public ProblemPriors {
  public:
   static constexpr int CAM_STATE_SIZE = 10;  // bal_problem.hpp:72
 
@@ -140,18 +157,6 @@ class BalProblemSoA {
   std::vector<int64_t> lm_off;    // [nl + 1]
   std::vector<int32_t> obs_cam;   // ascending inside a landmark
   std::vector<Scalar> obs_xy;     // [nobs][2]
-  std::vector<uint8_t> camera_fixed;  // [nc] RBA_FIX_* bits (rba_set_camera_fixed), forwarded by LinearizorQR::create; empty = all free
-  // Gaussian camera priors (rba_set_camera_prior), forwarded by LinearizorQR::create; empty = no priors.
-  std::vector<double> camera_prior_mean;       // [nc][10] qx,qy,qz,qw, centre, f, k1, k2
-  std::vector<double> camera_prior_sqrt_info;  // [nc][81] row-major L
-  // Relative pose priors between pairs of cameras (rba_set_camera_pair_prior), forwarded by LinearizorQR::create; empty = none.
-  std::vector<int32_t> camera_pair_prior_pairs;    // [m][2] (i, j)
-  std::vector<double> camera_pair_prior_mean;      // [m][7] qx,qy,qz,qw, t0
-  std::vector<double> camera_pair_prior_sqrt_info; // [m][36] row-major L
-  // Gaussian priors on landmark positions (rba_set_landmark_prior), forwarded by LinearizorQR::create; empty = none.
-  std::vector<int32_t> landmark_prior_idx;         // [m]
-  std::vector<double> landmark_prior_mean;         // [m][3] x0
-  std::vector<double> landmark_prior_sqrt_info;    // [m][9] row-major L
 
   int num_cameras() const { return nc; }
   int num_landmarks() const { return nl; }

@@ -19,7 +19,7 @@
 namespace rootba_b200 {
 
 template <typename Scalar>
-class BalProblem {
+class BalProblem : public ProblemPriors {
  public:
   static constexpr int CAM_STATE_SIZE = 10;  // bal_problem.hpp:72
   using FrameIdx = int;                      // common_types.hpp:44-45
@@ -219,23 +219,6 @@ class BalProblem {
     for (size_t i = 0; i < cameras_.size(); ++i) std::copy(cams.begin() + CAM_STATE_SIZE * i, cams.begin() + CAM_STATE_SIZE * (i + 1), cameras_[i].params.begin());
     for (size_t i = 0; i < landmarks_.size(); ++i) std::copy(lms.begin() + 3 * i, lms.begin() + 3 * (i + 1), landmarks_[i].p_w.begin());
   }
-
-  // RBA_FIX_* bits per camera (rba_set_camera_fixed), forwarded by LinearizorQR::create; empty = every parameter free.
-  // Not in the reference.
-  std::vector<uint8_t> camera_fixed;
-  // Gaussian camera priors (rba_set_camera_prior), forwarded by LinearizorQR::create; empty = no priors.  Not in the reference.
-  std::vector<double> camera_prior_mean;       // [nc][10] qx,qy,qz,qw (R0), camera centre c0, f0, k1_0, k2_0
-  std::vector<double> camera_prior_sqrt_info;  // [nc][81] row-major square-root information L
-  // Relative pose priors between pairs of cameras (rba_set_camera_pair_prior), forwarded by LinearizorQR::create; empty = none.
-  // Not in the reference.
-  std::vector<int32_t> camera_pair_prior_pairs;    // [m][2] cameras (i, j)
-  std::vector<double> camera_pair_prior_mean;      // [m][7] qx,qy,qz,qw (R0), t0 of T_i T_j^-1
-  std::vector<double> camera_pair_prior_sqrt_info; // [m][36] row-major square-root information L
-  // Gaussian priors on landmark positions (rba_set_landmark_prior), forwarded by LinearizorQR::create; empty = none.
-  // Not in the reference.
-  std::vector<int32_t> landmark_prior_idx;         // [m] landmark indices
-  std::vector<double> landmark_prior_mean;         // [m][3] prior position x0
-  std::vector<double> landmark_prior_sqrt_info;    // [m][9] row-major square-root information L
 
  private:
   static void fail(FILE* f, const std::string& path) { std::fclose(f); throw std::runtime_error("Failed to parse '" + path + "'"); }

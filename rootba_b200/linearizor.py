@@ -78,23 +78,33 @@ def _camera_fixed_array(flags, num_cameras: int):
     return np.ascontiguousarray(a, dtype=np.uint8).copy()
 
 
+def _prior_arrays(name, mean, sqrt_info, dtype, m, mean_len, dim, check_index=None, item=None):
+    """validated contiguous copies (mean [m, mean_len], sqrt_info [m, dim, dim]) in `dtype` of the priors `name`.  The checks
+    run in this order: the shapes, the kind's own index checks (`check_index`), finiteness and, for a kind whose mean
+    starts with a quaternion (`item` names its entries), the quaternion norm."""
+    mean = np.array(mean, dtype=dtype, order="C", copy=True)
+    sqrt_info = np.array(sqrt_info, dtype=dtype, order="C", copy=True)
+    if mean.shape != (m, mean_len):
+        raise ValueError(f"{name} mean must have shape ({m}, {mean_len}), got {mean.shape}")
+    if sqrt_info.shape != (m, dim, dim):
+        raise ValueError(f"{name} sqrt_info must have shape ({m}, {dim}, {dim}), got {sqrt_info.shape}")
+    if check_index is not None:
+        check_index()
+    if not (np.all(np.isfinite(mean)) and np.all(np.isfinite(sqrt_info))):
+        raise ValueError(f"{name} entries must be finite")
+    if item is not None:
+        qn = np.linalg.norm(mean[:, :4].astype(np.float64), axis=1)
+        if np.any(np.abs(qn - 1.0) > 1e-3):
+            raise ValueError(f"{name} mean quaternions must have norm 1 (within 1e-3); {item} {int(np.argmax(np.abs(qn - 1.0)))} has {qn.max():.6g}")
+    return mean, sqrt_info
+
+
 def _camera_prior_arrays(prior, num_cameras: int, dtype):
     """None, or validated contiguous copies (mean [nc,10], sqrt_info [nc,9,9]) of a camera prior in the problem's dtype"""
     if prior is None:
         return None
     mean, sqrt_info = prior
-    mean = np.array(mean, dtype=dtype, order="C", copy=True)
-    sqrt_info = np.array(sqrt_info, dtype=dtype, order="C", copy=True)
-    if mean.shape != (num_cameras, 10):
-        raise ValueError(f"camera_prior mean must have shape ({num_cameras}, 10), got {mean.shape}")
-    if sqrt_info.shape != (num_cameras, 9, 9):
-        raise ValueError(f"camera_prior sqrt_info must have shape ({num_cameras}, 9, 9), got {sqrt_info.shape}")
-    if not (np.all(np.isfinite(mean)) and np.all(np.isfinite(sqrt_info))):
-        raise ValueError("camera_prior entries must be finite")
-    qn = np.linalg.norm(mean[:, :4].astype(np.float64), axis=1)
-    if np.any(np.abs(qn - 1.0) > 1e-3):
-        raise ValueError(f"camera_prior mean quaternions must have norm 1 (within 1e-3); camera {int(np.argmax(np.abs(qn - 1.0)))} has {qn.max():.6g}")
-    return mean, sqrt_info
+    return _prior_arrays("camera_prior", mean, sqrt_info, dtype, num_cameras, 10, 9, item="camera")
 
 
 def _camera_pair_prior_arrays(prior, num_cameras: int, dtype):
@@ -104,23 +114,14 @@ def _camera_pair_prior_arrays(prior, num_cameras: int, dtype):
         return None
     pairs, mean, sqrt_info = prior
     pairs = np.array(pairs, dtype=np.int32, order="C", copy=True)
-    mean = np.array(mean, dtype=dtype, order="C", copy=True)
-    sqrt_info = np.array(sqrt_info, dtype=dtype, order="C", copy=True)
     m = pairs.shape[0] if pairs.ndim == 2 else -1
     if pairs.shape != (m, 2):
         raise ValueError(f"camera_pair_prior pairs must have shape (m, 2), got {pairs.shape}")
-    if mean.shape != (m, 7):
-        raise ValueError(f"camera_pair_prior mean must have shape ({m}, 7), got {mean.shape}")
-    if sqrt_info.shape != (m, 6, 6):
-        raise ValueError(f"camera_pair_prior sqrt_info must have shape ({m}, 6, 6), got {sqrt_info.shape}")
-    if np.any(pairs < 0) or np.any(pairs >= num_cameras) or np.any(pairs[:, 0] == pairs[:, 1]):
-        raise ValueError(f"camera_pair_prior pairs must join two different cameras in [0, {num_cameras})")
-    if not (np.all(np.isfinite(mean)) and np.all(np.isfinite(sqrt_info))):
-        raise ValueError("camera_pair_prior entries must be finite")
-    qn = np.linalg.norm(mean[:, :4].astype(np.float64), axis=1)
-    if np.any(np.abs(qn - 1.0) > 1e-3):
-        raise ValueError(f"camera_pair_prior mean quaternions must have norm 1 (within 1e-3); pair {int(np.argmax(np.abs(qn - 1.0)))} has {qn.max():.6g}")
-    return pairs, mean, sqrt_info
+
+    def check_index():
+        if np.any(pairs < 0) or np.any(pairs >= num_cameras) or np.any(pairs[:, 0] == pairs[:, 1]):
+            raise ValueError(f"camera_pair_prior pairs must join two different cameras in [0, {num_cameras})")
+    return (pairs, *_prior_arrays("camera_pair_prior", mean, sqrt_info, dtype, m, 7, 6, check_index, item="pair"))
 
 
 def _landmark_prior_arrays(prior, num_landmarks: int, dtype):
@@ -130,22 +131,16 @@ def _landmark_prior_arrays(prior, num_landmarks: int, dtype):
         return None
     idx, mean, sqrt_info = prior
     idx = np.array(idx, dtype=np.int32, order="C", copy=True)
-    mean = np.array(mean, dtype=dtype, order="C", copy=True)
-    sqrt_info = np.array(sqrt_info, dtype=dtype, order="C", copy=True)
     m = idx.shape[0] if idx.ndim == 1 else -1
     if idx.shape != (m,):
         raise ValueError(f"landmark_prior idx must have shape (m,), got {idx.shape}")
-    if mean.shape != (m, 3):
-        raise ValueError(f"landmark_prior mean must have shape ({m}, 3), got {mean.shape}")
-    if sqrt_info.shape != (m, 3, 3):
-        raise ValueError(f"landmark_prior sqrt_info must have shape ({m}, 3, 3), got {sqrt_info.shape}")
-    if np.any(idx < 0) or np.any(idx >= num_landmarks):
-        raise ValueError(f"landmark_prior idx must be landmark indices in [0, {num_landmarks})")
-    if len(np.unique(idx)) != m:
-        raise ValueError("landmark_prior idx must not repeat a landmark")
-    if not (np.all(np.isfinite(mean)) and np.all(np.isfinite(sqrt_info))):
-        raise ValueError("landmark_prior entries must be finite")
-    return idx, mean, sqrt_info
+
+    def check_index():
+        if np.any(idx < 0) or np.any(idx >= num_landmarks):
+            raise ValueError(f"landmark_prior idx must be landmark indices in [0, {num_landmarks})")
+        if len(np.unique(idx)) != m:
+            raise ValueError("landmark_prior idx must not repeat a landmark")
+    return (idx, *_prior_arrays("landmark_prior", mean, sqrt_info, dtype, m, 3, 3, check_index))
 
 
 class BalProblem:
