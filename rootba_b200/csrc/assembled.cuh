@@ -4,10 +4,10 @@
 // co-visible camera pairs) is several times smaller than the panels it is built from.
 //   k_rcs_terms     once per linearisation: S_u = sum over panel rows 0..2n-4 (lambda-independent, the reference's rows
 //   k_rcs_combine   3..2n-1 of the landmark block);  once per solve: S = S_u + sum over the three damping rows that
-//                   k_stage2 has just written (rows 2n-3..2n-1).  The 9 x 9 block of every term (slot_a, slot_b) of a
-//                   landmark is evaluated landmark by landmark into a staging buffer of bounded size, then every co-visible
-//                   camera pair (ca >= cb) adds its terms in the order of the host-built list (pair_terms), range by range:
-//                   no atomics, fixed order.
+//                   k_stage2 has just written (rows 2n-3..2n-1).  The 9 x 9 block of every term (slot_a, slot_b) of every
+//                   landmark is evaluated landmark by landmark into a staging buffer that holds all of them, then every
+//                   co-visible camera pair (ca >= cb) adds its terms in the order of the host-built list
+//                   (build_pair_list, layout.hpp): no atomics, fixed order.
 //   k_rcs_spmv      y = S x over a camera-major block-row CSR of the full matrix (both triangles, diagonal included).
 #pragma once
 
@@ -15,30 +15,21 @@
 
 namespace rba {
 
-// One term (slot_a, slot_b) of a pair, resolved on the host to what the kernel needs to address the panel: base = the tile's
-// panel offset + 2 G g (g = the landmark inside the tile); ij = ia | ib << 16 (observations of slot_a / slot_b inside the landmark);
-// meta = n | log2(G) << 15 | KP << 18.  Column c of the landmark in row r is at base + r KP 64 + 2 ((c/2 >> lg) 32 +
-// (c/2 & (G - 1))) + c % 2 (the tile layout of layout.hpp).
-struct AsmTerm {
-  long long base;
-  int ij, meta;
-};
-
-// Landmark-major evaluation of the terms w0 .. w1 - 1 (the terms of a range of landmarks, landmarks in problem order): warp
-// per three consecutive terms, lane 9 g + p (g = 0..2, p = 0..8; lanes 27..31 idle) computes row p of the 9 x 9 block of
-// term w0 + 3 k + g over the panel rows [0, 2n - 3) (damping = 0: the lambda-independent rows) or [2n - 3, 2n) (damping = 1:
-// the damping rows of the last k_stage2) into stage[81 (w - w0)].  Neighbouring warps read the same landmark's panel, so
-// it is read from HBM about once.  Block entry (p, q) = sum_r P[r][9 ia + p] P[r][9 ib + q]; on the diagonal (sa == sb)
-// it is symmetric bit for bit (fma commutes).
+// Landmark-major evaluation of the nt terms (landmarks in problem order): warp per three consecutive terms, lane 9 g + p
+// (g = 0..2, p = 0..8; lanes 27..31 idle) computes row p of the 9 x 9 block of term 3 k + g over the panel rows
+// [0, 2n - 3) (damping = 0: the lambda-independent rows) or [2n - 3, 2n) (damping = 1: the damping rows of the last
+// k_stage2) into stage[81 w].  Neighbouring warps read the same landmark's panel, so it is read from HBM about once.
+// Block entry (p, q) = sum_r P[r][9 ia + p] P[r][9 ib + q]; on the diagonal (sa == sb) it is symmetric bit for bit (fma
+// commutes).
 template <class S>
-__global__ void __launch_bounds__(256) k_rcs_terms(const S* __restrict__ panel, const AsmTerm* __restrict__ terms, long long w0,
-                                                   long long w1, int damping, S* __restrict__ stage) {
+__global__ void __launch_bounds__(256) k_rcs_terms(const S* __restrict__ panel, const AsmTerm* __restrict__ terms, long long nt,
+                                                   int damping, S* __restrict__ stage) {
   using V2 = typename ST<S>::V2;
   const int lane = threadIdx.x & 31;
   const int g = lane / 9, p = lane - 9 * g;
   if (lane >= 27) return;
   const long long warps = (long long)gridDim.x * (blockDim.x >> 5);
-  for (long long w = w0 + 3 * (blockIdx.x * (long long)(blockDim.x >> 5) + (threadIdx.x >> 5)) + g; w < w1; w += 3 * warps) {
+  for (long long w = 3 * (blockIdx.x * (long long)(blockDim.x >> 5) + (threadIdx.x >> 5)) + g; w < nt; w += 3 * warps) {
     const AsmTerm at = terms[w];
     const int n = at.meta & 0x7fff, lg = (at.meta >> 15) & 7, KP = at.meta >> 18, G = 1 << lg;
     const int ia = at.ij & 0xffff, ib = at.ij >> 16;
@@ -68,40 +59,26 @@ __global__ void __launch_bounds__(256) k_rcs_terms(const S* __restrict__ panel, 
 #pragma unroll
       for (int q = 0; q < 9; ++q) acc[q] = fma(va, odd ? el[q + 1] : el[q], acc[q]);
     }
-    S* o = stage + 81 * (size_t)(w - w0) + 9 * p;
+    S* o = stage + 81 * (size_t)w + 9 * p;
 #pragma unroll
     for (int q = 0; q < 9; ++q) o[q] = acc[q];
   }
 }
 
-// Thread per entry of a pair block (ca >= cb): adds the pair's terms that lie in the staged range [w0, w1), in the pair's
-// list order (landmark order), to the block's running sum.  wpos[t] = landmark-major index of the pair-sorted term t, so
-// the staged terms of a pair are a contiguous run of its list (two binary searches).  The running sum starts, at the first
-// range (first = 1), from `base` (the lambda-independent part) or 0; it lives in out[81 pos.x] (pos == nullptr: out[81 bi],
-// S_u), and off the diagonal its transpose is written to out[81 pos.y] (the full CSR).  The result does not depend on how
-// the terms are cut into ranges.
+// Thread per entry of a pair block (ca >= cb): `base` (the lambda-independent part S_u) or 0, plus the pair's staged terms
+// in the pair's list order (landmark order); wpos[t] = landmark-major index of the pair-sorted term t.  The sum goes to
+// out[81 pos.x] (pos == nullptr: out[81 bi], S_u), and off the diagonal its transpose to out[81 pos.y] (the full CSR).
 template <class S>
-__global__ void k_rcs_combine(const int* __restrict__ blk_ptr, const int* __restrict__ wpos, int nblk, long long w0, long long w1,
-                              const S* __restrict__ stage, const S* __restrict__ base, const int2* __restrict__ pos, int first,
-                              S* __restrict__ out) {
+__global__ void k_rcs_combine(const int* __restrict__ blk_ptr, const int* __restrict__ wpos, int nblk, const S* __restrict__ stage,
+                              const S* __restrict__ base, const int2* __restrict__ pos, S* __restrict__ out) {
   const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
   if (i >= 81LL * nblk) return;
   const int bi = (int)(i / 81), e = (int)(i - 81LL * bi);
-  auto lower = [&](long long w) {
-    int lo = blk_ptr[bi], hi = blk_ptr[bi + 1];
-    while (lo < hi) {
-      const int mid = (lo + hi) >> 1;
-      if (wpos[mid] < w) lo = mid + 1; else hi = mid;
-    }
-    return lo;
-  };
-  const int t0 = lower(w0), t1 = lower(w1);
+  const S* st = stage + e;
+  S s = base ? base[81 * (size_t)bi + e] : S(0);
+  for (int t = blk_ptr[bi]; t < blk_ptr[bi + 1]; ++t) s += st[81 * (size_t)wpos[t]];
   const int2 ps = pos ? pos[bi] : make_int2(bi, -1);
-  S* lo = out + 81 * (size_t)ps.x + e;
-  if (t0 == t1 && !first) return;
-  S s = first ? (base ? base[81 * (size_t)bi + e] : S(0)) : *lo;
-  for (int t = t0; t < t1; ++t) s += stage[81 * (size_t)(wpos[t] - w0) + e];
-  *lo = s;
+  out[81 * (size_t)ps.x + e] = s;
   if (ps.y >= 0) out[81 * (size_t)ps.y + 9 * (e % 9) + e / 9] = s;
 }
 

@@ -1,5 +1,6 @@
-// Host-side data model: landmark sharding, track-length classes, warp tiles, matvec work items and
-// the camera-major CSR used by the deterministic scatter (two-phase reduction).
+// Host-side data model: landmark sharding, track-length classes, warp tiles, matvec work items,
+// the camera-major CSR used by the deterministic scatter (two-phase reduction), the co-visible camera
+// pairs and the structure of the assembled reduced camera matrix.
 //
 // Replaces (reference, relative to src/rootba/):
 //   qr/landmark_block.cpp:51-80      LandmarkBlockFactory: static classes n=2..8 + dynamic
@@ -8,7 +9,9 @@
 #pragma once
 
 #include <algorithm>
+#include <cmath>
 #include <cstdint>
+#include <limits>
 #include <numeric>
 #include <string>
 #include <utility>
@@ -302,6 +305,150 @@ inline std::string build_layout(int nc, int nl, const int64_t* lm_off, const int
     L.k4_scratch_per_warp = std::max(L.k4_scratch_per_warp, T.KP > kp_max ? 2 * 64 * (int)T.KP : W * CS);
   }
   return "";
+}
+
+// Two ints; uploaded as the device's int2 (solver.cu checks that the sizes match).
+struct IntPair {
+  int x, y;
+};
+
+// Co-visible camera pairs, shared by the assembled operator and rba_compute_covariance.  Per landmark its first slot and
+// track length; per co-visible camera pair (ca >= cb), ascending (ca, cb), the terms (slot_a, slot_b) of every landmark
+// that sees both, landmarks in problem order and within a landmark in observation order: the fixed summation order of
+// k_rcs_combine and k_cov_assemble.  wpos[t] = position of term t in the landmark-major enumeration (landmarks in
+// problem order, then a = 0..n-1, b = 0..a), the order of k_rcs_terms.
+struct PairList {
+  std::vector<int> slot0, nn;      // [nl_local]
+  std::vector<IntPair> blk_cam;    // [nblk] (ca, cb)
+  std::vector<int> blk_ptr;        // [nblk + 1] into terms
+  std::vector<IntPair> terms;      // (slot_a, slot_b)
+  std::vector<int> wpos;           // landmark-major position of each term
+};
+
+// Returns "" on success or an error message.
+inline std::string build_pair_list(const Layout& L, PairList& P) {
+  const int nl = L.nl_local, nc = L.nc;
+  P = PairList();
+  P.slot0.resize(nl); P.nn.resize(nl);
+  long long nt = 0;
+  for (int lm = 0; lm < nl; ++lm) {
+    const int sidx = L.sorted_of_lm[lm];
+    const TileInfo& T = L.tiles[L.tile_of_sorted[sidx]];
+    P.slot0[lm] = T.slot_base + (sidx - T.lm_base) * T.n;
+    P.nn[lm] = T.n;
+    nt += (long long)T.n * (T.n + 1) / 2;
+  }
+  if (nt > std::numeric_limits<int>::max()) return "more than 2^31 camera-pair terms";
+  // landmark-major list, then two stable counting sorts of its positions (by cb, then by ca): ascending (ca, cb),
+  // landmark order kept
+  std::vector<IntPair> raw;
+  raw.reserve((size_t)nt);
+  for (int lm = 0; lm < nl; ++lm)
+    for (int a = 0; a < P.nn[lm]; ++a)
+      for (int b = 0; b <= a; ++b) raw.push_back({P.slot0[lm] + a, P.slot0[lm] + b});  // camera(a) >= camera(b)
+  std::vector<int> idx(raw.size()), tmp(raw.size());
+  std::iota(idx.begin(), idx.end(), 0);
+  std::vector<long long> cnt((size_t)nc + 1);
+  auto pass = [&](const std::vector<int>& src, std::vector<int>& dst, bool by_a) {
+    std::fill(cnt.begin(), cnt.end(), 0LL);
+    for (int w : src) ++cnt[L.slot_cam[by_a ? raw[w].x : raw[w].y] + 1];
+    for (int c = 0; c < nc; ++c) cnt[c + 1] += cnt[c];
+    for (int w : src) dst[cnt[L.slot_cam[by_a ? raw[w].x : raw[w].y]]++] = w;
+  };
+  pass(idx, tmp, false);
+  pass(tmp, idx, true);
+  tmp.clear(); tmp.shrink_to_fit();
+  P.terms.resize(raw.size());
+  for (size_t t = 0; t < idx.size(); ++t) P.terms[t] = raw[idx[t]];
+  P.wpos.swap(idx);
+  for (size_t t = 0; t < P.terms.size(); ++t) {
+    const IntPair cc{L.slot_cam[P.terms[t].x], L.slot_cam[P.terms[t].y]};
+    if (t == 0 || cc.x != P.blk_cam.back().x || cc.y != P.blk_cam.back().y) {
+      P.blk_cam.push_back(cc);
+      P.blk_ptr.push_back((int)t);
+    }
+  }
+  P.blk_ptr.push_back((int)P.terms.size());
+  return "";
+}
+
+// One term (slot_a, slot_b) of a pair, resolved on the host to what k_rcs_terms needs to address the panel: base = the
+// tile's panel offset + 2 G g (g = the landmark inside the tile); ij = ia | ib << 16 (observations of slot_a / slot_b inside
+// the landmark); meta = n | log2(G) << 15 | KP << 18.  Column c of the landmark in row r is at base + r KP 64 +
+// 2 ((c/2 >> lg) 32 + (c/2 & (G - 1))) + c % 2 (the tile layout above).  Every field fits for n <= 20000 (build_layout).
+struct AsmTerm {
+  long long base;
+  int ij, meta;
+};
+inline AsmTerm pack_asm_term(long long base, int ia, int ib, int n, int G, int KP) {
+  int lg = 0;
+  while ((1 << lg) < G) ++lg;
+  return {base, ia | ib << 16, n | lg << 15 | KP << 18};
+}
+
+// Staging bound of the assembled operator: every term's 9 x 9 block is staged at once.  Range by range, with the combine
+// searching every pair's terms once per range, the assembly cost more than the panel product saves (DESIGN.md section 11).
+constexpr long long ASM_STAGE_BYTES = (long long)2 << 30;
+
+// PCG iteration at which a solve switches to S: building it costs about twice its staging traffic (stage 1 + stage 2,
+// each written and read once) in units of operator time, and every iteration with S saves the panel bytes minus the bytes
+// of S.
+inline int asm_switch_iteration(long long nt, long long panel_scalars, long long s_bytes, int scalar_size) {
+  const double staged = 4.0 * (double)nt * 81 * scalar_size, saved = (double)panel_scalars * scalar_size - (double)s_bytes;
+  return 1 + (int)std::ceil(2.0 * staged / std::max(saved, 1.0));
+}
+
+// The assembled operator's host-side structure.  `fits`: S is at most a quarter of the panel bytes and all terms stage
+// in one pass; only then are row_ptr, col, pos and terms built.  `device_bytes`: what its device buffers take.
+struct AsmPlan {
+  long long nt = 0, nblk = 0, nnzb = 0, s_bytes = 0, device_bytes = 0;
+  bool fits = false;
+  int switch_iteration = 0;
+  std::vector<int> row_ptr;        // [nc + 1] camera-major block-row CSR of the full S (both triangles, diagonal included)
+  std::vector<int> col;            // [nnzb] ascending in every row
+  std::vector<IntPair> pos;        // [nblk] the pair's lower (ca, cb) and upper (cb, ca) block in the CSR; -1: diagonal
+  std::vector<AsmTerm> terms;      // [nt] landmark-major
+};
+
+inline void plan_assembled(const Layout& L, const PairList& P, int scalar_size, AsmPlan& A) {
+  A = AsmPlan();
+  const int nc = L.nc;
+  A.nblk = (long long)P.blk_cam.size();
+  A.nt = (long long)P.terms.size();
+  long long ndiag = 0;
+  for (const IntPair& c : P.blk_cam) ndiag += c.x == c.y;
+  A.nnzb = 2 * A.nblk - ndiag;
+  A.s_bytes = A.nnzb * 81 * scalar_size;
+  A.switch_iteration = asm_switch_iteration(A.nt, L.panel_scalars, A.s_bytes, scalar_size);
+  A.fits = 4 * A.s_bytes <= L.panel_scalars * scalar_size && 81 * A.nt * scalar_size <= ASM_STAGE_BYTES;
+  if (!A.fits) return;
+  // S, S_u and the staging buffer; the terms and wpos; blk_ptr, row_ptr, col; pos
+  A.device_bytes = A.s_bytes + (A.nblk + A.nt) * 81 * scalar_size + A.nt * (long long)(sizeof(AsmTerm) + sizeof(int)) +
+                   (A.nblk + A.nnzb + nc + 2) * (long long)sizeof(int) + A.nblk * (long long)sizeof(IntPair);
+  // row ca gets (ca, cb) and row cb the transpose; iterating the pairs in (ca, cb) order fills every row in ascending
+  // column order (lower blocks, the diagonal, then upper blocks)
+  A.row_ptr.assign((size_t)nc + 1, 0);
+  A.col.resize((size_t)A.nnzb);
+  for (const IntPair& c : P.blk_cam) { ++A.row_ptr[c.x + 1]; if (c.x != c.y) ++A.row_ptr[c.y + 1]; }
+  for (int c = 0; c < nc; ++c) A.row_ptr[c + 1] += A.row_ptr[c];
+  std::vector<int> fill(A.row_ptr.begin(), A.row_ptr.end() - 1);
+  A.pos.resize((size_t)A.nblk);
+  for (long long b = 0; b < A.nblk; ++b) {
+    const IntPair c = P.blk_cam[b];
+    const int lo = fill[c.x]++;
+    A.col[lo] = c.y;
+    int up = -1;
+    if (c.x != c.y) { up = fill[c.y]++; A.col[up] = c.x; }
+    A.pos[b] = {lo, up};
+  }
+  A.terms.reserve((size_t)A.nt);
+  for (int lm = 0; lm < L.nl_local; ++lm) {
+    const int sidx = L.sorted_of_lm[lm];
+    const TileInfo& T = L.tiles[L.tile_of_sorted[sidx]];
+    const int g = sidx - T.lm_base;
+    for (int a = 0; a < T.n; ++a)
+      for (int b = 0; b <= a; ++b) A.terms.push_back(pack_asm_term(T.panel_off + 2LL * g * T.G, a, b, T.n, T.G, T.KP));
+  }
 }
 
 }  // namespace rba

@@ -24,6 +24,9 @@ namespace rba {
 
 thread_local std::string g_err;
 
+// the host builds the pair lists as IntPair (layout.hpp); the kernels read them as int2
+static_assert(sizeof(IntPair) == sizeof(int2), "IntPair must have the layout of int2");
+
 #define CU(call)                                                                                   \
   do {                                                                                             \
     cudaError_t e__ = (call);                                                                      \
@@ -216,17 +219,16 @@ struct Solver : rba_handle {
   // landmark's first slot and track length, built at the first call
   bool cov_ready = false;
   int cov_nblk = 0;
-  int2* d_cov_blk_cam = nullptr; int* d_cov_blk_ptr = nullptr; int2* d_cov_terms = nullptr;
+  IntPair* d_cov_blk_cam = nullptr; int* d_cov_blk_ptr = nullptr; IntPair* d_cov_terms = nullptr;
   int* d_cov_lm_slot0 = nullptr; int* d_cov_lm_n = nullptr;
   // assembled operator (setup_assembled, assembled.cuh): the terms as panel addresses in landmark-major order, the pair
   // list (term ranges, landmark-major position of every term), per pair its positions (lower, upper or -1) in the full
-  // block-row CSR of S, the landmark ranges staged at a time, the staging buffer, S_u per pair and S
+  // block-row CSR of S, the staging buffer of all terms, S_u per pair and S
   // asm_on: the structure exists; su_valid: S_u belongs to the current linearisation; s_valid: S = S_u + the damping part of
   // the last solve's lambda, and that solve (and rba_right_multiply / rba_time_matvec after it) applies S
   bool asm_on = false, su_valid = false, s_valid = false;
-  int asm_nblk = 0, asm_switch = 0; long long asm_nnzb = 0;
-  std::vector<long long> asm_ranges;
-  AsmTerm* d_asm_terms = nullptr; int* d_asm_wpos = nullptr; int* d_asm_blk_ptr = nullptr; int2* d_asm_pos = nullptr;
+  int asm_nblk = 0, asm_switch = 0; long long asm_nt = 0, asm_nnzb = 0;
+  AsmTerm* d_asm_terms = nullptr; int* d_asm_wpos = nullptr; int* d_asm_blk_ptr = nullptr; IntPair* d_asm_pos = nullptr;
   int* d_asm_row_ptr = nullptr; int* d_asm_col = nullptr;
   S* d_asm_stage = nullptr; S* d_asm_Su = nullptr; S* d_asm_S = nullptr;
 
@@ -1561,152 +1563,42 @@ struct Solver : rba_handle {
   int synchronize() override { CU(cudaStreamSynchronize(stream)); return RBA_OK; }
 
   // ------------------------------------------------------------------------------------------
-  // Co-visible camera pairs, shared by the assembled operator and rba_compute_covariance.  Per landmark its first slot and
-  // track length; per co-visible camera pair (ca >= cb), ascending (ca, cb), the terms (slot_a, slot_b) of every landmark
-  // that sees both, landmarks in problem order and within a landmark in observation order: the fixed summation order of
-  // k_rcs_combine and k_cov_assemble.  wpos[t] = position of term t in the landmark-major enumeration (landmarks in
-  // problem order, then a = 0..n-1, b = 0..a), the order of k_rcs_terms.
-  struct PairTerms {
-    std::vector<int> slot0, nn;      // [nl_local]
-    std::vector<int2> blk_cam;       // [nblk] (ca, cb)
-    std::vector<int> blk_ptr;        // [nblk + 1] into terms
-    std::vector<int2> terms;         // (slot_a, slot_b)
-    std::vector<int> wpos;           // landmark-major position of each term
-  };
-  int pair_terms(PairTerms& P) {
-    const int nl = L.nl_local;
-    P.slot0.resize(nl); P.nn.resize(nl);
-    long long nt = 0;
-    for (int lm = 0; lm < nl; ++lm) {
-      const int sidx = L.sorted_of_lm[lm];
-      const TileInfo& T = L.tiles[L.tile_of_sorted[sidx]];
-      P.slot0[lm] = T.slot_base + (sidx - T.lm_base) * T.n;
-      P.nn[lm] = T.n;
-      nt += (long long)T.n * (T.n + 1) / 2;
-    }
-    if (nt > std::numeric_limits<int>::max()) { g_err = "more than 2^31 camera-pair terms"; return RBA_ERR_UNSUPPORTED; }
-    // landmark-major list, then two stable counting sorts of its positions (by cb, then by ca): ascending (ca, cb),
-    // landmark order kept
-    std::vector<int2> raw;
-    raw.reserve((size_t)nt);
-    for (int lm = 0; lm < nl; ++lm)
-      for (int a = 0; a < P.nn[lm]; ++a)
-        for (int b = 0; b <= a; ++b) raw.push_back(make_int2(P.slot0[lm] + a, P.slot0[lm] + b));  // camera(a) >= camera(b)
-    std::vector<int> idx(raw.size()), tmp(raw.size());
-    std::iota(idx.begin(), idx.end(), 0);
-    std::vector<long long> cnt((size_t)nc + 1);
-    auto pass = [&](const std::vector<int>& src, std::vector<int>& dst, bool by_a) {
-      std::fill(cnt.begin(), cnt.end(), 0LL);
-      for (int w : src) ++cnt[L.slot_cam[by_a ? raw[w].x : raw[w].y] + 1];
-      for (int c = 0; c < nc; ++c) cnt[c + 1] += cnt[c];
-      for (int w : src) dst[cnt[L.slot_cam[by_a ? raw[w].x : raw[w].y]]++] = w;
-    };
-    pass(idx, tmp, false);
-    pass(tmp, idx, true);
-    tmp.clear(); tmp.shrink_to_fit();
-    P.terms.resize(raw.size());
-    for (size_t t = 0; t < idx.size(); ++t) P.terms[t] = raw[idx[t]];
-    P.wpos.swap(idx);
-    P.blk_cam.clear(); P.blk_ptr.clear();
-    for (size_t t = 0; t < P.terms.size(); ++t) {
-      const int2 cc = make_int2(L.slot_cam[P.terms[t].x], L.slot_cam[P.terms[t].y]);
-      if (t == 0 || cc.x != P.blk_cam.back().x || cc.y != P.blk_cam.back().y) {
-        P.blk_cam.push_back(cc);
-        P.blk_ptr.push_back((int)t);
-      }
-    }
-    P.blk_ptr.push_back((int)P.terms.size());
-    return RBA_OK;
-  }
-
-  // The assembled operator (assembled.cuh, DESIGN.md section 4): taken with one GPU and the dense operator when S is at
-  // most a quarter of the panel bytes and its storage fits in the free device memory; else the panel product.  Built here,
-  // once: the terms as panel addresses in landmark-major order, the pair list, the full block-row CSR and the positions of
-  // every pair's blocks in it, and the landmark ranges whose terms fit in the staging buffer (at most 2 GB, or one
-  // landmark's terms if more).
+  // The assembled operator (assembled.cuh, DESIGN.md section 4): taken with one GPU and the dense operator when its
+  // structure passes the size rules (plan_assembled) and its buffers fit in the free device memory; else the panel
+  // product.
   int setup_assembled() {
     if (!asm_hook || opt.nranks != 1 || implicit_op) return RBA_OK;
-    PairTerms P;
-    TRY(pair_terms(P));
-    const long long nblk = (long long)P.blk_cam.size(), nt = (long long)P.terms.size();
-    long long ndiag = 0;
-    for (const int2& c : P.blk_cam) ndiag += c.x == c.y;
-    const long long nnzb = 2 * nblk - ndiag;
-    const size_t s_bytes = (size_t)nnzb * 81 * sizeof(S);
-    if (4 * s_bytes > (size_t)L.panel_scalars * sizeof(S)) return RBA_OK;
-    const long long cap = std::max<long long>(1, ((long long)2 << 30) / (81 * (long long)sizeof(S)));
-    std::vector<long long> ranges{0};
-    long long w = 0, stage_terms = 0;
-    for (int lm = 0; lm < L.nl_local; ++lm) {
-      const long long k = (long long)P.nn[lm] * (P.nn[lm] + 1) / 2;
-      if (w + k - ranges.back() > cap && w > ranges.back()) ranges.push_back(w);
-      w += k;
-      stage_terms = std::max(stage_terms, w - ranges.back());
-    }
-    ranges.push_back(nt);
-    // range by range the combine searches every pair's terms once per range: measured slower than the panel product on
-    // Final-13682 (21 ranges); one range only
-    if (ranges.size() > 2) return RBA_OK;
-    const size_t need = s_bytes + (size_t)(nblk + stage_terms) * 81 * sizeof(S) + (size_t)nt * (sizeof(AsmTerm) + sizeof(int)) +
-                        (size_t)(nblk + nnzb + nc + 2) * sizeof(int) + (size_t)nblk * sizeof(int2);
+    PairList P;
+    const std::string msg = build_pair_list(L, P);
+    if (!msg.empty()) { g_err = msg; return RBA_ERR_UNSUPPORTED; }
+    AsmPlan A;
+    plan_assembled(L, P, sizeof(S), A);
+    if (!A.fits) return RBA_OK;
     size_t free_b = 0, total_b = 0;
     CU(cudaMemGetInfo(&free_b, &total_b));
-    if (need + ((size_t)256 << 20) > free_b) return RBA_OK;  // keep 256 MB for the rest of the handle and the caller
-    // full CSR: row ca gets (ca, cb) and row cb the transpose; iterating the pairs in (ca, cb) order fills every row in
-    // ascending column order (lower blocks, the diagonal, then upper blocks)
-    std::vector<int> row_ptr((size_t)nc + 1, 0), colv((size_t)nnzb);
-    for (const int2& c : P.blk_cam) { ++row_ptr[c.x + 1]; if (c.x != c.y) ++row_ptr[c.y + 1]; }
-    for (int c = 0; c < nc; ++c) row_ptr[c + 1] += row_ptr[c];
-    std::vector<int> fill(row_ptr.begin(), row_ptr.end() - 1);
-    std::vector<int2> posv((size_t)nblk);
-    for (long long b = 0; b < nblk; ++b) {
-      const int2 c = P.blk_cam[b];
-      const int lo = fill[c.x]++;
-      colv[lo] = c.y;
-      int up = -1;
-      if (c.x != c.y) { up = fill[c.y]++; colv[up] = c.x; }
-      posv[b] = make_int2(lo, up);
-    }
-    std::vector<AsmTerm> at;
-    at.reserve((size_t)nt);
-    for (int lm = 0; lm < L.nl_local; ++lm) {
-      const int sidx = L.sorted_of_lm[lm];
-      const TileInfo& T = L.tiles[L.tile_of_sorted[sidx]];
-      const int g = sidx - T.lm_base;
-      for (int a = 0; a < T.n; ++a)
-        for (int b = 0; b <= a; ++b)
-          at.push_back({T.panel_off + 2LL * g * T.G, a | b << 16, T.n | (31 - __builtin_clz((unsigned)T.G)) << 15 | (int)T.KP << 18});
-    }
-    TRY(upload(&d_asm_terms, at));
+    if ((size_t)A.device_bytes + ((size_t)256 << 20) > free_b) return RBA_OK;  // keep 256 MB for the rest of the handle and the caller
+    TRY(upload(&d_asm_terms, A.terms));
     TRY(upload(&d_asm_wpos, P.wpos));
     TRY(upload(&d_asm_blk_ptr, P.blk_ptr));
-    TRY(upload(&d_asm_pos, posv));
-    TRY(upload(&d_asm_row_ptr, row_ptr));
-    TRY(upload(&d_asm_col, colv));
-    TRY(dalloc(&d_asm_stage, (size_t)stage_terms * 81, false));
-    TRY(dalloc(&d_asm_Su, (size_t)nblk * 81));
-    TRY(dalloc(&d_asm_S, (size_t)nnzb * 81));
-    asm_ranges = ranges;
-    asm_nblk = (int)nblk; asm_nnzb = nnzb;
-    // Switch point: building S costs about twice its staging traffic (stage 1 + stage 2, each written and read once) in
-    // units of operator time, and every iteration with S saves the panel bytes minus the bytes of S (measured on H100:
-    // Ladybug-1723 f32 breaks even after ~23 iterations, Trafalgar-257 f64 after ~24)
-    const double staged = 4.0 * (double)nt * 81 * sizeof(S), saved = (double)L.panel_scalars * sizeof(S) - (double)s_bytes;
-    asm_switch = asm_at > 0 ? asm_at : 1 + (int)std::ceil(2.0 * staged / std::max(saved, 1.0));
+    TRY(upload(&d_asm_pos, A.pos));
+    TRY(upload(&d_asm_row_ptr, A.row_ptr));
+    TRY(upload(&d_asm_col, A.col));
+    TRY(dalloc(&d_asm_stage, (size_t)A.nt * 81, false));
+    TRY(dalloc(&d_asm_Su, (size_t)A.nblk * 81));
+    TRY(dalloc(&d_asm_S, (size_t)A.nnzb * 81));
+    asm_nt = A.nt; asm_nblk = (int)A.nblk; asm_nnzb = A.nnzb;
+    asm_switch = asm_at > 0 ? asm_at : A.switch_iteration;
     asm_on = true;
     return RBA_OK;
   }
-  // S_u (stage 1, damping = 0) or S = S_u + the damping rows' part (stage 2, damping = 1), one landmark range at a time
+  // S_u (stage 1, damping = 0) or S = S_u + the damping rows' part (stage 2, damping = 1)
   void assemble(int damping) {
-    for (size_t k = 0; k + 1 < asm_ranges.size(); ++k) {
-      const long long w0 = asm_ranges[k], w1 = asm_ranges[k + 1];
-      const int grid = (int)std::max<long long>(1, std::min<long long>((w1 - w0 + 23) / 24, (long long)sm_count * 16));
-      k_rcs_terms<S><<<grid, 256, 0, stream>>>(D.panel, d_asm_terms, w0, w1, damping, d_asm_stage);
-      k_rcs_combine<S><<<(unsigned)((81LL * asm_nblk + 255) / 256), 256, 0, stream>>>(
-          d_asm_blk_ptr, d_asm_wpos, asm_nblk, w0, w1, d_asm_stage, damping ? (const S*)d_asm_Su : nullptr,
-          damping ? (const int2*)d_asm_pos : nullptr, (int)(k == 0), damping ? d_asm_S : d_asm_Su);
-      launches += 2;
-    }
+    const int grid = (int)std::max<long long>(1, std::min<long long>((asm_nt + 23) / 24, (long long)sm_count * 16));
+    k_rcs_terms<S><<<grid, 256, 0, stream>>>(D.panel, d_asm_terms, asm_nt, damping, d_asm_stage);
+    k_rcs_combine<S><<<(unsigned)((81LL * asm_nblk + 255) / 256), 256, 0, stream>>>(
+        d_asm_blk_ptr, d_asm_wpos, asm_nblk, d_asm_stage, damping ? (const S*)d_asm_Su : nullptr,
+        damping ? (const int2*)d_asm_pos : nullptr, damping ? d_asm_S : d_asm_Su);
+    launches += 2;
   }
 
   // ------------------------------------------------------------------------------------------
@@ -1722,11 +1614,12 @@ struct Solver : rba_handle {
     *p = (T*)q;
     return RBA_OK;
   }
-  // The term lists of rba_compute_covariance (pair_terms), built at the first call.
+  // The term lists of rba_compute_covariance (build_pair_list), built at the first call.
   int cov_build_lists() {
     if (cov_ready) return RBA_OK;
-    PairTerms P;
-    TRY(pair_terms(P));
+    PairList P;
+    const std::string msg = build_pair_list(L, P);
+    if (!msg.empty()) { g_err = msg; return RBA_ERR_UNSUPPORTED; }
     TRY(cov_upload(&d_cov_blk_cam, P.blk_cam));
     TRY(cov_upload(&d_cov_blk_ptr, P.blk_ptr));
     TRY(cov_upload(&d_cov_terms, P.terms));
@@ -1785,8 +1678,8 @@ struct Solver : rba_handle {
       k_cov_landmark<S, true><<<wgrid, 128, 0, stream>>>(D, ko, d_cov_lm_slot0, d_cov_lm_n, nl, jp, kb, wl, rk, d_lmp_of_lm);
     else
       k_cov_landmark<S><<<wgrid, 128, 0, stream>>>(D, ko, d_cov_lm_slot0, d_cov_lm_n, nl, jp, kb, wl, rk);
-    k_cov_assemble<<<std::max(1, std::min((cov_nblk + 7) / 8, sm_count * 8)), 256, 0, stream>>>(d_cov_blk_cam, d_cov_blk_ptr, d_cov_terms,
-                                                                                                  cov_nblk, jp, kb, A, np);
+    k_cov_assemble<<<std::max(1, std::min((cov_nblk + 7) / 8, sm_count * 8)), 256, 0, stream>>>(
+        (const int2*)d_cov_blk_cam, d_cov_blk_ptr, (const int2*)d_cov_terms, cov_nblk, jp, kb, A, np);
     if (has_abs_prior || n_pairs > 0)
       k_cov_priors<S><<<(nc + 127) / 128, 128, 0, stream>>>(D.cams, nc, has_abs_prior ? d_prior_mean : nullptr, d_prior_L, d_pair_ij,
                                                             d_pair_mean, d_pair_L, n_pairs > 0 ? d_pair_ptr : nullptr, d_pair_item,
