@@ -1933,7 +1933,7 @@ __device__ __forceinline__ void matvec_item_tma(const DevPtrs<S>& D, const Matve
 // Minimum resident CTAs: 5 for float32 (the shared-memory limit), 2 for float64 (register-limited).
 template <class S, int WARPS, int NS, int STAGE_BYTES>
 __global__ void __launch_bounds__(WARPS * 32, sizeof(S) == 4 ? 5 : 2) k_matvec_small_tma(DevPtrs<S> D, const MatvecItem* __restrict__ items,
-                                                                  int item_begin, int item_end, int scratch_per_warp,
+                                                                  int item_begin, int item_end,
                                                                   const S* __restrict__ xvec, const int* done, int pdl) {
   extern __shared__ __align__(128) unsigned char smem_tma[];
   __shared__ __align__(8) uint64_t bars_all[WARPS][NS];

@@ -124,8 +124,9 @@ struct Solver : rba_handle {
   // camera-major CSR the operator's per-slot output is reduced over: the y-slot CSR of the dense form (one slot per
   // observation and row chunk) or the observation CSR of the implicit form
   const int* op_slots = nullptr; const ReduceItem* op_items = nullptr; const int* op_item_ptr = nullptr; int n_op_items = 0;
-  bool implicit_op = false;
-  bool panel_form = true;        // gradient and SCHUR_JACOBI blocks from the Q2 panels (reference form) instead of the identities
+  // the Q2 panels exist: the dense operator (k_matvec_small_tma, k_matvec_large) stores and reads them; the implicit
+  // operator, which the Schur-complement solvers share, has none (validate_options)
+  bool panels = true;
   ReduceItem* d_pb_items = nullptr; int* d_pb_item_ptr = nullptr; int n_pb_items = 0;
   // launch geometry and work orders of the persistent kernels (deal_work, setup_kernels)
   Scratch<S> k1_sc{}, k2_sc{};
@@ -324,16 +325,16 @@ struct Solver : rba_handle {
     if (opt.residual_reset_period <= 0) opt.residual_reset_period = 10;
     if (opt.power_order <= 0) opt.power_order = 20;  // solver_options.hpp:270
     // the Schur-complement solvers share the per-observation records and the implicit operator kernels (k_sc_stage2)
-    implicit_op = opt.operator_form == 1 || opt.solver_type != 0;
-    // gradient / SCHUR_JACOBI blocks from the stored Q2 panels like the reference, unless there are no panels (implicit operator)
-    panel_form = !implicit_op && opt.stage2_form == 0;
+    panels = opt.operator_form == 0 && opt.solver_type == 0;
     ko.use_valid_projections_only = opt.use_valid_projections_only;
     ko.robust_norm = opt.robust_norm;
-    ko.write_panel = implicit_op ? 0 : 1;
+    ko.write_panel = panels;
     ko.huber = opt.huber_parameter;
     ko.jacobi_eps = opt.jacobi_scaling_epsilon > 0 ? opt.jacobi_scaling_epsilon : (double)ST<S>::eps_sqrt();  // ref: linearizor_base.cpp:72-79
     return RBA_OK;
   }
+  // gradient and SCHUR_JACOBI blocks from the stored Q2 panels like the reference, instead of the orthogonality identities
+  bool panel_form() const { return panels && opt.stage2_form == 0; }
 
   // Test hooks, not options: each forces at small size a path that the solver also takes on its own.
   //   RBA_PCG_PARTIALS=0  PCG without the per-segment hand-over to the vector kernel (taken above 1808 cameras)
@@ -380,8 +381,8 @@ struct Solver : rba_handle {
       TRY(upload(&d_csr_y_item_ptr, L.csr_y.cam_item_ptr));
       n_y_items = (int)L.csr_y.items.size();
     }
-    if (implicit_op) { op_slots = d_csr_obs_slots; op_items = d_csr_obs_items; op_item_ptr = d_csr_obs_item_ptr; n_op_items = n_obs_items; }
-    else { op_slots = d_csr_y_slots; op_items = d_csr_y_items; op_item_ptr = d_csr_y_item_ptr; n_op_items = n_y_items; }
+    if (panels) { op_slots = d_csr_y_slots; op_items = d_csr_y_items; op_item_ptr = d_csr_y_item_ptr; n_op_items = n_y_items; }
+    else { op_slots = d_csr_obs_slots; op_items = d_csr_obs_items; op_item_ptr = d_csr_obs_item_ptr; n_op_items = n_obs_items; }
     TRY(upload(&d_pb_items, L.pb_items));
     TRY(upload(&d_pb_item_ptr, L.pb_cam_item_ptr));
     n_pb_items = (int)L.pb_items.size();
@@ -390,15 +391,15 @@ struct Solver : rba_handle {
 
   // The grids of the persistent kernels and the order in which their warps take the work.
   int deal_work() {
-    if (implicit_op) {
+    if (panels) {
+      TRY(deal_matvec_items());
+    } else {
       while (imp_tile_split < (int)L.tiles.size() && (32 / L.tiles[imp_tile_split].G) * L.tiles[imp_tile_split].n <= IMP_MAXSLOTS) ++imp_tile_split;
       imp_smem = (size_t)IMP_WARPS * IMP_NS * (size_t)IMP_MAXSLOTS * 48 * sizeof(S);
       CU(cudaFuncSetAttribute((k_matvec_implicit_tma<S, IMP_WARPS, IMP_MAXSLOTS, IMP_NS>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)imp_smem));
       int bps = 0;
       CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, (k_matvec_implicit_tma<S, IMP_WARPS, IMP_MAXSLOTS, IMP_NS>), IMP_WARPS * 32, imp_smem));
       imp_grid = std::max(1, std::min((imp_tile_split + IMP_WARPS - 1) / IMP_WARPS, sm_count * std::max(1, bps)));
-    } else {
-      TRY(deal_matvec_items());
     }
     // the tile kernels' scratch decides k_linearize_qr's grid
     long long need1 = 0, need2 = 0;
@@ -479,7 +480,7 @@ struct Solver : rba_handle {
   int alloc_buffers() {
     TRY(dalloc(&D.cams, (size_t)10 * nc)); TRY(dalloc(&cams_bk, (size_t)10 * nc));
     TRY(dalloc(&D.lms, (size_t)3 * L.nl_local)); TRY(dalloc(&lms_bk, (size_t)3 * L.nl_local));
-    if (ko.write_panel) TRY(dalloc(&D.panel, (size_t)L.panel_scalars));  // the implicit operator never touches the panels
+    if (panels) TRY(dalloc(&D.panel, (size_t)L.panel_scalars));
     TRY(dalloc(&D.jp, (size_t)20 * L.nslots));
     TRY(dalloc(&D.q1u, (size_t)28 * L.nslots));
     TRY(dalloc(&D.q1d, (size_t)28 * L.nslots));
@@ -487,7 +488,7 @@ struct Solver : rba_handle {
     TRY(dalloc(&D.res, (size_t)2 * L.nslots));
     TRY(dalloc(&D.lmk, (size_t)24 * L.sorted_lm.size()));
     TRY(dalloc(&D.qtr, (size_t)2 * L.nslots));
-    if (panel_form) {
+    if (panel_form()) {
       TRY(dalloc(&D.dmp, (size_t)28 * L.nslots));
       if (opt.preconditioner_type == 1) TRY(dalloc(&D.blk0, (size_t)48 * L.nslots));
       TRY(dalloc(&D.blocks0, (size_t)81 * nc));
@@ -999,7 +1000,7 @@ struct Solver : rba_handle {
                                                             d_prior_H, d_prior_g, jac ? D.jblocks : nullptr, d_pair_O);
       launches += 2;
     }
-    if (panel_form) {
+    if (panel_form()) {
       // rows 3..2n-1 of the Q2 panels do not change with lambda: their part of the gradient (ipp:443-466) and of the
       // SCHUR_JACOBI blocks (ipp:520-552) is accumulated once per linearisation (this shard only; the sum over the
       // shards happens in solve() together with the damping-row part)
@@ -1047,58 +1048,77 @@ struct Solver : rba_handle {
     return reduce_ranks ? allreduce(dst, (size_t)81 * nc) : RBA_OK;
   }
 
-  // one complete operator application outside PCG: y = sum over the landmarks of P^T P x_red (this shard), per camera in D.y
-  int matvec_launch(const S* xvec) {
-    matvec_kernels(xvec, nullptr, false);
-    return s_valid ? RBA_OK : cam_reduce_final(false, 0, false);
+  // How the operator's output reaches the vector step, decided in one place (handover()):
+  enum class Handover {
+    Assembled,  // S is assembled for this solve's lambda (setup_assembled): k_rcs_spmv writes D.y
+    Partials,   // one GPU, PCG, while a cluster CTA's share of the cameras fits the vector kernel's registers (9 ceil(nc /
+                // cluster) <= VEC_THREADS VEC_EPT: <= 1808 cameras with 16 CTAs, <= 904 with 8): k_cam_reduce writes the
+                // per-segment sums and k_pcg_vec adds them in the order of k_cam_reduce_final's last arriver (bit-identical,
+                // without its arrival counters and fences)
+    Counter,    // one GPU otherwise (the power series, and larger camera counts such as Final-13682, the combination
+                // measured there): k_cam_reduce_final<false> writes D.y
+    Peer,       // several ranks, peers mapped (rba_ipc_import): k_cam_reduce_final<true> into every rank's staging area,
+                // which k_pcg_vec sums
+    Nccl,       // several ranks otherwise: D.y cleared, k_cam_reduce_final<false>, all-reduced, vector step without PDL
+  };
+  // k_cam_reduce_final never writes a camera without observations in this shard.  So Counter needs D.y cleared once per
+  // solve and before rba_right_multiply (an earlier call may have left other values: rba_right_multiply stores lambda x
+  // there), and Nccl before every application (the in-place all-reduce would carry the previous sum into the next).  The
+  // others need no clear: k_rcs_spmv writes every camera, k_pcg_vec takes 0 for a camera without segments, and a peer
+  // staging slot that is never written stays zero.
+  Handover handover() const {
+    if (s_valid) return Handover::Assembled;
+    if (opt.nranks > 1) return peer_ok ? Handover::Peer : Handover::Nccl;
+    const bool vec_cached = 9 * ((nc + pcg_cluster - 1) / pcg_cluster) <= VEC_THREADS * VEC_EPT;
+    return pcg_partials && vec_cached && opt.solver_type != 2 ? Handover::Partials : Handover::Counter;
   }
-  // operator part of one matvec: yobs = P^T P x_red for every landmark (e0_only: the implicit operator's E_0 x alone);
-  // assembled operator: D.y = S x_red, complete
-  void matvec_kernels(const S* xvec, const int* done, bool pdl, int e0_only = 0) {
-    if (s_valid) {
-      launch_ex(k_rcs_spmv<S>, nc, SPMV_WARPS * 32, 0, pdl, 1, (const int*)d_asm_row_ptr, (const int*)d_asm_col, (const S*)d_asm_S, xvec,
-                D.y, done, (int)pdl);
-      ++tm.matvec_launches;
-      return;
-    }
-    if (implicit_op) {
+  // One operator application H x (e0_only: the implicit operator's E_0 x alone) and the reduction of hand-over h; the caller
+  // then launches its vector kernel.  In a solve the kernels return at once when it has ended, and those that may are
+  // launched dependent on their predecessor.
+  int apply_operator(const S* xvec, Handover h, bool in_solve, int e0_only = 0) {
+    const int* done = in_solve ? &d_state->done : nullptr;
+    const bool pdl = in_solve;
+    ++tm.matvec_launches;
+    if (h == Handover::Assembled)
+      return launch_ex(k_rcs_spmv<S>, nc, SPMV_WARPS * 32, 0, pdl, 1, (const int*)d_asm_row_ptr, (const int*)d_asm_col, (const S*)d_asm_S, xvec, D.y, done, (int)pdl);
+    if (panels) {  // yobs = P^T P x
+      if (L.n_items_large > 0) {
+        k_matvec_large<S, K4_WARPS, KPMAX><<<grid_for(L.n_items_large, K4_WARPS, 4), K4_WARPS * 32, k4_smem_small, stream>>>(
+            D, d_items, 0, L.n_items_large, L.k4_scratch_per_warp, xvec, done);
+        ++launches;
+      }
+      const bool p = pdl && L.n_items_large == 0;
+      if (n_dealt > L.n_items_large)
+        TRY(launch_ex(k_matvec_small_tma<S, K4_WARPS, K4_NS, K4_STAGE>, tma_grid, K4_WARPS * 32, K4_SMEM_TMA, p, 1, D, (const MatvecItem*)d_items, L.n_items_large, n_dealt, xvec, done, (int)p));
+    } else {
       const int ntl = (int)L.tiles.size();
       const bool p = pdl && imp_tile_split == ntl;  // a single kernel between the PCG vector step and the reduction
       if (imp_tile_split > 0)
-        launch_ex((k_matvec_implicit_tma<S, IMP_WARPS, IMP_MAXSLOTS, IMP_NS>), imp_grid, IMP_WARPS * 32, imp_smem, p, 1, D, imp_tile_split, xvec, done, (int)p, e0_only);
+        TRY(launch_ex((k_matvec_implicit_tma<S, IMP_WARPS, IMP_MAXSLOTS, IMP_NS>), imp_grid, IMP_WARPS * 32, imp_smem, p, 1, D, imp_tile_split, xvec, done, (int)p, e0_only));
       if (imp_tile_split < ntl)
-        launch_ex(k_matvec_implicit<S>, (ntl - imp_tile_split + TILE_WARPS - 1) / TILE_WARPS, TILE_WARPS * 32, 0, false, 1, D, imp_tile_split, xvec, done, 0, e0_only);
-      ++tm.matvec_launches;
-      return;
+        TRY(launch_ex(k_matvec_implicit<S>, (ntl - imp_tile_split + TILE_WARPS - 1) / TILE_WARPS, TILE_WARPS * 32, 0, false, 1, D, imp_tile_split, xvec, done, 0, e0_only));
     }
-    if (L.n_items_large > 0) {
-      k_matvec_large<S, K4_WARPS, KPMAX><<<grid_for(L.n_items_large, K4_WARPS, 4), K4_WARPS * 32, k4_smem_small, stream>>>(
-          D, d_items, 0, L.n_items_large, L.k4_scratch_per_warp, xvec, done);
-      ++launches;
-    }
-    if (n_dealt > L.n_items_large) {
-      const bool p = pdl && L.n_items_large == 0;
-      launch_ex(k_matvec_small_tma<S, K4_WARPS, K4_NS, K4_STAGE>, tma_grid, K4_WARPS * 32, K4_SMEM_TMA, p, 1, D, (const MatvecItem*)d_items,
-                L.n_items_large, n_dealt, L.k4_scratch_per_warp, xvec, done, (int)p);
-    }
-    ++tm.matvec_launches;
+    const int grid = grid_for(n_op_items, 8, 8);
+    if (h == Handover::Partials)
+      return launch_ex(k_cam_reduce<S>, grid, 256, 0, pdl, 1, (const S*)D.yobs, op_slots, op_items, n_op_items, D.partial, done, (int)pdl);
+    if (h == Handover::Peer) ++ar_seq;
+    if (h == Handover::Nccl) CU(cudaMemsetAsync(D.y, 0, (size_t)9 * nc * sizeof(S), stream));
+    auto kern = h == Handover::Peer ? k_cam_reduce_final<S, true> : k_cam_reduce_final<S, false>;
+    TRY(launch_ex(kern, grid, 256, 0, pdl, 1, (const S*)D.yobs, op_slots, op_items, n_op_items, op_item_ptr, D.partial, d_cam_cnt, D.y, done, (int)pdl, pc, ar_seq, nc));
+    return h == Handover::Nccl ? allreduce(D.y, (size_t)9 * nc) : RBA_OK;
   }
-  // per-camera sums of the operator output into D.y (peers: into every rank's staging area of the peer exchange).  Inside a
-  // solve it is launched dependent on its predecessor and returns at once when the solve has ended.
-  int cam_reduce_final(bool peers, int seq, bool in_solve) {
-    auto kern = peers ? k_cam_reduce_final<S, true> : k_cam_reduce_final<S, false>;
-    return launch_ex(kern, grid_for(n_op_items, 8, 8), 256, 0, in_solve, 1, (const S*)D.yobs, op_slots, op_items, n_op_items, op_item_ptr,
-                     D.partial, d_cam_cnt, D.y, in_solve ? (const int*)&d_state->done : nullptr, (int)in_solve, pc, seq, nc);
+  // one operator application outside PCG (rba_right_multiply, rba_time_matvec): this shard's H x in D.y
+  int matvec_launch(const S* xvec, bool clear_y) {
+    const Handover h = handover() == Handover::Assembled ? Handover::Assembled : Handover::Counter;
+    if (clear_y && h == Handover::Counter) CU(cudaMemsetAsync(D.y, 0, (size_t)9 * nc * sizeof(S), stream));
+    return apply_operator(xvec, h, false);
   }
+  // the PCG vector step; pair priors: O v of the step's vector (v = x in the refresh's second half, else p) into D.pair_ov first
   int pcg_vec(int i, int mode, bool pdl, int is_last, S lambda, bool fused_ar = false, bool from_partials = false) {
     PeerComm c = pc;
     if (!fused_ar) c.nranks = 1;
-    if (D.pair_ov) {  // pair priors: O v of the step's vector (v = x in the refresh's second half, else p) into D.pair_ov first
-      if (mode != 3) TRY(pair_ov(mode == 2 ? D.x : D.p, pdl));
-      return launch_ex(k_pcg_vec<S, true, true>, pcg_cluster, VEC_THREADS, 0, pdl, pcg_cluster, D, d_state, lambda, i, mode, (double)opt.eta,
-                       (int)opt.min_linear_solver_iterations, is_last, (int)pdl, c, ar_seq, from_partials ? op_item_ptr : (const int*)nullptr, d_prog);
-    }
-    auto kern = D.prior_H ? k_pcg_vec<S, true> : k_pcg_vec<S, false>;
+    if (D.pair_ov && mode != 3) TRY(pair_ov(mode == 2 ? D.x : D.p, pdl));
+    auto kern = D.pair_ov ? k_pcg_vec<S, true, true> : D.prior_H ? k_pcg_vec<S, true> : k_pcg_vec<S, false>;
     return launch_ex(kern, pcg_cluster, VEC_THREADS, 0, pdl, pcg_cluster, D, d_state, lambda, i, mode, (double)opt.eta,
                      (int)opt.min_linear_solver_iterations, is_last, (int)pdl, c, ar_seq, from_partials ? op_item_ptr : (const int*)nullptr, d_prog);
   }
@@ -1106,34 +1126,10 @@ struct Solver : rba_handle {
   int pair_ov(const S* v, bool pdl) {
     return launch_ex(k_pair_ov<S>, (9 * nc + 255) / 256, 256, 0, pdl, 1, D, (const PcgState*)d_state, v);
   }
-  // The hand-over through per-segment sums is taken when a cluster CTA's share of the cameras fits the vector kernel's
-  // register-resident layout (9 ceil(nc / cluster) <= VEC_THREADS VEC_EPT: <= 1808 cameras with a 16-CTA cluster, <= 904
-  // with 8); larger camera counts on one GPU (Final-13682) keep the arrival-counter reduction into D.y, the combination that
-  // was measured at that size.
-  bool pcg_from_partials() const {
-    const bool vec_cached = 9 * ((nc + pcg_cluster - 1) / pcg_cluster) <= VEC_THREADS * VEC_EPT;
-    return opt.nranks == 1 && pcg_partials && vec_cached;
-  }
-  // finish one operator application inside PCG (H v for v = p in mode 0/1, x in mode 2) and do the vector step
-  int pcg_apply(int i, int mode, int is_last, S lambda) {
-    if (s_valid) return pcg_vec(i, mode, true, is_last, lambda);  // k_rcs_spmv has written D.y
-    if (pcg_from_partials()) {
-      // one GPU: the vector kernel adds the per-segment sums itself (same order as k_cam_reduce_final's last arriver:
-      // bit-identical) -- no arrival counters, fences or second pass in the reduction
-      TRY(launch_ex(k_cam_reduce<S>, grid_for(n_op_items, 8, 8), 256, 0, true, 1, (const S*)D.yobs, op_slots, op_items, n_op_items, D.partial,
-                    (const int*)&d_state->done, 1));
-      return pcg_vec(i, mode, true, is_last, lambda, false, true);
-    }
-    const bool fused = opt.nranks > 1 && peer_ok;
-    if (fused) ++ar_seq;
-    // NCCL path: k_cam_reduce_final writes y only for cameras that have observations in this shard; D.y is all-reduced IN
-    // PLACE, so without this the other cameras would carry the previous iteration's global sum into the next all-reduce
-    if (opt.nranks > 1 && !fused) CU(cudaMemsetAsync(D.y, 0, (size_t)9 * nc * sizeof(S), stream));
-    TRY(cam_reduce_final(fused, ar_seq, true));
-    if (opt.nranks == 1) return pcg_vec(i, mode, true, is_last, lambda);
-    if (fused) return pcg_vec(i, mode, true, is_last, lambda, true);
-    TRY(allreduce(D.y, (size_t)9 * nc));
-    return pcg_vec(i, mode, false, is_last, lambda);
+  // one operator application inside PCG (H v for v = p in mode 0/1, x in mode 2) and the vector step after it
+  int pcg_step(int i, int mode, int is_last, S lambda, Handover h) {
+    TRY(apply_operator(mode == 2 ? D.x : D.p, h, true));
+    return pcg_vec(i, mode, h != Handover::Nccl, is_last, lambda, h == Handover::Peer, h == Handover::Partials);
   }
   // Enqueue iterations 1..last in chunks of `chunk` (enqueue(i)); after each chunk the PcgState is copied into one of two
   // pinned slots, and the host waits for the copy of the chunk before and stops once it shows the solve ended.
@@ -1161,8 +1157,9 @@ struct Solver : rba_handle {
   // ref: solver/linearizor_qr.cpp:140-265
   // Power-series solve of the reduced camera system (ref: sc/linearization_power_sc.hpp:130-160, driven by
   // solver/linearizor_power_sc.cpp:140-160 with q_tolerance = eta): per term one E_0 application (the implicit operator
-  // kernels with e0_only), the per-camera reduction and k_power_vec; the device convergence flag is polled like in PCG.
-  int power_enqueue(void* inc_out) {
+  // kernels with e0_only), the per-camera reduction of hand-over h (Counter) and k_power_vec; the device convergence flag
+  // is polled like in PCG.
+  int power_enqueue(Handover h, void* inc_out) {
     TRY(start(ev_pcg));
     CU(cudaMemsetAsync(d_state, 0, sizeof(PcgState), stream));
     const int order = opt.power_order;
@@ -1170,8 +1167,7 @@ struct Solver : rba_handle {
     auto kern = D.pair_ov ? k_power_vec<S, true> : k_power_vec<S, false>;
     TRY(launch_ex(kern, pcg_cluster, VEC_THREADS, 0, false, pcg_cluster, D, d_state, 0, (double)opt.eta, 0, 0));
     TRY(enqueue_polled(order, opt.pcg_check_period, [&](int i) -> int {
-      matvec_kernels(D.p, &d_state->done, true, 1);
-      TRY(cam_reduce_final(false, 0, true));
+      TRY(apply_operator(D.p, h, true, 1));
       if (D.pair_ov) TRY(pair_ov(D.p, true));
       return launch_ex(kern, pcg_cluster, VEC_THREADS, 0, true, pcg_cluster, D, d_state, i, (double)opt.eta, (int)(i == order), 1);
     }));
@@ -1197,15 +1193,15 @@ struct Solver : rba_handle {
       auto k = lmp ? k_sc_stage2<S, true> : k_sc_stage2<S>;
       k<<<tile_grid(sm_count * 8), TILE_WARPS * 32, 0, stream>>>(D, lambda);
     } else {
-      auto k = panel_form ? (lmp ? k_stage2<S, true, true> : k_stage2<S, true>) : (lmp ? k_stage2<S, false, true> : k_stage2<S, false>);
-      k<<<tile_grid(k2_max_blocks), TILE_WARPS * 32, k2_smem, stream>>>(D, lambda, k2_sc, ko.write_panel);
+      auto k = panel_form() ? (lmp ? k_stage2<S, true, true> : k_stage2<S, true>) : (lmp ? k_stage2<S, false, true> : k_stage2<S, false>);
+      k<<<tile_grid(k2_max_blocks), TILE_WARPS * 32, k2_smem, stream>>>(D, lambda, k2_sc, (int)panels);
     }
     ++launches;
     s_valid = false;  // S of the previous lambda; rebuilt if this solve runs long enough (solve_enqueue)
-    rc = camera_reduce(d_csr_obs_slots, d_csr_obs_items, n_obs_items, d_csr_obs_item_ptr, D.b, panel_form ? D.b0 : nullptr); if (rc) return rc;
+    rc = camera_reduce(d_csr_obs_slots, d_csr_obs_items, n_obs_items, d_csr_obs_item_ptr, D.b, panel_form() ? D.b0 : nullptr); if (rc) return rc;
     const bool power = opt.solver_type == 2;
     const bool schur = opt.preconditioner_type == 1 && !power;  // Power-SC inverts Hpp = sum Jp^T Jp + lambda I instead
-    if (schur) { rc = panel_form ? precond_blocks(2, D.blocks, D.blocks0, true) : precond_blocks(1, D.blocks, nullptr, true); if (rc) return rc; }
+    if (schur) { rc = panel_form() ? precond_blocks(2, D.blocks, D.blocks0, true) : precond_blocks(1, D.blocks, nullptr, true); if (rc) return rc; }
     rc = stop(ev_stage2); if (rc) return rc;
     rc = start(ev_precond); if (rc) return rc;
     // pose damping lambda*I added to the blocks, then explicit inverse (ref: linearization_qr.hpp:796-802, linearizor_qr.cpp:228-237)
@@ -1232,12 +1228,9 @@ struct Solver : rba_handle {
       new_linearization_point = false;
       return RBA_OK;
     }
-    // k_cam_reduce_final writes D.y only for cameras with observations, and an earlier call may have left other values in
-    // the remaining entries (rba_right_multiply stores lambda x there for every camera).  The one-GPU consumers that read
-    // D.y (k_power_vec, and k_pcg_vec without the per-segment hand-over) need the operator's 0 for a camera without
-    // observations: cleared once per solve, outside the iteration.
-    if (opt.nranks == 1 && (power || !pcg_from_partials())) CU(cudaMemsetAsync(D.y, 0, (size_t)9 * nc * sizeof(S), stream));
-    if (power) return power_enqueue(inc_out);
+    Handover h = handover();
+    if (h == Handover::Counter) CU(cudaMemsetAsync(D.y, 0, (size_t)9 * nc * sizeof(S), stream));  // see handover()
+    if (power) return power_enqueue(h, inc_out);
     // PCG (ref: cg/conjugate_gradient.hpp:113-298 ; linearizor_base.cpp:81-103)
     rc = start(ev_pcg); if (rc) return rc;
     CU(cudaMemsetAsync(d_state, 0, sizeof(PcgState), stream));
@@ -1255,15 +1248,13 @@ struct Solver : rba_handle {
     rc = pcg_vec(0, 3, false, 0, lambda); if (rc) return rc;  // x = 0, r = b, z = M^-1 r, rho, p = z
     auto enqueue_iteration = [&](int i) -> int {
       const int is_last = (i == max_it) ? 1 : 0;
-      matvec_kernels(D.p, &d_state->done, true);
       if (i % period == 0) {
-        int r2 = pcg_apply(i, 1, 0, lambda); if (r2) return r2;
-        matvec_kernels(D.x, &d_state->done, true);
-        return pcg_apply(i, 2, is_last, lambda);
+        TRY(pcg_step(i, 1, 0, lambda, h));
+        return pcg_step(i, 2, is_last, lambda, h);
       }
-      return pcg_apply(i, 0, is_last, lambda);
+      return pcg_step(i, 0, is_last, lambda, h);
     };
-    if (opt.nranks > 1 && !peer_ok) {
+    if (h == Handover::Nccl) {
       // NCCL exchange: every rank must enqueue the SAME number of all-reduces, so the decision to stop may depend only on
       // the iteration count -- the flag is polled once per chunk of `depth` iterations, one chunk behind
       TRY(enqueue_polled(max_it, depth, enqueue_iteration));
@@ -1283,6 +1274,7 @@ struct Solver : rba_handle {
           if (!su_valid) assemble(0);
           assemble(1);
           su_valid = s_valid = true;
+          h = handover();
         }
         rc = enqueue_iteration(i); if (rc) return rc;
       }
@@ -1499,8 +1491,8 @@ struct Solver : rba_handle {
     out->panel_scalars_algorithmic = 18 * L.sum_n2;
     out->device_bytes = (int64_t)device_bytes;
     // the operator the last solve ended with: the panels, or S (blocks, column indices, row pointers, x read and y written once)
-    out->matvec_algorithmic_bytes = s_valid ? (81 * asm_nnzb + 18 * (int64_t)nc) * (int64_t)sizeof(S) + 4 * (asm_nnzb + nc + 1)
-                                           : (18 * L.sum_n2 + 18 * L.nobs_local) * (int64_t)sizeof(S) + 4 * L.nobs_local;
+    out->matvec_algorithmic_bytes = handover() == Handover::Assembled ? (81 * asm_nnzb + 18 * (int64_t)nc) * (int64_t)sizeof(S) + 4 * (asm_nnzb + nc + 1)
+                                                                        : (18 * L.sum_n2 + 18 * L.nobs_local) * (int64_t)sizeof(S) + 4 * L.nobs_local;
     out->landmark_begin = L.lm_begin;
     out->landmark_end = L.lm_end;
     out->num_matvec_items = (int)L.items.size();
@@ -1528,8 +1520,7 @@ struct Solver : rba_handle {
   int right_multiply(const void* x, void* y) override {
     if (!linearized || !damping_valid) { g_err = "rba_right_multiply needs rba_linearize + rba_solve first"; return RBA_ERR_STATE; }
     CU(cudaMemcpyAsync(D.z, x, (size_t)9 * nc * sizeof(S), cudaMemcpyHostToDevice, stream));
-    CU(cudaMemsetAsync(D.y, 0, (size_t)9 * nc * sizeof(S), stream));  // cameras without observations in this shard are not written
-    TRY(matvec_launch(D.z));
+    TRY(matvec_launch(D.z, true));
     TRY(allreduce(D.y, (size_t)9 * nc));  // no-op on one GPU
     k_pcg_q<S><<<NPART, 128, 0, stream>>>(D, D.y, D.z, D.y, last_lambda);
     ++launches;
@@ -1541,9 +1532,9 @@ struct Solver : rba_handle {
 
   int time_matvec(int reps, double* sec) override {
     if (!linearized || !damping_valid) { g_err = "rba_time_matvec needs rba_linearize + rba_solve first"; return RBA_ERR_STATE; }
-    TRY(matvec_launch(D.p));  // warm-up
+    TRY(matvec_launch(D.p, false));  // warm-up
     TRY(start(ev_mv));
-    for (int r = 0; r < reps; ++r) TRY(matvec_launch(D.p));
+    for (int r = 0; r < reps; ++r) TRY(matvec_launch(D.p, false));
     TRY(stop(ev_mv));
     CU(cudaStreamSynchronize(stream));
     CU(cudaGetLastError());
@@ -1567,7 +1558,7 @@ struct Solver : rba_handle {
   // structure passes the size rules (plan_assembled) and its buffers fit in the free device memory; else the panel
   // product.
   int setup_assembled() {
-    if (!asm_hook || opt.nranks != 1 || implicit_op) return RBA_OK;
+    if (!asm_hook || opt.nranks != 1 || !panels) return RBA_OK;
     PairList P;
     const std::string msg = build_pair_list(L, P);
     if (!msg.empty()) { g_err = msg; return RBA_ERR_UNSUPPORTED; }

@@ -12,7 +12,7 @@ The per-camera kernels branch on the number of slots a camera owns (rootba_b200/
   grid_for(n, 8, 8)     at most 8 blocks of 8 warps per SM: more reduce items than warps re-stage in the grid-stride loop
   cluster c             k_pcg_vec / k_power_vec give each CTA ceil(nc / c) cameras: empty CTAs when nc < c, a ragged last
                         CTA, register-resident while 9 ceil(nc / c) <= 1024 (up to 113 c cameras), a camera's 9 entries
-                        straddling thread element 512 from 57 cameras per CTA; pcg_from_partials switches the hand-over at
+                        straddling thread element 512 from 57 cameras per CTA; Solver::handover switches the hand-over at
                         the same threshold
 A degree case is a problem whose landmarks all have ONE track length n (2, a G = 4 length, two chunked lengths) and whose
 "hub" cameras have exactly the degrees of HUB_DEGREES; filler cameras complete the tracks.  Every camera is checked on its
@@ -106,7 +106,7 @@ def vec_partition(nc, cluster):
     cached = 9 * per <= VEC_THREADS * VEC_EPT
     return {"per_cta": per, "empty": sum(s == 0 for s in sizes), "ragged": sizes[last] < per, "cached": cached,
             "straddle": cached and 9 * per > VEC_THREADS,  # a camera's 9 entries cross thread element 512
-            "partials": cached,                            # pcg_from_partials on one GPU
+            "partials": cached,                            # the Partials hand-over (Solver::handover) on one GPU
             "last_range": (last * per, last * per + sizes[last])}
 
 
