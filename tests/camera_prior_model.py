@@ -115,18 +115,36 @@ def sqrt_info_kind(kind, rng, scale=1.0):
     return L
 
 
-def dense_system_with_prior(prob, mean, sqrt_info):
-    """the dense system of tests/test_oracle_dense_numpy.py::_dense_system with the prior rows appended: 9 rows per camera,
-    pose columns L de/d(inc), zero landmark columns, residual L e.  _reduced() of it is the total (reprojection + prior) LM
-    step: the Jacobi scaling over the whole Jacobian, H, b, inc = -H^-1 b, l_diff."""
-    from test_oracle_dense_numpy import _dense_system
-    Jp, Jl, r = _dense_system(prob)
-    A, rp = rows(prob.cams, mean, sqrt_info)
-    nc = prob.nc
-    Jp_p = np.zeros((9 * nc, Jp.shape[1]))
-    for c in range(nc):
-        Jp_p[9 * c:9 * c + 9, 9 * c:9 * c + 9] = A[c]
-    return np.vstack([Jp, Jp_p]), np.vstack([Jl, np.zeros((9 * nc, Jl.shape[1]))]), np.concatenate([r, rp.ravel()])
+def prior_case(nc=7, nl=90, seed=21, unobserved=True):
+    """synth_bal(7, 90) (+ one camera without observations): a mix of dense, centre-only, intrinsics-only and no priors,
+    centred near the cameras; the unobserved camera carries a dense prior"""
+    from rootba_b200.synthetic import BalArrays, synth_bal
+    prob = synth_bal(nc, nl, 3.6, seed=seed)
+    cams = np.asarray(prob.cams, np.float64)
+    if unobserved:
+        extra = cams[0].copy()
+        extra[4:7] += [0.3, -0.2, 0.1]
+        cams = np.vstack([cams, extra])
+        prob = BalArrays(cams, prob.lms, prob.lm_off, prob.obs_cam, prob.obs_xy)
+    rng = np.random.default_rng(seed + 1)
+    mean = mean_at(cams)
+    mean[:, 4:7] += rng.normal(0, 0.05, (len(cams), 3))
+    mean[:, :4] = [(Rotation.from_rotvec(rng.normal(0, 0.01, 3)) * Rotation.from_quat(q)).as_quat() for q in mean[:, :4]]
+    mean[:, 7] += rng.normal(0, 2.0, len(cams))
+    kinds = ["dense", "centre", "intrinsics", "none"]
+    L = np.stack([sqrt_info_kind(kinds[c % 4], rng) for c in range(len(cams))])
+    if unobserved:
+        L[-1] = sqrt_info_kind("dense", rng)
+    return prob, mean, L
+
+
+def small_prior(problem, seed=3):
+    """centre, dense and intrinsics priors in turn, centres moved by N(0, 0.05): (mean, L)"""
+    rng = np.random.default_rng(seed)
+    mean = mean_at(problem.cams)
+    mean[:, 4:7] += rng.normal(0, 0.05, (problem.nc, 3))
+    L = np.stack([sqrt_info_kind(["centre", "dense", "intrinsics"][c % 3], rng) for c in range(problem.nc)])
+    return mean, L
 
 
 # ------------------------------------------------------------------------------------------------

@@ -22,7 +22,7 @@ def fixed_mask(flags, nc):
     """[9 nc] bool of the held increment entries (RBA_FIX_* bits per camera), all False for None"""
     if flags is None:
         return np.zeros(9 * nc, bool)
-    from test_fixed_cameras import fixed_entries
+    from objective_checks import fixed_entries
     return fixed_entries(np.asarray(flags))
 
 

@@ -3,9 +3,10 @@
   prior p on landmark l_p: residual e = x - x0, cost 1/2 |L e|^2, L a 3x3 square-root information (any rank)
   rows of the total Jacobian: [0 (cameras) | L (columns of landmark l_p) | L e]
 
-The total objective is reprojection (tests/camera_model.py) plus these rows, optionally plus the camera priors of
-tests/camera_prior_model.py and the pair priors of tests/pair_prior_model.py.  The dense LM step is that of the whole
-Jacobian with the Jacobi scaling of its columns (prior columns included): (J_s^T J_s + lambda I) d = -J_s^T r.
+The total objective (tests/objective_checks.py: dense_system, total_cost) is reprojection (tests/camera_model.py) plus these
+rows, optionally plus the camera priors of tests/camera_prior_model.py and the pair priors of tests/pair_prior_model.py.  The
+dense LM step is that of the whole Jacobian with the Jacobi scaling of its columns (prior columns included):
+(J_s^T J_s + lambda I) d = -J_s^T r.
 
 The device folds a prior into the landmark's damping rows: the QR of [L~; sqrt(lambda) I] with the residual [g; 0]
 (L~ = L diag(jls), g = L e) gives 3 rows [C | 0 | c], and the damping rotations fold them into the landmark's R.  `compress`
@@ -60,33 +61,6 @@ def append_rows(system, nl, lms, idx, mean, sqrt_info):
     for p, l in enumerate(np.asarray(idx)):
         Jl_p[3 * p:3 * p + 3, 3 * l:3 * l + 3] = A[p]
     return np.vstack([Jp, np.zeros((3 * m, Jp.shape[1]))]), np.vstack([Jl, Jl_p]), np.concatenate([r, rp.ravel()])
-
-
-def dense_system(prob, lm_prior, cam_prior=None, pair_prior=None):
-    """the dense (Jp, Jl, r) of the total objective: reprojection (+ camera priors) (+ pair priors) + landmark priors"""
-    if pair_prior is not None:
-        import pair_prior_model as qm
-        base = qm.dense_system_with_pairs(prob, pair_prior, cam_prior)
-    elif cam_prior is not None:
-        import camera_prior_model as pm
-        base = pm.dense_system_with_prior(prob, *cam_prior)
-    else:
-        from test_oracle_dense_numpy import _dense_system
-        base = _dense_system(prob)
-    return append_rows(base, prob.nl, prob.lms, *lm_prior)
-
-
-def total_cost(prob, lm_prior, cam_prior=None, pair_prior=None):
-    """reprojection (camera_model, no robust loss) + camera priors + pair priors + landmark priors"""
-    import camera_model as cm
-    import camera_prior_model as pm
-    import pair_prior_model as qm
-    c = float(cm.compute_error(prob)["all"]["error"]) + cost(prob.lms, *lm_prior)
-    if cam_prior is not None:
-        c += pm.cost(prob.cams, *cam_prior)
-    if pair_prior is not None:
-        c += qm.cost(prob.cams, *pair_prior)
-    return c
 
 
 def scaling(Jp, Jl, eps):

@@ -90,26 +90,6 @@ def cost(cams, pairs, mean, sqrt_info):
                      for p, (i, j) in enumerate(pairs)))
 
 
-def dense_system_with_pairs(prob, pair_prior, camera_prior=None):
-    """the dense system of tests/test_oracle_dense_numpy.py::_dense_system with the pair rows (and, when given, the absolute
-    prior rows of camera_prior_model) appended: pose columns L de/d(inc), zero landmark columns, residual L e.  _reduced()
-    of it is the total LM step."""
-    from test_oracle_dense_numpy import _dense_system
-    if camera_prior is not None:
-        Jp, Jl, r = pm.dense_system_with_prior(prob, *camera_prior)
-    else:
-        Jp, Jl, r = _dense_system(prob)
-    Jq, rq = rows(prob.cams, *pair_prior)
-    return np.vstack([Jp, Jq]), np.vstack([Jl, np.zeros((Jq.shape[0], Jl.shape[1]))]), np.concatenate([r, rq])
-
-
-def total_cost(prob, pair_prior, camera_prior=None):
-    e = float(cm.compute_error(prob)["all"]["error"]) + cost(prob.cams, *pair_prior)
-    if camera_prior is not None:
-        e += pm.cost(prob.cams, *camera_prior)
-    return e
-
-
 def pair_case(nc=7, nl=90, seed=41, unobserved=True):
     """synth_bal(nc, nl) (+ one camera without observations, tied by a dense pair prior to camera 0): pairs between
     consecutive cameras with dense, translation-only, rotation-only and zero L, a repeated pair, a reversed pair, and means

@@ -4,7 +4,6 @@ import numpy as np
 import pytest
 from scipy.spatial.transform import Rotation
 
-import camera_model as cm
 import camera_prior_model as pm
 
 
@@ -50,51 +49,25 @@ def test_cost_is_half_the_squared_whitened_residual():
     assert np.allclose(pm.residual(cam, pm.mean_at(cam[None])[0]), 0, atol=1e-12)
 
 
-def prior_case(nc=7, nl=90, seed=21, unobserved=True):
-    """synth_bal(7, 90) (+ one camera without observations): a mix of dense, centre-only, intrinsics-only and no priors,
-    centred near the cameras; the unobserved camera carries a dense prior"""
-    from rootba_b200.synthetic import BalArrays, synth_bal
-    prob = synth_bal(nc, nl, 3.6, seed=seed)
-    cams = np.asarray(prob.cams, np.float64)
-    if unobserved:
-        extra = cams[0].copy()
-        extra[4:7] += [0.3, -0.2, 0.1]
-        cams = np.vstack([cams, extra])
-        prob = BalArrays(cams, prob.lms, prob.lm_off, prob.obs_cam, prob.obs_xy)
-    rng = np.random.default_rng(seed + 1)
-    mean = pm.mean_at(cams)
-    mean[:, 4:7] += rng.normal(0, 0.05, (len(cams), 3))
-    mean[:, :4] = [(Rotation.from_rotvec(rng.normal(0, 0.01, 3)) * Rotation.from_quat(q)).as_quat() for q in mean[:, :4]]
-    mean[:, 7] += rng.normal(0, 2.0, len(cams))
-    kinds = ["dense", "centre", "intrinsics", "none"]
-    L = np.stack([pm.sqrt_info_kind(kinds[c % 4], rng) for c in range(len(cams))])
-    if unobserved:
-        L[-1] = pm.sqrt_info_kind("dense", rng)
-    return prob, mean, L
-
-
-def total_cost(prob, mean, L):
-    return float(cm.compute_error(prob)["all"]["error"]) + pm.cost(prob.cams, mean, L)
-
-
 def test_first_order_model_of_the_total_objective_predicts_the_true_cost_change():
     """the dense LM step of the total problem (scaling over reprojection + prior columns, H, b, inc, l_diff): for a heavily
     damped step the model decrease matches the true decrease of reprojection + prior cost"""
     from rootba_b200.synthetic import BalArrays
+    from objective_checks import dense_system, total_cost
     from test_oracle_dense_numpy import _reduced
-    prob, mean, L = prior_case()
-    Jp, Jl, r = pm.dense_system_with_prior(prob, mean, L)
+    prob, mean, L = pm.prior_case()
+    Jp, Jl, r = dense_system(prob, camera=(mean, L))
     lam = 1e4
     D, sl, Jps, Jls, Minv, H, b = _reduced(Jp, Jl, r, lam, prob.nl, float(np.sqrt(1e-10)))
     assert np.all(D[-9:] < 1e3)  # the unobserved camera is scaled by its prior, not by 1 / eps
     inc = -np.linalg.solve(H, b)
     dl_s = -Minv @ (Jls.T @ r + Jls.T @ (Jps @ inc))
     l_diff = 0.5 * r @ r - 0.5 * np.sum((r + Jps @ inc + Jls @ dl_s) ** 2)
-    e0 = total_cost(prob, mean, L)
+    e0 = total_cost(prob, camera=(mean, L))
     assert 0.5 * r @ r == pytest.approx(e0, rel=1e-12)
     d = (D * inc).reshape(-1, 9)
     cams1 = np.stack([pm.apply_inc(prob.cams[c], d[c]) for c in range(prob.nc)])
     lms1 = np.asarray(prob.lms) + (sl * dl_s).reshape(-1, 3)
-    e1 = total_cost(BalArrays(cams1, lms1, prob.lm_off, prob.obs_cam, prob.obs_xy), mean, L)
+    e1 = total_cost(BalArrays(cams1, lms1, prob.lm_off, prob.obs_cam, prob.obs_xy), camera=(mean, L))
     assert l_diff > 0 and e0 > e1
     assert (e0 - e1) / l_diff == pytest.approx(1.0, abs=5e-2)

@@ -11,22 +11,8 @@ import numpy as np
 import pytest
 
 from conftest import ROOT, rel_err
+from objective_checks import MASK, fixed_entries
 from pcg_replay import pcg_replay
-
-FIX_POSE, FIX_F, FIX_K1, FIX_K2 = 1, 2, 4, 8
-# every bit, a combination of intrinsics, one fully fixed camera, free cameras
-MASK = np.array([FIX_POSE, FIX_F, FIX_K1 | FIX_K2, FIX_POSE | FIX_F | FIX_K1 | FIX_K2, 0, FIX_F | FIX_K1 | FIX_K2, FIX_K2], np.uint8)
-
-
-def fixed_entries(flags):
-    """[9 nc] bool: increment entries (t, r, f, k1, k2 per camera) held by the RBA_FIX_* bits"""
-    fx = np.zeros((len(flags), 9), bool)
-    fx[:, :6] = (flags & FIX_POSE)[:, None] != 0
-    fx[:, 6] = (flags & FIX_F) != 0
-    fx[:, 7] = (flags & FIX_K1) != 0
-    fx[:, 8] = (flags & FIX_K2) != 0
-    return fx.ravel()
-
 
 def masked_block_inverse(blocks, fixed):
     """k_precond_invert with flags: fixed rows / columns of each 9x9 block -> identity, invert, zero them in the inverse"""

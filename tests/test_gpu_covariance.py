@@ -18,9 +18,8 @@ import camera_model as cm
 import camera_prior_model as pm
 import covariance_model as cvm
 import pair_prior_model as qm
-from test_fixed_cameras import MASK
+from objective_checks import CONFIGS, MASK
 from rootba_b200._lib import RBA_NUMERICAL_FAILURE
-from test_gpu_fixed_cameras import CONFIGS
 
 pytestmark = pytest.mark.gpu
 
@@ -277,8 +276,7 @@ def test_gauge_not_fixed(size):
 
 def test_free_camera_without_observations():
     import rootba_b200 as rb
-    from test_camera_prior_model import prior_case
-    prob, _, _ = prior_case(7, 90)  # camera 7 has no observation
+    prob, _, _ = pm.prior_case(7, 90)  # camera 7 has no observation
     mean, L = _centre_priors(prob)
     L[-1] = 0.0
     lin = _handle(prob, np.float64, absp=(mean, L))

@@ -155,14 +155,13 @@ def test_large_prior_rotations(dtype):
 
 @pytest.mark.parametrize("cfg", [{}, dict(solver_type="POWER_SCHUR_COMPLEMENT")], ids=["default", "power-sc"])
 @pytest.mark.parametrize("dtype", [np.float64, np.float32], ids=["f64", "f32"])
-def test_large_prior_rotations_through_the_solve(cfg, dtype, monkeypatch):
+def test_large_prior_rotations_through_the_solve(cfg, dtype):
     """scaling, b, the preconditioner blocks, the operator, the increment, l_diff and the cost of one LM step with the same
-    priors, by the dense checks of test_gpu_camera_priors / test_gpu_pair_priors"""
-    import test_gpu_camera_priors as tcp
-    import test_gpu_pair_priors as tpp
+    priors, by objective_checks.check_against_dense as test_gpu_camera_priors / test_gpu_pair_priors call it"""
+    from objective_checks import check_against_dense
     prob, absp, pair = _rotation_case()
-    tcp._check_against_dense(cfg, prob, *absp, {}, monkeypatch, dtype=dtype)
-    tpp._check_against_dense(cfg, prob, pair, {}, monkeypatch, dtype=dtype, absp=absp)
+    check_against_dense(cfg, prob, camera=absp, dtype=dtype)
+    check_against_dense(cfg, prob, camera=absp, pairs=pair, dtype=dtype, inc_eta_kappa=True)
 
 
 def test_moved_state():

@@ -2,135 +2,54 @@
 system, no behaviour change without flags, fixed parameters bit-identical through whole LM runs, the no-free-parameter
 case, bad input, the C++ host and the sharded path."""
 import ctypes as C
-import json
-import os
 import subprocess
-import sys
 
 import numpy as np
 import pytest
 
-from conftest import ROOT, rel_err
-from test_fixed_cameras import MASK, fixed_entries
+from conftest import rel_err
+from objective_checks import CONFIGS, MASK, cfg_id, check_against_dense, check_two_rank_step, dense_system, fixed_entries, \
+    fixed_params, reduced
 
 pytestmark = pytest.mark.gpu
-
-# camera parameter columns (quat xyzw, t, f, k1, k2) held by each RBA_FIX_* bit
-_PARAM_COLS = {1: [0, 1, 2, 3, 4, 5, 6], 2: [7], 4: [8], 8: [9]}
-
-
-def fixed_params(flags):
-    """[nc, 10] bool: camera parameters that must stay bit-identical"""
-    out = np.zeros((len(flags), 10), bool)
-    for bit, cols in _PARAM_COLS.items():
-        out[np.ix_((flags & bit) != 0, cols)] = True
-    return out
 
 
 def _dense_case(nc=7, nl=90):
     from rootba_b200.synthetic import synth_bal
-    from test_oracle_dense_numpy import _dense_system, _reduced
     prob = synth_bal(nc, nl, 3.6, seed=21)
-    Jp, Jl, r = _dense_system(prob)
+    Jp, Jl, r = dense_system(prob)
     lam = 1e-3
-    return prob, lam, r, _reduced(Jp, Jl, r, lam, prob.nl, float(np.sqrt(1e-10)))
+    return prob, lam, r, reduced(Jp, Jl, r, lam, prob.nl)
 
 
-CONFIGS = [dict(solver_type="SQUARE_ROOT", operator_form=op, use_householder_marginalization=hh, preconditioner_type=pc)
-           for op in ("DENSE", "IMPLICIT") for hh in (True, False) for pc in ("JACOBI", "SCHUR_JACOBI")]
-CONFIGS += [dict(solver_type="SCHUR_COMPLEMENT"), dict(solver_type="POWER_SCHUR_COMPLEMENT")]
+@pytest.mark.parametrize("cfg", CONFIGS, ids=cfg_id)
+def test_f64_against_restricted_dense_system(cfg):
+    _check_restricted(cfg, 7, 90, {})
 
 
-@pytest.mark.parametrize("cfg", CONFIGS, ids=lambda c: "-".join(str(v) for v in c.values()))
-def test_f64_against_restricted_dense_system(cfg, monkeypatch):
-    _check_restricted(cfg, 7, 90, {}, monkeypatch)
-
-
-@pytest.mark.parametrize("cfg", CONFIGS, ids=lambda c: "-".join(str(v) for v in c.values()))
-def test_f64_uncached_vector_step_against_restricted_dense_system(cfg, monkeypatch):
+@pytest.mark.parametrize("cfg", CONFIGS, ids=cfg_id)
+def test_f64_uncached_vector_step_against_restricted_dense_system(cfg):
     """120 cameras with a one-CTA PCG vector kernel (RBA_PCG_CLUSTER=1): from 114 cameras on, its share of the vectors is no
     longer register-resident and it reads the camera-reduced operator output (DESIGN.md section 13)"""
-    _check_restricted(cfg, 120, 500, {"RBA_PCG_CLUSTER": "1"}, monkeypatch)
+    _check_restricted(cfg, 120, 500, {"RBA_PCG_CLUSTER": "1"})
 
 
-def _check_restricted(cfg, nc, nl, env, monkeypatch):
-    import rootba_b200 as rb
-    prob, lam, r, (D, sl, Jps, Jls, Minv, H, b) = _dense_case(nc, nl)
-    mask = np.resize(MASK, nc)
-    fixed = fixed_entries(mask)
-    free = ~fixed
-    bp = rb.BalProblem.from_arrays(prob, np.float64)
-    bp.camera_fixed = mask
-    so = rb.SolverOptions(eta=1e-13, **cfg)
-    with monkeypatch.context() as m:
-        for k, v in env.items():
-            m.setenv(k, v)
-        lin = rb.LinearizorQR.create(bp, so)
-    cams0 = bp.cams.copy()
-    lin.compute_error()
-    lin.linearize()
-    inc = lin.solve(lam)
-    assert rel_err(lin.get_rhs(), np.where(fixed, 0.0, b)) < 1e-9
-    assert np.all(inc[fixed] == 0)
-    Hff, bf = H[np.ix_(free, free)], b[free]
-    if cfg["solver_type"] == "POWER_SCHUR_COMPLEMENT":
-        # the series of k_power_vec on the restricted system: Hpp_ff^-1, E0_ff, the zeta rule, power_order terms at most
-        W = Jps.T @ Jls
-        E0 = (W @ Minv @ W.T)[np.ix_(free, free)]
-        Hinv = np.linalg.inv((Jps.T @ Jps + lam * np.eye(H.shape[0]))[np.ix_(free, free)])
-        tmp = -Hinv @ bf
-        acc = tmp.copy()
-        for i in range(1, so.power_order + 1):
-            tmp = Hinv @ (E0 @ tmp)
-            acc = acc + tmp
-            if i * np.linalg.norm(tmp) / np.linalg.norm(acc) < so.eta:
-                break
-        assert rel_err(inc[free], acc) < 1e-9
-    else:
-        assert lin.last_cg.termination_type == 1
-        assert rel_err(inc[free], -np.linalg.solve(Hff, bf)) < 1e-6
-    dl_s = -Minv @ (Jls.T @ r + Jls.T @ (Jps @ inc))
-    want_l = 0.5 * r @ r - 0.5 * np.sum((r + Jps @ inc + Jls @ dl_s) ** 2)
-    l_diff = lin.apply(None)  # the device-resident increment
-    assert abs(l_diff - want_l) <= 1e-8 * abs(want_l)
-    lin.download_state()
-    assert rel_err(bp.lms, prob.lms + (sl * dl_s).reshape(-1, 3)) < 1e-10
-    fp = fixed_params(mask)
-    assert np.array_equal(bp.cams[fp], cams0[fp])
-    assert not np.array_equal(bp.cams[~fp], cams0[~fp])
-    lin.close()
-
-
-def _lm_steps(arrays, dtype, solver_type, flags_mode, steps=3):
-    import rootba_b200 as rb
-    bp = rb.BalProblem.from_arrays(arrays, dtype)
-    lin = rb.LinearizorQR.create(bp, rb.SolverOptions(solver_type=solver_type))
-    if flags_mode == "zeros":
-        lin.set_camera_fixed(np.zeros(bp.num_cameras(), np.uint8))
-    elif flags_mode == "set_then_none":
-        lin.set_camera_fixed(np.full(bp.num_cameras(), rb.FIX_ALL, np.uint8))
-        lin.set_camera_fixed(None)
-    out = []
-    lin.compute_error()
-    for _ in range(steps):
-        lin.linearize()
-        inc = lin.solve(1e-4)
-        l_diff = lin.apply(None)
-        lin.download_state()
-        out.append((inc, l_diff, bp.cams.copy(), bp.lms.copy()))
-    lin.close()
-    return out
+def _check_restricted(cfg, nc, nl, env):
+    from rootba_b200.synthetic import synth_bal
+    check_against_dense(cfg, synth_bal(nc, nl, 3.6, seed=21), mask=np.resize(MASK, nc), env=env)
 
 
 @pytest.mark.parametrize("solver_type", ["SQUARE_ROOT", "SCHUR_COMPLEMENT"])
 @pytest.mark.parametrize("dtype", [np.float32, np.float64])
 def test_no_behaviour_change_without_flags(small_problem, dtype, solver_type):
-    ref = _lm_steps(small_problem, dtype, solver_type, "never")
+    import rootba_b200 as rb
+    from objective_checks import assert_identical_steps, lm_steps
+    opt = dict(solver_type=solver_type)
+    ref = lm_steps(small_problem, dtype, opt, "never")
     for mode in ("zeros", "set_then_none"):
-        got = _lm_steps(small_problem, dtype, solver_type, mode)
-        for (a, b) in zip(ref, got):
-            assert np.array_equal(a[0], b[0]) and a[1] == b[1], mode
-            assert np.array_equal(a[2], b[2]) and np.array_equal(a[3], b[3]), mode
+        got = lm_steps(small_problem, dtype, opt, mode, rb.LinearizorQR.set_camera_fixed,
+                       np.full(small_problem.nc, rb.FIX_ALL, np.uint8))
+        assert_identical_steps(ref, got, mode)
 
 
 def _run_flags(nc):
@@ -266,25 +185,8 @@ def test_bal_qr_fixed_matches_python_host(tmp_path, use_double):
     assert free["iterations"][-1]["cost"]["all"]["error"] != summ["iterations"][-1]["cost"]["all"]["error"]
 
 
-def _ngpu():
-    import torch
-    return torch.cuda.device_count() if torch.cuda.is_available() else 0
-
-
 @pytest.mark.parametrize("peer", ["1", "0"])
 @pytest.mark.parametrize("sfx", ["f32", "f64"])
 def test_two_ranks_with_fixed_cameras(tmp_path, peer, sfx):
-    if _ngpu() < 2:
-        pytest.skip("needs 2 GPUs")
-    out = tmp_path / "res.json"
-    env = dict(os.environ, RBA_PEER_AR=peer, MASTER_ADDR="127.0.0.1")
-    port = 27500 + (os.getpid() + (7 if peer == "1" else 0) + (13 if sfx == "f32" else 0)) % 2000
-    cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node", "2", "--master-addr", "127.0.0.1",
-           "--master-port", str(port), os.path.join(ROOT, "tests", "multirank_fixed_worker.py"), str(out), sfx]
-    r = subprocess.run(cmd, env=env, capture_output=True, text=True, timeout=200)
-    assert r.returncode == 0, r.stdout[-3000:] + r.stderr[-3000:]
-    res = json.loads(out.read_text())
-    tols = 1e-4 if sfx == "f32" else 1e-8  # the bars of test_gpu_multirank.py
-    assert res["replicas_identical"] and res["fixed_inc_zero"] and res["fixed_params_identical"], res
-    assert res["b"] < 4 * tols and res["inc"] < tols and res["l_diff"] < 20 * tols, res
-    assert res["lms"] < 10 * tols and res["cams"] < tols, res
+    res = check_two_rank_step(tmp_path, "fixed", sfx, peer, 27500, (7 if peer == "1" else 0) + (13 if sfx == "f32" else 0))
+    assert res["fixed_inc_zero"] and res["fixed_params_identical"], res

@@ -4,10 +4,6 @@ landmark with prior and prior-free landmarks in one tile, lambda = 0, rank-defic
 observation, no behaviour change without priors, bad input, an end-to-end minimum against scipy with every other prior
 kind and held cameras, covariances with the gauge fixed by landmark priors, and the sharded path."""
 import ctypes as C
-import json
-import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -16,114 +12,20 @@ import camera_model as cm
 import camera_prior_model as pm
 import landmark_prior_model as lp
 import pair_prior_model as qm
-from conftest import ROOT, rel_err
-from test_camera_prior_model import prior_case as camera_prior_case
-from test_fixed_cameras import fixed_entries
-from test_gpu_camera_priors import BARS, _ID, _ngpu, _reduced
-from test_gpu_fixed_cameras import CONFIGS, fixed_params
+from conftest import rel_err
+from objective_checks import CONFIGS, cfg_id, check_against_dense, check_two_rank_step, dense_system, fixed_entries, reduced
 
 pytestmark = pytest.mark.gpu
 
-# CONFIGS of test_gpu_fixed_cameras (SQUARE_ROOT dense / implicit x Householder / Givens x JACOBI / SCHUR_JACOBI, SC, Power-SC)
+# CONFIGS of objective_checks (SQUARE_ROOT dense / implicit x Householder / Givens x JACOBI / SCHUR_JACOBI, SC, Power-SC)
 # and the dense operator with stage2_form = IDENTITY (k_stage2<S, false>)
 CONFIGS_LMP = CONFIGS + [dict(solver_type="SQUARE_ROOT", operator_form="DENSE", use_householder_marginalization=hh,
                               preconditioner_type=pc, stage2_form="IDENTITY") for hh in (True, False) for pc in ("JACOBI", "SCHUR_JACOBI")]
 
 
-def _stored(prob, dtype):
-    """prob with its state and observations rounded to the handle's scalar type (compared in float64 from there)"""
-    from rootba_b200.synthetic import BalArrays
-    f = lambda a: np.asarray(np.asarray(a, dtype), np.float64)
-    return BalArrays(f(prob.cams), f(prob.lms), prob.lm_off, prob.obs_cam, f(prob.obs_xy))
-
-
-def _check_against_dense(cfg, prob, prior, dtype=np.float64, cam_prior=None, mask=None, lam=1e-3, env=None, monkeypatch=None):
-    import rootba_b200 as rb
-    from rootba_b200.synthetic import BalArrays
-    bars = BARS[dtype]
-    idx, mean, L = prior
-    sprior = (idx, np.asarray(np.asarray(mean, dtype), np.float64), np.asarray(np.asarray(L, dtype), np.float64))
-    sprob = _stored(prob, dtype)
-    Jp, Jl, r = lp.dense_system(sprob, sprior, cam_prior)
-    D, sl, Jps, Jls, Minv, H, b = _reduced(Jp, Jl, r, lam, prob.nl, dtype)
-    n = H.shape[0]
-    fixed = fixed_entries(mask) if mask is not None else np.zeros(n, bool)
-    free = ~fixed
-    bp = rb.BalProblem.from_arrays(prob, dtype)
-    bp.landmark_prior = prior
-    if cam_prior is not None:
-        bp.camera_prior = cam_prior
-    if mask is not None:
-        bp.camera_fixed = mask
-    so = rb.SolverOptions(eta=1e-13, **cfg)
-    if monkeypatch is not None:
-        with monkeypatch.context() as m:
-            for k, v in (env or {}).items():
-                m.setenv(k, v)
-            lin = rb.LinearizorQR.create(bp, so)
-    else:
-        lin = rb.LinearizorQR.create(bp, so)
-    cams0 = bp.cams.copy()
-    e0 = lin.compute_error()["all"]["error"]
-    assert abs(e0 - lp.total_cost(sprob, sprior, cam_prior)) <= bars["cost"] * e0
-    lin.linearize()
-    inc = lin.solve(lam)
-    s, _ = lin.get_jacobian_scaling()
-    assert rel_err(s, D) < bars["scaling"]
-    assert rel_err(lin.get_rhs(), np.where(fixed, 0.0, b)) < bars["b"]
-    inv, blk = lin.get_preconditioner()
-    power = cfg.get("solver_type") == "POWER_SCHUR_COMPLEMENT"
-    jacobi = power or cfg.get("preconditioner_type") == "JACOBI"
-    Hp = Jps.T @ Jps + lam * np.eye(n) if jacobi else H  # the landmark-prior rows have no camera columns
-    for c in range(prob.nc):
-        sel = slice(9 * c, 9 * c + 9)
-        f = free[sel]
-        want = np.zeros((9, 9))
-        want[np.ix_(f, f)] = np.linalg.inv(Hp[sel, sel][np.ix_(f, f)])
-        assert rel_err(inv[c], want) < bars["inv"], c
-        if not jacobi:
-            assert rel_err(blk[c], Hp[sel, sel]) < bars["blocks"], c
-    x = np.random.default_rng(1).uniform(-1, 1, n)
-    assert rel_err(lin.right_multiply(x), H @ x) < bars["op"]
-    assert np.all(inc[fixed] == 0)
-    Hff, bf = H[np.ix_(free, free)], b[free]
-    tol_inc = bars["inc"]
-    if dtype == np.float32:
-        tol_inc = max(tol_inc, 100 * 2.0 ** -24 * np.linalg.cond(Hff))  # as test_gpu_camera_priors
-    if power:
-        W = Jps.T @ Jls
-        E0 = (W @ Minv @ W.T)[np.ix_(free, free)]
-        Hinv = np.linalg.inv((Jps.T @ Jps + lam * np.eye(n))[np.ix_(free, free)])
-        tmp = -Hinv @ bf
-        acc = tmp.copy()
-        for i in range(1, so.power_order + 1):
-            tmp = Hinv @ (E0 @ tmp)
-            acc = acc + tmp
-            if i * np.linalg.norm(tmp) / np.linalg.norm(acc) < so.eta:
-                break
-        assert rel_err(inc[free], acc) < (1e-9 if dtype == np.float64 else tol_inc)
-    else:
-        if dtype == np.float64:
-            assert lin.last_cg.termination_type == 1
-            tol_inc = max(tol_inc, np.sqrt(so.eta * np.linalg.cond(Hff)))  # as test_gpu_pair_priors
-        assert rel_err(inc[free], -np.linalg.solve(Hff, bf)) < tol_inc
-    inc64 = np.asarray(inc, np.float64)
-    dl_s = -Minv @ (Jls.T @ r + Jls.T @ (Jps @ inc64))
-    want_l = 0.5 * r @ r - 0.5 * np.sum((r + Jps @ inc64 + Jls @ dl_s) ** 2)
-    l_diff = lin.apply(None)
-    assert abs(l_diff - want_l) <= bars["l_diff"] * abs(want_l)
-    lin.download_state()
-    want_lms = sprob.lms + (sl * dl_s).reshape(-1, 3)
-    assert rel_err(bp.lms, want_lms) < bars["lms"]
-    e1 = lin.compute_error()["all"]["error"]
-    new = BalArrays(bp.cams.astype(np.float64), bp.lms.astype(np.float64), prob.lm_off, prob.obs_cam, sprob.obs_xy)
-    want_e1 = lp.total_cost(new, sprior, cam_prior)
-    assert abs(e1 - want_e1) <= bars["cost"] * want_e1
-    if mask is not None:
-        fp = fixed_params(mask)
-        assert np.array_equal(bp.cams[fp], cams0[fp])
-    lin.close()
-    return dl_s, sl
+def _check(cfg, prob, prior, **kw):
+    """check_against_dense with landmark priors: in float64 the PCG increment bar widens to sqrt(eta kappa)"""
+    check_against_dense(cfg, prob, landmarks=prior, inc_eta_kappa=True, **kw)
 
 
 @pytest.fixture(scope="module")
@@ -133,34 +35,34 @@ def case7():
     return prob, lp.prior_case(prob.lms, every=3, seed=5)
 
 
-@pytest.mark.parametrize("cfg", CONFIGS_LMP, ids=_ID)
+@pytest.mark.parametrize("cfg", CONFIGS_LMP, ids=cfg_id)
 def test_f64_against_dense_system_with_landmark_priors(cfg, case7):
-    _check_against_dense(cfg, *case7)
+    _check(cfg, *case7)
 
 
-@pytest.mark.parametrize("cfg", CONFIGS_LMP, ids=_ID)
+@pytest.mark.parametrize("cfg", CONFIGS_LMP, ids=cfg_id)
 def test_f32_against_dense_system_with_landmark_priors(cfg, case7):
-    _check_against_dense(cfg, *case7, dtype=np.float32)
+    _check(cfg, *case7, dtype=np.float32)
 
 
-@pytest.mark.parametrize("cfg", CONFIGS_LMP, ids=_ID)
+@pytest.mark.parametrize("cfg", CONFIGS_LMP, ids=cfg_id)
 def test_f64_landmark_and_camera_priors_with_held_parameters(cfg):
     """with the camera priors of test_camera_prior_model.prior_case (an unobserved camera held by its prior) and a held
     camera"""
-    prob, mean_c, L_c = camera_prior_case(7, 90)
+    prob, mean_c, L_c = pm.prior_case(7, 90)
     mask = np.zeros(prob.nc, np.uint8)
     mask[2] = 15
     mask[4] = 14
-    _check_against_dense(cfg, prob, lp.prior_case(prob.lms, every=2, seed=8), cam_prior=(mean_c, L_c), mask=mask)
+    _check(cfg, prob, lp.prior_case(prob.lms, every=2, seed=8), camera=(mean_c, L_c), mask=mask)
 
 
-@pytest.mark.parametrize("cfg", [CONFIGS_LMP[i] for i in (0, 3, 5, 8, 9, 10)], ids=_ID)
+@pytest.mark.parametrize("cfg", [CONFIGS_LMP[i] for i in (0, 3, 5, 8, 9, 10)], ids=cfg_id)
 def test_lambda_zero_and_rank_one_priors(cfg):
     """lambda = 0: the prior landmarks' damping rows are [C | 0 | c] of L~ alone (the lambda = 0 shortcut must not skip
     them); height-only (rank-1) priors in the mix; the gauge fixed by camera priors"""
-    prob, mean_c, L_c = camera_prior_case(7, 90)
+    prob, mean_c, L_c = pm.prior_case(7, 90)
     prior = lp.prior_case(prob.lms, every=2, seed=9, kinds=("height", "dense", "height", "rank2"))
-    _check_against_dense(cfg, prob, prior, cam_prior=(mean_c, L_c), lam=0.0)
+    _check(cfg, prob, prior, camera=(mean_c, L_c), lam=0.0)
 
 
 # ---- every track-length class, landmark by landmark ---------------------------------------------------------------------
@@ -169,7 +71,7 @@ def _class_ns():
     return [n for n in CASES if n == 2 or _signature(n) != _signature(n - 1)]
 
 
-@pytest.mark.parametrize("cfg", [CONFIGS_LMP[i] for i in (0, 4, 12, 8)], ids=_ID)
+@pytest.mark.parametrize("cfg", [CONFIGS_LMP[i] for i in (0, 4, 12, 8)], ids=cfg_id)
 @pytest.mark.parametrize("n", _class_ns())
 def test_every_track_length_class_landmark_by_landmark(n, cfg):
     """W + 1 landmarks of track length n (one full tile, one ragged tile) with priors on every other landmark, so prior and
@@ -180,8 +82,8 @@ def test_every_track_length_class_landmark_by_landmark(n, cfg):
     prob = problem(n)
     prior = lp.prior_case(prob.lms, every=2, seed=n, sigma=0.02)
     lam = 1e-3
-    Jp, Jl, r = lp.dense_system(prob, prior)
-    D, sl, Jps, Jls, Minv, H, b = _reduced(Jp, Jl, r, lam, prob.nl, np.float64)
+    Jp, Jl, r = dense_system(prob, landmarks=prior)
+    D, sl, Jps, Jls, Minv, H, b = reduced(Jp, Jl, r, lam, prob.nl)
     bp = rb.BalProblem.from_arrays(prob, np.float64)
     bp.landmark_prior = prior
     lin = rb.LinearizorQR.create(bp, rb.SolverOptions(eta=1e-13, **cfg))
@@ -209,7 +111,7 @@ def _two_turned():
     return turn_cameras_around(a, [0, 1])
 
 
-@pytest.mark.parametrize("cfg", [CONFIGS_LMP[i] for i in (0, 4, 8, 9)], ids=_ID)
+@pytest.mark.parametrize("cfg", [CONFIGS_LMP[i] for i in (0, 4, 8, 9)], ids=cfg_id)
 def test_priors_on_landmarks_with_one_and_without_valid_observations(cfg):
     """ERROR_VALID: cameras 0 and 1 have no valid observation and are held; landmark 0 (rank-2 Jl) carries a height-only
     prior, landmark 1 (no valid row) a dense one.  Both are full rank only with their prior: the step is finite (no NaN
@@ -232,7 +134,7 @@ def test_priors_on_landmarks_with_one_and_without_valid_observations(cfg):
         Jl[2 * k:2 * k + 2, 3 * lm_of_obs[k]:3 * lm_of_obs[k] + 3] = jl[k]
     Jp, Jl, r = lp.append_rows((Jp, Jl, res.ravel()), nl, prob.lms, idx, mean, L)
     lam = 1e-3
-    D, sl, Jps, Jls, Minv, H, b = _reduced(Jp, Jl, r, lam, nl, np.float64)
+    D, sl, Jps, Jls, Minv, H, b = reduced(Jp, Jl, r, lam, nl)
     free = ~fixed_entries(mask)
     bp = rb.BalProblem.from_arrays(prob, np.float64)
     bp.landmark_prior = (idx, mean, L)
@@ -255,43 +157,18 @@ def test_priors_on_landmarks_with_one_and_without_valid_observations(cfg):
 
 
 # ---- no behaviour change without priors, bad input ---------------------------------------------------------------------
-def _lm_steps(arrays, dtype, cfg, mode, steps=3):
-    import rootba_b200 as rb
-    bp = rb.BalProblem.from_arrays(arrays, dtype)
-    lin = rb.LinearizorQR.create(bp, rb.SolverOptions(**cfg))
-    prior = lp.prior_case(arrays.lms, every=5, seed=2)
-    if mode == "set_then_none":
-        lin.set_landmark_prior(prior)
-        lin.set_landmark_prior(None)
-    elif mode == "set_then_empty":
-        lin.set_landmark_prior(prior)
-        lin.set_landmark_prior((np.zeros(0, np.int32), np.zeros((0, 3)), np.zeros((0, 3, 3))))
-    elif mode == "zeros":
-        lin.set_landmark_prior((prior[0], prior[1], np.zeros_like(prior[2])))
-    out = []
-    cost = lin.compute_error()["all"]["error"]
-    for _ in range(steps):
-        lin.linearize()
-        inc = lin.solve(1e-4)
-        l_diff = lin.apply(None)
-        lin.download_state()
-        out.append((inc, l_diff, bp.cams.copy(), bp.lms.copy(), lin.compute_error()["all"]["error"]))
-    lin.close()
-    return cost, out
-
-
-@pytest.mark.parametrize("cfg", [CONFIGS_LMP[i] for i in (0, 4, 12, 8, 9)], ids=_ID)
+@pytest.mark.parametrize("cfg", [CONFIGS_LMP[i] for i in (0, 4, 12, 8, 9)], ids=cfg_id)
 @pytest.mark.parametrize("dtype", [np.float32, np.float64])
 def test_no_behaviour_change_without_landmark_priors(small_problem, dtype, cfg):
     """priors set and cleared (None or num = 0), or all with a zero L: the LM trajectory of a handle that never had any, bit
     for bit"""
-    c0, ref = _lm_steps(small_problem, dtype, cfg, "never")
+    import rootba_b200 as rb
+    from objective_checks import assert_identical_steps, lm_steps
+    run = lambda mode: lm_steps(small_problem, dtype, cfg, mode, rb.LinearizorQR.set_landmark_prior,
+                                lp.prior_case(small_problem.lms, every=5, seed=2))
+    ref = run("never")
     for mode in ("set_then_none", "set_then_empty", "zeros"):
-        c1, got = _lm_steps(small_problem, dtype, cfg, mode)
-        assert c0 == c1, mode
-        for a, b in zip(ref, got):
-            assert np.array_equal(a[0], b[0]) and a[1] == b[1] and a[4] == b[4], mode
-            assert np.array_equal(a[2], b[2]) and np.array_equal(a[3], b[3]), mode
+        assert_identical_steps(ref, run(mode), mode)
 
 
 def test_bad_input_keeps_the_previous_landmark_priors(small_problem):
@@ -364,41 +241,13 @@ def _e2e_problem():
     return BalArrays(cams, lms, prob.lm_off, prob.obs_cam, prob.obs_xy), (idx, mean, L), (pairs, pmean, pL), (cmean, cL), mask
 
 
-def _scipy_minimum(prob, lmp, pair, camp, mask):
-    from scipy.optimize import least_squares
-    from scipy.spatial.transform import Rotation
-    nc, nl = prob.nc, prob.nl
-    free_c = np.flatnonzero(mask == 0)
-    lm_of_obs = np.repeat(np.arange(nl), np.diff(prob.lm_off))
-    base = np.asarray(prob.cams, np.float64)
-
-    def unpack(x):
-        pc = x[:9 * len(free_c)].reshape(-1, 9)
-        cams = base.copy()
-        cams[free_c, :4] = Rotation.from_rotvec(pc[:, :3]).as_quat()
-        cams[free_c, 4:7], cams[free_c, 7:10] = pc[:, 3:6], pc[:, 6:9]
-        return cams, x[9 * len(free_c):].reshape(nl, 3)
-
-    def fun(x):
-        cams, lms = unpack(x)
-        res = cm.linearize(cams[prob.obs_cam], lms[lm_of_obs], prob.obs_xy)["res"].ravel()
-        pri = [L @ (lms[i] - m) for i, m, L in zip(*lmp)]
-        pri += [pair[2][p] @ qm.residual(cams[i], cams[j], pair[1][p]) for p, (i, j) in enumerate(pair[0])]
-        pri += [camp[1][c] @ pm.residual(cams[c], camp[0][c]) for c in range(nc)]
-        return np.concatenate([res, np.concatenate(pri)])
-
-    x0 = np.concatenate([np.hstack([Rotation.from_quat(base[free_c, :4]).as_rotvec(), base[free_c, 4:10]]).ravel(), np.ravel(prob.lms)])
-    sol = least_squares(fun, x0, method="trf", x_scale="jac", xtol=1e-15, ftol=1e-15, gtol=1e-15, max_nfev=200)
-    cams, lms = unpack(sol.x)
-    return cams, lms, float(sol.cost)
-
-
 def test_lm_run_reaches_the_scipy_minimum_with_every_prior_kind_and_held_cameras():
     """the ground control points, the held camera and the camera prior fix the gauge, so the landmarks themselves are
     compared"""
     import rootba_b200 as rb
+    from objective_checks import scipy_minimum
     prob, lmp, pair, camp, mask = _e2e_problem()
-    _, lms_s, cost_s = _scipy_minimum(prob, lmp, pair, camp, mask)
+    _, lms_s, cost_s = scipy_minimum(prob, camera=camp, pairs=pair, landmarks=lmp, mask=mask)
     so = rb.SolverOptions(max_num_iterations=60, function_tolerance=1e-15, eta=1e-10)
     runs = {}
     for dtype in (np.float64, np.float32):
@@ -458,7 +307,7 @@ def test_covariance_with_the_gauge_fixed_by_landmark_priors_alone():
     lin = rb.LinearizorQR.create(bp, rb.SolverOptions())
     cam, lm = lin.covariance()
     lin.close()
-    Jp, Jl, _ = lp.dense_system(prob, prior)
+    Jp, Jl, _ = dense_system(prob, landmarks=prior)
     _dense_covariance_check(cam, lm, Jp, Jl, np.zeros(9 * prob.nc, bool))
     # without the priors the gauge is free
     bp2 = rb.BalProblem.from_arrays(prob, np.float64)
@@ -502,17 +351,5 @@ def test_covariance_of_a_rank2_landmark_with_a_prior_is_finite():
 @pytest.mark.parametrize("sfx", ["f32", "f64"])
 def test_two_ranks_with_landmark_priors(tmp_path, peer, sfx):
     """each shard adds its own landmark priors before the sum over the shards: the sharded step equals the single-rank step"""
-    if _ngpu() < 2:
-        pytest.skip("needs 2 GPUs")
-    out = tmp_path / "res.json"
-    env = dict(os.environ, RBA_PEER_AR=peer, MASTER_ADDR="127.0.0.1")
-    port = 29500 + (os.getpid() + (23 if peer == "1" else 0) + (29 if sfx == "f32" else 0)) % 2000
-    cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node", "2", "--master-addr", "127.0.0.1",
-           "--master-port", str(port), os.path.join(ROOT, "tests", "multirank_landmark_prior_worker.py"), str(out), sfx]
-    r = subprocess.run(cmd, env=env, capture_output=True, text=True, timeout=200)
-    assert r.returncode == 0, r.stdout[-3000:] + r.stderr[-3000:]
-    res = json.loads(out.read_text())
-    tols = 1e-4 if sfx == "f32" else 1e-8  # the bars of test_gpu_multirank.py
-    assert res["replicas_identical"] and min(res["priors_per_shard"]) > 0, res
-    assert res["b"] < 4 * tols and res["inc"] < tols and res["l_diff"] < 20 * tols, res
-    assert res["lms"] < 10 * tols and res["cams"] < tols and res["cost"] < tols and res["cost0"] < tols, res
+    res = check_two_rank_step(tmp_path, "landmark", sfx, peer, 29500, (23 if peer == "1" else 0) + (29 if sfx == "f32" else 0))
+    assert min(res["priors_per_shard"]) > 0, res

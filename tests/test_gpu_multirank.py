@@ -2,36 +2,18 @@
 through both exchange paths -- the peer-memory exchange over NVLink fused into the PCG kernels (default) and NCCL
 all-reduces (RBA_PEER_AR=0).  Skipped on a box with fewer than 2 GPUs."""
 import json
-import os
-import subprocess
-import sys
 
-import numpy as np
 import pytest
 
-from conftest import ROOT
+from objective_checks import run_two_ranks
 
 pytestmark = pytest.mark.gpu
-
-
-def _ngpu():
-    import torch
-    return torch.cuda.device_count() if torch.cuda.is_available() else 0
 
 
 @pytest.mark.parametrize("peer", ["1", "0"])
 @pytest.mark.parametrize("sfx", ["f32", "f64"])
 def test_two_ranks_against_oracle(tmp_path, peer, sfx):
-    if _ngpu() < 2:
-        pytest.skip("needs 2 GPUs")
-    out = tmp_path / "res.json"
-    env = dict(os.environ, RBA_PEER_AR=peer, MASTER_ADDR="127.0.0.1")
-    port = 29500 + (os.getpid() + (7 if peer == "1" else 0) + (13 if sfx == "f32" else 0)) % 2000
-    cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node", "2", "--master-addr", "127.0.0.1",
-           "--master-port", str(port), os.path.join(ROOT, "tests", "multirank_gpu_worker.py"), str(out), sfx]
-    r = subprocess.run(cmd, env=env, capture_output=True, text=True, timeout=200)
-    assert r.returncode == 0, r.stdout[-3000:] + r.stderr[-3000:]
-    res = json.loads(out.read_text())
+    res = run_two_ranks(tmp_path, "multirank_gpu_worker.py", sfx, peer, 29500, (7 if peer == "1" else 0) + (13 if sfx == "f32" else 0))
     tol1, tols, tolb = (1e-5, 1e-4, 1e-4) if sfx == "f32" else (1e-11, 1e-8, 1e-8)
     print("multirank result", json.dumps(res))
     assert res["cams_without_obs_here"] > 0, res

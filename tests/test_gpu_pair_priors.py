@@ -3,103 +3,20 @@ float64 algebra of the total (reprojection + pair prior) problem, with absolute 
 PCG iterates, no behaviour change without pair priors, an observation-free camera, an end-to-end minimum against scipy, bad
 input and the sharded path."""
 import ctypes as C
-import json
-import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
 
-import camera_model as cm
 import camera_prior_model as pm
 import pair_prior_model as qm
-from conftest import ROOT, rel_err
-from test_camera_prior_model import prior_case
-from test_fixed_cameras import MASK, fixed_entries
-from test_gpu_camera_priors import BARS, _ID, _ngpu, _reduced, _small_prior
-from test_gpu_fixed_cameras import CONFIGS, fixed_params
+from objective_checks import CONFIGS, MASK, cfg_id, check_against_dense, check_two_rank_step
 
 pytestmark = pytest.mark.gpu
 
 
-def _check_against_dense(cfg, prob, pair, env, monkeypatch, dtype=np.float64, mask=None, absp=None):
-    import rootba_b200 as rb
-    from rootba_b200.synthetic import BalArrays
-    bars = BARS[dtype]
-    lam = 1e-3
-    Jp, Jl, r = qm.dense_system_with_pairs(prob, pair, absp)
-    D, sl, Jps, Jls, Minv, H, b = _reduced(Jp, Jl, r, lam, prob.nl, dtype)
-    n = H.shape[0]
-    fixed = fixed_entries(mask) if mask is not None else np.zeros(n, bool)
-    free = ~fixed
-    bp = rb.BalProblem.from_arrays(prob, dtype)
-    bp.camera_pair_prior = pair
-    if absp is not None:
-        bp.camera_prior = absp
-    if mask is not None:
-        bp.camera_fixed = mask
-    so = rb.SolverOptions(eta=1e-13, **cfg)
-    with monkeypatch.context() as m:
-        for k, v in env.items():
-            m.setenv(k, v)
-        lin = rb.LinearizorQR.create(bp, so)
-    cams0 = bp.cams.copy()
-    e0 = lin.compute_error()["all"]["error"]
-    assert abs(e0 - qm.total_cost(prob, pair, absp)) <= bars["cost"] * e0
-    lin.linearize()
-    inc = lin.solve(lam)
-    s, _ = lin.get_jacobian_scaling()
-    assert rel_err(s, D) < bars["scaling"]
-    assert rel_err(lin.get_rhs(), np.where(fixed, 0.0, b)) < bars["b"]
-    inv, blk = lin.get_preconditioner()
-    power = cfg.get("solver_type") == "POWER_SCHUR_COMPLEMENT"
-    jacobi = power or cfg.get("preconditioner_type") == "JACOBI"
-    Hpp, O = qm.power_split(Jps, lam)  # Hpp: the JACOBI blocks with the pairs' diagonal blocks
-    for c in range(prob.nc):
-        sel = slice(9 * c, 9 * c + 9)
-        Hc = Hpp[sel, sel] if jacobi else H[sel, sel]
-        f = free[sel]
-        want = np.zeros((9, 9))
-        want[np.ix_(f, f)] = np.linalg.inv(Hc[np.ix_(f, f)])
-        assert rel_err(inv[c], want) < bars["inv"], c
-        if not jacobi:  # the blocks are written with SCHUR_JACOBI (rba_get_preconditioner)
-            assert rel_err(blk[c], H[sel, sel]) < bars["blocks"], c
-    # the full operator, off-diagonal pair blocks included
-    assert np.max(np.abs(O)) > 0
-    x = np.random.default_rng(1).uniform(-1, 1, n)
-    assert rel_err(lin.right_multiply(x), H @ x) < bars["op"]
-    assert np.all(inc[fixed] == 0)
-    Hff, bf = H[np.ix_(free, free)], b[free]
-    tol_inc = bars["inc"]
-    if dtype == np.float32:
-        tol_inc = max(tol_inc, 100 * 2.0 ** -24 * np.linalg.cond(Hff))  # as test_gpu_camera_priors
-    if power:
-        # the series of k_power_vec on Hpp^-1 (E_0 - O), E_0 - O = Hpp - H, on the free entries
-        acc = qm.power_series(Hpp[np.ix_(free, free)], (Hpp - H)[np.ix_(free, free)], bf, so.power_order, so.eta)
-        assert rel_err(inc[free], acc) < (1e-9 if dtype == np.float64 else tol_inc)
-    else:
-        if dtype == np.float64:
-            assert lin.last_cg.termination_type == 1
-            # the stopping test bounds the change of the quadratic model, which is second order in the error of the
-            # iterate: a converged increment is accurate to about sqrt(eta kappa), above the bar for some configurations
-            tol_inc = max(tol_inc, np.sqrt(so.eta * np.linalg.cond(Hff)))
-        assert rel_err(inc[free], -np.linalg.solve(Hff, bf)) < tol_inc
-    inc64 = np.asarray(inc, np.float64)
-    dl_s = -Minv @ (Jls.T @ r + Jls.T @ (Jps @ inc64))
-    want_l = 0.5 * r @ r - 0.5 * np.sum((r + Jps @ inc64 + Jls @ dl_s) ** 2)
-    l_diff = lin.apply(None)
-    assert abs(l_diff - want_l) <= bars["l_diff"] * abs(want_l)
-    lin.download_state()
-    assert rel_err(bp.lms, prob.lms + (sl * dl_s).reshape(-1, 3)) < bars["lms"]
-    e1 = lin.compute_error()["all"]["error"]
-    want_e1 = qm.total_cost(BalArrays(bp.cams.astype(np.float64), bp.lms.astype(np.float64), prob.lm_off, prob.obs_cam, prob.obs_xy),
-                            pair, absp)
-    assert abs(e1 - want_e1) <= bars["cost"] * want_e1
-    if mask is not None:
-        fp = fixed_params(mask)
-        assert np.array_equal(bp.cams[fp], cams0[fp])
-    lin.close()
+def _check(cfg, prob, pair, **kw):
+    """check_against_dense with pair priors: in float64 the PCG increment bar widens to sqrt(eta kappa)"""
+    check_against_dense(cfg, prob, pairs=pair, inc_eta_kappa=True, **kw)
 
 
 @pytest.fixture(scope="module")
@@ -112,41 +29,38 @@ def case120():
     return qm.pair_case(120, 500, seed=5)
 
 
-@pytest.mark.parametrize("cfg", CONFIGS, ids=_ID)
-def test_f64_against_dense_system_with_pair_priors(cfg, case7, monkeypatch):
-    _check_against_dense(cfg, *case7, {}, monkeypatch)
+@pytest.mark.parametrize("cfg", CONFIGS, ids=cfg_id)
+def test_f64_against_dense_system_with_pair_priors(cfg, case7):
+    _check(cfg, *case7)
 
 
 @pytest.mark.parametrize("env", [{"RBA_PCG_CLUSTER": "1"}, {"RBA_PCG_PARTIALS": "0"}], ids=["one-cta", "no-partials"])
-@pytest.mark.parametrize("cfg", CONFIGS, ids=_ID)
-def test_f64_120_cameras_against_dense_system_with_pair_priors(cfg, env, case120, monkeypatch):
+@pytest.mark.parametrize("cfg", CONFIGS, ids=cfg_id)
+def test_f64_120_cameras_against_dense_system_with_pair_priors(cfg, env, case120):
     """RBA_PCG_CLUSTER=1: 120 cameras leave the register-resident layout of the vector step (its uncached path)"""
-    _check_against_dense(cfg, *case120, env, monkeypatch)
+    _check(cfg, *case120, env=env)
 
 
-@pytest.mark.parametrize("cfg", [CONFIGS[0], CONFIGS[2], CONFIGS[5], CONFIGS[8], CONFIGS[9]], ids=_ID)
-def test_f32_against_dense_system_with_pair_priors(cfg, case7, monkeypatch):
-    _check_against_dense(cfg, *case7, {}, monkeypatch, dtype=np.float32)
+@pytest.mark.parametrize("cfg", [CONFIGS[0], CONFIGS[2], CONFIGS[5], CONFIGS[8], CONFIGS[9]], ids=cfg_id)
+def test_f32_against_dense_system_with_pair_priors(cfg, case7):
+    _check(cfg, *case7, dtype=np.float32)
 
 
-@pytest.mark.parametrize("cfg", CONFIGS, ids=_ID)
-def test_f64_pair_and_absolute_priors_against_dense_system(cfg, case7, monkeypatch):
+@pytest.mark.parametrize("cfg", CONFIGS, ids=cfg_id)
+def test_f64_pair_and_absolute_priors_against_dense_system(cfg, case7):
     prob, pair = case7
-    _, mean_a, L_a = prior_case(7, 90)
-    _check_against_dense(cfg, prob, pair, {}, monkeypatch, absp=(mean_a, L_a))
+    _, mean_a, L_a = pm.prior_case(7, 90)
+    _check(cfg, prob, pair, camera=(mean_a, L_a))
 
 
-@pytest.mark.parametrize("cfg", CONFIGS, ids=_ID)
-def test_f64_pair_priors_with_held_parameters_against_restricted_dense_system(cfg, case7, monkeypatch):
+@pytest.mark.parametrize("cfg", CONFIGS, ids=cfg_id)
+def test_f64_pair_priors_with_held_parameters_against_restricted_dense_system(cfg, case7):
     """MASK holds every parameter of camera 3, which pairs (2, 3) and (3, 4) join to free cameras"""
     prob = case7[0]
-    _check_against_dense(cfg, *case7, {}, monkeypatch, mask=np.resize(MASK, prob.nc))
+    _check(cfg, *case7, mask=np.resize(MASK, prob.nc))
 
 
 # ---- truncated PCG iterates -------------------------------------------------------------------------------------------
-K_TRUNC = 8
-
-
 @pytest.fixture(scope="module")
 def seq_pairs():
     from rootba_b200.synthetic import synth_config
@@ -160,43 +74,13 @@ def seq_pairs():
     return arrays, (pairs, mean, L)
 
 
-def _pair_handle(arrays, pair, dtype, **opt):
-    import rootba_b200 as rb
-    bp = rb.BalProblem.from_arrays(arrays, dtype)
-    bp.camera_pair_prior = pair
-    lin = rb.LinearizorQR.create(bp, rb.SolverOptions(**opt))
-    lin.linearize()
-    return lin
-
-
 @pytest.mark.parametrize("operator_form", ["DENSE", "IMPLICIT"])
 @pytest.mark.parametrize("precond", ["JACOBI", "SCHUR_JACOBI"])
 def test_pcg_truncated_iterates_with_pair_priors(seq_pairs, operator_form, precond):
-    """pcg_replay on the handle's own b, M^-1 and right_multiply (which includes the off-diagonal pair blocks): iterates
-    k = 1..8 at the bar of test_gpu_pcg_iterates (10 k u kappa)"""
-    from pcg_replay import NO_CONVERGENCE, lanczos_condition, pcg_replay
-    from test_gpu_pcg_iterates import C_BAR, NEVER, U
+    """the replay's operator includes the off-diagonal pair blocks"""
+    from objective_checks import check_truncated_pcg_iterates
     arrays, pair = seq_pairs
-    opt = dict(operator_form=operator_form, preconditioner_type=precond)
-    lam = 1e-3
-    lin = _pair_handle(arrays, pair, np.float64, **opt)
-    lin.solve(lam)
-    b, inv = lin.get_rhs(), lin.get_preconditioner()[0]
-    op = lambda v: lin.right_multiply(np.asarray(v, np.float64))
-    full = pcg_replay(op, b, inv, eta=0.0, max_it=600)
-    lmin, lmax = lanczos_condition(full["alphas"], full["betas"])
-    bars = [C_BAR * max(k, 1) * U[np.float64] * lmax / lmin for k in range(K_TRUNC + 1)]
-    assert full["iterations"] >= K_TRUNC and bars[K_TRUNC] <= 1e-8
-    ref = pcg_replay(op, b, inv, eta=NEVER, max_it=K_TRUNC)
-    lin.close()
-    for k in range(1, K_TRUNC + 1):
-        assert rel_err(ref["xs"][k], ref["xs"][k - 1]) > 100 * bars[k], k
-        h = _pair_handle(arrays, pair, np.float64, eta=NEVER, max_linear_solver_iterations=k, **opt)
-        inc = h.solve(lam)
-        assert np.array_equal(h.get_rhs(), b) and np.array_equal(h.get_preconditioner()[0], inv), k
-        assert (h.last_cg.termination_type, h.last_cg.num_iterations) == (NO_CONVERGENCE, k)
-        assert rel_err(inc, -ref["xs"][k]) < bars[k], (k, rel_err(inc, -ref["xs"][k]), bars[k])
-        h.close()
+    check_truncated_pcg_iterates(arrays, operator_form, precond, camera_pair_prior=pair)
 
 
 # ---- no behaviour change without pair priors ----------------------------------------------------------------------------
@@ -209,43 +93,19 @@ def _chain_pairs(problem, seed=4):
     return pairs, mean, L
 
 
-def _lm_steps(arrays, dtype, solver_type, mode, absolute=False, steps=3):
-    import rootba_b200 as rb
-    bp = rb.BalProblem.from_arrays(arrays, dtype)
-    if absolute:
-        bp.camera_prior = _small_prior(arrays)
-    lin = rb.LinearizorQR.create(bp, rb.SolverOptions(solver_type=solver_type))
-    if mode == "set_then_none":
-        lin.set_camera_pair_prior(_chain_pairs(arrays))
-        lin.set_camera_pair_prior(None)
-    elif mode == "zeros":
-        pairs, mean, L = _chain_pairs(arrays)
-        lin.set_camera_pair_prior((pairs, mean, np.zeros_like(L)))
-    out = []
-    cost = lin.compute_error()["all"]["error"]
-    for _ in range(steps):
-        lin.linearize()
-        inc = lin.solve(1e-4)
-        l_diff = lin.apply(None)
-        lin.download_state()
-        out.append((inc, l_diff, bp.cams.copy(), bp.lms.copy(), lin.compute_error()["all"]["error"]))
-    lin.close()
-    return cost, out
-
-
 @pytest.mark.parametrize("absolute", [False, True], ids=["no-priors", "absolute-priors"])
 @pytest.mark.parametrize("solver_type", ["SQUARE_ROOT", "SCHUR_COMPLEMENT", "POWER_SCHUR_COMPLEMENT"])
 @pytest.mark.parametrize("dtype", [np.float32, np.float64])
 def test_no_behaviour_change_without_pair_priors(small_problem, dtype, solver_type, absolute):
     """pair priors set and cleared, or all with a zero L: the LM trajectory of a handle that never had any, bit for bit
     (with and without absolute priors)"""
-    c0, ref = _lm_steps(small_problem, dtype, solver_type, "never", absolute)
+    import rootba_b200 as rb
+    from objective_checks import assert_identical_steps, lm_steps
+    run = lambda mode: lm_steps(small_problem, dtype, dict(solver_type=solver_type), mode, rb.LinearizorQR.set_camera_pair_prior,
+                                _chain_pairs(small_problem), camera_prior=pm.small_prior(small_problem) if absolute else None)
+    ref = run("never")
     for mode in ("set_then_none", "zeros"):
-        c1, got = _lm_steps(small_problem, dtype, solver_type, mode, absolute)
-        assert c0 == c1, mode
-        for a, b in zip(ref, got):
-            assert np.array_equal(a[0], b[0]) and a[1] == b[1] and a[4] == b[4], mode
-            assert np.array_equal(a[2], b[2]) and np.array_equal(a[3], b[3]), mode
+        assert_identical_steps(ref, run(mode), mode)
 
 
 # ---- an observation-free camera ---------------------------------------------------------------------------------------
@@ -301,38 +161,13 @@ def _e2e_problem():
     return BalArrays(cams, lms, prob.lm_off, prob.obs_cam, prob.obs_xy), (pairs, mean, L)
 
 
-def _scipy_minimum(prob, pair):
-    from scipy.optimize import least_squares
-    from scipy.spatial.transform import Rotation
-    nc, nl = prob.nc, prob.nl
-    pairs, mean, L = pair
-    lm_of_obs = np.repeat(np.arange(nl), np.diff(prob.lm_off))
-
-    def unpack(x):
-        pc = x[:9 * nc].reshape(nc, 9)
-        cams = np.zeros((nc, 10))
-        cams[:, :4] = Rotation.from_rotvec(pc[:, :3]).as_quat()
-        cams[:, 4:7], cams[:, 7:10] = pc[:, 3:6], pc[:, 6:9]
-        return cams, x[9 * nc:].reshape(nl, 3)
-
-    def fun(x):
-        cams, lms = unpack(x)
-        res = cm.linearize(cams[prob.obs_cam], lms[lm_of_obs], prob.obs_xy)["res"].ravel()
-        pri = np.concatenate([L[p] @ qm.residual(cams[i], cams[j], mean[p]) for p, (i, j) in enumerate(pairs)])
-        return np.concatenate([res, pri])
-
-    x0 = np.concatenate([np.hstack([Rotation.from_quat(prob.cams[:, :4]).as_rotvec(), prob.cams[:, 4:10]]).ravel(), np.ravel(prob.lms)])
-    sol = least_squares(fun, x0, method="trf", x_scale="jac", xtol=1e-15, ftol=1e-15, gtol=1e-15, max_nfev=200)
-    cams, lms = unpack(sol.x)
-    return cams, lms, float(sol.cost)
-
-
 def test_lm_run_reaches_the_scipy_minimum_of_the_total_objective():
     """the cost at the minimum is gauge-free; the relative poses of the pairs are compared (the pair priors and reprojections
     leave the similarity gauge free, so absolute poses may differ between the two solvers)"""
     import rootba_b200 as rb
+    from objective_checks import scipy_minimum
     prob, pair = _e2e_problem()
-    cams_s, _, cost_s = _scipy_minimum(prob, pair)
+    cams_s, _, cost_s = scipy_minimum(prob, pairs=pair)
     so = rb.SolverOptions(max_num_iterations=60, function_tolerance=1e-15, eta=1e-10)
     runs = {}
     for dtype in (np.float64, np.float32):
@@ -355,23 +190,9 @@ def test_lm_run_reaches_the_scipy_minimum_of_the_total_objective():
 
 def test_lm_run_with_pair_priors_equals_the_python_host_loop():
     import rootba_b200 as rb
+    from objective_checks import check_lm_run_equals_host_loop
     prob, pair = _e2e_problem()
-    so = rb.SolverOptions(max_num_iterations=10)
-    bp = rb.BalProblem.from_arrays(prob, np.float64)
-    bp.camera_pair_prior = pair
-    lin = rb.LinearizorQR.create(bp, so)
-    its, _, _ = lin.lm_run(64)
-    lin.download_state()
-    lin.close()
-    bp2 = rb.BalProblem.from_arrays(prob, np.float64)
-    bp2.camera_pair_prior = pair
-    summ = rb.bundle_adjust_manual(bp2, so)
-    host = summ["iterations"][1:]
-    assert len(host) == len(its) and len(its) >= 2
-    for h, n in zip(host, its):
-        assert bool(h["step_is_successful"]) == n["accepted"] and h["lam"] == n["lambda"]
-        assert h["linear_solver_iterations"] == n["cg_iterations"] and h["cost"]["all"]["error"] == n["cost"]
-    assert np.array_equal(bp2.cams, bp.cams) and np.array_equal(bp2.lms, bp.lms)
+    check_lm_run_equals_host_loop(prob, rb.SolverOptions(max_num_iterations=10), camera_pair_prior=pair)
 
 
 # ---- bad input --------------------------------------------------------------------------------------------------------
@@ -425,17 +246,4 @@ def test_bad_input_keeps_the_previous_pair_priors(small_problem):
 @pytest.mark.parametrize("sfx", ["f32", "f64"])
 def test_two_ranks_with_pair_priors(tmp_path, peer, sfx):
     """every pair term is added once, after the sum over the shards: the sharded step equals the single-rank step"""
-    if _ngpu() < 2:
-        pytest.skip("needs 2 GPUs")
-    out = tmp_path / "res.json"
-    env = dict(os.environ, RBA_PEER_AR=peer, MASTER_ADDR="127.0.0.1")
-    port = 29500 + (os.getpid() + (11 if peer == "1" else 0) + (17 if sfx == "f32" else 0)) % 2000
-    cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node", "2", "--master-addr", "127.0.0.1",
-           "--master-port", str(port), os.path.join(ROOT, "tests", "multirank_pair_worker.py"), str(out), sfx]
-    r = subprocess.run(cmd, env=env, capture_output=True, text=True, timeout=200)
-    assert r.returncode == 0, r.stdout[-3000:] + r.stderr[-3000:]
-    res = json.loads(out.read_text())
-    tols = 1e-4 if sfx == "f32" else 1e-8  # the bars of test_gpu_multirank.py
-    assert res["replicas_identical"], res
-    assert res["b"] < 4 * tols and res["inc"] < tols and res["l_diff"] < 20 * tols, res
-    assert res["lms"] < 10 * tols and res["cams"] < tols and res["cost"] < tols and res["cost0"] < tols, res
+    check_two_rank_step(tmp_path, "pair", sfx, peer, 29500, (11 if peer == "1" else 0) + (17 if sfx == "f32" else 0))

@@ -32,7 +32,7 @@ import pytest
 
 from conftest import rel_err
 from pcg_replay import NO_CONVERGENCE, SUCCESS, lanczos_condition, pcg_replay, power_replay
-from test_fixed_cameras import MASK, fixed_entries
+from objective_checks import MASK, fixed_entries
 from test_pcg_replay import zeta_gap
 
 pytestmark = pytest.mark.gpu
@@ -252,7 +252,7 @@ def test_check_period_does_not_change_results(seq_problem, dtype, solver_type):
 
 @pytest.mark.parametrize("dtype", [np.float32, np.float64])
 def test_pcg_with_held_cameras(seq_problem, dtype):
-    """the replay on the masked b and M^-1 of test_fixed_cameras.MASK (on the first cameras); held entries exactly 0"""
+    """the replay on the masked b and M^-1 of objective_checks.MASK (on the first cameras); held entries exactly 0"""
     mask = np.zeros(seq_problem.nc, np.uint8)
     mask[:MASK.size] = MASK
     fixed = fixed_entries(mask)

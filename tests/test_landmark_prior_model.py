@@ -5,6 +5,7 @@ import numpy as np
 import pytest
 
 import landmark_prior_model as lp
+from objective_checks import dense_system, total_cost
 
 EPS = 1e-5  # the float64 Jacobi-scaling epsilon
 
@@ -18,14 +19,14 @@ def case():
 
 def _cost_at(prob, lms, prior):
     from rootba_b200.synthetic import BalArrays
-    return lp.total_cost(BalArrays(prob.cams, lms, prob.lm_off, prob.obs_cam, prob.obs_xy), prior)
+    return total_cost(BalArrays(prob.cams, lms, prob.lm_off, prob.obs_cam, prob.obs_xy), landmarks=prior)
 
 
 def test_landmark_jacobian_of_the_total_objective_matches_central_differences(case):
     """the gradient J^T r of the dense system (reprojection + prior rows) in the landmark columns against central differences
     of the total cost"""
     prob, prior = case
-    Jp, Jl, r = lp.dense_system(prob, prior)
+    Jp, Jl, r = dense_system(prob, landmarks=prior)
     grad = Jl.T @ r
     h = 1e-6
     for l in list(prior[0][:4]) + [1, 3]:
@@ -51,12 +52,12 @@ def test_dense_lm_step_predicts_the_true_cost_change(case):
     from rootba_b200.synthetic import BalArrays
     import camera_prior_model as pm
     prob, prior = case
-    Jp, Jl, r = lp.dense_system(prob, prior)
+    Jp, Jl, r = dense_system(prob, landmarks=prior)
     dp, dl, l_diff, D, sl = lp.lm_step(Jp, Jl, r, 1e-6, EPS)
     step = 1e-3
     cams = np.array([pm.apply_inc(prob.cams[c], step * D[9 * c:9 * c + 9] * dp[9 * c:9 * c + 9]) for c in range(prob.nc)])
     lms = np.asarray(prob.lms, np.float64) + step * (sl * dl).reshape(-1, 3)
-    true = lp.total_cost(prob, prior) - lp.total_cost(BalArrays(cams, lms, prob.lm_off, prob.obs_cam, prob.obs_xy), prior)
+    true = total_cost(prob, landmarks=prior) - total_cost(BalArrays(cams, lms, prob.lm_off, prob.obs_cam, prob.obs_xy), landmarks=prior)
     Js = np.hstack([Jp * D, Jl * sl])
     d = np.concatenate([dp, dl])
     model = -(step * (Js @ d) @ r + 0.5 * step ** 2 * np.sum((Js @ d) ** 2))
@@ -66,7 +67,7 @@ def test_dense_lm_step_predicts_the_true_cost_change(case):
 
 def test_prior_columns_enter_the_jacobi_scaling(case):
     prob, prior = case
-    Jp, Jl, r = lp.dense_system(prob, prior)
+    Jp, Jl, r = dense_system(prob, landmarks=prior)
     from test_oracle_dense_numpy import _dense_system
     _, Jl0, _ = _dense_system(prob)
     idx, _, L = prior
@@ -129,7 +130,7 @@ def test_fold_checker_rejects_planted_faults(fault):
 def test_scaling_checker_rejects_L_without_the_landmark_scaling(case):
     """the step from the prior rows scaled by diag(jls) is the model's; one with L taken as is in the scaled space is not"""
     prob, prior = case
-    Jp, Jl, r = lp.dense_system(prob, prior)
+    Jp, Jl, r = dense_system(prob, landmarks=prior)
     lam = 1e-3
     dp, dl, l_diff, D, sl = lp.lm_step(Jp, Jl, r, lam, EPS)
     # the faulty variant: the reprojection part scaled, the prior rows' landmark columns not

@@ -64,23 +64,23 @@ def test_first_order_model_of_the_total_objective_predicts_the_true_cost_change(
     """the dense LM step of reprojection + absolute + pair rows (scaling over the whole Jacobian, H, b, inc, l_diff): for a
     heavily damped step the model decrease matches the true decrease of the total cost"""
     from rootba_b200.synthetic import BalArrays
-    from test_camera_prior_model import prior_case
+    from objective_checks import dense_system, total_cost
     from test_oracle_dense_numpy import _reduced
     prob, pair = qm.pair_case()
-    _, mean_a, L_a = prior_case(7, 90)
+    _, mean_a, L_a = pm.prior_case(7, 90)
     absp = (pm.mean_at(prob.cams), L_a)
-    Jp, Jl, r = qm.dense_system_with_pairs(prob, pair, absp)
+    Jp, Jl, r = dense_system(prob, camera=absp, pairs=pair)
     lam = 1e4
     D, sl, Jps, Jls, Minv, H, b = _reduced(Jp, Jl, r, lam, prob.nl, float(np.sqrt(1e-10)))
     inc = -np.linalg.solve(H, b)
     dl_s = -Minv @ (Jls.T @ r + Jls.T @ (Jps @ inc))
     l_diff = 0.5 * r @ r - 0.5 * np.sum((r + Jps @ inc + Jls @ dl_s) ** 2)
-    e0 = qm.total_cost(prob, pair, absp)
+    e0 = total_cost(prob, camera=absp, pairs=pair)
     assert 0.5 * r @ r == pytest.approx(e0, rel=1e-12)
     d = (D * inc).reshape(-1, 9)
     cams1 = np.stack([pm.apply_inc(prob.cams[c], d[c]) for c in range(prob.nc)])
     lms1 = np.asarray(prob.lms) + (sl * dl_s).reshape(-1, 3)
-    e1 = qm.total_cost(BalArrays(cams1, lms1, prob.lm_off, prob.obs_cam, prob.obs_xy), pair, absp)
+    e1 = total_cost(BalArrays(cams1, lms1, prob.lm_off, prob.obs_cam, prob.obs_xy), camera=absp, pairs=pair)
     assert l_diff > 0 and e0 > e1
     assert (e0 - e1) / l_diff == pytest.approx(1.0, abs=5e-2)
 
@@ -90,11 +90,12 @@ def test_first_order_model_of_the_total_objective_predicts_the_true_cost_change(
 def test_power_series_on_E0_minus_O_converges_to_the_direct_solve(seed, lam):
     """Hpp - (E_0 - O) and Hpp + (E_0 - O) are both positive definite, so the eigenvalues of Hpp^-1 (E_0 - O) lie in (-1, 1)
     and the series reaches the solve of the total reduced system"""
+    from objective_checks import dense_system
     from test_oracle_dense_numpy import _reduced
     rng = np.random.default_rng(100 + seed)
     prob, (pairs, mean, L) = qm.pair_case(6 + seed % 3, 70, seed=200 + seed)
     L = L * rng.uniform(0.5, 20.0)  # weak to strong pair priors
-    Jp, Jl, r = qm.dense_system_with_pairs(prob, (pairs, mean, L))
+    Jp, Jl, r = dense_system(prob, pairs=(pairs, mean, L))
     D, sl, Jps, Jls, Minv, H, b = _reduced(Jp, Jl, r, lam, prob.nl, float(np.sqrt(1e-10)))
     Hpp, O = qm.power_split(Jps, lam)
     assert np.max(np.abs(O)) > 0
