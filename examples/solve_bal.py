@@ -3,7 +3,7 @@
 
     python examples/solve_bal.py problem-49-7776-pre.txt [--float] [--max-num-iterations 20] [--operator-form DENSE|IMPLICIT]
         [--fix-intrinsics] [--fix-cameras I,J,...] [--camera-prior FILE.npz] [--camera-pair-prior FILE.npz]
-        [--landmark-prior FILE.npz] [--covariance OUT.npz]
+        [--landmark-prior FILE.npz] [--shared-intrinsics | --intrinsics-groups FILE.npy] [--covariance OUT.npz]
 
 Mirrors what `bal_qr --input ...` of the reference does (src/app/bal_qr.cpp): load + normalise (bal_problem.cpp:773-852),
 optimize_lm_ours with the QR linearizor (solver/bal_bundle_adjustment.cpp:249-544), log (bal/ba_log.hpp)."""
@@ -41,6 +41,12 @@ def main():
     ap.add_argument("--landmark-prior", default=None, metavar="FILE.npz",
                     help="Gaussian priors on landmark positions (e.g. ground control points): arrays `idx` [m], `mean` [m, 3] and "
                          "`sqrt_info` [m, 3, 3] in the coordinates of the loaded (normalised) problem (DESIGN.md section 17)")
+    groups = ap.add_mutually_exclusive_group()
+    groups.add_argument("--shared-intrinsics", action="store_true",
+                        help="every camera shares one f, k1, k2, those of camera 0 at the start (DESIGN.md section 18)")
+    groups.add_argument("--intrinsics-groups", default=None, metavar="FILE.npy",
+                        help="an int array [nc] of intrinsics group ids, -1 = the camera keeps its own; the cameras of a group "
+                             "share one f, k1, k2, those of its lowest-index camera at the start (DESIGN.md section 18)")
     ap.add_argument("--covariance", default=None, metavar="OUT.npz",
                     help="after the solve, write the marginal covariances `cam` [nc, 9, 9] (tx,ty,tz, rx,ry,rz, f,k1,k2) and `lm` "
                          "[nl, 3, 3] at the final state (DESIGN.md section 16); the gauge must be fixed by priors or held "
@@ -87,6 +93,13 @@ def main():
                 problem.landmark_prior = (f["idx"], f["mean"], f["sqrt_info"])
             except ValueError as e:
                 ap.error(f"--landmark-prior: {e}")
+    if args.shared_intrinsics:
+        problem.intrinsics_group = np.zeros(problem.num_cameras(), np.int32)
+    elif args.intrinsics_groups:
+        try:
+            problem.intrinsics_group = np.load(args.intrinsics_groups)
+        except ValueError as e:
+            ap.error(f"--intrinsics-groups: {e}")
     options = rb.SolverOptions(max_num_iterations=args.max_num_iterations, preconditioner_type=args.preconditioner_type,
                                operator_form=args.operator_form, use_double=not args.float)
     summary = rb.bundle_adjust_manual(problem, options, verbose=True)

@@ -302,6 +302,31 @@ int32_t rba_set_camera_pair_prior(rba_handle* h, int32_t num_pairs, const int32_
  * RBA_ERR_INVALID_ARGUMENT, and the previous landmark priors stay in force. */
 int32_t rba_set_landmark_prior(rba_handle* h, int32_t num, const int32_t* lm_idx, const void* mean, const void* sqrt_info);
 
+/* ---- Intrinsics shared across groups of cameras (DESIGN.md section 18) -------------------- */
+
+/* Not in the reference.  Images taken by one physical camera share one set of intrinsics (f, k1, k2 together).
+ * group [num_cameras of the full problem] int32: -1 = the camera keeps its own intrinsics; g >= 0 = group id (any
+ * non-negative value below Nc).  NULL = no groups (the default).  A group's lead is its lowest-index camera; a group of one
+ * camera is an ungrouped camera, bit for bit.  Every rank of a sharded problem passes the same array.
+ * The solve gives the LM step of the tied problem (a pose per camera, one f, k1, k2 per group): with x = P u (P copies a
+ * group's intrinsics into every member), (P^T D J^T J D P + lambda I) u = -P^T D J^T r, D the Jacobi scaling of the merged
+ * columns J P, lambda once per group.  The call copies the lead's f, k1, k2 into the other members of its group (state and
+ * backup), and so does every later rba_set_state; the members then stay bit-identical through rba_apply, rba_lm_step,
+ * rba_lm_run, rba_backup and rba_restore.  A host increment given to rba_apply / rba_back_substitute has the members'
+ * entries 6..8 replaced by the lead's before the back-substitution.
+ * rba_get_jacobian_scaling gives every member the group-summed norms; rba_get_rhs the contracted b (the lead's entries 6..8
+ * hold the group's sum, the other members' are 0); rba_get_preconditioner the inverse PCG uses (the lead's block is
+ * blkdiag(pose^-1, G^-1) with G the members' summed intrinsics blocks + lambda I, another member's the pose inverse with
+ * zero intrinsics rows and columns).  rba_right_multiply stays the full, ungrouped operator; rba_compute_error is unchanged.
+ * After a call rba_solve returns RBA_ERR_STATE until the next rba_linearize; the device-resident increment and the cached
+ * error are discarded.
+ * An id outside [-1, Nc), or RBA_FIX_F / K1 / K2 bits that differ between members of one group (checked here and by
+ * rba_set_camera_fixed) -> RBA_ERR_INVALID_ARGUMENT, and the previous groups (or flags) stay in force.  Groups of >= 2
+ * cameras with solver_type = 2 (POWER_SCHUR_COMPLEMENT: Hpp of the tied problem is not block-diagonal) -> RBA_ERR_UNSUPPORTED.
+ * rba_compute_covariance gives the covariance of the tied problem, P (P^T H P)^-1 P^T: every member's 9x9 block carries the
+ * group's intrinsics covariance and its own pose-intrinsics cross terms, and the landmark blocks use the same matrix. */
+int32_t rba_set_intrinsics_groups(rba_handle* h, const int32_t* group);
+
 /* ---- Marginal covariances (DESIGN.md section 16) ------------------------------------------ */
 
 /* Not in the reference.  DESIGN.md section 16.  The covariance of the Gauss-Newton step of the total objective (reprojection

@@ -18,6 +18,7 @@
 #include "kernels.cuh"
 #include "covariance.cuh"
 #include "assembled.cuh"
+#include "groups.cuh"
 #include "nccl_dyn.hpp"
 
 namespace rba {
@@ -58,6 +59,7 @@ struct rba_handle {
   virtual int set_camera_prior(const void* mean, const void* sqrt_info) = 0;
   virtual int set_camera_pair_prior(int32_t num_pairs, const int32_t* pairs, const void* mean, const void* sqrt_info) = 0;
   virtual int set_landmark_prior(int32_t num, const int32_t* lm_idx, const void* mean, const void* sqrt_info) = 0;
+  virtual int set_intrinsics_groups(const int32_t* group) = 0;
   virtual int compute_error(rba_residual_info* out) = 0;
   virtual int linearize() = 0;
   virtual int solve(double lambda, void* inc_out, rba_cg_summary* cg) = 0;
@@ -202,6 +204,15 @@ struct Solver : rba_handle {
   S* d_lmp_mean = nullptr;         // [m][3]
   S* d_lmp_L = nullptr;            // [m][9]
   S* d_lmp_Lg = nullptr;           // [m][12]
+  // intrinsics groups (rba_set_intrinsics_groups, DESIGN.md section 18): n_groups groups of >= 2 cameras; 0 = the
+  // unmodified path
+  int n_groups = 0;
+  std::vector<int> h_grp_lead;     // [nc] lead of the camera's group, -1 = own intrinsics (also a group of one)
+  std::vector<uint8_t> h_fixed;    // [nc] the flags of rba_set_camera_fixed, empty = none
+  int* d_grp_lead = nullptr; int* d_grp_ptr = nullptr; int* d_grp_mem = nullptr;
+  uint8_t* d_grp_fixed = nullptr;  // [nc] the user's flags + RBA_FIX_INTRINSICS on every member but the lead
+  S* d_grp_ve = nullptr;           // [9 nc] the expanded operator input P v
+  S* d_grp_y = nullptr;            // [9 nc] the contracted operator output the vector step reads
   rba_stage_timings tm{};
   EventPair ev_stage1, ev_stage2, ev_precond, ev_pcg, ev_backsub, ev_update, ev_error, ev_mv, ev_user;
   long long launches = 0;
@@ -638,6 +649,12 @@ struct Solver : rba_handle {
   // ------------------------------------------------------------------------------------------
   int set_state(const void* cams, const void* lms) override {
     ++state_version;
+    std::vector<S> tied;
+    if (n_groups) {  // the members take their lead's f, k1, k2
+      tied.assign((const S*)cams, (const S*)cams + (size_t)10 * nc);
+      tie_intrinsics(tied.data());
+      cams = tied.data();
+    }
     CU(cudaMemcpyAsync(D.cams, cams, (size_t)10 * nc * sizeof(S), cudaMemcpyHostToDevice, stream));
     CU(cudaMemcpyAsync(D.lms, (const S*)lms + (size_t)3 * L.lm_begin, (size_t)3 * L.nl_local * sizeof(S), cudaMemcpyHostToDevice, stream));
     CU(cudaStreamSynchronize(stream));
@@ -673,6 +690,12 @@ struct Solver : rba_handle {
         any = any || flags[c] != 0;
         all = all && flags[c] == RBA_FIX_ALL;
       }
+    std::vector<uint8_t> fl;
+    if (any) fl.assign(flags, flags + nc);
+    if (n_groups) {
+      const std::string why = group_flags_mismatch(h_grp_lead, fl);
+      if (!why.empty()) { g_err = "rba_set_camera_fixed: " + why; return RBA_ERR_INVALID_ARGUMENT; }
+    }
     if (any) {
       if (!d_cam_fixed) { int rc = dalloc(&d_cam_fixed, (size_t)nc, false); if (rc) return rc; }
       CU(cudaMemcpyAsync(d_cam_fixed, flags, (size_t)nc, cudaMemcpyHostToDevice, stream));
@@ -680,8 +703,105 @@ struct Solver : rba_handle {
     }
     D.cam_fixed = any ? d_cam_fixed : nullptr;
     all_cams_fixed = all;
+    h_fixed = std::move(fl);
+    if (n_groups) TRY(upload_group_fixed());
     have_inc = false;  // the device-resident increment was solved under the previous flags
     return RBA_OK;
+  }
+
+  // Intrinsics shared across groups of cameras (DESIGN.md section 18).  Every check runs before anything changes, so a
+  // rejected call leaves the previous groups.  No group of >= 2 cameras = the unmodified path (n_groups == 0).
+  int set_intrinsics_groups(const int32_t* group) override {
+    auto fail = [&](int rc, const std::string& what) { g_err = "rba_set_intrinsics_groups: " + what; return rc; };
+    std::vector<int> lead((size_t)nc, -1), first((size_t)nc, -1), count((size_t)nc, 0);
+    if (group) {
+      for (int c = 0; c < nc; ++c) {
+        const int g = group[c];
+        if (g < -1 || g >= nc)
+          return fail(RBA_ERR_INVALID_ARGUMENT, "camera " + std::to_string(c) + " has group id " + std::to_string(g) + ", outside [-1, " + std::to_string(nc) + ")");
+        if (g >= 0 && count[g]++ == 0) first[g] = c;
+      }
+      for (int c = 0; c < nc; ++c)
+        if (group[c] >= 0 && count[group[c]] >= 2) lead[c] = first[group[c]];
+    }
+    // groups in the order of their leads, members ascending (the lead first)
+    std::vector<int> gidx((size_t)nc, -1), ptr(1, 0), mem;
+    int ng = 0;
+    for (int c = 0; c < nc; ++c)
+      if (lead[c] == c) gidx[c] = ng++;
+    if (ng > 0 && opt.solver_type == 2)
+      return fail(RBA_ERR_UNSUPPORTED, "POWER_SCHUR_COMPLEMENT does not support groups of >= 2 cameras (Hpp of the tied problem is not block-diagonal)");
+    const std::string why = group_flags_mismatch(lead, h_fixed);
+    if (!why.empty()) return fail(RBA_ERR_INVALID_ARGUMENT, why);
+    ptr.assign((size_t)ng + 1, 0);
+    for (int c = 0; c < nc; ++c)
+      if (lead[c] >= 0) ++ptr[gidx[lead[c]] + 1];
+    for (int g = 0; g < ng; ++g) ptr[g + 1] += ptr[g];
+    mem.resize((size_t)ptr[ng]);
+    std::vector<int> fill(ptr.begin(), ptr.end() - 1);
+    for (int c = 0; c < nc; ++c)
+      if (lead[c] >= 0) mem[fill[gidx[lead[c]]]++] = c;
+    if (ng > 0) {
+      // the new lists go to fresh buffers and replace the previous ones only once every allocation has succeeded, so a
+      // failed call leaves the previous groups in force
+      int *lead_d = nullptr, *ptr_d = nullptr, *mem_d = nullptr;
+      TRY(upload(&lead_d, lead));
+      TRY(upload(&ptr_d, ptr));
+      TRY(upload(&mem_d, mem));
+      if (!d_grp_ve) {
+        S *ve = nullptr, *y = nullptr; uint8_t* fx = nullptr;
+        TRY(dalloc(&ve, (size_t)9 * nc)); TRY(dalloc(&y, (size_t)9 * nc)); TRY(dalloc(&fx, (size_t)nc));
+        d_grp_ve = ve; d_grp_y = y; d_grp_fixed = fx;
+      }
+      CU(cudaStreamSynchronize(stream));
+      TRY(dfree(d_grp_lead)); TRY(dfree(d_grp_ptr)); TRY(dfree(d_grp_mem));
+      d_grp_lead = lead_d; d_grp_ptr = ptr_d; d_grp_mem = mem_d;
+    }
+    n_groups = ng;
+    h_grp_lead = std::move(lead);
+    if (ng > 0) {
+      TRY(upload_group_fixed());
+      // the current state and its backup take the tied values
+      std::vector<S> c((size_t)10 * nc);
+      for (S* d : std::initializer_list<S*>{D.cams, cams_bk}) {
+        CU(cudaMemcpyAsync(c.data(), d, c.size() * sizeof(S), cudaMemcpyDeviceToHost, stream));
+        CU(cudaStreamSynchronize(stream));
+        tie_intrinsics(c.data());
+        CU(cudaMemcpyAsync(d, c.data(), c.size() * sizeof(S), cudaMemcpyHostToDevice, stream));
+      }
+      CU(cudaStreamSynchronize(stream));
+      ++state_version;
+    }
+    // the scaling, b and the blocks of the last linearisation belong to the previous groups
+    return priors_changed();
+  }
+  // "" when every group's members agree on RBA_FIX_F / K1 / K2, else which camera does not
+  std::string group_flags_mismatch(const std::vector<int>& lead, const std::vector<uint8_t>& flags) const {
+    if (flags.empty()) return "";
+    for (int c = 0; c < nc; ++c)
+      if (lead[c] >= 0 && (flags[c] & RBA_FIX_INTRINSICS) != (flags[lead[c]] & RBA_FIX_INTRINSICS))
+        return "camera " + std::to_string(c) + " has RBA_FIX_F / K1 / K2 bits " + std::to_string(flags[c] & RBA_FIX_INTRINSICS) +
+               " that differ from those of its group's lead, camera " + std::to_string(lead[c]) + " (" + std::to_string(flags[lead[c]] & RBA_FIX_INTRINSICS) + ")";
+    return "";
+  }
+  void tie_intrinsics(S* cams) const {
+    for (int c = 0; c < nc; ++c)
+      if (h_grp_lead[c] >= 0 && h_grp_lead[c] != c)
+        for (int k = 7; k < 10; ++k) cams[10 * (size_t)c + k] = cams[10 * (size_t)h_grp_lead[c] + k];
+  }
+  // the flags k_precond_invert masks with: the user's, and the intrinsics of every member but the lead
+  int upload_group_fixed() {
+    std::vector<uint8_t> f((size_t)nc, 0);
+    for (int c = 0; c < nc; ++c)
+      f[c] = (uint8_t)((h_fixed.empty() ? 0 : h_fixed[c]) | (h_grp_lead[c] >= 0 && h_grp_lead[c] != c ? RBA_FIX_INTRINSICS : 0));
+    CU(cudaMemcpyAsync(d_grp_fixed, f.data(), (size_t)nc, cudaMemcpyHostToDevice, stream));
+    CU(cudaStreamSynchronize(stream));
+    return RBA_OK;
+  }
+  GroupView groups() const { return {d_grp_lead, d_grp_ptr, d_grp_mem, n_groups}; }
+  int group_expand(const S* v, S* out, bool in_solve) {
+    return launch_ex(k_group_expand<S>, (9 * nc + 255) / 256, 256, 0, in_solve, 1, v, out, (const int*)d_grp_lead, nc,
+                     in_solve ? (const PcgState*)d_state : (const PcgState*)nullptr);
   }
   // Gaussian priors on the camera parameters.  They are part of the linearisation (Jacobi scaling, A, r), so a change needs a
   // new rba_linearize; the device-resident increment and the cost cache are discarded.  No prior (both NULL, or every L_c
@@ -977,6 +1097,10 @@ struct Solver : rba_handle {
       k_pair_diag2<S><<<(nc + 127) / 128, 128, 0, stream>>>(d_pair_A, d_pair_ptr, d_pair_item, nc, D.diag2);
       launches += 2;
     }
+    if (n_groups) {  // the merged intrinsics columns' norms for every member, after the sum over the shards and the priors
+      k_group_sum_diag2<S><<<n_groups, GROUP_THREADS, 0, stream>>>(D.diag2, groups());
+      ++launches;
+    }
     k_scaling<S><<<(9 * nc + 255) / 256, 256, 0, stream>>>(D.diag2, D.scaling, 9 * nc, (S)ko.jacobi_eps);
     // pass B: linearize (scaled) + Jl scaling + Householder QR + panel write
     // (+ the landmark priors' column norms, L~ and g: the LMP instances)
@@ -1066,8 +1190,11 @@ struct Solver : rba_handle {
   // there), and Nccl before every application (the in-place all-reduce would carry the previous sum into the next).  The
   // others need no clear: k_rcs_spmv writes every camera, k_pcg_vec takes 0 for a camera without segments, and a peer
   // staging slot that is never written stays zero.
+  // With intrinsics groups the operator output is contracted (k_group_contract) between the reduction and the vector step,
+  // so it must exist as one vector: Partials and Peer, which sum the segments inside k_pcg_vec, give way to Counter / Nccl.
   Handover handover() const {
     if (s_valid) return Handover::Assembled;
+    if (n_groups) return opt.nranks > 1 ? Handover::Nccl : Handover::Counter;
     if (opt.nranks > 1) return peer_ok ? Handover::Peer : Handover::Nccl;
     const bool vec_cached = 9 * ((nc + pcg_cluster - 1) / pcg_cluster) <= VEC_THREADS * VEC_EPT;
     return pcg_partials && vec_cached && opt.solver_type != 2 ? Handover::Partials : Handover::Counter;
@@ -1117,9 +1244,13 @@ struct Solver : rba_handle {
   int pcg_vec(int i, int mode, bool pdl, int is_last, S lambda, bool fused_ar = false, bool from_partials = false) {
     PeerComm c = pc;
     if (!fused_ar) c.nranks = 1;
-    if (D.pair_ov && mode != 3) TRY(pair_ov(mode == 2 ? D.x : D.p, pdl));
-    auto kern = D.pair_ov ? k_pcg_vec<S, true, true> : D.prior_H ? k_pcg_vec<S, true> : k_pcg_vec<S, false>;
-    return launch_ex(kern, pcg_cluster, VEC_THREADS, 0, pdl, pcg_cluster, D, d_state, lambda, i, mode, (double)opt.eta,
+    DevPtrs<S> Dv = D;
+    if (n_groups) {  // the contracted output, which holds the prior terms already (k_group_contract)
+      Dv.y = d_grp_y; Dv.prior_H = nullptr; Dv.pair_ov = nullptr;
+    }
+    if (Dv.pair_ov && mode != 3) TRY(pair_ov(mode == 2 ? D.x : D.p, pdl));
+    auto kern = Dv.pair_ov ? k_pcg_vec<S, true, true> : Dv.prior_H ? k_pcg_vec<S, true> : k_pcg_vec<S, false>;
+    return launch_ex(kern, pcg_cluster, VEC_THREADS, 0, pdl, pcg_cluster, Dv, d_state, lambda, i, mode, (double)opt.eta,
                      (int)opt.min_linear_solver_iterations, is_last, (int)pdl, c, ar_seq, from_partials ? op_item_ptr : (const int*)nullptr, d_prog);
   }
   // D.pair_ov = sum_j O_ij v_j (k_pair_ov), ahead of the vector step that consumes it
@@ -1127,8 +1258,17 @@ struct Solver : rba_handle {
     return launch_ex(k_pair_ov<S>, (9 * nc + 255) / 256, 256, 0, pdl, 1, D, (const PcgState*)d_state, v);
   }
   // one operator application inside PCG (H v for v = p in mode 0/1, x in mode 2) and the vector step after it
+  // (intrinsics groups: H_u v = P^T H P v, with P v in d_grp_ve and P^T (H P v) in d_grp_y)
   int pcg_step(int i, int mode, int is_last, S lambda, Handover h) {
-    TRY(apply_operator(mode == 2 ? D.x : D.p, h, true));
+    const S* v = mode == 2 ? D.x : D.p;
+    if (n_groups) {
+      TRY(group_expand(v, d_grp_ve, true));
+      v = d_grp_ve;
+    }
+    TRY(apply_operator(v, h, true));
+    if (n_groups)
+      TRY(launch_ex(k_group_contract<S>, (nc + GROUP_THREADS - 1) / GROUP_THREADS + n_groups, GROUP_THREADS, 0, h != Handover::Nccl, 1,
+                    D, (const S*)d_grp_ve, d_grp_y, groups(), (nc + GROUP_THREADS - 1) / GROUP_THREADS, (const PcgState*)d_state));
     return pcg_vec(i, mode, h != Handover::Nccl, is_last, lambda, h == Handover::Peer, h == Handover::Partials);
   }
   // Enqueue iterations 1..last in chunks of `chunk` (enqueue(i)); after each chunk the PcgState is copied into one of two
@@ -1207,10 +1347,20 @@ struct Solver : rba_handle {
     // pose damping lambda*I added to the blocks, then explicit inverse (ref: linearization_qr.hpp:796-802, linearizor_qr.cpp:228-237)
     // (+ the masking of the held camera parameters, D.cam_fixed; + the camera priors: A^T A into the SCHUR_JACOBI blocks -- the
     // JACOBI blocks hold it already -- and A^T r into b, both after the sum over the shards and before the masking)
-    k_precond_invert<S><<<(nc + 63) / 64, 64, 0, stream>>>(schur ? D.blocks : D.jblocks, lambda, nc, schur ? D.blocks : nullptr, D.inv,
-                                                           D.cam_fixed, D.b, schur ? (const S*)D.prior_H : nullptr,
-                                                           D.prior_H ? (const S*)d_prior_g : nullptr);
-    ++launches;
+    if (n_groups) {
+      // (intrinsics groups: the priors' terms, the contraction of b and the merged blocks first, into D.blocks; DESIGN.md
+      // section 18)
+      const int ncb = (nc + GROUP_THREADS - 1) / GROUP_THREADS;
+      k_group_precond<S><<<ncb + n_groups, GROUP_THREADS, 0, stream>>>(schur ? D.blocks : D.jblocks, schur ? (const S*)D.prior_H : nullptr,
+                                                                       D.prior_H ? (const S*)d_prior_g : nullptr, D.b, D.blocks, groups(), nc, ncb);
+      k_precond_invert<S><<<(nc + 63) / 64, 64, 0, stream>>>(D.blocks, lambda, nc, schur ? D.blocks : nullptr, D.inv, d_grp_fixed, D.b);
+      launches += 2;
+    } else {
+      k_precond_invert<S><<<(nc + 63) / 64, 64, 0, stream>>>(schur ? D.blocks : D.jblocks, lambda, nc, schur ? D.blocks : nullptr, D.inv,
+                                                             D.cam_fixed, D.b, schur ? (const S*)D.prior_H : nullptr,
+                                                             D.prior_H ? (const S*)d_prior_g : nullptr);
+      ++launches;
+    }
     rc = stop(ev_precond); if (rc) return rc;
     last_lambda = lambda;
     damping_valid = true;
@@ -1279,6 +1429,7 @@ struct Solver : rba_handle {
         rc = enqueue_iteration(i); if (rc) return rc;
       }
     }
+    if (n_groups) TRY(group_expand(D.inc, D.inc, false));  // inc = P u for the back-substitution, the update and inc_out
     CU(cudaMemcpyAsync(&h_state[0], d_state, sizeof(PcgState), cudaMemcpyDeviceToHost, stream));
     if (inc_out) CU(cudaMemcpyAsync(inc_out, D.inc, (size_t)9 * nc * sizeof(S), cudaMemcpyDeviceToHost, stream));
     rc = stop(ev_pcg); if (rc) return rc;
@@ -1321,6 +1472,7 @@ struct Solver : rba_handle {
         k_mask_fixed_inc<S><<<(9 * nc + 255) / 256, 256, 0, stream>>>(D.inc, D.cam_fixed, nc);
         ++launches;
       }
+      if (n_groups) TRY(group_expand(D.inc, D.inc, false));  // the members take the lead's f, k1, k2 entries
     } else if (!have_inc) { g_err = "no device-resident increment (none solved since rba_linearize or rba_set_camera_fixed)"; return RBA_ERR_STATE; }
     int rc = start(ev_backsub); if (rc) return rc;
     CU(cudaMemsetAsync(d_flags, 0, 4 * sizeof(int), stream));
@@ -1631,6 +1783,14 @@ struct Solver : rba_handle {
     CU(cudaMemcpy2DAsync(dst, dld * sizeof(double), src, sld * sizeof(double), rows * sizeof(double), cols, cudaMemcpyDeviceToDevice, stream));
     return RBA_OK;
   }
+  // P^T A P (expand = 0) or P A P^T (expand = 1) of the symmetric matrix whose lower triangle A holds, in place (full)
+  int cov_group_passes(double* A, long long ld, long long n, int expand) {
+    k_cov_group_symmetrize<<<dim3((unsigned)((n + 31) / 32), (unsigned)((n + 7) / 8)), dim3(32, 8), 0, stream>>>(A, ld, n);
+    for (int columns = 0; columns < 2; ++columns)
+      k_cov_group_pass<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(A, ld, n, groups(), columns, expand);
+    CU(cudaGetLastError());
+    return RBA_OK;
+  }
   int compute_covariance(double* cam_cov, double* lm_cov) override {
     if (!cam_cov && !lm_cov) { g_err = "rba_compute_covariance: cam_cov and lm_cov are both NULL"; return RBA_ERR_INVALID_ARGUMENT; }
     if (opt.nranks > 1) {
@@ -1675,8 +1835,14 @@ struct Solver : rba_handle {
       k_cov_priors<S><<<(nc + 127) / 128, 128, 0, stream>>>(D.cams, nc, has_abs_prior ? d_prior_mean : nullptr, d_prior_L, d_pair_ij,
                                                             d_pair_mean, d_pair_L, n_pairs > 0 ? d_pair_ptr : nullptr, d_pair_item,
                                                             d_pair_nbr, A, np);
-    k_cov_diag<<<(unsigned)((np + 255) / 256), 256, 0, stream>>>(A, np, n, np, D.cam_fixed, d);
-    k_cov_equil<<<dim3((unsigned)(np / 32), (unsigned)(np / 8)), dim3(32, 8), 0, stream>>>(A, np, n, np, D.cam_fixed, d);
+    // intrinsics groups (DESIGN.md section 18): S_u = P^T S P, the members' entries 6..8 then held like the user's
+    const uint8_t* held = D.cam_fixed;
+    if (n_groups) {
+      TRY(cov_group_passes(A, np, n, 0));
+      held = d_grp_fixed;
+    }
+    k_cov_diag<<<(unsigned)((np + 255) / 256), 256, 0, stream>>>(A, np, n, np, held, d);
+    k_cov_equil<<<dim3((unsigned)(np / 32), (unsigned)(np / 8)), dim3(32, 8), 0, stream>>>(A, np, n, np, held, d);
     // 3a. potrf, right-looking: factor the diagonal tile, panel <- panel L_kk^-T, trailing lower tiles -= panel panel^T
     for (int k = 0; k < nt; ++k) {
       const long long k0 = k * TB, m = np - k0 - TB;
@@ -1721,6 +1887,11 @@ struct Solver : rba_handle {
       }
       k_cov_tile_lauu2<<<1, 256, 0, stream>>>(A, np, r0);
       if (kk > 0) cov_gemm<true, false>(TB, r0 + TB, kk, 1.0, A + (r0 + TB) + r0 * np, np, A + (r0 + TB), np, 1.0, A + r0, np, 0, 0);
+    }
+    // (intrinsics groups: P S_u^-1 P^T, the members' rows and columns 6..8 and equilibration those of the lead)
+    if (n_groups) {
+      TRY(cov_group_passes(A, np, n, 1));
+      k_cov_group_d<<<1, 1, 0, stream>>>(d, groups());
     }
     // 4. extraction
     if (cam_cov) {
@@ -1976,6 +2147,7 @@ int32_t rba_set_camera_pair_prior(rba_handle* h, int32_t num_pairs, const int32_
 int32_t rba_set_landmark_prior(rba_handle* h, int32_t num, const int32_t* lm_idx, const void* mean, const void* sqrt_info) {
   return h->set_landmark_prior(num, lm_idx, mean, sqrt_info);
 }
+int32_t rba_set_intrinsics_groups(rba_handle* h, const int32_t* group) { return h->set_intrinsics_groups(group); }
 int32_t rba_compute_error(rba_handle* h, rba_residual_info* out) { return h->compute_error(out); }
 int32_t rba_linearize(rba_handle* h) { return h->linearize(); }
 

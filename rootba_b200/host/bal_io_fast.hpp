@@ -132,6 +132,7 @@ struct FileBuffer {
 // Both problem classes (BalProblemSoA, BalProblem) carry them.
 struct ProblemPriors {
   std::vector<uint8_t> camera_fixed;               // [nc] RBA_FIX_* bits (rba_set_camera_fixed)
+  std::vector<int32_t> intrinsics_group;           // [nc] group id, -1 = own intrinsics (rba_set_intrinsics_groups); empty = none
   // Gaussian camera priors (rba_set_camera_prior)
   std::vector<double> camera_prior_mean;           // [nc][10] qx,qy,qz,qw (R0), camera centre c0, f0, k1_0, k2_0
   std::vector<double> camera_prior_sqrt_info;      // [nc][81] row-major square-root information L

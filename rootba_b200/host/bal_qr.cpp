@@ -2,7 +2,7 @@
 //   bal_qr --input <bal file> [--no-use-double] [--max-num-iterations N] [--preconditioner-type JACOBI|SCHUR_JACOBI]
 //          [--residual-robust-norm NONE|HUBER] [--residual-huber-parameter X] [--no-normalize] [--dump-problem out.bin]
 //          [--loader parallel|map] [--num-threads T] [--operator-form dense|implicit] [--init-depth-threshold Z]
-//          [--fix-intrinsics] [--fix-cameras I,J,...]
+//          [--fix-intrinsics] [--fix-cameras I,J,...] [--shared-intrinsics]
 //   --loader parallel (default): mmap + multi-threaded parse into flat arrays (bal_io_fast.hpp);
 //   --loader map: the reference-style fscanf + std::map loader (bal_problem.hpp).  Both give identical problems.
 #include <chrono>
@@ -22,6 +22,7 @@ static double seconds_since(std::chrono::steady_clock::time_point t0) {
 // camera parameters held constant (rba_set_camera_fixed): --fix-intrinsics, --fix-cameras I,J,...
 struct FixOptions {
   bool intrinsics = false;
+  bool shared_intrinsics = false;  // every camera in one intrinsics group (rba_set_intrinsics_groups)
   std::vector<long long> cameras;  // indices into the loaded problem
 };
 
@@ -69,6 +70,7 @@ int solve_and_log(Problem& problem, const SolverOptions& o, const FixOptions& fi
       problem.camera_fixed[(size_t)c] = (uint8_t)RBA_FIX_ALL;
     }
   }
+  if (fix.shared_intrinsics) problem.intrinsics_group.assign((size_t)problem.num_cameras(), 0);
   const DatasetSummary ds = summarize_problem<S>(problem, input);
   SolverSummary summary;
   bundle_adjust_manual<S>(problem, o, &summary);
@@ -147,6 +149,7 @@ int main(int argc, char** argv) {
     else if (a == "--init-depth-threshold") depth_thr = std::stod(next());
     else if (a == "--dump-problem") dump = next();
     else if (a == "--fix-intrinsics") fix.intrinsics = true;
+    else if (a == "--shared-intrinsics") fix.shared_intrinsics = true;
     else if (a == "--fix-cameras") {
       const std::string v = next();
       if (!parse_camera_list(v, fix.cameras)) { std::cerr << "--fix-cameras expects a comma-separated list of camera indices, got '" << v << "'\n"; return 2; }
@@ -155,6 +158,7 @@ int main(int argc, char** argv) {
     else if (a == "--help" || a == "-h") {
       std::cout << "usage: bal_qr --input <bal file> [--no-use-double] [--max-num-iterations N] [--preconditioner-type JACOBI|SCHUR_JACOBI] ...\n"
                    "  --fix-intrinsics      hold f, k1, k2 of every camera constant\n"
+                   "  --shared-intrinsics   every camera shares one f, k1, k2 (camera 0's at the start)\n"
                    "  --fix-cameras I,J,... hold every parameter of the listed cameras constant; indices refer to the loaded problem\n"
                    "                        (a Bundler file's cameras with focal length 0 are dropped by the loader first)\n";
       return 0;

@@ -178,6 +178,10 @@ class LinearizorQR {
       if ((int)bp.camera_fixed.size() != bp.num_cameras()) throw std::runtime_error("camera_fixed must have one entry per camera");
       check(rba_set_camera_fixed(h_, bp.camera_fixed.data()));
     }
+    if (!bp.intrinsics_group.empty()) {
+      if ((int)bp.intrinsics_group.size() != bp.num_cameras()) throw std::runtime_error("intrinsics_group must have one entry per camera");
+      check(rba_set_intrinsics_groups(h_, bp.intrinsics_group.data()));
+    }
     if (!bp.camera_prior_mean.empty() || !bp.camera_prior_sqrt_info.empty()) {
       if (bp.camera_prior_mean.size() != (size_t)10 * bp.num_cameras() || bp.camera_prior_sqrt_info.size() != (size_t)81 * bp.num_cameras())
         throw std::runtime_error("camera priors must have 10 mean and 81 sqrt_info entries per camera");

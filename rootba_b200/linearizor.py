@@ -78,6 +78,18 @@ def _camera_fixed_array(flags, num_cameras: int):
     return np.ascontiguousarray(a, dtype=np.uint8).copy()
 
 
+def _intrinsics_group_array(group, num_cameras: int):
+    """None, or a validated int32 copy of one group id per camera (-1 = own intrinsics, else an id in [0, num_cameras))"""
+    if group is None:
+        return None
+    a = np.asarray(group)
+    if a.shape != (num_cameras,):
+        raise ValueError(f"intrinsics_group must have one entry per camera ({num_cameras}), got shape {a.shape}")
+    if a.dtype.kind not in "iu" or np.any(a < -1) or np.any(a >= num_cameras):
+        raise ValueError(f"intrinsics_group entries must be integers in [-1, {num_cameras})")
+    return np.ascontiguousarray(a, dtype=np.int32).copy()
+
+
 def _prior_arrays(name, mean, sqrt_info, dtype, m, mean_len, dim, check_index=None, item=None):
     """validated contiguous copies (mean [m, mean_len], sqrt_info [m, dim, dim]) in `dtype` of the priors `name`.  The checks
     run in this order: the shapes, the kind's own index checks (`check_index`), finiteness and, for a kind whose mean
@@ -154,7 +166,9 @@ class BalProblem:
     T_i T_j^-1 ~ (R0, t0) with the cost 1/2 |L e|^2, e = (t_i - R_i R_j^T t_j - t0, Log(R_i R_j^T R0^T))
     (rba_set_camera_pair_prior, DESIGN.md section 15); mean rows are (qx,qy,qz,qw of R0, t0).  Forwarded likewise.
     `landmark_prior` (not in the reference): None or (idx [m] int32, mean [m,3], sqrt_info [m,3,3]), Gaussian priors on
-    landmark positions with the cost 1/2 |L (x - x0)|^2 (rba_set_landmark_prior, DESIGN.md section 17).  Forwarded likewise."""
+    landmark positions with the cost 1/2 |L (x - x0)|^2 (rba_set_landmark_prior, DESIGN.md section 17).  Forwarded likewise.
+    `intrinsics_group` (not in the reference): None or one int32 group id per camera (-1 = own intrinsics); the cameras of a
+    group share one f, k1, k2 (rba_set_intrinsics_groups, DESIGN.md section 18).  Forwarded likewise."""
 
     def __init__(self, cams, lms, lm_off, obs_cam, obs_xy, dtype=np.float64):
         self.dtype = np.dtype(dtype)
@@ -171,6 +185,18 @@ class BalProblem:
         self._camera_prior = None
         self._camera_pair_prior = None
         self._landmark_prior = None
+        self._intrinsics_group = None
+
+    @property
+    def intrinsics_group(self):
+        return self._intrinsics_group
+
+    @intrinsics_group.setter
+    def intrinsics_group(self, group):
+        g = _intrinsics_group_array(group, self.num_cameras())
+        if self._linearizor is not None:
+            self._linearizor._upload_intrinsics_group(g)  # raises on rejection: the previous groups stay in force
+        self._intrinsics_group = g
 
     @property
     def landmark_prior(self):
@@ -323,6 +349,8 @@ class LinearizorQR:
             self._upload_camera_pair_prior(bal_problem.camera_pair_prior)
         if bal_problem.landmark_prior is not None:
             self._upload_landmark_prior(bal_problem.landmark_prior)
+        if bal_problem.intrinsics_group is not None:
+            self._upload_intrinsics_group(bal_problem.intrinsics_group)
 
     # factory like Linearizor::create (linearizor.cpp:47-65)
     @staticmethod
@@ -390,6 +418,15 @@ class LinearizorQR:
             check(_lib.lib().rba_set_landmark_prior(self.h, 0, None, None, None))
         else:
             check(_lib.lib().rba_set_landmark_prior(self.h, len(prior[0]), _p(prior[0]), _p(prior[1]), _p(prior[2])))
+
+    def set_intrinsics_groups(self, group):
+        """intrinsics shared across groups of cameras (rba_set_intrinsics_groups): None, or one int32 group id per camera
+        (-1 = own intrinsics).  The members take their lead's f, k1, k2; needs a new linearize before the next solve.  The
+        groups are stored on the BalProblem."""
+        self.bal_problem.intrinsics_group = group  # validates and forwards to _upload_intrinsics_group
+
+    def _upload_intrinsics_group(self, group):
+        check(_lib.lib().rba_set_intrinsics_groups(self.h, None if group is None else _p(group)))
 
     def _backup(self):
         check(_lib.lib().rba_backup(self.h))
