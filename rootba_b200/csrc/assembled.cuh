@@ -3,8 +3,9 @@
 // instead of P^T (P x): the same products of panel entries, associated differently, and S (9 x 9 blocks over the
 // co-visible camera pairs) is several times smaller than the panels it is built from.
 //   k_rcs_terms     once per linearisation: S_u = sum over panel rows 0..2n-4 (lambda-independent, the reference's rows
-//   k_rcs_combine   3..2n-1 of the landmark block);  once per solve: S = S_u + sum over the three damping rows that
-//                   k_stage2 has just written (rows 2n-3..2n-1).  The 9 x 9 block of every term (slot_a, slot_b) of every
+//   k_rcs_combine   3..2n-1 of the landmark block);  once per solve that reaches iteration asm_switch: S = S_u + sum
+//                   over the three damping rows that k_stage2 has just written (rows 2n-3..2n-1).  Both return at once
+//                   when the solve has ended before.  The 9 x 9 block of every term (slot_a, slot_b) of every
 //                   landmark is evaluated landmark by landmark into a staging buffer that holds all of them, then every
 //                   co-visible camera pair (ca >= cb) adds its terms in the order of the host-built list
 //                   (build_pair_list, layout.hpp): no atomics, fixed order.
@@ -20,11 +21,13 @@ namespace rba {
 // [0, 2n - 3) (damping = 0: the lambda-independent rows) or [2n - 3, 2n) (damping = 1: the damping rows of the last
 // k_stage2) into stage[81 w].  Neighbouring warps read the same landmark's panel, so it is read from HBM about once.
 // Block entry (p, q) = sum_r P[r][9 ia + p] P[r][9 ib + q]; on the diagonal (sa == sb) it is symmetric bit for bit (fma
-// commutes).
+// commutes).  Enqueued by the host ahead of PCG iteration asm_switch, after the vector step of the iteration before, so it
+// reads the solve's `done` flag in stream order and returns at once when the solve has already ended (as k_rcs_combine).
 template <class S>
 __global__ void __launch_bounds__(256) k_rcs_terms(const S* __restrict__ panel, const AsmTerm* __restrict__ terms, long long nt,
-                                                   int damping, S* __restrict__ stage) {
+                                                   int damping, S* __restrict__ stage, const int* __restrict__ done) {
   using V2 = typename ST<S>::V2;
+  if (*done) return;
   const int lane = threadIdx.x & 31;
   const int g = lane / 9, p = lane - 9 * g;
   if (lane >= 27) return;
@@ -68,9 +71,11 @@ __global__ void __launch_bounds__(256) k_rcs_terms(const S* __restrict__ panel, 
 // Thread per entry of a pair block (ca >= cb): `base` (the lambda-independent part S_u) or 0, plus the pair's staged terms
 // in the pair's list order (landmark order); wpos[t] = landmark-major index of the pair-sorted term t.  The sum goes to
 // out[81 pos.x] (pos == nullptr: out[81 bi], S_u), and off the diagonal its transpose to out[81 pos.y] (the full CSR).
+// Nothing is written when the solve has ended (`done`).
 template <class S>
 __global__ void k_rcs_combine(const int* __restrict__ blk_ptr, const int* __restrict__ wpos, int nblk, const S* __restrict__ stage,
-                              const S* __restrict__ base, const int2* __restrict__ pos, S* __restrict__ out) {
+                              const S* __restrict__ base, const int2* __restrict__ pos, S* __restrict__ out, const int* __restrict__ done) {
+  if (*done) return;
   const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
   if (i >= 81LL * nblk) return;
   const int bi = (int)(i / 81), e = (int)(i - 81LL * bi);

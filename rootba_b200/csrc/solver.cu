@@ -237,8 +237,9 @@ struct Solver : rba_handle {
   // list (term ranges, landmark-major position of every term), per pair its positions (lower, upper or -1) in the full
   // block-row CSR of S, the staging buffer of all terms, S_u per pair and S
   // asm_on: the structure exists; su_valid: S_u belongs to the current linearisation; s_valid: S = S_u + the damping part of
-  // the last solve's lambda, and that solve (and rba_right_multiply / rba_time_matvec after it) applies S
-  bool asm_on = false, su_valid = false, s_valid = false;
+  // the last solve's lambda, and that solve (and rba_right_multiply / rba_time_matvec after it) applies S; su_new: this solve
+  // enqueued the build of S_u (both reset when a solve starts)
+  bool asm_on = false, su_valid = false, s_valid = false, su_new = false;
   int asm_nblk = 0, asm_switch = 0; long long asm_nt = 0, asm_nnzb = 0;
   AsmTerm* d_asm_terms = nullptr; int* d_asm_wpos = nullptr; int* d_asm_blk_ptr = nullptr; IntPair* d_asm_pos = nullptr;
   int* d_asm_row_ptr = nullptr; int* d_asm_col = nullptr;
@@ -1337,7 +1338,7 @@ struct Solver : rba_handle {
       k<<<tile_grid(k2_max_blocks), TILE_WARPS * 32, k2_smem, stream>>>(D, lambda, k2_sc, (int)panels);
     }
     ++launches;
-    s_valid = false;  // S of the previous lambda; rebuilt if this solve runs long enough (solve_enqueue)
+    s_valid = su_new = false;  // S of the previous lambda; rebuilt if this solve runs long enough (solve_enqueue)
     rc = camera_reduce(d_csr_obs_slots, d_csr_obs_items, n_obs_items, d_csr_obs_item_ptr, D.b, panel_form() ? D.b0 : nullptr); if (rc) return rc;
     const bool power = opt.solver_type == 2;
     const bool schur = opt.preconditioner_type == 1 && !power;  // Power-SC inverts Hpp = sum Jp^T Jp + lambda I instead
@@ -1420,8 +1421,11 @@ struct Solver : rba_handle {
         // follow it, whatever the host's pace: the enqueued work does not depend on timing
         if (prog[1] && i - prog[0] > depth) break;
         if (asm_on && i == asm_switch) {
-          // the solve has run asm_switch - 1 iterations: from here on S x (S_u once per linearisation, then S for lambda)
-          if (!su_valid) assemble(0);
+          // the solve has run asm_switch - 1 iterations: from here on S x (S_u once per linearisation, then S for lambda).
+          // The host may enqueue this after the solve has ended (one of the no-op iterations that follow the end): then
+          // the assembly kernels do nothing and solve_finish withdraws what is set here.
+          su_new = !su_valid;
+          if (su_new) assemble(0);
           assemble(1);
           su_valid = s_valid = true;
           h = handover();
@@ -1448,6 +1452,12 @@ struct Solver : rba_handle {
       cg->num_iterations = h_state[0].iter;
       cg->reason = h_state[0].reason;
       cg->num_matvecs = h_state[0].iter + h_state[0].iter / opt.residual_reset_period;
+    }
+    if (s_valid && h_state[0].iter < asm_switch) {
+      // the solve ended before iteration asm_switch, so the assembly enqueued after its end did nothing: the solve ended
+      // with the panel product, and S_u exists only if an earlier solve of this linearisation built it
+      s_valid = false;
+      if (su_new) su_valid = false;
     }
     if (h_state[0].reason == 99) {
       g_err = "PCG: a peer rank did not publish its operator output in time (peer-memory exchange timed out)";
@@ -1735,12 +1745,15 @@ struct Solver : rba_handle {
     return RBA_OK;
   }
   // S_u (stage 1, damping = 0) or S = S_u + the damping rows' part (stage 2, damping = 1)
+  // (inside a solve only: both kernels do nothing once its `done` flag is set.  They read it without a fence, which is
+  // ordered only because they are plain stream launches after the vector step that sets it: not launched with PDL.)
   void assemble(int damping) {
     const int grid = (int)std::max<long long>(1, std::min<long long>((asm_nt + 23) / 24, (long long)sm_count * 16));
-    k_rcs_terms<S><<<grid, 256, 0, stream>>>(D.panel, d_asm_terms, asm_nt, damping, d_asm_stage);
+    const int* done = &d_state->done;
+    k_rcs_terms<S><<<grid, 256, 0, stream>>>(D.panel, d_asm_terms, asm_nt, damping, d_asm_stage, done);
     k_rcs_combine<S><<<(unsigned)((81LL * asm_nblk + 255) / 256), 256, 0, stream>>>(
         d_asm_blk_ptr, d_asm_wpos, asm_nblk, d_asm_stage, damping ? (const S*)d_asm_Su : nullptr,
-        damping ? (const int2*)d_asm_pos : nullptr, damping ? d_asm_S : d_asm_Su);
+        damping ? (const int2*)d_asm_pos : nullptr, damping ? d_asm_S : d_asm_Su, done);
     launches += 2;
   }
 
