@@ -1209,6 +1209,15 @@ __global__ void __launch_bounds__(128) k_stage2(DevPtrs<S> D, S lambda, Scratch<
     {
       const int nsl = T.nvalid * n;
       for (int e = lane; e < nsl * 9; e += 32) D.yobs[9 * (size_t)T.slot_base + e] = sG[e];
+      if constexpr (!PANEL) {
+        // the dmp records, kept here only for the assembly of S (allocated when the handle may build it): from the rows in
+        // shared memory, the same values as the panel rows below
+        if (D.dmp)
+          for (int e = lane; e < nsl * 28; e += 32) {
+            const int sl = e / 28, k = e - 28 * sl, gg = sl / n, d = k / 9;
+            D.dmp[28 * (size_t)T.slot_base + e] = k < 27 ? sD[(d * W + gg) * CS + 9 * (sl - gg * n) + (k - 9 * d)] : S(0);
+          }
+      }
       if (active && write_panel) {
         V2* ptile = reinterpret_cast<V2*>(D.panel + T.panel_off) + (size_t)(2 * n - 3) * KP * 32 + lane;
         for (int k = 0; k < KP; ++k) {

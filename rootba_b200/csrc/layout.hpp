@@ -422,8 +422,8 @@ inline void plan_assembled(const Layout& L, const PairList& P, int scalar_size, 
   A.switch_iteration = asm_switch_iteration(A.nt, L.panel_scalars, A.s_bytes, scalar_size);
   A.fits = 4 * A.s_bytes <= L.panel_scalars * scalar_size && 81 * A.nt * scalar_size <= ASM_STAGE_BYTES;
   if (!A.fits) return;
-  // S, S_u and the staging buffer; the terms and wpos; blk_ptr, row_ptr, col; pos
-  A.device_bytes = A.s_bytes + (A.nblk + A.nt) * 81 * scalar_size + A.nt * (long long)(sizeof(AsmTerm) + sizeof(int)) +
+  // S, S_u and the staging buffer; the terms as panel addresses, wpos and the terms as slot pairs; blk_ptr, row_ptr, col; pos
+  A.device_bytes = A.s_bytes + (A.nblk + A.nt) * 81 * scalar_size + A.nt * (long long)(sizeof(AsmTerm) + sizeof(int) + sizeof(IntPair)) +
                    (A.nblk + A.nnzb + nc + 2) * (long long)sizeof(int) + A.nblk * (long long)sizeof(IntPair);
   // row ca gets (ca, cb) and row cb the transpose; iterating the pairs in (ca, cb) order fills every row in ascending
   // column order (lower blocks, the diagonal, then upper blocks)

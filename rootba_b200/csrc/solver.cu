@@ -242,6 +242,7 @@ struct Solver : rba_handle {
   bool asm_on = false, su_valid = false, s_valid = false, su_new = false;
   int asm_nblk = 0, asm_switch = 0; long long asm_nt = 0, asm_nnzb = 0;
   AsmTerm* d_asm_terms = nullptr; int* d_asm_wpos = nullptr; int* d_asm_blk_ptr = nullptr; IntPair* d_asm_pos = nullptr;
+  IntPair* d_asm_slots = nullptr;
   int* d_asm_row_ptr = nullptr; int* d_asm_col = nullptr;
   S* d_asm_stage = nullptr; S* d_asm_Su = nullptr; S* d_asm_S = nullptr;
 
@@ -500,8 +501,9 @@ struct Solver : rba_handle {
     TRY(dalloc(&D.res, (size_t)2 * L.nslots));
     TRY(dalloc(&D.lmk, (size_t)24 * L.sorted_lm.size()));
     TRY(dalloc(&D.qtr, (size_t)2 * L.nslots));
+    // the damping rows per slot: read by the SCHUR_JACOBI blocks of the panel form and by the assembly of S
+    if (panel_form() || asm_candidate()) TRY(dalloc(&D.dmp, (size_t)28 * L.nslots));
     if (panel_form()) {
-      TRY(dalloc(&D.dmp, (size_t)28 * L.nslots));
       if (opt.preconditioner_type == 1) TRY(dalloc(&D.blk0, (size_t)48 * L.nslots));
       TRY(dalloc(&D.blocks0, (size_t)81 * nc));
       TRY(dalloc(&D.b0, (size_t)9 * nc));
@@ -1719,8 +1721,9 @@ struct Solver : rba_handle {
   // The assembled operator (assembled.cuh, DESIGN.md section 4): taken with one GPU and the dense operator when its
   // structure passes the size rules (plan_assembled) and its buffers fit in the free device memory; else the panel
   // product.
+  bool asm_candidate() const { return asm_hook && opt.nranks == 1 && panels; }
   int setup_assembled() {
-    if (!asm_hook || opt.nranks != 1 || !panels) return RBA_OK;
+    if (!asm_candidate()) return RBA_OK;
     PairList P;
     const std::string msg = build_pair_list(L, P);
     if (!msg.empty()) { g_err = msg; return RBA_ERR_UNSUPPORTED; }
@@ -1732,6 +1735,7 @@ struct Solver : rba_handle {
     if ((size_t)A.device_bytes + ((size_t)256 << 20) > free_b) return RBA_OK;  // keep 256 MB for the rest of the handle and the caller
     TRY(upload(&d_asm_terms, A.terms));
     TRY(upload(&d_asm_wpos, P.wpos));
+    TRY(upload(&d_asm_slots, P.terms));
     TRY(upload(&d_asm_blk_ptr, P.blk_ptr));
     TRY(upload(&d_asm_pos, A.pos));
     TRY(upload(&d_asm_row_ptr, A.row_ptr));
@@ -1744,16 +1748,22 @@ struct Solver : rba_handle {
     asm_on = true;
     return RBA_OK;
   }
-  // S_u (stage 1, damping = 0) or S = S_u + the damping rows' part (stage 2, damping = 1)
-  // (inside a solve only: both kernels do nothing once its `done` flag is set.  They read it without a fence, which is
+  // S_u (damping = 0: every term over the lambda-independent panel rows, staged and combined) or S = S_u + the damping
+  // rows' part (damping = 1: from the dmp records of this solve's k_stage2, no staging; then the upper blocks)
+  // (inside a solve only: all four kernels do nothing once its `done` flag is set.  They read it without a fence, which is
   // ordered only because they are plain stream launches after the vector step that sets it: not launched with PDL.)
   void assemble(int damping) {
-    const int grid = (int)std::max<long long>(1, std::min<long long>((asm_nt + 23) / 24, (long long)sm_count * 16));
     const int* done = &d_state->done;
-    k_rcs_terms<S><<<grid, 256, 0, stream>>>(D.panel, d_asm_terms, asm_nt, damping, d_asm_stage, done);
-    k_rcs_combine<S><<<(unsigned)((81LL * asm_nblk + 255) / 256), 256, 0, stream>>>(
-        d_asm_blk_ptr, d_asm_wpos, asm_nblk, d_asm_stage, damping ? (const S*)d_asm_Su : nullptr,
-        damping ? (const int2*)d_asm_pos : nullptr, damping ? d_asm_S : d_asm_Su, done);
+    const unsigned per_entry = (unsigned)((81LL * asm_nblk + 255) / 256);
+    if (damping) {
+      k_rcs_damping<S><<<(asm_nblk + DMP_WARPS - 1) / DMP_WARPS, DMP_WARPS * 32, 0, stream>>>(
+          d_asm_blk_ptr, (const int2*)d_asm_slots, asm_nblk, D.dmp, d_asm_Su, (const int2*)d_asm_pos, d_asm_S, done);
+      k_rcs_mirror<S><<<per_entry, 256, 0, stream>>>((const int2*)d_asm_pos, asm_nblk, d_asm_S, done);
+    } else {
+      const int grid = (int)std::max<long long>(1, std::min<long long>((asm_nt + 23) / 24, (long long)sm_count * 16));
+      k_rcs_terms<S><<<grid, 256, 0, stream>>>(D.panel, d_asm_terms, asm_nt, 0, d_asm_stage, done);
+      k_rcs_combine<S><<<per_entry, 256, 0, stream>>>(d_asm_blk_ptr, d_asm_wpos, asm_nblk, d_asm_stage, d_asm_Su, done);
+    }
     launches += 2;
   }
 
