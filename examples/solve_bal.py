@@ -4,6 +4,7 @@
     python examples/solve_bal.py problem-49-7776-pre.txt [--float] [--max-num-iterations 20] [--operator-form DENSE|IMPLICIT]
         [--fix-intrinsics] [--fix-cameras I,J,...] [--camera-prior FILE.npz] [--camera-pair-prior FILE.npz]
         [--landmark-prior FILE.npz] [--shared-intrinsics | --intrinsics-groups FILE.npy] [--covariance OUT.npz]
+        [--observation-info FILE.npy] [--residuals OUT.npz]
 
 Mirrors what `bal_qr --input ...` of the reference does (src/app/bal_qr.cpp): load + normalise (bal_problem.cpp:773-852),
 optimize_lm_ours with the QR linearizor (solver/bal_bundle_adjustment.cpp:249-544), log (bal/ba_log.hpp)."""
@@ -51,6 +52,14 @@ def main():
                     help="after the solve, write the marginal covariances `cam` [nc, 9, 9] (tx,ty,tz, rx,ry,rz, f,k1,k2) and `lm` "
                          "[nl, 3, 3] at the final state (DESIGN.md section 16); the gauge must be fixed by priors or held "
                          "parameters")
+    ap.add_argument("--observation-info", default=None, metavar="FILE.npy",
+                    help="square-root information of the keypoints: an array [Nobs] (1 / sigma per observation) or [Nobs, 2, 2] "
+                         "(a square root W of the inverse 2x2 keypoint covariance) in the order of the loaded problem's "
+                         "observations, in the units of the loaded (normalised) image coordinates; zero switches an observation "
+                         "off (DESIGN.md section 19)")
+    ap.add_argument("--residuals", default=None, metavar="OUT.npz",
+                    help="after the solve, write per observation `residual` [Nobs, 2] (W r), `robust_weight` [Nobs] and `flags` "
+                         "[Nobs] (bit 0 = projection valid, bit 1 = in use) at the final state (DESIGN.md section 19)")
     args = ap.parse_args()
     try:
         fix_cameras = [int(v) for v in args.fix_cameras.split(",")] if args.fix_cameras else []
@@ -100,20 +109,38 @@ def main():
             problem.intrinsics_group = np.load(args.intrinsics_groups)
         except ValueError as e:
             ap.error(f"--intrinsics-groups: {e}")
+    if args.observation_info:
+        info = np.load(args.observation_info)
+        nobs = problem.num_observations()
+        if info.shape not in ((nobs,), (nobs, 2, 2)):
+            ap.error(f"--observation-info: {args.observation_info} has shape {info.shape}; the loaded problem has {nobs} observations"
+                     + (f" after --init-depth-threshold {args.init_depth_threshold} removed some" if args.init_depth_threshold > 0 else "")
+                     + f", so the array must have shape ({nobs},) or ({nobs}, 2, 2)")
+        try:
+            problem.observation_sqrt_info = info
+        except ValueError as e:
+            ap.error(f"--observation-info: {e}")
     options = rb.SolverOptions(max_num_iterations=args.max_num_iterations, preconditioner_type=args.preconditioner_type,
                                operator_form=args.operator_form, use_double=not args.float)
     summary = rb.bundle_adjust_manual(problem, options, verbose=True)
     print(summary["termination_type"], summary["message"])
     rb.save_ba_log(args.log_path, summary, problem, args.input, {"load": t_load, "optimize": summary["total_time"]})
     print("wrote", args.log_path)
-    if args.covariance:
-        lin = rb.LinearizorQR.create(problem, options)  # at the final state, with the same priors and held parameters
+    if args.covariance or args.residuals:
+        lin = rb.LinearizorQR.create(problem, options)  # at the final state, with the same priors, information and held parameters
         try:
-            cam, lm = lin.covariance()
+            if args.covariance:
+                cam, lm = lin.covariance()
+            if args.residuals:
+                res, hw, flags = lin.observation_residuals()
         finally:
             lin.close()
-        np.savez(args.covariance, cam=cam, lm=lm)
-        print("wrote", args.covariance)
+        if args.covariance:
+            np.savez(args.covariance, cam=cam, lm=lm)
+            print("wrote", args.covariance)
+        if args.residuals:
+            np.savez(args.residuals, residual=res, robust_weight=hw, flags=flags)
+            print("wrote", args.residuals)
 
 
 if __name__ == "__main__":

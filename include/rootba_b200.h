@@ -327,11 +327,43 @@ int32_t rba_set_landmark_prior(rba_handle* h, int32_t num, const int32_t* lm_idx
  * group's intrinsics covariance and its own pose-intrinsics cross terms, and the landmark blocks use the same matrix. */
 int32_t rba_set_intrinsics_groups(rba_handle* h, const int32_t* group);
 
+/* ---- Per-observation square-root information and residual read-back (DESIGN.md section 19) -- */
+
+/* Not in the reference, where every reprojection term has unit weight.  Observation o (index in the problem's CSR order, the
+ * order of obs_cam_idx / obs_xy) gets a row-major 2x2 W_o; its rows become sqrt(hw) W_o [Jp | Jl | r] and its cost
+ * rho(|W_o r|^2), rho the handle's robust norm, so the Huber parameter is in units of sigma.  W_o = Sigma_o^-1/2 (any square
+ * root: W need not be symmetric or triangular) is the Gaussian case, sqrt(w) I a scalar weight, rank 1 a constraint along one
+ * image direction, and W_o = 0 switches the observation off: it gives the all-zero rows of a projection dropped by
+ * use_valid_projections_only.  Projection validity (z >= eps_sqrt) does not depend on W.
+ * sqrt_info [4*num_observations of the full problem] Scalar, row-major 2x2 per observation in problem order;
+ * NULL = identity everywhere, the default.  Every rank of a sharded problem passes the same full array and keeps the
+ * entries of its own landmark shard.  An array that is the identity bit for bit is the same as NULL: the unmodified kernels
+ * run and every result is bit-identical to a handle that never had information set.
+ * rba_compute_error: all_error / valid_error sum rho(|W r|^2), all_residual_sum / valid_residual_sum sum |W r|.  A switched-off
+ * observation stays in all_num_obs (contributing 0) and is not counted in valid_num_obs, valid_error, valid_residual_sum,
+ * whatever its projection validity; a projection of it that is not finite neither clears is_numerically_valid nor fails
+ * rba_linearize.  Everything derived from the Jacobian uses the whitened rows: rba_get_jacobian_scaling, rba_get_rhs,
+ * rba_get_preconditioner, rba_right_multiply, rba_debug_get_block, rba_compute_covariance.
+ * After a successful call rba_solve returns RBA_ERR_STATE until the next rba_linearize; the device-resident increment and the
+ * cached error are discarded.  A non-finite entry -> RBA_ERR_INVALID_ARGUMENT, and the previous information stays in force.
+ * The information costs 4 Scalars per observation slot of device memory, counted in rba_workload_stats::device_bytes from
+ * the first call that sets one on. */
+int32_t rba_set_observation_info(rba_handle* h, const void* sqrt_info);
+
+/* Per observation at the handle's CURRENT state, in problem order; any pointer may be NULL (all NULL ->
+ * RBA_ERR_INVALID_ARGUMENT).  residual [2*Nobs] Scalar: the whitened residual W r (the raw r without observation
+ * info); robust_weight [Nobs] Scalar: hw of error_weight on |W r|^2 (1 with robust_norm NONE); flags [Nobs] uint8:
+ * bit 0 = projection valid (z >= eps_sqrt), bit 1 = in use (W != 0).  A sharded handle writes only the observations of
+ * its own landmark shard.  Needs no rba_linearize; changes nothing of the handle (scratch device memory is allocated for the
+ * call and freed before it returns). */
+int32_t rba_get_observation_residuals(rba_handle* h, void* residual, void* robust_weight, uint8_t* flags);
+
 /* ---- Marginal covariances (DESIGN.md section 16) ------------------------------------------ */
 
 /* Not in the reference.  DESIGN.md section 16.  The covariance of the Gauss-Newton step of the total objective (reprojection
  * terms + camera priors + pair priors) at lambda = 0 and the handle's current state: the inverse of H = J^T J, with J the rows
- * rba_linearize would build (sqrt(w)-weighted by the robust norm, the rows use_valid_projections_only drops set to zero), and
+ * rba_linearize would build (whitened by the observation information of rba_set_observation_info when it is set, sqrt(w)-weighted
+ * by the robust norm, the rows use_valid_projections_only drops set to zero), and
  * the parameters held by rba_set_camera_fixed as constants (their rows and columns are exactly 0).  Evaluated in float64 for
  * either Scalar; unscaled (no Jacobi scaling); independent of solver_type, operator_form, stage2_form, preconditioner_type and
  * the QR variant (bit-identical output within one Scalar).

@@ -69,7 +69,8 @@ __device__ __forceinline__ void cov_sym3_eig(double (&A)[9], double (&V)[9]) {
 // eigenvalues zero), and per landmark wl [9] = V Lambda^-1/2 (row-major; columns of dropped eigenvalues zero) and its rank.
 // LMP (landmark priors, DESIGN.md section 17): Hll += L^T L (unscaled, in double) for a landmark with prior slot
 // lmp_of_lm[lm] >= 0, so a landmark with fewer than 2 valid observations can be full rank.
-template <class S, bool LMP = false>
+// OBSW (observation information, DESIGN.md section 19): the rows are whitened in double, sqrt(w) W [Jp | Jl], w from |W r|^2.
+template <class S, bool LMP = false, bool OBSW = false>
 __global__ void __launch_bounds__(128) k_cov_landmark(DevPtrs<S> D, KOpts o, const int* __restrict__ lm_slot0,
                                                       const int* __restrict__ lm_n, int nl, double* __restrict__ jpw,
                                                       double* __restrict__ kb, double* __restrict__ wl, int* __restrict__ rank,
@@ -90,7 +91,8 @@ __global__ void __launch_bounds__(128) k_cov_landmark(DevPtrs<S> D, KOpts o, con
       double res[2], Jp[18], Jl[6];
       linearize_point<double, true>(obs, pw, cam, res, Jp, Jl);
       bool keep = true;
-      if (o.use_valid_projections_only) {  // the handle's own validity threshold (that of its Scalar)
+      if constexpr (OBSW) keep = !whiten_observation<double, true>(D.obs_W, s, res, Jp, Jl);
+      if (keep && o.use_valid_projections_only) {  // the handle's own validity threshold (that of its Scalar)
         double R[9];
         quat_to_rot(cam, R);
         const double z = R[6] * pw[0] + R[7] * pw[1] + R[8] * pw[2] + cam[6];

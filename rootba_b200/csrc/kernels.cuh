@@ -103,6 +103,9 @@ struct DevPtrs {
   const S* lmp_mean;         // [m][3] x0
   const S* lmp_L;            // [m][9] row-major square-root information L (unscaled)
   S* lmp_Lg;                 // [m][12] L diag(jls) (9, row-major) and g = L (x - x0) (3) of the last linearisation
+  // observation information (rba_set_observation_info, DESIGN.md section 19); nullptr = none (identity everywhere) in this
+  // shard.  Only the kernels' OBSW instances, k_obs_residuals and k_cov_landmark read it.
+  const S* obs_W;            // [nslots][4] row-major 2x2 square-root information W of each slot (padding slots zero)
 };
 
 // increment entries (tx,ty,tz, rx,ry,rz, f,k1,k2) held by a camera's RBA_FIX_* bits, as a 9-bit mask
@@ -181,6 +184,40 @@ __device__ __forceinline__ void error_weight(const KOpts& o, S rsq, S& err, S& w
   }
 }
 
+// Observation information (DESIGN.md section 19): res <- W res and, with JAC, the two rows of Jp and Jl <- W [row 0; row 1],
+// W = obs_W[slot] (row-major 2x2, stored in SW, applied in S).  Returns W == 0, the observation is switched off: then res,
+// Jp and Jl are set to zero whatever they held (a projection that is not finite must not survive as 0 * NaN).
+template <class S, bool JAC, class SW>
+__device__ __forceinline__ bool whiten_observation(const SW* __restrict__ obs_W, size_t slot, S* res, S* Jp, S* Jl) {
+  S W[4];
+  if constexpr (sizeof(SW) == 4) {
+    const float4 v = *reinterpret_cast<const float4*>(obs_W + 4 * slot);
+    W[0] = (S)v.x; W[1] = (S)v.y; W[2] = (S)v.z; W[3] = (S)v.w;
+  } else {
+    const double2 a = *reinterpret_cast<const double2*>(obs_W + 4 * slot), b = *reinterpret_cast<const double2*>(obs_W + 4 * slot + 2);
+    W[0] = (S)a.x; W[1] = (S)a.y; W[2] = (S)b.x; W[3] = (S)b.y;
+  }
+  const bool off = W[0] == S(0) && W[1] == S(0) && W[2] == S(0) && W[3] == S(0);
+  const S r0 = res[0], r1 = res[1];
+  res[0] = off ? S(0) : W[0] * r0 + W[1] * r1;
+  res[1] = off ? S(0) : W[2] * r0 + W[3] * r1;
+  if (JAC) {
+#pragma unroll
+    for (int c = 0; c < 9; ++c) {
+      const S a = Jp[c], b = Jp[9 + c];
+      Jp[c] = off ? S(0) : W[0] * a + W[1] * b;
+      Jp[9 + c] = off ? S(0) : W[2] * a + W[3] * b;
+    }
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      const S a = Jl[c], b = Jl[3 + c];
+      Jl[c] = off ? S(0) : W[0] * a + W[1] * b;
+      Jl[3 + c] = off ? S(0) : W[2] * a + W[3] * b;
+    }
+  }
+  return off;
+}
+
 template <class T>
 __device__ __forceinline__ T group_sum(T v, int G) {
   for (int o = G >> 1; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
@@ -241,8 +278,10 @@ __device__ __forceinline__ double block_sum_partials(const double* part, int n, 
 // ------------------------------------------------------------------------------------------------
 // K0  error  (ref: bal/bal_bundle_adjustment_helper.cpp:68-109, residual_info.cpp:97-110)
 //     thread per observation slot; accumulation in double; out partials [gridDim][6]
+//     OBSW (observation information, DESIGN.md section 19): the residual is W r; a switched-off observation (W == 0) counts
+//     in "all" only and its projection is not checked for finiteness.
 // ------------------------------------------------------------------------------------------------
-template <class S>
+template <class S, bool OBSW = false>
 __global__ void __launch_bounds__(256) k_error(DevPtrs<S> D, KOpts o, double* partials, int* bad_flag) {
   double acc[6] = {0, 0, 0, 0, 0, 0};  // all: n, err, res ; valid: n, err, res
   bool bad = false;
@@ -256,7 +295,8 @@ __global__ void __launch_bounds__(256) k_error(DevPtrs<S> D, KOpts o, double* pa
 #pragma unroll
     for (int k = 0; k < 10; ++k) cam[k] = cp[k];
     S res[2];
-    const bool pv = linearize_point<S, false>(obs, pw, cam, res, nullptr, nullptr);
+    bool pv = linearize_point<S, false>(obs, pw, cam, res, nullptr, nullptr);
+    if constexpr (OBSW) pv = !whiten_observation<S, false>(D.obs_W, s, res, nullptr, nullptr) && pv;
     if (!(finite_s(res[0]) && finite_s(res[1]))) bad = true;
     const S rsq = res[0] * res[0] + res[1] * res[1];
     S err, w;
@@ -271,6 +311,33 @@ __global__ void __launch_bounds__(256) k_error(DevPtrs<S> D, KOpts o, double* pa
   block_sum_store<6>(acc, partials);
 }
 
+// rba_get_observation_residuals: k_error per slot without the reduction.  res [nslots][2] = W r (r without observation
+// information), hw [nslots] = the robust weight of error_weight on |W r|^2, flags [nslots]: bit 0 = projection valid,
+// bit 1 = in use (W != 0).  Padding slots are not written.
+template <class S>
+__global__ void __launch_bounds__(256) k_obs_residuals(DevPtrs<S> D, KOpts o, S* __restrict__ res_out, S* __restrict__ hw_out,
+                                                       uint8_t* __restrict__ flags_out) {
+  const int s = blockIdx.x * blockDim.x + threadIdx.x;
+  if (s >= D.nslots) return;
+  const int lm = D.slot_lm[s];
+  if (lm < 0) return;
+  S obs[2] = {D.slot_xy[2 * s], D.slot_xy[2 * s + 1]};
+  S pw[3] = {D.lms[3 * lm], D.lms[3 * lm + 1], D.lms[3 * lm + 2]};
+  S cam[10];
+  const S* cp = D.cams + 10 * (size_t)D.slot_cam[s];
+#pragma unroll
+  for (int k = 0; k < 10; ++k) cam[k] = cp[k];
+  S res[2];
+  const bool pv = linearize_point<S, false>(obs, pw, cam, res, nullptr, nullptr);
+  const bool off = D.obs_W && whiten_observation<S, false>(D.obs_W, s, res, nullptr, nullptr);
+  S err, w;
+  error_weight(o, res[0] * res[0] + res[1] * res[1], err, w);
+  res_out[2 * (size_t)s] = res[0];
+  res_out[2 * (size_t)s + 1] = res[1];
+  hw_out[s] = w;
+  flags_out[s] = (uint8_t)((pv ? 1 : 0) | (off ? 0 : 2));
+}
+
 // sums [n][K] double partials -> out[K]   (single block)
 template <int K>
 __global__ void k_sum_partials(const double* part, int n, double* out) {
@@ -283,8 +350,9 @@ __global__ void k_sum_partials(const double* part, int n, double* out) {
 // ------------------------------------------------------------------------------------------------
 // K1a  squared column norms of sqrt(w) * Jp per observation  (ref: qr/impl/landmark_block_base.ipp:493-518)
 //      thread per slot -> yobs[slot][9]; reduced per camera by k_cam_reduce (deterministic)
+//      OBSW (observation information, DESIGN.md section 19): the norms of sqrt(w) * W Jp, w from |W r|^2
 // ------------------------------------------------------------------------------------------------
-template <class S>
+template <class S, bool OBSW = false>
 __global__ void __launch_bounds__(256) k_jp_norms(DevPtrs<S> D, KOpts o, int* bad_flag) {
   for (int s = blockIdx.x * blockDim.x + threadIdx.x; s < D.nslots; s += gridDim.x * blockDim.x) {
     const int lm = D.slot_lm[s];
@@ -297,6 +365,7 @@ __global__ void __launch_bounds__(256) k_jp_norms(DevPtrs<S> D, KOpts o, int* ba
     for (int k = 0; k < 10; ++k) cam[k] = cp[k];
     S res[2], Jp[18], Jl[6];
     const bool valid = linearize_point<S, true>(obs, pw, cam, res, Jp, Jl);
+    if constexpr (OBSW) whiten_observation<S, true>(D.obs_W, s, res, Jp, Jl);
     S out[9];
     if (!o.use_valid_projections_only || valid) {
       bool fin = finite_s(res[0]) && finite_s(res[1]);
@@ -673,7 +742,9 @@ __device__ __forceinline__ void rot_apply(const Rot<S>& g, S& x, S& y) {
 // ------------------------------------------------------------------------------------------------
 //   LMP (landmark priors, DESIGN.md section 17): the prior's squared column norms |L col c|^2 join the landmark's column
 //   norms behind jls (the scaling of the whole Jacobian), and lane 0 of the group writes L diag(jls) and g = L (x - x0).
-template <class S, bool GIVENS, bool LMP = false>
+//   OBSW (observation information, DESIGN.md section 19): the rows of an observation are sqrt(w) W [Jp | Jl | r], w from
+//   |W r|^2; W == 0 gives the all-zero record of a dropped projection.
+template <class S, bool GIVENS, bool LMP = false, bool OBSW = false>
 __global__ void __launch_bounds__(128) k_linearize_qr(DevPtrs<S> D, KOpts o, Scratch<S> sc, int* bad_flag, TileOrder to) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   using V2 = typename ST<S>::V2;
@@ -715,6 +786,7 @@ __global__ void __launch_bounds__(128) k_linearize_qr(DevPtrs<S> D, KOpts o, Scr
         for (int k = 0; k < 10; ++k) cam[k] = cp[k];
         S res[2], Jp[18], Jl[6];
         const bool valid = linearize_point<S, true>(obs, pw, cam, res, Jp, Jl);
+        if constexpr (OBSW) whiten_observation<S, true>(D.obs_W, s, res, Jp, Jl);
         if (!o.use_valid_projections_only || valid) {
           bool fin = finite_s(res[0]) && finite_s(res[1]);
 #pragma unroll

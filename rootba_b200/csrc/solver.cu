@@ -60,6 +60,8 @@ struct rba_handle {
   virtual int set_camera_pair_prior(int32_t num_pairs, const int32_t* pairs, const void* mean, const void* sqrt_info) = 0;
   virtual int set_landmark_prior(int32_t num, const int32_t* lm_idx, const void* mean, const void* sqrt_info) = 0;
   virtual int set_intrinsics_groups(const int32_t* group) = 0;
+  virtual int set_observation_info(const void* sqrt_info) = 0;
+  virtual int get_observation_residuals(void* residual, void* robust_weight, uint8_t* flags) = 0;
   virtual int compute_error(rba_residual_info* out) = 0;
   virtual int linearize() = 0;
   virtual int solve(double lambda, void* inc_out, rba_cg_summary* cg) = 0;
@@ -109,6 +111,7 @@ struct Solver : rba_handle {
   KOpts ko{};
   Layout L;
   int nc = 0, nl_total = 0;
+  long long nobs_total = 0;        // observations of the full problem (every shard)
   int device = 0;
   int sm_count = 132;
   cudaStream_t stream = nullptr;
@@ -213,6 +216,8 @@ struct Solver : rba_handle {
   uint8_t* d_grp_fixed = nullptr;  // [nc] the user's flags + RBA_FIX_INTRINSICS on every member but the lead
   S* d_grp_ve = nullptr;           // [9 nc] the expanded operator input P v
   S* d_grp_y = nullptr;            // [9 nc] the contracted operator output the vector step reads
+  // observation information (rba_set_observation_info, DESIGN.md section 19): D.obs_W points here while it is set
+  S* d_obs_W = nullptr;            // [nslots][4]
   rba_stage_timings tm{};
   EventPair ev_stage1, ev_stage2, ev_precond, ev_pcg, ev_backsub, ev_update, ev_error, ev_mv, ev_user;
   long long launches = 0;
@@ -366,6 +371,7 @@ struct Solver : rba_handle {
   int upload_layout(const rba_problem_view* pv) {
     nc = pv->num_cameras;
     nl_total = pv->num_landmarks;
+    nobs_total = pv->lm_obs_offset[nl_total];
     std::string msg = build_layout(nc, nl_total, pv->lm_obs_offset, pv->obs_cam_idx, opt.rank, opt.nranks, KPMAX, L);
     if (!msg.empty()) { g_err = msg; return RBA_ERR_INVALID_ARGUMENT; }
     // observation coordinates in slot order
@@ -547,6 +553,11 @@ struct Solver : rba_handle {
     CU(cudaFuncSetAttribute((k_linearize_qr<S, true, true>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)k1_smem));
     CU(cudaFuncSetAttribute((k_stage2<S, true, true>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)k2_smem));
     CU(cudaFuncSetAttribute((k_stage2<S, false, true>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)k2_smem));
+    // the observation-information instances (DESIGN.md section 19)
+    CU(cudaFuncSetAttribute((k_linearize_qr<S, false, false, true>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)k1_smem));
+    CU(cudaFuncSetAttribute((k_linearize_qr<S, true, false, true>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)k1_smem));
+    CU(cudaFuncSetAttribute((k_linearize_qr<S, false, true, true>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)k1_smem));
+    CU(cudaFuncSetAttribute((k_linearize_qr<S, true, true, true>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)k1_smem));
     k4_smem_small = (size_t)K4_WARPS * L.k4_scratch_per_warp * sizeof(S);
     if (k4_smem_small > 200 * 1024) { g_err = "matvec scratch exceeds shared memory"; return RBA_ERR_UNSUPPORTED; }
     CU(cudaFuncSetAttribute((k_matvec_large<S, K4_WARPS, KPMAX>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(k4_smem_small, 1024)));
@@ -993,6 +1004,67 @@ struct Solver : rba_handle {
     return priors_changed();
   }
 
+  // A square-root information W (row-major 2x2) per observation of the full problem (DESIGN.md section 19).  Part of the
+  // linearisation like the priors.  Every rank receives the full array and keeps the entries of its own landmark shard, in
+  // slot order.  NULL, or an identity bit for bit on every observation of the shard, = the unmodified kernels
+  // (D.obs_W == nullptr).  Every check runs before anything changes, so a rejected call leaves the previous information.
+  int set_observation_info(const void* sqrt_info_v) override {
+    const S* W = (const S*)sqrt_info_v;
+    bool any = false;
+    std::vector<S> w;
+    if (W) {
+      for (long long k = 0; k < 4 * nobs_total; ++k)
+        if (!std::isfinite((double)W[k])) {
+          g_err = "rba_set_observation_info: observation " + std::to_string(k / 4) + " has a non-finite sqrt_info";
+          return RBA_ERR_INVALID_ARGUMENT;
+        }
+      static const S eye[4] = {S(1), S(0), S(0), S(1)};
+      w.assign((size_t)4 * L.nslots, S(0));
+      for (int s = 0; s < L.nslots; ++s) {
+        if (L.slot_obs[s] < 0) continue;
+        const S* src = W + 4 * (size_t)L.slot_obs[s];
+        std::copy(src, src + 4, w.begin() + 4 * (size_t)s);
+        any = any || std::memcmp(src, eye, sizeof(eye)) != 0;
+      }
+    }
+    if (any) {
+      TRY(grow_upload(!d_obs_W, dbuf(d_obs_W, w.size(), &w)));
+      CU(cudaStreamSynchronize(stream));
+    }
+    D.obs_W = any ? d_obs_W : nullptr;
+    su_valid = s_valid = false;  // the assembled matrix belongs to the previous rows
+    return priors_changed();
+  }
+  // Per observation at the current state, in problem order (DESIGN.md section 19).  Nothing of the handle changes: the
+  // slot-ordered scratch is allocated for the call and freed before it returns.
+  int get_observation_residuals(void* residual, void* robust_weight, uint8_t* flags) override {
+    if (!residual && !robust_weight && !flags) {
+      g_err = "rba_get_observation_residuals: residual, robust_weight and flags are all NULL";
+      return RBA_ERR_INVALID_ARGUMENT;
+    }
+    const size_t ns = (size_t)L.nslots;
+    char* base = nullptr;
+    CU(cudaMalloc(&base, ns * (3 * sizeof(S) + 1)));
+    struct Scratch1 { char* p; ~Scratch1() { cudaFree(p); } } scratch{base};
+    S* d_res = (S*)base; S* d_hw = d_res + 2 * ns; uint8_t* d_fl = (uint8_t*)(d_hw + ns);
+    k_obs_residuals<S><<<(unsigned)((ns + 255) / 256), 256, 0, stream>>>(D, ko, d_res, d_hw, d_fl);
+    std::vector<S> res(2 * ns), hw(ns);
+    std::vector<uint8_t> fl(ns);
+    CU(cudaMemcpyAsync(res.data(), d_res, 2 * ns * sizeof(S), cudaMemcpyDeviceToHost, stream));
+    CU(cudaMemcpyAsync(hw.data(), d_hw, ns * sizeof(S), cudaMemcpyDeviceToHost, stream));
+    CU(cudaMemcpyAsync(fl.data(), d_fl, ns, cudaMemcpyDeviceToHost, stream));
+    CU(cudaStreamSynchronize(stream));
+    CU(cudaGetLastError());
+    for (size_t s = 0; s < ns; ++s) {
+      const long long ob = L.slot_obs[s];
+      if (ob < 0) continue;
+      if (residual) { ((S*)residual)[2 * ob] = res[2 * s]; ((S*)residual)[2 * ob + 1] = res[2 * s + 1]; }
+      if (robust_weight) ((S*)robust_weight)[ob] = hw[s];
+      if (flags) flags[ob] = fl[s];
+    }
+    return RBA_OK;
+  }
+
   // launch with optional programmatic dependent launch (the kernel may start before its predecessor in the stream has
   // finished and orders itself with griddepcontrol.wait) and optional thread-block-cluster dimension
   template <class... KArgs, class... Args>
@@ -1034,7 +1106,8 @@ struct Solver : rba_handle {
     if (error_cache_valid && error_cache_version == state_version) return RBA_OK;  // answered from the cache in finish
     int rc = start(ev_error); if (rc) return rc;
     CU(cudaMemsetAsync(d_flags, 0, 4 * sizeof(int), stream));
-    k_error<S><<<EBLOCKS, 256, 0, stream>>>(D, ko, d_epart, d_flags);
+    auto ke = D.obs_W ? k_error<S, true> : k_error<S>;  // OBSW: the whitened residuals (DESIGN.md section 19)
+    ke<<<EBLOCKS, 256, 0, stream>>>(D, ko, d_epart, d_flags);
     k_sum_partials<6><<<1, 256, 0, stream>>>(d_epart, EBLOCKS, d_red);
     launches += 2;
     if (n_lmp > 0) {  // + this shard's landmark priors' 1/2 |L e|^2, BEFORE the sum over the shards (landmark-owned)
@@ -1088,7 +1161,8 @@ struct Solver : rba_handle {
     int rc = start(ev_stage1); if (rc) return rc;
     CU(cudaMemsetAsync(d_flags, 0, 4 * sizeof(int), stream));
     // pass A: squared column norms of the weighted pose Jacobians -> pose_jacobian_scaling_
-    k_jp_norms<S><<<grid_for(L.nslots, 256, 8), 256, 0, stream>>>(D, ko, d_flags);
+    auto kn = D.obs_W ? k_jp_norms<S, true> : k_jp_norms<S>;
+    kn<<<grid_for(L.nslots, 256, 8), 256, 0, stream>>>(D, ko, d_flags);
     ++launches;
     rc = camera_reduce(d_csr_obs_slots, d_csr_obs_items, n_obs_items, d_csr_obs_item_ptr, D.diag2); if (rc) return rc;
     if (has_abs_prior) {  // prior Jacobian and its column norms (scaling from the whole Jacobian), after the sum over the shards
@@ -1106,10 +1180,13 @@ struct Solver : rba_handle {
     }
     k_scaling<S><<<(9 * nc + 255) / 256, 256, 0, stream>>>(D.diag2, D.scaling, 9 * nc, (S)ko.jacobi_eps);
     // pass B: linearize (scaled) + Jl scaling + Householder QR + panel write
-    // (+ the landmark priors' column norms, L~ and g: the LMP instances)
+    // (+ the landmark priors' column norms, L~ and g: the LMP instances; + the observation information: the OBSW instances)
     const bool lmp = D.lmp_slot != nullptr;
     auto k1 = opt.use_householder_marginalization ? (lmp ? k_linearize_qr<S, false, true> : k_linearize_qr<S, false>)
                                                   : (lmp ? k_linearize_qr<S, true, true> : k_linearize_qr<S, true>);  // ref: ipp:149-163 selects perform_qr_givens
+    if (D.obs_W)
+      k1 = opt.use_householder_marginalization ? (lmp ? k_linearize_qr<S, false, true, true> : k_linearize_qr<S, false, false, true>)
+                                               : (lmp ? k_linearize_qr<S, true, true, true> : k_linearize_qr<S, true, false, true>);
     k1<<<tile_grid(k1_max_blocks), TILE_WARPS * 32, k1_smem, stream>>>(D, ko, k1_sc, d_flags, order_k1);
     launches += 2;
     if (opt.preconditioner_type == 0 || opt.solver_type == 2) {
@@ -1848,10 +1925,10 @@ struct Solver : rba_handle {
     CU(cudaMemsetAsync(A, 0, (size_t)(np * np) * 8, stream));
     CU(cudaMemsetAsync(fail, 0x7f, 4, stream));
     const int wgrid = std::max(1, std::min((nl + 3) / 4, sm_count * 16));
-    if (n_lmp > 0)  // + L^T L of the landmark priors in Hll
-      k_cov_landmark<S, true><<<wgrid, 128, 0, stream>>>(D, ko, d_cov_lm_slot0, d_cov_lm_n, nl, jp, kb, wl, rk, d_lmp_of_lm);
-    else
-      k_cov_landmark<S><<<wgrid, 128, 0, stream>>>(D, ko, d_cov_lm_slot0, d_cov_lm_n, nl, jp, kb, wl, rk);
+    // LMP: + L^T L of the landmark priors in Hll; OBSW: the rows whitened by the observation information
+    auto kcov = n_lmp > 0 ? (D.obs_W ? k_cov_landmark<S, true, true> : k_cov_landmark<S, true>)
+                          : (D.obs_W ? k_cov_landmark<S, false, true> : k_cov_landmark<S>);
+    kcov<<<wgrid, 128, 0, stream>>>(D, ko, d_cov_lm_slot0, d_cov_lm_n, nl, jp, kb, wl, rk, n_lmp > 0 ? d_lmp_of_lm : nullptr);
     k_cov_assemble<<<std::max(1, std::min((cov_nblk + 7) / 8, sm_count * 8)), 256, 0, stream>>>(
         (const int2*)d_cov_blk_cam, d_cov_blk_ptr, (const int2*)d_cov_terms, cov_nblk, jp, kb, A, np);
     if (has_abs_prior || n_pairs > 0)
@@ -2171,6 +2248,10 @@ int32_t rba_set_landmark_prior(rba_handle* h, int32_t num, const int32_t* lm_idx
   return h->set_landmark_prior(num, lm_idx, mean, sqrt_info);
 }
 int32_t rba_set_intrinsics_groups(rba_handle* h, const int32_t* group) { return h->set_intrinsics_groups(group); }
+int32_t rba_set_observation_info(rba_handle* h, const void* sqrt_info) { return h->set_observation_info(sqrt_info); }
+int32_t rba_get_observation_residuals(rba_handle* h, void* residual, void* robust_weight, uint8_t* flags) {
+  return h->get_observation_residuals(residual, robust_weight, flags);
+}
 int32_t rba_compute_error(rba_handle* h, rba_residual_info* out) { return h->compute_error(out); }
 int32_t rba_linearize(rba_handle* h) { return h->linearize(); }
 

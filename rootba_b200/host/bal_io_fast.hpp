@@ -128,7 +128,7 @@ struct FileBuffer {
 
 }  // namespace detail
 
-// Held cameras and priors of a problem (not in the reference), forwarded by LinearizorQR::create; an empty field = none.
+// Held cameras, priors and observation information of a problem (not in the reference), forwarded by LinearizorQR::create; an empty field = none.
 // Both problem classes (BalProblemSoA, BalProblem) carry them.
 struct ProblemPriors {
   std::vector<uint8_t> camera_fixed;               // [nc] RBA_FIX_* bits (rba_set_camera_fixed)
@@ -144,6 +144,8 @@ struct ProblemPriors {
   std::vector<int32_t> landmark_prior_idx;         // [m] landmark indices
   std::vector<double> landmark_prior_mean;         // [m][3] prior position x0
   std::vector<double> landmark_prior_sqrt_info;    // [m][9] row-major square-root information L
+  // Square-root information of the observations (rba_set_observation_info)
+  std::vector<double> obs_sqrt_info;               // [nobs][4] row-major 2x2 W in the order of the observations; 0 = switched off
 };
 
 // Flat mirror of rootba::BalProblem<Scalar> with the member surface LinearizorQR / bundle_adjust_manual need.

@@ -206,6 +206,12 @@ class LinearizorQR {
       const VecX L(bp.landmark_prior_sqrt_info.begin(), bp.landmark_prior_sqrt_info.end());
       check(rba_set_landmark_prior(h_, (int32_t)np, bp.landmark_prior_idx.data(), m.data(), L.data()));
     }
+    if (!bp.obs_sqrt_info.empty()) {
+      if ((int64_t)bp.obs_sqrt_info.size() != 4 * (int64_t)bp.num_observations())
+        throw std::runtime_error("obs_sqrt_info must have 4 entries (a row-major 2x2) per observation");
+      const VecX W(bp.obs_sqrt_info.begin(), bp.obs_sqrt_info.end());
+      check(rba_set_observation_info(h_, W.data()));
+    }
   }
   Problem& bal_problem_;
   SolverSummary* summary_ = nullptr;

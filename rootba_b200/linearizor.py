@@ -155,6 +155,23 @@ def _landmark_prior_arrays(prior, num_landmarks: int, dtype):
     return (idx, *_prior_arrays("landmark_prior", mean, sqrt_info, dtype, m, 3, 3, check_index))
 
 
+def _observation_info_array(info, num_observations: int, dtype):
+    """None, or a validated contiguous copy [Nobs, 2, 2] in `dtype` of per-observation square-root information given as
+    [Nobs] (1 / sigma, expanded to I / sigma) or [Nobs, 2, 2]"""
+    if info is None:
+        return None
+    a = np.array(info, dtype=dtype, order="C", copy=True)
+    if a.shape == (num_observations,):
+        w = np.zeros((num_observations, 2, 2), dtype)
+        w[:, 0, 0] = w[:, 1, 1] = a
+        a = w
+    if a.shape != (num_observations, 2, 2):
+        raise ValueError(f"observation_sqrt_info must have shape ({num_observations},) or ({num_observations}, 2, 2), got {a.shape}")
+    if not np.all(np.isfinite(a)):
+        raise ValueError("observation_sqrt_info entries must be finite")
+    return a
+
+
 class BalProblem:
     """SoA BalProblem: cameras [nc,10] (quat xyzw, t, f,k1,k2), landmarks [nl,3], observations in
     CSR-by-landmark order with ascending camera index.  `camera_fixed` (not in the reference): None or one uint8 of FIX_*
@@ -168,7 +185,11 @@ class BalProblem:
     `landmark_prior` (not in the reference): None or (idx [m] int32, mean [m,3], sqrt_info [m,3,3]), Gaussian priors on
     landmark positions with the cost 1/2 |L (x - x0)|^2 (rba_set_landmark_prior, DESIGN.md section 17).  Forwarded likewise.
     `intrinsics_group` (not in the reference): None or one int32 group id per camera (-1 = own intrinsics); the cameras of a
-    group share one f, k1, k2 (rba_set_intrinsics_groups, DESIGN.md section 18).  Forwarded likewise."""
+    group share one f, k1, k2 (rba_set_intrinsics_groups, DESIGN.md section 18).  Forwarded likewise.
+    `observation_sqrt_info` (not in the reference): None, [Nobs] (1 / sigma per observation) or [Nobs,2,2] (a square root W of
+    the inverse keypoint covariance per observation, in the order of obs_cam / obs_xy); the observation's cost becomes
+    rho(|W r|^2) and W = 0 switches it off (rba_set_observation_info, DESIGN.md section 19).  Stored as [Nobs,2,2]; forwarded
+    likewise."""
 
     def __init__(self, cams, lms, lm_off, obs_cam, obs_xy, dtype=np.float64):
         self.dtype = np.dtype(dtype)
@@ -186,6 +207,18 @@ class BalProblem:
         self._camera_pair_prior = None
         self._landmark_prior = None
         self._intrinsics_group = None
+        self._observation_sqrt_info = None
+
+    @property
+    def observation_sqrt_info(self):
+        return self._observation_sqrt_info
+
+    @observation_sqrt_info.setter
+    def observation_sqrt_info(self, info):
+        w = _observation_info_array(info, self.num_observations(), self.dtype)
+        if self._linearizor is not None:
+            self._linearizor._upload_observation_info(w)  # raises on rejection: the previous information stays in force
+        self._observation_sqrt_info = w
 
     @property
     def intrinsics_group(self):
@@ -351,6 +384,8 @@ class LinearizorQR:
             self._upload_landmark_prior(bal_problem.landmark_prior)
         if bal_problem.intrinsics_group is not None:
             self._upload_intrinsics_group(bal_problem.intrinsics_group)
+        if bal_problem.observation_sqrt_info is not None:
+            self._upload_observation_info(bal_problem.observation_sqrt_info)
 
     # factory like Linearizor::create (linearizor.cpp:47-65)
     @staticmethod
@@ -427,6 +462,24 @@ class LinearizorQR:
 
     def _upload_intrinsics_group(self, group):
         check(_lib.lib().rba_set_intrinsics_groups(self.h, None if group is None else _p(group)))
+
+    def set_observation_info(self, info):
+        """per-observation square-root information (rba_set_observation_info): None, [Nobs] (1 / sigma) or [Nobs,2,2] in the
+        order of the problem's observations; zero switches an observation off.  Needs a new linearize before the next solve;
+        the information is stored on the BalProblem."""
+        self.bal_problem.observation_sqrt_info = info  # validates and forwards to _upload_observation_info
+
+    def _upload_observation_info(self, info):
+        check(_lib.lib().rba_set_observation_info(self.h, None if info is None else _p(info)))
+
+    def observation_residuals(self):
+        """per observation at the current state, in the order of the problem's observations (rba_get_observation_residuals):
+        (residual [Nobs,2] = W r, robust_weight [Nobs], flags [Nobs] uint8: bit 0 = projection valid, bit 1 = in use).  A
+        sharded handle fills only the observations of its own landmark shard (the others stay 0)."""
+        nobs = self.bal_problem.num_observations()
+        res, hw, flags = np.zeros((nobs, 2), self.dtype), np.zeros(nobs, self.dtype), np.zeros(nobs, np.uint8)
+        check(_lib.lib().rba_get_observation_residuals(self.h, _p(res), _p(hw), _p(flags)))
+        return res, hw, flags
 
     def _backup(self):
         check(_lib.lib().rba_backup(self.h))
