@@ -4,7 +4,7 @@
     python examples/solve_bal.py problem-49-7776-pre.txt [--float] [--max-num-iterations 20] [--operator-form DENSE|IMPLICIT]
         [--fix-intrinsics] [--fix-cameras I,J,...] [--camera-prior FILE.npz] [--camera-pair-prior FILE.npz]
         [--landmark-prior FILE.npz] [--shared-intrinsics | --intrinsics-groups FILE.npy] [--covariance OUT.npz]
-        [--observation-info FILE.npy] [--residuals OUT.npz]
+        [--relative-covariance PAIRS.npy] [--observation-info FILE.npy] [--residuals OUT.npz]
 
 Mirrors what `bal_qr --input ...` of the reference does (src/app/bal_qr.cpp): load + normalise (bal_problem.cpp:773-852),
 optimize_lm_ours with the QR linearizor (solver/bal_bundle_adjustment.cpp:249-544), log (bal/ba_log.hpp)."""
@@ -52,6 +52,10 @@ def main():
                     help="after the solve, write the marginal covariances `cam` [nc, 9, 9] (tx,ty,tz, rx,ry,rz, f,k1,k2) and `lm` "
                          "[nl, 3, 3] at the final state (DESIGN.md section 16); the gauge must be fixed by priors or held "
                          "parameters")
+    ap.add_argument("--relative-covariance", default=None, metavar="PAIRS.npy",
+                    help="with --covariance: an int array [m, 2] of camera pairs (i, j), i != j; adds to the --covariance file "
+                         "`relative` [m, 6, 6], the covariance of the relative pose T_i T_j^-1 as the residual (e_t, e_r) of "
+                         "--camera-pair-prior at the final state, and `relative_pairs` (DESIGN.md section 20)")
     ap.add_argument("--observation-info", default=None, metavar="FILE.npy",
                     help="square-root information of the keypoints: an array [Nobs] (1 / sigma per observation) or [Nobs, 2, 2] "
                          "(a square root W of the inverse 2x2 keypoint covariance) in the order of the loaded problem's "
@@ -61,6 +65,14 @@ def main():
                     help="after the solve, write per observation `residual` [Nobs, 2] (W r), `robust_weight` [Nobs] and `flags` "
                          "[Nobs] (bit 0 = projection valid, bit 1 = in use) at the final state (DESIGN.md section 19)")
     args = ap.parse_args()
+    if args.relative_covariance and not args.covariance:
+        ap.error("--relative-covariance requires --covariance")
+    rel_pairs = None
+    if args.relative_covariance:
+        rel_pairs = np.load(args.relative_covariance)
+        if rel_pairs.ndim != 2 or rel_pairs.shape[1] != 2 or not np.issubdtype(rel_pairs.dtype, np.integer):
+            ap.error(f"--relative-covariance: {args.relative_covariance} must hold an int array [m, 2], got {rel_pairs.dtype} "
+                     f"{rel_pairs.shape}")
     try:
         fix_cameras = [int(v) for v in args.fix_cameras.split(",")] if args.fix_cameras else []
     except ValueError:
@@ -129,14 +141,15 @@ def main():
     if args.covariance or args.residuals:
         lin = rb.LinearizorQR.create(problem, options)  # at the final state, with the same priors, information and held parameters
         try:
-            if args.covariance:
-                cam, lm = lin.covariance()
+            if args.covariance:  # one factorisation for the marginals and the relative poses
+                blocks = lin.covariance_blocks(relative=rel_pairs, marginals=True)
             if args.residuals:
                 res, hw, flags = lin.observation_residuals()
         finally:
             lin.close()
         if args.covariance:
-            np.savez(args.covariance, cam=cam, lm=lm)
+            extra = {} if rel_pairs is None else dict(relative=blocks["relative"], relative_pairs=rel_pairs)
+            np.savez(args.covariance, cam=blocks["cam"], lm=blocks["lm"], **extra)
             print("wrote", args.covariance)
         if args.residuals:
             np.savez(args.residuals, residual=res, robust_weight=hw, flags=flags)

@@ -379,6 +379,44 @@ int32_t rba_get_observation_residuals(rba_handle* h, void* residual, void* robus
  * RBA_ERR_INVALID_ARGUMENT: both pointers NULL. */
 int32_t rba_compute_covariance(rba_handle* h, double* cam_cov, double* lm_cov);
 
+/* ---- Covariance blocks (DESIGN.md section 20) ------------------------------------------------ */
+
+/* Not in the reference.  DESIGN.md section 20.  Blocks of the same covariance H^-1 as rba_compute_covariance (same H, held
+ * parameters, intrinsics groups, priors, observation information, robust weights and validity; float64 for either Scalar;
+ * increments (tx,ty,tz, rx,ry,rz, f,k1,k2) per camera and (x,y,z) per landmark in problem order), for chosen pairs, from one
+ * factorisation.  Output k belongs to request k; repeated requests and any order are allowed.
+ *   camera_cross [81*k]: Cov(d_a, d_b), 9x9 row-major, rows of camera a; (a, a) is bit-identical to cam_cov[a], (b, a) is the
+ *     transpose of (a, b) to one rounding; the rows and columns of held entries are 0.
+ *   camera_landmark_cross [27*k]: Cov(d_c, d_l), 9x3 row-major.
+ *   landmark_cross [9*k]: Cov(d_l, d_m), 3x3 row-major; (l, l) is bit-identical to lm_cov[l].
+ *   relative_cov [36*k]: the 6x6 covariance of the pair-prior residual e = (e_t, e_r) of rba_set_camera_pair_prior for the
+ *     pair (i, j) (i != j), linearised at the current state with its mean at the current relative pose
+ *     (R0 = R_i R_j^T, t0 = t_i - R_i R_j^T t_j): A Sigma A^T with A = [[I, -[t_rel]x, -M, 0], [0, I, 0, -M]] on
+ *     (v_i, w_i, v_j, w_j), M = R_i R_j^T.  That mean with any L with L^T L = relative_cov^-1, given to
+ *     rba_set_camera_pair_prior, carries the same first-order information on that relative pose.  Exactly symmetric; 0 between
+ *     two cameras whose poses are held.
+ *   cam_cov, lm_cov: optional (NULL: skipped), exactly rba_compute_covariance's outputs.
+ * Every block that involves a landmark whose Jl^T Jl has rank < 3 is all NaN; the other blocks stay valid.
+ * No prior rba_linearize is needed and nothing of the handle changes; scratch device memory is allocated for the call and freed
+ * before it returns.  On every failure the outputs are not written:
+ * RBA_ERR_INVALID_ARGUMENT (checked before any device work): q NULL, a negative count, a NULL array with a positive count, an
+ *   index out of range, i == j for a relative pose, or nothing requested (all counts 0 and both marginal pointers NULL).
+ * RBA_NUMERICAL_FAILURE, RBA_ERR_UNSUPPORTED: as rba_compute_covariance (the byte count includes the requests and outputs). */
+typedef struct {
+  int32_t num_camera_pairs, num_camera_landmark, num_landmark_pairs, num_relative_poses;
+  const int32_t* camera_pairs;      /* [2*num_camera_pairs]     (a, b), 0 <= a, b < Nc                    */
+  const int32_t* camera_landmark;   /* [2*num_camera_landmark]  (c, l), camera c, landmark l (problem order) */
+  const int32_t* landmark_pairs;    /* [2*num_landmark_pairs]   (l, m)                                     */
+  const int32_t* relative_pairs;    /* [2*num_relative_poses]   (i, j), i != j                             */
+  double* camera_cross;             /* [81*num_camera_pairs]                                                */
+  double* camera_landmark_cross;    /* [27*num_camera_landmark]                                             */
+  double* landmark_cross;           /* [9*num_landmark_pairs]                                               */
+  double* relative_cov;             /* [36*num_relative_poses]                                              */
+  double* cam_cov;                  /* [81*Nc] or NULL                                                      */
+  double* lm_cov;                   /* [9*Nl] or NULL                                                       */
+} rba_covariance_query;             /* no implicit padding: 16 + 10*8 = 96 bytes on LP64 */
+int32_t rba_compute_covariance_blocks(rba_handle* h, const rba_covariance_query* q);
+
 /* ---- Linearizor interface (solver/linearizor.hpp:56-82) ---------------------------------- */
 
 /* LinearizorBase::compute_error (linearizor_base.cpp:59-67) -> BalBundleAdjustmentHelper::compute_error

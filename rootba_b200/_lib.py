@@ -92,6 +92,14 @@ class WorkloadStats(C.Structure):
                 ("landmark_end", C.c_int32), ("num_matvec_items", C.c_int32), ("reserved_", C.c_int32)]
 
 
+class CovarianceQuery(C.Structure):
+    _fields_ = [("num_camera_pairs", C.c_int32), ("num_camera_landmark", C.c_int32), ("num_landmark_pairs", C.c_int32),
+                ("num_relative_poses", C.c_int32), ("camera_pairs", C.c_void_p), ("camera_landmark", C.c_void_p),
+                ("landmark_pairs", C.c_void_p), ("relative_pairs", C.c_void_p), ("camera_cross", C.c_void_p),
+                ("camera_landmark_cross", C.c_void_p), ("landmark_cross", C.c_void_p), ("relative_cov", C.c_void_p),
+                ("cam_cov", C.c_void_p), ("lm_cov", C.c_void_p)]
+
+
 def struct_to_dict(s: C.Structure) -> dict:
     out = {}
     for name, _ in s._fields_:
@@ -130,6 +138,7 @@ def lib():
         _lib.rba_last_error.restype = C.c_char_p
         _lib.rba_stream.restype = C.c_void_p
         _lib.rba_compute_covariance.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+        _lib.rba_compute_covariance_blocks.argtypes = [C.c_void_p, C.POINTER(CovarianceQuery)]
         _lib.rba_set_landmark_prior.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
     return _lib
 

@@ -11,6 +11,8 @@
 //      FP64 tensor-core GEMM (mma.sync m8n8k4 .f64) for every O(N^3) update
 //   4. k_cov_cam_out      9x9 diagonal blocks of D S^-1 D;  k_cov_lm_marginal  per landmark
 //                         W (I + sum_ab K_a S^-1_ab K_b^T) W^T,  W = V Lambda^-1/2
+//   5. (rba_compute_covariance_blocks, DESIGN.md section 20) k_cov_cam_cross, k_cov_cam_lm, k_cov_lm_cross, k_cov_rel_pose:
+//                         the blocks of chosen camera pairs, camera-landmark pairs, landmark pairs and relative poses
 // The dense matrix is column-major with a leading dimension padded to a multiple of COV_TB; only its lower triangle is
 // meaningful.
 #pragma once
@@ -464,6 +466,61 @@ __global__ void k_cov_cam_out(const double* __restrict__ A, long long ld, const 
   out[e] = cov_sinv(A, ld, d, cam_fixed, 9 * c + p, 9 * c + q);
 }
 
+// One warp: the 3x3 block W_l (delta_lm I + sum_ab K_a Sigma_ab K_b^T) W_m^T of landmarks l and m (a over the slots of l,
+// b over those of m), lanes over the n_l n_m slot pairs, fixed-order butterfly sum, written by lane 0 to out [9]; all NaN
+// when the Hll of either has rank < 3.  With l == m it performs k_cov_lm_marginal's operations in its order (same lane
+// partition, butterfly and final products), so (l, l) is bit-identical to lm_cov[l].  k_cov_lm_marginal itself is left as
+// it was, so that rba_compute_covariance keeps its instructions.
+__device__ __forceinline__ void cov_lm_block(const double* __restrict__ A, long long ld, const double* __restrict__ d,
+                                             const uint8_t* __restrict__ cam_fixed, const int* __restrict__ slot_cam,
+                                             const int* __restrict__ lm_slot0, const int* __restrict__ lm_n,
+                                             const double* __restrict__ kb, const double* __restrict__ wl,
+                                             const int* __restrict__ rank, int l, int m, int lane, double* __restrict__ out) {
+  if (rank[l] < 3 || rank[m] < 3) {
+    if (lane < 9) out[lane] = __longlong_as_double(0x7ff8000000000000LL);
+    return;
+  }
+  const int s0 = lm_slot0[l], n = lm_n[l], s1 = lm_slot0[m], nm = lm_n[m];
+  double acc[9];
+#pragma unroll
+  for (int k = 0; k < 9; ++k) acc[k] = 0.0;
+  for (int t = lane; t < n * nm; t += 32) {
+    const int a = t / nm, b = t % nm;
+    const long long ra = 9LL * slot_cam[s0 + a], rb = 9LL * slot_cam[s1 + b];
+    const double* ka = kb + 27 * (size_t)(s0 + a);
+    const double* kq = kb + 27 * (size_t)(s1 + b);
+    for (int p = 0; p < 9; ++p) {
+      double u[3] = {0.0, 0.0, 0.0};  // (Sigma_ab K_b^T) row p
+      for (int q = 0; q < 9; ++q) {
+        const double sv = cov_sinv(A, ld, d, cam_fixed, ra + p, rb + q);
+#pragma unroll
+        for (int j = 0; j < 3; ++j) u[j] += sv * kq[9 * j + q];
+      }
+#pragma unroll
+      for (int k = 0; k < 3; ++k)
+#pragma unroll
+        for (int j = 0; j < 3; ++j) acc[3 * k + j] += ka[9 * k + p] * u[j];
+    }
+  }
+#pragma unroll
+  for (int k = 0; k < 9; ++k) acc[k] = warp_sum(acc[k]);
+  if (lane == 0) {
+    const double* Wl = wl + 9 * (size_t)l;
+    const double* Wm = wl + 9 * (size_t)m;
+    const double diag = l == m ? 1.0 : 0.0;
+    double X[9];
+#pragma unroll
+    for (int k = 0; k < 9; ++k) X[k] = acc[k] + (k % 4 == 0 ? diag : 0.0);
+    for (int r = 0; r < 3; ++r)
+      for (int c = 0; c < 3; ++c) {
+        double v = 0.0;
+        for (int k = 0; k < 3; ++k)
+          for (int j = 0; j < 3; ++j) v += Wl[3 * r + k] * X[3 * k + j] * Wm[3 * c + j];
+        out[3 * r + c] = v;
+      }
+  }
+}
+
 // lm_cov [nl][9], warp per landmark: W (I + sum_ab K_a Sigma_ab K_b^T) W^T over the n^2 camera pairs of its track (lanes
 // over the pairs, fixed-order butterfly sum); all NaN when Hll has rank < 3.
 __global__ void __launch_bounds__(128) k_cov_lm_marginal(const double* __restrict__ A, long long ld, const double* __restrict__ d,
@@ -514,6 +571,135 @@ __global__ void __launch_bounds__(128) k_cov_lm_marginal(const double* __restric
             for (int l = 0; l < 3; ++l) v += W[3 * r + k] * X[3 * k + l] * W[3 * c + l];
           out[9 * (size_t)lm + 3 * r + c] = v;
         }
+    }
+  }
+}
+
+
+// ------------------------------------------------------------------------------------------------
+// 5. covariance blocks of chosen pairs (rba_compute_covariance_blocks, DESIGN.md section 20).  Grid-stride loops over the
+//    requests, fixed-order sums, no atomics: the same output on every run, and request k depends on request k alone.
+// ------------------------------------------------------------------------------------------------
+// camera_cross [m][81] = Cov(d_a, d_b) of the requests (a, b), thread per entry; (a, a) is k_cov_cam_out's block a.
+__global__ void __launch_bounds__(256) k_cov_cam_cross(const double* __restrict__ A, long long ld, const double* __restrict__ d,
+                                                       const uint8_t* __restrict__ cam_fixed, const int2* __restrict__ req, int m,
+                                                       double* __restrict__ out) {
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < 81LL * m; e += stride) {
+    const int2 ab = req[e / 81];
+    const int p = (int)(e % 81) / 9, q = (int)(e % 9);
+    out[e] = cov_sinv(A, ld, d, cam_fixed, 9LL * ab.x + p, 9LL * ab.y + q);
+  }
+}
+
+// camera_landmark_cross [m][27] = Cov(d_c, d_l) = -(sum_i Sigma_{c,a_i} K_i^T) W_l^T of the requests (c, l), warp per request,
+// lanes over the slots i of landmark l (camera a_i), fixed-order butterfly sum; all NaN when Hll has rank < 3.
+__global__ void __launch_bounds__(128) k_cov_cam_lm(const double* __restrict__ A, long long ld, const double* __restrict__ d,
+                                                    const uint8_t* __restrict__ cam_fixed, const int* __restrict__ slot_cam,
+                                                    const int* __restrict__ lm_slot0, const int* __restrict__ lm_n,
+                                                    const double* __restrict__ kb, const double* __restrict__ wl,
+                                                    const int* __restrict__ rank, const int2* __restrict__ req, int m,
+                                                    double* __restrict__ out) {
+  const int lane = threadIdx.x & 31;
+  const int warps = gridDim.x * (blockDim.x >> 5);
+  for (int k = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); k < m; k += warps) {
+    const int2 cl = req[k];
+    double* o = out + 27 * (size_t)k;
+    if (rank[cl.y] < 3) {
+      if (lane < 27) o[lane] = __longlong_as_double(0x7ff8000000000000LL);
+      continue;
+    }
+    const int s0 = lm_slot0[cl.y], n = lm_n[cl.y];
+    const long long rc = 9LL * cl.x;
+    double u[27];  // (sum_i Sigma_{c,a_i} K_i^T) [9][3]
+#pragma unroll
+    for (int e = 0; e < 27; ++e) u[e] = 0.0;
+    for (int i = lane; i < n; i += 32) {
+      const long long ra = 9LL * slot_cam[s0 + i];
+      const double* ki = kb + 27 * (size_t)(s0 + i);
+#pragma unroll
+      for (int p = 0; p < 9; ++p)
+        for (int q = 0; q < 9; ++q) {
+          const double sv = cov_sinv(A, ld, d, cam_fixed, rc + p, ra + q);
+#pragma unroll
+          for (int j = 0; j < 3; ++j) u[3 * p + j] += sv * ki[9 * j + q];
+        }
+    }
+#pragma unroll
+    for (int e = 0; e < 27; ++e) u[e] = warp_sum(u[e]);
+    if (lane == 0) {
+      const double* W = wl + 9 * (size_t)cl.y;
+#pragma unroll
+      for (int p = 0; p < 9; ++p)
+#pragma unroll
+        for (int r = 0; r < 3; ++r) o[3 * p + r] = -(u[3 * p] * W[3 * r] + u[3 * p + 1] * W[3 * r + 1] + u[3 * p + 2] * W[3 * r + 2]);
+    }
+  }
+}
+
+// landmark_cross [m][9] = Cov(d_l, d_m) of the requests (l, m), warp per request (cov_lm_block: (l, l) is l's marginal)
+__global__ void __launch_bounds__(128) k_cov_lm_cross(const double* __restrict__ A, long long ld, const double* __restrict__ d,
+                                                      const uint8_t* __restrict__ cam_fixed, const int* __restrict__ slot_cam,
+                                                      const int* __restrict__ lm_slot0, const int* __restrict__ lm_n,
+                                                      const double* __restrict__ kb, const double* __restrict__ wl,
+                                                      const int* __restrict__ rank, const int2* __restrict__ req, int m,
+                                                      double* __restrict__ out) {
+  const int lane = threadIdx.x & 31;
+  const int warps = gridDim.x * (blockDim.x >> 5);
+  for (int k = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); k < m; k += warps)
+    cov_lm_block(A, ld, d, cam_fixed, slot_cam, lm_slot0, lm_n, kb, wl, rank, req[k].x, req[k].y, lane, out + 9 * (size_t)k);
+}
+
+// relative_cov [m][36] of the requests (i, j), thread per request: the covariance A Sigma_P A^T of the pair-prior residual
+// e = (e_t, e_r) at the mean equal to the current relative pose (e = 0, J_l^-1 = I), Sigma_P [12][12] the pose entries
+// (v_i, w_i, v_j, w_j) of the joint block of cameras i and j, A = [A_i | A_j] the rows pair_jac_rows builds with L = I.
+// Each thread keeps its A [6][12] in shared memory, entry-major (a warp's accesses are conflict-free): in registers it would
+// need dynamic indexing, and holding Sigma_P instead spills.  The lower triangle is computed and mirrored, so the output is
+// exactly symmetric.
+constexpr int COV_REL_THREADS = 64;
+template <class S>
+__global__ void __launch_bounds__(COV_REL_THREADS) k_cov_rel_pose(const double* __restrict__ A, long long ld, const double* __restrict__ d,
+                                                                  const uint8_t* __restrict__ cam_fixed, const S* __restrict__ cams,
+                                                                  const int2* __restrict__ req, int m, double* __restrict__ out) {
+  __shared__ double As[72][COV_REL_THREADS];
+  const int tid = threadIdx.x;
+  const int stride = gridDim.x * blockDim.x;
+  for (int k = blockIdx.x * blockDim.x + tid; k < m; k += stride) {
+    const int2 ij = req[k];
+    double ci[10], cj[10];
+#pragma unroll
+    for (int e = 0; e < 10; ++e) { ci[e] = (double)cams[10 * (size_t)ij.x + e]; cj[e] = (double)cams[10 * (size_t)ij.y + e]; }
+    const double ident[7] = {0.0, 0.0, 0.0, 1.0, 0.0, 0.0, 0.0};  // e is not used: only M and t_rel
+    const double I3[9] = {1.0, 0.0, 0.0, 0.0, 1.0, 0.0, 0.0, 0.0, 1.0};
+    double e6[6], M[9], tr[3];
+    pair_residual<double, false>(ci, cj, ident, e6, M, tr, nullptr, nullptr);
+    for (int r = 0; r < 6; ++r) {  // row r of A: the rows of pair_jac_rows for the row e_r of L = I
+      double l[6], ri[6], rj[6];
+#pragma unroll
+      for (int q = 0; q < 6; ++q) l[q] = q == r ? 1.0 : 0.0;
+      pair_jac_rows(l, M, tr, I3, M, ri, rj);
+#pragma unroll
+      for (int q = 0; q < 6; ++q) { As[12 * r + q][tid] = ri[q]; As[12 * r + 6 + q][tid] = rj[q]; }
+    }
+    auto idx = [&](int q) { return q < 6 ? 9LL * ij.x + q : 9LL * ij.y + q - 6; };
+    double* o = out + 36 * (size_t)k;
+    for (int r = 0; r < 6; ++r) {
+      double t[12];  // row r of A Sigma_P
+#pragma unroll
+      for (int q = 0; q < 12; ++q) t[q] = 0.0;
+      for (int p = 0; p < 12; ++p) {
+        const double arp = As[12 * r + p][tid];
+        const long long rp = idx(p);
+#pragma unroll
+        for (int q = 0; q < 12; ++q) t[q] += arp * cov_sinv(A, ld, d, cam_fixed, rp, idx(q));
+      }
+      for (int c = 0; c <= r; ++c) {
+        double v = 0.0;
+#pragma unroll
+        for (int q = 0; q < 12; ++q) v += t[q] * As[12 * c + q][tid];
+        o[6 * r + c] = v;
+        o[6 * c + r] = v;
+      }
     }
   }
 }

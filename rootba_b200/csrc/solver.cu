@@ -76,6 +76,7 @@ struct rba_handle {
   virtual int right_multiply(const void* x, void* y) = 0;
   virtual int debug_get_block(int lm, void* out, int rows, int cols, void* jls) = 0;
   virtual int compute_covariance(double* cam_cov, double* lm_cov) = 0;
+  virtual int compute_covariance_blocks(const rba_covariance_query* q) = 0;
   virtual int time_matvec(int reps, double* sec) = 0;
   virtual int timer_start() = 0;
   virtual int timer_stop(double* sec) = 0;
@@ -1891,10 +1892,23 @@ struct Solver : rba_handle {
     CU(cudaGetLastError());
     return RBA_OK;
   }
-  int compute_covariance(double* cam_cov, double* lm_cov) override {
-    if (!cam_cov && !lm_cov) { g_err = "rba_compute_covariance: cam_cov and lm_cov are both NULL"; return RBA_ERR_INVALID_ARGUMENT; }
+  // The dense inverse of one covariance call and what its extraction kernels read; the scratch is freed (after the kernels
+  // have finished: cudaFree waits for them) when it goes out of scope.
+  struct CovInverse {
+    char* base = nullptr;
+    ~CovInverse() { cudaFree(base); }
+    double* A = nullptr;  // S_eq^-1 (lower triangle, leading dimension np); cov_sinv reads D S_eq^-1 D from it
+    double* d = nullptr;  // the diagonal of D
+    double* kb = nullptr; double* wl = nullptr; int* rk = nullptr;  // K per slot, W and rank per landmark
+    long long np = 0;
+    int wgrid = 1;        // grid of the warp-per-landmark kernels
+  };
+  // Steps 1-3 of DESIGN.md section 16, shared by rba_compute_covariance and rba_compute_covariance_blocks (`fn` names the entry
+  // point in the messages).  One device allocation holds the pipeline's scratch followed by the caller's buffers of `extra`
+  // bytes each (their addresses are returned in `out`); the byte count of the out-of-memory message includes them.
+  int cov_factor_inverse(const char* fn, const std::vector<size_t>& extra, CovInverse& c, std::vector<char*>& out) {
     if (opt.nranks > 1) {
-      g_err = "rba_compute_covariance: sharded handles (nranks > 1) are not supported: the reduced camera matrix would need a cross-rank sum";
+      g_err = std::string(fn) + ": sharded handles (nranks > 1) are not supported: the reduced camera matrix would need a cross-rank sum";
       return RBA_ERR_UNSUPPORTED;
     }
     TRY(cov_build_lists());
@@ -1905,26 +1919,30 @@ struct Solver : rba_handle {
     auto carve = [&](size_t bytes) { const size_t o = total; total += (bytes + 255) & ~size_t(255); return o; };
     const size_t o_A = carve((size_t)(np * np) * 8), o_W = carve((size_t)(np * TB) * 8), o_Y = carve((size_t)(np * TB) * 8),
                  o_T = carve((size_t)(TB * TB) * 8), o_d = carve((size_t)np * 8), o_jp = carve((size_t)ns * 18 * 8),
-                 o_kb = carve((size_t)ns * 27 * 8), o_wl = carve((size_t)nl * 9 * 8), o_rk = carve((size_t)nl * 4), o_fail = carve(4),
-                 o_cam = carve((size_t)nc * 81 * 8), o_lm = carve(lm_cov ? (size_t)nl * 9 * 8 : 0);
+                 o_kb = carve((size_t)ns * 27 * 8), o_wl = carve((size_t)nl * 9 * 8), o_rk = carve((size_t)nl * 4), o_fail = carve(4);
+    std::vector<size_t> o_extra;
+    for (size_t b : extra) o_extra.push_back(carve(b));
     size_t free_b = 0, total_b = 0;
     CU(cudaMemGetInfo(&free_b, &total_b));
     if (total > free_b) {
-      g_err = "rba_compute_covariance needs " + std::to_string(total) + " bytes of device memory (a dense " + std::to_string(n) + " x " +
+      g_err = std::string(fn) + " needs " + std::to_string(total) + " bytes of device memory (a dense " + std::to_string(n) + " x " +
               std::to_string(n) + " float64 reduced camera matrix plus scratch); " + std::to_string(free_b) + " bytes are free";
       return RBA_ERR_UNSUPPORTED;
     }
     char* base = nullptr;
     CU(cudaMalloc(&base, total));
-    struct CovScratch { char* p; ~CovScratch() { cudaFree(p); } } scratch{base};  // cudaFree waits for the kernels
+    c.base = base;
     double* A = (double*)(base + o_A); double* W = (double*)(base + o_W); double* Y = (double*)(base + o_Y);
     double* Tt = (double*)(base + o_T); double* d = (double*)(base + o_d); double* jp = (double*)(base + o_jp);
     double* kb = (double*)(base + o_kb); double* wl = (double*)(base + o_wl); int* rk = (int*)(base + o_rk);
-    int* fail = (int*)(base + o_fail); double* cam_out = (double*)(base + o_cam); double* lm_out = (double*)(base + o_lm);
+    int* fail = (int*)(base + o_fail);
+    out.clear();
+    for (size_t o : o_extra) out.push_back(base + o);
+    const int wgrid = std::max(1, std::min((nl + 3) / 4, sm_count * 16));
+    c.A = A; c.d = d; c.kb = kb; c.wl = wl; c.rk = rk; c.np = np; c.wgrid = wgrid;
     // 1.-2. elimination, assembly, priors, held parameters, equilibration
     CU(cudaMemsetAsync(A, 0, (size_t)(np * np) * 8, stream));
     CU(cudaMemsetAsync(fail, 0x7f, 4, stream));
-    const int wgrid = std::max(1, std::min((nl + 3) / 4, sm_count * 16));
     // LMP: + L^T L of the landmark priors in Hll; OBSW: the rows whitened by the observation information
     auto kcov = n_lmp > 0 ? (D.obs_W ? k_cov_landmark<S, true, true> : k_cov_landmark<S, true>)
                           : (D.obs_W ? k_cov_landmark<S, false, true> : k_cov_landmark<S>);
@@ -1960,7 +1978,7 @@ struct Solver : rba_handle {
     CU(cudaGetLastError());
     if (h_fail < n) {
       static const char* names[9] = {"tx", "ty", "tz", "rx", "ry", "rz", "f", "k1", "k2"};
-      g_err = "rba_compute_covariance: the reduced camera matrix is singular: Cholesky pivot <= " + std::to_string(COV_PIVOT_TAU) +
+      g_err = std::string(fn) + ": the reduced camera matrix is singular: Cholesky pivot <= " + std::to_string(COV_PIVOT_TAU) +
               " of the equilibrated matrix at camera " + std::to_string(h_fail / 9) + ", increment entry " + std::to_string(h_fail % 9) +
               " (" + names[h_fail % 9] + "). The gauge is not fixed, or a free camera has no observation and no prior: hold parameters "
               "with rba_set_camera_fixed or add priors with rba_set_camera_prior";
@@ -1993,15 +2011,93 @@ struct Solver : rba_handle {
       TRY(cov_group_passes(A, np, n, 1));
       k_cov_group_d<<<1, 1, 0, stream>>>(d, groups());
     }
-    // 4. extraction
+    return RBA_OK;
+  }
+  // 4. the marginals cam_cov [81 nc] and lm_cov [9 nl] (either may be NULL) through the device buffers cam_out, lm_out
+  int cov_marginals(const CovInverse& c, double* cam_cov, double* lm_cov, double* cam_out, double* lm_out) {
     if (cam_cov) {
-      k_cov_cam_out<<<(81 * nc + 255) / 256, 256, 0, stream>>>(A, np, d, D.cam_fixed, nc, cam_out);
+      k_cov_cam_out<<<(81 * nc + 255) / 256, 256, 0, stream>>>(c.A, c.np, c.d, D.cam_fixed, nc, cam_out);
       CU(cudaMemcpyAsync(cam_cov, cam_out, (size_t)81 * nc * sizeof(double), cudaMemcpyDeviceToHost, stream));
     }
     if (lm_cov) {
-      k_cov_lm_marginal<<<wgrid, 128, 0, stream>>>(A, np, d, D.cam_fixed, D.slot_cam, d_cov_lm_slot0, d_cov_lm_n, nl, kb, wl, rk, lm_out);
-      CU(cudaMemcpyAsync(lm_cov, lm_out, (size_t)9 * nl * sizeof(double), cudaMemcpyDeviceToHost, stream));
+      k_cov_lm_marginal<<<c.wgrid, 128, 0, stream>>>(c.A, c.np, c.d, D.cam_fixed, D.slot_cam, d_cov_lm_slot0, d_cov_lm_n, L.nl_local,
+                                                     c.kb, c.wl, c.rk, lm_out);
+      CU(cudaMemcpyAsync(lm_cov, lm_out, (size_t)9 * L.nl_local * sizeof(double), cudaMemcpyDeviceToHost, stream));
     }
+    return RBA_OK;
+  }
+  int compute_covariance(double* cam_cov, double* lm_cov) override {
+    if (!cam_cov && !lm_cov) { g_err = "rba_compute_covariance: cam_cov and lm_cov are both NULL"; return RBA_ERR_INVALID_ARGUMENT; }
+    CovInverse c;
+    std::vector<char*> buf;
+    TRY(cov_factor_inverse("rba_compute_covariance", {(size_t)nc * 81 * 8, lm_cov ? (size_t)L.nl_local * 9 * 8 : 0}, c, buf));
+    TRY(cov_marginals(c, cam_cov, lm_cov, (double*)buf[0], (double*)buf[1]));
+    CU(cudaGetLastError());
+    CU(cudaStreamSynchronize(stream));
+    return RBA_OK;
+  }
+
+  // Covariance blocks of chosen pairs (DESIGN.md section 20): the pipeline of rba_compute_covariance, then the extraction
+  // kernels of the requests.  The requests are copied into the call's scratch and the outputs copied back at the end.
+  int compute_covariance_blocks(const rba_covariance_query* q) override {
+    auto bad = [](const std::string& m) { g_err = "rba_compute_covariance_blocks: " + m; return RBA_ERR_INVALID_ARGUMENT; };
+    if (!q) return bad("q is NULL");
+    struct Kind { const char* name; int m; const int32_t* req; double* out; int lim0, lim1, width; };
+    const Kind kinds[4] = {{"camera_pairs", q->num_camera_pairs, q->camera_pairs, q->camera_cross, nc, nc, 81},
+                           {"camera_landmark", q->num_camera_landmark, q->camera_landmark, q->camera_landmark_cross, nc, nl_total, 27},
+                           {"landmark_pairs", q->num_landmark_pairs, q->landmark_pairs, q->landmark_cross, nl_total, nl_total, 9},
+                           {"relative_pairs", q->num_relative_poses, q->relative_pairs, q->relative_cov, nc, nc, 36}};
+    bool any = q->cam_cov || q->lm_cov;
+    for (int k = 0; k < 4; ++k) {
+      const Kind& K = kinds[k];
+      if (K.m < 0) return bad(std::string("num_") + K.name + " is negative");
+      if (K.m == 0) continue;
+      any = true;
+      if (!K.req || !K.out) return bad(std::string(K.name) + " or its output is NULL with a positive count");
+      for (int r = 0; r < K.m; ++r) {
+        const int32_t a = K.req[2 * r], b = K.req[2 * r + 1];
+        if (a < 0 || a >= K.lim0 || b < 0 || b >= K.lim1)
+          return bad(std::string(K.name) + " request " + std::to_string(r) + " (" + std::to_string(a) + ", " + std::to_string(b) +
+                     ") is out of range");
+        if (k == 3 && a == b) return bad("relative_pairs request " + std::to_string(r) + " has i == j");
+      }
+    }
+    if (!any) return bad("nothing is requested (all counts are 0 and cam_cov and lm_cov are NULL)");
+    // the requests and outputs of each kind; no landmark output space unless a landmark block or lm_cov is asked for
+    std::vector<size_t> extra = {q->cam_cov ? (size_t)nc * 81 * 8 : 0, q->lm_cov ? (size_t)L.nl_local * 9 * 8 : 0};
+    for (const Kind& K : kinds) {
+      extra.push_back((size_t)K.m * 8);
+      extra.push_back((size_t)K.m * K.width * 8);
+    }
+    CovInverse c;
+    std::vector<char*> buf;
+    TRY(cov_factor_inverse("rba_compute_covariance_blocks", extra, c, buf));
+    TRY(cov_marginals(c, q->cam_cov, q->lm_cov, (double*)buf[0], (double*)buf[1]));
+    const int2* req[4];
+    double* dout[4];
+    for (int k = 0; k < 4; ++k) {
+      req[k] = (const int2*)buf[2 + 2 * k];
+      dout[k] = (double*)buf[3 + 2 * k];
+      if (kinds[k].m > 0)
+        CU(cudaMemcpyAsync(buf[2 + 2 * k], kinds[k].req, (size_t)kinds[k].m * 8, cudaMemcpyHostToDevice, stream));
+    }
+    const auto grid = [&](long long items, int per_block) {
+      return (unsigned)std::max<long long>(1, std::min<long long>((items + per_block - 1) / per_block, (long long)sm_count * 16));
+    };
+    if (kinds[0].m > 0)
+      k_cov_cam_cross<<<grid(81LL * kinds[0].m, 256), 256, 0, stream>>>(c.A, c.np, c.d, D.cam_fixed, req[0], kinds[0].m, dout[0]);
+    if (kinds[1].m > 0)
+      k_cov_cam_lm<<<grid(kinds[1].m, 4), 128, 0, stream>>>(c.A, c.np, c.d, D.cam_fixed, D.slot_cam, d_cov_lm_slot0, d_cov_lm_n, c.kb,
+                                                            c.wl, c.rk, req[1], kinds[1].m, dout[1]);
+    if (kinds[2].m > 0)
+      k_cov_lm_cross<<<grid(kinds[2].m, 4), 128, 0, stream>>>(c.A, c.np, c.d, D.cam_fixed, D.slot_cam, d_cov_lm_slot0, d_cov_lm_n, c.kb,
+                                                              c.wl, c.rk, req[2], kinds[2].m, dout[2]);
+    if (kinds[3].m > 0)
+      k_cov_rel_pose<S><<<grid(kinds[3].m, COV_REL_THREADS), COV_REL_THREADS, 0, stream>>>(c.A, c.np, c.d, D.cam_fixed, D.cams, req[3],
+                                                                                         kinds[3].m, dout[3]);
+    for (int k = 0; k < 4; ++k)
+      if (kinds[k].m > 0)
+        CU(cudaMemcpyAsync(kinds[k].out, dout[k], (size_t)kinds[k].m * kinds[k].width * 8, cudaMemcpyDeviceToHost, stream));
     CU(cudaGetLastError());
     CU(cudaStreamSynchronize(stream));
     return RBA_OK;
@@ -2288,6 +2384,7 @@ int32_t rba_debug_get_block(rba_handle* h, int32_t lm, void* out, int32_t rows, 
   return h->debug_get_block(lm, out, rows, cols, jls);
 }
 int32_t rba_compute_covariance(rba_handle* h, double* cam_cov, double* lm_cov) { return h->compute_covariance(cam_cov, lm_cov); }
+int32_t rba_compute_covariance_blocks(rba_handle* h, const rba_covariance_query* q) { return h->compute_covariance_blocks(q); }
 int32_t rba_time_matvec(rba_handle* h, int32_t reps, double* sec) { return h->time_matvec(reps, sec); }
 int32_t rba_timer_start(rba_handle* h) { return h->timer_start(); }
 int32_t rba_timer_stop(rba_handle* h, double* sec) { return h->timer_stop(sec); }

@@ -635,6 +635,36 @@ class LinearizorQR:
         check(_lib.lib().rba_compute_covariance(self.h, cam.ctypes.data, None if lm is None else lm.ctypes.data))
         return cam, lm
 
+    def covariance_blocks(self, cameras=None, camera_landmark=None, landmarks=None, relative=None, marginals: bool = False):
+        """covariance blocks of chosen pairs at the current state from one factorisation (rba_compute_covariance_blocks,
+        DESIGN.md section 20).  Each request argument is an int array [m, 2] or None: cameras (a, b) -> 'cameras' [m, 9, 9]
+        Cov(d_a, d_b); camera_landmark (c, l) -> 'camera_landmark' [m, 9, 3]; landmarks (l, m) -> 'landmarks' [m, 3, 3];
+        relative (i, j), i != j -> 'relative' [m, 6, 6], the covariance of the pair-prior residual (e_t, e_r) at the current
+        relative pose.  marginals=True adds 'cam' [nc, 9, 9] and 'lm' [nl, 3, 3], exactly covariance()'s.  float64 arrays;
+        raises RbaError like covariance() (code -1 for an invalid request)."""
+        q = _lib.CovarianceQuery()
+        out, keep = {}, []
+        for key, req, count, src, dst, shape in (("cameras", cameras, "num_camera_pairs", "camera_pairs", "camera_cross", (9, 9)),
+                                                 ("camera_landmark", camera_landmark, "num_camera_landmark", "camera_landmark",
+                                                  "camera_landmark_cross", (9, 3)),
+                                                 ("landmarks", landmarks, "num_landmark_pairs", "landmark_pairs", "landmark_cross", (3, 3)),
+                                                 ("relative", relative, "num_relative_poses", "relative_pairs", "relative_cov", (6, 6))):
+            if req is None:
+                continue
+            r = np.ascontiguousarray(np.asarray(req).reshape(-1, 2), dtype=np.int32)
+            o = np.empty((len(r),) + shape, np.float64)
+            keep.append(r)
+            setattr(q, count, len(r))
+            setattr(q, src, r.ctypes.data if len(r) else None)
+            setattr(q, dst, o.ctypes.data if len(r) else None)
+            out[key] = o
+        if marginals:
+            out["cam"] = np.empty((self.nc, 9, 9), np.float64)
+            out["lm"] = np.empty((self.nl, 3, 3), np.float64)
+            q.cam_cov, q.lm_cov = out["cam"].ctypes.data, out["lm"].ctypes.data
+        check(_lib.lib().rba_compute_covariance_blocks(self.h, C.byref(q)))
+        return out
+
     def timer_start(self):
         check(_lib.lib().rba_timer_start(self.h))
 
