@@ -9,10 +9,11 @@
 //      k_cov_diag/_equil  held rows and columns -> identity, equilibration D S D with D = diag(S)^-1/2, padding -> identity
 //   3. dense SPD inverse in place: blocked potrf, trtri, lauum (LAPACK's potri) with the diagonal-tile kernels and one
 //      FP64 tensor-core GEMM (mma.sync m8n8k4 .f64) for every O(N^3) update
-//   4. k_cov_cam_out      9x9 diagonal blocks of D S^-1 D;  k_cov_lm_marginal  per landmark
-//                         W (I + sum_ab K_a S^-1_ab K_b^T) W^T,  W = V Lambda^-1/2
-//   5. (rba_compute_covariance_blocks, DESIGN.md section 20) k_cov_cam_cross, k_cov_cam_lm, k_cov_lm_cross, k_cov_rel_pose:
-//                         the blocks of chosen camera pairs, camera-landmark pairs, landmark pairs and relative poses
+//   4. cov_sinv           entry of D S^-1 D;  cov_lm_block  landmark pair W_l (delta_lm I + sum_ab K_a S^-1_ab K_b^T) W_m^T,
+//                         W = V Lambda^-1/2
+//   5. (DESIGN.md section 20) k_cov_cam_cross, k_cov_cam_lm, k_cov_lm_cross, k_cov_rel_pose: the blocks of chosen camera
+//                         pairs, camera-landmark pairs, landmark pairs and relative poses.  The marginals cam_cov and lm_cov
+//                         are the diagonal requests (k, k) of k_cov_cam_cross and k_cov_lm_cross
 // The dense matrix is column-major with a leading dimension padded to a multiple of COV_TB; only its lower triangle is
 // meaningful.
 #pragma once
@@ -456,21 +457,10 @@ __device__ __forceinline__ double cov_sinv(const double* __restrict__ A, long lo
   return v * d[r] * d[c];
 }
 
-// cam_cov [nc][81], thread per entry
-__global__ void k_cov_cam_out(const double* __restrict__ A, long long ld, const double* __restrict__ d,
-                              const uint8_t* __restrict__ cam_fixed, int nc, double* __restrict__ out) {
-  const long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x;
-  if (e >= 81LL * nc) return;
-  const long long c = e / 81;
-  const int p = (int)(e % 81) / 9, q = (int)(e % 9);
-  out[e] = cov_sinv(A, ld, d, cam_fixed, 9 * c + p, 9 * c + q);
-}
-
 // One warp: the 3x3 block W_l (delta_lm I + sum_ab K_a Sigma_ab K_b^T) W_m^T of landmarks l and m (a over the slots of l,
 // b over those of m), lanes over the n_l n_m slot pairs, fixed-order butterfly sum, written by lane 0 to out [9]; all NaN
-// when the Hll of either has rank < 3.  With l == m it performs k_cov_lm_marginal's operations in its order (same lane
-// partition, butterfly and final products), so (l, l) is bit-identical to lm_cov[l].  k_cov_lm_marginal itself is left as
-// it was, so that rba_compute_covariance keeps its instructions.
+// when the Hll of either has rank < 3.  With l == m it is the marginal W (I + sum_ab K_a Sigma_ab K_b^T) W^T over the n^2
+// camera pairs of the landmark's track.
 __device__ __forceinline__ void cov_lm_block(const double* __restrict__ A, long long ld, const double* __restrict__ d,
                                              const uint8_t* __restrict__ cam_fixed, const int* __restrict__ slot_cam,
                                              const int* __restrict__ lm_slot0, const int* __restrict__ lm_n,
@@ -521,72 +511,18 @@ __device__ __forceinline__ void cov_lm_block(const double* __restrict__ A, long 
   }
 }
 
-// lm_cov [nl][9], warp per landmark: W (I + sum_ab K_a Sigma_ab K_b^T) W^T over the n^2 camera pairs of its track (lanes
-// over the pairs, fixed-order butterfly sum); all NaN when Hll has rank < 3.
-__global__ void __launch_bounds__(128) k_cov_lm_marginal(const double* __restrict__ A, long long ld, const double* __restrict__ d,
-                                                         const uint8_t* __restrict__ cam_fixed, const int* __restrict__ slot_cam,
-                                                         const int* __restrict__ lm_slot0, const int* __restrict__ lm_n, int nl,
-                                                         const double* __restrict__ kb, const double* __restrict__ wl,
-                                                         const int* __restrict__ rank, double* __restrict__ out) {
-  const int lane = threadIdx.x & 31;
-  const int warps = gridDim.x * (blockDim.x >> 5);
-  for (int lm = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); lm < nl; lm += warps) {
-    if (rank[lm] < 3) {
-      if (lane < 9) out[9 * (size_t)lm + lane] = __longlong_as_double(0x7ff8000000000000LL);
-      continue;
-    }
-    const int s0 = lm_slot0[lm], n = lm_n[lm];
-    double m[9];
-#pragma unroll
-    for (int k = 0; k < 9; ++k) m[k] = 0.0;
-    for (int t = lane; t < n * n; t += 32) {
-      const int a = t / n, b = t % n;
-      const long long ra = 9LL * slot_cam[s0 + a], rb = 9LL * slot_cam[s0 + b];
-      const double* ka = kb + 27 * (size_t)(s0 + a);
-      const double* kq = kb + 27 * (size_t)(s0 + b);
-      for (int p = 0; p < 9; ++p) {
-        double u[3] = {0.0, 0.0, 0.0};  // (Sigma_ab K_b^T) row p
-        for (int q = 0; q < 9; ++q) {
-          const double sv = cov_sinv(A, ld, d, cam_fixed, ra + p, rb + q);
-#pragma unroll
-          for (int l = 0; l < 3; ++l) u[l] += sv * kq[9 * l + q];
-        }
-#pragma unroll
-        for (int k = 0; k < 3; ++k)
-#pragma unroll
-          for (int l = 0; l < 3; ++l) m[3 * k + l] += ka[9 * k + p] * u[l];
-      }
-    }
-#pragma unroll
-    for (int k = 0; k < 9; ++k) m[k] = warp_sum(m[k]);
-    if (lane == 0) {
-      const double* W = wl + 9 * (size_t)lm;
-      double X[9];
-#pragma unroll
-      for (int k = 0; k < 9; ++k) X[k] = m[k] + (k % 4 == 0 ? 1.0 : 0.0);
-      for (int r = 0; r < 3; ++r)
-        for (int c = 0; c < 3; ++c) {
-          double v = 0.0;
-          for (int k = 0; k < 3; ++k)
-            for (int l = 0; l < 3; ++l) v += W[3 * r + k] * X[3 * k + l] * W[3 * c + l];
-          out[9 * (size_t)lm + 3 * r + c] = v;
-        }
-    }
-  }
-}
-
-
 // ------------------------------------------------------------------------------------------------
-// 5. covariance blocks of chosen pairs (rba_compute_covariance_blocks, DESIGN.md section 20).  Grid-stride loops over the
-//    requests, fixed-order sums, no atomics: the same output on every run, and request k depends on request k alone.
+// 5. covariance blocks of chosen pairs (DESIGN.md section 20).  Grid-stride loops over the requests, fixed-order sums, no
+//    atomics: the same output on every run, and request k depends on request k alone.
 // ------------------------------------------------------------------------------------------------
-// camera_cross [m][81] = Cov(d_a, d_b) of the requests (a, b), thread per entry; (a, a) is k_cov_cam_out's block a.
+// camera_cross [m][81] = Cov(d_a, d_b) of the requests (a, b), thread per entry.  req == nullptr: request k is (k, k), the
+// marginals cam_cov.
 __global__ void __launch_bounds__(256) k_cov_cam_cross(const double* __restrict__ A, long long ld, const double* __restrict__ d,
                                                        const uint8_t* __restrict__ cam_fixed, const int2* __restrict__ req, int m,
                                                        double* __restrict__ out) {
   const long long stride = (long long)gridDim.x * blockDim.x;
   for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < 81LL * m; e += stride) {
-    const int2 ab = req[e / 81];
+    const int2 ab = req ? req[e / 81] : make_int2((int)(e / 81), (int)(e / 81));
     const int p = (int)(e % 81) / 9, q = (int)(e % 9);
     out[e] = cov_sinv(A, ld, d, cam_fixed, 9LL * ab.x + p, 9LL * ab.y + q);
   }
@@ -637,7 +573,10 @@ __global__ void __launch_bounds__(128) k_cov_cam_lm(const double* __restrict__ A
   }
 }
 
-// landmark_cross [m][9] = Cov(d_l, d_m) of the requests (l, m), warp per request (cov_lm_block: (l, l) is l's marginal)
+// landmark_cross [m][9] = Cov(d_l, d_m) of the requests (l, m), warp per request (cov_lm_block: (l, l) is l's marginal).
+// MARGINALS: request k is (k, k) and req is not read, the marginals lm_cov.  That is an instantiation of its own because
+// with l == m known the kernel needs 70 registers instead of 94, and the higher occupancy makes the marginals faster.
+template <bool MARGINALS>
 __global__ void __launch_bounds__(128) k_cov_lm_cross(const double* __restrict__ A, long long ld, const double* __restrict__ d,
                                                       const uint8_t* __restrict__ cam_fixed, const int* __restrict__ slot_cam,
                                                       const int* __restrict__ lm_slot0, const int* __restrict__ lm_n,
@@ -646,8 +585,10 @@ __global__ void __launch_bounds__(128) k_cov_lm_cross(const double* __restrict__
                                                       double* __restrict__ out) {
   const int lane = threadIdx.x & 31;
   const int warps = gridDim.x * (blockDim.x >> 5);
-  for (int k = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); k < m; k += warps)
-    cov_lm_block(A, ld, d, cam_fixed, slot_cam, lm_slot0, lm_n, kb, wl, rank, req[k].x, req[k].y, lane, out + 9 * (size_t)k);
+  for (int k = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); k < m; k += warps) {
+    const int2 lm = MARGINALS ? make_int2(k, k) : req[k];
+    cov_lm_block(A, ld, d, cam_fixed, slot_cam, lm_slot0, lm_n, kb, wl, rank, lm.x, lm.y, lane, out + 9 * (size_t)k);
+  }
 }
 
 // relative_cov [m][36] of the requests (i, j), thread per request: the covariance A Sigma_P A^T of the pair-prior residual

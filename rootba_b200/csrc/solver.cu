@@ -8,6 +8,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <chrono>
+#include <array>
 #include <limits>
 #include <memory>
 #include <string>
@@ -1901,7 +1902,6 @@ struct Solver : rba_handle {
     double* d = nullptr;  // the diagonal of D
     double* kb = nullptr; double* wl = nullptr; int* rk = nullptr;  // K per slot, W and rank per landmark
     long long np = 0;
-    int wgrid = 1;        // grid of the warp-per-landmark kernels
   };
   // Steps 1-3 of DESIGN.md section 16, shared by rba_compute_covariance and rba_compute_covariance_blocks (`fn` names the entry
   // point in the messages).  One device allocation holds the pipeline's scratch followed by the caller's buffers of `extra`
@@ -1939,7 +1939,7 @@ struct Solver : rba_handle {
     out.clear();
     for (size_t o : o_extra) out.push_back(base + o);
     const int wgrid = std::max(1, std::min((nl + 3) / 4, sm_count * 16));
-    c.A = A; c.d = d; c.kb = kb; c.wl = wl; c.rk = rk; c.np = np; c.wgrid = wgrid;
+    c.A = A; c.d = d; c.kb = kb; c.wl = wl; c.rk = rk; c.np = np;
     // 1.-2. elimination, assembly, priors, held parameters, equilibration
     CU(cudaMemsetAsync(A, 0, (size_t)(np * np) * 8, stream));
     CU(cudaMemsetAsync(fail, 0x7f, 4, stream));
@@ -2013,43 +2013,30 @@ struct Solver : rba_handle {
     }
     return RBA_OK;
   }
-  // 4. the marginals cam_cov [81 nc] and lm_cov [9 nl] (either may be NULL) through the device buffers cam_out, lm_out
-  int cov_marginals(const CovInverse& c, double* cam_cov, double* lm_cov, double* cam_out, double* lm_out) {
-    if (cam_cov) {
-      k_cov_cam_out<<<(81 * nc + 255) / 256, 256, 0, stream>>>(c.A, c.np, c.d, D.cam_fixed, nc, cam_out);
-      CU(cudaMemcpyAsync(cam_cov, cam_out, (size_t)81 * nc * sizeof(double), cudaMemcpyDeviceToHost, stream));
-    }
-    if (lm_cov) {
-      k_cov_lm_marginal<<<c.wgrid, 128, 0, stream>>>(c.A, c.np, c.d, D.cam_fixed, D.slot_cam, d_cov_lm_slot0, d_cov_lm_n, L.nl_local,
-                                                     c.kb, c.wl, c.rk, lm_out);
-      CU(cudaMemcpyAsync(lm_cov, lm_out, (size_t)9 * L.nl_local * sizeof(double), cudaMemcpyDeviceToHost, stream));
-    }
-    return RBA_OK;
+  // The request kinds of an rba_covariance_query in the order of its fields: the ranges of a request's indices (a, b) and
+  // the doubles of its block.
+  struct CovKind { const char* name; int m; const int32_t* req; double* out; int lim0, lim1, width; };
+  std::array<CovKind, 4> cov_kinds(const rba_covariance_query& q) const {
+    return {{{"camera_pairs", q.num_camera_pairs, q.camera_pairs, q.camera_cross, nc, nc, 81},
+             {"camera_landmark", q.num_camera_landmark, q.camera_landmark, q.camera_landmark_cross, nc, nl_total, 27},
+             {"landmark_pairs", q.num_landmark_pairs, q.landmark_pairs, q.landmark_cross, nl_total, nl_total, 9},
+             {"relative_pairs", q.num_relative_poses, q.relative_pairs, q.relative_cov, nc, nc, 36}}};
   }
   int compute_covariance(double* cam_cov, double* lm_cov) override {
     if (!cam_cov && !lm_cov) { g_err = "rba_compute_covariance: cam_cov and lm_cov are both NULL"; return RBA_ERR_INVALID_ARGUMENT; }
-    CovInverse c;
-    std::vector<char*> buf;
-    TRY(cov_factor_inverse("rba_compute_covariance", {(size_t)nc * 81 * 8, lm_cov ? (size_t)L.nl_local * 9 * 8 : 0}, c, buf));
-    TRY(cov_marginals(c, cam_cov, lm_cov, (double*)buf[0], (double*)buf[1]));
-    CU(cudaGetLastError());
-    CU(cudaStreamSynchronize(stream));
-    return RBA_OK;
+    rba_covariance_query q = {};
+    q.cam_cov = cam_cov;
+    q.lm_cov = lm_cov;
+    return cov_compute("rba_compute_covariance", q);
   }
-
-  // Covariance blocks of chosen pairs (DESIGN.md section 20): the pipeline of rba_compute_covariance, then the extraction
-  // kernels of the requests.  The requests are copied into the call's scratch and the outputs copied back at the end.
+  // Covariance blocks of chosen pairs (DESIGN.md section 20): every request is checked before any device work.
   int compute_covariance_blocks(const rba_covariance_query* q) override {
     auto bad = [](const std::string& m) { g_err = "rba_compute_covariance_blocks: " + m; return RBA_ERR_INVALID_ARGUMENT; };
     if (!q) return bad("q is NULL");
-    struct Kind { const char* name; int m; const int32_t* req; double* out; int lim0, lim1, width; };
-    const Kind kinds[4] = {{"camera_pairs", q->num_camera_pairs, q->camera_pairs, q->camera_cross, nc, nc, 81},
-                           {"camera_landmark", q->num_camera_landmark, q->camera_landmark, q->camera_landmark_cross, nc, nl_total, 27},
-                           {"landmark_pairs", q->num_landmark_pairs, q->landmark_pairs, q->landmark_cross, nl_total, nl_total, 9},
-                           {"relative_pairs", q->num_relative_poses, q->relative_pairs, q->relative_cov, nc, nc, 36}};
+    const std::array<CovKind, 4> kinds = cov_kinds(*q);
     bool any = q->cam_cov || q->lm_cov;
     for (int k = 0; k < 4; ++k) {
-      const Kind& K = kinds[k];
+      const CovKind& K = kinds[k];
       if (K.m < 0) return bad(std::string("num_") + K.name + " is negative");
       if (K.m == 0) continue;
       any = true;
@@ -2063,16 +2050,23 @@ struct Solver : rba_handle {
       }
     }
     if (!any) return bad("nothing is requested (all counts are 0 and cam_cov and lm_cov are NULL)");
-    // the requests and outputs of each kind; no landmark output space unless a landmark block or lm_cov is asked for
-    std::vector<size_t> extra = {q->cam_cov ? (size_t)nc * 81 * 8 : 0, q->lm_cov ? (size_t)L.nl_local * 9 * 8 : 0};
-    for (const Kind& K : kinds) {
+    return cov_compute("rba_compute_covariance_blocks", *q);
+  }
+  // One covariance call on a query its entry point `fn` (named in the messages) has checked: cov_factor_inverse, then the
+  // extraction kernels.  The marginals cam_cov and lm_cov are the diagonal requests (k, k) of k_cov_cam_cross and
+  // k_cov_lm_cross (req == nullptr, no request list).  Output space is carved only for what is asked for; the requests are
+  // copied into the call's scratch and the outputs copied back at the end.
+  int cov_compute(const char* fn, const rba_covariance_query& q) {
+    const int nl = L.nl_local;
+    const std::array<CovKind, 4> kinds = cov_kinds(q);
+    std::vector<size_t> extra = {q.cam_cov ? (size_t)nc * 81 * 8 : 0, q.lm_cov ? (size_t)nl * 9 * 8 : 0};
+    for (const CovKind& K : kinds) {
       extra.push_back((size_t)K.m * 8);
       extra.push_back((size_t)K.m * K.width * 8);
     }
     CovInverse c;
     std::vector<char*> buf;
-    TRY(cov_factor_inverse("rba_compute_covariance_blocks", extra, c, buf));
-    TRY(cov_marginals(c, q->cam_cov, q->lm_cov, (double*)buf[0], (double*)buf[1]));
+    TRY(cov_factor_inverse(fn, extra, c, buf));
     const int2* req[4];
     double* dout[4];
     for (int k = 0; k < 4; ++k) {
@@ -2084,17 +2078,25 @@ struct Solver : rba_handle {
     const auto grid = [&](long long items, int per_block) {
       return (unsigned)std::max<long long>(1, std::min<long long>((items + per_block - 1) / per_block, (long long)sm_count * 16));
     };
-    if (kinds[0].m > 0)
-      k_cov_cam_cross<<<grid(81LL * kinds[0].m, 256), 256, 0, stream>>>(c.A, c.np, c.d, D.cam_fixed, req[0], kinds[0].m, dout[0]);
+    const auto cam_cross = [&](const int2* r, int m, double* out) {
+      k_cov_cam_cross<<<grid(81LL * m, 256), 256, 0, stream>>>(c.A, c.np, c.d, D.cam_fixed, r, m, out);
+    };
+    const auto lm_cross = [&](const int2* r, int m, double* out) {
+      (r ? k_cov_lm_cross<false> : k_cov_lm_cross<true>)<<<grid(m, 4), 128, 0, stream>>>(
+          c.A, c.np, c.d, D.cam_fixed, D.slot_cam, d_cov_lm_slot0, d_cov_lm_n, c.kb, c.wl, c.rk, r, m, out);
+    };
+    if (q.cam_cov) cam_cross(nullptr, nc, (double*)buf[0]);
+    if (q.lm_cov) lm_cross(nullptr, nl, (double*)buf[1]);
+    if (kinds[0].m > 0) cam_cross(req[0], kinds[0].m, dout[0]);
     if (kinds[1].m > 0)
       k_cov_cam_lm<<<grid(kinds[1].m, 4), 128, 0, stream>>>(c.A, c.np, c.d, D.cam_fixed, D.slot_cam, d_cov_lm_slot0, d_cov_lm_n, c.kb,
                                                             c.wl, c.rk, req[1], kinds[1].m, dout[1]);
-    if (kinds[2].m > 0)
-      k_cov_lm_cross<<<grid(kinds[2].m, 4), 128, 0, stream>>>(c.A, c.np, c.d, D.cam_fixed, D.slot_cam, d_cov_lm_slot0, d_cov_lm_n, c.kb,
-                                                              c.wl, c.rk, req[2], kinds[2].m, dout[2]);
+    if (kinds[2].m > 0) lm_cross(req[2], kinds[2].m, dout[2]);
     if (kinds[3].m > 0)
       k_cov_rel_pose<S><<<grid(kinds[3].m, COV_REL_THREADS), COV_REL_THREADS, 0, stream>>>(c.A, c.np, c.d, D.cam_fixed, D.cams, req[3],
                                                                                          kinds[3].m, dout[3]);
+    if (q.cam_cov) CU(cudaMemcpyAsync(q.cam_cov, buf[0], (size_t)nc * 81 * 8, cudaMemcpyDeviceToHost, stream));
+    if (q.lm_cov) CU(cudaMemcpyAsync(q.lm_cov, buf[1], (size_t)nl * 9 * 8, cudaMemcpyDeviceToHost, stream));
     for (int k = 0; k < 4; ++k)
       if (kinds[k].m > 0)
         CU(cudaMemcpyAsync(kinds[k].out, dout[k], (size_t)kinds[k].m * kinds[k].width * 8, cudaMemcpyDeviceToHost, stream));
