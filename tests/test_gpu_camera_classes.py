@@ -507,60 +507,82 @@ def _vec_params():
 
 
 def _vec_setup(c, nc, dtype, **opt):
-    from test_gpu_pcg_iterates import operator_of
     arrays = vec_problem(nc, (c, nc) in UNOBSERVED_LAST)
-    env = {"RBA_PCG_CLUSTER": str(c)}
-    lin = _handle(arrays, dtype, env, **opt)
-    lin.solve(LAM_POWER if opt.get("solver_type") == "POWER_SCHUR_COMPLEMENT" else LAM_PCG)
-    b, inv = lin.get_rhs(), lin.get_preconditioner()[0]
-    op = operator_of(lin, dtype)
-    return arrays, env, lin, b, inv, op
+    return arrays, {"RBA_PCG_CLUSTER": str(c)}
 
 
-def _truncated(arrays, dtype, env, lam, **opt):
-    lin = _handle(arrays, dtype, env, **opt)
+def _plain_operator(lin, dtype):
+    from test_gpu_pcg_iterates import operator_of
+    return operator_of(lin, dtype), (lambda v: v)
+
+
+def _truncated(arrays, dtype, env, lam, handle=_handle, **opt):
+    lin = handle(arrays, dtype, env, **opt)
     inc = lin.solve(lam)
     out = (inc, lin.last_cg.termination_type, lin.last_cg.num_iterations, lin.get_rhs(), lin.get_preconditioner()[0])
     lin.close()
     return out
 
 
-@pytest.mark.parametrize("c,nc,dtype", _vec_params())
-def test_pcg_iterates_at_camera_count_edges(c, nc, dtype):
-    """PCG truncated at 1, 2, 3 iterations and at convergence against pcg_replay on the handle's own b, M^-1 and operator"""
-    arrays, env, lin, b, inv, op = _vec_setup(c, nc, dtype)
-    if (c, nc) in UNOBSERVED_LAST:
-        assert np.all(b[-9:] == 0)
+SENSITIVITY_TRIALS = 8
+
+
+def replay_sensitivity(op, b, inv, n_it, u, n):
+    """S_k: the largest relative deviation of iterate k over SENSITIVITY_TRIALS float64 replays whose every operator
+    application is perturbed entry by entry by a uniform C_BAR u (|H| |v|), H assembled from the n unit vectors"""
+    H = np.stack([np.asarray(op(np.eye(n)[j]), np.float64) for j in range(n)], axis=1)
+    ref = pcg_replay(lambda v: H @ v, b, inv, eta=NEVER, max_it=n_it)["xs"]
+    rng = np.random.default_rng(0)
+    S = np.zeros(len(ref))
+    for _ in range(SENSITIVITY_TRIALS):
+        pert = lambda v: H @ v + rng.uniform(-1, 1, n) * C_BAR * u * (np.abs(H) @ np.abs(v))
+        xs = pcg_replay(pert, b, inv, eta=NEVER, max_it=n_it)["xs"]
+        S[:len(xs)] = np.maximum(S[:len(xs)], [rel_err(x, y) for x, y in zip(xs, ref)])
+    return S
+
+
+def pcg_edge_sweep(arrays, dtype, env, handle=_handle, operator=_plain_operator, sensitivity=False):
+    """PCG truncated at 1, 2, 3 iterations and at convergence against pcg_replay on the handle's own b, M^-1 and operator.
+    handle(arrays, dtype, env, **opt) makes a linearised handle; operator(lin, dtype) gives the replay's operator and the map
+    from the replay's vector to the increment.  sensitivity: the bar of iterate k is at least 4 S_k (replay_sensitivity)"""
+    lin = handle(arrays, dtype, env)
+    lin.solve(LAM_PCG)
     try:
-        full = pcg_replay(op, b, inv, eta=NEVER, max_it=min(600, 9 * nc))
+        b, inv = lin.get_rhs(), lin.get_preconditioner()[0]
+        op, expand = operator(lin, dtype)
+        full = pcg_replay(op, b, inv, eta=NEVER, max_it=min(600, 9 * arrays.nc))
+        xs = full["xs"]
+        # converged: the first step that changes the iterate by less than 1e-4; kappa from the Lanczos tridiagonal of the
+        # coefficients up to there (beyond it they are rounding noise and the Ritz values lose their meaning)
+        k_conv = next((k for k in range(1, len(xs)) if rel_err(xs[k], xs[k - 1]) < 1e-4), len(xs) - 1)
+        S = replay_sensitivity(op, b, inv, k_conv, _u(dtype), 9 * arrays.nc) if sensitivity else np.zeros(k_conv + 1)
     finally:
         lin.close()
-    xs = full["xs"]
-    # converged: the first step that changes the iterate by less than 1e-4; kappa from the Lanczos tridiagonal of the
-    # coefficients up to there (beyond it they are rounding noise and the Ritz values lose their meaning)
-    k_conv = next((k for k in range(1, len(xs)) if rel_err(xs[k], xs[k - 1]) < 1e-4), len(xs) - 1)
     lmin, lmax = lanczos_condition(full["alphas"][:k_conv], full["betas"][:k_conv - 1])
     assert lmin > 0, (lmin, lmax)
     kappa = lmax / lmin
     ks = sorted({k for k in (1, 2, 3) if k < len(xs)} | {k_conv})
     for k in ks:
-        bar = C_BAR * k * _u(dtype) * kappa
+        bar = max(C_BAR * k * _u(dtype) * kappa, 4 * S[k])
         assert bar <= (BAR_MAX_CONVERGED if k == k_conv else BAR_MAX)[dtype], (k, kappa, bar)
         if dtype == np.float64 and k <= 3 and k < k_conv:
             assert rel_err(xs[k], xs[k - 1]) > 100 * bar, k
-        inc, term, it, b_k, inv_k = _truncated(arrays, dtype, env, LAM_PCG, eta=NEVER, max_linear_solver_iterations=k)
+        inc, term, it, b_k, inv_k = _truncated(arrays, dtype, env, LAM_PCG, handle, eta=NEVER, max_linear_solver_iterations=k)
         assert np.array_equal(b_k, b) and np.array_equal(inv_k, inv), k
         assert (term, it) == (NO_CONVERGENCE, k), (k, term, it)
-        assert rel_err(inc, -xs[k]) < bar, (k, rel_err(inc, -xs[k]), bar)
+        assert rel_err(inc, -expand(xs[k])) < bar, (k, rel_err(inc, -expand(xs[k])), bar)
+    return b
 
 
-@pytest.mark.parametrize("c,nc,dtype", _vec_params())
-def test_power_series_at_camera_count_edges(c, nc, dtype):
+def power_edge_sweep(arrays, dtype, env, handle=_handle):
     """POWER_SCHUR_COMPLEMENT truncated at 1, 2, 3 and CONVERGED_POWER terms against power_replay"""
+    from test_gpu_pcg_iterates import operator_of
     opt = {"solver_type": "POWER_SCHUR_COMPLEMENT"}
-    arrays, env, lin, b, inv, op = _vec_setup(c, nc, dtype, power_order=CONVERGED_POWER, eta=0.0, **opt)
+    lin = handle(arrays, dtype, env, power_order=CONVERGED_POWER, eta=0.0, **opt)
+    lin.solve(LAM_POWER)
     try:
-        full = power_replay(op, inv, b, order=CONVERGED_POWER, eta=0.0)
+        b, inv = lin.get_rhs(), lin.get_preconditioner()[0]
+        full = power_replay(operator_of(lin, dtype), inv, b, order=CONVERGED_POWER, eta=0.0)
     finally:
         lin.close()
     sums = full["sums"]
@@ -572,7 +594,23 @@ def test_power_series_at_camera_count_edges(c, nc, dtype):
     for k in (1, 2, 3, CONVERGED_POWER):
         bar = C_BAR * k * _u(dtype) * kappa_b * min(k, 1 / (1 - rho))
         assert bar <= (BAR_MAX_CONVERGED if k == CONVERGED_POWER else BAR_MAX)[dtype], (k, kappa_b, rho, bar)
-        inc, term, it, b_k, inv_k = _truncated(arrays, dtype, env, LAM_POWER, power_order=k, eta=0.0, **opt)
+        inc, term, it, b_k, inv_k = _truncated(arrays, dtype, env, LAM_POWER, handle, power_order=k, eta=0.0, **opt)
         assert np.array_equal(b_k, b) and np.array_equal(inv_k, inv), k
         assert (term, it) == (NO_CONVERGENCE, k), (k, term, it)
         assert rel_err(inc, sums[k]) < bar, (k, rel_err(inc, sums[k]), bar)
+
+
+@pytest.mark.parametrize("c,nc,dtype", _vec_params())
+def test_pcg_iterates_at_camera_count_edges(c, nc, dtype):
+    """PCG truncated at 1, 2, 3 iterations and at convergence against pcg_replay on the handle's own b, M^-1 and operator"""
+    arrays, env = _vec_setup(c, nc, dtype)
+    b = pcg_edge_sweep(arrays, dtype, env)
+    if (c, nc) in UNOBSERVED_LAST:
+        assert np.all(b[-9:] == 0)
+
+
+@pytest.mark.parametrize("c,nc,dtype", _vec_params())
+def test_power_series_at_camera_count_edges(c, nc, dtype):
+    """POWER_SCHUR_COMPLEMENT truncated at 1, 2, 3 and CONVERGED_POWER terms against power_replay"""
+    arrays, env = _vec_setup(c, nc, dtype)
+    power_edge_sweep(arrays, dtype, env)
