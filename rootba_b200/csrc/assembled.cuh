@@ -11,7 +11,8 @@
 //   k_rcs_mirror    k_stage2 has just written, every term formed from the two slots' dmp records (no staging), added in
 //                   the same list order; then the upper blocks as transposes of the lower ones.
 //                   All four return at once when the solve has ended before.
-//   k_rcs_spmv      y = S x over a camera-major block-row CSR of the full matrix (both triangles, diagonal included).
+//   k_rcs_spmv      y = S x over a camera-major block-row CSR of the full matrix (both triangles, diagonal included), its
+//                   rows dealt over one wave of persistent CTAs and S staged through shared memory by bulk copies.
 #pragma once
 
 #include "kernels.cuh"
@@ -166,60 +167,161 @@ __global__ void k_rcs_mirror(const int2* __restrict__ pos, int nblk, S* val, con
   if (ps.y >= 0) val[81 * (size_t)ps.y + e] = val[81 * (size_t)ps.x + 9 * (e % 9) + e / 9];
 }
 
-// y[9 row .. 9 row + 8] = sum over the blocks k of the row of S_k x[col_k]: CTA of 4 warps per block row, warp w takes the
-// blocks k0 + w, k0 + w + 4, ... in that order, lane l entries l, l + 32, l + 64 of each 81-entry block (coalesced); the
-// partial rows are added in shared memory in a fixed order (warp, then column).  A row without blocks (a camera without
-// observations) gets y = 0.  In PCG it is launched dependent on the vector step and returns at once when the solve has
-// ended (the `done` flag, as k_matvec_small_tma).
-constexpr int SPMV_WARPS = 4;
-constexpr int SPMV_UNROLL = 4;
+// y = S x over the rows of the host's deal (deal_spmv, layout.hpp): a grid of co-resident CTAs of SPMV_CLASSES warps, each
+// taking its chunks in order.  Thread 0 brings a chunk's blocks of S into one stage of an SPMV_NS-stage shared-memory ring
+// with a cp.async.bulk copy (mbarrier complete_tx), under an L2 evict_last policy: S is read again by every later PCG
+// iteration.  A bulk copy wants 16-byte addresses and sizes and a block is 81 scalars, so each copy starts at the 16-byte
+// boundary at or below the chunk's first entry and its size is rounded up (the buffer of S ends in 16 bytes of padding);
+// the stage is read from that offset.  x is gathered window by window: the col entries of a window of whole chunks (at
+// most XWIN blocks, usually all of a CTA's chunks) into shared memory, then x[col] of all of them at once, so that the
+// latency of the gathers is paid once per window and not once per chunk.  The first stages and the first window's col
+// entries are requested before griddepcontrol.wait; only x and `done` are read after it.  That needs S and col written
+// before the kernel right before this one: col and the deal are uploaded with the handle, and S is written by the
+// assembly, after which the host launches the next k_rcs_spmv without PDL (Solver::s_fresh), so that stream order puts it
+// after the assembly has completed.  Every later launch of the solve follows k_pcg_vec, with S unchanged since.  Warp c runs chain c (layout.hpp): blocks c, c + SPMV_CLASSES, ... of every chunk of the row in order, lane l
+// entries l, l + 32, l + 64 of each block; at the row's last chunk the chains' partials are added in shared memory in the
+// fixed order (chain, then column).  A row without blocks (a camera without observations) gets y = 0.  In PCG it is
+// launched dependent on the vector step and returns at once when the solve has ended (the `done` flag, as
+// k_matvec_small_tma).
+constexpr int SPMV_NS = 3;
 template <class S>
-__global__ void __launch_bounds__(SPMV_WARPS * 32) k_rcs_spmv(const int* __restrict__ row_ptr, const int* __restrict__ col,
-                                                               const S* __restrict__ val, const S* __restrict__ x, S* __restrict__ y,
-                                                               const int* done, int pdl) {
-  __shared__ S part[SPMV_WARPS][81];
-  if (done && *reinterpret_cast<const volatile int*>(done)) return;
-  const int row = blockIdx.x, w = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int k0 = row_ptr[row], k1 = row_ptr[row + 1];
+__global__ void __launch_bounds__(SPMV_CLASSES * 32) k_rcs_spmv(const SpmvChunk* __restrict__ chunks, const int* __restrict__ chunk_ptr,
+                                                                 const int* __restrict__ col, const S* __restrict__ val,
+                                                                 const S* __restrict__ x, S* __restrict__ y, const int* done, int pdl) {
+  constexpr int CH = SPMV_STAGE_BYTES / (81 * (int)sizeof(S)), U = CH / SPMV_CLASSES;  // spmv_chunk_blocks
+  constexpr int VB = CH * 81 * (int)sizeof(S) + 16;                                     // stage bytes, alignment slack included
+  constexpr int XWIN = sizeof(S) == 4 ? 256 : 128;                                      // blocks per x window
+  static_assert(CH % SPMV_CLASSES == 0 && VB % 16 == 0 && XWIN >= CH, "k_rcs_spmv stage layout");
+  __shared__ __align__(128) unsigned char sval[SPMV_NS][VB];
+  __shared__ S sx[XWIN * 9];
+  __shared__ int scol[XWIN];
+  __shared__ __align__(8) uint64_t bars[SPMV_NS];
+  __shared__ S part[SPMV_CLASSES][81];
+  __shared__ int quit;
+  // `done` only ever goes 0 -> 1 inside one solve, and may do so while the vector step runs: thread 0 reads it once for
+  // the whole CTA (a stale 0 is harmless, it is read again after griddepcontrol.wait)
+  if (threadIdx.x == 0) {
+    quit = done && *reinterpret_cast<const volatile int*>(done);
+    if (!quit) {
+      for (int s = 0; s < SPMV_NS; ++s) mbar_init(&bars[s], 1);
+      mbar_fence_init();
+    }
+  }
+  __syncthreads();
+  if (quit) return;
+  const int c0 = chunk_ptr[blockIdx.x], n = chunk_ptr[blockIdx.x + 1] - c0;
+  const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const uint64_t policy = l2_evict_last_policy();
+  constexpr uintptr_t A16 = ~(uintptr_t)15;
+  // (thread 0) chunk i into stage i % SPMV_NS.  An empty chunk copies nothing when its start is 16-byte aligned and the
+  // 16 bytes at that boundary otherwise (inside the padding at the end of S when it is the last); nothing of it is read
+  auto request = [&](int i) {
+    const SpmvChunk ch = chunks[c0 + i];
+    const int s = i % SPMV_NS;
+    const uintptr_t v0 = (uintptr_t)(val + 81 * (size_t)ch.kb) & A16, v1 = ((uintptr_t)(val + 81 * (size_t)ch.ke) + 15) & A16;
+    mbar_expect_tx(&bars[s], (uint32_t)(v1 - v0));
+    if (v1 > v0) bulk_g2s(sval[s], (const void*)v0, (uint32_t)(v1 - v0), &bars[s], policy);
+  };
+  // the window from chunk i0: whole chunks while their blocks fit in XWIN; its col entries into scol (warp c takes chunks
+  // c, c + SPMV_CLASSES, ... of it).  Returns its end and block count.
+  auto window = [&](int i0, int& nblk) {
+    int i = i0, off = 0;
+    for (; i < n; ++i) {
+      const SpmvChunk ch = chunks[c0 + i];
+      const int nb = ch.ke - ch.kb;
+      if (off + nb > XWIN) break;
+      if ((i - i0) % SPMV_CLASSES == w)
+        for (int t = lane; t < nb; t += 32) scol[off + t] = __ldg(col + ch.kb + t);
+      off += nb;
+    }
+    nblk = off;
+    return i;
+  };
+  // x[col] of the window's blocks into sx, all loads of a thread in flight together
+  auto gather_x = [&](int nblk) {
+    constexpr int B = 8;
+    for (int t0 = threadIdx.x; t0 < 9 * nblk; t0 += B * SPMV_CLASSES * 32) {
+      S v[B];
+#pragma unroll
+      for (int j = 0; j < B; ++j) {
+        const int t = t0 + j * SPMV_CLASSES * 32;
+        v[j] = t < 9 * nblk ? __ldcg(x + 9 * (size_t)scol[t / 9] + t % 9) : S(0);
+      }
+#pragma unroll
+      for (int j = 0; j < B; ++j) {
+        const int t = t0 + j * SPMV_CLASSES * 32;
+        if (t < 9 * nblk) sx[t] = v[j];
+      }
+    }
+  };
+  const int primed = min(n, SPMV_NS);
+  if (threadIdx.x == 0)
+    for (int i = 0; i < primed; ++i) request(i);
+  int nblk = 0;
+  int wend = window(0, nblk);
+  if (pdl) asm volatile("griddepcontrol.wait;" ::: "memory");
+  if (done && *done) {
+    // drain the bulk copies already in flight before the CTA may exit
+    for (int i = 0; i < primed; ++i) mbar_wait(&bars[i], 0);
+    return;
+  }
+  if (pdl) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  __syncthreads();  // scol of the first window
+  gather_x(nblk);
+  __syncthreads();
   int qe[3];
 #pragma unroll
   for (int u = 0; u < 3; ++u) qe[u] = (lane + 32 * u) % 9;
-  if (pdl) asm volatile("griddepcontrol.wait;" ::: "memory");
-  if (done && *done) return;
-  if (pdl) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   S acc[3] = {0, 0, 0};
-  for (int k = k0 + w; k < k1; k += SPMV_WARPS * SPMV_UNROLL) {
-    S v[SPMV_UNROLL][3], xv[SPMV_UNROLL][3];
+  for (int i = 0, jb = 0; i < n; ++i) {
+    if (i == wend) {  // the next window (the last iteration ended in __syncthreads: scol and sx are free)
+      wend = window(i, nblk);
+      __syncthreads();
+      gather_x(nblk);
+      __syncthreads();
+      jb = 0;
+    }
+    const SpmvChunk ch = chunks[c0 + i];
+    const int s = i % SPMV_NS, nb = ch.ke - ch.kb;
+    if (ch.flags & SPMV_FIRST) acc[0] = acc[1] = acc[2] = 0;
+    mbar_wait(&bars[s], (i / SPMV_NS) & 1u);
+    const S* vs = reinterpret_cast<const S*>(sval[s] + ((uintptr_t)(val + 81 * (size_t)ch.kb) & 15));
+    const S* xs = sx + 9 * jb;
+    S v[U][3], xv[U][3];
 #pragma unroll
-    for (int j = 0; j < SPMV_UNROLL; ++j) {
-      const int kk = k + SPMV_WARPS * j;
-      const bool in = kk < k1;
-      const S* blk = val + 81 * (size_t)(in ? kk : k0);
-      const S* xc = x + 9 * (size_t)(in ? __ldg(col + kk) : 0);
+    for (int j = 0; j < U; ++j) {
+      const int b = w + SPMV_CLASSES * j;
 #pragma unroll
       for (int u = 0; u < 3; ++u) {
-        const bool e_in = in && lane + 32 * u < 81;
-        v[j][u] = e_in ? __ldg(blk + lane + 32 * u) : S(0);
-        xv[j][u] = e_in ? __ldcg(xc + qe[u]) : S(0);
+        const bool e_in = b < nb && lane + 32 * u < 81;
+        v[j][u] = e_in ? vs[81 * b + lane + 32 * u] : S(0);
+        xv[j][u] = e_in ? xs[9 * b + qe[u]] : S(0);
       }
     }
 #pragma unroll
-    for (int j = 0; j < SPMV_UNROLL; ++j)
+    for (int j = 0; j < U; ++j)
+      if (w + SPMV_CLASSES * j < nb) {
 #pragma unroll
-      for (int u = 0; u < 3; ++u) acc[u] = fma(v[j][u], xv[j][u], acc[u]);
-  }
+        for (int u = 0; u < 3; ++u) acc[u] = fma(v[j][u], xv[j][u], acc[u]);
+      }
+    jb += nb;
+    if (ch.flags & SPMV_LAST) {
 #pragma unroll
-  for (int u = 0; u < 3; ++u)
-    if (lane + 32 * u < 81) part[w][lane + 32 * u] = acc[u];
-  __syncthreads();
-  if (threadIdx.x < 9) {
-    const int p = threadIdx.x;
-    S s = 0;
+      for (int u = 0; u < 3; ++u)
+        if (lane + 32 * u < 81) part[w][lane + 32 * u] = acc[u];
+      __syncthreads();
+      if (threadIdx.x < 9) {
+        const int p = threadIdx.x;
+        S t = 0;
 #pragma unroll
-    for (int ww = 0; ww < SPMV_WARPS; ++ww)
+        for (int c = 0; c < SPMV_CLASSES; ++c)
 #pragma unroll
-      for (int q = 0; q < 9; ++q) s += part[ww][9 * p + q];
-    y[9 * (size_t)row + p] = s;
+          for (int q = 0; q < 9; ++q) t += part[c][9 * p + q];
+        y[9 * (size_t)ch.row + p] = t;
+      }
+    }
+    __syncthreads();  // every warp is done with the stage (and with `part`) before the stage is requested again
+    if (threadIdx.x == 0 && i + SPMV_NS < n) request(i + SPMV_NS);
   }
 }
 

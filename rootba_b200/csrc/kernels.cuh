@@ -1863,6 +1863,12 @@ __device__ __forceinline__ uint64_t l2_evict_first_policy() {
   asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
   return pol;
 }
+// The assembled S is smaller than L2 and read again by every PCG iteration after the switch: keep it there.
+__device__ __forceinline__ uint64_t l2_evict_last_policy() {
+  uint64_t pol;
+  asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol));
+  return pol;
+}
 __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar, uint64_t policy) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;" ::"r"(
                    smem_u32(dst)),

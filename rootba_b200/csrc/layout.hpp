@@ -398,8 +398,55 @@ inline int asm_switch_iteration(long long nt, long long panel_scalars, long long
   return 1 + (int)std::ceil(2.0 * staged / std::max(saved, 1.0));
 }
 
+// The product y = S x (k_rcs_spmv) sums every entry e = 9 p + q of a block row in a fixed order: SPMV_CLASSES fma chains,
+// chain c over the row's blocks k with k - (row start) = c mod SPMV_CLASSES in ascending order, each starting from 0 with
+// the terms S_k[e] x[col_k][q]; then the chains' 9 SPMV_CLASSES partials of output p added from 0, chain by chain, q
+// ascending.  Its persistent CTAs take their block rows from a host-built deal: the rows dealt longest-first on block count
+// (deal_lpt) over the CTAs, each row cut into chunks of at most spmv_chunk_blocks blocks (a multiple of SPMV_CLASSES, so
+// a block's chain is its position in its chunk mod SPMV_CLASSES), one chunk per shared-memory stage.  A row without
+// blocks is one empty chunk (its y is 0).
+constexpr int SPMV_CLASSES = 4;
+constexpr int SPMV_STAGE_BYTES = 32 * 81 * 4;  // blocks of S per stage: 32 in float32, 16 in float64
+constexpr int spmv_chunk_blocks(int scalar_size) { return SPMV_STAGE_BYTES / (81 * scalar_size); }
+struct SpmvChunk {
+  int row, kb, ke;  // blocks [kb, ke) of the CSR, all in block row `row`
+  int flags;        // SPMV_FIRST: the row's first chunk; SPMV_LAST: its last
+};
+constexpr int SPMV_FIRST = 1, SPMV_LAST = 2;
+struct SpmvDeal {
+  int ctas = 0;
+  std::vector<int> chunk_ptr;       // [ctas + 1]: CTA b takes chunks chunk_ptr[b] .. chunk_ptr[b + 1] - 1 in that order
+  std::vector<SpmvChunk> chunks;    // a CTA's rows longest first, each row's chunks consecutive and ascending
+};
+// ctas (>= 1) is the most CTAs to deal to; fewer are used when there are fewer rows.
+inline void deal_spmv(const std::vector<int>& row_ptr, int ctas, int chunk_blocks, SpmvDeal& D) {
+  D = SpmvDeal();
+  const int nrows = (int)row_ptr.size() - 1;
+  D.ctas = std::max(1, std::min(ctas, nrows));
+  std::vector<long long> cost((size_t)std::max(nrows, 0));
+  for (int r = 0; r < nrows; ++r) cost[r] = row_ptr[r + 1] - row_ptr[r];
+  const std::vector<int> order = deal_lpt(cost, D.ctas);
+  D.chunk_ptr.assign((size_t)D.ctas + 1, 0);
+  for (int b = 0; b < D.ctas; ++b) {
+    D.chunk_ptr[b] = (int)D.chunks.size();
+    for (size_t k = b; k < order.size(); k += D.ctas) {
+      const int r = order[k];
+      if (r < 0) break;
+      const int k0 = row_ptr[r], k1 = row_ptr[r + 1];
+      int kb = k0;
+      do {
+        const int ke = std::min(k1, kb + chunk_blocks);
+        D.chunks.push_back({r, kb, ke, (kb == k0 ? SPMV_FIRST : 0) | (ke == k1 ? SPMV_LAST : 0)});
+        kb = ke;
+      } while (kb < k1);
+    }
+  }
+  D.chunk_ptr[D.ctas] = (int)D.chunks.size();
+}
+
 // The assembled operator's host-side structure.  `fits`: S is at most a quarter of the panel bytes and all terms stage
-// in one pass; only then are row_ptr, col, pos and terms built.  `device_bytes`: what its device buffers take.
+// in one pass; only then are row_ptr, col, pos and terms built, and the product's deal for spmv_ctas CTAs (none when
+// spmv_ctas = 0).  `device_bytes`: what its device buffers take.
 struct AsmPlan {
   long long nt = 0, nblk = 0, nnzb = 0, s_bytes = 0, device_bytes = 0;
   bool fits = false;
@@ -408,9 +455,10 @@ struct AsmPlan {
   std::vector<int> col;            // [nnzb] ascending in every row
   std::vector<IntPair> pos;        // [nblk] the pair's lower (ca, cb) and upper (cb, ca) block in the CSR; -1: diagonal
   std::vector<AsmTerm> terms;      // [nt] landmark-major
+  SpmvDeal spmv;                   // the rows of k_rcs_spmv's CTAs
 };
 
-inline void plan_assembled(const Layout& L, const PairList& P, int scalar_size, AsmPlan& A) {
+inline void plan_assembled(const Layout& L, const PairList& P, int scalar_size, AsmPlan& A, int spmv_ctas = 0) {
   A = AsmPlan();
   const int nc = L.nc;
   A.nblk = (long long)P.blk_cam.size();
@@ -422,9 +470,10 @@ inline void plan_assembled(const Layout& L, const PairList& P, int scalar_size, 
   A.switch_iteration = asm_switch_iteration(A.nt, L.panel_scalars, A.s_bytes, scalar_size);
   A.fits = 4 * A.s_bytes <= L.panel_scalars * scalar_size && 81 * A.nt * scalar_size <= ASM_STAGE_BYTES;
   if (!A.fits) return;
-  // S, S_u and the staging buffer; the terms as panel addresses, wpos and the terms as slot pairs; blk_ptr, row_ptr, col; pos
-  A.device_bytes = A.s_bytes + (A.nblk + A.nt) * 81 * scalar_size + A.nt * (long long)(sizeof(AsmTerm) + sizeof(int) + sizeof(IntPair)) +
-                   (A.nblk + A.nnzb + nc + 2) * (long long)sizeof(int) + A.nblk * (long long)sizeof(IntPair);
+  // S (and 16 bytes of padding), S_u and the staging buffer; the terms as panel addresses, wpos and the terms as slot pairs;
+  // blk_ptr, col; pos; the product's deal below
+  A.device_bytes = A.s_bytes + 16 + (A.nblk + A.nt) * 81 * scalar_size + A.nt * (long long)(sizeof(AsmTerm) + sizeof(int) + sizeof(IntPair)) +
+                   (A.nblk + 1 + A.nnzb) * (long long)sizeof(int) + A.nblk * (long long)sizeof(IntPair);
   // row ca gets (ca, cb) and row cb the transpose; iterating the pairs in (ca, cb) order fills every row in ascending
   // column order (lower blocks, the diagonal, then upper blocks)
   A.row_ptr.assign((size_t)nc + 1, 0);
@@ -448,6 +497,10 @@ inline void plan_assembled(const Layout& L, const PairList& P, int scalar_size, 
     const int g = sidx - T.lm_base;
     for (int a = 0; a < T.n; ++a)
       for (int b = 0; b <= a; ++b) A.terms.push_back(pack_asm_term(T.panel_off + 2LL * g * T.G, a, b, T.n, T.G, T.KP));
+  }
+  if (spmv_ctas > 0) {
+    deal_spmv(A.row_ptr, spmv_ctas, spmv_chunk_blocks(scalar_size), A.spmv);
+    A.device_bytes += (long long)A.spmv.chunks.size() * (long long)sizeof(SpmvChunk) + (A.spmv.ctas + 1) * (long long)sizeof(int);
   }
 }
 

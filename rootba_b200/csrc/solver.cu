@@ -250,8 +250,14 @@ struct Solver : rba_handle {
   int asm_nblk = 0, asm_switch = 0; long long asm_nt = 0, asm_nnzb = 0;
   AsmTerm* d_asm_terms = nullptr; int* d_asm_wpos = nullptr; int* d_asm_blk_ptr = nullptr; IntPair* d_asm_pos = nullptr;
   IntPair* d_asm_slots = nullptr;
-  int* d_asm_row_ptr = nullptr; int* d_asm_col = nullptr;
+  int* d_asm_col = nullptr;
   S* d_asm_stage = nullptr; S* d_asm_Su = nullptr; S* d_asm_S = nullptr;
+  // k_rcs_spmv's deal (deal_spmv): its chunks, CTA by CTA, for spmv_grid co-resident CTAs
+  SpmvChunk* d_spmv_chunks = nullptr; int* d_spmv_chunk_ptr = nullptr; int spmv_grid = 0, spmv_cap = 0;
+  // s_fresh: the assembly has just been enqueued, so the next k_rcs_spmv must not read S before the assembly has completed:
+  // it is a plain stream launch (its bulk copies of S start before griddepcontrol.wait, which orders only against the
+  // kernel right before it, and k_rcs_mirror, the last writer of S, never triggers its dependents)
+  bool s_fresh = false;
 
   ~Solver() override {
     if (comm && nccl) nccl->CommDestroy(comm);
@@ -362,12 +368,15 @@ struct Solver : rba_handle {
   //   RBA_PEER_AR=0       NCCL for the reductions across shards (taken when the IPC mapping of a peer fails)
   //   RBA_ASSEMBLED_RCS=0 the panel product P^T (P x) instead of the assembled S x (taken when S does not qualify)
   //   RBA_ASSEMBLED_AT=k  S built at PCG iteration k instead of the break-even iteration (taken by solves that run long)
+  //   RBA_SPMV_CTAS=k     S x dealt over at most k CTAs (several rows and stage-ring wraps per CTA, taken by problems with
+  //                       more block rows than co-resident CTAs)
   void read_test_hooks() {
     if (const char* e = getenv("RBA_PCG_PARTIALS")) pcg_partials = atoi(e) != 0;
     if (const char* e = getenv("RBA_PCG_CLUSTER")) pcg_cluster = std::max(1, std::min(atoi(e), 16));
     if (const char* e = getenv("RBA_PEER_AR")) peer_ar = atoi(e) != 0;
     if (const char* e = getenv("RBA_ASSEMBLED_RCS")) asm_hook = atoi(e) != 0;
     if (const char* e = getenv("RBA_ASSEMBLED_AT")) asm_at = std::max(0, atoi(e));
+    if (const char* e = getenv("RBA_SPMV_CTAS")) spmv_cap = std::max(1, atoi(e));
   }
 
   int upload_layout(const rba_problem_view* pv) {
@@ -1288,8 +1297,12 @@ struct Solver : rba_handle {
     const int* done = in_solve ? &d_state->done : nullptr;
     const bool pdl = in_solve;
     ++tm.matvec_launches;
-    if (h == Handover::Assembled)
-      return launch_ex(k_rcs_spmv<S>, nc, SPMV_WARPS * 32, 0, pdl, 1, (const int*)d_asm_row_ptr, (const int*)d_asm_col, (const S*)d_asm_S, xvec, D.y, done, (int)pdl);
+    if (h == Handover::Assembled) {
+      const bool p = pdl && !s_fresh;
+      s_fresh = false;
+      return launch_ex(k_rcs_spmv<S>, spmv_grid, SPMV_CLASSES * 32, 0, p, 1, (const SpmvChunk*)d_spmv_chunks, (const int*)d_spmv_chunk_ptr,
+                       (const int*)d_asm_col, (const S*)d_asm_S, xvec, D.y, done, (int)p);
+    }
     if (panels) {  // yobs = P^T P x
       if (L.n_items_large > 0) {
         k_matvec_large<S, K4_WARPS, KPMAX><<<grid_for(L.n_items_large, K4_WARPS, 4), K4_WARPS * 32, k4_smem_small, stream>>>(
@@ -1508,7 +1521,7 @@ struct Solver : rba_handle {
           su_new = !su_valid;
           if (su_new) assemble(0);
           assemble(1);
-          su_valid = s_valid = true;
+          su_valid = s_valid = s_fresh = true;
           h = handover();
         }
         rc = enqueue_iteration(i); if (rc) return rc;
@@ -1806,8 +1819,12 @@ struct Solver : rba_handle {
     PairList P;
     const std::string msg = build_pair_list(L, P);
     if (!msg.empty()) { g_err = msg; return RBA_ERR_UNSUPPORTED; }
+    // the product's deal is for the CTAs that are co-resident on an idle GPU
+    int occ = 0;
+    CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_rcs_spmv<S>, SPMV_CLASSES * 32, 0));
     AsmPlan A;
-    plan_assembled(L, P, sizeof(S), A);
+    const int ctas = std::max(1, occ) * sm_count;
+    plan_assembled(L, P, sizeof(S), A, spmv_cap > 0 ? std::min(spmv_cap, ctas) : ctas);
     if (!A.fits) return RBA_OK;
     size_t free_b = 0, total_b = 0;
     CU(cudaMemGetInfo(&free_b, &total_b));
@@ -1817,11 +1834,13 @@ struct Solver : rba_handle {
     TRY(upload(&d_asm_slots, P.terms));
     TRY(upload(&d_asm_blk_ptr, P.blk_ptr));
     TRY(upload(&d_asm_pos, A.pos));
-    TRY(upload(&d_asm_row_ptr, A.row_ptr));
     TRY(upload(&d_asm_col, A.col));
+    TRY(upload(&d_spmv_chunks, A.spmv.chunks));
+    TRY(upload(&d_spmv_chunk_ptr, A.spmv.chunk_ptr));
+    spmv_grid = A.spmv.ctas;
     TRY(dalloc(&d_asm_stage, (size_t)A.nt * 81, false));
     TRY(dalloc(&d_asm_Su, (size_t)A.nblk * 81));
-    TRY(dalloc(&d_asm_S, (size_t)A.nnzb * 81));
+    TRY(dalloc(&d_asm_S, (size_t)A.nnzb * 81 + 16 / sizeof(S)));  // + 16 bytes: k_rcs_spmv's bulk copies round up
     asm_nt = A.nt; asm_nblk = (int)A.nblk; asm_nnzb = A.nnzb;
     asm_switch = asm_at > 0 ? asm_at : A.switch_iteration;
     asm_on = true;
