@@ -13,7 +13,8 @@ covariance_model.landmark_factors) and K_i = W_l^T Jl_i^T Jp_i per slot i of l (
 - factors: S, K, W, rank and kappa_l by the device's eigen-elimination, with landmark priors (Hll += L^T L).
 - reference: Sigma (held entries deleted, intrinsics groups expanded P S_u^-1 P^T), the condition kappa of the equilibrated S,
   and sigma = sqrt(diag Sigma).
-- blocks: the four formulas for the requests, vectorised; `fault` plants one of the errors the check must catch.
+- blocks: the four formulas for the requests, vectorised; `fault` plants one of the errors the check must catch: BASE_FAULTS
+  in the formulas themselves, CLASS_FAULTS in the loops and inputs of the kernels (tests/covariance_block_classes.py).
 - dense_blocks: the same blocks cut from the full inverse of the dense total system (the definition).
 - bar_scales / check: the componentwise check of the device tests, bars c (N kappa + n kappa_l) u as in section 16.
 """
@@ -24,7 +25,14 @@ import covariance_model as cvm
 
 U = 2.0 ** -53
 KINDS = ("cameras", "camera_landmark", "landmarks", "relative")
-FAULTS = ("cam_lm_sign", "identity_off_diagonal", "transposed_cameras", "aj_sign", "no_t_rel")
+BASE_FAULTS = ("cam_lm_sign", "identity_off_diagonal", "transposed_cameras", "aj_sign", "no_t_rel")
+# slot_pair_order: a landmark pair's slot pairs decoded as (t / n_l, t % n_l) instead of (t / n_m, t % n_m) (slots past the
+#   landmark's own are its neighbours', as the kernel would read them); first_pass_only: only the first 32 slots (camera-
+#   landmark) or slot pairs (landmark pairs) summed, one pass of the warp; w_swapped: W_m on the left of a landmark pair;
+#   member_not_expanded: the intrinsics rows and columns of Sigma of the members of an intrinsics group left 0;
+#   lm_prior_dropped: the landmark priors' L^T L left out of Hll
+CLASS_FAULTS = ("slot_pair_order", "first_pass_only", "w_swapped", "member_not_expanded", "lm_prior_dropped")
+FAULTS = BASE_FAULTS + CLASS_FAULTS
 
 
 def factors(jp, jl, obs_cam, lm_off, nc, H_extra=None, lm_info=None):
@@ -83,7 +91,9 @@ def reference(jp, jl, obs_cam, lm_off, cams, H_extra=None, lm_info=None, fixed=N
     Sig[:, fixed] = 0.0
     sigma = np.sqrt(np.diag(Sig))
     return dict(Sig=Sig, K=K, W=W, rank=rank, kappa_l=kappa_l, kappa=kappa, sigma=sigma, N=int(fu.sum()),
-                obs_cam=np.asarray(obs_cam), lm_off=np.asarray(lm_off), cams=cams)
+                obs_cam=np.asarray(obs_cam), lm_off=np.asarray(lm_off), cams=cams, lead=lead,
+                inputs=dict(jp=jp, jl=jl, obs_cam=obs_cam, lm_off=lm_off, cams=cams, H_extra=H_extra, lm_info=lm_info,
+                            fixed=fixed, lead=lead))
 
 
 def relative_jacobian(ci, cj, device_rot=True, fault=None):
@@ -124,8 +134,16 @@ def _sum_by(k, v, m):
 def blocks(ref, cameras=None, camera_landmark=None, landmarks=None, relative=None, fault=None, chunk=1 << 16):
     """the four formulas for the requests ([m, 2] int arrays or None) from reference(): dict of [m, 9, 9], [m, 9, 3],
     [m, 3, 3], [m, 6, 6]; blocks of a landmark of rank < 3 are NaN.  fault: one of FAULTS."""
+    if fault == "lm_prior_dropped":
+        ref, fault = reference(**dict(ref["inputs"], lm_info=None)), None
     Sig, K, W, rank, obs_cam, lm_off = ref["Sig"], ref["K"], ref["W"], ref["rank"], ref["obs_cam"], ref["lm_off"]
     nc = Sig.shape[0] // 9
+    if fault == "member_not_expanded" and ref["lead"] is not None:
+        import shared_intrinsics_model as sim
+        Sig = Sig.copy()
+        mem = sim.members(ref["lead"])
+        Sig[mem, :] = 0.0
+        Sig[:, mem] = 0.0
     S4 = Sig.reshape(nc, 9, nc, 9)
     out = {}
     if cameras is not None:
@@ -134,6 +152,9 @@ def blocks(ref, cameras=None, camera_landmark=None, landmarks=None, relative=Non
     if camera_landmark is not None:
         c, l = np.asarray(camera_landmark).T
         k, s = _slot_pairs(lm_off, l)
+        if fault == "first_pass_only":
+            first = s - lm_off[l[k]] < 32
+            k, s = k[first], s[first]
         u = _sum_by(k, np.einsum("kpq,kjq->kpj", S4[c[k], :, obs_cam[s], :], K[s]), len(c))
         o = -np.einsum("kpj,krj->kpr", u, W[l])
         if fault == "cam_lm_sign":
@@ -148,15 +169,18 @@ def blocks(ref, cameras=None, camera_landmark=None, landmarks=None, relative=Non
         cnt = n[lq] * n[mq]
         kk = np.repeat(np.arange(len(lq)), cnt)
         t = np.arange(cnt.sum()) - np.repeat(np.cumsum(cnt) - cnt, cnt)
-        si = lm_off[lq][kk] + t // n[mq][kk]
-        sj = lm_off[mq][kk] + t % n[mq][kk]
+        dec = n[lq][kk] if fault == "slot_pair_order" else n[mq][kk]
+        si = np.minimum(lm_off[lq][kk] + t // dec, len(obs_cam) - 1)
+        sj = np.minimum(lm_off[mq][kk] + t % dec, len(obs_cam) - 1)
+        if fault == "first_pass_only":
+            kk, si, sj = kk[t < 32], si[t < 32], sj[t < 32]
         for c0 in range(0, len(kk), chunk):
             sl = slice(c0, c0 + chunk)
             v = np.einsum("kap,kpq,kbq->kab", K[si[sl]], S4[obs_cam[si[sl]], :, obs_cam[sj[sl]], :], K[sj[sl]], optimize=True)
             np.add.at(X, kk[sl], v)
         same = (lq == mq) if fault != "identity_off_diagonal" else np.ones(len(lq), bool)
         X[same] += np.eye(3)
-        o = np.einsum("kix,kxy,kjy->kij", W[lq], X, W[mq])
+        o = np.einsum("kix,kxy,kjy->kij", W[mq] if fault == "w_swapped" else W[lq], X, W[mq])
         o[(rank[lq] < 3) | (rank[mq] < 3)] = np.nan
         out["landmarks"] = o
     if relative is not None:

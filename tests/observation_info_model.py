@@ -40,10 +40,11 @@ def random_info(nobs, seed, cond=10.0, lo=0.3, hi=3.0):
     return orth() @ S @ np.swapaxes(orth(), 1, 2)
 
 
-def whitened(arrays, W, dtype=np.float64, threshold=None, valid_only=False, fault=None):
+def whitened(arrays, W, dtype=np.float64, threshold=None, valid_only=False, fault=None, device_rot=False):
     """per observation the rows sqrt(hw) W [Jp (2x9) | Jl (2x3) | r], the whitened residual W r, hw, the projection validity
-    and the in-use mask (W != 0).  Rows of a switched-off observation, and with valid_only of an invalid projection, are 0."""
-    L = cm.linearize(*cm.observations(arrays), dtype=dtype)
+    and the in-use mask (W != 0).  Rows of a switched-off observation, and with valid_only of an invalid projection, are 0.
+    device_rot: rotations as the kernels build them (camera_model.linearize)."""
+    L = cm.linearize(*cm.observations(arrays), dtype=dtype, device_rot=device_rot)
     W = expand(W, len(L["res"]))
     on = np.any(W.reshape(-1, 4) != 0, axis=1)
     Wj = np.swapaxes(W, 1, 2) if fault == "transposed" else W

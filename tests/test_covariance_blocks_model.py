@@ -157,7 +157,7 @@ def test_halving_identity():
     assert np.abs(after - before / 2).max() <= 1e-9 * np.abs(before).max()
 
 
-@pytest.mark.parametrize("fault", cbm.FAULTS)
+@pytest.mark.parametrize("fault", cbm.BASE_FAULTS)
 def test_planted_faults_are_rejected(fault):
     nc, nl = 6, 40
     prob, jp, jl, Jc, _, _ = _instance(nc, nl, 11)
