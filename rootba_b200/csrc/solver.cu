@@ -12,6 +12,7 @@
 #include <limits>
 #include <memory>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "../../include/rootba_b200.h"
@@ -42,6 +43,21 @@ static_assert(sizeof(IntPair) == sizeof(int2), "IntPair must have the layout of 
 struct EventPair {
   cudaEvent_t a = nullptr, b = nullptr;
   bool used = false;
+};
+
+// Owns one cudaMalloc'd array of `size()` entries (Solver::alloc makes them) and frees it with itself.  Move-only.
+template <class T>
+class DeviceBuffer {
+  T* p_ = nullptr; size_t n_ = 0;
+ public:
+  DeviceBuffer() = default;
+  DeviceBuffer(T* p, size_t n) : p_(p), n_(n) {}
+  DeviceBuffer(DeviceBuffer&& o) noexcept : p_(std::exchange(o.p_, nullptr)), n_(std::exchange(o.n_, 0)) {}
+  DeviceBuffer& operator=(DeviceBuffer&& o) noexcept { std::swap(p_, o.p_); std::swap(n_, o.n_); return *this; }  // o frees the old array
+  ~DeviceBuffer() { if (p_) cudaFree(p_); }
+  T* get() const { return p_; }
+  size_t size() const { return n_; }  // the entries asked for
+  void take(DeviceBuffer& o) { if (o.p_) *this = std::move(o); }  // a setter's commit: o's array, if it has one
 };
 
 }  // namespace rba
@@ -117,7 +133,7 @@ struct Solver : rba_handle {
   int device = 0;
   int sm_count = 132;
   cudaStream_t stream = nullptr;
-  std::vector<void*> allocs;
+  std::vector<DeviceBuffer<char>> owned;  // the buffers of set-up (dalloc), freed with the handle
   size_t device_bytes = 0;
   DevPtrs<S> D{};
   // device-only helpers
@@ -176,50 +192,56 @@ struct Solver : rba_handle {
   bool have_inc = false;
   S last_lambda = 0;
   bool damping_valid = false;
-  uint8_t* d_cam_fixed = nullptr;  // [nc] flags of rba_set_camera_fixed; D.cam_fixed points here while any flag is set
-  bool all_cams_fixed = false;     // no free camera parameter: the reduced system is empty and its solve is skipped
-  // camera priors (rba_set_camera_prior, DESIGN.md section 14); has_abs_prior while any L_c is non-zero.  D.prior_H points at
-  // d_prior_H while there are absolute or pair priors.
-  bool has_abs_prior = false;
-  S* d_prior_mean = nullptr;       // [nc][10] mean, quaternion normalised
-  S* d_prior_L = nullptr;          // [nc][81] square-root information
-  S* d_prior_A = nullptr;          // [nc][81] L de/d(inc): unscaled after k_prior_linearize, scaled after k_prior_scale
-  S* d_prior_r = nullptr;          // [nc][9]  L e at the linearisation point
-  S* d_prior_H = nullptr;          // [nc][81] A^T A (+ the pair priors' diagonal blocks)
-  S* d_prior_g = nullptr;          // [nc][9]  A^T r (+ the pair priors' A_s^T r)
-  // pair priors (rba_set_camera_pair_prior, DESIGN.md section 15): n_pairs pairs with a non-zero L, D.pair_ov set while
-  // n_pairs > 0.  Buffers are sized for pair_cap pairs.
-  int n_pairs = 0, pair_cap = 0;
-  int* d_pair_ij = nullptr;        // [m][2] cameras (i, j)
-  S* d_pair_mean = nullptr;        // [m][7] R0 quaternion (normalised), t0
-  S* d_pair_L = nullptr;           // [m][36] square-root information
-  S* d_pair_A = nullptr;           // [m][2][36] pose blocks A_i, A_j: unscaled after k_pair_linearize, scaled after k_pair_scale
-  S* d_pair_r = nullptr;           // [m][6] L e at the linearisation point
-  int* d_pair_item = nullptr;      // [2m] incident sides 2 p + side, camera-major (CSR d_pair_ptr)
-  int* d_pair_nbr = nullptr;       // [2m] the other camera of each side
-  S* d_pair_O = nullptr;           // [2m][36] O of each directed edge
-  int* d_pair_ptr = nullptr;       // [nc + 1]
-  S* d_pair_ov = nullptr;          // [9 nc]
-  // landmark priors (rba_set_landmark_prior, DESIGN.md section 17): the n_lmp priors of this shard with a non-zero L;
-  // D.lmp_slot set while n_lmp > 0.  Buffers are sized for lmp_cap priors.
-  int n_lmp = 0, lmp_cap = 0;
-  int* d_lmp_slot = nullptr;       // [nsorted] prior slot per sorted landmark, -1 = none
-  int* d_lmp_of_lm = nullptr;      // [nl_local] prior slot per local landmark, -1 = none (rba_compute_covariance)
-  int* d_lmp_lm = nullptr;         // [m] local landmark of each prior
-  S* d_lmp_mean = nullptr;         // [m][3]
-  S* d_lmp_L = nullptr;            // [m][9]
-  S* d_lmp_Lg = nullptr;           // [m][12]
-  // intrinsics groups (rba_set_intrinsics_groups, DESIGN.md section 18): n_groups groups of >= 2 cameras; 0 = the
-  // unmodified path
-  int n_groups = 0;
-  std::vector<int> h_grp_lead;     // [nc] lead of the camera's group, -1 = own intrinsics (also a group of one)
-  std::vector<uint8_t> h_fixed;    // [nc] the flags of rba_set_camera_fixed, empty = none
-  int* d_grp_lead = nullptr; int* d_grp_ptr = nullptr; int* d_grp_mem = nullptr;
-  uint8_t* d_grp_fixed = nullptr;  // [nc] the user's flags + RBA_FIX_INTRINSICS on every member but the lead
-  S* d_grp_ve = nullptr;           // [9 nc] the expanded operator input P v
-  S* d_grp_y = nullptr;            // [9 nc] the contracted operator output the vector step reads
-  // observation information (rba_set_observation_info, DESIGN.md section 19): D.obs_W points here while it is set
-  S* d_obs_W = nullptr;            // [nslots][4]
+  // The problem terms of the setters.  A setter fills the term's buffers while the new lists fit in them (their size is the
+  // capacity), else new ones in a local term, which it adopts once every buffer exists and is filled: a failed call leaves
+  // the previous term in force.  point_at_terms derives the kernels' pointers from the terms.
+  struct HeldTerm {                // rba_set_camera_fixed; D.cam_fixed = flags while any flag is set
+    std::vector<uint8_t> host;     // [nc] the flags, empty = none
+    DeviceBuffer<uint8_t> flags;   // [nc]
+    bool all = false;              // no free camera parameter: the reduced system is empty and its solve is skipped
+  } held;
+  struct CameraPriorTerm {         // rba_set_camera_prior, DESIGN.md section 14; D.prior_H = H while there are absolute or pair priors
+    bool on = false;               // any L_c is non-zero
+    DeviceBuffer<S> mean;          // [nc][10] mean, quaternion normalised
+    DeviceBuffer<S> L;             // [nc][81] square-root information
+    DeviceBuffer<S> A;             // [nc][81] L de/d(inc): unscaled after k_prior_linearize, scaled after k_prior_scale
+    DeviceBuffer<S> r;             // [nc][9]  L e at the linearisation point
+    DeviceBuffer<S> H;             // [nc][81] A^T A (+ the pair priors' diagonal blocks)
+    DeviceBuffer<S> g;             // [nc][9]  A^T r (+ the pair priors' A_s^T r)
+    void adopt(CameraPriorTerm& o) { mean.take(o.mean); L.take(o.L); A.take(o.A); r.take(o.r); H.take(o.H); g.take(o.g); }
+  } cprior;
+  struct PairPriorTerm {           // rba_set_camera_pair_prior, DESIGN.md section 15; D.pair_ov set while n > 0
+    int n = 0;                     // pairs with a non-zero L (m: the capacity)
+    DeviceBuffer<int> ij;          // [m][2] cameras (i, j)
+    DeviceBuffer<S> mean;          // [m][7] R0 quaternion (normalised), t0
+    DeviceBuffer<S> L;             // [m][36] square-root information
+    DeviceBuffer<S> A;             // [m][2][36] pose blocks A_i, A_j: unscaled after k_pair_linearize, scaled after k_pair_scale
+    DeviceBuffer<S> r;             // [m][6] L e at the linearisation point
+    DeviceBuffer<int> item;        // [2m] incident sides 2 p + side, camera-major (CSR ptr)
+    DeviceBuffer<int> nbr;         // [2m] the other camera of each side
+    DeviceBuffer<S> O;             // [2m][36] O of each directed edge
+    DeviceBuffer<int> ptr;         // [nc + 1]
+    DeviceBuffer<S> ov;            // [9 nc]
+    void adopt(PairPriorTerm& o) { ij.take(o.ij); mean.take(o.mean); L.take(o.L); A.take(o.A); r.take(o.r); item.take(o.item);
+                                   nbr.take(o.nbr); O.take(o.O); ptr.take(o.ptr); ov.take(o.ov); }
+  } pprior;
+  struct LandmarkPriorTerm {       // rba_set_landmark_prior, DESIGN.md section 17; D.lmp_slot set while n > 0
+    int n = 0;                     // priors of this shard with a non-zero L (m: the capacity)
+    DeviceBuffer<int> slot;        // [nsorted] prior slot per sorted landmark, -1 = none
+    DeviceBuffer<int> of_lm;       // [nl_local] prior slot per local landmark, -1 = none (rba_compute_covariance)
+    DeviceBuffer<int> lm;          // [m] local landmark of each prior
+    DeviceBuffer<S> mean, L, Lg;   // [m][3], [m][9], [m][12]
+    void adopt(LandmarkPriorTerm& o) { slot.take(o.slot); of_lm.take(o.of_lm); lm.take(o.lm); mean.take(o.mean); L.take(o.L); Lg.take(o.Lg); }
+  } lprior;
+  struct GroupTerm {               // rba_set_intrinsics_groups, DESIGN.md section 18
+    int n = 0;                     // groups of >= 2 cameras; 0 = the unmodified path
+    std::vector<int> host_lead;    // [nc] lead of the camera's group, -1 = own intrinsics (also a group of one)
+    DeviceBuffer<int> lead, ptr, mem;  // new lists ({} to fit) at every call with groups
+    DeviceBuffer<uint8_t> fixed;   // [nc] the user's flags + RBA_FIX_INTRINSICS on every member but the lead
+    DeviceBuffer<S> ve, y;         // [9 nc] the expanded operator input P v, the contracted output the vector step reads
+    void adopt(GroupTerm& o) { lead.take(o.lead); ptr.take(o.ptr); mem.take(o.mem); fixed.take(o.fixed); ve.take(o.ve); y.take(o.y); }
+  } grp;
+  struct { bool on = false; DeviceBuffer<S> W; } obs;  // rba_set_observation_info, DESIGN.md section 19: W [nslots][4] = D.obs_W while on
   rba_stage_timings tm{};
   EventPair ev_stage1, ev_stage2, ev_precond, ev_pcg, ev_backsub, ev_update, ev_error, ev_mv, ev_user;
   long long launches = 0;
@@ -262,7 +284,6 @@ struct Solver : rba_handle {
   ~Solver() override {
     if (comm && nccl) nccl->CommDestroy(comm);
     for (void* p : ipc_opened) cudaIpcCloseMemHandle(p);
-    for (void* p : allocs) cudaFree(p);
     if (h_prog) cudaFreeHost(h_prog);
     if (h_state) cudaFreeHost(h_state);
     if (h_res) cudaFreeHost(h_res);
@@ -274,30 +295,43 @@ struct Solver : rba_handle {
     if (stream) cudaStreamDestroy(stream);
   }
 
+  // Every device allocation of the handle: max(count, 1) entries, zeroed on the stream when asked; device_bytes counts all but
+  // the covariance lists and per-call scratch (`counted` false) and never goes down (the most the handle has allocated).
   template <class T>
-  int dalloc(T** p, size_t count, bool zero = true) {
+  int alloc(DeviceBuffer<T>& b, size_t count, bool zero, bool counted = true) {
     const size_t bytes = std::max<size_t>(count, 1) * sizeof(T);
     void* q = nullptr;
     CU(cudaMalloc(&q, bytes));
-    allocs.push_back(q);
-    device_bytes += bytes;
+    b = DeviceBuffer<T>((T*)q, count);
+    if (counted) device_bytes += bytes;
     if (zero) CU(cudaMemsetAsync(q, 0, bytes, stream));
-    *p = (T*)q;
-    return RBA_OK;
-  }
-  // frees a buffer of dalloc (nullptr: nothing to do); device_bytes keeps counting it (the most the handle has allocated)
-  int dfree(void* q) {
-    if (!q) return RBA_OK;
-    allocs.erase(std::find(allocs.begin(), allocs.end(), q));
-    CU(cudaFree(q));
     return RBA_OK;
   }
   template <class T>
-  int upload(T** p, const std::vector<T>& v) {
-    int rc = dalloc(p, v.size(), false);
-    if (rc) return rc;
-    if (!v.empty()) CU(cudaMemcpyAsync(*p, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice, stream));
+  int copy_in(T* dst, const std::vector<T>& v) {
+    if (!v.empty()) CU(cudaMemcpyAsync(dst, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice, stream));
     return RBA_OK;
+  }
+  // A buffer that lives as long as the handle (set-up), owned as max(count, 1) * sizeof(T) bytes.
+  template <class T>
+  int dalloc(T** p, size_t count, bool zero = true, bool counted = true) {
+    DeviceBuffer<char> b;
+    TRY(alloc(b, std::max<size_t>(count, 1) * sizeof(T), zero, counted));
+    *p = (T*)b.get();
+    owned.push_back(std::move(b));
+    return RBA_OK;
+  }
+  template <class T>
+  int upload(T** p, const std::vector<T>& v, bool counted = true) {
+    TRY(dalloc(p, v.size(), false, counted));
+    return copy_in(*p, v);
+  }
+  // A setter's buffer of `count` entries: the term's own `cur` while it holds as many, else a new one (not zeroed) in
+  // `next`, which the setter adopts once every buffer of its call exists.  `src` is copied into the one chosen.
+  template <class T>
+  int fit(DeviceBuffer<T>& next, const DeviceBuffer<T>& cur, size_t count, const std::vector<T>* src = nullptr) {
+    if (!cur.get() || cur.size() < count) TRY(alloc(next, count, false));
+    return src ? copy_in(next.get() ? next.get() : cur.get(), *src) : RBA_OK;
   }
 
   int start(EventPair& e) { e.used = true; CU(cudaEventRecord(e.a, stream)); return RBA_OK; }
@@ -675,7 +709,7 @@ struct Solver : rba_handle {
   int set_state(const void* cams, const void* lms) override {
     ++state_version;
     std::vector<S> tied;
-    if (n_groups) {  // the members take their lead's f, k1, k2
+    if (grp.n) {  // the members take their lead's f, k1, k2
       tied.assign((const S*)cams, (const S*)cams + (size_t)10 * nc);
       tie_intrinsics(tied.data());
       cams = tied.data();
@@ -717,25 +751,25 @@ struct Solver : rba_handle {
       }
     std::vector<uint8_t> fl;
     if (any) fl.assign(flags, flags + nc);
-    if (n_groups) {
-      const std::string why = group_flags_mismatch(h_grp_lead, fl);
+    if (grp.n) {
+      const std::string why = group_flags_mismatch(grp.host_lead, fl);
       if (!why.empty()) { g_err = "rba_set_camera_fixed: " + why; return RBA_ERR_INVALID_ARGUMENT; }
     }
     if (any) {
-      if (!d_cam_fixed) { int rc = dalloc(&d_cam_fixed, (size_t)nc, false); if (rc) return rc; }
-      CU(cudaMemcpyAsync(d_cam_fixed, flags, (size_t)nc, cudaMemcpyHostToDevice, stream));
+      DeviceBuffer<uint8_t> next; TRY(fit(next, held.flags, (size_t)nc, &fl));
       CU(cudaStreamSynchronize(stream));
+      held.flags.take(next);
     }
-    D.cam_fixed = any ? d_cam_fixed : nullptr;
-    all_cams_fixed = all;
-    h_fixed = std::move(fl);
-    if (n_groups) TRY(upload_group_fixed());
+    held.all = all;
+    held.host = std::move(fl);
+    point_at_terms();
+    if (grp.n) TRY(upload_group_fixed());
     have_inc = false;  // the device-resident increment was solved under the previous flags
     return RBA_OK;
   }
 
   // Intrinsics shared across groups of cameras (DESIGN.md section 18).  Every check runs before anything changes, so a
-  // rejected call leaves the previous groups.  No group of >= 2 cameras = the unmodified path (n_groups == 0).
+  // rejected call leaves the previous groups.  No group of >= 2 cameras = the unmodified path (grp.n == 0).
   int set_intrinsics_groups(const int32_t* group) override {
     auto fail = [&](int rc, const std::string& what) { g_err = "rba_set_intrinsics_groups: " + what; return rc; };
     std::vector<int> lead((size_t)nc, -1), first((size_t)nc, -1), count((size_t)nc, 0);
@@ -756,7 +790,7 @@ struct Solver : rba_handle {
       if (lead[c] == c) gidx[c] = ng++;
     if (ng > 0 && opt.solver_type == 2)
       return fail(RBA_ERR_UNSUPPORTED, "POWER_SCHUR_COMPLEMENT does not support groups of >= 2 cameras (Hpp of the tied problem is not block-diagonal)");
-    const std::string why = group_flags_mismatch(lead, h_fixed);
+    const std::string why = group_flags_mismatch(lead, held.host);
     if (!why.empty()) return fail(RBA_ERR_INVALID_ARGUMENT, why);
     ptr.assign((size_t)ng + 1, 0);
     for (int c = 0; c < nc; ++c)
@@ -767,23 +801,14 @@ struct Solver : rba_handle {
     for (int c = 0; c < nc; ++c)
       if (lead[c] >= 0) mem[fill[gidx[lead[c]]]++] = c;
     if (ng > 0) {
-      // the new lists go to fresh buffers and replace the previous ones only once every allocation has succeeded, so a
-      // failed call leaves the previous groups in force
-      int *lead_d = nullptr, *ptr_d = nullptr, *mem_d = nullptr;
-      TRY(upload(&lead_d, lead));
-      TRY(upload(&ptr_d, ptr));
-      TRY(upload(&mem_d, mem));
-      if (!d_grp_ve) {
-        S *ve = nullptr, *y = nullptr; uint8_t* fx = nullptr;
-        TRY(dalloc(&ve, (size_t)9 * nc)); TRY(dalloc(&y, (size_t)9 * nc)); TRY(dalloc(&fx, (size_t)nc));
-        d_grp_ve = ve; d_grp_y = y; d_grp_fixed = fx;
-      }
+      GroupTerm next;
+      TRY(fit(next.lead, {}, lead.size(), &lead)); TRY(fit(next.ptr, {}, ptr.size(), &ptr)); TRY(fit(next.mem, {}, mem.size(), &mem));
+      if (!grp.ve.get()) { TRY(alloc(next.ve, (size_t)9 * nc, true)); TRY(alloc(next.y, (size_t)9 * nc, true)); TRY(alloc(next.fixed, (size_t)nc, true)); }
       CU(cudaStreamSynchronize(stream));
-      TRY(dfree(d_grp_lead)); TRY(dfree(d_grp_ptr)); TRY(dfree(d_grp_mem));
-      d_grp_lead = lead_d; d_grp_ptr = ptr_d; d_grp_mem = mem_d;
+      grp.adopt(next);
     }
-    n_groups = ng;
-    h_grp_lead = std::move(lead);
+    grp.n = ng;
+    grp.host_lead = std::move(lead);
     if (ng > 0) {
       TRY(upload_group_fixed());
       // the current state and its backup take the tied values
@@ -811,21 +836,21 @@ struct Solver : rba_handle {
   }
   void tie_intrinsics(S* cams) const {
     for (int c = 0; c < nc; ++c)
-      if (h_grp_lead[c] >= 0 && h_grp_lead[c] != c)
-        for (int k = 7; k < 10; ++k) cams[10 * (size_t)c + k] = cams[10 * (size_t)h_grp_lead[c] + k];
+      if (grp.host_lead[c] >= 0 && grp.host_lead[c] != c)
+        for (int k = 7; k < 10; ++k) cams[10 * (size_t)c + k] = cams[10 * (size_t)grp.host_lead[c] + k];
   }
   // the flags k_precond_invert masks with: the user's, and the intrinsics of every member but the lead
   int upload_group_fixed() {
     std::vector<uint8_t> f((size_t)nc, 0);
     for (int c = 0; c < nc; ++c)
-      f[c] = (uint8_t)((h_fixed.empty() ? 0 : h_fixed[c]) | (h_grp_lead[c] >= 0 && h_grp_lead[c] != c ? RBA_FIX_INTRINSICS : 0));
-    CU(cudaMemcpyAsync(d_grp_fixed, f.data(), (size_t)nc, cudaMemcpyHostToDevice, stream));
+      f[c] = (uint8_t)((held.host.empty() ? 0 : held.host[c]) | (grp.host_lead[c] >= 0 && grp.host_lead[c] != c ? RBA_FIX_INTRINSICS : 0));
+    TRY(copy_in(grp.fixed.get(), f));
     CU(cudaStreamSynchronize(stream));
     return RBA_OK;
   }
-  GroupView groups() const { return {d_grp_lead, d_grp_ptr, d_grp_mem, n_groups}; }
+  GroupView groups() const { return {grp.lead.get(), grp.ptr.get(), grp.mem.get(), grp.n}; }
   int group_expand(const S* v, S* out, bool in_solve) {
-    return launch_ex(k_group_expand<S>, (9 * nc + 255) / 256, 256, 0, in_solve, 1, v, out, (const int*)d_grp_lead, nc,
+    return launch_ex(k_group_expand<S>, (9 * nc + 255) / 256, 256, 0, in_solve, 1, v, out, (const int*)grp.lead.get(), nc,
                      in_solve ? (const PcgState*)d_state : (const PcgState*)nullptr);
   }
   // Gaussian priors on the camera parameters.  They are part of the linearisation (Jacobi scaling, A, r), so a change needs a
@@ -854,12 +879,14 @@ struct Solver : rba_handle {
       }
     }
     if (any) {
-      TRY(grow_upload(!d_prior_mean, dbuf(d_prior_mean, (size_t)10 * nc, &mean), dbuf(d_prior_L, (size_t)81 * nc, &Lsq),
-                      dbuf(d_prior_A, (size_t)81 * nc), dbuf(d_prior_r, (size_t)9 * nc)));
-      TRY(alloc_prior_diag());
+      CameraPriorTerm next;
+      TRY(fit(next.mean, cprior.mean, (size_t)10 * nc, &mean)); TRY(fit(next.L, cprior.L, (size_t)81 * nc, &Lsq));
+      TRY(fit(next.A, cprior.A, (size_t)81 * nc)); TRY(fit(next.r, cprior.r, (size_t)9 * nc));
+      TRY(fit(next.H, cprior.H, (size_t)81 * nc)); TRY(fit(next.g, cprior.g, (size_t)9 * nc));
       CU(cudaStreamSynchronize(stream));
+      cprior.adopt(next);
     }
-    has_abs_prior = any;
+    cprior.on = any;
     return priors_changed();
   }
   // The checks of every prior setter on one prior, in this order: a finite mean (nm entries), a finite sqrt_info (nL
@@ -883,33 +910,20 @@ struct Solver : rba_handle {
     }
     return "";
   }
-  // One device buffer of a group: its entries when (re)allocated and, for an input, the host data copied into it.
-  template <class T>
-  struct DevBuf { T*& p; size_t count; const std::vector<T>* src; };
-  template <class T>
-  static DevBuf<T> dbuf(T*& p, size_t count, const std::vector<T>* src = nullptr) { return {p, count, src}; }
-  // Reallocates every buffer of the group when `grow` (contents not kept), then queues the copies of the inputs on the stream.
-  template <class... T>
-  int grow_upload(bool grow, DevBuf<T>... b) {
-    int rc = RBA_OK;
-    if (grow) {
-      ((rc = rc ? rc : dfree(b.p)), ...);
-      ((rc = rc ? rc : dalloc(&b.p, b.count, false)), ...);
-    }
-    ((rc = rc ? rc : copy_in(b.p, b.src)), ...);
-    return rc;
+  CameraPrior<S> camera_prior() const { return {D.cams, cprior.mean.get(), cprior.L.get(), cprior.A.get(), cprior.r.get()}; }
+  PairPrior<S> pair_prior() const { return {D.cams, pprior.ij.get(), pprior.mean.get(), pprior.L.get(), pprior.A.get(), pprior.r.get()}; }
+  // The kernels' optional pointers, from the problem terms (nullptr = the kernels without the term)
+  void point_at_terms() {
+    D.cam_fixed = held.host.empty() ? nullptr : held.flags.get();
+    D.prior_H = cprior.on || pprior.n > 0 ? cprior.H.get() : nullptr;
+    D.pair_ptr = pprior.ptr.get(); D.pair_nbr = pprior.nbr.get(); D.pair_O = pprior.O.get();
+    D.pair_ov = pprior.n > 0 ? pprior.ov.get() : nullptr;
+    D.lmp_slot = lprior.n > 0 ? lprior.slot.get() : nullptr;
+    D.lmp_mean = lprior.mean.get(); D.lmp_L = lprior.L.get(); D.lmp_Lg = lprior.Lg.get();
+    D.obs_W = obs.on ? obs.W.get() : nullptr;
   }
-  template <class T>
-  int copy_in(T* dst, const std::vector<T>* src) {
-    if (src) CU(cudaMemcpyAsync(dst, src->data(), src->size() * sizeof(T), cudaMemcpyHostToDevice, stream));
-    return RBA_OK;
-  }
-  int alloc_prior_diag() { return grow_upload(!d_prior_H, dbuf(d_prior_H, (size_t)81 * nc), dbuf(d_prior_g, (size_t)9 * nc)); }
-  CameraPrior<S> camera_prior() const { return {D.cams, d_prior_mean, d_prior_L, d_prior_A, d_prior_r}; }
-  PairPrior<S> pair_prior() const { return {D.cams, d_pair_ij, d_pair_mean, d_pair_L, d_pair_A, d_pair_r}; }
   int priors_changed() {
-    D.prior_H = (has_abs_prior || n_pairs > 0) ? d_prior_H : nullptr;
-    D.pair_ov = n_pairs > 0 ? d_pair_ov : nullptr;
+    point_at_terms();
     linearized = false;  // the scaling, A and r of the last linearisation belong to the previous priors
     damping_valid = false;
     have_inc = false;
@@ -954,18 +968,17 @@ struct Solver : rba_handle {
         item[q] = k;            // 2 p + side
         nbr[q] = ij[k ^ 1];
       }
-      TRY(grow_upload(np > pair_cap, dbuf(d_pair_ij, 2 * (size_t)np, &ij), dbuf(d_pair_mean, 7 * (size_t)np, &mean),
-                      dbuf(d_pair_L, 36 * (size_t)np, &Lsq), dbuf(d_pair_A, 72 * (size_t)np), dbuf(d_pair_r, 6 * (size_t)np),
-                      dbuf(d_pair_item, 2 * (size_t)np, &item), dbuf(d_pair_nbr, 2 * (size_t)np, &nbr), dbuf(d_pair_O, 72 * (size_t)np)));
-      pair_cap = std::max(pair_cap, np);
-      TRY(grow_upload(!d_pair_ptr, dbuf(d_pair_ptr, (size_t)nc + 1, &ptr), dbuf(d_pair_ov, 9 * (size_t)nc)));
-      TRY(alloc_prior_diag());
+      PairPriorTerm next; CameraPriorTerm diag;  // diag: H and g
+      TRY(fit(next.ij, pprior.ij, 2 * (size_t)np, &ij)); TRY(fit(next.mean, pprior.mean, 7 * (size_t)np, &mean));
+      TRY(fit(next.L, pprior.L, 36 * (size_t)np, &Lsq)); TRY(fit(next.A, pprior.A, 72 * (size_t)np));
+      TRY(fit(next.r, pprior.r, 6 * (size_t)np)); TRY(fit(next.item, pprior.item, 2 * (size_t)np, &item));
+      TRY(fit(next.nbr, pprior.nbr, 2 * (size_t)np, &nbr)); TRY(fit(next.O, pprior.O, 72 * (size_t)np));
+      TRY(fit(next.ptr, pprior.ptr, (size_t)nc + 1, &ptr)); TRY(fit(next.ov, pprior.ov, 9 * (size_t)nc));
+      TRY(fit(diag.H, cprior.H, (size_t)81 * nc)); TRY(fit(diag.g, cprior.g, (size_t)9 * nc));
       CU(cudaStreamSynchronize(stream));
+      pprior.adopt(next); cprior.adopt(diag);
     }
-    n_pairs = np;
-    D.pair_ptr = d_pair_ptr;
-    D.pair_nbr = d_pair_nbr;
-    D.pair_O = d_pair_O;
+    pprior.n = np;
     return priors_changed();
   }
 
@@ -1001,17 +1014,14 @@ struct Solver : rba_handle {
     }
     const int np = (int)lm.size();
     if (np > 0) {
-      TRY(grow_upload(np > lmp_cap, dbuf(d_lmp_lm, (size_t)np, &lm), dbuf(d_lmp_mean, 3 * (size_t)np, &mean),
-                      dbuf(d_lmp_L, 9 * (size_t)np, &Lsq), dbuf(d_lmp_Lg, 12 * (size_t)np)));
-      lmp_cap = std::max(lmp_cap, np);
-      TRY(grow_upload(!d_lmp_slot, dbuf(d_lmp_slot, slot.size(), &slot), dbuf(d_lmp_of_lm, of_lm.size(), &of_lm)));
+      LandmarkPriorTerm next;
+      TRY(fit(next.lm, lprior.lm, (size_t)np, &lm)); TRY(fit(next.mean, lprior.mean, 3 * (size_t)np, &mean));
+      TRY(fit(next.L, lprior.L, 9 * (size_t)np, &Lsq)); TRY(fit(next.Lg, lprior.Lg, 12 * (size_t)np));
+      TRY(fit(next.slot, lprior.slot, slot.size(), &slot)); TRY(fit(next.of_lm, lprior.of_lm, of_lm.size(), &of_lm));
       CU(cudaStreamSynchronize(stream));
+      lprior.adopt(next);
     }
-    n_lmp = np;
-    D.lmp_slot = np > 0 ? d_lmp_slot : nullptr;
-    D.lmp_mean = d_lmp_mean;
-    D.lmp_L = d_lmp_L;
-    D.lmp_Lg = d_lmp_Lg;
+    lprior.n = np;
     return priors_changed();
   }
 
@@ -1039,10 +1049,11 @@ struct Solver : rba_handle {
       }
     }
     if (any) {
-      TRY(grow_upload(!d_obs_W, dbuf(d_obs_W, w.size(), &w)));
+      DeviceBuffer<S> next; TRY(fit(next, obs.W, w.size(), &w));
       CU(cudaStreamSynchronize(stream));
+      obs.W.take(next);
     }
-    D.obs_W = any ? d_obs_W : nullptr;
+    obs.on = any;
     su_valid = s_valid = false;  // the assembled matrix belongs to the previous rows
     return priors_changed();
   }
@@ -1054,10 +1065,9 @@ struct Solver : rba_handle {
       return RBA_ERR_INVALID_ARGUMENT;
     }
     const size_t ns = (size_t)L.nslots;
-    char* base = nullptr;
-    CU(cudaMalloc(&base, ns * (3 * sizeof(S) + 1)));
-    struct Scratch1 { char* p; ~Scratch1() { cudaFree(p); } } scratch{base};
-    S* d_res = (S*)base; S* d_hw = d_res + 2 * ns; uint8_t* d_fl = (uint8_t*)(d_hw + ns);
+    DeviceBuffer<char> scratch;  // per-call
+    TRY(alloc(scratch, ns * (3 * sizeof(S) + 1), false, false));
+    S* d_res = (S*)scratch.get(); S* d_hw = d_res + 2 * ns; uint8_t* d_fl = (uint8_t*)(d_hw + ns);
     k_obs_residuals<S><<<(unsigned)((ns + 255) / 256), 256, 0, stream>>>(D, ko, d_res, d_hw, d_fl);
     std::vector<S> res(2 * ns), hw(ns);
     std::vector<uint8_t> fl(ns);
@@ -1121,17 +1131,17 @@ struct Solver : rba_handle {
     ke<<<EBLOCKS, 256, 0, stream>>>(D, ko, d_epart, d_flags);
     k_sum_partials<6><<<1, 256, 0, stream>>>(d_epart, EBLOCKS, d_red);
     launches += 2;
-    if (n_lmp > 0) {  // + this shard's landmark priors' 1/2 |L e|^2, BEFORE the sum over the shards (landmark-owned)
-      k_prior_cost<<<1, 256, 0, stream>>>(LandmarkPrior<S>{D.lms, d_lmp_lm, d_lmp_mean, d_lmp_L}, n_lmp, d_red, d_flags);
+    if (lprior.n > 0) {  // + this shard's landmark priors' 1/2 |L e|^2, BEFORE the sum over the shards (landmark-owned)
+      k_prior_cost<<<1, 256, 0, stream>>>(LandmarkPrior<S>{D.lms, lprior.lm.get(), lprior.mean.get(), lprior.L.get()}, lprior.n, d_red, d_flags);
       ++launches;
     }
     rc = allreduce_scalars(6); if (rc) return rc;
-    if (has_abs_prior) {  // + sum of 1/2 |L e|^2, once, after the sum over the shards
+    if (cprior.on) {  // + sum of 1/2 |L e|^2, once, after the sum over the shards
       k_prior_cost<<<1, 256, 0, stream>>>(camera_prior(), nc, d_red, d_flags);
       ++launches;
     }
-    if (n_pairs > 0) {  // + the pair priors' 1/2 |L e|^2, likewise
-      k_prior_cost<<<1, 256, 0, stream>>>(pair_prior(), n_pairs, d_red, d_flags);
+    if (pprior.n > 0) {  // + the pair priors' 1/2 |L e|^2, likewise
+      k_prior_cost<<<1, 256, 0, stream>>>(pair_prior(), pprior.n, d_red, d_flags);
       ++launches;
     }
     CU(cudaMemcpyAsync(h_res->error, d_red, sizeof(h_res->error), cudaMemcpyDeviceToHost, stream));
@@ -1169,6 +1179,7 @@ struct Solver : rba_handle {
   // ref: solver/linearizor_qr.cpp:78-138 (staged: LinearizationQR::get_stage1, linearization_qr.hpp:634-712)
   int linearize_enqueue() {
     lin_l0 = launches;
+    const int n_pairs = pprior.n, n_groups = grp.n;
     int rc = start(ev_stage1); if (rc) return rc;
     CU(cudaMemsetAsync(d_flags, 0, 4 * sizeof(int), stream));
     // pass A: squared column norms of the weighted pose Jacobians -> pose_jacobian_scaling_
@@ -1176,13 +1187,13 @@ struct Solver : rba_handle {
     kn<<<grid_for(L.nslots, 256, 8), 256, 0, stream>>>(D, ko, d_flags);
     ++launches;
     rc = camera_reduce(d_csr_obs_slots, d_csr_obs_items, n_obs_items, d_csr_obs_item_ptr, D.diag2); if (rc) return rc;
-    if (has_abs_prior) {  // prior Jacobian and its column norms (scaling from the whole Jacobian), after the sum over the shards
-      k_prior_linearize<S><<<(nc + 127) / 128, 128, 0, stream>>>(D.cams, d_prior_mean, d_prior_L, nc, D.diag2, d_prior_A, d_prior_r);
+    if (cprior.on) {  // prior Jacobian and its column norms (scaling from the whole Jacobian), after the sum over the shards
+      k_prior_linearize<S><<<(nc + 127) / 128, 128, 0, stream>>>(D.cams, cprior.mean.get(), cprior.L.get(), nc, D.diag2, cprior.A.get(), cprior.r.get());
       ++launches;
     }
     if (n_pairs > 0) {  // pair-prior blocks and their column norms, likewise
-      k_pair_linearize<S><<<(n_pairs + 127) / 128, 128, 0, stream>>>(D.cams, d_pair_ij, d_pair_mean, d_pair_L, n_pairs, d_pair_A, d_pair_r);
-      k_pair_diag2<S><<<(nc + 127) / 128, 128, 0, stream>>>(d_pair_A, d_pair_ptr, d_pair_item, nc, D.diag2);
+      k_pair_linearize<S><<<(n_pairs + 127) / 128, 128, 0, stream>>>(D.cams, pprior.ij.get(), pprior.mean.get(), pprior.L.get(), n_pairs, pprior.A.get(), pprior.r.get());
+      k_pair_diag2<S><<<(nc + 127) / 128, 128, 0, stream>>>(pprior.A.get(), pprior.ptr.get(), pprior.item.get(), nc, D.diag2);
       launches += 2;
     }
     if (n_groups) {  // the merged intrinsics columns' norms for every member, after the sum over the shards and the priors
@@ -1205,14 +1216,14 @@ struct Solver : rba_handle {
       rc = precond_blocks(0, D.jblocks, nullptr, true); if (rc) return rc;
     }
     const bool jac = opt.preconditioner_type == 0 || opt.solver_type == 2;
-    if (has_abs_prior) {  // scaled prior Jacobian, A^T A (+ into the JACOBI blocks), A^T r
-      k_prior_scale<S><<<(nc + 127) / 128, 128, 0, stream>>>(d_prior_A, d_prior_r, D.scaling, nc, d_prior_H, d_prior_g, jac ? D.jblocks : nullptr);
+    if (cprior.on) {  // scaled prior Jacobian, A^T A (+ into the JACOBI blocks), A^T r
+      k_prior_scale<S><<<(nc + 127) / 128, 128, 0, stream>>>(cprior.A.get(), cprior.r.get(), D.scaling, nc, cprior.H.get(), cprior.g.get(), jac ? D.jblocks : nullptr);
       ++launches;
     }
     if (n_pairs > 0) {  // scaled pair blocks; their diagonal blocks and A^T r added to the absolute priors', the O_ij of every edge
-      k_pair_scale<S><<<(n_pairs + 127) / 128, 128, 0, stream>>>(d_pair_A, d_pair_ij, D.scaling, n_pairs);
-      k_pair_accum<S><<<(nc + 127) / 128, 128, 0, stream>>>(d_pair_A, d_pair_r, d_pair_ptr, d_pair_item, nc, (int)has_abs_prior,
-                                                            d_prior_H, d_prior_g, jac ? D.jblocks : nullptr, d_pair_O);
+      k_pair_scale<S><<<(n_pairs + 127) / 128, 128, 0, stream>>>(pprior.A.get(), pprior.ij.get(), D.scaling, n_pairs);
+      k_pair_accum<S><<<(nc + 127) / 128, 128, 0, stream>>>(pprior.A.get(), pprior.r.get(), pprior.ptr.get(), pprior.item.get(), nc, (int)cprior.on,
+                                                            cprior.H.get(), cprior.g.get(), jac ? D.jblocks : nullptr, pprior.O.get());
       launches += 2;
     }
     if (panel_form()) {
@@ -1285,7 +1296,7 @@ struct Solver : rba_handle {
   // so it must exist as one vector: Partials and Peer, which sum the segments inside k_pcg_vec, give way to Counter / Nccl.
   Handover handover() const {
     if (s_valid) return Handover::Assembled;
-    if (n_groups) return opt.nranks > 1 ? Handover::Nccl : Handover::Counter;
+    if (grp.n) return opt.nranks > 1 ? Handover::Nccl : Handover::Counter;
     if (opt.nranks > 1) return peer_ok ? Handover::Peer : Handover::Nccl;
     const bool vec_cached = 9 * ((nc + pcg_cluster - 1) / pcg_cluster) <= VEC_THREADS * VEC_EPT;
     return pcg_partials && vec_cached && opt.solver_type != 2 ? Handover::Partials : Handover::Counter;
@@ -1340,8 +1351,8 @@ struct Solver : rba_handle {
     PeerComm c = pc;
     if (!fused_ar) c.nranks = 1;
     DevPtrs<S> Dv = D;
-    if (n_groups) {  // the contracted output, which holds the prior terms already (k_group_contract)
-      Dv.y = d_grp_y; Dv.prior_H = nullptr; Dv.pair_ov = nullptr;
+    if (grp.n) {  // the contracted output, which holds the prior terms already (k_group_contract)
+      Dv.y = grp.y.get(); Dv.prior_H = nullptr; Dv.pair_ov = nullptr;
     }
     if (Dv.pair_ov && mode != 3) TRY(pair_ov(mode == 2 ? D.x : D.p, pdl));
     auto kern = Dv.pair_ov ? k_pcg_vec<S, true, true> : Dv.prior_H ? k_pcg_vec<S, true> : k_pcg_vec<S, false>;
@@ -1353,17 +1364,17 @@ struct Solver : rba_handle {
     return launch_ex(k_pair_ov<S>, (9 * nc + 255) / 256, 256, 0, pdl, 1, D, (const PcgState*)d_state, v);
   }
   // one operator application inside PCG (H v for v = p in mode 0/1, x in mode 2) and the vector step after it
-  // (intrinsics groups: H_u v = P^T H P v, with P v in d_grp_ve and P^T (H P v) in d_grp_y)
+  // (intrinsics groups: H_u v = P^T H P v, with P v in grp.ve and P^T (H P v) in grp.y)
   int pcg_step(int i, int mode, int is_last, S lambda, Handover h) {
     const S* v = mode == 2 ? D.x : D.p;
-    if (n_groups) {
-      TRY(group_expand(v, d_grp_ve, true));
-      v = d_grp_ve;
+    if (grp.n) {
+      TRY(group_expand(v, grp.ve.get(), true));
+      v = grp.ve.get();
     }
     TRY(apply_operator(v, h, true));
-    if (n_groups)
-      TRY(launch_ex(k_group_contract<S>, (nc + GROUP_THREADS - 1) / GROUP_THREADS + n_groups, GROUP_THREADS, 0, h != Handover::Nccl, 1,
-                    D, (const S*)d_grp_ve, d_grp_y, groups(), (nc + GROUP_THREADS - 1) / GROUP_THREADS, (const PcgState*)d_state));
+    if (grp.n)
+      TRY(launch_ex(k_group_contract<S>, (nc + GROUP_THREADS - 1) / GROUP_THREADS + grp.n, GROUP_THREADS, 0, h != Handover::Nccl, 1,
+                    D, (const S*)grp.ve.get(), grp.y.get(), groups(), (nc + GROUP_THREADS - 1) / GROUP_THREADS, (const PcgState*)d_state));
     return pcg_vec(i, mode, h != Handover::Nccl, is_last, lambda, h == Handover::Peer, h == Handover::Partials);
   }
   // Enqueue iterations 1..last in chunks of `chunk` (enqueue(i)); after each chunk the PcgState is copied into one of two
@@ -1442,24 +1453,24 @@ struct Solver : rba_handle {
     // pose damping lambda*I added to the blocks, then explicit inverse (ref: linearization_qr.hpp:796-802, linearizor_qr.cpp:228-237)
     // (+ the masking of the held camera parameters, D.cam_fixed; + the camera priors: A^T A into the SCHUR_JACOBI blocks -- the
     // JACOBI blocks hold it already -- and A^T r into b, both after the sum over the shards and before the masking)
-    if (n_groups) {
+    if (grp.n) {
       // (intrinsics groups: the priors' terms, the contraction of b and the merged blocks first, into D.blocks; DESIGN.md
       // section 18)
-      const int ncb = (nc + GROUP_THREADS - 1) / GROUP_THREADS;
+      const int ncb = (nc + GROUP_THREADS - 1) / GROUP_THREADS, n_groups = grp.n;
       k_group_precond<S><<<ncb + n_groups, GROUP_THREADS, 0, stream>>>(schur ? D.blocks : D.jblocks, schur ? (const S*)D.prior_H : nullptr,
-                                                                       D.prior_H ? (const S*)d_prior_g : nullptr, D.b, D.blocks, groups(), nc, ncb);
-      k_precond_invert<S><<<(nc + 63) / 64, 64, 0, stream>>>(D.blocks, lambda, nc, schur ? D.blocks : nullptr, D.inv, d_grp_fixed, D.b);
+                                                                       D.prior_H ? (const S*)cprior.g.get() : nullptr, D.b, D.blocks, groups(), nc, ncb);
+      k_precond_invert<S><<<(nc + 63) / 64, 64, 0, stream>>>(D.blocks, lambda, nc, schur ? D.blocks : nullptr, D.inv, grp.fixed.get(), D.b);
       launches += 2;
     } else {
       k_precond_invert<S><<<(nc + 63) / 64, 64, 0, stream>>>(schur ? D.blocks : D.jblocks, lambda, nc, schur ? D.blocks : nullptr, D.inv,
                                                              D.cam_fixed, D.b, schur ? (const S*)D.prior_H : nullptr,
-                                                             D.prior_H ? (const S*)d_prior_g : nullptr);
+                                                             D.prior_H ? (const S*)cprior.g.get() : nullptr);
       ++launches;
     }
     rc = stop(ev_precond); if (rc) return rc;
     last_lambda = lambda;
     damping_valid = true;
-    if (all_cams_fixed) {
+    if (held.all) {
       // no free camera parameter: inc = 0 without PCG / power series (whose stopping tests would divide 0 by 0); stage 2
       // above still ran for the damped landmark factors of the back-substitution.  Every rank skips alike.
       rc = start(ev_pcg); if (rc) return rc;
@@ -1527,7 +1538,7 @@ struct Solver : rba_handle {
         rc = enqueue_iteration(i); if (rc) return rc;
       }
     }
-    if (n_groups) TRY(group_expand(D.inc, D.inc, false));  // inc = P u for the back-substitution, the update and inc_out
+    if (grp.n) TRY(group_expand(D.inc, D.inc, false));  // inc = P u for the back-substitution, the update and inc_out
     CU(cudaMemcpyAsync(&h_state[0], d_state, sizeof(PcgState), cudaMemcpyDeviceToHost, stream));
     if (inc_out) CU(cudaMemcpyAsync(inc_out, D.inc, (size_t)9 * nc * sizeof(S), cudaMemcpyDeviceToHost, stream));
     rc = stop(ev_pcg); if (rc) return rc;
@@ -1576,7 +1587,7 @@ struct Solver : rba_handle {
         k_mask_fixed_inc<S><<<(9 * nc + 255) / 256, 256, 0, stream>>>(D.inc, D.cam_fixed, nc);
         ++launches;
       }
-      if (n_groups) TRY(group_expand(D.inc, D.inc, false));  // the members take the lead's f, k1, k2 entries
+      if (grp.n) TRY(group_expand(D.inc, D.inc, false));  // the members take the lead's f, k1, k2 entries
     } else if (!have_inc) { g_err = "no device-resident increment (none solved since rba_linearize or rba_set_camera_fixed)"; return RBA_ERR_STATE; }
     int rc = start(ev_backsub); if (rc) return rc;
     CU(cudaMemsetAsync(d_flags, 0, 4 * sizeof(int), stream));
@@ -1586,12 +1597,12 @@ struct Solver : rba_handle {
     k_sum_partials<1><<<1, 256, 0, stream>>>(d_epart, grid, d_red);
     launches += 2;
     rc = allreduce_scalars(1); if (rc) return rc;
-    if (has_abs_prior) {  // the prior part of the model cost change, once, after the sum over the shards
+    if (cprior.on) {  // the prior part of the model cost change, once, after the sum over the shards
       k_prior_ldiff<<<1, 256, 0, stream>>>(camera_prior(), D.inc, nc, d_red);
       ++launches;
     }
-    if (n_pairs > 0) {  // the pair priors' part, likewise
-      k_prior_ldiff<<<1, 256, 0, stream>>>(pair_prior(), D.inc, n_pairs, d_red);
+    if (pprior.n > 0) {  // the pair priors' part, likewise
+      k_prior_ldiff<<<1, 256, 0, stream>>>(pair_prior(), D.inc, pprior.n, d_red);
       ++launches;
     }
     rc = stop(ev_backsub); if (rc) return rc;
@@ -1868,27 +1879,17 @@ struct Solver : rba_handle {
   // ------------------------------------------------------------------------------------------
   // Marginal covariances (DESIGN.md section 16).  Nothing of the handle changes: the scratch is allocated for the call and
   // freed before it returns; the state, the linearisation, the increment, the error cache and the timings are not touched.
-  // The term lists built at the first call stay on the handle (not counted in device_bytes).
-  template <class T>
-  int cov_upload(T** p, const std::vector<T>& v) {
-    void* q = nullptr;
-    CU(cudaMalloc(&q, std::max<size_t>(v.size(), 1) * sizeof(T)));
-    allocs.push_back(q);
-    if (!v.empty()) CU(cudaMemcpy(q, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice));
-    *p = (T*)q;
-    return RBA_OK;
-  }
-  // The term lists of rba_compute_covariance (build_pair_list), built at the first call.
+  // The term lists (build_pair_list) built at the first call stay on the handle (not counted in device_bytes).
   int cov_build_lists() {
     if (cov_ready) return RBA_OK;
     PairList P;
     const std::string msg = build_pair_list(L, P);
     if (!msg.empty()) { g_err = msg; return RBA_ERR_UNSUPPORTED; }
-    TRY(cov_upload(&d_cov_blk_cam, P.blk_cam));
-    TRY(cov_upload(&d_cov_blk_ptr, P.blk_ptr));
-    TRY(cov_upload(&d_cov_terms, P.terms));
-    TRY(cov_upload(&d_cov_lm_slot0, P.slot0));
-    TRY(cov_upload(&d_cov_lm_n, P.nn));
+    TRY(upload(&d_cov_blk_cam, P.blk_cam, false));
+    TRY(upload(&d_cov_blk_ptr, P.blk_ptr, false));
+    TRY(upload(&d_cov_terms, P.terms, false));
+    TRY(upload(&d_cov_lm_slot0, P.slot0, false));
+    TRY(upload(&d_cov_lm_n, P.nn, false));
     cov_nblk = (int)P.blk_cam.size();
     cov_ready = true;
     return RBA_OK;
@@ -1915,8 +1916,7 @@ struct Solver : rba_handle {
   // The dense inverse of one covariance call and what its extraction kernels read; the scratch is freed (after the kernels
   // have finished: cudaFree waits for them) when it goes out of scope.
   struct CovInverse {
-    char* base = nullptr;
-    ~CovInverse() { cudaFree(base); }
+    DeviceBuffer<char> scratch;
     double* A = nullptr;  // S_eq^-1 (lower triangle, leading dimension np); cov_sinv reads D S_eq^-1 D from it
     double* d = nullptr;  // the diagonal of D
     double* kb = nullptr; double* wl = nullptr; int* rk = nullptr;  // K per slot, W and rank per landmark
@@ -1933,7 +1933,7 @@ struct Solver : rba_handle {
     TRY(cov_build_lists());
     constexpr long long TB = COV_TB;
     const long long n = 9LL * nc, np = (n + TB - 1) / TB * TB, ns = L.nslots;
-    const int nl = L.nl_local, nt = (int)(np / TB);
+    const int nl = L.nl_local, nt = (int)(np / TB), n_lmp = lprior.n;
     size_t total = 0;
     auto carve = [&](size_t bytes) { const size_t o = total; total += (bytes + 255) & ~size_t(255); return o; };
     const size_t o_A = carve((size_t)(np * np) * 8), o_W = carve((size_t)(np * TB) * 8), o_Y = carve((size_t)(np * TB) * 8),
@@ -1948,9 +1948,8 @@ struct Solver : rba_handle {
               std::to_string(n) + " float64 reduced camera matrix plus scratch); " + std::to_string(free_b) + " bytes are free";
       return RBA_ERR_UNSUPPORTED;
     }
-    char* base = nullptr;
-    CU(cudaMalloc(&base, total));
-    c.base = base;
+    TRY(alloc(c.scratch, total, false, false));
+    char* base = c.scratch.get();
     double* A = (double*)(base + o_A); double* W = (double*)(base + o_W); double* Y = (double*)(base + o_Y);
     double* Tt = (double*)(base + o_T); double* d = (double*)(base + o_d); double* jp = (double*)(base + o_jp);
     double* kb = (double*)(base + o_kb); double* wl = (double*)(base + o_wl); int* rk = (int*)(base + o_rk);
@@ -1965,18 +1964,18 @@ struct Solver : rba_handle {
     // LMP: + L^T L of the landmark priors in Hll; OBSW: the rows whitened by the observation information
     auto kcov = n_lmp > 0 ? (D.obs_W ? k_cov_landmark<S, true, true> : k_cov_landmark<S, true>)
                           : (D.obs_W ? k_cov_landmark<S, false, true> : k_cov_landmark<S>);
-    kcov<<<wgrid, 128, 0, stream>>>(D, ko, d_cov_lm_slot0, d_cov_lm_n, nl, jp, kb, wl, rk, n_lmp > 0 ? d_lmp_of_lm : nullptr);
+    kcov<<<wgrid, 128, 0, stream>>>(D, ko, d_cov_lm_slot0, d_cov_lm_n, nl, jp, kb, wl, rk, n_lmp > 0 ? lprior.of_lm.get() : nullptr);
     k_cov_assemble<<<std::max(1, std::min((cov_nblk + 7) / 8, sm_count * 8)), 256, 0, stream>>>(
         (const int2*)d_cov_blk_cam, d_cov_blk_ptr, (const int2*)d_cov_terms, cov_nblk, jp, kb, A, np);
-    if (has_abs_prior || n_pairs > 0)
-      k_cov_priors<S><<<(nc + 127) / 128, 128, 0, stream>>>(D.cams, nc, has_abs_prior ? d_prior_mean : nullptr, d_prior_L, d_pair_ij,
-                                                            d_pair_mean, d_pair_L, n_pairs > 0 ? d_pair_ptr : nullptr, d_pair_item,
-                                                            d_pair_nbr, A, np);
+    if (cprior.on || pprior.n > 0)
+      k_cov_priors<S><<<(nc + 127) / 128, 128, 0, stream>>>(D.cams, nc, cprior.on ? cprior.mean.get() : nullptr, cprior.L.get(), pprior.ij.get(),
+                                                            pprior.mean.get(), pprior.L.get(), pprior.n > 0 ? pprior.ptr.get() : nullptr, pprior.item.get(),
+                                                            pprior.nbr.get(), A, np);
     // intrinsics groups (DESIGN.md section 18): S_u = P^T S P, the members' entries 6..8 then held like the user's
     const uint8_t* held = D.cam_fixed;
-    if (n_groups) {
+    if (grp.n) {
       TRY(cov_group_passes(A, np, n, 0));
-      held = d_grp_fixed;
+      held = grp.fixed.get();
     }
     k_cov_diag<<<(unsigned)((np + 255) / 256), 256, 0, stream>>>(A, np, n, np, held, d);
     k_cov_equil<<<dim3((unsigned)(np / 32), (unsigned)(np / 8)), dim3(32, 8), 0, stream>>>(A, np, n, np, held, d);
@@ -2026,7 +2025,7 @@ struct Solver : rba_handle {
       if (kk > 0) cov_gemm<true, false>(TB, r0 + TB, kk, 1.0, A + (r0 + TB) + r0 * np, np, A + (r0 + TB), np, 1.0, A + r0, np, 0, 0);
     }
     // (intrinsics groups: P S_u^-1 P^T, the members' rows and columns 6..8 and equilibration those of the lead)
-    if (n_groups) {
+    if (grp.n) {
       TRY(cov_group_passes(A, np, n, 1));
       k_cov_group_d<<<1, 1, 0, stream>>>(d, groups());
     }
