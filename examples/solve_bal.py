@@ -4,7 +4,8 @@
     python examples/solve_bal.py problem-49-7776-pre.txt [--float] [--max-num-iterations 20] [--operator-form DENSE|IMPLICIT]
         [--fix-intrinsics] [--fix-cameras I,J,...] [--camera-prior FILE.npz] [--camera-pair-prior FILE.npz]
         [--landmark-prior FILE.npz] [--shared-intrinsics | --intrinsics-groups FILE.npy] [--covariance OUT.npz]
-        [--relative-covariance PAIRS.npy] [--observation-info FILE.npy] [--residuals OUT.npz]
+        [--relative-covariance PAIRS.npy] [--observation-info FILE.npy] [--observation-loss KIND:SCALE | FILE.npz]
+        [--residuals OUT.npz]
 
 Mirrors what `bal_qr --input ...` of the reference does (src/app/bal_qr.cpp): load + normalise (bal_problem.cpp:773-852),
 optimize_lm_ours with the QR linearizor (solver/bal_bundle_adjustment.cpp:249-544), log (bal/ba_log.hpp)."""
@@ -61,6 +62,11 @@ def main():
                          "(a square root W of the inverse 2x2 keypoint covariance) in the order of the loaded problem's "
                          "observations, in the units of the loaded (normalised) image coordinates; zero switches an observation "
                          "off (DESIGN.md section 19)")
+    ap.add_argument("--observation-loss", default=None, metavar="KIND:SCALE | FILE.npz",
+                    help="a robust loss per observation (DESIGN.md section 21): KIND:SCALE for every observation (KIND one of "
+                         "NONE, HUBER, CAUCHY, SOFT_L1, TUKEY; SCALE the inlier threshold in units of sigma), or a .npz with the "
+                         "arrays `kind` [Nobs] (names or RBA_LOSS_* ints) and `scale` [Nobs] in the order of the loaded problem's "
+                         "observations")
     ap.add_argument("--residuals", default=None, metavar="OUT.npz",
                     help="after the solve, write per observation `residual` [Nobs, 2] (W r), `robust_weight` [Nobs] and `flags` "
                          "[Nobs] (bit 0 = projection valid, bit 1 = in use) at the final state (DESIGN.md section 19)")
@@ -132,6 +138,20 @@ def main():
             problem.observation_sqrt_info = info
         except ValueError as e:
             ap.error(f"--observation-info: {e}")
+    if args.observation_loss:
+        try:
+            if args.observation_loss.endswith(".npz"):
+                with np.load(args.observation_loss) as f:
+                    if "kind" not in f or "scale" not in f:
+                        ap.error(f"--observation-loss: {args.observation_loss} must hold the arrays `kind` and `scale`")
+                    problem.observation_loss = (f["kind"], f["scale"])
+            else:
+                kind, sep, scale = args.observation_loss.partition(":")
+                if not sep:
+                    ap.error("--observation-loss: expected KIND:SCALE (e.g. CAUCHY:2) or FILE.npz")
+                problem.observation_loss = (kind, float(scale))
+        except ValueError as e:
+            ap.error(f"--observation-loss: {e}")
     options = rb.SolverOptions(max_num_iterations=args.max_num_iterations, preconditioner_type=args.preconditioner_type,
                                operator_form=args.operator_form, use_double=not args.float)
     summary = rb.bundle_adjust_manual(problem, options, verbose=True)

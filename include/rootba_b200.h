@@ -352,18 +352,56 @@ int32_t rba_set_observation_info(rba_handle* h, const void* sqrt_info);
 
 /* Per observation at the handle's CURRENT state, in problem order; any pointer may be NULL (all NULL ->
  * RBA_ERR_INVALID_ARGUMENT).  residual [2*Nobs] Scalar: the whitened residual W r (the raw r without observation
- * info); robust_weight [Nobs] Scalar: hw of error_weight on |W r|^2 (1 with robust_norm NONE); flags [Nobs] uint8:
+ * info); robust_weight [Nobs] Scalar: the robust weight w on |W r|^2 of the observation's own loss (rba_set_observation_loss;
+ * without one the handle's robust norm, 1 with robust_norm NONE); flags [Nobs] uint8:
  * bit 0 = projection valid (z >= eps_sqrt), bit 1 = in use (W != 0).  A sharded handle writes only the observations of
  * its own landmark shard.  Needs no rba_linearize; changes nothing of the handle (scratch device memory is allocated for the
  * call and freed before it returns). */
 int32_t rba_get_observation_residuals(rba_handle* h, void* residual, void* robust_weight, uint8_t* flags);
+
+/* ---- Robust loss per observation (DESIGN.md section 21) ------------------------------------- */
+
+#define RBA_LOSS_NONE    0
+#define RBA_LOSS_HUBER   1
+#define RBA_LOSS_CAUCHY  2
+#define RBA_LOSS_SOFT_L1 3
+#define RBA_LOSS_TUKEY   4
+
+/* Not in the reference, where one robust norm (robust_norm, huber_parameter) applies to every observation.  Observation o
+ * (index in the problem's CSR order) gets its own loss kind[o] with the scale a = scale[o], the inlier threshold in units of
+ * sigma.  With s = |W r|^2 (W of rba_set_observation_info, or the identity) its cost is rho(s)/2, its robust weight
+ * w = rho'(s) and its rows sqrt(w) W [Jp | Jl | r] (IRLS weighting as for Huber, no second-order correction):
+ *   RBA_LOSS_NONE     rho = s                                                       w = 1           (scale ignored)
+ *   RBA_LOSS_HUBER    rho = s if s < a^2, else 2 a sqrt(s) - a^2                    w = 1, else a / sqrt(s)
+ *   RBA_LOSS_CAUCHY   rho = a^2 log1p(s / a^2)                                      w = 1 / (1 + s / a^2)
+ *   RBA_LOSS_SOFT_L1  rho = 2 a^2 (sqrt(1 + s / a^2) - 1)                           w = 1 / sqrt(1 + s / a^2)
+ *   RBA_LOSS_TUKEY    rho = (a^2 / 3) (1 - (1 - u)^3), u = s / a^2 < 1; else a^2/3  w = (1 - u)^2, else 0
+ * Every rho has rho(s) ~ s and w -> 1 as s -> 0.  HUBER is exactly the handle's Huber norm; HUBER, CAUCHY and SOFT_L1 are
+ * scipy.optimize.least_squares' losses with f_scale = a, and TUKEY is twice Ceres' TukeyLoss.
+ * kind [Nobs] uint8 and scale [Nobs] Scalar of the full problem in problem order; both NULL = every observation uses the
+ * handle's robust_norm / huber_parameter, the default.  Every rank of a sharded problem passes the same full arrays and keeps
+ * the entries of its own landmark shard.  Arrays equal to the handle's own choice on every observation of the shard
+ * ((RBA_LOSS_HUBER, (Scalar)huber_parameter) with robust_norm = 1, else RBA_LOSS_NONE) are the same as NULL: the unmodified
+ * kernels run, bit for bit.  rba_solver_opts is unchanged.
+ * A TUKEY observation beyond its scale (w = 0) has all-zero rows like a dropped projection, but still counts as valid in
+ * rba_compute_error and adds a^2/6 to all_error / valid_error.  A switched-off observation (W = 0) stays off whatever its
+ * loss.  A non-finite residual fails rba_linearize and clears is_numerically_valid as before, whatever the loss.
+ * rba_get_observation_residuals returns each observation's own w; rba_compute_covariance and rba_compute_covariance_blocks
+ * use it.  After a successful call rba_solve returns RBA_ERR_STATE until the next rba_linearize; the device-resident
+ * increment and the cached error are discarded.
+ * RBA_ERR_INVALID_ARGUMENT, with the previous losses kept in force: exactly one pointer NULL, a kind above RBA_LOSS_TUKEY, or
+ * a kind other than RBA_LOSS_NONE with a scale that is not finite or <= 0.
+ * The losses cost 8 bytes (float) or 9 bytes (double) per observation slot of device memory, counted in
+ * rba_workload_stats::device_bytes from the first call that sets a loss other than the handle's own. */
+int32_t rba_set_observation_loss(rba_handle* h, const uint8_t* kind, const void* scale);
 
 /* ---- Marginal covariances (DESIGN.md section 16) ------------------------------------------ */
 
 /* Not in the reference.  DESIGN.md section 16.  The covariance of the Gauss-Newton step of the total objective (reprojection
  * terms + camera priors + pair priors) at lambda = 0 and the handle's current state: the inverse of H = J^T J, with J the rows
  * rba_linearize would build (whitened by the observation information of rba_set_observation_info when it is set, sqrt(w)-weighted
- * by the robust norm, the rows use_valid_projections_only drops set to zero), and
+ * by each observation's robust weight -- its own loss of rba_set_observation_loss, else the handle's robust norm -- the rows
+ * use_valid_projections_only drops set to zero), and
  * the parameters held by rba_set_camera_fixed as constants (their rows and columns are exactly 0).  Evaluated in float64 for
  * either Scalar; unscaled (no Jacobi scaling); independent of solver_type, operator_form, stage2_form, preconditioner_type and
  * the QR variant (bit-identical output within one Scalar).
@@ -382,7 +420,7 @@ int32_t rba_compute_covariance(rba_handle* h, double* cam_cov, double* lm_cov);
 /* ---- Covariance blocks (DESIGN.md section 20) ------------------------------------------------ */
 
 /* Not in the reference.  DESIGN.md section 20.  Blocks of the same covariance H^-1 as rba_compute_covariance (same H, held
- * parameters, intrinsics groups, priors, observation information, robust weights and validity; float64 for either Scalar;
+ * parameters, intrinsics groups, priors, observation information, per-observation robust weights and validity; float64 for either Scalar;
  * increments (tx,ty,tz, rx,ry,rz, f,k1,k2) per camera and (x,y,z) per landmark in problem order), for chosen pairs, from one
  * factorisation.  Output k belongs to request k; repeated requests and any order are allowed.
  *   camera_cross [81*k]: Cov(d_a, d_b), 9x9 row-major, rows of camera a; (a, a) is bit-identical to cam_cov[a], (b, a) is the

@@ -26,6 +26,14 @@ FIX_K2 = 8          # entry 8
 FIX_INTRINSICS = FIX_F | FIX_K1 | FIX_K2
 FIX_ALL = FIX_POSE | FIX_INTRINSICS
 
+# robust loss kinds per observation (RBA_LOSS_*, rba_set_observation_loss)
+LOSS_NONE = 0
+LOSS_HUBER = 1
+LOSS_CAUCHY = 2
+LOSS_SOFT_L1 = 3
+LOSS_TUKEY = 4
+LOSS_KINDS = {"NONE": LOSS_NONE, "HUBER": LOSS_HUBER, "CAUCHY": LOSS_CAUCHY, "SOFT_L1": LOSS_SOFT_L1, "TUKEY": LOSS_TUKEY}
+
 
 class RbaError(RuntimeError):
     def __init__(self, code: int, msg: str):
@@ -140,6 +148,7 @@ def lib():
         _lib.rba_compute_covariance.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
         _lib.rba_compute_covariance_blocks.argtypes = [C.c_void_p, C.POINTER(CovarianceQuery)]
         _lib.rba_set_landmark_prior.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
+        _lib.rba_set_observation_loss.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
     return _lib
 
 

@@ -73,7 +73,8 @@ __device__ __forceinline__ void cov_sym3_eig(double (&A)[9], double (&V)[9]) {
 // LMP (landmark priors, DESIGN.md section 17): Hll += L^T L (unscaled, in double) for a landmark with prior slot
 // lmp_of_lm[lm] >= 0, so a landmark with fewer than 2 valid observations can be full rank.
 // OBSW (observation information, DESIGN.md section 19): the rows are whitened in double, sqrt(w) W [Jp | Jl], w from |W r|^2.
-template <class S, bool LMP = false, bool OBSW = false>
+// OBSL (observation losses, DESIGN.md section 21): w from the slot's own loss, evaluated in double.
+template <class S, bool LMP = false, bool OBSW = false, bool OBSL = false>
 __global__ void __launch_bounds__(128) k_cov_landmark(DevPtrs<S> D, KOpts o, const int* __restrict__ lm_slot0,
                                                       const int* __restrict__ lm_n, int nl, double* __restrict__ jpw,
                                                       double* __restrict__ kb, double* __restrict__ wl, int* __restrict__ rank,
@@ -104,7 +105,7 @@ __global__ void __launch_bounds__(128) k_cov_landmark(DevPtrs<S> D, KOpts o, con
       double sw = 0.0;
       if (keep) {
         double err, w;
-        error_weight(o, res[0] * res[0] + res[1] * res[1], err, w);
+        slot_error_weight<OBSL>(o, D.obs_loss, D.nslots, s, res[0] * res[0] + res[1] * res[1], err, w);
         sw = sqrt(w);
       }
 #pragma unroll

@@ -106,6 +106,9 @@ struct DevPtrs {
   // observation information (rba_set_observation_info, DESIGN.md section 19); nullptr = none (identity everywhere) in this
   // shard.  Only the kernels' OBSW instances, k_obs_residuals and k_cov_landmark read it.
   const S* obs_W;            // [nslots][4] row-major 2x2 square-root information W of each slot (padding slots zero)
+  // robust loss per observation (rba_set_observation_loss, DESIGN.md section 21); nullptr = the handle's robust_norm on every
+  // observation of this shard.  Only the kernels' OBSL instances, k_obs_residuals and k_cov_landmark read it (slot_loss).
+  const S* obs_loss;         // float: [nslots] {scale, uint32 kind}; double: [nslots] scale, then [nslots] uint8 kind (padding NONE)
 };
 
 // increment entries (tx,ty,tz, rx,ry,rz, f,k1,k2) held by a camera's RBA_FIX_* bits, as a 9-bit mask
@@ -218,6 +221,70 @@ __device__ __forceinline__ bool whiten_observation(const SW* __restrict__ obs_W,
   return off;
 }
 
+// Robust loss of one observation (DESIGN.md section 21), kind = RBA_LOSS_* (0 NONE, 1 HUBER, 2 CAUCHY, 3 SOFT_L1, 4 TUKEY),
+// a the scale (inlier threshold in units of sigma), s = |W r|^2, u = s / a^2.  err = rho(s) / 2 and w = rho'(s), each rho
+// normalised to rho(s) ~ s, w -> 1 as s -> 0.  Any other kind is NONE.
+//   HUBER    w = 1 if s < a^2, else a / sqrt(s); err = 1/2 (2 - w) w s: error_weight's arithmetic with th = a
+//   CAUCHY   rho = a^2 log1p(u);  w = 1 / (1 + u) = a^2 / (a^2 + s)
+//   SOFT_L1  rho = 2 a^2 (sqrt(1 + u) - 1) = 2 s / (sqrt(1 + u) + 1);  w = 1 / sqrt(1 + u) = a / sqrt(a^2 + s)
+//   TUKEY    rho = (a^2 / 3) (1 - (1 - u)^3) = (a^2 / 3) u (3 - 3u + u^2) for u < 1, else a^2 / 3;  w = (1 - u)^2, else 0,
+//            1 - u = (a^2 - s) / a^2
+// w of every kind takes one square root and one division, like error_weight (each correctly rounded, so HUBER gives
+// error_weight's values bit for bit): the float32 Householder linearisation has no registers for more.  The divisions of
+// err are dead code in the kernels that need w only.
+template <class S>
+__device__ __forceinline__ void observation_loss(unsigned kind, S a, S s, S& err, S& w) {
+  const S a2 = a * a;
+  const bool hub = kind == 1, cau = kind == 2, tuk = kind == 4;
+  const S t = sqrt(hub ? s : a2 + s);                                           // HUBER sqrt(s), SOFT_L1 sqrt(a^2 + s)
+  const S q = (cau ? a2 : tuk ? a2 - s : a) / (cau ? a2 + s : tuk ? a2 : t);  // w of HUBER beyond a, CAUCHY, SOFT_L1; 1 - u of TUKEY
+  if (hub) {
+    w = s < a2 ? S(1) : q;
+    err = S(0.5) * (S(2) - w) * w * s;
+  } else if (cau) {
+    w = q;
+    err = S(0.5) * a2 * log1p(s / a2);
+  } else if (kind == 3) {
+    w = q;
+    err = a * s / (t + a);  // s / (sqrt(1 + u) + 1)
+  } else if (tuk) {
+    const S u = s / a2, c = a2 * S(1.0 / 6.0);
+    w = s < a2 ? q * q : S(0);
+    err = s < a2 ? c * (u * (S(3) - S(3) * u + u * u)) : c;
+  } else {
+    w = S(1);
+    err = S(0.5) * s;
+  }
+}
+
+// The loss of a slot from the records of rba_set_observation_loss: float one 8-byte {scale, uint32 kind} per slot (one load),
+// double the scales [nslots] followed by one uint8 kind per slot.
+template <class SL>
+__device__ __forceinline__ void slot_loss(const SL* __restrict__ loss, int nslots, size_t slot, unsigned& kind, SL& a) {
+  if constexpr (sizeof(SL) == 4) {
+    const uint2 v = *reinterpret_cast<const uint2*>(loss + 2 * slot);
+    a = __uint_as_float(v.x);
+    kind = v.y;
+  } else {
+    a = loss[slot];
+    kind = reinterpret_cast<const uint8_t*>(loss + nslots)[slot];
+  }
+}
+
+// err and w of a slot at s = |W r|^2: OBSL the slot's own loss (evaluated in S), else the handle's (error_weight)
+template <bool OBSL, class S, class SL>
+__device__ __forceinline__ void slot_error_weight(const KOpts& o, const SL* __restrict__ loss, int nslots, size_t slot, S s,
+                                                  S& err, S& w) {
+  if constexpr (OBSL) {
+    unsigned kind;
+    SL a;
+    slot_loss(loss, nslots, slot, kind, a);
+    observation_loss<S>(kind, (S)a, s, err, w);
+  } else {
+    error_weight(o, s, err, w);
+  }
+}
+
 template <class T>
 __device__ __forceinline__ T group_sum(T v, int G) {
   for (int o = G >> 1; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
@@ -280,8 +347,9 @@ __device__ __forceinline__ double block_sum_partials(const double* part, int n, 
 //     thread per observation slot; accumulation in double; out partials [gridDim][6]
 //     OBSW (observation information, DESIGN.md section 19): the residual is W r; a switched-off observation (W == 0) counts
 //     in "all" only and its projection is not checked for finiteness.
+//     OBSL (observation losses, DESIGN.md section 21): err from the slot's own loss (observation_loss) instead of error_weight.
 // ------------------------------------------------------------------------------------------------
-template <class S, bool OBSW = false>
+template <class S, bool OBSW = false, bool OBSL = false>
 __global__ void __launch_bounds__(256) k_error(DevPtrs<S> D, KOpts o, double* partials, int* bad_flag) {
   double acc[6] = {0, 0, 0, 0, 0, 0};  // all: n, err, res ; valid: n, err, res
   bool bad = false;
@@ -300,7 +368,7 @@ __global__ void __launch_bounds__(256) k_error(DevPtrs<S> D, KOpts o, double* pa
     if (!(finite_s(res[0]) && finite_s(res[1]))) bad = true;
     const S rsq = res[0] * res[0] + res[1] * res[1];
     S err, w;
-    error_weight(o, rsq, err, w);
+    slot_error_weight<OBSL>(o, D.obs_loss, D.nslots, s, rsq, err, w);
     const double rn = (double)sqrt(rsq);
     acc[0] += 1.0; acc[1] += (double)err; acc[2] += rn;
     // ref: with the validity check enabled linearize_point returns false for invalid projections and they
@@ -312,8 +380,8 @@ __global__ void __launch_bounds__(256) k_error(DevPtrs<S> D, KOpts o, double* pa
 }
 
 // rba_get_observation_residuals: k_error per slot without the reduction.  res [nslots][2] = W r (r without observation
-// information), hw [nslots] = the robust weight of error_weight on |W r|^2, flags [nslots]: bit 0 = projection valid,
-// bit 1 = in use (W != 0).  Padding slots are not written.
+// information), hw [nslots] = the robust weight on |W r|^2 (the slot's own loss while D.obs_loss is set, else error_weight),
+// flags [nslots]: bit 0 = projection valid, bit 1 = in use (W != 0).  Padding slots are not written.
 template <class S>
 __global__ void __launch_bounds__(256) k_obs_residuals(DevPtrs<S> D, KOpts o, S* __restrict__ res_out, S* __restrict__ hw_out,
                                                        uint8_t* __restrict__ flags_out) {
@@ -331,7 +399,8 @@ __global__ void __launch_bounds__(256) k_obs_residuals(DevPtrs<S> D, KOpts o, S*
   const bool pv = linearize_point<S, false>(obs, pw, cam, res, nullptr, nullptr);
   const bool off = D.obs_W && whiten_observation<S, false>(D.obs_W, s, res, nullptr, nullptr);
   S err, w;
-  error_weight(o, res[0] * res[0] + res[1] * res[1], err, w);
+  if (D.obs_loss) slot_error_weight<true>(o, D.obs_loss, D.nslots, s, res[0] * res[0] + res[1] * res[1], err, w);
+  else error_weight(o, res[0] * res[0] + res[1] * res[1], err, w);
   res_out[2 * (size_t)s] = res[0];
   res_out[2 * (size_t)s + 1] = res[1];
   hw_out[s] = w;
@@ -351,8 +420,9 @@ __global__ void k_sum_partials(const double* part, int n, double* out) {
 // K1a  squared column norms of sqrt(w) * Jp per observation  (ref: qr/impl/landmark_block_base.ipp:493-518)
 //      thread per slot -> yobs[slot][9]; reduced per camera by k_cam_reduce (deterministic)
 //      OBSW (observation information, DESIGN.md section 19): the norms of sqrt(w) * W Jp, w from |W r|^2
+//      OBSL (observation losses, DESIGN.md section 21): w from the slot's own loss
 // ------------------------------------------------------------------------------------------------
-template <class S, bool OBSW = false>
+template <class S, bool OBSW = false, bool OBSL = false>
 __global__ void __launch_bounds__(256) k_jp_norms(DevPtrs<S> D, KOpts o, int* bad_flag) {
   for (int s = blockIdx.x * blockDim.x + threadIdx.x; s < D.nslots; s += gridDim.x * blockDim.x) {
     const int lm = D.slot_lm[s];
@@ -375,7 +445,7 @@ __global__ void __launch_bounds__(256) k_jp_norms(DevPtrs<S> D, KOpts o, int* ba
       for (int k = 0; k < 6; ++k) fin = fin && finite_s(Jl[k]);
       if (!fin) atomicOr(bad_flag, 1);
       S err, w;
-      error_weight(o, res[0] * res[0] + res[1] * res[1], err, w);
+      slot_error_weight<OBSL>(o, D.obs_loss, D.nslots, s, res[0] * res[0] + res[1] * res[1], err, w);
       const S sw = sqrt(w);
 #pragma unroll
       for (int c = 0; c < 9; ++c) {
@@ -744,7 +814,9 @@ __device__ __forceinline__ void rot_apply(const Rot<S>& g, S& x, S& y) {
 //   norms behind jls (the scaling of the whole Jacobian), and lane 0 of the group writes L diag(jls) and g = L (x - x0).
 //   OBSW (observation information, DESIGN.md section 19): the rows of an observation are sqrt(w) W [Jp | Jl | r], w from
 //   |W r|^2; W == 0 gives the all-zero record of a dropped projection.
-template <class S, bool GIVENS, bool LMP = false, bool OBSW = false>
+//   OBSL (observation losses, DESIGN.md section 21): w from the slot's own loss; w == 0 (TUKEY beyond its scale) gives rows
+//   of zeros.
+template <class S, bool GIVENS, bool LMP = false, bool OBSW = false, bool OBSL = false>
 __global__ void __launch_bounds__(128) k_linearize_qr(DevPtrs<S> D, KOpts o, Scratch<S> sc, int* bad_flag, TileOrder to) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   using V2 = typename ST<S>::V2;
@@ -795,19 +867,42 @@ __global__ void __launch_bounds__(128) k_linearize_qr(DevPtrs<S> D, KOpts o, Scr
           for (int k = 0; k < 6; ++k) fin = fin && finite_s(Jl[k]);
           if (!fin) atomicOr(bad_flag, 1);
           S err, w;
-          error_weight(o, res[0] * res[0] + res[1] * res[1], err, w);
-          const S sw = sqrt(w);
-          const S* sc = D.scaling + 9 * (size_t)cam_i;
+          if constexpr (OBSL) {
+            // the unweighted rows first, so that the registers of Jp and Jl are free while the slot's loss is evaluated (the
+            // compiler barrier keeps them from being forwarded), then weighted in place with the arithmetic below
 #pragma unroll
-          for (int c = 0; c < 9; ++c) {
-            const S d = sc[c];
-            e[c] = (sw * Jp[c]) * d;
-            e[9 + c] = (sw * Jp[9 + c]) * d;
+            for (int c = 0; c < 18; ++c) e[c] = Jp[c];
+#pragma unroll
+            for (int c = 0; c < 6; ++c) e[18 + c] = Jl[c];
+            asm volatile("" ::: "memory");
+            slot_error_weight<true>(o, D.obs_loss, D.nslots, s, res[0] * res[0] + res[1] * res[1], err, w);
+            const S sw = sqrt(w);
+            const S* sc = D.scaling + 9 * (size_t)cam_i;
+#pragma unroll
+            for (int c = 0; c < 9; ++c) {
+              const S d = sc[c];
+              e[c] = (sw * e[c]) * d;
+              e[9 + c] = (sw * e[9 + c]) * d;
+            }
+#pragma unroll
+            for (int c = 0; c < 6; ++c) e[18 + c] = sw * e[18 + c];
+            e[24] = sw * res[0];
+            e[25] = sw * res[1];
+          } else {
+            error_weight(o, res[0] * res[0] + res[1] * res[1], err, w);
+            const S sw = sqrt(w);
+            const S* sc = D.scaling + 9 * (size_t)cam_i;
+#pragma unroll
+            for (int c = 0; c < 9; ++c) {
+              const S d = sc[c];
+              e[c] = (sw * Jp[c]) * d;
+              e[9 + c] = (sw * Jp[9 + c]) * d;
+            }
+#pragma unroll
+            for (int c = 0; c < 6; ++c) e[18 + c] = sw * Jl[c];
+            e[24] = sw * res[0];
+            e[25] = sw * res[1];
           }
-#pragma unroll
-          for (int c = 0; c < 6; ++c) e[18 + c] = sw * Jl[c];
-          e[24] = sw * res[0];
-          e[25] = sw * res[1];
           wrote = true;
         }
       }

@@ -78,6 +78,7 @@ struct rba_handle {
   virtual int set_landmark_prior(int32_t num, const int32_t* lm_idx, const void* mean, const void* sqrt_info) = 0;
   virtual int set_intrinsics_groups(const int32_t* group) = 0;
   virtual int set_observation_info(const void* sqrt_info) = 0;
+  virtual int set_observation_loss(const uint8_t* kind, const void* scale) = 0;
   virtual int get_observation_residuals(void* residual, void* robust_weight, uint8_t* flags) = 0;
   virtual int compute_error(rba_residual_info* out) = 0;
   virtual int linearize() = 0;
@@ -241,7 +242,12 @@ struct Solver : rba_handle {
     DeviceBuffer<S> ve, y;         // [9 nc] the expanded operator input P v, the contracted output the vector step reads
     void adopt(GroupTerm& o) { lead.take(o.lead); ptr.take(o.ptr); mem.take(o.mem); fixed.take(o.fixed); ve.take(o.ve); y.take(o.y); }
   } grp;
-  struct { bool on = false; DeviceBuffer<S> W; } obs;  // rba_set_observation_info, DESIGN.md section 19: W [nslots][4] = D.obs_W while on
+  struct ObservationTerm {
+    bool on = false;               // rba_set_observation_info, DESIGN.md section 19: W [nslots][4] = D.obs_W while on
+    DeviceBuffer<S> W;
+    bool loss_on = false;          // rba_set_observation_loss, DESIGN.md section 21: the loss records = D.obs_loss while loss_on
+    DeviceBuffer<S> loss;          // float [nslots] {scale, uint32 kind}; double [nslots] scale + [nslots] uint8 kind (loss_records)
+  } obs;
   rba_stage_timings tm{};
   EventPair ev_stage1, ev_stage2, ev_precond, ev_pcg, ev_backsub, ev_update, ev_error, ev_mv, ev_user;
   long long launches = 0;
@@ -586,23 +592,40 @@ struct Solver : rba_handle {
     return RBA_OK;
   }
 
+  // The per-observation instances of the kernels that evaluate the reprojection terms: OBSW with observation information
+  // (D.obs_W, section 19), OBSL with observation losses (D.obs_loss, section 21); both off = the unmodified kernels
+  static auto k_error_instance(bool obsw, bool obsl) {
+    return obsw ? (obsl ? k_error<S, true, true> : k_error<S, true>) : (obsl ? k_error<S, false, true> : k_error<S>);
+  }
+  static auto k_jp_norms_instance(bool obsw, bool obsl) {
+    return obsw ? (obsl ? k_jp_norms<S, true, true> : k_jp_norms<S, true>) : (obsl ? k_jp_norms<S, false, true> : k_jp_norms<S>);
+  }
+  template <bool GIVENS, bool LMP>
+  static auto k1_of(bool obsw, bool obsl) {
+    return obsw ? (obsl ? k_linearize_qr<S, GIVENS, LMP, true, true> : k_linearize_qr<S, GIVENS, LMP, true>)
+                : (obsl ? k_linearize_qr<S, GIVENS, LMP, false, true> : k_linearize_qr<S, GIVENS, LMP>);
+  }
+  static auto k1_instance(bool givens, bool lmp, bool obsw, bool obsl) {  // + LMP: the landmark priors (section 17)
+    return givens ? (lmp ? k1_of<true, true>(obsw, obsl) : k1_of<true, false>(obsw, obsl))
+                  : (lmp ? k1_of<false, true>(obsw, obsl) : k1_of<false, false>(obsw, obsl));
+  }
+  template <bool LMP>
+  static auto kcov_of(bool obsw, bool obsl) {
+    return obsw ? (obsl ? k_cov_landmark<S, LMP, true, true> : k_cov_landmark<S, LMP, true>)
+                : (obsl ? k_cov_landmark<S, LMP, false, true> : k_cov_landmark<S, LMP>);
+  }
+
   int setup_kernels() {
     if (k1_sc.gstride) TRY(dalloc(&k1_sc.gbase, (size_t)(k1_max_blocks * TILE_WARPS) * k1_sc.gstride, false));
     if (k2_sc.gstride) TRY(dalloc(&k2_sc.gbase, (size_t)(k2_max_blocks * TILE_WARPS) * k2_sc.gstride, false));
-    CU(cudaFuncSetAttribute((k_linearize_qr<S, false>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)k1_smem));
-    CU(cudaFuncSetAttribute((k_linearize_qr<S, true>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)k1_smem));
+    // every k_linearize_qr instance: both QR variants, with and without landmark priors (section 17), observation
+    // information (section 19) and observation losses (section 21)
+    for (int v = 0; v < 16; ++v)
+      CU(cudaFuncSetAttribute(k1_instance(v & 8, v & 4, v & 2, v & 1), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)k1_smem));
     CU(cudaFuncSetAttribute((k_stage2<S, true>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)k2_smem));
     CU(cudaFuncSetAttribute((k_stage2<S, false>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)k2_smem));
-    // the landmark-prior instances (DESIGN.md section 17)
-    CU(cudaFuncSetAttribute((k_linearize_qr<S, false, true>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)k1_smem));
-    CU(cudaFuncSetAttribute((k_linearize_qr<S, true, true>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)k1_smem));
     CU(cudaFuncSetAttribute((k_stage2<S, true, true>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)k2_smem));
     CU(cudaFuncSetAttribute((k_stage2<S, false, true>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)k2_smem));
-    // the observation-information instances (DESIGN.md section 19)
-    CU(cudaFuncSetAttribute((k_linearize_qr<S, false, false, true>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)k1_smem));
-    CU(cudaFuncSetAttribute((k_linearize_qr<S, true, false, true>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)k1_smem));
-    CU(cudaFuncSetAttribute((k_linearize_qr<S, false, true, true>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)k1_smem));
-    CU(cudaFuncSetAttribute((k_linearize_qr<S, true, true, true>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)k1_smem));
     k4_smem_small = (size_t)K4_WARPS * L.k4_scratch_per_warp * sizeof(S);
     if (k4_smem_small > 200 * 1024) { g_err = "matvec scratch exceeds shared memory"; return RBA_ERR_UNSUPPORTED; }
     CU(cudaFuncSetAttribute((k_matvec_large<S, K4_WARPS, KPMAX>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(k4_smem_small, 1024)));
@@ -921,6 +944,7 @@ struct Solver : rba_handle {
     D.lmp_slot = lprior.n > 0 ? lprior.slot.get() : nullptr;
     D.lmp_mean = lprior.mean.get(); D.lmp_L = lprior.L.get(); D.lmp_Lg = lprior.Lg.get();
     D.obs_W = obs.on ? obs.W.get() : nullptr;
+    D.obs_loss = obs.loss_on ? obs.loss.get() : nullptr;
   }
   int priors_changed() {
     point_at_terms();
@@ -1057,6 +1081,54 @@ struct Solver : rba_handle {
     su_valid = s_valid = false;  // the assembled matrix belongs to the previous rows
     return priors_changed();
   }
+  // Scalars of the loss records of nslots slots (D.obs_loss): float {scale, uint32 kind} per slot; double the scales, then
+  // one uint8 kind per slot, rounded up to whole doubles
+  static size_t loss_records(int nslots) { return sizeof(S) == 4 ? 2 * (size_t)nslots : (size_t)nslots + ((size_t)nslots + 7) / 8; }
+  // A robust loss (RBA_LOSS_*, scale) per observation of the full problem (DESIGN.md section 21).  Part of the linearisation
+  // like the observation information, and landmark-owned like it: every rank receives the full arrays and keeps its own
+  // shard's slots.  NULL, or the handle's own choice (robust_norm, huber_parameter) on every observation of the shard, = the
+  // unmodified kernels (D.obs_loss == nullptr).  Every check runs before anything changes, so a rejected call leaves the
+  // previous losses.
+  int set_observation_loss(const uint8_t* kind, const void* scale_v) override {
+    auto bad = [&](const std::string& what) { g_err = "rba_set_observation_loss: " + what; return RBA_ERR_INVALID_ARGUMENT; };
+    if (!kind != !scale_v) return bad("kind and scale must both be given or both be NULL");
+    const S* a = (const S*)scale_v;
+    bool any = false;
+    std::vector<S> rec;
+    if (kind) {
+      for (long long o = 0; o < nobs_total; ++o) {
+        if (kind[o] > RBA_LOSS_TUKEY) return bad("observation " + std::to_string(o) + " has kind " + std::to_string(kind[o]) + " (must be 0..4)");
+        if (kind[o] != RBA_LOSS_NONE && !(std::isfinite((double)a[o]) && a[o] > S(0)))
+          return bad("observation " + std::to_string(o) + " has the scale " + std::to_string((double)a[o]) + " (must be finite and > 0)");
+      }
+      const uint8_t own = opt.robust_norm == 1 ? RBA_LOSS_HUBER : RBA_LOSS_NONE;
+      const S own_a = (S)opt.huber_parameter;
+      rec.assign(loss_records(L.nslots), S(0));  // padding slots: NONE
+      for (int s = 0; s < L.nslots; ++s) {
+        const long long o = L.slot_obs[s];
+        if (o < 0) continue;
+        const uint8_t k = kind[o];
+        const S sc = k == RBA_LOSS_NONE ? S(0) : a[o];  // NONE ignores its scale
+        any = any || k != own || (k == RBA_LOSS_HUBER && sc != own_a);
+        if constexpr (sizeof(S) == 4) {
+          const uint32_t k32 = k;
+          rec[2 * (size_t)s] = sc;
+          std::memcpy(&rec[2 * (size_t)s + 1], &k32, 4);
+        } else {
+          rec[s] = sc;
+          reinterpret_cast<uint8_t*>(rec.data() + L.nslots)[s] = k;
+        }
+      }
+    }
+    if (any) {
+      DeviceBuffer<S> next; TRY(fit(next, obs.loss, rec.size(), &rec));
+      CU(cudaStreamSynchronize(stream));
+      obs.loss.take(next);
+    }
+    obs.loss_on = any;
+    su_valid = s_valid = false;  // the assembled matrix belongs to the previous rows
+    return priors_changed();
+  }
   // Per observation at the current state, in problem order (DESIGN.md section 19).  Nothing of the handle changes: the
   // slot-ordered scratch is allocated for the call and freed before it returns.
   int get_observation_residuals(void* residual, void* robust_weight, uint8_t* flags) override {
@@ -1127,7 +1199,7 @@ struct Solver : rba_handle {
     if (error_cache_valid && error_cache_version == state_version) return RBA_OK;  // answered from the cache in finish
     int rc = start(ev_error); if (rc) return rc;
     CU(cudaMemsetAsync(d_flags, 0, 4 * sizeof(int), stream));
-    auto ke = D.obs_W ? k_error<S, true> : k_error<S>;  // OBSW: the whitened residuals (DESIGN.md section 19)
+    auto ke = k_error_instance(D.obs_W, D.obs_loss);  // OBSW: the whitened residuals (section 19); OBSL: their own losses (section 21)
     ke<<<EBLOCKS, 256, 0, stream>>>(D, ko, d_epart, d_flags);
     k_sum_partials<6><<<1, 256, 0, stream>>>(d_epart, EBLOCKS, d_red);
     launches += 2;
@@ -1183,7 +1255,7 @@ struct Solver : rba_handle {
     int rc = start(ev_stage1); if (rc) return rc;
     CU(cudaMemsetAsync(d_flags, 0, 4 * sizeof(int), stream));
     // pass A: squared column norms of the weighted pose Jacobians -> pose_jacobian_scaling_
-    auto kn = D.obs_W ? k_jp_norms<S, true> : k_jp_norms<S>;
+    auto kn = k_jp_norms_instance(D.obs_W, D.obs_loss);
     kn<<<grid_for(L.nslots, 256, 8), 256, 0, stream>>>(D, ko, d_flags);
     ++launches;
     rc = camera_reduce(d_csr_obs_slots, d_csr_obs_items, n_obs_items, d_csr_obs_item_ptr, D.diag2); if (rc) return rc;
@@ -1202,13 +1274,9 @@ struct Solver : rba_handle {
     }
     k_scaling<S><<<(9 * nc + 255) / 256, 256, 0, stream>>>(D.diag2, D.scaling, 9 * nc, (S)ko.jacobi_eps);
     // pass B: linearize (scaled) + Jl scaling + Householder QR + panel write
-    // (+ the landmark priors' column norms, L~ and g: the LMP instances; + the observation information: the OBSW instances)
-    const bool lmp = D.lmp_slot != nullptr;
-    auto k1 = opt.use_householder_marginalization ? (lmp ? k_linearize_qr<S, false, true> : k_linearize_qr<S, false>)
-                                                  : (lmp ? k_linearize_qr<S, true, true> : k_linearize_qr<S, true>);  // ref: ipp:149-163 selects perform_qr_givens
-    if (D.obs_W)
-      k1 = opt.use_householder_marginalization ? (lmp ? k_linearize_qr<S, false, true, true> : k_linearize_qr<S, false, false, true>)
-                                               : (lmp ? k_linearize_qr<S, true, true, true> : k_linearize_qr<S, true, false, true>);
+    // (+ the landmark priors' column norms, L~ and g: the LMP instances; + the observation information: the OBSW instances;
+    // + the observation losses: the OBSL instances).  ref: ipp:149-163 selects perform_qr_givens
+    auto k1 = k1_instance(!opt.use_householder_marginalization, D.lmp_slot, D.obs_W, D.obs_loss);
     k1<<<tile_grid(k1_max_blocks), TILE_WARPS * 32, k1_smem, stream>>>(D, ko, k1_sc, d_flags, order_k1);
     launches += 2;
     if (opt.preconditioner_type == 0 || opt.solver_type == 2) {
@@ -1961,9 +2029,11 @@ struct Solver : rba_handle {
     // 1.-2. elimination, assembly, priors, held parameters, equilibration
     CU(cudaMemsetAsync(A, 0, (size_t)(np * np) * 8, stream));
     CU(cudaMemsetAsync(fail, 0x7f, 4, stream));
-    // LMP: + L^T L of the landmark priors in Hll; OBSW: the rows whitened by the observation information
+    // LMP: + L^T L of the landmark priors in Hll; OBSW: the rows whitened by the observation information; OBSL: the
+    // observations' own losses
     auto kcov = n_lmp > 0 ? (D.obs_W ? k_cov_landmark<S, true, true> : k_cov_landmark<S, true>)
                           : (D.obs_W ? k_cov_landmark<S, false, true> : k_cov_landmark<S>);
+    if (D.obs_loss) kcov = n_lmp > 0 ? kcov_of<true>(D.obs_W, true) : kcov_of<false>(D.obs_W, true);
     kcov<<<wgrid, 128, 0, stream>>>(D, ko, d_cov_lm_slot0, d_cov_lm_n, nl, jp, kb, wl, rk, n_lmp > 0 ? lprior.of_lm.get() : nullptr);
     k_cov_assemble<<<std::max(1, std::min((cov_nblk + 7) / 8, sm_count * 8)), 256, 0, stream>>>(
         (const int2*)d_cov_blk_cam, d_cov_blk_ptr, (const int2*)d_cov_terms, cov_nblk, jp, kb, A, np);
@@ -2365,6 +2435,7 @@ int32_t rba_set_landmark_prior(rba_handle* h, int32_t num, const int32_t* lm_idx
 }
 int32_t rba_set_intrinsics_groups(rba_handle* h, const int32_t* group) { return h->set_intrinsics_groups(group); }
 int32_t rba_set_observation_info(rba_handle* h, const void* sqrt_info) { return h->set_observation_info(sqrt_info); }
+int32_t rba_set_observation_loss(rba_handle* h, const uint8_t* kind, const void* scale) { return h->set_observation_loss(kind, scale); }
 int32_t rba_get_observation_residuals(rba_handle* h, void* residual, void* robust_weight, uint8_t* flags) {
   return h->get_observation_residuals(residual, robust_weight, flags);
 }

@@ -146,6 +146,9 @@ struct ProblemPriors {
   std::vector<double> landmark_prior_sqrt_info;    // [m][9] row-major square-root information L
   // Square-root information of the observations (rba_set_observation_info)
   std::vector<double> obs_sqrt_info;               // [nobs][4] row-major 2x2 W in the order of the observations; 0 = switched off
+  // Robust loss per observation (rba_set_observation_loss); both empty = the options' robust norm everywhere
+  std::vector<uint8_t> obs_loss_kind;              // [nobs] RBA_LOSS_*
+  std::vector<double> obs_loss_scale;              // [nobs] scale (inlier threshold in units of sigma; ignored for NONE)
 };
 
 // Flat mirror of rootba::BalProblem<Scalar> with the member surface LinearizorQR / bundle_adjust_manual need.

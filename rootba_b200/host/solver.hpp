@@ -212,6 +212,12 @@ class LinearizorQR {
       const VecX W(bp.obs_sqrt_info.begin(), bp.obs_sqrt_info.end());
       check(rba_set_observation_info(h_, W.data()));
     }
+    if (!bp.obs_loss_kind.empty() || !bp.obs_loss_scale.empty()) {
+      if ((int64_t)bp.obs_loss_kind.size() != (int64_t)bp.num_observations() || bp.obs_loss_scale.size() != bp.obs_loss_kind.size())
+        throw std::runtime_error("obs_loss_kind and obs_loss_scale must have one entry per observation");
+      const VecX a(bp.obs_loss_scale.begin(), bp.obs_loss_scale.end());
+      check(rba_set_observation_loss(h_, bp.obs_loss_kind.data(), a.data()));
+    }
   }
   Problem& bal_problem_;
   SolverSummary* summary_ = nullptr;

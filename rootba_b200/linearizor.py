@@ -172,6 +172,43 @@ def _observation_info_array(info, num_observations: int, dtype):
     return a
 
 
+def _observation_loss_arrays(loss, num_observations: int, dtype):
+    """None, or validated contiguous (kind [Nobs] uint8, scale [Nobs] in `dtype`) of per-observation robust losses given as
+    (kind, scale): kind a name of LOSS_KINDS, an RBA_LOSS_* int or an [Nobs] array of either, scale a scalar or [Nobs];
+    scalars are broadcast.  The checks of rba_set_observation_loss: a known kind, and a finite scale > 0 for every kind but
+    NONE (whose scale is ignored)."""
+    if loss is None:
+        return None
+    try:
+        kind, scale = loss
+    except (TypeError, ValueError):
+        raise ValueError("observation_loss must be None or (kind, scale)") from None
+    k = np.asarray(kind)
+    if k.dtype.kind in "US":
+        names = [str(x).upper() for x in k.ravel()]
+        bad = sorted(set(names) - set(_lib.LOSS_KINDS))
+        if bad:
+            raise ValueError(f"observation_loss kind must be one of {sorted(_lib.LOSS_KINDS)}, got {bad}")
+        k = np.array([_lib.LOSS_KINDS[n] for n in names], np.int64).reshape(k.shape)
+    elif k.dtype.kind not in "iu":
+        raise ValueError(f"observation_loss kind must be names or integers, got dtype {k.dtype}")
+    if k.ndim == 0:
+        k = np.full(num_observations, k)
+    if k.shape != (num_observations,):
+        raise ValueError(f"observation_loss kind must be a scalar or have shape ({num_observations},), got {k.shape}")
+    if np.any((k < 0) | (k > _lib.LOSS_TUKEY)):
+        raise ValueError(f"observation_loss kinds must be in 0..{_lib.LOSS_TUKEY}")
+    a = np.array(scale, dtype=dtype, copy=True)
+    if a.ndim == 0:
+        a = np.full(num_observations, a, dtype)
+    if a.shape != (num_observations,):
+        raise ValueError(f"observation_loss scale must be a scalar or have shape ({num_observations},), got {a.shape}")
+    robust = k != _lib.LOSS_NONE
+    if not np.all(np.isfinite(a[robust]) & (a[robust] > 0)):
+        raise ValueError("observation_loss scales must be finite and > 0 for every kind but NONE")
+    return np.ascontiguousarray(k, np.uint8), np.ascontiguousarray(a)
+
+
 class BalProblem:
     """SoA BalProblem: cameras [nc,10] (quat xyzw, t, f,k1,k2), landmarks [nl,3], observations in
     CSR-by-landmark order with ascending camera index.  `camera_fixed` (not in the reference): None or one uint8 of FIX_*
@@ -189,7 +226,11 @@ class BalProblem:
     `observation_sqrt_info` (not in the reference): None, [Nobs] (1 / sigma per observation) or [Nobs,2,2] (a square root W of
     the inverse keypoint covariance per observation, in the order of obs_cam / obs_xy); the observation's cost becomes
     rho(|W r|^2) and W = 0 switches it off (rba_set_observation_info, DESIGN.md section 19).  Stored as [Nobs,2,2]; forwarded
-    likewise."""
+    likewise.
+    `observation_loss` (not in the reference): None (every observation uses the options' robust_norm) or (kind, scale), a
+    robust loss per observation: kind "NONE" | "HUBER" | "CAUCHY" | "SOFT_L1" | "TUKEY" (or RBA_LOSS_* ints), scale the inlier
+    threshold in units of sigma, each a scalar (broadcast) or one entry per observation (rba_set_observation_loss, DESIGN.md
+    section 21).  Stored as (kind [Nobs] uint8, scale [Nobs]); forwarded likewise."""
 
     def __init__(self, cams, lms, lm_off, obs_cam, obs_xy, dtype=np.float64):
         self.dtype = np.dtype(dtype)
@@ -208,6 +249,18 @@ class BalProblem:
         self._landmark_prior = None
         self._intrinsics_group = None
         self._observation_sqrt_info = None
+        self._observation_loss = None
+
+    @property
+    def observation_loss(self):
+        return self._observation_loss
+
+    @observation_loss.setter
+    def observation_loss(self, loss):
+        ls = _observation_loss_arrays(loss, self.num_observations(), self.dtype)
+        if self._linearizor is not None:
+            self._linearizor._upload_observation_loss(ls)  # raises on rejection: the previous losses stay in force
+        self._observation_loss = ls
 
     @property
     def observation_sqrt_info(self):
@@ -386,6 +439,8 @@ class LinearizorQR:
             self._upload_intrinsics_group(bal_problem.intrinsics_group)
         if bal_problem.observation_sqrt_info is not None:
             self._upload_observation_info(bal_problem.observation_sqrt_info)
+        if bal_problem.observation_loss is not None:
+            self._upload_observation_loss(bal_problem.observation_loss)
 
     # factory like Linearizor::create (linearizor.cpp:47-65)
     @staticmethod
@@ -472,9 +527,21 @@ class LinearizorQR:
     def _upload_observation_info(self, info):
         check(_lib.lib().rba_set_observation_info(self.h, None if info is None else _p(info)))
 
+    def set_observation_loss(self, kind, scale=1.0):
+        """a robust loss per observation (rba_set_observation_loss): kind None (the options' robust_norm everywhere) or a name /
+        RBA_LOSS_* int, scalar or [Nobs]; scale scalar or [Nobs], the inlier threshold in units of sigma.  Needs a new linearize
+        before the next solve; the losses are stored on the BalProblem."""
+        self.bal_problem.observation_loss = None if kind is None else (kind, scale)  # validates, forwards to _upload_observation_loss
+
+    def _upload_observation_loss(self, loss):
+        if loss is None:
+            check(_lib.lib().rba_set_observation_loss(self.h, None, None))
+        else:
+            check(_lib.lib().rba_set_observation_loss(self.h, _p(loss[0]), _p(loss[1])))
+
     def observation_residuals(self):
         """per observation at the current state, in the order of the problem's observations (rba_get_observation_residuals):
-        (residual [Nobs,2] = W r, robust_weight [Nobs], flags [Nobs] uint8: bit 0 = projection valid, bit 1 = in use).  A
+        (residual [Nobs,2] = W r, robust_weight [Nobs] (of each observation's own loss), flags [Nobs] uint8: bit 0 = projection valid, bit 1 = in use).  A
         sharded handle fills only the observations of its own landmark shard (the others stay 0)."""
         nobs = self.bal_problem.num_observations()
         res, hw, flags = np.zeros((nobs, 2), self.dtype), np.zeros(nobs, self.dtype), np.zeros(nobs, np.uint8)
