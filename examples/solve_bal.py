@@ -5,7 +5,8 @@
         [--fix-intrinsics] [--fix-cameras I,J,...] [--camera-prior FILE.npz] [--camera-pair-prior FILE.npz]
         [--landmark-prior FILE.npz] [--shared-intrinsics | --intrinsics-groups FILE.npy] [--covariance OUT.npz]
         [--relative-covariance PAIRS.npy] [--observation-info FILE.npy] [--observation-loss KIND:SCALE | FILE.npz]
-        [--residuals OUT.npz]
+        [--residuals OUT.npz] [--camera-prior-loss KIND:SCALE | FILE.npz] [--pair-prior-loss KIND:SCALE | FILE.npz]
+        [--landmark-prior-loss KIND:SCALE | FILE.npz] [--prior-residuals OUT.npz]
 
 Mirrors what `bal_qr --input ...` of the reference does (src/app/bal_qr.cpp): load + normalise (bal_problem.cpp:773-852),
 optimize_lm_ours with the QR linearizor (solver/bal_bundle_adjustment.cpp:249-544), log (bal/ba_log.hpp)."""
@@ -18,6 +19,22 @@ import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import rootba_b200 as rb  # noqa: E402
+
+
+def read_loss(ap, flag, value):
+    """(kind, scale) of a KIND:SCALE or FILE.npz (arrays `kind`, `scale`) loss argument"""
+    if value.endswith(".npz"):
+        with np.load(value) as f:
+            if "kind" not in f or "scale" not in f:
+                ap.error(f"{flag}: {value} must hold the arrays `kind` and `scale`")
+            return f["kind"], f["scale"]
+    kind, sep, scale = value.partition(":")
+    if not sep:
+        ap.error(f"{flag}: expected KIND:SCALE (e.g. CAUCHY:2) or FILE.npz")
+    try:
+        return kind, float(scale)
+    except ValueError:
+        ap.error(f"{flag}: the scale of {value!r} is not a number")
 
 
 def main():
@@ -70,6 +87,15 @@ def main():
     ap.add_argument("--residuals", default=None, metavar="OUT.npz",
                     help="after the solve, write per observation `residual` [Nobs, 2] (W r), `robust_weight` [Nobs] and `flags` "
                          "[Nobs] (bit 0 = projection valid, bit 1 = in use) at the final state (DESIGN.md section 19)")
+    for flag, what in (("--camera-prior-loss", "camera of --camera-prior"), ("--pair-prior-loss", "pair of --camera-pair-prior"),
+                       ("--landmark-prior-loss", "prior of --landmark-prior")):
+        ap.add_argument(flag, default=None, metavar="KIND:SCALE | FILE.npz",
+                        help=f"a robust loss per {what} (DESIGN.md section 22): KIND:SCALE for every one (KIND as for "
+                             "--observation-loss; SCALE the threshold on |L e|, e.g. 2.80 for a 95 %% gate on 3 degrees of freedom, "
+                             "3.55 on 6), or a .npz with the arrays `kind` and `scale`, one entry each in the prior's order")
+    ap.add_argument("--prior-residuals", default=None, metavar="OUT.npz",
+                    help="after the solve, write per prior kind given `<kind>_residual` [num, 9 | 6 | 3] (L e) and "
+                         "`<kind>_robust_weight` [num] at the final state, kind camera, pair or landmark (DESIGN.md section 22)")
     args = ap.parse_args()
     if args.relative_covariance and not args.covariance:
         ap.error("--relative-covariance requires --covariance")
@@ -138,33 +164,35 @@ def main():
             problem.observation_sqrt_info = info
         except ValueError as e:
             ap.error(f"--observation-info: {e}")
-    if args.observation_loss:
-        try:
-            if args.observation_loss.endswith(".npz"):
-                with np.load(args.observation_loss) as f:
-                    if "kind" not in f or "scale" not in f:
-                        ap.error(f"--observation-loss: {args.observation_loss} must hold the arrays `kind` and `scale`")
-                    problem.observation_loss = (f["kind"], f["scale"])
-            else:
-                kind, sep, scale = args.observation_loss.partition(":")
-                if not sep:
-                    ap.error("--observation-loss: expected KIND:SCALE (e.g. CAUCHY:2) or FILE.npz")
-                problem.observation_loss = (kind, float(scale))
-        except ValueError as e:
-            ap.error(f"--observation-loss: {e}")
+    for flag, value, attr in (("--observation-loss", args.observation_loss, "observation_loss"),
+                              ("--camera-prior-loss", args.camera_prior_loss, "camera_prior_loss"),
+                              ("--pair-prior-loss", args.pair_prior_loss, "camera_pair_prior_loss"),
+                              ("--landmark-prior-loss", args.landmark_prior_loss, "landmark_prior_loss")):
+        if value:
+            loss = read_loss(ap, flag, value)
+            try:
+                setattr(problem, attr, loss)
+            except ValueError as e:
+                ap.error(f"{flag}: {e}")
     options = rb.SolverOptions(max_num_iterations=args.max_num_iterations, preconditioner_type=args.preconditioner_type,
                                operator_form=args.operator_form, use_double=not args.float)
     summary = rb.bundle_adjust_manual(problem, options, verbose=True)
     print(summary["termination_type"], summary["message"])
     rb.save_ba_log(args.log_path, summary, problem, args.input, {"load": t_load, "optimize": summary["total_time"]})
     print("wrote", args.log_path)
-    if args.covariance or args.residuals:
+    if args.covariance or args.residuals or args.prior_residuals:
         lin = rb.LinearizorQR.create(problem, options)  # at the final state, with the same priors, information and held parameters
         try:
             if args.covariance:  # one factorisation for the marginals and the relative poses
                 blocks = lin.covariance_blocks(relative=rel_pairs, marginals=True)
             if args.residuals:
                 res, hw, flags = lin.observation_residuals()
+            prior_res = {}
+            if args.prior_residuals:
+                for kind, prior in (("camera", problem.camera_prior), ("pair", problem.camera_pair_prior),
+                                    ("landmark", problem.landmark_prior)):
+                    if prior is not None:
+                        prior_res[kind + "_residual"], prior_res[kind + "_robust_weight"] = lin.prior_residuals(kind)
         finally:
             lin.close()
         if args.covariance:
@@ -174,6 +202,9 @@ def main():
         if args.residuals:
             np.savez(args.residuals, residual=res, robust_weight=hw, flags=flags)
             print("wrote", args.residuals)
+        if args.prior_residuals:
+            np.savez(args.prior_residuals, **prior_res)
+            print("wrote", args.prior_residuals)
 
 
 if __name__ == "__main__":

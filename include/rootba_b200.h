@@ -247,7 +247,8 @@ int32_t rba_set_camera_fixed(rba_handle* h, const uint8_t* flags);
  *   CENTRE c0 in the world frame, not t), f0, k1_0, k2_0.
  * sqrt_info [81*Nc] Scalar: per camera a row-major 9x9 square-root information L_c.  Residual order
  *   e = (c - c0 [3], Log(R R0^T) [3], f - f0, k1 - k1_0, k2 - k2_0),  c = -R^T t.
- *   The prior cost is 1/2 |L_c e_c|^2, in the same convention as the reprojection terms (err = 1/2 r^2), not robustified.
+ *   The prior cost is 1/2 |L_c e_c|^2, in the same convention as the reprojection terms (err = 1/2 r^2); a robust loss per
+ *   camera is set by rba_set_prior_loss (DESIGN.md section 22).
  *   An all-zero L_c means no prior on camera c.  Partial priors are rows of L (e.g. centre only).
  * Both NULL: no priors, the default.  Every rank of a sharded problem passes the same arrays.
  * The prior Jacobian is part of the linearisation: the Jacobi scaling is computed from the whole Jacobian (reprojection and
@@ -271,7 +272,7 @@ int32_t rba_set_camera_prior(rba_handle* h, const void* mean, const void* sqrt_i
  *   the default.  Residual (split form, not the SE(3) logarithm)
  *     e_t = t_i - R_i R_j^T t_j - t0   (= R_i (c_j - c_i) - t0, the centre of j seen from camera i),
  *     e_r = Log(R_i R_j^T R0^T)        (angle in [0, pi]),
- *   cost 1/2 |L (e_t, e_r)|^2, not robustified.  An all-zero L has no effect.  Several pairs on the same cameras, and both
+ *   cost 1/2 |L (e_t, e_r)|^2 (a robust loss per pair: rba_set_prior_loss, DESIGN.md section 22).  An all-zero L has no effect.  Several pairs on the same cameras, and both
  *   (i, j) and (j, i), are allowed: each is one more measurement.  Every rank of a sharded problem passes the same arrays.
  * Like the absolute priors the pair priors are part of the linearisation (Jacobi scaling, rba_get_rhs,
  * rba_get_preconditioner, rba_right_multiply, rba_compute_error include them), combine with rba_set_camera_prior and
@@ -288,8 +289,8 @@ int32_t rba_set_camera_pair_prior(rba_handle* h, int32_t num_pairs, const int32_
 /* Not in the reference.  A soft prior on the world position of selected landmarks (surveyed ground control points, depth
  * or LiDAR points, points of an earlier map).  Prior p is on landmark lm_idx[p] (problem order):
  *   lm_idx [num] int32;  mean [3*num] Scalar, the prior position x0 (world frame);  sqrt_info [9*num] Scalar, row-major
- *   3x3 L.  num == 0 (pointers ignored): no landmark priors, the default.  Residual e = x - x0, cost 1/2 |L e|^2, not
- *   robustified.  L need not have full rank (a height-only prior is one non-zero row); an all-zero L is dropped.  Every
+ *   3x3 L.  num == 0 (pointers ignored): no landmark priors, the default.  Residual e = x - x0, cost 1/2 |L e|^2 (a
+ *   robust loss per prior: rba_set_prior_loss, DESIGN.md section 22).  L need not have full rank (a height-only prior is one non-zero row); an all-zero L is dropped.  Every
  *   rank of a sharded problem passes the same full list and keeps the priors of its own landmark shard.
  * The priors are part of the linearisation: the landmark Jacobi scaling is that of the whole Jacobian, and the solve, the
  * back-substitution, l_diff of rba_apply, rba_compute_error and rba_compute_covariance include them (a prior can give a
@@ -394,6 +395,44 @@ int32_t rba_get_observation_residuals(rba_handle* h, void* residual, void* robus
  * The losses cost 8 bytes (float) or 9 bytes (double) per observation slot of device memory, counted in
  * rba_workload_stats::device_bytes from the first call that sets a loss other than the handle's own. */
 int32_t rba_set_observation_loss(rba_handle* h, const uint8_t* kind, const void* scale);
+
+/* ---- Robust losses on the priors (DESIGN.md section 22) ------------------------------------- */
+
+#define RBA_PRIOR_CAMERA   0   /* rba_set_camera_prior:      one entry per camera, num = Nc            */
+#define RBA_PRIOR_PAIR     1   /* rba_set_camera_pair_prior: one entry per pair, in the caller's order */
+#define RBA_PRIOR_LANDMARK 2   /* rba_set_landmark_prior:    one entry per prior, in the caller's order */
+
+/* Not in the reference.  Prior p of any kind has the whitened residual L_p e_p (e as defined for its kind) and
+ * s_p = |L_p e_p|^2.  With a loss kind[p] and scale a = scale[p] (RBA_LOSS_*, the same rho as rba_set_observation_loss, from
+ * the same device function) its cost is rho(s_p)/2, its robust weight w_p = rho'(s_p) and its rows sqrt(w_p) L_p de/d(inc)
+ * and sqrt(w_p) L_p e_p (IRLS weighting, no second-order correction).  One weight per prior, on its whole squared
+ * Mahalanobis distance (not per component): a is compared with |L e|.  A 95 % gate is a = sqrt(chi2_0.95(dof)): a ~ 3.55 for
+ * a 6-DoF pair prior, a ~ 2.80 for a 3-DoF centre or landmark prior.  A TUKEY prior beyond its scale has w = 0: all-zero
+ * rows, and a^2/6 in all_error and valid_error.
+ * prior_kind RBA_PRIOR_*; kind [num] uint8 and scale [num] Scalar in the caller's order of that kind's setter: num = Nc for
+ * camera priors, else the num (num_pairs) of the last successful call of its setter.  Priors dropped for an all-zero L, and
+ * landmark priors of another shard, take their entries and ignore them.  Both NULL, or NONE on every entry, = no losses on
+ * that kind, the default: the unmodified kernels run.  The handle's robust_norm never applies to priors; rba_solver_opts
+ * is unchanged.  A later successful call of the kind's setter clears its losses back to NONE.
+ * The rows and costs of every entry point (rba_linearize, rba_solve, rba_get_rhs, rba_get_preconditioner,
+ * rba_right_multiply, rba_compute_error, l_diff) use the weighted priors, w taken at the state of rba_linearize for the
+ * rows and at the current state for the cost; rba_compute_covariance and rba_compute_covariance_blocks evaluate w in
+ * double at their current state.
+ * After a successful call rba_solve returns RBA_ERR_STATE until the next rba_linearize; the device-resident increment and
+ * the cached error are discarded.  RBA_ERR_INVALID_ARGUMENT, with the previous losses kept in force: an unknown prior_kind,
+ * a num that does not match, exactly one pointer NULL, a kind above RBA_LOSS_TUKEY, or a kind other than RBA_LOSS_NONE with
+ * a scale that is not finite or <= 0.
+ * The losses cost the loss records (8 bytes (float) or 9 bytes (double) per prior) and a copy of the priors' L of device
+ * memory, counted in rba_workload_stats::device_bytes from the first call that sets a loss other than NONE. */
+int32_t rba_set_prior_loss(rba_handle* h, int32_t prior_kind, int32_t num, const uint8_t* kind, const void* scale);
+
+/* Per prior of one kind at the handle's CURRENT state, in the caller's order of its setter (num entries as for
+ * rba_set_prior_loss); either pointer may be NULL, not both (-> RBA_ERR_INVALID_ARGUMENT, as is an unknown prior_kind).
+ * residual [9 / 6 / 3 * num] Scalar: L e, with the unweighted L; robust_weight [num] Scalar: w of the prior's loss (1 with
+ * NONE).  A camera with an all-zero L, or a dropped pair or landmark prior, gives 0 and weight 1.  A sharded handle writes
+ * every camera and pair entry, but only the landmark priors of its own shard.  Needs no rba_linearize; changes nothing of
+ * the handle (scratch device memory is allocated for the call and freed before it returns). */
+int32_t rba_get_prior_residuals(rba_handle* h, int32_t prior_kind, void* residual, void* robust_weight);
 
 /* ---- Marginal covariances (DESIGN.md section 16) ------------------------------------------ */
 

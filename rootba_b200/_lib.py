@@ -34,6 +34,13 @@ LOSS_SOFT_L1 = 3
 LOSS_TUKEY = 4
 LOSS_KINDS = {"NONE": LOSS_NONE, "HUBER": LOSS_HUBER, "CAUCHY": LOSS_CAUCHY, "SOFT_L1": LOSS_SOFT_L1, "TUKEY": LOSS_TUKEY}
 
+# prior kinds of rba_set_prior_loss / rba_get_prior_residuals (RBA_PRIOR_*) and the rows of L e of each
+PRIOR_CAMERA = 0
+PRIOR_PAIR = 1
+PRIOR_LANDMARK = 2
+PRIOR_KINDS = {"camera": PRIOR_CAMERA, "pair": PRIOR_PAIR, "landmark": PRIOR_LANDMARK}
+PRIOR_ROWS = {PRIOR_CAMERA: 9, PRIOR_PAIR: 6, PRIOR_LANDMARK: 3}
+
 
 class RbaError(RuntimeError):
     def __init__(self, code: int, msg: str):
@@ -149,6 +156,8 @@ def lib():
         _lib.rba_compute_covariance_blocks.argtypes = [C.c_void_p, C.POINTER(CovarianceQuery)]
         _lib.rba_set_landmark_prior.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
         _lib.rba_set_observation_loss.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+        _lib.rba_set_prior_loss.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
+        _lib.rba_get_prior_residuals.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]
     return _lib
 
 

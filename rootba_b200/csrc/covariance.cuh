@@ -74,7 +74,9 @@ __device__ __forceinline__ void cov_sym3_eig(double (&A)[9], double (&V)[9]) {
 // lmp_of_lm[lm] >= 0, so a landmark with fewer than 2 valid observations can be full rank.
 // OBSW (observation information, DESIGN.md section 19): the rows are whitened in double, sqrt(w) W [Jp | Jl], w from |W r|^2.
 // OBSL (observation losses, DESIGN.md section 21): w from the slot's own loss, evaluated in double.
-template <class S, bool LMP = false, bool OBSW = false, bool OBSL = false>
+// LMPL (losses on the landmark priors, DESIGN.md section 22; implies LMP): Hll += w L^T L, with the unweighted L (D.lmp_Lu)
+// and w of the prior's loss on |L (x - x0)|^2, evaluated in double at the current state.
+template <class S, bool LMP = false, bool OBSW = false, bool OBSL = false, bool LMPL = false>
 __global__ void __launch_bounds__(128) k_cov_landmark(DevPtrs<S> D, KOpts o, const int* __restrict__ lm_slot0,
                                                       const int* __restrict__ lm_n, int nl, double* __restrict__ jpw,
                                                       double* __restrict__ kb, double* __restrict__ wl, int* __restrict__ rank,
@@ -124,10 +126,27 @@ __global__ void __launch_bounds__(128) k_cov_landmark(DevPtrs<S> D, KOpts o, con
     if constexpr (LMP) {
       const int lp = lmp_of_lm[lm];
       if (lp >= 0) {
-        const S* Lp = D.lmp_L + 9 * (size_t)lp;
+        const S* Lp = (LMPL ? D.lmp_Lu : D.lmp_L) + 9 * (size_t)lp;
+        double sw = 1.0;
+        if constexpr (LMPL) {
+          const double e[3] = {pw[0] - (double)D.lmp_mean[3 * lp], pw[1] - (double)D.lmp_mean[3 * lp + 1], pw[2] - (double)D.lmp_mean[3 * lp + 2]};
+          double s = 0.0;
+#pragma unroll
+          for (int r = 0; r < 3; ++r) {
+            const double v = (double)Lp[3 * r] * e[0] + (double)Lp[3 * r + 1] * e[1] + (double)Lp[3 * r + 2] * e[2];
+            s += v * v;
+          }
+          unsigned kind;
+          S a;
+          slot_loss(D.lmp_loss, D.lmp_n, (size_t)lp, kind, a);
+          double err, w;
+          observation_loss<double>(kind, (double)a, s, err, w);
+          sw = sqrt(w);
+        }
 #pragma unroll
         for (int r = 0; r < 3; ++r) {
-          const double a0 = (double)Lp[3 * r], a1 = (double)Lp[3 * r + 1], a2 = (double)Lp[3 * r + 2];
+          double a0 = (double)Lp[3 * r], a1 = (double)Lp[3 * r + 1], a2 = (double)Lp[3 * r + 2];
+          if constexpr (LMPL) { a0 *= sw; a1 *= sw; a2 *= sw; }  // the row of sqrt(w) L
           h[0] += a0 * a0; h[1] += a0 * a1; h[2] += a0 * a2; h[3] += a1 * a1; h[4] += a1 * a2; h[5] += a2 * a2;
         }
       }
@@ -211,11 +230,33 @@ __global__ void __launch_bounds__(256) k_cov_assemble(const int2* __restrict__ b
 // in list order, the pair blocks A_s^T A_s (diagonal) and A_s^T A_o (to the column block of the other camera o < c).
 // The rows are those of k_prior_linearize / k_pair_linearize (prior_jac_row, pair_jac_rows), unscaled, evaluated in double
 // from the stored means and L.
-template <class S>
+// LOSS (losses on the priors, DESIGN.md section 22): the rows of a prior with a loss record (ploss over the nc cameras,
+// qloss over the nq pairs; nullptr = every prior of that kind NONE) are those of sqrt(w) L, w of its loss on |L e|^2,
+// evaluated in double at the current state from the unweighted L.
+template <int NR, class S>
+__device__ __forceinline__ double cov_prior_sqrt_weight(const S* __restrict__ loss, int n, int p, const S* __restrict__ Lp,
+                                                        const double* e) {
+  double s = 0.0;
+#pragma unroll
+  for (int i = 0; i < NR; ++i) {
+    double v = 0.0;
+#pragma unroll
+    for (int k = 0; k < NR; ++k) v += (double)Lp[NR * i + k] * e[k];
+    s += v * v;
+  }
+  unsigned kind;
+  S a;
+  slot_loss(loss, n, (size_t)p, kind, a);
+  double err, w;
+  observation_loss<double>(kind, (double)a, s, err, w);
+  return sqrt(w);
+}
+template <class S, bool LOSS = false>
 __global__ void k_cov_priors(const S* __restrict__ cams, int nc, const S* __restrict__ pmean, const S* __restrict__ pL,
                              const int* __restrict__ pairs, const S* __restrict__ qmean, const S* __restrict__ qL,
                              const int* __restrict__ qptr, const int* __restrict__ qitem, const int* __restrict__ qnbr,
-                             double* __restrict__ A, long long ld) {
+                             double* __restrict__ A, long long ld, const S* __restrict__ ploss = nullptr,
+                             const S* __restrict__ qloss = nullptr, int nq = 0) {
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= nc) return;
   double* Acc = A + 9 * (long long)c + 9 * (long long)c * ld;  // diagonal block (c, c)
@@ -224,10 +265,18 @@ __global__ void k_cov_priors(const S* __restrict__ cams, int nc, const S* __rest
 #pragma unroll
     for (int k = 0; k < 10; ++k) { cam[k] = (double)cams[10 * (size_t)c + k]; mean[k] = (double)pmean[10 * (size_t)c + k]; }
     prior_residual<double, true>(cam, mean, e, Jinv, R);
+    double sw = 1.0;
+    if constexpr (LOSS) {
+      if (ploss) sw = cov_prior_sqrt_weight<9>(ploss, nc, c, pL + 81 * (size_t)c, e);
+    }
     for (int i = 0; i < 9; ++i) {
       double l[9], row[9];
 #pragma unroll
       for (int k = 0; k < 9; ++k) l[k] = (double)pL[81 * (size_t)c + 9 * i + k];
+      if constexpr (LOSS) {
+#pragma unroll
+        for (int k = 0; k < 9; ++k) l[k] *= sw;
+      }
       prior_jac_row(l, R, Jinv, row);
       for (int a = 0; a < 9; ++a)
         for (int b = 0; b <= a; ++b) Acc[a + b * ld] += row[a] * row[b];
@@ -246,10 +295,18 @@ __global__ void k_cov_priors(const S* __restrict__ cams, int nc, const S* __rest
       for (int k = 0; k < 7; ++k) mean[k] = (double)qmean[7 * (size_t)p + k];
       pair_residual<double, true>(ci, cj, mean, e, M, tr, Jinv, JM);
       double* Aco = A + 9 * (long long)c + 9 * (long long)o * ld;  // block (c, o), used when o < c
+      double sw = 1.0;
+      if constexpr (LOSS) {
+        if (qloss) sw = cov_prior_sqrt_weight<6>(qloss, nq, p, qL + 36 * (size_t)p, e);
+      }
       for (int i = 0; i < 6; ++i) {
         double l[6], ri[6], rj[6];
 #pragma unroll
         for (int k = 0; k < 6; ++k) l[k] = (double)qL[36 * (size_t)p + 6 * i + k];
+        if constexpr (LOSS) {
+#pragma unroll
+          for (int k = 0; k < 6; ++k) l[k] *= sw;
+        }
         pair_jac_rows(l, M, tr, Jinv, JM, ri, rj);
         const double* own = side ? rj : ri;
         const double* oth = side ? ri : rj;

@@ -109,6 +109,11 @@ struct DevPtrs {
   // robust loss per observation (rba_set_observation_loss, DESIGN.md section 21); nullptr = the handle's robust_norm on every
   // observation of this shard.  Only the kernels' OBSL instances, k_obs_residuals and k_cov_landmark read it (slot_loss).
   const S* obs_loss;         // float: [nslots] {scale, uint32 kind}; double: [nslots] scale, then [nslots] uint8 kind (padding NONE)
+  // robust losses on the landmark priors (rba_set_prior_loss, DESIGN.md section 22); lmp_loss == nullptr = none.  While they
+  // are on, lmp_L is sqrt(w) L of the last linearisation; k_cov_landmark's LMPL instances re-weight the unweighted L here.
+  const S* lmp_Lu;           // [m][9] the unweighted L
+  const S* lmp_loss;         // the loss records of the lmp_n priors (slot_loss layout)
+  int lmp_n;
 };
 
 // increment entries (tx,ty,tz, rx,ry,rz, f,k1,k2) held by a camera's RBA_FIX_* bits, as a 9-bit mask
@@ -3089,27 +3094,34 @@ __device__ __forceinline__ void prior_jac_row(const S* l, const S* R, const S* J
 }
 
 // The per-item terms of the one-block kernels k_prior_cost and k_prior_ldiff, one struct per prior kind (item = camera,
-// pair or landmark prior).  sq_norm(p) = |L e|^2 of item p, model_change(inc, p) = (A d)^T (1/2 A d + r) for its part d
-// of the increment; each kind keeps its own summation order.
+// pair or landmark prior).  rows_of(p, f) calls f(i, (L e)_i) row by row (k_prior_residuals reads them), sq_norm(p) =
+// |L e|^2 of item p, model_change(inc, p) = (A d)^T (1/2 A d + r) for its part d of the increment; each kind keeps its own
+// summation order.
 template <class S>
 struct CameraPrior {
   using Scalar = S;
+  static constexpr int NR = 9;  // rows of L e; L is NR x NR
   const S* cams;
   const S* mean;  // [nc][10]
   const S* L;     // [nc][81]
   const S* A;     // [nc][81]
   const S* r;     // [nc][9]
-  __device__ S sq_norm(int cam) const {
+  // f(i, (L e)_i) for the rows i of item cam in order
+  template <class F>
+  __device__ void rows_of(int cam, F f) const {
     S e[9];
     prior_residual<S, false>(cams + 10 * (size_t)cam, mean + 10 * (size_t)cam, e, nullptr, nullptr);
     const S* Lc = L + 81 * (size_t)cam;
-    S c2 = 0;
     for (int i = 0; i < 9; ++i) {
       S ri = 0;
 #pragma unroll
       for (int k = 0; k < 9; ++k) ri += Lc[9 * i + k] * e[k];
-      c2 += ri * ri;
+      f(i, ri);
     }
+  }
+  __device__ S sq_norm(int cam) const {
+    S c2 = 0;
+    rows_of(cam, [&](int, S ri) { c2 += ri * ri; });
     return c2;
   }
   __device__ S model_change(const S* inc, int cam) const {
@@ -3228,24 +3240,85 @@ __global__ void k_prior_ldiff(K k, const typename K::Scalar* __restrict__ inc, i
 // each once.  Their share of l_diff is computed per landmark in k_back_substitute.
 template <class S>
 struct LandmarkPrior {
+  using Scalar = S;
+  static constexpr int NR = 3;
   const S* lms;
   const int* lm;   // [m]
   const S* mean;   // [m][3]
   const S* L;      // [m][9]
-  __device__ S sq_norm(int p) const {
+  template <class F>
+  __device__ void rows_of(int p, F f) const {
     const S* x = lms + 3 * (size_t)lm[p];
     const S* x0 = mean + 3 * (size_t)p;
     const S e0 = x[0] - x0[0], e1 = x[1] - x0[1], e2 = x[2] - x0[2];
     const S* Lp = L + 9 * (size_t)p;
-    S c2 = 0;
 #pragma unroll
-    for (int r = 0; r < 3; ++r) {
-      const S v = Lp[3 * r] * e0 + Lp[3 * r + 1] * e1 + Lp[3 * r + 2] * e2;
-      c2 += v * v;
-    }
+    for (int r = 0; r < 3; ++r) f(r, Lp[3 * r] * e0 + Lp[3 * r + 1] * e1 + Lp[3 * r + 2] * e2);
+  }
+  __device__ S sq_norm(int p) const {
+    S c2 = 0;
+    rows_of(p, [&](int, S v) { c2 += v * v; });
     return c2;
   }
 };
+
+// Robust losses on the priors (rba_set_prior_loss, DESIGN.md section 22).  Prior kind K with one loss record per item
+// (slot_loss layout over its n items) and the loss function of the observations, observation_loss, on s = |L e|^2:
+// sq_norm(p) = rho(s), which k_prior_cost halves into the cost rho(s)/2; loss_of gives err = rho(s)/2 and w = rho'(s).
+template <class K>
+struct RobustPrior {
+  using Scalar = typename K::Scalar;
+  K k;
+  const Scalar* loss;
+  int n;
+  __device__ void loss_of(int p, Scalar s, Scalar& err, Scalar& w) const {
+    unsigned kind;
+    Scalar a;
+    slot_loss(loss, n, (size_t)p, kind, a);
+    observation_loss<Scalar>(kind, a, s, err, w);
+  }
+  __device__ Scalar sq_norm(int p) const {
+    Scalar err, w;
+    loss_of(p, k.sq_norm(p), err, w);
+    return Scalar(2) * err;
+  }
+};
+
+// Once per linearisation, before the kernels that read L (k_prior_linearize, k_pair_linearize, the LMP instances of
+// k_linearize_qr): Lw = sqrt(w) L per item, w at the linearisation point.  Everything the solve derives from a prior is
+// linear in L, so its rows become sqrt(w) L de/d(inc) and sqrt(w) L e.  NONE gives w = 1 and Lw = L bit for bit; TUKEY
+// beyond its scale w = 0 and all-zero rows.  Thread per item.
+template <class K>
+__global__ void k_prior_weight(RobustPrior<K> rk, typename K::Scalar* __restrict__ Lw) {
+  using S = typename K::Scalar;
+  constexpr int NL = K::NR * K::NR;
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= rk.n) return;
+  S err, w;
+  rk.loss_of(p, rk.k.sq_norm(p), err, w);
+  const S sw = sqrt(w);
+  const S* Lp = rk.k.L + NL * (size_t)p;
+  S* out = Lw + NL * (size_t)p;
+  for (int i = 0; i < NL; ++i) out[i] = sw * Lp[i];
+}
+
+// rba_get_prior_residuals: per item at the current state res [NR] = L e (unweighted L) and w = rho'(|L e|^2) of its loss
+// (loss == nullptr: every item NONE, w = 1).  Thread per item.
+template <class K>
+__global__ void k_prior_residuals(K k, const typename K::Scalar* __restrict__ loss, int n, typename K::Scalar* __restrict__ res,
+                                  typename K::Scalar* __restrict__ wout) {
+  using S = typename K::Scalar;
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= n) return;
+  S s = 0;
+  k.rows_of(p, [&](int i, S ri) { res[K::NR * (size_t)p + i] = ri; s += ri * ri; });
+  S w = S(1);
+  if (loss) {
+    S err;
+    RobustPrior<K>{k, loss, n}.loss_of(p, s, err, w);
+  }
+  wout[p] = w;
+}
 
 // ------------------------------------------------------------------------------------------------
 // K9  Relative pose priors between two cameras (rba_set_camera_pair_prior, DESIGN.md section 15).  Pair p = (i, j) with the
@@ -3312,24 +3385,29 @@ __device__ __forceinline__ void pair_jac_rows(const S* l, const S* M, const S* t
 template <class S>
 struct PairPrior {
   using Scalar = S;
+  static constexpr int NR = 6;
   const S* cams;
   const int* pairs;  // [m][2]
   const S* mean;     // [m][7]
   const S* L;        // [m][36]
   const S* A;        // [m][2][36]
   const S* r;        // [m][6]
-  __device__ S sq_norm(int p) const {
+  template <class F>
+  __device__ void rows_of(int p, F f) const {
     S e[6], M[9], tr[3];
     pair_residual<S, false>(cams + 10 * (size_t)pairs[2 * p], cams + 10 * (size_t)pairs[2 * p + 1], mean + 7 * (size_t)p, e, M, tr,
                             nullptr, nullptr);
     const S* Lp = L + 36 * (size_t)p;
-    S c2 = 0;
     for (int i = 0; i < 6; ++i) {
       S ri = 0;
 #pragma unroll
       for (int k = 0; k < 6; ++k) ri += Lp[6 * i + k] * e[k];
-      c2 += ri * ri;
+      f(i, ri);
     }
+  }
+  __device__ S sq_norm(int p) const {
+    S c2 = 0;
+    rows_of(p, [&](int, S ri) { c2 += ri * ri; });
     return c2;
   }
   __device__ S model_change(const S* inc, int p) const {

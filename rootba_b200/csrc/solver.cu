@@ -79,6 +79,8 @@ struct rba_handle {
   virtual int set_intrinsics_groups(const int32_t* group) = 0;
   virtual int set_observation_info(const void* sqrt_info) = 0;
   virtual int set_observation_loss(const uint8_t* kind, const void* scale) = 0;
+  virtual int set_prior_loss(int32_t prior_kind, int32_t num, const uint8_t* kind, const void* scale) = 0;
+  virtual int get_prior_residuals(int32_t prior_kind, void* residual, void* robust_weight) = 0;
   virtual int get_observation_residuals(void* residual, void* robust_weight, uint8_t* flags) = 0;
   virtual int compute_error(rba_residual_info* out) = 0;
   virtual int linearize() = 0;
@@ -201,8 +203,16 @@ struct Solver : rba_handle {
     DeviceBuffer<uint8_t> flags;   // [nc]
     bool all = false;              // no free camera parameter: the reduced system is empty and its solve is skipped
   } held;
+  // The robust losses of one prior kind (rba_set_prior_loss, DESIGN.md section 22), owned by its term: on while an item of the
+  // term has a loss other than NONE.  The setters of the kind clear them (on = false).
+  struct PriorLoss {
+    bool on = false;
+    DeviceBuffer<S> rec;           // the loss records of the term's n items (loss_records layout, read by slot_loss)
+    DeviceBuffer<S> Lw;            // sqrt(w) L of the last linearisation (k_prior_weight), read in place of L
+  };
   struct CameraPriorTerm {         // rba_set_camera_prior, DESIGN.md section 14; D.prior_H = H while there are absolute or pair priors
     bool on = false;               // any L_c is non-zero
+    PriorLoss loss;                // item = camera
     DeviceBuffer<S> mean;          // [nc][10] mean, quaternion normalised
     DeviceBuffer<S> L;             // [nc][81] square-root information
     DeviceBuffer<S> A;             // [nc][81] L de/d(inc): unscaled after k_prior_linearize, scaled after k_prior_scale
@@ -213,6 +223,8 @@ struct Solver : rba_handle {
   } cprior;
   struct PairPriorTerm {           // rba_set_camera_pair_prior, DESIGN.md section 15; D.pair_ov set while n > 0
     int n = 0;                     // pairs with a non-zero L (m: the capacity)
+    std::vector<int> item_of;      // [num_pairs of the last call] the pair's index among the n, -1 = dropped (all-zero L)
+    PriorLoss loss;
     DeviceBuffer<int> ij;          // [m][2] cameras (i, j)
     DeviceBuffer<S> mean;          // [m][7] R0 quaternion (normalised), t0
     DeviceBuffer<S> L;             // [m][36] square-root information
@@ -228,6 +240,8 @@ struct Solver : rba_handle {
   } pprior;
   struct LandmarkPriorTerm {       // rba_set_landmark_prior, DESIGN.md section 17; D.lmp_slot set while n > 0
     int n = 0;                     // priors of this shard with a non-zero L (m: the capacity)
+    std::vector<int> item_of;      // [num of the last call] the prior's index among the n, -1 = dropped (all-zero L), -2 = other shard
+    PriorLoss loss;
     DeviceBuffer<int> slot;        // [nsorted] prior slot per sorted landmark, -1 = none
     DeviceBuffer<int> of_lm;       // [nl_local] prior slot per local landmark, -1 = none (rba_compute_covariance)
     DeviceBuffer<int> lm;          // [m] local landmark of each prior
@@ -614,6 +628,10 @@ struct Solver : rba_handle {
     return obsw ? (obsl ? k_cov_landmark<S, LMP, true, true> : k_cov_landmark<S, LMP, true>)
                 : (obsl ? k_cov_landmark<S, LMP, false, true> : k_cov_landmark<S, LMP>);
   }
+  static auto kcov_lmpl(bool obsw, bool obsl) {  // + LMPL: the landmark priors' losses (section 22)
+    return obsw ? (obsl ? k_cov_landmark<S, true, true, true, true> : k_cov_landmark<S, true, true, false, true>)
+                : (obsl ? k_cov_landmark<S, true, false, true, true> : k_cov_landmark<S, true, false, false, true>);
+  }
 
   int setup_kernels() {
     if (k1_sc.gstride) TRY(dalloc(&k1_sc.gbase, (size_t)(k1_max_blocks * TILE_WARPS) * k1_sc.gstride, false));
@@ -910,6 +928,7 @@ struct Solver : rba_handle {
       cprior.adopt(next);
     }
     cprior.on = any;
+    cprior.loss.on = false;
     return priors_changed();
   }
   // The checks of every prior setter on one prior, in this order: a finite mean (nm entries), a finite sqrt_info (nL
@@ -935,6 +954,25 @@ struct Solver : rba_handle {
   }
   CameraPrior<S> camera_prior() const { return {D.cams, cprior.mean.get(), cprior.L.get(), cprior.A.get(), cprior.r.get()}; }
   PairPrior<S> pair_prior() const { return {D.cams, pprior.ij.get(), pprior.mean.get(), pprior.L.get(), pprior.A.get(), pprior.r.get()}; }
+  LandmarkPrior<S> landmark_prior() const { return {D.lms, lprior.lm.get(), lprior.mean.get(), lprior.L.get()}; }
+  // The cost of the n items of one prior kind into the error sums (k_prior_cost): rho(s)/2 of their losses while `loss` is on
+  // (section 22), else 1/2 s
+  template <class K>
+  int prior_cost(K k, int n, const PriorLoss& loss) {
+    if (loss.on) k_prior_cost<<<1, 256, 0, stream>>>(RobustPrior<K>{k, loss.rec.get(), n}, n, d_red, d_flags);
+    else k_prior_cost<<<1, 256, 0, stream>>>(k, n, d_red, d_flags);
+    ++launches;
+    return RBA_OK;
+  }
+  // Before the kernels of a linearisation read a prior kind's L: sqrt(w) L into loss.Lw while its losses are on (section 22).
+  // Returns the L those kernels read.
+  template <class K>
+  const S* weighted_L(K k, int n, PriorLoss& loss) {
+    if (!loss.on) return k.L;
+    k_prior_weight<<<(n + 127) / 128, 128, 0, stream>>>(RobustPrior<K>{k, loss.rec.get(), n}, loss.Lw.get());
+    ++launches;
+    return loss.Lw.get();
+  }
   // The kernels' optional pointers, from the problem terms (nullptr = the kernels without the term)
   void point_at_terms() {
     D.cam_fixed = held.host.empty() ? nullptr : held.flags.get();
@@ -942,7 +980,10 @@ struct Solver : rba_handle {
     D.pair_ptr = pprior.ptr.get(); D.pair_nbr = pprior.nbr.get(); D.pair_O = pprior.O.get();
     D.pair_ov = pprior.n > 0 ? pprior.ov.get() : nullptr;
     D.lmp_slot = lprior.n > 0 ? lprior.slot.get() : nullptr;
-    D.lmp_mean = lprior.mean.get(); D.lmp_L = lprior.L.get(); D.lmp_Lg = lprior.Lg.get();
+    D.lmp_mean = lprior.mean.get(); D.lmp_Lg = lprior.Lg.get();
+    // losses on the landmark priors (section 22): the kernels that read L take sqrt(w) L
+    D.lmp_L = lprior.loss.on ? lprior.loss.Lw.get() : lprior.L.get();
+    D.lmp_Lu = lprior.L.get(); D.lmp_loss = lprior.loss.on ? lprior.loss.rec.get() : nullptr; D.lmp_n = lprior.n;
     D.obs_W = obs.on ? obs.W.get() : nullptr;
     D.obs_loss = obs.loss_on ? obs.loss.get() : nullptr;
   }
@@ -963,7 +1004,7 @@ struct Solver : rba_handle {
     if (num_pairs > 0 && (!pairs || !mean_v || !sqrt_info_v)) return bad("pairs, mean and sqrt_info must be given when num_pairs > 0");
     const S* m = (const S*)mean_v;
     const S* Ls = (const S*)sqrt_info_v;
-    std::vector<int> ij;
+    std::vector<int> ij, item_of((size_t)std::max(num_pairs, 0), -1);
     std::vector<S> mean, Lsq;
     for (int p = 0; p < num_pairs; ++p) {
       const int i = pairs[2 * p], j = pairs[2 * p + 1];
@@ -975,6 +1016,7 @@ struct Solver : rba_handle {
       const std::string why = check_prior(m + 7 * (size_t)p, 7, Ls + 36 * (size_t)p, 36, nonzero, q);
       if (!why.empty()) return bad(tag + " " + why);
       if (!nonzero) continue;
+      item_of[p] = (int)(ij.size() / 2);
       ij.push_back(i); ij.push_back(j);
       mean.insert(mean.end(), q, q + 4);
       mean.insert(mean.end(), m + 7 * (size_t)p + 4, m + 7 * (size_t)(p + 1));
@@ -1003,6 +1045,8 @@ struct Solver : rba_handle {
       pprior.adopt(next); cprior.adopt(diag);
     }
     pprior.n = np;
+    pprior.item_of = std::move(item_of);
+    pprior.loss.on = false;
     return priors_changed();
   }
 
@@ -1017,7 +1061,7 @@ struct Solver : rba_handle {
     const S* m = (const S*)mean_v;
     const S* Ls = (const S*)sqrt_info_v;
     std::vector<uint8_t> seen((size_t)nl_total, 0);
-    std::vector<int> slot(L.sorted_lm.size(), -1), of_lm((size_t)L.nl_local, -1), lm;
+    std::vector<int> slot(L.sorted_lm.size(), -1), of_lm((size_t)L.nl_local, -1), lm, item_of((size_t)std::max(num, 0), -1);
     std::vector<S> mean, Lsq;
     for (int p = 0; p < num; ++p) {
       const int l = idx[p];
@@ -1028,8 +1072,10 @@ struct Solver : rba_handle {
       bool nonzero;
       const std::string why = check_prior(m + 3 * (size_t)p, 3, Ls + 9 * (size_t)p, 9, nonzero);
       if (!why.empty()) return bad(tag + " " + why);
+      if (l < L.lm_begin || l >= L.lm_end) item_of[p] = -2;
       if (!nonzero || l < L.lm_begin || l >= L.lm_end) continue;
       const int q = (int)lm.size();
+      item_of[p] = q;
       lm.push_back(l - L.lm_begin);
       slot[L.sorted_of_lm[l - L.lm_begin]] = q;
       of_lm[l - L.lm_begin] = q;
@@ -1046,6 +1092,8 @@ struct Solver : rba_handle {
       lprior.adopt(next);
     }
     lprior.n = np;
+    lprior.item_of = std::move(item_of);
+    lprior.loss.on = false;
     return priors_changed();
   }
 
@@ -1084,6 +1132,25 @@ struct Solver : rba_handle {
   // Scalars of the loss records of nslots slots (D.obs_loss): float {scale, uint32 kind} per slot; double the scales, then
   // one uint8 kind per slot, rounded up to whole doubles
   static size_t loss_records(int nslots) { return sizeof(S) == 4 ? 2 * (size_t)nslots : (size_t)nslots + ((size_t)nslots + 7) / 8; }
+  // record s of the nslots records in rec (loss_records layout); NONE ignores its scale
+  static void put_loss(std::vector<S>& rec, int nslots, size_t s, uint8_t k, S a) {
+    const S sc = k == RBA_LOSS_NONE ? S(0) : a;
+    if constexpr (sizeof(S) == 4) {
+      const uint32_t k32 = k;
+      rec[2 * s] = sc;
+      std::memcpy(&rec[2 * s + 1], &k32, 4);
+    } else {
+      rec[s] = sc;
+      reinterpret_cast<uint8_t*>(rec.data() + nslots)[s] = k;
+    }
+  }
+  // The checks of rba_set_observation_loss and rba_set_prior_loss on one entry: why it is rejected ("" = accepted)
+  static std::string check_loss(uint8_t kind, S a) {
+    if (kind > RBA_LOSS_TUKEY) return "has kind " + std::to_string(kind) + " (must be 0..4)";
+    if (kind != RBA_LOSS_NONE && !(std::isfinite((double)a) && a > S(0)))
+      return "has the scale " + std::to_string((double)a) + " (must be finite and > 0)";
+    return "";
+  }
   // A robust loss (RBA_LOSS_*, scale) per observation of the full problem (DESIGN.md section 21).  Part of the linearisation
   // like the observation information, and landmark-owned like it: every rank receives the full arrays and keeps its own
   // shard's slots.  NULL, or the handle's own choice (robust_norm, huber_parameter) on every observation of the shard, = the
@@ -1097,9 +1164,8 @@ struct Solver : rba_handle {
     std::vector<S> rec;
     if (kind) {
       for (long long o = 0; o < nobs_total; ++o) {
-        if (kind[o] > RBA_LOSS_TUKEY) return bad("observation " + std::to_string(o) + " has kind " + std::to_string(kind[o]) + " (must be 0..4)");
-        if (kind[o] != RBA_LOSS_NONE && !(std::isfinite((double)a[o]) && a[o] > S(0)))
-          return bad("observation " + std::to_string(o) + " has the scale " + std::to_string((double)a[o]) + " (must be finite and > 0)");
+        const std::string why = check_loss(kind[o], a[o]);
+        if (!why.empty()) return bad("observation " + std::to_string(o) + " " + why);
       }
       const uint8_t own = opt.robust_norm == 1 ? RBA_LOSS_HUBER : RBA_LOSS_NONE;
       const S own_a = (S)opt.huber_parameter;
@@ -1108,16 +1174,8 @@ struct Solver : rba_handle {
         const long long o = L.slot_obs[s];
         if (o < 0) continue;
         const uint8_t k = kind[o];
-        const S sc = k == RBA_LOSS_NONE ? S(0) : a[o];  // NONE ignores its scale
-        any = any || k != own || (k == RBA_LOSS_HUBER && sc != own_a);
-        if constexpr (sizeof(S) == 4) {
-          const uint32_t k32 = k;
-          rec[2 * (size_t)s] = sc;
-          std::memcpy(&rec[2 * (size_t)s + 1], &k32, 4);
-        } else {
-          rec[s] = sc;
-          reinterpret_cast<uint8_t*>(rec.data() + L.nslots)[s] = k;
-        }
+        any = any || k != own || (k == RBA_LOSS_HUBER && a[o] != own_a);
+        put_loss(rec, L.nslots, (size_t)s, k, a[o]);
       }
     }
     if (any) {
@@ -1128,6 +1186,87 @@ struct Solver : rba_handle {
     obs.loss_on = any;
     su_valid = s_valid = false;  // the assembled matrix belongs to the previous rows
     return priors_changed();
+  }
+  // One prior kind's term as rba_set_prior_loss and rba_get_prior_residuals see it: its loss, its n items, the entries of a
+  // row of L (nr) and the caller's entries (num) with their items (item(p): >= 0 the item, -1 dropped, -2 other shard)
+  struct PriorKindView {
+    PriorLoss* loss;
+    int n, nr, num;
+    const std::vector<int>* item_of;  // nullptr = the cameras: item p = camera p while there are camera priors
+    int item(int p, bool on) const { return item_of ? (*item_of)[p] : on ? p : -1; }
+  };
+  PriorKindView prior_kind_view(int32_t k) {
+    if (k == RBA_PRIOR_CAMERA) return {&cprior.loss, cprior.on ? nc : 0, 9, nc, nullptr};
+    if (k == RBA_PRIOR_PAIR) return {&pprior.loss, pprior.n, 6, (int)pprior.item_of.size(), &pprior.item_of};
+    return {&lprior.loss, lprior.n, 3, (int)lprior.item_of.size(), &lprior.item_of};
+  }
+  // A robust loss per prior of one kind, in the caller's order of its setter (DESIGN.md section 22).  Part of the
+  // linearisation like the priors.  NULL, or NONE on every prior, = the unmodified kernels.  Every check runs before anything
+  // changes, so a rejected call leaves the previous losses.
+  int set_prior_loss(int32_t which, int32_t num, const uint8_t* kind, const void* scale_v) override {
+    auto bad = [&](const std::string& what) { g_err = "rba_set_prior_loss: " + what; return RBA_ERR_INVALID_ARGUMENT; };
+    if (which != RBA_PRIOR_CAMERA && which != RBA_PRIOR_PAIR && which != RBA_PRIOR_LANDMARK)
+      return bad("prior_kind must be RBA_PRIOR_CAMERA, RBA_PRIOR_PAIR or RBA_PRIOR_LANDMARK, got " + std::to_string(which));
+    const PriorKindView v = prior_kind_view(which);
+    if (num != v.num)
+      return bad("num is " + std::to_string(num) + ", but this prior kind has " + std::to_string(v.num) +
+                 (which == RBA_PRIOR_CAMERA ? " cameras" : " entries in the last call of its setter"));
+    if (!kind != !scale_v) return bad("kind and scale must both be given or both be NULL");
+    const S* a = (const S*)scale_v;
+    bool any = false;
+    std::vector<S> rec(loss_records(v.n), S(0));
+    if (kind) {
+      for (int p = 0; p < num; ++p) {
+        const std::string why = check_loss(kind[p], a[p]);
+        if (!why.empty()) return bad("prior " + std::to_string(p) + " " + why);
+      }
+      for (int p = 0; p < num; ++p) {
+        const int q = v.item(p, true);
+        if (q < 0 || q >= v.n) continue;
+        put_loss(rec, v.n, (size_t)q, kind[p], a[p]);
+        any = any || kind[p] != RBA_LOSS_NONE;
+      }
+    }
+    if (any) {
+      DeviceBuffer<S> next_rec, next_Lw;
+      TRY(fit(next_rec, v.loss->rec, rec.size(), &rec)); TRY(fit(next_Lw, v.loss->Lw, (size_t)v.nr * v.nr * v.n));
+      CU(cudaStreamSynchronize(stream));
+      v.loss->rec.take(next_rec); v.loss->Lw.take(next_Lw);
+    }
+    v.loss->on = any;
+    return priors_changed();
+  }
+  // Per prior of one kind at the current state, in the caller's order (DESIGN.md section 22): L e and w.  Nothing of the
+  // handle changes: the scratch is allocated for the call and freed before it returns.
+  int get_prior_residuals(int32_t which, void* residual, void* robust_weight) override {
+    auto bad = [&](const std::string& what) { g_err = "rba_get_prior_residuals: " + what; return RBA_ERR_INVALID_ARGUMENT; };
+    if (which != RBA_PRIOR_CAMERA && which != RBA_PRIOR_PAIR && which != RBA_PRIOR_LANDMARK)
+      return bad("prior_kind must be RBA_PRIOR_CAMERA, RBA_PRIOR_PAIR or RBA_PRIOR_LANDMARK, got " + std::to_string(which));
+    if (!residual && !robust_weight) return bad("residual and robust_weight are both NULL");
+    const PriorKindView v = prior_kind_view(which);
+    const size_t n = (size_t)v.n;
+    std::vector<S> res(v.nr * n), w(n);
+    if (n > 0) {
+      DeviceBuffer<S> scratch;  // per-call
+      TRY(alloc(scratch, (v.nr + 1) * n, false, false));
+      S* d_res = scratch.get(); S* d_w = d_res + v.nr * n;
+      const S* loss = v.loss->on ? v.loss->rec.get() : nullptr;
+      const unsigned grid = (unsigned)((n + 127) / 128);
+      if (which == RBA_PRIOR_CAMERA) k_prior_residuals<<<grid, 128, 0, stream>>>(camera_prior(), loss, v.n, d_res, d_w);
+      else if (which == RBA_PRIOR_PAIR) k_prior_residuals<<<grid, 128, 0, stream>>>(pair_prior(), loss, v.n, d_res, d_w);
+      else k_prior_residuals<<<grid, 128, 0, stream>>>(landmark_prior(), loss, v.n, d_res, d_w);
+      CU(cudaMemcpyAsync(res.data(), d_res, v.nr * n * sizeof(S), cudaMemcpyDeviceToHost, stream));
+      CU(cudaMemcpyAsync(w.data(), d_w, n * sizeof(S), cudaMemcpyDeviceToHost, stream));
+      CU(cudaStreamSynchronize(stream));
+      CU(cudaGetLastError());
+    }
+    for (int p = 0; p < v.num; ++p) {
+      const int q = v.item(p, v.n > 0);
+      if (q == -2) continue;  // a landmark prior of another shard
+      for (int i = 0; i < v.nr; ++i) if (residual) ((S*)residual)[(size_t)v.nr * p + i] = q < 0 ? S(0) : res[(size_t)v.nr * q + i];
+      if (robust_weight) ((S*)robust_weight)[p] = q < 0 ? S(1) : w[q];
+    }
+    return RBA_OK;
   }
   // Per observation at the current state, in problem order (DESIGN.md section 19).  Nothing of the handle changes: the
   // slot-ordered scratch is allocated for the call and freed before it returns.
@@ -1203,18 +1342,16 @@ struct Solver : rba_handle {
     ke<<<EBLOCKS, 256, 0, stream>>>(D, ko, d_epart, d_flags);
     k_sum_partials<6><<<1, 256, 0, stream>>>(d_epart, EBLOCKS, d_red);
     launches += 2;
+    // (each prior's cost is rho(|L e|^2)/2 of its loss while its kind has losses, DESIGN.md section 22)
     if (lprior.n > 0) {  // + this shard's landmark priors' 1/2 |L e|^2, BEFORE the sum over the shards (landmark-owned)
-      k_prior_cost<<<1, 256, 0, stream>>>(LandmarkPrior<S>{D.lms, lprior.lm.get(), lprior.mean.get(), lprior.L.get()}, lprior.n, d_red, d_flags);
-      ++launches;
+      rc = prior_cost(landmark_prior(), lprior.n, lprior.loss); if (rc) return rc;
     }
     rc = allreduce_scalars(6); if (rc) return rc;
     if (cprior.on) {  // + sum of 1/2 |L e|^2, once, after the sum over the shards
-      k_prior_cost<<<1, 256, 0, stream>>>(camera_prior(), nc, d_red, d_flags);
-      ++launches;
+      rc = prior_cost(camera_prior(), nc, cprior.loss); if (rc) return rc;
     }
     if (pprior.n > 0) {  // + the pair priors' 1/2 |L e|^2, likewise
-      k_prior_cost<<<1, 256, 0, stream>>>(pair_prior(), pprior.n, d_red, d_flags);
-      ++launches;
+      rc = prior_cost(pair_prior(), pprior.n, pprior.loss); if (rc) return rc;
     }
     CU(cudaMemcpyAsync(h_res->error, d_red, sizeof(h_res->error), cudaMemcpyDeviceToHost, stream));
     CU(cudaMemcpyAsync(h_res->error_flags, d_flags, sizeof(h_res->error_flags), cudaMemcpyDeviceToHost, stream));
@@ -1259,12 +1396,15 @@ struct Solver : rba_handle {
     kn<<<grid_for(L.nslots, 256, 8), 256, 0, stream>>>(D, ko, d_flags);
     ++launches;
     rc = camera_reduce(d_csr_obs_slots, d_csr_obs_items, n_obs_items, d_csr_obs_item_ptr, D.diag2); if (rc) return rc;
+    // (the priors' losses: sqrt(w) L in place of L, DESIGN.md section 22)
     if (cprior.on) {  // prior Jacobian and its column norms (scaling from the whole Jacobian), after the sum over the shards
-      k_prior_linearize<S><<<(nc + 127) / 128, 128, 0, stream>>>(D.cams, cprior.mean.get(), cprior.L.get(), nc, D.diag2, cprior.A.get(), cprior.r.get());
+      const S* Lc = weighted_L(camera_prior(), nc, cprior.loss);
+      k_prior_linearize<S><<<(nc + 127) / 128, 128, 0, stream>>>(D.cams, cprior.mean.get(), Lc, nc, D.diag2, cprior.A.get(), cprior.r.get());
       ++launches;
     }
     if (n_pairs > 0) {  // pair-prior blocks and their column norms, likewise
-      k_pair_linearize<S><<<(n_pairs + 127) / 128, 128, 0, stream>>>(D.cams, pprior.ij.get(), pprior.mean.get(), pprior.L.get(), n_pairs, pprior.A.get(), pprior.r.get());
+      const S* Lp = weighted_L(pair_prior(), n_pairs, pprior.loss);
+      k_pair_linearize<S><<<(n_pairs + 127) / 128, 128, 0, stream>>>(D.cams, pprior.ij.get(), pprior.mean.get(), Lp, n_pairs, pprior.A.get(), pprior.r.get());
       k_pair_diag2<S><<<(nc + 127) / 128, 128, 0, stream>>>(pprior.A.get(), pprior.ptr.get(), pprior.item.get(), nc, D.diag2);
       launches += 2;
     }
@@ -1277,6 +1417,7 @@ struct Solver : rba_handle {
     // (+ the landmark priors' column norms, L~ and g: the LMP instances; + the observation information: the OBSW instances;
     // + the observation losses: the OBSL instances).  ref: ipp:149-163 selects perform_qr_givens
     auto k1 = k1_instance(!opt.use_householder_marginalization, D.lmp_slot, D.obs_W, D.obs_loss);
+    if (lprior.n > 0) weighted_L(landmark_prior(), lprior.n, lprior.loss);  // into D.lmp_L while the losses are on
     k1<<<tile_grid(k1_max_blocks), TILE_WARPS * 32, k1_smem, stream>>>(D, ko, k1_sc, d_flags, order_k1);
     launches += 2;
     if (opt.preconditioner_type == 0 || opt.solver_type == 2) {
@@ -2034,13 +2175,17 @@ struct Solver : rba_handle {
     auto kcov = n_lmp > 0 ? (D.obs_W ? k_cov_landmark<S, true, true> : k_cov_landmark<S, true>)
                           : (D.obs_W ? k_cov_landmark<S, false, true> : k_cov_landmark<S>);
     if (D.obs_loss) kcov = n_lmp > 0 ? kcov_of<true>(D.obs_W, true) : kcov_of<false>(D.obs_W, true);
+    if (lprior.loss.on) kcov = kcov_lmpl(D.obs_W, D.obs_loss);  // LMPL: the landmark priors' losses (section 22)
     kcov<<<wgrid, 128, 0, stream>>>(D, ko, d_cov_lm_slot0, d_cov_lm_n, nl, jp, kb, wl, rk, n_lmp > 0 ? lprior.of_lm.get() : nullptr);
     k_cov_assemble<<<std::max(1, std::min((cov_nblk + 7) / 8, sm_count * 8)), 256, 0, stream>>>(
         (const int2*)d_cov_blk_cam, d_cov_blk_ptr, (const int2*)d_cov_terms, cov_nblk, jp, kb, A, np);
+    // LOSS: the camera and pair priors' losses (section 22), their weights re-evaluated in double at the current state
+    const bool prior_loss = cprior.loss.on || pprior.loss.on;
     if (cprior.on || pprior.n > 0)
-      k_cov_priors<S><<<(nc + 127) / 128, 128, 0, stream>>>(D.cams, nc, cprior.on ? cprior.mean.get() : nullptr, cprior.L.get(), pprior.ij.get(),
-                                                            pprior.mean.get(), pprior.L.get(), pprior.n > 0 ? pprior.ptr.get() : nullptr, pprior.item.get(),
-                                                            pprior.nbr.get(), A, np);
+      (prior_loss ? k_cov_priors<S, true> : k_cov_priors<S>)<<<(nc + 127) / 128, 128, 0, stream>>>(
+          D.cams, nc, cprior.on ? cprior.mean.get() : nullptr, cprior.L.get(), pprior.ij.get(), pprior.mean.get(), pprior.L.get(),
+          pprior.n > 0 ? pprior.ptr.get() : nullptr, pprior.item.get(), pprior.nbr.get(), A, np,
+          cprior.loss.on ? (const S*)cprior.loss.rec.get() : nullptr, pprior.loss.on ? (const S*)pprior.loss.rec.get() : nullptr, pprior.n);
     // intrinsics groups (DESIGN.md section 18): S_u = P^T S P, the members' entries 6..8 then held like the user's
     const uint8_t* held = D.cam_fixed;
     if (grp.n) {
@@ -2436,6 +2581,12 @@ int32_t rba_set_landmark_prior(rba_handle* h, int32_t num, const int32_t* lm_idx
 int32_t rba_set_intrinsics_groups(rba_handle* h, const int32_t* group) { return h->set_intrinsics_groups(group); }
 int32_t rba_set_observation_info(rba_handle* h, const void* sqrt_info) { return h->set_observation_info(sqrt_info); }
 int32_t rba_set_observation_loss(rba_handle* h, const uint8_t* kind, const void* scale) { return h->set_observation_loss(kind, scale); }
+int32_t rba_set_prior_loss(rba_handle* h, int32_t prior_kind, int32_t num, const uint8_t* kind, const void* scale) {
+  return h->set_prior_loss(prior_kind, num, kind, scale);
+}
+int32_t rba_get_prior_residuals(rba_handle* h, int32_t prior_kind, void* residual, void* robust_weight) {
+  return h->get_prior_residuals(prior_kind, residual, robust_weight);
+}
 int32_t rba_get_observation_residuals(rba_handle* h, void* residual, void* robust_weight, uint8_t* flags) {
   return h->get_observation_residuals(residual, robust_weight, flags);
 }

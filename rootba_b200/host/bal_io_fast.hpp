@@ -149,6 +149,13 @@ struct ProblemPriors {
   // Robust loss per observation (rba_set_observation_loss); both empty = the options' robust norm everywhere
   std::vector<uint8_t> obs_loss_kind;              // [nobs] RBA_LOSS_*
   std::vector<double> obs_loss_scale;              // [nobs] scale (inlier threshold in units of sigma; ignored for NONE)
+  // Robust loss per prior (rba_set_prior_loss), one entry per camera / pair / landmark prior in the order above; both empty = NONE
+  std::vector<uint8_t> camera_prior_loss_kind;     // [nc] RBA_LOSS_*
+  std::vector<double> camera_prior_loss_scale;     // [nc] threshold on |L e|
+  std::vector<uint8_t> camera_pair_prior_loss_kind;
+  std::vector<double> camera_pair_prior_loss_scale;
+  std::vector<uint8_t> landmark_prior_loss_kind;
+  std::vector<double> landmark_prior_loss_scale;
 };
 
 // Flat mirror of rootba::BalProblem<Scalar> with the member surface LinearizorQR / bundle_adjust_manual need.

@@ -218,6 +218,17 @@ class LinearizorQR {
       const VecX a(bp.obs_loss_scale.begin(), bp.obs_loss_scale.end());
       check(rba_set_observation_loss(h_, bp.obs_loss_kind.data(), a.data()));
     }
+    const struct { int32_t which; const std::vector<uint8_t>& kind; const std::vector<double>& scale; size_t num; const char* what; } prior_losses[] = {
+        {RBA_PRIOR_CAMERA, bp.camera_prior_loss_kind, bp.camera_prior_loss_scale, (size_t)bp.num_cameras(), "camera_prior_loss"},
+        {RBA_PRIOR_PAIR, bp.camera_pair_prior_loss_kind, bp.camera_pair_prior_loss_scale, bp.camera_pair_prior_pairs.size() / 2, "camera_pair_prior_loss"},
+        {RBA_PRIOR_LANDMARK, bp.landmark_prior_loss_kind, bp.landmark_prior_loss_scale, bp.landmark_prior_idx.size(), "landmark_prior_loss"}};
+    for (const auto& l : prior_losses) {
+      if (l.kind.empty() && l.scale.empty()) continue;
+      if (l.kind.size() != l.num || l.scale.size() != l.num)
+        throw std::runtime_error(std::string(l.what) + "_kind and _scale must have one entry per prior of the kind");
+      const VecX a(l.scale.begin(), l.scale.end());
+      check(rba_set_prior_loss(h_, l.which, (int32_t)l.num, l.kind.data(), a.data()));
+    }
   }
   Problem& bal_problem_;
   SolverSummary* summary_ = nullptr;

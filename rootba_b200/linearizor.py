@@ -172,40 +172,40 @@ def _observation_info_array(info, num_observations: int, dtype):
     return a
 
 
-def _observation_loss_arrays(loss, num_observations: int, dtype):
-    """None, or validated contiguous (kind [Nobs] uint8, scale [Nobs] in `dtype`) of per-observation robust losses given as
-    (kind, scale): kind a name of LOSS_KINDS, an RBA_LOSS_* int or an [Nobs] array of either, scale a scalar or [Nobs];
-    scalars are broadcast.  The checks of rba_set_observation_loss: a known kind, and a finite scale > 0 for every kind but
-    NONE (whose scale is ignored)."""
+def _loss_arrays(loss, num: int, dtype, name: str = "observation_loss"):
+    """None, or validated contiguous (kind [num] uint8, scale [num] in `dtype`) of robust losses given as (kind, scale): kind a
+    name of LOSS_KINDS, an RBA_LOSS_* int or a [num] array of either, scale a scalar or [num]; scalars are broadcast.  The
+    checks of rba_set_observation_loss and rba_set_prior_loss: a known kind, and a finite scale > 0 for every kind but NONE
+    (whose scale is ignored).  `name` names the losses in the messages."""
     if loss is None:
         return None
     try:
         kind, scale = loss
     except (TypeError, ValueError):
-        raise ValueError("observation_loss must be None or (kind, scale)") from None
+        raise ValueError(f"{name} must be None or (kind, scale)") from None
     k = np.asarray(kind)
     if k.dtype.kind in "US":
         names = [str(x).upper() for x in k.ravel()]
         bad = sorted(set(names) - set(_lib.LOSS_KINDS))
         if bad:
-            raise ValueError(f"observation_loss kind must be one of {sorted(_lib.LOSS_KINDS)}, got {bad}")
+            raise ValueError(f"{name} kind must be one of {sorted(_lib.LOSS_KINDS)}, got {bad}")
         k = np.array([_lib.LOSS_KINDS[n] for n in names], np.int64).reshape(k.shape)
     elif k.dtype.kind not in "iu":
-        raise ValueError(f"observation_loss kind must be names or integers, got dtype {k.dtype}")
+        raise ValueError(f"{name} kind must be names or integers, got dtype {k.dtype}")
     if k.ndim == 0:
-        k = np.full(num_observations, k)
-    if k.shape != (num_observations,):
-        raise ValueError(f"observation_loss kind must be a scalar or have shape ({num_observations},), got {k.shape}")
+        k = np.full(num, k)
+    if k.shape != (num,):
+        raise ValueError(f"{name} kind must be a scalar or have shape ({num},), got {k.shape}")
     if np.any((k < 0) | (k > _lib.LOSS_TUKEY)):
-        raise ValueError(f"observation_loss kinds must be in 0..{_lib.LOSS_TUKEY}")
+        raise ValueError(f"{name} kinds must be in 0..{_lib.LOSS_TUKEY}")
     a = np.array(scale, dtype=dtype, copy=True)
     if a.ndim == 0:
-        a = np.full(num_observations, a, dtype)
-    if a.shape != (num_observations,):
-        raise ValueError(f"observation_loss scale must be a scalar or have shape ({num_observations},), got {a.shape}")
+        a = np.full(num, a, dtype)
+    if a.shape != (num,):
+        raise ValueError(f"{name} scale must be a scalar or have shape ({num},), got {a.shape}")
     robust = k != _lib.LOSS_NONE
     if not np.all(np.isfinite(a[robust]) & (a[robust] > 0)):
-        raise ValueError("observation_loss scales must be finite and > 0 for every kind but NONE")
+        raise ValueError(f"{name} scales must be finite and > 0 for every kind but NONE")
     return np.ascontiguousarray(k, np.uint8), np.ascontiguousarray(a)
 
 
@@ -230,7 +230,11 @@ class BalProblem:
     `observation_loss` (not in the reference): None (every observation uses the options' robust_norm) or (kind, scale), a
     robust loss per observation: kind "NONE" | "HUBER" | "CAUCHY" | "SOFT_L1" | "TUKEY" (or RBA_LOSS_* ints), scale the inlier
     threshold in units of sigma, each a scalar (broadcast) or one entry per observation (rba_set_observation_loss, DESIGN.md
-    section 21).  Stored as (kind [Nobs] uint8, scale [Nobs]); forwarded likewise."""
+    section 21).  Stored as (kind [Nobs] uint8, scale [Nobs]); forwarded likewise.
+    `camera_prior_loss`, `camera_pair_prior_loss`, `landmark_prior_loss` (not in the reference): None (NONE on every prior of
+    that kind) or (kind, scale) as for observation_loss, one entry per camera / per pair / per landmark prior in the order of
+    the kind's prior (rba_set_prior_loss, DESIGN.md section 22): the prior's cost becomes rho(|L e|^2)/2.  Setting the kind's
+    prior clears its loss.  Forwarded likewise."""
 
     def __init__(self, cams, lms, lm_off, obs_cam, obs_xy, dtype=np.float64):
         self.dtype = np.dtype(dtype)
@@ -250,6 +254,46 @@ class BalProblem:
         self._intrinsics_group = None
         self._observation_sqrt_info = None
         self._observation_loss = None
+        self._prior_loss = {_lib.PRIOR_CAMERA: None, _lib.PRIOR_PAIR: None, _lib.PRIOR_LANDMARK: None}
+
+    def _prior_count(self, which: int) -> int:
+        """the entries of one prior kind's losses: the cameras, or the pairs / landmark priors of its prior (0 without one)"""
+        if which == _lib.PRIOR_CAMERA:
+            return self.num_cameras()
+        prior = self._camera_pair_prior if which == _lib.PRIOR_PAIR else self._landmark_prior
+        return 0 if prior is None else len(prior[0])
+
+    def _set_prior_loss(self, which: int, loss):
+        name = {_lib.PRIOR_CAMERA: "camera_prior_loss", _lib.PRIOR_PAIR: "camera_pair_prior_loss",
+                _lib.PRIOR_LANDMARK: "landmark_prior_loss"}[which]
+        ls = _loss_arrays(loss, self._prior_count(which), self.dtype, name)
+        if self._linearizor is not None:
+            self._linearizor._upload_prior_loss(which, ls)  # raises on rejection: the previous losses stay in force
+        self._prior_loss[which] = ls
+
+    @property
+    def camera_prior_loss(self):
+        return self._prior_loss[_lib.PRIOR_CAMERA]
+
+    @camera_prior_loss.setter
+    def camera_prior_loss(self, loss):
+        self._set_prior_loss(_lib.PRIOR_CAMERA, loss)
+
+    @property
+    def camera_pair_prior_loss(self):
+        return self._prior_loss[_lib.PRIOR_PAIR]
+
+    @camera_pair_prior_loss.setter
+    def camera_pair_prior_loss(self, loss):
+        self._set_prior_loss(_lib.PRIOR_PAIR, loss)
+
+    @property
+    def landmark_prior_loss(self):
+        return self._prior_loss[_lib.PRIOR_LANDMARK]
+
+    @landmark_prior_loss.setter
+    def landmark_prior_loss(self, loss):
+        self._set_prior_loss(_lib.PRIOR_LANDMARK, loss)
 
     @property
     def observation_loss(self):
@@ -257,7 +301,7 @@ class BalProblem:
 
     @observation_loss.setter
     def observation_loss(self, loss):
-        ls = _observation_loss_arrays(loss, self.num_observations(), self.dtype)
+        ls = _loss_arrays(loss, self.num_observations(), self.dtype)
         if self._linearizor is not None:
             self._linearizor._upload_observation_loss(ls)  # raises on rejection: the previous losses stay in force
         self._observation_loss = ls
@@ -294,6 +338,7 @@ class BalProblem:
         if self._linearizor is not None:
             self._linearizor._upload_landmark_prior(p)  # raises on rejection: the previous landmark priors stay in force
         self._landmark_prior = p
+        self._prior_loss[_lib.PRIOR_LANDMARK] = None  # the setter clears the kind's losses (rba_set_prior_loss)
 
     @property
     def camera_pair_prior(self):
@@ -305,6 +350,7 @@ class BalProblem:
         if self._linearizor is not None:
             self._linearizor._upload_camera_pair_prior(p)  # raises on rejection: the previous pair priors stay in force
         self._camera_pair_prior = p
+        self._prior_loss[_lib.PRIOR_PAIR] = None  # the setter clears the kind's losses (rba_set_prior_loss)
 
     @property
     def camera_prior(self):
@@ -316,6 +362,7 @@ class BalProblem:
         if self._linearizor is not None:
             self._linearizor._upload_camera_prior(p)  # raises on rejection: the previous priors stay in force
         self._camera_prior = p
+        self._prior_loss[_lib.PRIOR_CAMERA] = None  # the setter clears the kind's losses (rba_set_prior_loss)
 
     @property
     def camera_fixed(self):
@@ -441,6 +488,9 @@ class LinearizorQR:
             self._upload_observation_info(bal_problem.observation_sqrt_info)
         if bal_problem.observation_loss is not None:
             self._upload_observation_loss(bal_problem.observation_loss)
+        for which, loss in bal_problem._prior_loss.items():
+            if loss is not None:
+                self._upload_prior_loss(which, loss)
 
     # factory like Linearizor::create (linearizor.cpp:47-65)
     @staticmethod
@@ -538,6 +588,40 @@ class LinearizorQR:
             check(_lib.lib().rba_set_observation_loss(self.h, None, None))
         else:
             check(_lib.lib().rba_set_observation_loss(self.h, _p(loss[0]), _p(loss[1])))
+
+    @staticmethod
+    def _prior_kind(which) -> int:
+        if isinstance(which, str):
+            if which.lower() not in _lib.PRIOR_KINDS:
+                raise ValueError(f"prior kind must be one of {sorted(_lib.PRIOR_KINDS)}, got {which!r}")
+            return _lib.PRIOR_KINDS[which.lower()]
+        if which not in _lib.PRIOR_ROWS:
+            raise ValueError(f"prior kind must be one of {sorted(_lib.PRIOR_ROWS)} (RBA_PRIOR_*), got {which!r}")
+        return int(which)
+
+    def set_prior_loss(self, which, kind, scale=1.0):
+        """a robust loss per prior of one kind (rba_set_prior_loss): which "camera" | "pair" | "landmark" (or RBA_PRIOR_*
+        ints); kind None (NONE on every prior) or a name / RBA_LOSS_* int, scalar or one per camera / pair / landmark prior in
+        the order of the kind's prior; scale likewise, the threshold on |L e|.  Needs a new linearize before the next solve;
+        the losses are stored on the BalProblem."""
+        self.bal_problem._set_prior_loss(self._prior_kind(which), None if kind is None else (kind, scale))
+
+    def _upload_prior_loss(self, which: int, loss):
+        n = self.bal_problem._prior_count(which)
+        if loss is None:
+            check(_lib.lib().rba_set_prior_loss(self.h, which, n, None, None))
+        else:
+            check(_lib.lib().rba_set_prior_loss(self.h, which, n, _p(loss[0]), _p(loss[1])))
+
+    def prior_residuals(self, which):
+        """per prior of one kind at the current state, in the order of the kind's prior (rba_get_prior_residuals):
+        (residual [num, 9 | 6 | 3] = L e, robust_weight [num] = w of its loss).  A camera with an all-zero L or a dropped prior
+        gives 0 and 1; a sharded handle fills only the landmark priors of its own shard (the others stay 0)."""
+        k = self._prior_kind(which)
+        n = self.bal_problem._prior_count(k)
+        res, w = np.zeros((n, _lib.PRIOR_ROWS[k]), self.dtype), np.zeros(n, self.dtype)
+        check(_lib.lib().rba_get_prior_residuals(self.h, k, _p(res), _p(w)))
+        return res, w
 
     def observation_residuals(self):
         """per observation at the current state, in the order of the problem's observations (rba_get_observation_residuals):
