@@ -3,7 +3,7 @@
 
     python examples/solve_bal.py problem-49-7776-pre.txt [--float] [--max-num-iterations 20] [--operator-form DENSE|IMPLICIT]
         [--fix-intrinsics] [--fix-cameras I,J,...] [--camera-prior FILE.npz] [--camera-pair-prior FILE.npz]
-        [--landmark-prior FILE.npz] [--shared-intrinsics | --intrinsics-groups FILE.npy] [--covariance OUT.npz]
+        [--landmark-prior FILE.npz] [--shared-intrinsics | --intrinsics-groups FILE.npy] [--camera-rigs FILE.npz] [--covariance OUT.npz]
         [--relative-covariance PAIRS.npy] [--observation-info FILE.npy] [--observation-loss KIND:SCALE | FILE.npz]
         [--residuals OUT.npz] [--camera-prior-loss KIND:SCALE | FILE.npz] [--pair-prior-loss KIND:SCALE | FILE.npz]
         [--landmark-prior-loss KIND:SCALE | FILE.npz] [--prior-residuals OUT.npz]
@@ -66,6 +66,10 @@ def main():
     groups.add_argument("--intrinsics-groups", default=None, metavar="FILE.npy",
                         help="an int array [nc] of intrinsics group ids, -1 = the camera keeps its own; the cameras of a group "
                              "share one f, k1, k2, those of its lowest-index camera at the start (DESIGN.md section 18)")
+    ap.add_argument("--camera-rigs", default=None, metavar="FILE.npz",
+                    help="rigid camera rigs: arrays `rig` [nc] int (rig id, -1 = free camera) and `cam_from_rig` [nc, 7] "
+                         "(qx,qy,qz,qw, tx,ty,tz per camera, in the coordinates of the loaded (normalised) problem); every member "
+                         "is kept at its extrinsics relative to its rig's lowest-index camera (DESIGN.md section 23)")
     ap.add_argument("--covariance", default=None, metavar="OUT.npz",
                     help="after the solve, write the marginal covariances `cam` [nc, 9, 9] (tx,ty,tz, rx,ry,rz, f,k1,k2) and `lm` "
                          "[nl, 3, 3] at the final state (DESIGN.md section 16); the gauge must be fixed by priors or held "
@@ -153,6 +157,12 @@ def main():
             problem.intrinsics_group = np.load(args.intrinsics_groups)
         except ValueError as e:
             ap.error(f"--intrinsics-groups: {e}")
+    if args.camera_rigs:
+        with np.load(args.camera_rigs) as f:
+            try:
+                problem.camera_rig = (f["rig"], f["cam_from_rig"])
+            except ValueError as e:
+                ap.error(f"--camera-rigs: {e}")
     if args.observation_info:
         info = np.load(args.observation_info)
         nobs = problem.num_observations()

@@ -328,6 +328,40 @@ int32_t rba_set_landmark_prior(rba_handle* h, int32_t num, const int32_t* lm_idx
  * group's intrinsics covariance and its own pose-intrinsics cross terms, and the landmark blocks use the same matrix. */
 int32_t rba_set_intrinsics_groups(rba_handle* h, const int32_t* group);
 
+/* ---- Rigid camera rigs (DESIGN.md section 23) --------------------------------------------- */
+
+/* Not in the reference.  The cameras of a rigid multi-camera body (a stereo head, a vehicle's cameras, a spherical head)
+ * exposed together: one placement of the body is one rig.  Camera c of a rig has fixed extrinsics E_c = [R_e | t_e]
+ * (cam_from_rig) and pose T_c = E_c T_rig (world->camera, as in the state).
+ * rig [num_cameras of the full problem] int32: -1 = free camera; r >= 0 = rig id (any non-negative value below Nc).
+ * cam_from_rig [7*Nc] Scalar: qx,qy,qz,qw, tx,ty,tz of E_c (the entries of free cameras are ignored).  Both NULL = no rigs
+ * (the default).  A rig's lead is its lowest-index camera; a rig of one camera is a free camera, bit for bit.  Every rank
+ * of a sharded problem passes the same arrays.
+ * Every member j is kept at T_j = M_j T_lead, M_j = E_j E_lead^-1: the call sets the members' poses so (state and backup),
+ * and so does every later rba_set_state and every camera update of rba_apply / rba_lm_step / rba_lm_run (computed in
+ * double, rounded to Scalar), so rigs stay exactly rigid.  The solve gives the LM step of the tied problem (one pose per
+ * rig, every camera's own intrinsics): with x = P u, P mapping the rig's pose increment to member j through the adjoint
+ * A_j = [[R_m, [t_m]x R_m], [0, R_m]] of M_j = [R_m | t_m], (D_u P^T J^T J P D_u + lambda I) u = -D_u P^T J^T r, D_u the
+ * Jacobi scaling of the merged columns J P (the whole weighted Jacobian: observations, camera and pair priors), lambda
+ * once per rig pose parameter.  Combines with rba_set_intrinsics_groups (rigs tie entries 0..5, groups entries 6..8).
+ * A host increment given to rba_apply / rba_back_substitute has the members' pose entries replaced by D_j^-1 A_j D_lead
+ * times the lead's, so the increment rba_solve returns round-trips.
+ * rba_get_jacobian_scaling gives the per-camera scaling, unchanged; rba_get_rhs the contracted b (the members' pose
+ * entries 0); rba_get_preconditioner the inverse PCG uses (the lead's pose block from sum_j P~_j^T B_j P~_j, without the
+ * cross terms between members; the members' pose rows and columns 0); rba_right_multiply stays the full, untied operator;
+ * rba_compute_error is unchanged.
+ * After a call rba_solve returns RBA_ERR_STATE until the next rba_linearize; the device-resident increment and the cached
+ * error are discarded.
+ * Exactly one NULL pointer, an id outside [-1, Nc), a non-finite entry or a quaternion whose norm is not within 1e-3 of 1
+ * on a camera with an id, or RBA_FIX_POSE bits that differ between members of one rig (checked here and by
+ * rba_set_camera_fixed) -> RBA_ERR_INVALID_ARGUMENT, and the previous rigs (or flags) stay in force; so do they when an
+ * allocation fails.  A valid quaternion is normalised in double.  Rigs of >= 2 cameras with solver_type = 2
+ * (POWER_SCHUR_COMPLEMENT: Hpp of the tied problem is not block-diagonal) -> RBA_ERR_UNSUPPORTED.
+ * rba_compute_covariance and rba_compute_covariance_blocks give the covariance of the tied problem, P (P^T H P)^-1 P^T with
+ * the unscaled A_j: every member's block carries its rig's pose covariance mapped through A_j, and the relative-pose
+ * covariance of two members of one rig is 0 to rounding. */
+int32_t rba_set_camera_rigs(rba_handle* h, const int32_t* rig, const void* cam_from_rig);
+
 /* ---- Per-observation square-root information and residual read-back (DESIGN.md section 19) -- */
 
 /* Not in the reference, where every reprojection term has unit weight.  Observation o (index in the problem's CSR order, the

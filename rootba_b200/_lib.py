@@ -158,6 +158,7 @@ def lib():
         _lib.rba_set_observation_loss.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
         _lib.rba_set_prior_loss.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
         _lib.rba_get_prior_residuals.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]
+        _lib.rba_set_camera_rigs.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
     return _lib
 
 

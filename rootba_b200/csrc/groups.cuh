@@ -128,29 +128,33 @@ __global__ void __launch_bounds__(256) k_group_expand(const S* v, S* out, const 
   }
 }
 
-// out = P^T (y + A^T A ve + O ve): the camera-reduced operator output y = D.y of the expanded vector ve = P v, plus the
-// camera priors' and pair priors' terms of the full operator, contracted into the leads.  The vector step that follows
-// adds lambda v on the contracted v (lambda once per group) and runs without prior terms of its own.  Blocks [0, ncb):
-// thread per camera (pose rows, and every row of an ungrouped camera), blocks [ncb, ncb + ng): one per group (the lead's
-// rows 6..8 = the members' sum, the other members' 0).  The pair priors act on poses only, so rows 6..8 carry no pair term.
+// Row a of camera cam of the full operator at the expanded vector ve: the camera-reduced operator output y = D.y plus the
+// camera priors' and pair priors' terms.  The pair priors act on poses only, so rows 6..8 carry no pair term.
+template <class S>
+__device__ __forceinline__ S operator_row(const DevPtrs<S>& D, const S* __restrict__ ve, size_t cam, int a) {
+  S t = __ldcg(D.y + 9 * cam + a);
+  if (D.prior_H) {
+    const S* hr = D.prior_H + 81 * cam + 9 * a;
+    S h = 0;
+#pragma unroll
+    for (int k = 0; k < 9; ++k) h += hr[k] * ve[9 * cam + k];
+    t += h;
+  }
+  if (D.pair_ov && a < 6) t += pair_ov_entry(D, ve, (int)(9 * cam) + a);
+  return t;
+}
+
+// out = P^T (y + A^T A ve + O ve): the rows of the full operator at the expanded vector ve = P v (operator_row),
+// contracted into the leads.  The vector step that follows adds lambda v on the contracted v (lambda once per group) and
+// runs without prior terms of its own.  Blocks [0, ncb): thread per camera (pose rows, and every row of an ungrouped
+// camera), blocks [ncb, ncb + ng): one per group (the lead's rows 6..8 = the members' sum, the other members' 0).
 template <class S>
 __global__ void __launch_bounds__(GROUP_THREADS) k_group_contract(DevPtrs<S> D, const S* __restrict__ ve, S* __restrict__ out,
                                                                   GroupView G, int ncb, const PcgState* st) {
   asm volatile("griddepcontrol.wait;" ::: "memory");
   if (*reinterpret_cast<const volatile int*>(&st->done)) return;
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-  auto row = [&](size_t cam, int a) -> S {
-    S t = __ldcg(D.y + 9 * cam + a);
-    if (D.prior_H) {
-      const S* hr = D.prior_H + 81 * cam + 9 * a;
-      S h = 0;
-#pragma unroll
-      for (int k = 0; k < 9; ++k) h += hr[k] * ve[9 * cam + k];
-      t += h;
-    }
-    if (D.pair_ov && a < 6) t += pair_ov_entry(D, ve, (int)(9 * cam) + a);
-    return t;
-  };
+  auto row = [&](size_t cam, int a) -> S { return operator_row(D, ve, cam, a); };
   if ((int)blockIdx.x < ncb) {
     const int cam = blockIdx.x * GROUP_THREADS + threadIdx.x;
     if (cam >= D.nc) return;

@@ -20,7 +20,7 @@
 #include "kernels.cuh"
 #include "covariance.cuh"
 #include "assembled.cuh"
-#include "groups.cuh"
+#include "rigs.cuh"
 #include "nccl_dyn.hpp"
 
 namespace rba {
@@ -77,6 +77,7 @@ struct rba_handle {
   virtual int set_camera_pair_prior(int32_t num_pairs, const int32_t* pairs, const void* mean, const void* sqrt_info) = 0;
   virtual int set_landmark_prior(int32_t num, const int32_t* lm_idx, const void* mean, const void* sqrt_info) = 0;
   virtual int set_intrinsics_groups(const int32_t* group) = 0;
+  virtual int set_camera_rigs(const int32_t* rig, const void* cam_from_rig) = 0;
   virtual int set_observation_info(const void* sqrt_info) = 0;
   virtual int set_observation_loss(const uint8_t* kind, const void* scale) = 0;
   virtual int set_prior_loss(int32_t prior_kind, int32_t num, const uint8_t* kind, const void* scale) = 0;
@@ -256,6 +257,19 @@ struct Solver : rba_handle {
     DeviceBuffer<S> ve, y;         // [9 nc] the expanded operator input P v, the contracted output the vector step reads
     void adopt(GroupTerm& o) { lead.take(o.lead); ptr.take(o.ptr); mem.take(o.mem); fixed.take(o.fixed); ve.take(o.ve); y.take(o.y); }
   } grp;
+  struct RigTerm {                 // rba_set_camera_rigs, DESIGN.md section 23
+    int n = 0;                     // rigs of >= 2 cameras; 0 = the unmodified path
+    std::vector<int> host_lead;    // [nc] lead of the camera's rig, -1 = free camera (also a rig of one)
+    DeviceBuffer<int> lead, ptr, mem;  // new lists ({} to fit) at every call with rigs
+    DeviceBuffer<S> adj;           // [nc][36] A_j
+    DeviceBuffer<double> M;        // [nc][7] M_j = E_j E_lead^-1
+    DeviceBuffer<S> pt;            // [nc][36] P~_j of the last linearisation
+    DeviceBuffer<S> du;            // [nr][6] D_u of the last linearisation
+    DeviceBuffer<uint8_t> fixed;   // [nc] the user's flags + RBA_FIX_POSE on every member but the lead (+ the groups' bits)
+    DeviceBuffer<S> ve, y;         // [9 nc] the expanded operator input P~ v, the contracted output the vector step reads
+    void adopt(RigTerm& o) { lead.take(o.lead); ptr.take(o.ptr); mem.take(o.mem); adj.take(o.adj); M.take(o.M); pt.take(o.pt);
+                             du.take(o.du); fixed.take(o.fixed); ve.take(o.ve); y.take(o.y); }
+  } rig;
   struct ObservationTerm {
     bool on = false;               // rba_set_observation_info, DESIGN.md section 19: W [nslots][4] = D.obs_W while on
     DeviceBuffer<S> W;
@@ -757,6 +771,7 @@ struct Solver : rba_handle {
     }
     CU(cudaMemcpyAsync(D.cams, cams, (size_t)10 * nc * sizeof(S), cudaMemcpyHostToDevice, stream));
     CU(cudaMemcpyAsync(D.lms, (const S*)lms + (size_t)3 * L.lm_begin, (size_t)3 * L.nl_local * sizeof(S), cudaMemcpyHostToDevice, stream));
+    if (rig.n) TRY(rig_retie(D.cams));  // the members take M_j T_lead
     CU(cudaStreamSynchronize(stream));
     return RBA_OK;
   }
@@ -796,6 +811,10 @@ struct Solver : rba_handle {
       const std::string why = group_flags_mismatch(grp.host_lead, fl);
       if (!why.empty()) { g_err = "rba_set_camera_fixed: " + why; return RBA_ERR_INVALID_ARGUMENT; }
     }
+    if (rig.n) {
+      const std::string why = rig_flags_mismatch(rig.host_lead, fl);
+      if (!why.empty()) { g_err = "rba_set_camera_fixed: " + why; return RBA_ERR_INVALID_ARGUMENT; }
+    }
     if (any) {
       DeviceBuffer<uint8_t> next; TRY(fit(next, held.flags, (size_t)nc, &fl));
       CU(cudaStreamSynchronize(stream));
@@ -804,7 +823,7 @@ struct Solver : rba_handle {
     held.all = all;
     held.host = std::move(fl);
     point_at_terms();
-    if (grp.n) TRY(upload_group_fixed());
+    TRY(upload_tied_fixed());
     have_inc = false;  // the device-resident increment was solved under the previous flags
     return RBA_OK;
   }
@@ -850,8 +869,8 @@ struct Solver : rba_handle {
     }
     grp.n = ng;
     grp.host_lead = std::move(lead);
+    TRY(upload_tied_fixed());
     if (ng > 0) {
-      TRY(upload_group_fixed());
       // the current state and its backup take the tied values
       std::vector<S> c((size_t)10 * nc);
       for (S* d : std::initializer_list<S*>{D.cams, cams_bk}) {
@@ -880,19 +899,157 @@ struct Solver : rba_handle {
       if (grp.host_lead[c] >= 0 && grp.host_lead[c] != c)
         for (int k = 7; k < 10; ++k) cams[10 * (size_t)c + k] = cams[10 * (size_t)grp.host_lead[c] + k];
   }
-  // the flags k_precond_invert masks with: the user's, and the intrinsics of every member but the lead
-  int upload_group_fixed() {
+  // the flags k_precond_invert masks with while groups or rigs exist (grp.fixed, rig.fixed): the user's, the intrinsics of
+  // every group member but the lead and the pose of every rig member but the lead
+  int upload_tied_fixed() {
+    if (!grp.n && !rig.n) return RBA_OK;
     std::vector<uint8_t> f((size_t)nc, 0);
+    auto member = [](const std::vector<int>& lead, int c) { return !lead.empty() && lead[c] >= 0 && lead[c] != c; };
     for (int c = 0; c < nc; ++c)
-      f[c] = (uint8_t)((held.host.empty() ? 0 : held.host[c]) | (grp.host_lead[c] >= 0 && grp.host_lead[c] != c ? RBA_FIX_INTRINSICS : 0));
-    TRY(copy_in(grp.fixed.get(), f));
+      f[c] = (uint8_t)((held.host.empty() ? 0 : held.host[c]) | (grp.n && member(grp.host_lead, c) ? RBA_FIX_INTRINSICS : 0) |
+                       (rig.n && member(rig.host_lead, c) ? RBA_FIX_POSE : 0));
+    if (grp.n) TRY(copy_in(grp.fixed.get(), f));
+    if (rig.n) TRY(copy_in(rig.fixed.get(), f));
     CU(cudaStreamSynchronize(stream));
     return RBA_OK;
   }
+  const uint8_t* tied_fixed() const { return rig.n ? rig.fixed.get() : grp.fixed.get(); }
   GroupView groups() const { return {grp.lead.get(), grp.ptr.get(), grp.mem.get(), grp.n}; }
   int group_expand(const S* v, S* out, bool in_solve) {
     return launch_ex(k_group_expand<S>, (9 * nc + 255) / 256, 256, 0, in_solve, 1, v, out, (const int*)grp.lead.get(), nc,
                      in_solve ? (const PcgState*)d_state : (const PcgState*)nullptr);
+  }
+  // Rigid camera rigs (DESIGN.md section 23).  Every check runs before anything changes, and the new buffers are adopted
+  // once they all exist, so a rejected call leaves the previous rigs.  No rig of >= 2 cameras = the unmodified path (rig.n
+  // == 0).
+  int set_camera_rigs(const int32_t* rid, const void* cam_from_rig) override {
+    auto fail = [&](int rc, const std::string& what) { g_err = "rba_set_camera_rigs: " + what; return rc; };
+    if (!rid != !cam_from_rig) return fail(RBA_ERR_INVALID_ARGUMENT, "rig and cam_from_rig must both be given or both be NULL");
+    std::vector<int> lead((size_t)nc, -1), first((size_t)nc, -1), count((size_t)nc, 0);
+    std::vector<double> E((size_t)7 * nc, 0.0);  // the extrinsics of every rigged camera, quaternion normalised
+    if (rid) {
+      const S* e = (const S*)cam_from_rig;
+      for (int c = 0; c < nc; ++c) {
+        const int r = rid[c];
+        if (r < -1 || r >= nc)
+          return fail(RBA_ERR_INVALID_ARGUMENT, "camera " + std::to_string(c) + " has rig id " + std::to_string(r) + ", outside [-1, " + std::to_string(nc) + ")");
+        if (r < 0) continue;
+        if (count[r]++ == 0) first[r] = c;
+        double qn = 0;
+        for (int k = 0; k < 7; ++k) {
+          const double v = (double)e[7 * (size_t)c + k];
+          if (!std::isfinite(v)) return fail(RBA_ERR_INVALID_ARGUMENT, "camera " + std::to_string(c) + " has a non-finite cam_from_rig");
+          E[7 * (size_t)c + k] = v;
+          if (k < 4) qn += v * v;
+        }
+        qn = std::sqrt(qn);
+        if (!(std::fabs(qn - 1.0) <= 1e-3))
+          return fail(RBA_ERR_INVALID_ARGUMENT, "camera " + std::to_string(c) + " has a cam_from_rig quaternion of norm " + std::to_string(qn) + " (must be within 1e-3 of 1)");
+        for (int k = 0; k < 4; ++k) E[7 * (size_t)c + k] /= qn;
+      }
+      for (int c = 0; c < nc; ++c)
+        if (rid[c] >= 0 && count[rid[c]] >= 2) lead[c] = first[rid[c]];
+    }
+    // rigs in the order of their leads, members ascending (the lead first)
+    std::vector<int> ridx((size_t)nc, -1), ptr(1, 0), mem;
+    int nr = 0;
+    for (int c = 0; c < nc; ++c)
+      if (lead[c] == c) ridx[c] = nr++;
+    if (nr > 0 && opt.solver_type == 2)
+      return fail(RBA_ERR_UNSUPPORTED, "POWER_SCHUR_COMPLEMENT does not support rigs of >= 2 cameras (Hpp of the tied problem is not block-diagonal)");
+    const std::string why = rig_flags_mismatch(lead, held.host);
+    if (!why.empty()) return fail(RBA_ERR_INVALID_ARGUMENT, why);
+    ptr.assign((size_t)nr + 1, 0);
+    for (int c = 0; c < nc; ++c)
+      if (lead[c] >= 0) ++ptr[ridx[lead[c]] + 1];
+    for (int r = 0; r < nr; ++r) ptr[r + 1] += ptr[r];
+    mem.resize((size_t)ptr[nr]);
+    std::vector<int> fill(ptr.begin(), ptr.end() - 1);
+    for (int c = 0; c < nc; ++c)
+      if (lead[c] >= 0) mem[fill[ridx[lead[c]]]++] = c;
+    if (nr > 0) {
+      // M_j = E_j E_lead^-1 (q_j conj(q_lead), t_j - R_M t_lead) and its adjoint A_j = [[R_M, [t_M]x R_M], [0, R_M]]
+      std::vector<double> M((size_t)7 * nc, 0.0);
+      std::vector<S> adj((size_t)36 * nc, S(0));
+      for (int c = 0; c < nc; ++c) {
+        if (lead[c] < 0) continue;
+        const double* a = &E[7 * (size_t)c];
+        const double* l = &E[7 * (size_t)lead[c]];
+        const double b0 = -l[0], b1 = -l[1], b2 = -l[2], b3 = l[3];
+        double* m = &M[7 * (size_t)c];
+        m[3] = a[3] * b3 - a[0] * b0 - a[1] * b1 - a[2] * b2;
+        m[0] = a[3] * b0 + a[0] * b3 + a[1] * b2 - a[2] * b1;
+        m[1] = a[3] * b1 + a[1] * b3 + a[2] * b0 - a[0] * b2;
+        m[2] = a[3] * b2 + a[2] * b3 + a[0] * b1 - a[1] * b0;
+        const double qn = std::sqrt(m[0] * m[0] + m[1] * m[1] + m[2] * m[2] + m[3] * m[3]);
+        for (int k = 0; k < 4; ++k) m[k] /= qn;
+        const double x = m[0], y = m[1], z = m[2], w = m[3];
+        const double R[9] = {1 - 2 * (y * y + z * z), 2 * (x * y - z * w), 2 * (x * z + y * w),
+                             2 * (x * y + z * w), 1 - 2 * (x * x + z * z), 2 * (y * z - x * w),
+                             2 * (x * z - y * w), 2 * (y * z + x * w), 1 - 2 * (x * x + y * y)};
+        for (int r = 0; r < 3; ++r) m[4 + r] = a[4 + r] - (R[3 * r] * l[4] + R[3 * r + 1] * l[5] + R[3 * r + 2] * l[6]);
+        const double tx[9] = {0, -m[6], m[5], m[6], 0, -m[4], -m[5], m[4], 0};
+        S* A = &adj[36 * (size_t)c];
+        for (int r = 0; r < 3; ++r)
+          for (int k = 0; k < 3; ++k) {
+            double txr = 0;
+            for (int i = 0; i < 3; ++i) txr += tx[3 * r + i] * R[3 * i + k];
+            A[6 * r + k] = (S)R[3 * r + k];
+            A[6 * r + 3 + k] = (S)txr;
+            A[6 * (3 + r) + 3 + k] = (S)R[3 * r + k];
+          }
+        if (c == lead[c])  // exactly the identity
+          for (int k = 0; k < 36; ++k) A[k] = (k % 7 == 0) ? S(1) : S(0);
+      }
+      RigTerm next;
+      TRY(fit(next.lead, {}, lead.size(), &lead)); TRY(fit(next.ptr, {}, ptr.size(), &ptr)); TRY(fit(next.mem, {}, mem.size(), &mem));
+      TRY(fit(next.adj, {}, adj.size(), &adj)); TRY(fit(next.M, {}, M.size(), &M));
+      TRY(fit(next.du, rig.du, (size_t)6 * nr));
+      if (!rig.ve.get()) {
+        TRY(alloc(next.pt, (size_t)36 * nc, true)); TRY(alloc(next.fixed, (size_t)nc, true));
+        TRY(alloc(next.ve, (size_t)9 * nc, true)); TRY(alloc(next.y, (size_t)9 * nc, true));
+      }
+      CU(cudaStreamSynchronize(stream));
+      rig.adopt(next);
+    }
+    rig.n = nr;
+    rig.host_lead = std::move(lead);
+    TRY(upload_tied_fixed());
+    if (nr > 0) {  // the current state and its backup take the tied poses
+      TRY(rig_retie(D.cams)); TRY(rig_retie(cams_bk));
+      CU(cudaStreamSynchronize(stream));
+      ++state_version;
+    }
+    // the blocks and b of the last linearisation belong to the previous rigs
+    return priors_changed();
+  }
+  // "" when every rig's members agree on RBA_FIX_POSE, else which camera does not
+  std::string rig_flags_mismatch(const std::vector<int>& lead, const std::vector<uint8_t>& flags) const {
+    if (flags.empty()) return "";
+    for (int c = 0; c < nc; ++c)
+      if (lead[c] >= 0 && (flags[c] & RBA_FIX_POSE) != (flags[lead[c]] & RBA_FIX_POSE))
+        return "camera " + std::to_string(c) + " has the RBA_FIX_POSE bit " + std::to_string(flags[c] & RBA_FIX_POSE) +
+               " that differs from that of its rig's lead, camera " + std::to_string(lead[c]) + " (" + std::to_string(flags[lead[c]] & RBA_FIX_POSE) + ")";
+    return "";
+  }
+  RigView<S> rigs() const {
+    return {rig.lead.get(), rig.ptr.get(), rig.mem.get(), rig.adj.get(), rig.M.get(), rig.pt.get(), rig.du.get(), rig.n};
+  }
+  int rig_ncb() const { return (nc + GROUP_THREADS - 1) / GROUP_THREADS; }
+  int rig_retie(S* cams) {
+    k_rig_retie<S><<<(nc + 127) / 128, 128, 0, stream>>>(cams, rigs(), nc);
+    ++launches;
+    return RBA_OK;
+  }
+  int rig_expand(const S* v, S* out, bool in_solve, int host = 0) {
+    return launch_ex(k_rig_expand<S>, rig_ncb() + rig.n, GROUP_THREADS, 0, in_solve, 1, v, out, rigs(), nc, rig_ncb(), host,
+                     in_solve ? (const PcgState*)d_state : (const PcgState*)nullptr);
+  }
+  // inc = P~ u (and P u of the groups) for the back-substitution, the update and inc_out
+  int tie_expand(S* inc) {
+    if (rig.n) TRY(rig_expand(inc, inc, false));
+    if (grp.n) TRY(group_expand(inc, inc, false));
+    return RBA_OK;
   }
   // Gaussian priors on the camera parameters.  They are part of the linearisation (Jacobi scaling, A, r), so a change needs a
   // new rba_linearize; the device-resident increment and the cost cache are discarded.  No prior (both NULL, or every L_c
@@ -1435,6 +1592,14 @@ struct Solver : rba_handle {
                                                             cprior.H.get(), cprior.g.get(), jac ? D.jblocks : nullptr, pprior.O.get());
       launches += 2;
     }
+    if (rig.n) {
+      // (rigs: D_u from the per-camera Gram of the scaled rows and P~ of every member, DESIGN.md section 23.  The JACOBI blocks
+      // hold the observation Gram and the priors' H; with SCHUR_JACOBI they are unused, so they take the observation Gram
+      // here and the priors' H is added in k_rig_scaling)
+      if (!jac) { rc = precond_blocks(0, D.jblocks, nullptr, true); if (rc) return rc; }
+      k_rig_scaling<S><<<rig.n, GROUP_THREADS, 0, stream>>>(D.jblocks, jac ? nullptr : (const S*)D.prior_H, D, rigs(), (S)ko.jacobi_eps);
+      ++launches;
+    }
     if (panel_form()) {
       // rows 3..2n-1 of the Q2 panels do not change with lambda: their part of the gradient (ipp:443-466) and of the
       // SCHUR_JACOBI blocks (ipp:520-552) is accumulated once per linearisation (this shard only; the sum over the
@@ -1501,11 +1666,12 @@ struct Solver : rba_handle {
   // there), and Nccl before every application (the in-place all-reduce would carry the previous sum into the next).  The
   // others need no clear: k_rcs_spmv writes every camera, k_pcg_vec takes 0 for a camera without segments, and a peer
   // staging slot that is never written stays zero.
-  // With intrinsics groups the operator output is contracted (k_group_contract) between the reduction and the vector step,
-  // so it must exist as one vector: Partials and Peer, which sum the segments inside k_pcg_vec, give way to Counter / Nccl.
+  // With intrinsics groups or rigs the operator output is contracted (k_group_contract, k_rig_contract) between the
+  // reduction and the vector step, so it must exist as one vector: Partials and Peer, which sum the segments inside
+  // k_pcg_vec, give way to Counter / Nccl.
   Handover handover() const {
     if (s_valid) return Handover::Assembled;
-    if (grp.n) return opt.nranks > 1 ? Handover::Nccl : Handover::Counter;
+    if (grp.n || rig.n) return opt.nranks > 1 ? Handover::Nccl : Handover::Counter;
     if (opt.nranks > 1) return peer_ok ? Handover::Peer : Handover::Nccl;
     const bool vec_cached = 9 * ((nc + pcg_cluster - 1) / pcg_cluster) <= VEC_THREADS * VEC_EPT;
     return pcg_partials && vec_cached && opt.solver_type != 2 ? Handover::Partials : Handover::Counter;
@@ -1560,8 +1726,8 @@ struct Solver : rba_handle {
     PeerComm c = pc;
     if (!fused_ar) c.nranks = 1;
     DevPtrs<S> Dv = D;
-    if (grp.n) {  // the contracted output, which holds the prior terms already (k_group_contract)
-      Dv.y = grp.y.get(); Dv.prior_H = nullptr; Dv.pair_ov = nullptr;
+    if (grp.n || rig.n) {  // the contracted output, which holds the prior terms already (k_group_contract, k_rig_contract)
+      Dv.y = grp.n ? grp.y.get() : rig.y.get(); Dv.prior_H = nullptr; Dv.pair_ov = nullptr;
     }
     if (Dv.pair_ov && mode != 3) TRY(pair_ov(mode == 2 ? D.x : D.p, pdl));
     auto kern = Dv.pair_ov ? k_pcg_vec<S, true, true> : Dv.prior_H ? k_pcg_vec<S, true> : k_pcg_vec<S, false>;
@@ -1573,17 +1739,29 @@ struct Solver : rba_handle {
     return launch_ex(k_pair_ov<S>, (9 * nc + 255) / 256, 256, 0, pdl, 1, D, (const PcgState*)d_state, v);
   }
   // one operator application inside PCG (H v for v = p in mode 0/1, x in mode 2) and the vector step after it
-  // (intrinsics groups: H_u v = P^T H P v, with P v in grp.ve and P^T (H P v) in grp.y)
+  // (intrinsics groups: H_u v = P^T H P v, with P v in grp.ve and P^T (H P v) in grp.y; rigs: P~^T K P~ v likewise in rig.ve
+  // and rig.y; both: P~ v into rig.ve, P of it in place, the group contraction into grp.y and the rigs' in place there)
   int pcg_step(int i, int mode, int is_last, S lambda, Handover h) {
     const S* v = mode == 2 ? D.x : D.p;
+    if (rig.n) {
+      TRY(rig_expand(v, rig.ve.get(), true));
+      v = rig.ve.get();
+    }
     if (grp.n) {
-      TRY(group_expand(v, grp.ve.get(), true));
-      v = grp.ve.get();
+      S* ve = rig.n ? rig.ve.get() : grp.ve.get();
+      TRY(group_expand(v, ve, true));
+      v = ve;
     }
     TRY(apply_operator(v, h, true));
+    const bool pdl = h != Handover::Nccl;
     if (grp.n)
-      TRY(launch_ex(k_group_contract<S>, (nc + GROUP_THREADS - 1) / GROUP_THREADS + grp.n, GROUP_THREADS, 0, h != Handover::Nccl, 1,
-                    D, (const S*)grp.ve.get(), grp.y.get(), groups(), (nc + GROUP_THREADS - 1) / GROUP_THREADS, (const PcgState*)d_state));
+      TRY(launch_ex(k_group_contract<S>, (nc + GROUP_THREADS - 1) / GROUP_THREADS + grp.n, GROUP_THREADS, 0, pdl, 1,
+                    D, v, grp.y.get(), groups(), (nc + GROUP_THREADS - 1) / GROUP_THREADS, (const PcgState*)d_state));
+    if (rig.n) {
+      S* y = grp.n ? grp.y.get() : rig.y.get();
+      TRY(launch_ex(k_rig_contract<S>, rig_ncb() + rig.n, GROUP_THREADS, 0, pdl, 1, D, v, grp.n ? (const S*)y : (const S*)nullptr,
+                    y, rigs(), rig_ncb(), (const PcgState*)d_state));
+    }
     return pcg_vec(i, mode, h != Handover::Nccl, is_last, lambda, h == Handover::Peer, h == Handover::Partials);
   }
   // Enqueue iterations 1..last in chunks of `chunk` (enqueue(i)); after each chunk the PcgState is copied into one of two
@@ -1662,14 +1840,20 @@ struct Solver : rba_handle {
     // pose damping lambda*I added to the blocks, then explicit inverse (ref: linearization_qr.hpp:796-802, linearizor_qr.cpp:228-237)
     // (+ the masking of the held camera parameters, D.cam_fixed; + the camera priors: A^T A into the SCHUR_JACOBI blocks -- the
     // JACOBI blocks hold it already -- and A^T r into b, both after the sum over the shards and before the masking)
-    if (grp.n) {
-      // (intrinsics groups: the priors' terms, the contraction of b and the merged blocks first, into D.blocks; DESIGN.md
-      // section 18)
+    if (grp.n || rig.n) {
+      // (intrinsics groups, rigs: the priors' terms, the contraction of b and the merged blocks first, into D.blocks; DESIGN.md
+      // sections 18 and 23.  With both, the rigs' pass runs on the groups' output, whose priors' terms are in already)
       const int ncb = (nc + GROUP_THREADS - 1) / GROUP_THREADS, n_groups = grp.n;
-      k_group_precond<S><<<ncb + n_groups, GROUP_THREADS, 0, stream>>>(schur ? D.blocks : D.jblocks, schur ? (const S*)D.prior_H : nullptr,
-                                                                       D.prior_H ? (const S*)cprior.g.get() : nullptr, D.b, D.blocks, groups(), nc, ncb);
-      k_precond_invert<S><<<(nc + 63) / 64, 64, 0, stream>>>(D.blocks, lambda, nc, schur ? D.blocks : nullptr, D.inv, grp.fixed.get(), D.b);
-      launches += 2;
+      const S* src = schur ? D.blocks : D.jblocks;
+      const S* pH = schur ? (const S*)D.prior_H : nullptr;
+      const S* pg = D.prior_H ? (const S*)cprior.g.get() : nullptr;
+      if (grp.n) {
+        k_group_precond<S><<<ncb + n_groups, GROUP_THREADS, 0, stream>>>(src, pH, pg, D.b, D.blocks, groups(), nc, ncb);
+        src = D.blocks; pH = nullptr; pg = nullptr;
+      }
+      if (rig.n) k_rig_precond<S><<<ncb + rig.n, GROUP_THREADS, 0, stream>>>(src, pH, pg, D.b, D.blocks, rigs(), nc, ncb);
+      k_precond_invert<S><<<(nc + 63) / 64, 64, 0, stream>>>(D.blocks, lambda, nc, schur ? D.blocks : nullptr, D.inv, tied_fixed(), D.b);
+      launches += 1 + (grp.n > 0) + (rig.n > 0);
     } else {
       k_precond_invert<S><<<(nc + 63) / 64, 64, 0, stream>>>(schur ? D.blocks : D.jblocks, lambda, nc, schur ? D.blocks : nullptr, D.inv,
                                                              D.cam_fixed, D.b, schur ? (const S*)D.prior_H : nullptr,
@@ -1747,7 +1931,7 @@ struct Solver : rba_handle {
         rc = enqueue_iteration(i); if (rc) return rc;
       }
     }
-    if (grp.n) TRY(group_expand(D.inc, D.inc, false));  // inc = P u for the back-substitution, the update and inc_out
+    TRY(tie_expand(D.inc));  // inc = P u for the back-substitution, the update and inc_out
     CU(cudaMemcpyAsync(&h_state[0], d_state, sizeof(PcgState), cudaMemcpyDeviceToHost, stream));
     if (inc_out) CU(cudaMemcpyAsync(inc_out, D.inc, (size_t)9 * nc * sizeof(S), cudaMemcpyDeviceToHost, stream));
     rc = stop(ev_pcg); if (rc) return rc;
@@ -1796,7 +1980,9 @@ struct Solver : rba_handle {
         k_mask_fixed_inc<S><<<(9 * nc + 255) / 256, 256, 0, stream>>>(D.inc, D.cam_fixed, nc);
         ++launches;
       }
-      if (grp.n) TRY(group_expand(D.inc, D.inc, false));  // the members take the lead's f, k1, k2 entries
+      // the rig members take the lead's pose increment mapped through D_j^-1 A_j D_lead, the group members the lead's f, k1, k2
+      if (rig.n) TRY(rig_expand(D.inc, D.inc, false, 1));
+      if (grp.n) TRY(group_expand(D.inc, D.inc, false));
     } else if (!have_inc) { g_err = "no device-resident increment (none solved since rba_linearize or rba_set_camera_fixed)"; return RBA_ERR_STATE; }
     int rc = start(ev_backsub); if (rc) return rc;
     CU(cudaMemsetAsync(d_flags, 0, 4 * sizeof(int), stream));
@@ -1821,6 +2007,7 @@ struct Solver : rba_handle {
       // then rejects the step and restores the backup, so updating unconditionally is equivalent for the caller.
       k_camera_update<S><<<(nc + 127) / 128, 128, 0, stream>>>(D, D.inc);
       ++launches;
+      if (rig.n) TRY(rig_retie(D.cams));  // the members exactly at M_j T_lead: no drift over the iterations
     }
     rc = stop(ev_update); if (rc) return rc;
     CU(cudaMemcpyAsync(&h_res->l_diff, d_red, sizeof(double), cudaMemcpyDeviceToHost, stream));
@@ -2122,6 +2309,14 @@ struct Solver : rba_handle {
     CU(cudaGetLastError());
     return RBA_OK;
   }
+  // P^T A P (expand = 0) or P A P^T (expand = 1) of the rigs' adjoint map, in place (full; DESIGN.md section 23)
+  int cov_rig_passes(double* A, long long ld, long long n, int expand) {
+    k_cov_group_symmetrize<<<dim3((unsigned)((n + 31) / 32), (unsigned)((n + 7) / 8)), dim3(32, 8), 0, stream>>>(A, ld, n);
+    for (int columns = 0; columns < 2; ++columns)
+      k_cov_rig_pass<S><<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(A, ld, n, rigs(), columns, expand);
+    CU(cudaGetLastError());
+    return RBA_OK;
+  }
   // The dense inverse of one covariance call and what its extraction kernels read; the scratch is freed (after the kernels
   // have finished: cudaFree waits for them) when it goes out of scope.
   struct CovInverse {
@@ -2187,11 +2382,11 @@ struct Solver : rba_handle {
           pprior.n > 0 ? pprior.ptr.get() : nullptr, pprior.item.get(), pprior.nbr.get(), A, np,
           cprior.loss.on ? (const S*)cprior.loss.rec.get() : nullptr, pprior.loss.on ? (const S*)pprior.loss.rec.get() : nullptr, pprior.n);
     // intrinsics groups (DESIGN.md section 18): S_u = P^T S P, the members' entries 6..8 then held like the user's
+    // (rigs, section 23: S_u = P^T S P through the adjoints, the members' pose entries then held)
     const uint8_t* held = D.cam_fixed;
-    if (grp.n) {
-      TRY(cov_group_passes(A, np, n, 0));
-      held = grp.fixed.get();
-    }
+    if (rig.n) TRY(cov_rig_passes(A, np, n, 0));
+    if (grp.n) TRY(cov_group_passes(A, np, n, 0));
+    if (grp.n || rig.n) held = tied_fixed();
     k_cov_diag<<<(unsigned)((np + 255) / 256), 256, 0, stream>>>(A, np, n, np, held, d);
     k_cov_equil<<<dim3((unsigned)(np / 32), (unsigned)(np / 8)), dim3(32, 8), 0, stream>>>(A, np, n, np, held, d);
     // 3a. potrf, right-looking: factor the diagonal tile, panel <- panel L_kk^-T, trailing lower tiles -= panel panel^T
@@ -2238,6 +2433,13 @@ struct Solver : rba_handle {
       }
       k_cov_tile_lauu2<<<1, 256, 0, stream>>>(A, np, r0);
       if (kk > 0) cov_gemm<true, false>(TB, r0 + TB, kk, 1.0, A + (r0 + TB) + r0 * np, np, A + (r0 + TB), np, 1.0, A + r0, np, 0, 0);
+    }
+    // (rigs: the inverse un-equilibrated, then P S_u^-1 P^T through the adjoints with a unit equilibration)
+    if (rig.n) {
+      k_cov_group_symmetrize<<<dim3((unsigned)((n + 31) / 32), (unsigned)((n + 7) / 8)), dim3(32, 8), 0, stream>>>(A, np, n);
+      k_cov_unequil<<<dim3((unsigned)((n + 31) / 32), (unsigned)((n + 7) / 8)), dim3(32, 8), 0, stream>>>(A, np, n, d);
+      k_cov_unit_d<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(d, n);
+      TRY(cov_rig_passes(A, np, n, 1));
     }
     // (intrinsics groups: P S_u^-1 P^T, the members' rows and columns 6..8 and equilibration those of the lead)
     if (grp.n) {
@@ -2579,6 +2781,7 @@ int32_t rba_set_landmark_prior(rba_handle* h, int32_t num, const int32_t* lm_idx
   return h->set_landmark_prior(num, lm_idx, mean, sqrt_info);
 }
 int32_t rba_set_intrinsics_groups(rba_handle* h, const int32_t* group) { return h->set_intrinsics_groups(group); }
+int32_t rba_set_camera_rigs(rba_handle* h, const int32_t* rig, const void* cam_from_rig) { return h->set_camera_rigs(rig, cam_from_rig); }
 int32_t rba_set_observation_info(rba_handle* h, const void* sqrt_info) { return h->set_observation_info(sqrt_info); }
 int32_t rba_set_observation_loss(rba_handle* h, const uint8_t* kind, const void* scale) { return h->set_observation_loss(kind, scale); }
 int32_t rba_set_prior_loss(rba_handle* h, int32_t prior_kind, int32_t num, const uint8_t* kind, const void* scale) {

@@ -90,6 +90,30 @@ def _intrinsics_group_array(group, num_cameras: int):
     return np.ascontiguousarray(a, dtype=np.int32).copy()
 
 
+def _camera_rig_arrays(rig, num_cameras: int, dtype):
+    """None, or validated contiguous copies (rig [nc] int32, cam_from_rig [nc,7] in `dtype`) of camera rigs: one rig id per
+    camera (-1 = free camera, else an id in [0, num_cameras)) and each camera's extrinsics qx,qy,qz,qw, tx,ty,tz; a rigged
+    camera's entries must be finite with a quaternion within 1e-3 of unit norm (the free cameras' are ignored)"""
+    if rig is None:
+        return None
+    rid, e = rig
+    a = np.asarray(rid)
+    if a.shape != (num_cameras,):
+        raise ValueError(f"camera_rig ids must have one entry per camera ({num_cameras}), got shape {a.shape}")
+    if a.dtype.kind not in "iu" or np.any(a < -1) or np.any(a >= num_cameras):
+        raise ValueError(f"camera_rig ids must be integers in [-1, {num_cameras})")
+    e = np.array(e, dtype=dtype, order="C", copy=True)
+    if e.shape != (num_cameras, 7):
+        raise ValueError(f"camera_rig cam_from_rig must have shape ({num_cameras}, 7), got {e.shape}")
+    r = a >= 0
+    if not np.all(np.isfinite(e[r])):
+        raise ValueError("camera_rig cam_from_rig entries of rigged cameras must be finite")
+    qn = np.linalg.norm(e[r, :4].astype(np.float64), axis=1)
+    if np.any(np.abs(qn - 1.0) > 1e-3):
+        raise ValueError("camera_rig cam_from_rig quaternions must have norm 1 (within 1e-3)")
+    return np.ascontiguousarray(a, dtype=np.int32).copy(), e
+
+
 def _prior_arrays(name, mean, sqrt_info, dtype, m, mean_len, dim, check_index=None, item=None):
     """validated contiguous copies (mean [m, mean_len], sqrt_info [m, dim, dim]) in `dtype` of the priors `name`.  The checks
     run in this order: the shapes, the kind's own index checks (`check_index`), finiteness and, for a kind whose mean
@@ -223,6 +247,10 @@ class BalProblem:
     landmark positions with the cost 1/2 |L (x - x0)|^2 (rba_set_landmark_prior, DESIGN.md section 17).  Forwarded likewise.
     `intrinsics_group` (not in the reference): None or one int32 group id per camera (-1 = own intrinsics); the cameras of a
     group share one f, k1, k2 (rba_set_intrinsics_groups, DESIGN.md section 18).  Forwarded likewise.
+    `camera_rig` (not in the reference): None or (rig [nc] int32, cam_from_rig [nc,7]), rigid camera rigs: one rig id per
+    camera (-1 = free camera) and each camera's fixed extrinsics (qx,qy,qz,qw, tx,ty,tz of cam_from_rig); the cameras of a rig
+    keep the relative poses of their extrinsics and the solve moves one pose per rig (rba_set_camera_rigs, DESIGN.md section
+    23).  Forwarded likewise.
     `observation_sqrt_info` (not in the reference): None, [Nobs] (1 / sigma per observation) or [Nobs,2,2] (a square root W of
     the inverse keypoint covariance per observation, in the order of obs_cam / obs_xy); the observation's cost becomes
     rho(|W r|^2) and W = 0 switches it off (rba_set_observation_info, DESIGN.md section 19).  Stored as [Nobs,2,2]; forwarded
@@ -252,6 +280,7 @@ class BalProblem:
         self._camera_pair_prior = None
         self._landmark_prior = None
         self._intrinsics_group = None
+        self._camera_rig = None
         self._observation_sqrt_info = None
         self._observation_loss = None
         self._prior_loss = {_lib.PRIOR_CAMERA: None, _lib.PRIOR_PAIR: None, _lib.PRIOR_LANDMARK: None}
@@ -327,6 +356,17 @@ class BalProblem:
         if self._linearizor is not None:
             self._linearizor._upload_intrinsics_group(g)  # raises on rejection: the previous groups stay in force
         self._intrinsics_group = g
+
+    @property
+    def camera_rig(self):
+        return self._camera_rig
+
+    @camera_rig.setter
+    def camera_rig(self, rig):
+        r = _camera_rig_arrays(rig, self.num_cameras(), self.dtype)
+        if self._linearizor is not None:
+            self._linearizor._upload_camera_rig(r)  # raises on rejection: the previous rigs stay in force
+        self._camera_rig = r
 
     @property
     def landmark_prior(self):
@@ -484,6 +524,8 @@ class LinearizorQR:
             self._upload_landmark_prior(bal_problem.landmark_prior)
         if bal_problem.intrinsics_group is not None:
             self._upload_intrinsics_group(bal_problem.intrinsics_group)
+        if bal_problem.camera_rig is not None:
+            self._upload_camera_rig(bal_problem.camera_rig)
         if bal_problem.observation_sqrt_info is not None:
             self._upload_observation_info(bal_problem.observation_sqrt_info)
         if bal_problem.observation_loss is not None:
@@ -567,6 +609,18 @@ class LinearizorQR:
 
     def _upload_intrinsics_group(self, group):
         check(_lib.lib().rba_set_intrinsics_groups(self.h, None if group is None else _p(group)))
+
+    def set_camera_rigs(self, rig, cam_from_rig=None):
+        """rigid camera rigs (rba_set_camera_rigs): rig None, or one int32 rig id per camera (-1 = free camera) with
+        cam_from_rig [nc,7] (qx,qy,qz,qw, tx,ty,tz per camera).  The members take M_j T_lead; needs a new linearize before the
+        next solve.  The rigs are stored on the BalProblem."""
+        self.bal_problem.camera_rig = None if rig is None else (rig, cam_from_rig)  # validates, forwards to _upload_camera_rig
+
+    def _upload_camera_rig(self, rig):
+        if rig is None:
+            check(_lib.lib().rba_set_camera_rigs(self.h, None, None))
+        else:
+            check(_lib.lib().rba_set_camera_rigs(self.h, _p(rig[0]), _p(rig[1])))
 
     def set_observation_info(self, info):
         """per-observation square-root information (rba_set_observation_info): None, [Nobs] (1 / sigma) or [Nobs,2,2] in the
