@@ -3,7 +3,7 @@
 
     python examples/solve_bal.py problem-49-7776-pre.txt [--float] [--max-num-iterations 20] [--operator-form DENSE|IMPLICIT]
         [--fix-intrinsics] [--fix-cameras I,J,...] [--camera-prior FILE.npz] [--camera-pair-prior FILE.npz]
-        [--landmark-prior FILE.npz] [--shared-intrinsics | --intrinsics-groups FILE.npy] [--camera-rigs FILE.npz] [--covariance OUT.npz]
+        [--landmark-prior FILE.npz] [--shared-intrinsics | --intrinsics-groups FILE.npy] [--camera-rigs FILE.npz] [--rig-extrinsics OUT.npy] [--covariance OUT.npz]
         [--relative-covariance PAIRS.npy] [--observation-info FILE.npy] [--observation-loss KIND:SCALE | FILE.npz]
         [--residuals OUT.npz] [--camera-prior-loss KIND:SCALE | FILE.npz] [--pair-prior-loss KIND:SCALE | FILE.npz]
         [--landmark-prior-loss KIND:SCALE | FILE.npz] [--prior-residuals OUT.npz]
@@ -69,7 +69,12 @@ def main():
     ap.add_argument("--camera-rigs", default=None, metavar="FILE.npz",
                     help="rigid camera rigs: arrays `rig` [nc] int (rig id, -1 = free camera) and `cam_from_rig` [nc, 7] "
                          "(qx,qy,qz,qw, tx,ty,tz per camera, in the coordinates of the loaded (normalised) problem); every member "
-                         "is kept at its extrinsics relative to its rig's lowest-index camera (DESIGN.md section 23)")
+                         "is kept at its extrinsics relative to its rig's lowest-index camera (DESIGN.md section 23); an "
+                         "optional array `sensor` [nc] int (-1 = held extrinsics) names the physical camera of each capture, "
+                         "whose extrinsics are estimated and shared by its captures (DESIGN.md section 24)")
+    ap.add_argument("--rig-extrinsics", default=None, metavar="OUT.npy",
+                    help="with --camera-rigs: after the solve, write every camera's refined cam_from_rig [nc, 7] (held ones as "
+                         "given, estimated sensors' from the final state, free cameras the identity)")
     ap.add_argument("--covariance", default=None, metavar="OUT.npz",
                     help="after the solve, write the marginal covariances `cam` [nc, 9, 9] (tx,ty,tz, rx,ry,rz, f,k1,k2) and `lm` "
                          "[nl, 3, 3] at the final state (DESIGN.md section 16); the gauge must be fixed by priors or held "
@@ -161,6 +166,8 @@ def main():
         with np.load(args.camera_rigs) as f:
             try:
                 problem.camera_rig = (f["rig"], f["cam_from_rig"])
+                if "sensor" in f.files:
+                    problem.rig_sensor = f["sensor"]
             except ValueError as e:
                 ap.error(f"--camera-rigs: {e}")
     if args.observation_info:
@@ -186,7 +193,19 @@ def main():
                 ap.error(f"{flag}: {e}")
     options = rb.SolverOptions(max_num_iterations=args.max_num_iterations, preconditioner_type=args.preconditioner_type,
                                operator_form=args.operator_form, use_double=not args.float)
-    summary = rb.bundle_adjust_manual(problem, options, verbose=True)
+    if args.rig_extrinsics and problem.camera_rig is None:
+        ap.error("--rig-extrinsics needs --camera-rigs")
+    lin_ba = rb.LinearizorQR.create(problem, options) if args.rig_extrinsics else None
+    summary = rb.bundle_adjust_manual(problem, options, linearizor=lin_ba, verbose=True)
+    if lin_ba is not None:
+        extrinsics = lin_ba.rig_extrinsics()
+        lin_ba.close()
+        np.save(args.rig_extrinsics, extrinsics)
+        print("wrote", args.rig_extrinsics)
+        if problem.rig_sensor is not None:  # a later handle ties the sensors' captures to the refined extrinsics
+            sensor = problem.rig_sensor
+            problem.camera_rig = (problem.camera_rig[0], extrinsics)
+            problem.rig_sensor = sensor
     print(summary["termination_type"], summary["message"])
     rb.save_ba_log(args.log_path, summary, problem, args.input, {"load": t_load, "optimize": summary["total_time"]})
     print("wrote", args.log_path)

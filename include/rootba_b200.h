@@ -362,6 +362,43 @@ int32_t rba_set_intrinsics_groups(rba_handle* h, const int32_t* group);
  * covariance of two members of one rig is 0 to rounding. */
 int32_t rba_set_camera_rigs(rba_handle* h, const int32_t* rig, const void* cam_from_rig);
 
+/* ---- Estimated rig extrinsics (DESIGN.md section 24) ------------------------------------------ */
+
+/* Not in the reference.  Rig bundle adjustment: the extrinsics of a physical camera of the rigs ("sensor") are estimated,
+ * one cam_from_rig shared by every capture of that sensor and refined together with the rig poses and the landmarks.
+ * sensor [num_cameras of the full problem] int32: -1 = the camera's cam_from_rig (rba_set_camera_rigs) is held, as before;
+ * s >= 0 = camera c is a capture of sensor s (any non-negative value below Nc), whose extrinsics are estimated and shared by
+ * every camera with id s.  NULL = no sensors (the default): rigs behave bit for bit as in section 23.  Every rank of a
+ * sharded problem passes the same array.
+ * Lead: with sensors a rig's lead (it carries the rig's pose) is its lowest-index camera with held extrinsics.  A held
+ * member stays at T_j = M_j T_lead, M_j = E_j E_lead^-1.  Sensor s has a home, its lowest-index camera; the state defines
+ * its extrinsics as the home's pose relative to its lead, E_s = T_home T_lead(home)^-1 E_lead(home), and every other camera
+ * j of s is kept at T_j = E_s E_lead(j)^-1 T_lead(j) (computed in double, rounded to Scalar) after every camera update and
+ * at every rba_set_state.  The extrinsics live in the camera state, so rba_backup / rba_restore, rba_get_state /
+ * rba_set_state, rba_lm_step and rba_lm_run carry them unchanged.  The call re-ties every member from its (possibly new)
+ * lead: held members through the extrinsics given to rba_set_camera_rigs, every camera of sensor s through those of s's home.
+ * The solve gives the LM step of the tied problem J P with one pose per rig, one pose per sensor and every camera's own
+ * intrinsics (or its group's): a sensor camera moves by A_j d_lead + d_s, d_s the left increment of E_s in the state's
+ * convention (R' = Exp(w) R, t' = Exp(w) t + v) and A_j the adjoint of the current M_j; the Jacobi scaling is that of the
+ * merged columns (with the pair-prior cross terms between two cameras of one sensor), lambda once per sensor pose parameter.
+ * A pair prior between a rig's lead and a capture of an estimated sensor acts on that sensor's extrinsics: a way to feed a
+ * factory calibration with its uncertainty.  RBA_FIX_POSE on a rig holds the rig's pose; the captures of an estimated
+ * sensor still move with it (give them -1 to hold a sensor).
+ * rba_get_rhs / rba_get_preconditioner give the contracted vectors, the home's pose entries holding the sensor's;
+ * rba_right_multiply stays the full operator; a host increment's sensor entries are recovered from the home's and its
+ * lead's entries, so the increment rba_solve returns round-trips through rba_apply.  rba_compute_covariance and
+ * rba_compute_covariance_blocks give P (P^T H P)^-1 P^T for this P: the relative_cov of a lead and a capture of sensor s is
+ * the uncertainty of that calibration.
+ * After a call rba_solve returns RBA_ERR_STATE until the next rba_linearize.  An id outside [-1, Nc), an id on a camera
+ * that is not in a rig of >= 2 cameras, two cameras of one rig with the same id, or a rig in which every camera has an id
+ * -> RBA_ERR_INVALID_ARGUMENT, and the previous sensors stay in force; so do they when an allocation fails.  A later
+ * successful rba_set_camera_rigs clears the sensors. */
+int32_t rba_set_rig_sensors(rba_handle* h, const int32_t* sensor);
+/* cam_from_rig [7*Nc] Scalar: every rigged camera's current extrinsics in the convention rba_set_camera_rigs takes, so the
+ * output can be passed back in: held ones as given (normalised), a sensor's E_s from the current state; free cameras (and
+ * rigs of one) the identity.  Needs no rba_linearize and changes nothing of the handle; a sharded handle writes every camera. */
+int32_t rba_get_rig_extrinsics(rba_handle* h, void* cam_from_rig);
+
 /* ---- Per-observation square-root information and residual read-back (DESIGN.md section 19) -- */
 
 /* Not in the reference, where every reprojection term has unit weight.  Observation o (index in the problem's CSR order, the

@@ -159,6 +159,8 @@ def lib():
         _lib.rba_set_prior_loss.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
         _lib.rba_get_prior_residuals.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]
         _lib.rba_set_camera_rigs.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+        _lib.rba_set_rig_sensors.argtypes = [C.c_void_p, C.c_void_p]
+        _lib.rba_get_rig_extrinsics.argtypes = [C.c_void_p, C.c_void_p]
     return _lib
 
 

@@ -10,7 +10,11 @@
 // the members' poses after every update.  Only rigs of >= 2 cameras exist here: a rig of one is a free camera.  Every sum
 // over a rig runs in a fixed order (members ascending per thread, then the fixed tree of group_block_sum), so the results
 // are deterministic.
+// Estimated extrinsics (rba_set_rig_sensors, DESIGN.md section 24) run in the SENS instances of these kernels, which take a
+// SensorView: the sensor's pose sits in its home's entries 0..5 of u, and every camera j of the sensor adds Q~_j u_s.
 #pragma once
+
+#include <type_traits>
 
 #include "groups.cuh"
 
@@ -28,13 +32,108 @@ struct RigView {
   int nr;
 };
 
+// Estimated extrinsics (rba_set_rig_sensors, DESIGN.md section 24), passed to the sensor instances of the rig kernels (the
+// others take NoSensors, so that their parameters are those of section 23).  The lead of a rig is then its lowest-index
+// camera with held extrinsics, first in its member list.  Sensor s has the home smem[sptr[s]] (its lowest-index camera),
+// whose entries 0..5 of u carry the sensor's pose; every camera j of s moves by A_j d_lead + d_s.
+template <class S>
+struct SensorView {
+  const int* home;   // [nc] the home of the camera's sensor, -1 = held extrinsics
+  const int* sptr;   // [ns + 1] cameras of sensor s: smem[sptr[s] .. sptr[s + 1]), ascending, so the home first
+  const int* smem;
+  const double* K;   // [nc][7] E_lead(home) E_lead(j)^-1 of every sensor camera j (the identity for a home)
+  S* qt;             // [nc][6] Q~_j = D_j^-1 D_s, diagonal (k_rig_scaling)
+  S* ds;             // [ns][6] D_s
+  const S* b;        // [9 nc] the copy of b that k_rig_precond reads
+  const uint8_t* fixed;  // [nc] the tied mask (the homes' pose entries free), read by the covariance expansion
+  int ns;
+};
+struct NoSensors {};
+template <class S, bool SENS>
+using SensorArg = std::conditional_t<SENS, SensorView<S>, NoSensors>;
+
+// ---- poses in double: (qx, qy, qz, qw, tx, ty, tz), T(x) = R x + t ----
+__device__ __forceinline__ void pose_mul(const double* a, const double* b, double* out) {  // a b
+  out[3] = a[3] * b[3] - a[0] * b[0] - a[1] * b[1] - a[2] * b[2];
+  out[0] = a[3] * b[0] + a[0] * b[3] + a[1] * b[2] - a[2] * b[1];
+  out[1] = a[3] * b[1] + a[1] * b[3] + a[2] * b[0] - a[0] * b[2];
+  out[2] = a[3] * b[2] + a[2] * b[3] + a[0] * b[1] - a[1] * b[0];
+  const double x = a[0], y = a[1], z = a[2], w = a[3];
+  const double R[9] = {1 - 2 * (y * y + z * z), 2 * (x * y - z * w), 2 * (x * z + y * w),
+                       2 * (x * y + z * w), 1 - 2 * (x * x + z * z), 2 * (y * z - x * w),
+                       2 * (x * z - y * w), 2 * (y * z + x * w), 1 - 2 * (x * x + y * y)};
+  for (int r = 0; r < 3; ++r) out[4 + r] = R[3 * r] * b[4] + R[3 * r + 1] * b[5] + R[3 * r + 2] * b[6] + a[4 + r];
+}
+__device__ __forceinline__ void pose_inv(const double* a, double* out) {
+  const double q[7] = {-a[0], -a[1], -a[2], a[3], 0, 0, 0};
+  double r[7];
+  pose_mul(q, a, r);  // rotation R^T, translation R^T t
+  for (int k = 0; k < 4; ++k) out[k] = q[k];
+  for (int k = 0; k < 3; ++k) out[4 + k] = -r[4 + k];
+}
+template <class S>
+__device__ __forceinline__ void load_pose(const S* cams, size_t cam, double* p) {
+  for (int k = 0; k < 7; ++k) p[k] = (double)cams[10 * cam + k];
+}
+// M_j = T_home T_lead(home)^-1 K_j of sensor camera j from the current state, the quaternion normalised: the extrinsics
+// E_s = T_home T_lead(home)^-1 E_lead(home) that the state defines, relative to j's lead
+template <class S>
+__device__ __forceinline__ void sensor_map(const S* cams, const RigView<S>& R, const SensorView<S>& Z, size_t cam, double* m) {
+  const int h = Z.home[cam];
+  double th[7], tl[7], il[7], hl[7];
+  load_pose(cams, h, th);
+  load_pose(cams, R.lead[h], tl);
+  pose_inv(tl, il);
+  pose_mul(th, il, hl);
+  pose_mul(hl, Z.K + 7 * cam, m);
+  const double n = 1.0 / sqrt(m[0] * m[0] + m[1] * m[1] + m[2] * m[2] + m[3] * m[3]);
+  for (int k = 0; k < 4; ++k) m[k] *= n;
+}
+
 // linearize, after k_scaling and the priors' scaled blocks: D_u of every rig and P~ of its members.  Block per rig.
 //   n_k^2 = sum_j (A_j e_k)^T G_j (A_j e_k) + sum over the directed pair edges (j, i) inside the rig of (A_j e_k)^T O_ji^u (A_i e_k)
 // with G_j = D_j^-1 B_j D_j^-1 the member's unscaled pose Gram (B_j: `blocks`, the scaled observation Gram, + prior_H when
 // given) and O^u = D_j^-1 O D_i^-1 the unscaled cross block of a pair prior (D.pair_O).  D_u,k = 1 / (eps + n_k) as k_scaling.
-template <class S>
+// SENS: blocks [nr, nr + ns) build D_s and Q~ of every sensor likewise, the sensor's column k being e_k on each of its cameras:
+//   n_k^2 = sum_j G_j,kk + sum over the directed pair edges (j, i) between two cameras of the sensor of O^u_ji,kk
+template <class S, bool SENS = false>
 __global__ void __launch_bounds__(GROUP_THREADS) k_rig_scaling(const S* __restrict__ blocks, const S* __restrict__ prior_H,
-                                                               DevPtrs<S> D, RigView<S> R, S eps) {
+                                                               DevPtrs<S> D, RigView<S> R, S eps,
+                                                               SensorArg<S, SENS> Z) {
+  if constexpr (SENS)
+    if ((int)blockIdx.x >= R.nr) {
+      const int sn = blockIdx.x - R.nr, m0 = Z.sptr[sn], m1 = Z.sptr[sn + 1];
+      S s[6] = {0, 0, 0, 0, 0, 0};
+      for (int q = m0 + threadIdx.x; q < m1; q += GROUP_THREADS) {
+        const size_t cam = Z.smem[q];
+        const S* B = blocks + 81 * cam;
+#pragma unroll
+        for (int k = 0; k < 6; ++k) {
+          const S dk = D.scaling[9 * cam + k];
+          S t = (B[10 * k] + (prior_H ? prior_H[81 * cam + 10 * k] : S(0))) / (dk * dk);
+          if (D.pair_ov)
+            for (int e = D.pair_ptr[cam], e1 = D.pair_ptr[cam + 1]; e < e1; ++e) {
+              const int nb = D.pair_nbr[e];
+              if (Z.home[nb] != Z.home[cam]) continue;
+              t += D.pair_O[36 * (size_t)e + 7 * k] / (dk * D.scaling[9 * (size_t)nb + k]);
+            }
+          s[k] += t;
+        }
+      }
+      group_block_sum<S, 6>(s);
+      S ds[6];
+#pragma unroll
+      for (int k = 0; k < 6; ++k) ds[k] = S(1) / (eps + sqrt(s[k] > S(0) ? s[k] : S(0)));
+      if (threadIdx.x == 0)
+#pragma unroll
+        for (int k = 0; k < 6; ++k) Z.ds[6 * (size_t)sn + k] = ds[k];
+      for (int q = m0 + threadIdx.x; q < m1; q += GROUP_THREADS) {
+        const size_t cam = Z.smem[q];
+#pragma unroll
+        for (int k = 0; k < 6; ++k) Z.qt[6 * cam + k] = ds[k] / D.scaling[9 * cam + k];
+      }
+      return;
+    }
   const int m0 = R.ptr[blockIdx.x], m1 = R.ptr[blockIdx.x + 1];
   const int lead = R.mem[m0];
   // (A_j e_k) / D_j of camera cam, entry r
@@ -89,9 +188,12 @@ __global__ void __launch_bounds__(GROUP_THREADS) k_rig_scaling(const S* __restri
 // entries before its barrier and writes after it.  Blocks [0, ncb): thread per camera (the copies), blocks
 // [ncb, ncb + nr): one per rig.  In a solve (st set) it is launched dependent on its predecessor and returns once the
 // solve has ended, like k_group_expand.
-template <class S>
+// SENS: every camera j of a sensor adds Q~_j u_s, u_s the home's entries 0..5 of v, so out must not be v (the homes' entries
+// are read across rigs).  host = 1: the home keeps its entries and u_s = (x_home - P~_home u_lead(home)) / Q~_home, which
+// reads only leads' and homes' entries, neither of which is written, so out may be v.
+template <class S, bool SENS = false>
 __global__ void __launch_bounds__(GROUP_THREADS) k_rig_expand(const S* v, S* out, RigView<S> R, int nc, int ncb, int host,
-                                                              const PcgState* st) {
+                                                              const PcgState* st, SensorArg<S, SENS> Z) {
   asm volatile("griddepcontrol.wait;" ::: "memory");
   if (st && *reinterpret_cast<const volatile int*>(&st->done)) return;
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
@@ -111,11 +213,37 @@ __global__ void __launch_bounds__(GROUP_THREADS) k_rig_expand(const S* v, S* out
   for (int q = m0 + (host ? 1 : 0) + threadIdx.x; q < m1; q += GROUP_THREADS) {
     const size_t cam = R.mem[q];
     const S* P = R.pt + 36 * cam;
+    S us[6] = {0, 0, 0, 0, 0, 0};
+    if constexpr (SENS) {
+      const int h = Z.home[cam];
+      if (h >= 0) {
+        if (host && h == (int)cam) continue;
+        if (host) {
+          const size_t hl = R.lead[h];
+          S ul[6];
+#pragma unroll
+          for (int k = 0; k < 6; ++k) ul[k] = v[9 * hl + k] / R.pt[36 * hl + 7 * k];
+#pragma unroll
+          for (int a = 0; a < 6; ++a) {
+            S t = v[9 * (size_t)h + a];
+#pragma unroll
+            for (int k = 0; k < 6; ++k) t -= R.pt[36 * (size_t)h + 6 * a + k] * ul[k];
+            us[a] = t / Z.qt[6 * (size_t)h + a];
+          }
+        } else {
+#pragma unroll
+          for (int a = 0; a < 6; ++a) us[a] = v[9 * (size_t)h + a];
+        }
+#pragma unroll
+        for (int a = 0; a < 6; ++a) us[a] *= Z.qt[6 * cam + a];
+      }
+    }
 #pragma unroll
     for (int a = 0; a < 6; ++a) {
       S t = 0;
 #pragma unroll
       for (int k = 0; k < 6; ++k) t += P[6 * a + k] * x[k];
+      if constexpr (SENS) t += us[a];
       out[9 * cam + a] = t;
     }
   }
@@ -126,19 +254,38 @@ __global__ void __launch_bounds__(GROUP_THREADS) k_rig_expand(const S* v, S* out
 // come from D (operator_row); else `in` holds them already (after k_group_contract) and only the rigs' pose rows are
 // contracted, in place when out == in.  Blocks [0, ncb): thread per camera (rows of the free cameras and the rigged cameras'
 // rows 6..8; nothing when in is given), blocks [ncb, ncb + nr): one per rig.
-template <class S>
+// SENS: blocks [ncb + nr, ncb + nr + ns) give each home's rows 0..5 u_s = sum_j Q~_j^T row_j over the sensor's cameras and
+// the other cameras' 0; the rig blocks leave the sensor cameras' rows to them.  A camera's rows feed a rig block and a sensor
+// block, so out must not be in: every block then reads rows no block writes.  The thread-per-camera blocks copy the rows
+// they own when in is given.
+template <class S, bool SENS = false>
 __global__ void __launch_bounds__(GROUP_THREADS) k_rig_contract(DevPtrs<S> D, const S* __restrict__ ve, const S* in, S* out,
-                                                                RigView<S> R, int ncb, const PcgState* st) {
+                                                                RigView<S> R, int ncb, const PcgState* st, SensorArg<S, SENS> Z) {
   asm volatile("griddepcontrol.wait;" ::: "memory");
   if (*reinterpret_cast<const volatile int*>(&st->done)) return;
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   auto row = [&](size_t cam, int a) -> S { return in ? in[9 * cam + a] : operator_row(D, ve, cam, a); };
   if ((int)blockIdx.x < ncb) {
     const int cam = blockIdx.x * GROUP_THREADS + threadIdx.x;
-    if (cam >= D.nc || in) return;
+    if (cam >= D.nc || (SENS ? in == out : in != nullptr)) return;
     for (int a = R.lead[cam] >= 0 ? 6 : 0; a < 9; ++a) out[9 * (size_t)cam + a] = row(cam, a);
     return;
   }
+  if constexpr (SENS)
+    if ((int)blockIdx.x >= ncb + R.nr) {
+      const int sn = blockIdx.x - ncb - R.nr, m0 = Z.sptr[sn], m1 = Z.sptr[sn + 1];
+      S s[6] = {0, 0, 0, 0, 0, 0};
+      for (int q = m0 + threadIdx.x; q < m1; q += GROUP_THREADS) {
+        const size_t cam = Z.smem[q];
+#pragma unroll
+        for (int a = 0; a < 6; ++a) s[a] += Z.qt[6 * cam + a] * row(cam, a);
+      }
+      group_block_sum<S, 6>(s);
+      for (int q = m0 + threadIdx.x; q < m1; q += GROUP_THREADS)
+#pragma unroll
+        for (int k = 0; k < 6; ++k) out[9 * (size_t)Z.smem[q] + k] = q == m0 ? s[k] : S(0);
+      return;
+    }
   const int r = blockIdx.x - ncb;
   const int m0 = R.ptr[r], m1 = R.ptr[r + 1];
   S s[6] = {0, 0, 0, 0, 0, 0};
@@ -154,9 +301,12 @@ __global__ void __launch_bounds__(GROUP_THREADS) k_rig_contract(DevPtrs<S> D, co
       for (int k = 0; k < 6; ++k) s[k] += P[6 * a + k] * y[a];
   }
   group_block_sum<S, 6>(s);  // every read above precedes its barriers, every write below follows them
-  for (int q = m0 + threadIdx.x; q < m1; q += GROUP_THREADS)
+  for (int q = m0 + threadIdx.x; q < m1; q += GROUP_THREADS) {
+    if constexpr (SENS)
+      if (Z.home[R.mem[q]] >= 0) continue;
 #pragma unroll
     for (int k = 0; k < 6; ++k) out[9 * (size_t)R.mem[q] + k] = q == m0 ? s[k] : S(0);
+  }
 }
 
 // solve, ahead of k_precond_invert: the preconditioner blocks in the block partition of the tied problem and the contracted
@@ -168,10 +318,18 @@ __global__ void __launch_bounds__(GROUP_THREADS) k_rig_contract(DevPtrs<S> D, co
 // The cross terms between members of one rig are not in the per-camera blocks and stay out.  k_precond_invert then adds
 // lambda once per parameter of the tied problem and masks the members' entries 0..5 as held.  The two roles touch disjoint
 // entries, so out may be src (SCHUR_JACOBI, and after k_group_precond).
-template <class S>
+// SENS: blocks [ncb + nr, ncb + nr + ns) put sum_j Q~_j B_j Q~_j (Q~ diagonal) and sum_j Q~_j (b_j + prior_g_j)[0..5] of
+// each sensor into its home's pose entries and 0 into its other cameras'; the rig blocks leave the sensor cameras' pose
+// entries to them.  A camera's pose block feeds a rig block and a sensor block, so every block reads src and Z.b, copies
+// that no block writes (out and b are other buffers).
+template <class S, bool SENS = false>
 __global__ void __launch_bounds__(GROUP_THREADS) k_rig_precond(const S* src, const S* __restrict__ prior_H,
                                                                const S* __restrict__ prior_g, S* __restrict__ b, S* out,
-                                                               RigView<S> R, int nc, int ncb) {
+                                                               RigView<S> R, int nc, int ncb, SensorArg<S, SENS> Z) {
+  auto b_in = [&](size_t e) -> S {
+    if constexpr (SENS) return Z.b[e];
+    else return b[e];
+  };
   if ((int)blockIdx.x < ncb) {
     const int cam = blockIdx.x * GROUP_THREADS + threadIdx.x;
     if (cam >= nc) return;
@@ -184,10 +342,47 @@ __global__ void __launch_bounds__(GROUP_THREADS) k_rig_precond(const S* src, con
         if (prior_H) a += prior_H[o + 9 * r + c];
         out[o + 9 * r + c] = (rigged && (r < 6) != (c < 6)) ? S(0) : a;
       }
-    if (prior_g)
+    if constexpr (SENS) {
+      for (int d = rigged ? 6 : 0; d < 9; ++d) b[9 * (size_t)cam + d] = Z.b[9 * (size_t)cam + d] + (prior_g ? prior_g[9 * (size_t)cam + d] : S(0));
+    } else if (prior_g) {
       for (int d = rigged ? 6 : 0; d < 9; ++d) b[9 * (size_t)cam + d] += prior_g[9 * (size_t)cam + d];
+    }
     return;
   }
+  if constexpr (SENS)
+    if ((int)blockIdx.x >= ncb + R.nr) {
+      const int sn = blockIdx.x - ncb - R.nr, m0 = Z.sptr[sn], m1 = Z.sptr[sn + 1];
+      S s[27];  // [0, 21): the upper triangle of the sensor's pose block, row by row; [21, 27): its b
+#pragma unroll
+      for (int k = 0; k < 27; ++k) s[k] = 0;
+      for (int q = m0 + threadIdx.x; q < m1; q += GROUP_THREADS) {
+        const size_t cam = Z.smem[q];
+        const S* Q = Z.qt + 6 * cam;
+#pragma unroll
+        for (int i = 0; i < 6; ++i) {
+#pragma unroll
+          for (int k = i; k < 6; ++k)
+            s[i * 6 - i * (i - 1) / 2 + (k - i)] +=
+                Q[i] * (src[81 * cam + 9 * i + k] + (prior_H ? prior_H[81 * cam + 9 * i + k] : S(0))) * Q[k];
+          s[21 + i] += Q[i] * (b_in(9 * cam + i) + (prior_g ? prior_g[9 * cam + i] : S(0)));
+        }
+      }
+      group_block_sum<S, 27>(s);
+      for (int q = m0 + threadIdx.x; q < m1; q += GROUP_THREADS) {
+        const size_t cam = Z.smem[q];
+        const bool home = q == m0;
+#pragma unroll
+        for (int i = 0; i < 6; ++i) {
+#pragma unroll
+          for (int k = 0; k < 6; ++k) {
+            const int lo = i < k ? i : k, hi = i < k ? k : i;
+            out[81 * cam + 9 * i + k] = home ? s[lo * 6 - lo * (lo - 1) / 2 + (hi - lo)] : S(0);
+          }
+          b[9 * cam + i] = home ? s[21 + i] : S(0);
+        }
+      }
+      return;
+    }
   const int rg = blockIdx.x - ncb;
   const int m0 = R.ptr[rg], m1 = R.ptr[rg + 1];
   S s[27];  // [0, 21): the upper triangle of the rig's pose block, row by row; [21, 27): its b
@@ -217,13 +412,15 @@ __global__ void __launch_bounds__(GROUP_THREADS) k_rig_precond(const S* src, con
       }
       S g = 0;
 #pragma unroll
-      for (int r = 0; r < 6; ++r) g += P[6 * r + k] * (b[9 * cam + r] + (prior_g ? prior_g[9 * cam + r] : S(0)));
+      for (int r = 0; r < 6; ++r) g += P[6 * r + k] * (b_in(9 * cam + r) + (prior_g ? prior_g[9 * cam + r] : S(0)));
       s[21 + k] += g;
     }
   }
   group_block_sum<S, 27>(s);  // every read above precedes its barriers, every write below follows them
   for (int q = m0 + threadIdx.x; q < m1; q += GROUP_THREADS) {
     const size_t cam = R.mem[q];
+    if constexpr (SENS)
+      if (Z.home[cam] >= 0) continue;
     const bool lead = q == m0;
 #pragma unroll
     for (int i = 0; i < 6; ++i) {
@@ -240,12 +437,7 @@ __global__ void __launch_bounds__(GROUP_THREADS) k_rig_precond(const S* src, con
 // every member's pose := M_j T_lead (R = R_m R_lead, t = R_m t_lead + t_m), in double, the quaternion normalised, rounded to
 // S.  Deterministic, so replicated cameras stay bit-identical across ranks.  Thread per camera.
 template <class S>
-__global__ void k_rig_retie(S* __restrict__ cams, RigView<S> R, int nc) {
-  const int cam = blockIdx.x * blockDim.x + threadIdx.x;
-  if (cam >= nc) return;
-  const int ld = R.lead[cam];
-  if (ld < 0 || ld == cam) return;
-  const double* m = R.M + 7 * (size_t)cam;
+__device__ __forceinline__ void retie_pose(S* __restrict__ cams, int cam, int ld, const double* m) {
   const S* cl = cams + 10 * (size_t)ld;
   const double a0 = m[0], a1 = m[1], a2 = m[2], a3 = m[3];
   const double b0 = cl[0], b1 = cl[1], b2 = cl[2], b3 = cl[3];
@@ -266,6 +458,29 @@ __global__ void k_rig_retie(S* __restrict__ cams, RigView<S> R, int nc) {
 #pragma unroll
   for (int r = 0; r < 3; ++r) cm[4 + r] = (S)(Rm[3 * r] * t0 + Rm[3 * r + 1] * t1 + Rm[3 * r + 2] * t2 + m[4 + r]);
 }
+template <class S>
+__global__ void k_rig_retie(S* __restrict__ cams, RigView<S> R, int nc) {
+  const int cam = blockIdx.x * blockDim.x + threadIdx.x;
+  if (cam >= nc) return;
+  const int ld = R.lead[cam];
+  if (ld < 0 || ld == cam) return;
+  retie_pose(cams, cam, ld, R.M + 7 * (size_t)cam);
+}
+// with sensors (section 24), after every camera update and at every rba_set_state: a member with held extrinsics as
+// k_rig_retie, a sensor camera other than the home at M_j = T_home T_lead(home)^-1 K_j from the state (sensor_map); the
+// home keeps its pose, which defines E_s.  Reads only leads and homes, which it does not write.  Thread per camera.
+template <class S>
+__global__ void k_sensor_retie(S* __restrict__ cams, RigView<S> R, SensorView<S> Z, int nc) {
+  const int cam = blockIdx.x * blockDim.x + threadIdx.x;
+  if (cam >= nc) return;
+  const int ld = R.lead[cam], h = Z.home[cam];
+  if (ld < 0 || ld == cam || h == cam) return;
+  double m[7];
+  if (h >= 0) sensor_map(cams, R, Z, cam, m);
+  else
+    for (int k = 0; k < 7; ++k) m[k] = R.M[7 * (size_t)cam + k];
+  retie_pose(cams, cam, ld, m);
+}
 
 // ---- rba_compute_covariance (DESIGN.md sections 16 and 23) on the dense np x np column-major matrix A (ld) ----
 // A_j of M_j in double, row-major 6x6
@@ -285,12 +500,30 @@ __device__ __forceinline__ void rig_adjoint(const double* __restrict__ m, double
       A[6 * (3 + r) + 3 + k] = R[3 * r + k];
     }
 }
+// M_j and A_j of every sensor camera from the current state (sensor_map), ahead of k_rig_scaling and of the covariance
+// passes: M in double, A_j rounded to S.  Thread per camera.
+template <class S>
+__global__ void k_sensor_tie(const S* __restrict__ cams, RigView<S> R, SensorView<S> Z, double* __restrict__ M, S* __restrict__ adj,
+                             int nc) {
+  const int cam = blockIdx.x * blockDim.x + threadIdx.x;
+  if (cam >= nc || Z.home[cam] < 0) return;
+  double m[7], A[36];
+  sensor_map(cams, R, Z, cam, m);
+  for (int k = 0; k < 7; ++k) M[7 * (size_t)cam + k] = m[k];
+  rig_adjoint(m, A);
+  for (int k = 0; k < 36; ++k) adj[36 * (size_t)cam + k] = (S)A[k];
+}
 // Row pass (thread per column i, which it alone touches) or column pass (thread per row i) over every rig's pose rows /
 // columns, members in order: contract (expand = 0) adds A_j^T times the member's rows / columns 0..5 to the lead's, which
 // applied as rows then columns gives P^T A P; expand (expand = 1) sets the member's to A_j times the lead's, which applied to
 // the (un-equilibrated) inverse gives P A P^T.  The full symmetric matrix is read (k_cov_group_symmetrize first).
-template <class S>
-__global__ void k_cov_rig_pass(double* __restrict__ A, long long ld, long long n, RigView<S> R, int columns, int expand) {
+// SENS (section 24, M_j of the sensor cameras from k_sensor_tie): contract then sums every sensor's rows / columns into its
+// home's, after the rigs' pass, which writes only leads; expand adds the home's to every camera of the sensor, the homes
+// last, so that each reads the home's contracted entries.  The inverse holds identity rows at held entries (k_cov_equil);
+// a sensor camera of a held rig is not held, so expand reads a held lead's entries as 0.
+template <class S, bool SENS = false>
+__global__ void k_cov_rig_pass(double* __restrict__ A, long long ld, long long n, RigView<S> R, int columns, int expand,
+                               SensorArg<S, SENS> Z) {
   const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
   if (i >= n) return;
   auto at = [&](long long j) -> double& { return columns ? A[i + j * ld] : A[j + i * ld]; };
@@ -299,14 +532,22 @@ __global__ void k_cov_rig_pass(double* __restrict__ A, long long ld, long long n
     const long long lead = 9LL * R.mem[m0];
     double x[6];
     for (int k = 0; k < 6; ++k) x[k] = at(lead + k);
+    if constexpr (SENS)
+      if (expand)
+        for (int k = 0; k < 6; ++k)
+          if ((fixed_entry_mask(Z.fixed[lead / 9]) >> k) & 1u) x[k] = 0.0;
     for (int q = m0 + 1; q < m1; ++q) {
       const long long cam = R.mem[q];
+      if constexpr (SENS)
+        if (expand && Z.home[cam] == cam) continue;
       double Aj[36];
       rig_adjoint(R.M + 7 * cam, Aj);
       if (expand) {
         for (int a = 0; a < 6; ++a) {
           double t = 0;
           for (int b = 0; b < 6; ++b) t += Aj[6 * a + b] * x[b];
+          if constexpr (SENS)
+            if (Z.home[cam] >= 0) t += at(9LL * Z.home[cam] + a);
           at(9 * cam + a) = t;
         }
       } else {
@@ -322,6 +563,29 @@ __global__ void k_cov_rig_pass(double* __restrict__ A, long long ld, long long n
     if (!expand)
       for (int k = 0; k < 6; ++k) at(lead + k) = x[k];
   }
+  if constexpr (SENS)
+    for (int sn = 0; sn < Z.ns; ++sn) {
+      const int m0 = Z.sptr[sn], m1 = Z.sptr[sn + 1];
+      const long long h = Z.smem[m0];
+      double x[6];
+      for (int k = 0; k < 6; ++k) x[k] = at(9 * h + k);
+      if (expand) {  // the home: A_home times its lead's entries plus the sensor's
+        const long long hl = 9LL * R.lead[h];
+        const unsigned lf = fixed_entry_mask(Z.fixed[R.lead[h]]);
+        double Aj[36];
+        rig_adjoint(R.M + 7 * h, Aj);
+        for (int a = 0; a < 6; ++a) {
+          double t = x[a];
+          for (int b = 0; b < 6; ++b)
+            if (!((lf >> b) & 1u)) t += Aj[6 * a + b] * at(hl + b);
+          at(9 * h + a) = t;
+        }
+      } else {
+        for (int q = m0 + 1; q < m1; ++q)
+          for (int k = 0; k < 6; ++k) x[k] += at(9LL * Z.smem[q] + k);
+        for (int k = 0; k < 6; ++k) at(9 * h + k) = x[k];
+      }
+    }
 }
 // the inverse of the equilibrated matrix back to the inverse of the matrix itself on the leading n x n (full) part, so that the
 // expansion through the unscaled A_j agrees with the equilibration: A <- D A D, then d <- 1 (k_cov_unit_d)

@@ -78,6 +78,8 @@ struct rba_handle {
   virtual int set_landmark_prior(int32_t num, const int32_t* lm_idx, const void* mean, const void* sqrt_info) = 0;
   virtual int set_intrinsics_groups(const int32_t* group) = 0;
   virtual int set_camera_rigs(const int32_t* rig, const void* cam_from_rig) = 0;
+  virtual int set_rig_sensors(const int32_t* sensor) = 0;
+  virtual int get_rig_extrinsics(void* cam_from_rig) = 0;
   virtual int set_observation_info(const void* sqrt_info) = 0;
   virtual int set_observation_loss(const uint8_t* kind, const void* scale) = 0;
   virtual int set_prior_loss(int32_t prior_kind, int32_t num, const uint8_t* kind, const void* scale) = 0;
@@ -260,6 +262,8 @@ struct Solver : rba_handle {
   struct RigTerm {                 // rba_set_camera_rigs, DESIGN.md section 23
     int n = 0;                     // rigs of >= 2 cameras; 0 = the unmodified path
     std::vector<int> host_lead;    // [nc] lead of the camera's rig, -1 = free camera (also a rig of one)
+    std::vector<int> host_first;   // [nc] the rig's lowest-index camera (its lead without sensors), -1 likewise
+    std::vector<double> host_E;    // [nc][7] the extrinsics given, quaternion normalised
     DeviceBuffer<int> lead, ptr, mem;  // new lists ({} to fit) at every call with rigs
     DeviceBuffer<S> adj;           // [nc][36] A_j
     DeviceBuffer<double> M;        // [nc][7] M_j = E_j E_lead^-1
@@ -270,6 +274,17 @@ struct Solver : rba_handle {
     void adopt(RigTerm& o) { lead.take(o.lead); ptr.take(o.ptr); mem.take(o.mem); adj.take(o.adj); M.take(o.M); pt.take(o.pt);
                              du.take(o.du); fixed.take(o.fixed); ve.take(o.ve); y.take(o.y); }
   } rig;
+  struct SensorTerm {              // rba_set_rig_sensors, DESIGN.md section 24
+    int n = 0;                     // sensors; 0 = rigs as in section 23
+    std::vector<int> host_home;    // [nc] the home of the camera's sensor, -1 = held extrinsics
+    DeviceBuffer<int> home, ptr, mem;  // new lists ({} to fit) at every call with sensors
+    DeviceBuffer<double> K;        // [nc][7] E_lead(home) E_lead(j)^-1
+    DeviceBuffer<S> qt, ds;        // [nc][6] Q~_j, [ns][6] D_s of the last linearisation
+    DeviceBuffer<uint8_t> cam_fixed;  // [nc] the user's flags without RBA_FIX_POSE on sensor cameras (D.cam_fixed)
+    DeviceBuffer<S> blk, b;        // [81 nc], [9 nc] the inputs of k_rig_precond, which writes D.blocks and D.b
+    void adopt(SensorTerm& o) { home.take(o.home); ptr.take(o.ptr); mem.take(o.mem); K.take(o.K); qt.take(o.qt); ds.take(o.ds);
+                                cam_fixed.take(o.cam_fixed); blk.take(o.blk); b.take(o.b); }
+  } sen;
   struct ObservationTerm {
     bool on = false;               // rba_set_observation_info, DESIGN.md section 19: W [nslots][4] = D.obs_W while on
     DeviceBuffer<S> W;
@@ -771,7 +786,7 @@ struct Solver : rba_handle {
     }
     CU(cudaMemcpyAsync(D.cams, cams, (size_t)10 * nc * sizeof(S), cudaMemcpyHostToDevice, stream));
     CU(cudaMemcpyAsync(D.lms, (const S*)lms + (size_t)3 * L.lm_begin, (size_t)3 * L.nl_local * sizeof(S), cudaMemcpyHostToDevice, stream));
-    if (rig.n) TRY(rig_retie(D.cams));  // the members take M_j T_lead
+    if (rig.n) TRY(rig_retie_state(D.cams));  // the members take M_j T_lead
     CU(cudaStreamSynchronize(stream));
     return RBA_OK;
   }
@@ -900,7 +915,9 @@ struct Solver : rba_handle {
         for (int k = 7; k < 10; ++k) cams[10 * (size_t)c + k] = cams[10 * (size_t)grp.host_lead[c] + k];
   }
   // the flags k_precond_invert masks with while groups or rigs exist (grp.fixed, rig.fixed): the user's, the intrinsics of
-  // every group member but the lead and the pose of every rig member but the lead
+  // every group member but the lead and the pose of every rig member but the lead.  With sensors (section 24) a home's pose
+  // entries carry its sensor's, which RBA_FIX_POSE on its rig does not hold; the camera update and the other users of
+  // D.cam_fixed then read the user's flags without RBA_FIX_POSE on the sensor cameras (sen.cam_fixed).
   int upload_tied_fixed() {
     if (!grp.n && !rig.n) return RBA_OK;
     std::vector<uint8_t> f((size_t)nc, 0);
@@ -908,6 +925,17 @@ struct Solver : rba_handle {
     for (int c = 0; c < nc; ++c)
       f[c] = (uint8_t)((held.host.empty() ? 0 : held.host[c]) | (grp.n && member(grp.host_lead, c) ? RBA_FIX_INTRINSICS : 0) |
                        (rig.n && member(rig.host_lead, c) ? RBA_FIX_POSE : 0));
+    if (sen.n) {
+      std::vector<uint8_t> user((size_t)nc, 0);
+      for (int c = 0; c < nc; ++c)
+        if (sen.host_home[c] >= 0) {
+          if (sen.host_home[c] == c) f[c] &= (uint8_t)~RBA_FIX_POSE;
+          if (!held.host.empty()) user[c] = (uint8_t)(held.host[c] & ~RBA_FIX_POSE);
+        } else if (!held.host.empty()) {
+          user[c] = held.host[c];
+        }
+      if (!held.host.empty()) TRY(copy_in(sen.cam_fixed.get(), user));
+    }
     if (grp.n) TRY(copy_in(grp.fixed.get(), f));
     if (rig.n) TRY(copy_in(rig.fixed.get(), f));
     CU(cudaStreamSynchronize(stream));
@@ -950,70 +978,24 @@ struct Solver : rba_handle {
       for (int c = 0; c < nc; ++c)
         if (rid[c] >= 0 && count[rid[c]] >= 2) lead[c] = first[rid[c]];
     }
-    // rigs in the order of their leads, members ascending (the lead first)
-    std::vector<int> ridx((size_t)nc, -1), ptr(1, 0), mem;
     int nr = 0;
-    for (int c = 0; c < nc; ++c)
-      if (lead[c] == c) ridx[c] = nr++;
+    for (int c = 0; c < nc; ++c) nr += lead[c] == c;
     if (nr > 0 && opt.solver_type == 2)
       return fail(RBA_ERR_UNSUPPORTED, "POWER_SCHUR_COMPLEMENT does not support rigs of >= 2 cameras (Hpp of the tied problem is not block-diagonal)");
     const std::string why = rig_flags_mismatch(lead, held.host);
     if (!why.empty()) return fail(RBA_ERR_INVALID_ARGUMENT, why);
-    ptr.assign((size_t)nr + 1, 0);
-    for (int c = 0; c < nc; ++c)
-      if (lead[c] >= 0) ++ptr[ridx[lead[c]] + 1];
-    for (int r = 0; r < nr; ++r) ptr[r + 1] += ptr[r];
-    mem.resize((size_t)ptr[nr]);
-    std::vector<int> fill(ptr.begin(), ptr.end() - 1);
-    for (int c = 0; c < nc; ++c)
-      if (lead[c] >= 0) mem[fill[ridx[lead[c]]]++] = c;
     if (nr > 0) {
-      // M_j = E_j E_lead^-1 (q_j conj(q_lead), t_j - R_M t_lead) and its adjoint A_j = [[R_M, [t_M]x R_M], [0, R_M]]
-      std::vector<double> M((size_t)7 * nc, 0.0);
-      std::vector<S> adj((size_t)36 * nc, S(0));
-      for (int c = 0; c < nc; ++c) {
-        if (lead[c] < 0) continue;
-        const double* a = &E[7 * (size_t)c];
-        const double* l = &E[7 * (size_t)lead[c]];
-        const double b0 = -l[0], b1 = -l[1], b2 = -l[2], b3 = l[3];
-        double* m = &M[7 * (size_t)c];
-        m[3] = a[3] * b3 - a[0] * b0 - a[1] * b1 - a[2] * b2;
-        m[0] = a[3] * b0 + a[0] * b3 + a[1] * b2 - a[2] * b1;
-        m[1] = a[3] * b1 + a[1] * b3 + a[2] * b0 - a[0] * b2;
-        m[2] = a[3] * b2 + a[2] * b3 + a[0] * b1 - a[1] * b0;
-        const double qn = std::sqrt(m[0] * m[0] + m[1] * m[1] + m[2] * m[2] + m[3] * m[3]);
-        for (int k = 0; k < 4; ++k) m[k] /= qn;
-        const double x = m[0], y = m[1], z = m[2], w = m[3];
-        const double R[9] = {1 - 2 * (y * y + z * z), 2 * (x * y - z * w), 2 * (x * z + y * w),
-                             2 * (x * y + z * w), 1 - 2 * (x * x + z * z), 2 * (y * z - x * w),
-                             2 * (x * z - y * w), 2 * (y * z + x * w), 1 - 2 * (x * x + y * y)};
-        for (int r = 0; r < 3; ++r) m[4 + r] = a[4 + r] - (R[3 * r] * l[4] + R[3 * r + 1] * l[5] + R[3 * r + 2] * l[6]);
-        const double tx[9] = {0, -m[6], m[5], m[6], 0, -m[4], -m[5], m[4], 0};
-        S* A = &adj[36 * (size_t)c];
-        for (int r = 0; r < 3; ++r)
-          for (int k = 0; k < 3; ++k) {
-            double txr = 0;
-            for (int i = 0; i < 3; ++i) txr += tx[3 * r + i] * R[3 * i + k];
-            A[6 * r + k] = (S)R[3 * r + k];
-            A[6 * r + 3 + k] = (S)txr;
-            A[6 * (3 + r) + 3 + k] = (S)R[3 * r + k];
-          }
-        if (c == lead[c])  // exactly the identity
-          for (int k = 0; k < 36; ++k) A[k] = (k % 7 == 0) ? S(1) : S(0);
-      }
       RigTerm next;
-      TRY(fit(next.lead, {}, lead.size(), &lead)); TRY(fit(next.ptr, {}, ptr.size(), &ptr)); TRY(fit(next.mem, {}, mem.size(), &mem));
-      TRY(fit(next.adj, {}, adj.size(), &adj)); TRY(fit(next.M, {}, M.size(), &M));
-      TRY(fit(next.du, rig.du, (size_t)6 * nr));
-      if (!rig.ve.get()) {
-        TRY(alloc(next.pt, (size_t)36 * nc, true)); TRY(alloc(next.fixed, (size_t)nc, true));
-        TRY(alloc(next.ve, (size_t)9 * nc, true)); TRY(alloc(next.y, (size_t)9 * nc, true));
-      }
+      TRY(rig_tables(lead, E, {}, next, nullptr));
       CU(cudaStreamSynchronize(stream));
       rig.adopt(next);
     }
     rig.n = nr;
+    rig.host_first = lead;
     rig.host_lead = std::move(lead);
+    rig.host_E = std::move(E);
+    sen.n = 0;  // the sensors belonged to the previous rigs
+    sen.host_home.clear();
     TRY(upload_tied_fixed());
     if (nr > 0) {  // the current state and its backup take the tied poses
       TRY(rig_retie(D.cams)); TRY(rig_retie(cams_bk));
@@ -1022,6 +1004,180 @@ struct Solver : rba_handle {
     }
     // the blocks and b of the last linearisation belong to the previous rigs
     return priors_changed();
+  }
+  // m = a b^-1 of two poses (qx,qy,qz,qw, tx,ty,tz) in double, the quaternion normalised
+  static void pose_ratio(const double* a, const double* l, double* m) {
+    const double b0 = -l[0], b1 = -l[1], b2 = -l[2], b3 = l[3];
+    m[3] = a[3] * b3 - a[0] * b0 - a[1] * b1 - a[2] * b2;
+    m[0] = a[3] * b0 + a[0] * b3 + a[1] * b2 - a[2] * b1;
+    m[1] = a[3] * b1 + a[1] * b3 + a[2] * b0 - a[0] * b2;
+    m[2] = a[3] * b2 + a[2] * b3 + a[0] * b1 - a[1] * b0;
+    const double qn = std::sqrt(m[0] * m[0] + m[1] * m[1] + m[2] * m[2] + m[3] * m[3]);
+    for (int k = 0; k < 4; ++k) m[k] /= qn;
+    const double R[9] = {1 - 2 * (m[1] * m[1] + m[2] * m[2]), 2 * (m[0] * m[1] - m[2] * m[3]), 2 * (m[0] * m[2] + m[1] * m[3]),
+                         2 * (m[0] * m[1] + m[2] * m[3]), 1 - 2 * (m[0] * m[0] + m[2] * m[2]), 2 * (m[1] * m[2] - m[0] * m[3]),
+                         2 * (m[0] * m[2] - m[1] * m[3]), 2 * (m[1] * m[2] + m[0] * m[3]), 1 - 2 * (m[0] * m[0] + m[1] * m[1])};
+    for (int r = 0; r < 3; ++r) m[4 + r] = a[4 + r] - (R[3 * r] * l[4] + R[3 * r + 1] * l[5] + R[3 * r + 2] * l[6]);
+  }
+  // The device tables of the rigs whose cameras have the leads `lead` (>= 1 rig of >= 2 cameras) and the extrinsics E, into
+  // next: the rigs in the order of their leads, each one's members with the lead first and the others ascending;
+  // M_j = E_j E_lead^-1 and its adjoint A_j = [[R_M, [t_M]x R_M], [0, R_M]] (the identity for a lead).  With sensors (home
+  // not empty) a sensor camera j takes M_j = E_home E_lead^-1 (the call ties it to its home's extrinsics) and
+  // K_j = E_lead(home) E_lead^-1 goes into *K.
+  int rig_tables(const std::vector<int>& lead, const std::vector<double>& E, const std::vector<int>& home, RigTerm& next,
+                 std::vector<double>* K) {
+    std::vector<int> ridx((size_t)nc, -1), ptr(1, 0), mem;
+    int nr = 0;
+    for (int c = 0; c < nc; ++c)
+      if (lead[c] == c) ridx[c] = nr++;
+    ptr.assign((size_t)nr + 1, 0);
+    for (int c = 0; c < nc; ++c)
+      if (lead[c] >= 0) ++ptr[ridx[lead[c]] + 1];
+    for (int r = 0; r < nr; ++r) ptr[r + 1] += ptr[r];
+    mem.resize((size_t)ptr[nr]);
+    std::vector<int> fill(ptr.begin(), ptr.end() - 1);
+    for (int c = 0; c < nc; ++c)
+      if (lead[c] == c) mem[fill[ridx[c]]++] = c;
+    for (int c = 0; c < nc; ++c)
+      if (lead[c] >= 0 && lead[c] != c) mem[fill[ridx[lead[c]]]++] = c;
+    std::vector<double> M((size_t)7 * nc, 0.0);
+    std::vector<S> adj((size_t)36 * nc, S(0));
+    if (K) K->assign((size_t)7 * nc, 0.0);
+    for (int c = 0; c < nc; ++c) {
+      if (lead[c] < 0) continue;
+      const int src = home.empty() || home[c] < 0 ? c : home[c];
+      double* m = &M[7 * (size_t)c];
+      pose_ratio(&E[7 * (size_t)src], &E[7 * (size_t)lead[c]], m);
+      if (src != c) pose_ratio(&E[7 * (size_t)lead[src]], &E[7 * (size_t)lead[c]], &(*K)[7 * (size_t)c]);
+      if (K && src == c && !home.empty() && home[c] == c) (*K)[7 * (size_t)c + 3] = 1.0;
+      const double x = m[0], y = m[1], z = m[2], w = m[3];
+      const double R[9] = {1 - 2 * (y * y + z * z), 2 * (x * y - z * w), 2 * (x * z + y * w),
+                           2 * (x * y + z * w), 1 - 2 * (x * x + z * z), 2 * (y * z - x * w),
+                           2 * (x * z - y * w), 2 * (y * z + x * w), 1 - 2 * (x * x + y * y)};
+      const double tx[9] = {0, -m[6], m[5], m[6], 0, -m[4], -m[5], m[4], 0};
+      S* A = &adj[36 * (size_t)c];
+      for (int r = 0; r < 3; ++r)
+        for (int k = 0; k < 3; ++k) {
+          double txr = 0;
+          for (int i = 0; i < 3; ++i) txr += tx[3 * r + i] * R[3 * i + k];
+          A[6 * r + k] = (S)R[3 * r + k];
+          A[6 * r + 3 + k] = (S)txr;
+          A[6 * (3 + r) + 3 + k] = (S)R[3 * r + k];
+        }
+      if (c == lead[c])  // exactly the identity
+        for (int k = 0; k < 36; ++k) A[k] = (k % 7 == 0) ? S(1) : S(0);
+    }
+    TRY(fit(next.lead, {}, lead.size(), &lead)); TRY(fit(next.ptr, {}, ptr.size(), &ptr)); TRY(fit(next.mem, {}, mem.size(), &mem));
+    TRY(fit(next.adj, {}, adj.size(), &adj)); TRY(fit(next.M, {}, M.size(), &M));
+    TRY(fit(next.du, rig.du, (size_t)6 * nr));
+    if (!rig.ve.get()) {
+      TRY(alloc(next.pt, (size_t)36 * nc, true)); TRY(alloc(next.fixed, (size_t)nc, true));
+      TRY(alloc(next.ve, (size_t)9 * nc, true)); TRY(alloc(next.y, (size_t)9 * nc, true));
+    }
+    return RBA_OK;
+  }
+  // Estimated extrinsics shared by the captures of one sensor (DESIGN.md section 24).  Every check runs before anything
+  // changes and the new buffers are adopted once they all exist, so a rejected or failed call leaves the previous sensors.
+  // No sensor id = the rigs of section 23 (sen.n == 0), their lead the lowest-index camera again.
+  int set_rig_sensors(const int32_t* sensor) override {
+    auto fail = [&](const std::string& what) { g_err = "rba_set_rig_sensors: " + what; return RBA_ERR_INVALID_ARGUMENT; };
+    std::vector<int> home((size_t)nc, -1), lead = rig.host_first;
+    int ns = 0;
+    if (sensor) {
+      std::vector<int> first((size_t)nc, -1), new_lead((size_t)nc, -1);
+      std::vector<std::pair<int, int>> rig_sensor;  // (the rig's lowest-index camera, sensor id) of every sensor camera
+      for (int c = 0; c < nc; ++c) {
+        const int sid = sensor[c];
+        if (sid < -1 || sid >= nc)
+          return fail("camera " + std::to_string(c) + " has sensor id " + std::to_string(sid) + ", outside [-1, " + std::to_string(nc) + ")");
+        if (sid < 0) {
+          if (rig.n && rig.host_first[c] >= 0 && new_lead[rig.host_first[c]] < 0) new_lead[rig.host_first[c]] = c;
+          continue;
+        }
+        if (!rig.n || rig.host_first[c] < 0)
+          return fail("camera " + std::to_string(c) + " has sensor id " + std::to_string(sid) + " but is not in a rig of >= 2 cameras");
+        if (first[sid] < 0) { first[sid] = c; ++ns; }
+        home[c] = first[sid];
+        rig_sensor.push_back({rig.host_first[c], sid});
+      }
+      std::sort(rig_sensor.begin(), rig_sensor.end());
+      for (size_t k = 1; k < rig_sensor.size(); ++k)
+        if (rig_sensor[k] == rig_sensor[k - 1])
+          return fail("two cameras of the rig led by camera " + std::to_string(rig_sensor[k].first) + " have sensor id " + std::to_string(rig_sensor[k].second));
+      for (int c = 0; c < nc; ++c)
+        if (rig.n && rig.host_first[c] == c && new_lead[c] < 0)
+          return fail("every camera of the rig led by camera " + std::to_string(c) + " has a sensor id: none is left to carry the rig's pose");
+      for (int c = 0; c < nc; ++c)
+        if (rig.n && rig.host_first[c] >= 0) lead[c] = new_lead[rig.host_first[c]];
+    }
+    if (!rig.n) {  // nothing to tie, nothing to clear
+      sen.n = 0;
+      return RBA_OK;
+    }
+    // the sensors in the order of their homes, each one's cameras ascending (the home first)
+    std::vector<int> sidx((size_t)nc, -1), sptr((size_t)ns + 1, 0), smem;
+    for (int c = 0, k = 0; c < nc; ++c)
+      if (home[c] == c) sidx[c] = k++;
+    for (int c = 0; c < nc; ++c)
+      if (home[c] >= 0) ++sptr[sidx[home[c]] + 1];
+    for (int k = 0; k < ns; ++k) sptr[k + 1] += sptr[k];
+    smem.resize((size_t)sptr[ns]);
+    std::vector<int> fill(sptr.begin(), sptr.end() - 1);
+    for (int c = 0; c < nc; ++c)
+      if (home[c] >= 0) smem[fill[sidx[home[c]]]++] = c;
+    RigTerm next;
+    SensorTerm snext;
+    std::vector<double> K;
+    TRY(rig_tables(lead, rig.host_E, ns ? home : std::vector<int>{}, next, ns ? &K : nullptr));
+    if (ns) {
+      TRY(fit(snext.home, {}, home.size(), &home)); TRY(fit(snext.ptr, {}, sptr.size(), &sptr)); TRY(fit(snext.mem, {}, smem.size(), &smem));
+      TRY(fit(snext.K, {}, K.size(), &K));
+      TRY(fit(snext.qt, sen.qt, (size_t)6 * nc)); TRY(fit(snext.ds, sen.ds, (size_t)6 * ns));
+      TRY(fit(snext.cam_fixed, sen.cam_fixed, (size_t)nc));
+      TRY(fit(snext.blk, sen.blk, (size_t)81 * nc)); TRY(fit(snext.b, sen.b, (size_t)9 * nc));
+    }
+    CU(cudaStreamSynchronize(stream));
+    rig.adopt(next);
+    sen.adopt(snext);
+    rig.host_lead = std::move(lead);
+    sen.n = ns;
+    sen.host_home = ns ? std::move(home) : std::vector<int>{};
+    point_at_terms();
+    TRY(upload_tied_fixed());
+    // every member re-tied from its lead: the held ones through their extrinsics, a sensor's cameras through its home's
+    TRY(rig_retie(D.cams)); TRY(rig_retie(cams_bk));
+    CU(cudaStreamSynchronize(stream));
+    ++state_version;
+    return priors_changed();
+  }
+  // The extrinsics of every camera in the convention of rba_set_camera_rigs: held ones as given (normalised), a sensor's
+  // E_s = T_home T_lead(home)^-1 E_lead(home) from the current state, free cameras the identity
+  int get_rig_extrinsics(void* out) override {
+    if (!out) { g_err = "rba_get_rig_extrinsics: cam_from_rig is NULL"; return RBA_ERR_INVALID_ARGUMENT; }
+    std::vector<S> cams((size_t)10 * nc);
+    CU(cudaMemcpyAsync(cams.data(), D.cams, cams.size() * sizeof(S), cudaMemcpyDeviceToHost, stream));
+    CU(cudaStreamSynchronize(stream));
+    S* o = (S*)out;
+    auto pose = [&](int c, double* p) { for (int k = 0; k < 7; ++k) p[k] = (double)cams[10 * (size_t)c + k]; };
+    for (int c = 0; c < nc; ++c) {
+      double e[7] = {0, 0, 0, 1, 0, 0, 0};
+      if (rig.n && rig.host_lead[c] >= 0) {
+        const int h = sen.n ? sen.host_home[c] : -1;
+        if (h < 0) {
+          for (int k = 0; k < 7; ++k) e[k] = rig.host_E[7 * (size_t)c + k];
+        } else {  // (T_home T_lead^-1) (E_lead^-1)^-1
+          const int l = rig.host_lead[h];
+          const double* el = &rig.host_E[7 * (size_t)l];
+          double th[7], tl[7], x[7], one[7] = {0, 0, 0, 1, 0, 0, 0}, ei[7];
+          pose(h, th); pose(l, tl);
+          pose_ratio(th, tl, x);
+          pose_ratio(one, el, ei);
+          pose_ratio(x, ei, e);
+        }
+      }
+      for (int k = 0; k < 7; ++k) o[7 * (size_t)c + k] = (S)e[k];
+    }
+    return RBA_OK;
   }
   // "" when every rig's members agree on RBA_FIX_POSE, else which camera does not
   std::string rig_flags_mismatch(const std::vector<int>& lead, const std::vector<uint8_t>& flags) const {
@@ -1035,19 +1191,48 @@ struct Solver : rba_handle {
   RigView<S> rigs() const {
     return {rig.lead.get(), rig.ptr.get(), rig.mem.get(), rig.adj.get(), rig.M.get(), rig.pt.get(), rig.du.get(), rig.n};
   }
+  SensorView<S> sensors() const {
+    return {sen.home.get(), sen.ptr.get(), sen.mem.get(), sen.K.get(), sen.qt.get(), sen.ds.get(), sen.b.get(), rig.fixed.get(), sen.n};
+  }
   int rig_ncb() const { return (nc + GROUP_THREADS - 1) / GROUP_THREADS; }
+  // every member at M_j T_lead through the stored M_j (at the setters' calls, and always without sensors)
   int rig_retie(S* cams) {
     k_rig_retie<S><<<(nc + 127) / 128, 128, 0, stream>>>(cams, rigs(), nc);
     ++launches;
     return RBA_OK;
   }
-  int rig_expand(const S* v, S* out, bool in_solve, int host = 0) {
-    return launch_ex(k_rig_expand<S>, rig_ncb() + rig.n, GROUP_THREADS, 0, in_solve, 1, v, out, rigs(), nc, rig_ncb(), host,
-                     in_solve ? (const PcgState*)d_state : (const PcgState*)nullptr);
+  // after a camera update or rba_set_state: with sensors their cameras follow their homes (k_sensor_retie)
+  int rig_retie_state(S* cams) {
+    if (!sen.n) return rig_retie(cams);
+    k_sensor_retie<S><<<(nc + 127) / 128, 128, 0, stream>>>(cams, rigs(), sensors(), nc);
+    ++launches;
+    return RBA_OK;
   }
-  // inc = P~ u (and P u of the groups) for the back-substitution, the update and inc_out
+  // M_j and A_j of the sensor cameras at the current state
+  int sensor_tie() {
+    k_sensor_tie<S><<<(nc + 127) / 128, 128, 0, stream>>>(D.cams, rigs(), sensors(), rig.M.get(), rig.adj.get(), nc);
+    ++launches;
+    return RBA_OK;
+  }
+  int rig_expand(const S* v, S* out, bool in_solve, int host = 0) {
+    const PcgState* st = in_solve ? (const PcgState*)d_state : (const PcgState*)nullptr;
+    if (sen.n)
+      return launch_ex(k_rig_expand<S, true>, rig_ncb() + rig.n, GROUP_THREADS, 0, in_solve, 1, v, out, rigs(), nc, rig_ncb(), host, st,
+                       sensors());
+    return launch_ex(k_rig_expand<S>, rig_ncb() + rig.n, GROUP_THREADS, 0, in_solve, 1, v, out, rigs(), nc, rig_ncb(), host, st,
+                     NoSensors{});
+  }
+  // the contracted operator output the vector step reads: the groups' unless rigs contract out of place (sensors)
+  S* tied_y() const { return grp.n && !sen.n ? grp.y.get() : rig.y.get(); }
+  // inc = P~ u (and P u of the groups) for the back-substitution, the update and inc_out (with sensors out of place: the
+  // homes' entries are read across rigs)
   int tie_expand(S* inc) {
-    if (rig.n) TRY(rig_expand(inc, inc, false));
+    if (rig.n && sen.n) {
+      CU(cudaMemcpyAsync(rig.ve.get(), inc, (size_t)9 * nc * sizeof(S), cudaMemcpyDeviceToDevice, stream));
+      TRY(rig_expand(rig.ve.get(), inc, false));
+    } else if (rig.n) {
+      TRY(rig_expand(inc, inc, false));
+    }
     if (grp.n) TRY(group_expand(inc, inc, false));
     return RBA_OK;
   }
@@ -1132,7 +1317,7 @@ struct Solver : rba_handle {
   }
   // The kernels' optional pointers, from the problem terms (nullptr = the kernels without the term)
   void point_at_terms() {
-    D.cam_fixed = held.host.empty() ? nullptr : held.flags.get();
+    D.cam_fixed = held.host.empty() ? nullptr : sen.n ? sen.cam_fixed.get() : held.flags.get();
     D.prior_H = cprior.on || pprior.n > 0 ? cprior.H.get() : nullptr;
     D.pair_ptr = pprior.ptr.get(); D.pair_nbr = pprior.nbr.get(); D.pair_O = pprior.O.get();
     D.pair_ov = pprior.n > 0 ? pprior.ov.get() : nullptr;
@@ -1597,7 +1782,13 @@ struct Solver : rba_handle {
       // hold the observation Gram and the priors' H; with SCHUR_JACOBI they are unused, so they take the observation Gram
       // here and the priors' H is added in k_rig_scaling)
       if (!jac) { rc = precond_blocks(0, D.jblocks, nullptr, true); if (rc) return rc; }
-      k_rig_scaling<S><<<rig.n, GROUP_THREADS, 0, stream>>>(D.jblocks, jac ? nullptr : (const S*)D.prior_H, D, rigs(), (S)ko.jacobi_eps);
+      // (sensors, section 24: A_j of their cameras from the state first, then D_s and Q~ in the blocks after the rigs')
+      if (sen.n) TRY(sensor_tie());
+      const S* pH = jac ? nullptr : (const S*)D.prior_H;
+      if (sen.n)
+        k_rig_scaling<S, true><<<rig.n + sen.n, GROUP_THREADS, 0, stream>>>(D.jblocks, pH, D, rigs(), (S)ko.jacobi_eps, sensors());
+      else
+        k_rig_scaling<S><<<rig.n, GROUP_THREADS, 0, stream>>>(D.jblocks, pH, D, rigs(), (S)ko.jacobi_eps, NoSensors{});
       ++launches;
     }
     if (panel_form()) {
@@ -1727,7 +1918,7 @@ struct Solver : rba_handle {
     if (!fused_ar) c.nranks = 1;
     DevPtrs<S> Dv = D;
     if (grp.n || rig.n) {  // the contracted output, which holds the prior terms already (k_group_contract, k_rig_contract)
-      Dv.y = grp.n ? grp.y.get() : rig.y.get(); Dv.prior_H = nullptr; Dv.pair_ov = nullptr;
+      Dv.y = tied_y(); Dv.prior_H = nullptr; Dv.pair_ov = nullptr;
     }
     if (Dv.pair_ov && mode != 3) TRY(pair_ov(mode == 2 ? D.x : D.p, pdl));
     auto kern = Dv.pair_ov ? k_pcg_vec<S, true, true> : Dv.prior_H ? k_pcg_vec<S, true> : k_pcg_vec<S, false>;
@@ -1757,11 +1948,13 @@ struct Solver : rba_handle {
     if (grp.n)
       TRY(launch_ex(k_group_contract<S>, (nc + GROUP_THREADS - 1) / GROUP_THREADS + grp.n, GROUP_THREADS, 0, pdl, 1,
                     D, v, grp.y.get(), groups(), (nc + GROUP_THREADS - 1) / GROUP_THREADS, (const PcgState*)d_state));
-    if (rig.n) {
-      S* y = grp.n ? grp.y.get() : rig.y.get();
-      TRY(launch_ex(k_rig_contract<S>, rig_ncb() + rig.n, GROUP_THREADS, 0, pdl, 1, D, v, grp.n ? (const S*)y : (const S*)nullptr,
-                    y, rigs(), rig_ncb(), (const PcgState*)d_state));
-    }
+    const S* in = grp.n ? (const S*)grp.y.get() : (const S*)nullptr;
+    if (rig.n && sen.n)  // (out of place, from the groups' output into rig.y)
+      TRY(launch_ex(k_rig_contract<S, true>, rig_ncb() + rig.n + sen.n, GROUP_THREADS, 0, pdl, 1, D, v, in, tied_y(), rigs(), rig_ncb(),
+                    (const PcgState*)d_state, sensors()));
+    else if (rig.n)
+      TRY(launch_ex(k_rig_contract<S>, rig_ncb() + rig.n, GROUP_THREADS, 0, pdl, 1, D, v, in, tied_y(), rigs(), rig_ncb(),
+                    (const PcgState*)d_state, NoSensors{}));
     return pcg_vec(i, mode, h != Handover::Nccl, is_last, lambda, h == Handover::Peer, h == Handover::Partials);
   }
   // Enqueue iterations 1..last in chunks of `chunk` (enqueue(i)); after each chunk the PcgState is copied into one of two
@@ -1851,7 +2044,14 @@ struct Solver : rba_handle {
         k_group_precond<S><<<ncb + n_groups, GROUP_THREADS, 0, stream>>>(src, pH, pg, D.b, D.blocks, groups(), nc, ncb);
         src = D.blocks; pH = nullptr; pg = nullptr;
       }
-      if (rig.n) k_rig_precond<S><<<ncb + rig.n, GROUP_THREADS, 0, stream>>>(src, pH, pg, D.b, D.blocks, rigs(), nc, ncb);
+      if (rig.n && sen.n) {  // (sensors: out of place, from copies of the blocks and b)
+        CU(cudaMemcpyAsync(sen.blk.get(), src, (size_t)81 * nc * sizeof(S), cudaMemcpyDeviceToDevice, stream));
+        CU(cudaMemcpyAsync(sen.b.get(), D.b, (size_t)9 * nc * sizeof(S), cudaMemcpyDeviceToDevice, stream));
+        k_rig_precond<S, true><<<ncb + rig.n + sen.n, GROUP_THREADS, 0, stream>>>(sen.blk.get(), pH, pg, D.b, D.blocks, rigs(), nc, ncb,
+                                                                                 sensors());
+      } else if (rig.n) {
+        k_rig_precond<S><<<ncb + rig.n, GROUP_THREADS, 0, stream>>>(src, pH, pg, D.b, D.blocks, rigs(), nc, ncb, NoSensors{});
+      }
       k_precond_invert<S><<<(nc + 63) / 64, 64, 0, stream>>>(D.blocks, lambda, nc, schur ? D.blocks : nullptr, D.inv, tied_fixed(), D.b);
       launches += 1 + (grp.n > 0) + (rig.n > 0);
     } else {
@@ -2007,7 +2207,7 @@ struct Solver : rba_handle {
       // then rejects the step and restores the backup, so updating unconditionally is equivalent for the caller.
       k_camera_update<S><<<(nc + 127) / 128, 128, 0, stream>>>(D, D.inc);
       ++launches;
-      if (rig.n) TRY(rig_retie(D.cams));  // the members exactly at M_j T_lead: no drift over the iterations
+      if (rig.n) TRY(rig_retie_state(D.cams));  // the members exactly at M_j T_lead: no drift over the iterations
     }
     rc = stop(ev_update); if (rc) return rc;
     CU(cudaMemcpyAsync(&h_res->l_diff, d_red, sizeof(double), cudaMemcpyDeviceToHost, stream));
@@ -2311,9 +2511,13 @@ struct Solver : rba_handle {
   }
   // P^T A P (expand = 0) or P A P^T (expand = 1) of the rigs' adjoint map, in place (full; DESIGN.md section 23)
   int cov_rig_passes(double* A, long long ld, long long n, int expand) {
+    if (sen.n && !expand) TRY(sensor_tie());  // (sensors: M_j at the state the matrix is assembled at)
     k_cov_group_symmetrize<<<dim3((unsigned)((n + 31) / 32), (unsigned)((n + 7) / 8)), dim3(32, 8), 0, stream>>>(A, ld, n);
     for (int columns = 0; columns < 2; ++columns)
-      k_cov_rig_pass<S><<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(A, ld, n, rigs(), columns, expand);
+      if (sen.n)
+        k_cov_rig_pass<S, true><<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(A, ld, n, rigs(), columns, expand, sensors());
+      else
+        k_cov_rig_pass<S><<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(A, ld, n, rigs(), columns, expand, NoSensors{});
     CU(cudaGetLastError());
     return RBA_OK;
   }
@@ -2782,6 +2986,8 @@ int32_t rba_set_landmark_prior(rba_handle* h, int32_t num, const int32_t* lm_idx
 }
 int32_t rba_set_intrinsics_groups(rba_handle* h, const int32_t* group) { return h->set_intrinsics_groups(group); }
 int32_t rba_set_camera_rigs(rba_handle* h, const int32_t* rig, const void* cam_from_rig) { return h->set_camera_rigs(rig, cam_from_rig); }
+int32_t rba_set_rig_sensors(rba_handle* h, const int32_t* sensor) { return h->set_rig_sensors(sensor); }
+int32_t rba_get_rig_extrinsics(rba_handle* h, void* cam_from_rig) { return h->get_rig_extrinsics(cam_from_rig); }
 int32_t rba_set_observation_info(rba_handle* h, const void* sqrt_info) { return h->set_observation_info(sqrt_info); }
 int32_t rba_set_observation_loss(rba_handle* h, const uint8_t* kind, const void* scale) { return h->set_observation_loss(kind, scale); }
 int32_t rba_set_prior_loss(rba_handle* h, int32_t prior_kind, int32_t num, const uint8_t* kind, const void* scale) {

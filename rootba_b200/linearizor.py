@@ -114,6 +114,32 @@ def _camera_rig_arrays(rig, num_cameras: int, dtype):
     return np.ascontiguousarray(a, dtype=np.int32).copy(), e
 
 
+def _rig_sensor_array(sensor, camera_rig, num_cameras: int):
+    """None, or a validated contiguous int32 copy of rig sensor ids (-1 = the camera's extrinsics are held, else an id in
+    [0, num_cameras) shared by every capture of one sensor): every camera with an id must be in a rig of >= 2 cameras of
+    `camera_rig`, no two cameras of one rig may share an id, and every rig keeps a camera without one"""
+    if sensor is None:
+        return None
+    a = np.asarray(sensor)
+    if a.shape != (num_cameras,):
+        raise ValueError(f"rig_sensor ids must have one entry per camera ({num_cameras}), got shape {a.shape}")
+    if a.dtype.kind not in "iu" or np.any(a < -1) or np.any(a >= num_cameras):
+        raise ValueError(f"rig_sensor ids must be integers in [-1, {num_cameras})")
+    a = np.ascontiguousarray(a, dtype=np.int32).copy()
+    rig = np.full(num_cameras, -1) if camera_rig is None else np.asarray(camera_rig[0])
+    rid, count = np.unique(rig[rig >= 0], return_counts=True)
+    in_rig = np.isin(rig, rid[count >= 2])
+    if np.any((a >= 0) & ~in_rig):
+        raise ValueError(f"rig_sensor: camera {int(np.flatnonzero((a >= 0) & ~in_rig)[0])} has a sensor id but is not in a rig of >= 2 cameras")
+    for r in rid[count >= 2]:
+        s = a[rig == r]
+        if np.all(s >= 0):
+            raise ValueError(f"rig_sensor: every camera of rig {int(r)} has a sensor id; none is left to carry the rig's pose")
+        if len(np.unique(s[s >= 0])) != int(np.sum(s >= 0)):
+            raise ValueError(f"rig_sensor: two cameras of rig {int(r)} have the same sensor id")
+    return a
+
+
 def _prior_arrays(name, mean, sqrt_info, dtype, m, mean_len, dim, check_index=None, item=None):
     """validated contiguous copies (mean [m, mean_len], sqrt_info [m, dim, dim]) in `dtype` of the priors `name`.  The checks
     run in this order: the shapes, the kind's own index checks (`check_index`), finiteness and, for a kind whose mean
@@ -251,6 +277,9 @@ class BalProblem:
     camera (-1 = free camera) and each camera's fixed extrinsics (qx,qy,qz,qw, tx,ty,tz of cam_from_rig); the cameras of a rig
     keep the relative poses of their extrinsics and the solve moves one pose per rig (rba_set_camera_rigs, DESIGN.md section
     23).  Forwarded likewise.
+    `rig_sensor` (not in the reference): None or one int32 sensor id per camera (-1 = the camera's extrinsics are held, as
+    given to camera_rig); the cameras with one id are captures of one physical camera whose extrinsics are estimated and
+    shared (rba_set_rig_sensors, DESIGN.md section 24).  Forwarded likewise; setting camera_rig clears it.
     `observation_sqrt_info` (not in the reference): None, [Nobs] (1 / sigma per observation) or [Nobs,2,2] (a square root W of
     the inverse keypoint covariance per observation, in the order of obs_cam / obs_xy); the observation's cost becomes
     rho(|W r|^2) and W = 0 switches it off (rba_set_observation_info, DESIGN.md section 19).  Stored as [Nobs,2,2]; forwarded
@@ -281,6 +310,7 @@ class BalProblem:
         self._landmark_prior = None
         self._intrinsics_group = None
         self._camera_rig = None
+        self._rig_sensor = None
         self._observation_sqrt_info = None
         self._observation_loss = None
         self._prior_loss = {_lib.PRIOR_CAMERA: None, _lib.PRIOR_PAIR: None, _lib.PRIOR_LANDMARK: None}
@@ -367,6 +397,18 @@ class BalProblem:
         if self._linearizor is not None:
             self._linearizor._upload_camera_rig(r)  # raises on rejection: the previous rigs stay in force
         self._camera_rig = r
+        self._rig_sensor = None  # the sensors belonged to the previous rigs
+
+    @property
+    def rig_sensor(self):
+        return self._rig_sensor
+
+    @rig_sensor.setter
+    def rig_sensor(self, sensor):
+        a = _rig_sensor_array(sensor, self._camera_rig, self.num_cameras())
+        if self._linearizor is not None:
+            self._linearizor._upload_rig_sensor(a)  # raises on rejection: the previous sensors stay in force
+        self._rig_sensor = a
 
     @property
     def landmark_prior(self):
@@ -526,6 +568,8 @@ class LinearizorQR:
             self._upload_intrinsics_group(bal_problem.intrinsics_group)
         if bal_problem.camera_rig is not None:
             self._upload_camera_rig(bal_problem.camera_rig)
+        if bal_problem.rig_sensor is not None:
+            self._upload_rig_sensor(bal_problem.rig_sensor)
         if bal_problem.observation_sqrt_info is not None:
             self._upload_observation_info(bal_problem.observation_sqrt_info)
         if bal_problem.observation_loss is not None:
@@ -621,6 +665,21 @@ class LinearizorQR:
             check(_lib.lib().rba_set_camera_rigs(self.h, None, None))
         else:
             check(_lib.lib().rba_set_camera_rigs(self.h, _p(rig[0]), _p(rig[1])))
+
+    def set_rig_sensors(self, sensor):
+        """estimated rig extrinsics (rba_set_rig_sensors): None, or one int32 sensor id per camera (-1 = held extrinsics).
+        Every member is re-tied from its lead; needs a new linearize before the next solve.  Stored on the BalProblem."""
+        self.bal_problem.rig_sensor = sensor  # validates, forwards to _upload_rig_sensor
+
+    def _upload_rig_sensor(self, sensor):
+        check(_lib.lib().rba_set_rig_sensors(self.h, None if sensor is None else _p(sensor)))
+
+    def rig_extrinsics(self):
+        """[nc, 7] every camera's current cam_from_rig (qx,qy,qz,qw, tx,ty,tz; rba_get_rig_extrinsics): held ones as given,
+        an estimated sensor's from the current state, free cameras the identity"""
+        out = np.zeros((self.bal_problem.num_cameras(), 7), self.bal_problem.dtype)
+        check(_lib.lib().rba_get_rig_extrinsics(self.h, _p(out)))
+        return out
 
     def set_observation_info(self, info):
         """per-observation square-root information (rba_set_observation_info): None, [Nobs] (1 / sigma) or [Nobs,2,2] in the

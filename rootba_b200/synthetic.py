@@ -330,3 +330,91 @@ def write_bal(prob: BalArrays, path: str) -> None:
         for i in range(prob.nl):
             for v in prob.lms[i]:
                 f.write(f"{v:.17g}\n")
+
+
+@dataclasses.dataclass
+class RigCapture:
+    """A synthetic capture of a rigid multi-camera body (synth_rig_capture) and its truth."""
+
+    prob: BalArrays          # the true cameras and landmarks, noise-free observations (nothing perturbed)
+    rig: np.ndarray          # [nc] int32 placement (rig id) of each camera: camera f * K + k is sensor k at placement f
+    sensor: np.ndarray       # [nc] int32 sensor of each camera
+    cam_from_rig: np.ndarray  # [nc, 7] the true extrinsics of each camera's sensor (qx,qy,qz,qw, tx,ty,tz)
+    rig_from_world: np.ndarray  # [F, 7] the true pose of every placement
+
+
+def synth_rig_capture(num_sensors: int, num_placements: int, num_landmarks: int, seed: int = 38401, *,
+                      radius: float = 0.15, step: float = 0.6, focal: float = 500.0, max_tan: float = 0.9,
+                      max_depth: float = 12.0) -> RigCapture:
+    """A seeded rig capture: `num_sensors` cameras on a ring of `radius` around the rig's origin, looking outward and evenly
+    spread in yaw (a spherical head), placed `num_placements` times along a gently curving path with `step` between
+    placements, and landmarks scattered 3 to 15 units beside the path.  Every landmark keeps the cameras it lies in front of,
+    at a depth below max_depth and within |x/z|, |y/z| <= max_tan; landmarks seen fewer than twice are dropped.  Returns the truth; perturb it to test."""
+    rng = np.random.default_rng(seed)
+    K, F = num_sensors, num_placements
+    # sensor k: yaw 2 pi k / K (+ a little tilt), centre on the ring; camera axes as rows (rig -> camera rotation)
+    E = np.zeros((K, 7))
+    for k in range(K):
+        yaw = 2 * np.pi * k / K + rng.normal(0, 0.02)
+        zc = np.array([np.cos(yaw), np.sin(yaw), rng.normal(0, 0.05)])
+        zc /= np.linalg.norm(zc)
+        xc = np.cross(zc, [0.0, 0.0, 1.0])
+        xc /= np.linalg.norm(xc)
+        yc = np.cross(zc, xc)
+        R = np.stack([xc, yc, zc])
+        c = radius * np.array([np.cos(yaw), np.sin(yaw), 0.0]) + rng.normal(0, 0.01, 3)
+        E[k, :4] = rot_to_quat(R)[0]
+        E[k, 4:] = -R @ c
+    # placements along the path: rig origin p_f, heading following the path
+    s = step * np.arange(F)
+    P = np.stack([s, 2.0 * np.sin(s / 15.0), 0.1 * np.sin(s / 4.0)], axis=1)
+    head = np.arctan2(np.gradient(P[:, 1]), np.gradient(P[:, 0]))
+    T = np.zeros((F, 7))
+    for f in range(F):
+        ch, sh = np.cos(head[f]), np.sin(head[f])
+        R = np.array([[ch, sh, 0.0], [-sh, ch, 0.0], [0.0, 0.0, 1.0]])  # world -> rig
+        T[f, :4] = rot_to_quat(R)[0]
+        T[f, 4:] = -R @ P[f]
+    # cameras T_c = E_k T_f
+    nc = K * F
+    cams = np.zeros((nc, 10))
+    cams[:, 7] = focal
+    for f in range(F):
+        Rf = quat_to_rot(T[f, :4])
+        for k in range(K):
+            Rk = quat_to_rot(E[k, :4])
+            c = f * K + k
+            cams[c, :4] = rot_to_quat(Rk @ Rf)[0]
+            cams[c, 4:7] = Rk @ T[f, 4:] + E[k, 4:]
+    # landmarks beside the path
+    i = rng.integers(0, F, num_landmarks)
+    dist = rng.uniform(3.0, 15.0, num_landmarks)
+    ang = rng.uniform(0, 2 * np.pi, num_landmarks)
+    lms = P[i] + np.stack([dist * np.cos(ang), dist * np.sin(ang), rng.normal(0, 2.0, num_landmarks)], axis=1)
+    obs_cam, lm_of, xy = [], [], []
+    for lo in range(0, num_landmarks, 4096):  # visibility in chunks of landmarks
+        l = np.arange(lo, min(lo + 4096, num_landmarks))
+        R = quat_to_rot(cams[:, :4])
+        pc = np.einsum("cij,lj->lci", R, lms[l]) + cams[None, :, 4:7]
+        z = pc[..., 2]
+        with np.errstate(divide="ignore", invalid="ignore"):
+            m = pc[..., :2] / z[..., None]
+        vis = (z > 0.5) & (z < max_depth) & (np.abs(m).max(axis=-1) <= max_tan)
+        ll, cc = np.nonzero(vis)
+        obs_cam.append(cc)
+        lm_of.append(l[ll])
+    obs_cam, lm_of = np.concatenate(obs_cam), np.concatenate(lm_of)
+    n = np.bincount(lm_of, minlength=num_landmarks)
+    ok = n >= 2
+    keep = ok[lm_of]
+    obs_cam, lm_of = obs_cam[keep], lm_of[keep]
+    new_id = np.cumsum(ok) - 1
+    lm_of = new_id[lm_of]
+    order = np.lexsort((obs_cam, lm_of))
+    obs_cam, lm_of = obs_cam[order].astype(np.int32), lm_of[order]
+    lms = lms[ok]
+    xy, _ = project(cams[obs_cam], lms[lm_of])
+    lm_off = np.concatenate([[0], np.cumsum(np.bincount(lm_of, minlength=lms.shape[0]))]).astype(np.int64)
+    rig = np.repeat(np.arange(F), K).astype(np.int32)
+    sensor = np.tile(np.arange(K), F).astype(np.int32)
+    return RigCapture(BalArrays(cams, lms, lm_off, obs_cam, xy), rig, sensor, E[sensor].copy(), T)
