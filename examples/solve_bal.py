@@ -7,6 +7,7 @@
         [--relative-covariance PAIRS.npy] [--observation-info FILE.npy] [--observation-loss KIND:SCALE | FILE.npz]
         [--residuals OUT.npz] [--camera-prior-loss KIND:SCALE | FILE.npz] [--pair-prior-loss KIND:SCALE | FILE.npz]
         [--landmark-prior-loss KIND:SCALE | FILE.npz] [--prior-residuals OUT.npz]
+        [--triangulate linear|refine|linear+refine [--triangulation OUT.npz]]
 
 Mirrors what `bal_qr --input ...` of the reference does (src/app/bal_qr.cpp): load + normalise (bal_problem.cpp:773-852),
 optimize_lm_ours with the QR linearizor (solver/bal_bundle_adjustment.cpp:249-544), log (bal/ba_log.hpp)."""
@@ -19,6 +20,7 @@ import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import rootba_b200 as rb  # noqa: E402
+from rootba_b200 import _lib  # noqa: E402
 
 
 def read_loss(ap, flag, value):
@@ -105,7 +107,13 @@ def main():
     ap.add_argument("--prior-residuals", default=None, metavar="OUT.npz",
                     help="after the solve, write per prior kind given `<kind>_residual` [num, 9 | 6 | 3] (L e) and "
                          "`<kind>_robust_weight` [num] at the final state, kind camera, pair or landmark (DESIGN.md section 22)")
+    ap.add_argument("--triangulate", default=None, choices=["linear", "refine", "linear+refine"],
+                    help="before the solve, re-initialise every landmark from the loaded cameras (DESIGN.md section 25)")
+    ap.add_argument("--triangulation", default=None, metavar="OUT.npz",
+                    help="with --triangulate, write per landmark `status` (RBA_TRI_* bits), `angle` [rad] and `cost`")
     args = ap.parse_args()
+    if args.triangulation and not args.triangulate:
+        ap.error("--triangulation requires --triangulate")
     if args.relative_covariance and not args.covariance:
         ap.error("--relative-covariance requires --covariance")
     rel_pairs = None
@@ -193,6 +201,16 @@ def main():
                 ap.error(f"{flag}: {e}")
     options = rb.SolverOptions(max_num_iterations=args.max_num_iterations, preconditioner_type=args.preconditioner_type,
                                operator_form=args.operator_form, use_double=not args.float)
+    if args.triangulate:
+        lin_tri = rb.LinearizorQR.create(problem, options)  # the new positions go back into `problem`
+        status, angle, cost = lin_tri.triangulate(mode=args.triangulate)
+        lin_tri.close()
+        written = int(np.count_nonzero(status & _lib.TRI_WRITTEN))
+        print(f"triangulated ({args.triangulate}): {written} of {len(status)} landmarks written, "
+              f"{int(np.count_nonzero(status & _lib.TRI_FEW_RAYS))} with fewer than 2 usable rays")
+        if args.triangulation:
+            np.savez(args.triangulation, status=status, angle=angle, cost=cost)
+            print("wrote", args.triangulation)
     if args.rig_extrinsics and problem.camera_rig is None:
         ap.error("--rig-extrinsics needs --camera-rigs")
     lin_ba = rb.LinearizorQR.create(problem, options) if args.rig_extrinsics else None

@@ -505,6 +505,57 @@ int32_t rba_set_prior_loss(rba_handle* h, int32_t prior_kind, int32_t num, const
  * the handle (scratch device memory is allocated for the call and freed before it returns). */
 int32_t rba_get_prior_residuals(rba_handle* h, int32_t prior_kind, void* residual, void* robust_weight);
 
+/* ---- Triangulation of landmarks from the current cameras (DESIGN.md section 25) ------------ */
+
+#define RBA_TRIANGULATE_LINEAR 1   /* replace the position by the linear estimate from the rays */
+#define RBA_TRIANGULATE_REFINE 2   /* minimise the landmark's own cost with the cameras held */
+
+#define RBA_TRI_WRITTEN     1u     /* the landmark's position changed */
+#define RBA_TRI_FEW_RAYS    2u     /* < 2 usable rays */
+#define RBA_TRI_SMALL_ANGLE 4u     /* largest ray angle < min_angle */
+#define RBA_TRI_AT_INFINITY 8u     /* linear estimate at (or beyond) infinity */
+#define RBA_TRI_BEHIND      16u    /* linear estimate behind a camera of a usable ray */
+#define RBA_TRI_REFINED     32u    /* the refinement accepted at least one step */
+#define RBA_TRI_CONVERGED   64u    /* the refinement met function_tolerance */
+
+typedef struct {
+  int32_t mode;               /* RBA_TRIANGULATE_* bits, 1..3; default LINEAR | REFINE */
+  int32_t max_iterations;     /* refinement iterations per landmark, rejected steps included; default 20 */
+  double min_angle;           /* radians, >= 0; default 0 */
+  double function_tolerance;  /* stop once a step changes the cost by less than this fraction; default 1e-10 */
+  int32_t reserved[2];
+} rba_triangulate_opts;       /* 32 bytes, no implicit padding */
+
+void rba_default_triangulate_opts(rba_triangulate_opts* o);
+/* Not in the reference.  Re-initialises landmark positions from the handle's current cameras, which are held: a problem
+ * assembled from feature tracks, landmarks left behind by an outlier loop (W = 0) or by moved rig extrinsics.
+ * lm_idx [num] int32 lists landmarks by problem index; NULL = every landmark, num must then be Nl.  Outputs are in the
+ * caller's order and any of them may be NULL: status [num] RBA_TRI_* bits, angle [num] the largest angle (radians) between
+ * two usable rays (0 with fewer than 2), cost [num] the landmark's share of rba_compute_error at its final stored position.
+ * A sharded handle follows rba_set_landmark_prior: every rank passes the same full list, works on the entries of its own
+ * shard and writes only those outputs.  Evaluated in float64 for either Scalar; a written position is rounded to Scalar.
+ * A usable ray is an observation in use (W != 0) with f != 0 whose distortion inverts: rho (1 + k1 rho^2 + k2 rho^4) =
+ * |obs| / |f| solved by Newton from rho = |obs / f| with a fixed iteration cap, failing when 1 + 3 k1 rho^2 + 5 k2 rho^4 <= 0
+ * at an iterate or when it does not converge.  The ray is R^T (m, 1) from the centre c = -R^T t.
+ * LINEAR: the homogeneous midpoint estimate (the smallest eigenvector of sum_i A_i^T A_i, A_i = (I - d d^T) [R | t], in
+ * coordinates centred on the track's mean camera centre and scaled by their RMS distance), rejected as AT_INFINITY when
+ * |X_h[3]| <= 1e-10 |X_h| and as BEHIND when its depth is below eps_sqrt of the Scalar in a camera of a usable ray; a
+ * rejected estimate is not written.  REFINE: Levenberg-Marquardt on the landmark's share of the cost (its observations' own
+ * losses or the handle's robust norm, the observation information, use_valid_projections_only, its landmark prior and that
+ * prior's loss), IRLS-weighted normal equations; a step is accepted only when the cost decreases and no observation in use
+ * goes from valid to invalid depth.  It starts from the position LINEAR left (or the current one without LINEAR), and its
+ * result is written only when its cost, after rounding to Scalar, is below the cost at its start.  FEW_RAYS and
+ * SMALL_ANGLE landmarks are left untouched, except that a FEW_RAYS landmark with a landmark prior is still refined.
+ * The call is a state change: the state version is bumped, the error cache and the device-resident increment are
+ * discarded and rba_solve returns RBA_ERR_STATE until the next rba_linearize.  rba_backup is untouched, so rba_restore
+ * brings the previous landmarks back.  Cameras, rigs, sensors, groups, held flags and priors are read only.  Scratch device
+ * memory is allocated for the call and freed before it returns.
+ * RBA_ERR_INVALID_ARGUMENT before any device work, with nothing changed: o NULL, mode outside 1..3, max_iterations < 0,
+ * min_angle or function_tolerance negative or not finite, num < 0, lm_idx NULL with num != Nl, an index outside [0, Nl) or
+ * a repeated index. */
+int32_t rba_triangulate_landmarks(rba_handle* h, const rba_triangulate_opts* o, int32_t num, const int32_t* lm_idx,
+                                  uint8_t* status, double* angle, double* cost);
+
 /* ---- Marginal covariances (DESIGN.md section 16) ------------------------------------------ */
 
 /* Not in the reference.  DESIGN.md section 16.  The covariance of the Gauss-Newton step of the total objective (reprojection

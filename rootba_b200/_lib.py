@@ -41,6 +41,19 @@ PRIOR_LANDMARK = 2
 PRIOR_KINDS = {"camera": PRIOR_CAMERA, "pair": PRIOR_PAIR, "landmark": PRIOR_LANDMARK}
 PRIOR_ROWS = {PRIOR_CAMERA: 9, PRIOR_PAIR: 6, PRIOR_LANDMARK: 3}
 
+# rba_triangulate_landmarks: mode bits (RBA_TRIANGULATE_*) and status bits (RBA_TRI_*)
+TRIANGULATE_LINEAR = 1
+TRIANGULATE_REFINE = 2
+TRIANGULATE_MODES = {"linear": TRIANGULATE_LINEAR, "refine": TRIANGULATE_REFINE,
+                     "linear+refine": TRIANGULATE_LINEAR | TRIANGULATE_REFINE}
+TRI_WRITTEN = 1
+TRI_FEW_RAYS = 2
+TRI_SMALL_ANGLE = 4
+TRI_AT_INFINITY = 8
+TRI_BEHIND = 16
+TRI_REFINED = 32
+TRI_CONVERGED = 64
+
 
 class RbaError(RuntimeError):
     def __init__(self, code: int, msg: str):
@@ -115,6 +128,11 @@ class CovarianceQuery(C.Structure):
                 ("cam_cov", C.c_void_p), ("lm_cov", C.c_void_p)]
 
 
+class TriangulateOpts(C.Structure):
+    _fields_ = [("mode", C.c_int32), ("max_iterations", C.c_int32), ("min_angle", C.c_double),
+                ("function_tolerance", C.c_double), ("reserved", C.c_int32 * 2)]
+
+
 def struct_to_dict(s: C.Structure) -> dict:
     out = {}
     for name, _ in s._fields_:
@@ -161,6 +179,10 @@ def lib():
         _lib.rba_set_camera_rigs.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
         _lib.rba_set_rig_sensors.argtypes = [C.c_void_p, C.c_void_p]
         _lib.rba_get_rig_extrinsics.argtypes = [C.c_void_p, C.c_void_p]
+        _lib.rba_default_triangulate_opts.argtypes = [C.POINTER(TriangulateOpts)]
+        _lib.rba_default_triangulate_opts.restype = None
+        _lib.rba_triangulate_landmarks.argtypes = [C.c_void_p, C.POINTER(TriangulateOpts), C.c_int32, C.c_void_p, C.c_void_p,
+                                                   C.c_void_p, C.c_void_p]
     return _lib
 
 

@@ -31,40 +31,67 @@ constexpr double COV_PIVOT_TAU = 1e-10;  // a Cholesky pivot <= this of the equi
 // ------------------------------------------------------------------------------------------------
 // 1. per-landmark elimination
 // ------------------------------------------------------------------------------------------------
-// symmetric 3x3 eigendecomposition by cyclic Jacobi rotations: on return A holds the eigenvalues on its diagonal and the
-// columns of V (row-major) the eigenvectors.  Fixed number of sweeps: the same operations on every run.
-__device__ __forceinline__ void cov_sym3_eig(double (&A)[9], double (&V)[9]) {
+// symmetric NxN eigendecomposition by cyclic Jacobi rotations, pairs (p, q) in row order: on return A holds the eigenvalues
+// on its diagonal and the columns of V (row-major) the eigenvectors.  Fixed number of sweeps: the same operations on every
+// run.  N = 3: the landmark blocks here; N = 4: the homogeneous triangulation (triangulate.cuh).
+template <int N>
+__device__ __forceinline__ void sym_eig(double (&A)[N * N], double (&V)[N * N]) {
 #pragma unroll
-  for (int k = 0; k < 9; ++k) V[k] = (k % 4 == 0) ? 1.0 : 0.0;
+  for (int k = 0; k < N * N; ++k) V[k] = (k % (N + 1) == 0) ? 1.0 : 0.0;
   for (int sweep = 0; sweep < 8; ++sweep) {
 #pragma unroll
-    for (int pq = 0; pq < 3; ++pq) {
-      const int p = pq == 2 ? 1 : 0, q = pq == 0 ? 1 : 2;
-      const double apq = A[3 * p + q];
-      if (apq == 0.0) continue;
-      const double th = (A[3 * q + q] - A[3 * p + p]) / (2.0 * apq);
-      const double t = (th >= 0 ? 1.0 : -1.0) / (fabs(th) + sqrt(th * th + 1.0));
-      const double c = 1.0 / sqrt(t * t + 1.0), s = t * c;
+    for (int p = 0; p < N - 1; ++p) {
 #pragma unroll
-      for (int k = 0; k < 3; ++k) {  // columns p, q
-        const double akp = A[3 * k + p], akq = A[3 * k + q];
-        A[3 * k + p] = c * akp - s * akq;
-        A[3 * k + q] = s * akp + c * akq;
-      }
+      for (int q = p + 1; q < N; ++q) {
+        const double apq = A[N * p + q];
+        if (apq == 0.0) continue;
+        const double th = (A[N * q + q] - A[N * p + p]) / (2.0 * apq);
+        const double t = (th >= 0 ? 1.0 : -1.0) / (fabs(th) + sqrt(th * th + 1.0));
+        const double c = 1.0 / sqrt(t * t + 1.0), s = t * c;
 #pragma unroll
-      for (int k = 0; k < 3; ++k) {  // rows p, q
-        const double apk = A[3 * p + k], aqk = A[3 * q + k];
-        A[3 * p + k] = c * apk - s * aqk;
-        A[3 * q + k] = s * apk + c * aqk;
-      }
+        for (int k = 0; k < N; ++k) {  // columns p, q
+          const double akp = A[N * k + p], akq = A[N * k + q];
+          A[N * k + p] = c * akp - s * akq;
+          A[N * k + q] = s * akp + c * akq;
+        }
 #pragma unroll
-      for (int k = 0; k < 3; ++k) {
-        const double vkp = V[3 * k + p], vkq = V[3 * k + q];
-        V[3 * k + p] = c * vkp - s * vkq;
-        V[3 * k + q] = s * vkp + c * vkq;
+        for (int k = 0; k < N; ++k) {  // rows p, q
+          const double apk = A[N * p + k], aqk = A[N * q + k];
+          A[N * p + k] = c * apk - s * aqk;
+          A[N * q + k] = s * apk + c * aqk;
+        }
+#pragma unroll
+        for (int k = 0; k < N; ++k) {
+          const double vkp = V[N * k + p], vkq = V[N * k + q];
+          V[N * k + p] = c * vkp - s * vkq;
+          V[N * k + q] = s * vkp + c * vkq;
+        }
       }
     }
   }
+}
+
+// Landmark prior lp of this shard at the position pw, in double from the unweighted L (D.lmp_Lu): r = L (pw - x0), returns
+// s = |r|^2.  lmp_loss gives err = rho(s)/2 and w = rho'(s) of its loss record (only while D.lmp_loss is set).
+template <class S>
+__device__ __forceinline__ double lmp_residual(const DevPtrs<S>& D, int lp, const double* pw, double (&r)[3]) {
+  const S* Lp = D.lmp_Lu + 9 * (size_t)lp;
+  const double e[3] = {pw[0] - (double)D.lmp_mean[3 * lp], pw[1] - (double)D.lmp_mean[3 * lp + 1], pw[2] - (double)D.lmp_mean[3 * lp + 2]};
+  double s = 0.0;
+#pragma unroll
+  for (int i = 0; i < 3; ++i) {
+    const double v = (double)Lp[3 * i] * e[0] + (double)Lp[3 * i + 1] * e[1] + (double)Lp[3 * i + 2] * e[2];
+    r[i] = v;
+    s += v * v;
+  }
+  return s;
+}
+template <class S>
+__device__ __forceinline__ void lmp_loss(const DevPtrs<S>& D, int lp, double s, double& err, double& w) {
+  unsigned kind;
+  S a;
+  slot_loss(D.lmp_loss, D.lmp_n, (size_t)lp, kind, a);
+  observation_loss<double>(kind, (double)a, s, err, w);
 }
 
 // Warp per landmark (problem order).  Re-linearises every observation in double with the weights and validity rule of
@@ -129,18 +156,8 @@ __global__ void __launch_bounds__(128) k_cov_landmark(DevPtrs<S> D, KOpts o, con
         const S* Lp = (LMPL ? D.lmp_Lu : D.lmp_L) + 9 * (size_t)lp;
         double sw = 1.0;
         if constexpr (LMPL) {
-          const double e[3] = {pw[0] - (double)D.lmp_mean[3 * lp], pw[1] - (double)D.lmp_mean[3 * lp + 1], pw[2] - (double)D.lmp_mean[3 * lp + 2]};
-          double s = 0.0;
-#pragma unroll
-          for (int r = 0; r < 3; ++r) {
-            const double v = (double)Lp[3 * r] * e[0] + (double)Lp[3 * r + 1] * e[1] + (double)Lp[3 * r + 2] * e[2];
-            s += v * v;
-          }
-          unsigned kind;
-          S a;
-          slot_loss(D.lmp_loss, D.lmp_n, (size_t)lp, kind, a);
-          double err, w;
-          observation_loss<double>(kind, (double)a, s, err, w);
+          double rp[3], err, w;
+          lmp_loss(D, lp, lmp_residual(D, lp, pw, rp), err, w);
           sw = sqrt(w);
         }
 #pragma unroll
@@ -152,7 +169,7 @@ __global__ void __launch_bounds__(128) k_cov_landmark(DevPtrs<S> D, KOpts o, con
       }
     }
     double A[9] = {h[0], h[1], h[2], h[1], h[3], h[4], h[2], h[4], h[5]}, V[9];
-    cov_sym3_eig(A, V);
+    sym_eig<3>(A, V);
     const double lmax = fmax(A[0], fmax(A[4], A[8]));
     double W[9];
     int r = 0;

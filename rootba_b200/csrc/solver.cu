@@ -21,6 +21,7 @@
 #include "covariance.cuh"
 #include "assembled.cuh"
 #include "rigs.cuh"
+#include "triangulate.cuh"
 #include "nccl_dyn.hpp"
 
 namespace rba {
@@ -29,6 +30,7 @@ thread_local std::string g_err;
 
 // the host builds the pair lists as IntPair (layout.hpp); the kernels read them as int2
 static_assert(sizeof(IntPair) == sizeof(int2), "IntPair must have the layout of int2");
+static_assert(sizeof(rba_triangulate_opts) == 32, "rba_triangulate_opts is 32 bytes without implicit padding");
 
 #define CU(call)                                                                                   \
   do {                                                                                             \
@@ -85,6 +87,8 @@ struct rba_handle {
   virtual int set_prior_loss(int32_t prior_kind, int32_t num, const uint8_t* kind, const void* scale) = 0;
   virtual int get_prior_residuals(int32_t prior_kind, void* residual, void* robust_weight) = 0;
   virtual int get_observation_residuals(void* residual, void* robust_weight, uint8_t* flags) = 0;
+  virtual int triangulate(const rba_triangulate_opts* o, int32_t num, const int32_t* lm_idx, uint8_t* status, double* angle,
+                          double* cost) = 0;
   virtual int compute_error(rba_residual_info* out) = 0;
   virtual int linearize() = 0;
   virtual int solve(double lambda, void* inc_out, rba_cg_summary* cg) = 0;
@@ -1639,6 +1643,75 @@ struct Solver : rba_handle {
     return RBA_OK;
   }
 
+  // Triangulation of the listed landmarks from the current cameras (DESIGN.md section 25): one k_triangulate launch over the
+  // entries of this shard, in the length-sorted order.  Every check runs before any device work.  A state change: the error
+  // cache, the linearisation and the device-resident increment are discarded; the backup is not touched.
+  int triangulate(const rba_triangulate_opts* o, int32_t num, const int32_t* lm_idx, uint8_t* status, double* angle,
+                  double* cost) override {
+    auto bad = [&](const std::string& what) { g_err = "rba_triangulate_landmarks: " + what; return RBA_ERR_INVALID_ARGUMENT; };
+    if (!o) return bad("o is NULL");
+    if (o->mode < 1 || o->mode > 3) return bad("mode must be 1..3 (RBA_TRIANGULATE_* bits), got " + std::to_string(o->mode));
+    if (o->max_iterations < 0) return bad("max_iterations must be >= 0, got " + std::to_string(o->max_iterations));
+    if (!std::isfinite(o->min_angle) || o->min_angle < 0) return bad("min_angle must be finite and >= 0");
+    if (!std::isfinite(o->function_tolerance) || o->function_tolerance < 0) return bad("function_tolerance must be finite and >= 0");
+    if (num < 0) return bad("num must be >= 0, got " + std::to_string(num));
+    if (!lm_idx && num != nl_total)
+      return bad("lm_idx is NULL, so num must be the number of landmarks " + std::to_string(nl_total) + ", got " + std::to_string(num));
+    std::vector<uint8_t> seen(lm_idx ? (size_t)nl_total : 0, 0);
+    std::vector<std::pair<int, int>> mine;  // (sorted index, caller position) of this shard's entries
+    for (int p = 0; p < num; ++p) {
+      const int l = lm_idx ? lm_idx[p] : p;
+      if (lm_idx) {
+        if (l < 0 || l >= nl_total) return bad("entry " + std::to_string(p) + " has a landmark index outside [0, " + std::to_string(nl_total) + ")");
+        if (seen[l]) return bad("entry " + std::to_string(p) + " repeats landmark " + std::to_string(l));
+        seen[l] = 1;
+      }
+      if (l >= L.lm_begin && l < L.lm_end) mine.push_back({L.sorted_of_lm[l - L.lm_begin], p});
+    }
+    std::sort(mine.begin(), mine.end());
+    const size_t ni = mine.size();
+    if (ni > 0) {
+      std::vector<TriItem> items(ni);
+      for (size_t k = 0; k < ni; ++k) {
+        const int sidx = mine[k].first;
+        const TileInfo& T = L.tiles[L.tile_of_sorted[sidx]];
+        items[k] = {L.sorted_lm[sidx], sidx, T.slot_base + (sidx - T.lm_base) * T.n, T.n};
+      }
+      DeviceBuffer<char> scratch;  // per-call: the rays, the items, the outputs and the validity bytes
+      const size_t ray_b = (size_t)L.nslots * sizeof(double4), item_b = ni * sizeof(TriItem);
+      TRY(alloc(scratch, ray_b + item_b + ni * (2 * sizeof(double) + 1) + (size_t)L.nslots, false, false));
+      double4* d_ray = (double4*)scratch.get();
+      TriItem* d_items = (TriItem*)(scratch.get() + ray_b);
+      double* d_angle = (double*)(scratch.get() + ray_b + item_b);
+      double* d_cost = d_angle + ni;
+      uint8_t* d_status = (uint8_t*)(d_cost + ni);
+      uint8_t* d_vb = d_status + ni;
+      CU(cudaMemcpyAsync(d_items, items.data(), item_b, cudaMemcpyHostToDevice, stream));
+      const TriOpts to{o->mode, o->max_iterations, o->min_angle, o->function_tolerance};
+      k_triangulate<S><<<grid_for((long long)ni, 4, 16), 128, 0, stream>>>(D, ko, to, d_items, (int)ni, d_ray, d_vb, d_status, d_angle, d_cost);
+      ++launches;
+      std::vector<uint8_t> st(ni);
+      std::vector<double> an(ni), co(ni);
+      CU(cudaMemcpyAsync(st.data(), d_status, ni, cudaMemcpyDeviceToHost, stream));
+      CU(cudaMemcpyAsync(an.data(), d_angle, ni * sizeof(double), cudaMemcpyDeviceToHost, stream));
+      CU(cudaMemcpyAsync(co.data(), d_cost, ni * sizeof(double), cudaMemcpyDeviceToHost, stream));
+      CU(cudaStreamSynchronize(stream));
+      CU(cudaGetLastError());
+      for (size_t k = 0; k < ni; ++k) {
+        const int p = mine[k].second;
+        if (status) status[p] = st[k];
+        if (angle) angle[p] = an[k];
+        if (cost) cost[p] = co[k];
+      }
+    }
+    ++state_version;
+    linearized = false;
+    damping_valid = false;
+    have_inc = false;
+    error_cache_valid = false;
+    return RBA_OK;
+  }
+
   // launch with optional programmatic dependent launch (the kernel may start before its predecessor in the stream has
   // finished and orders itself with griddepcontrol.wait) and optional thread-block-cluster dimension
   template <class... KArgs, class... Args>
@@ -2995,6 +3068,17 @@ int32_t rba_set_prior_loss(rba_handle* h, int32_t prior_kind, int32_t num, const
 }
 int32_t rba_get_prior_residuals(rba_handle* h, int32_t prior_kind, void* residual, void* robust_weight) {
   return h->get_prior_residuals(prior_kind, residual, robust_weight);
+}
+void rba_default_triangulate_opts(rba_triangulate_opts* o) {
+  *o = rba_triangulate_opts{};
+  o->mode = RBA_TRIANGULATE_LINEAR | RBA_TRIANGULATE_REFINE;
+  o->max_iterations = 20;
+  o->min_angle = 0.0;
+  o->function_tolerance = 1e-10;
+}
+int32_t rba_triangulate_landmarks(rba_handle* h, const rba_triangulate_opts* o, int32_t num, const int32_t* lm_idx,
+                                  uint8_t* status, double* angle, double* cost) {
+  return h->triangulate(o, num, lm_idx, status, angle, cost);
 }
 int32_t rba_get_observation_residuals(rba_handle* h, void* residual, void* robust_weight, uint8_t* flags) {
   return h->get_observation_residuals(residual, robust_weight, flags);

@@ -745,6 +745,29 @@ class LinearizorQR:
         check(_lib.lib().rba_get_observation_residuals(self.h, _p(res), _p(hw), _p(flags)))
         return res, hw, flags
 
+    def triangulate(self, landmarks=None, mode="linear+refine", max_iterations=20, min_angle_deg=0.0,
+                    function_tolerance=1e-10):
+        """Re-initialise landmark positions from the current cameras, which are held (rba_triangulate_landmarks, DESIGN.md
+        section 25).  landmarks None (every landmark) or problem indices; mode "linear", "refine" or "linear+refine" (or the
+        RBA_TRIANGULATE_* bits).  Returns (status uint8 RBA_TRI_* bits, angle [rad] the largest angle between two usable rays,
+        cost the landmark's share of compute_error at its final position), in the order of `landmarks`, and copies the new
+        positions into the BalProblem.  A sharded handle fills only the entries of its own shard (the others stay 0).  Needs a
+        new linearize before the next solve."""
+        m = _lib.TRIANGULATE_MODES.get(mode, mode) if isinstance(mode, str) else int(mode)
+        if isinstance(mode, str) and mode not in _lib.TRIANGULATE_MODES:
+            raise ValueError(f"mode must be one of {sorted(_lib.TRIANGULATE_MODES)}, got {mode!r}")
+        o = _lib.TriangulateOpts()
+        _lib.lib().rba_default_triangulate_opts(C.byref(o))
+        o.mode, o.max_iterations = m, int(max_iterations)
+        o.min_angle, o.function_tolerance = float(np.deg2rad(min_angle_deg)), float(function_tolerance)
+        idx = None if landmarks is None else np.ascontiguousarray(landmarks, np.int32)
+        num = self.nl if idx is None else len(idx)
+        status, angle, cost = np.zeros(num, np.uint8), np.zeros(num), np.zeros(num)
+        check(_lib.lib().rba_triangulate_landmarks(self.h, C.byref(o), int(num), None if idx is None else _p(idx), _p(status),
+                                                   _p(angle), _p(cost)))
+        self.download_state()
+        return status, angle, cost
+
     def _backup(self):
         check(_lib.lib().rba_backup(self.h))
 
