@@ -8,6 +8,7 @@
         [--residuals OUT.npz] [--camera-prior-loss KIND:SCALE | FILE.npz] [--pair-prior-loss KIND:SCALE | FILE.npz]
         [--landmark-prior-loss KIND:SCALE | FILE.npz] [--prior-residuals OUT.npz]
         [--triangulate linear|refine|linear+refine [--triangulation OUT.npz]]
+        [--resect linear|refine|linear+refine [--resect-intrinsics] [--resection OUT.npz]]
 
 Mirrors what `bal_qr --input ...` of the reference does (src/app/bal_qr.cpp): load + normalise (bal_problem.cpp:773-852),
 optimize_lm_ours with the QR linearizor (solver/bal_bundle_adjustment.cpp:249-544), log (bal/ba_log.hpp)."""
@@ -111,7 +112,18 @@ def main():
                     help="before the solve, re-initialise every landmark from the loaded cameras (DESIGN.md section 25)")
     ap.add_argument("--triangulation", default=None, metavar="OUT.npz",
                     help="with --triangulate, write per landmark `status` (RBA_TRI_* bits), `angle` [rad] and `cost`")
+    ap.add_argument("--resect", default=None, choices=["linear", "refine", "linear+refine"],
+                    help="before the solve (and before --triangulate), re-initialise every camera (rig) from the loaded "
+                         "landmarks (DESIGN.md section 26)")
+    ap.add_argument("--resect-intrinsics", action="store_true",
+                    help="with --resect: also refine the free f, k1, k2 of cameras outside rigs and intrinsics groups")
+    ap.add_argument("--resection", default=None, metavar="OUT.npz",
+                    help="with --resect, write per camera `status` (RBA_RES_* bits), `points` and `cost`")
     args = ap.parse_args()
+    if args.resection and not args.resect:
+        ap.error("--resection requires --resect")
+    if args.resect_intrinsics and not args.resect:
+        ap.error("--resect-intrinsics requires --resect")
     if args.triangulation and not args.triangulate:
         ap.error("--triangulation requires --triangulate")
     if args.relative_covariance and not args.covariance:
@@ -201,6 +213,16 @@ def main():
                 ap.error(f"{flag}: {e}")
     options = rb.SolverOptions(max_num_iterations=args.max_num_iterations, preconditioner_type=args.preconditioner_type,
                                operator_form=args.operator_form, use_double=not args.float)
+    if args.resect:
+        lin_res = rb.LinearizorQR.create(problem, options)  # the new cameras go back into `problem`
+        status, points, cost = lin_res.resect(mode=args.resect, intrinsics=args.resect_intrinsics)
+        lin_res.close()
+        written = int(np.count_nonzero(status & _lib.RES_WRITTEN))
+        print(f"resected ({args.resect}{', intrinsics' if args.resect_intrinsics else ''}): {written} of {len(status)} "
+              f"cameras written, {int(np.count_nonzero(status & _lib.RES_FEW_POINTS))} with fewer than 3 usable points")
+        if args.resection:
+            np.savez(args.resection, status=status, points=points, cost=cost)
+            print("wrote", args.resection)
     if args.triangulate:
         lin_tri = rb.LinearizorQR.create(problem, options)  # the new positions go back into `problem`
         status, angle, cost = lin_tri.triangulate(mode=args.triangulate)

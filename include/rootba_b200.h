@@ -556,6 +556,72 @@ void rba_default_triangulate_opts(rba_triangulate_opts* o);
 int32_t rba_triangulate_landmarks(rba_handle* h, const rba_triangulate_opts* o, int32_t num, const int32_t* lm_idx,
                                   uint8_t* status, double* angle, double* cost);
 
+/* ---- Resection of cameras from the current landmarks (DESIGN.md section 26) ---------------- */
+
+#define RBA_RESECT_LINEAR     1   /* replace the pose by the linear estimate from the 2D-3D correspondences */
+#define RBA_RESECT_REFINE     2   /* minimise the camera's (rig's) own cost with the landmarks held */
+#define RBA_RESECT_INTRINSICS 4   /* with REFINE: also refine the free f, k1, k2 of a single-camera unit */
+
+#define RBA_RES_WRITTEN     1u    /* the unit's pose (or intrinsics) changed */
+#define RBA_RES_FEW_POINTS  2u    /* < 3 usable points and no camera or pair prior on the unit: untouched */
+#define RBA_RES_DEGENERATE  4u    /* LINEAR asked for, but < 6 usable points, near-planar points or a singular estimate */
+#define RBA_RES_BEHIND      8u    /* linear estimate puts more than half of the usable points behind the camera */
+#define RBA_RES_REFINED    16u    /* the refinement accepted at least one step */
+#define RBA_RES_CONVERGED  32u    /* the refinement met function_tolerance */
+#define RBA_RES_HELD       64u    /* the unit has no free entry (RBA_FIX_*): untouched */
+
+typedef struct {
+  int32_t mode;               /* RBA_RESECT_* bits; default LINEAR | REFINE */
+  int32_t max_iterations;     /* refinement iterations per unit, rejected steps included; default 20 */
+  double function_tolerance;  /* stop once a step changes the cost by less than this fraction; default 1e-10 */
+  int32_t reserved[2];
+} rba_resect_opts;            /* 24 bytes, no implicit padding */
+
+void rba_default_resect_opts(rba_resect_opts* o);
+/* Not in the reference.  Re-initialises and refines camera poses from the handle's current landmarks, which are held
+ * (camera resection, motion-only bundle adjustment): an image registered against an existing map, cameras left behind by
+ * moved landmarks, an outlier loop (W = 0) or new ground control points.
+ * cam_idx [num] int32 lists cameras by index; NULL = every camera, num must then be Nc.  A free camera is a unit of one; a
+ * camera in a rig of >= 2 cameras stands for its whole rig, whose free pose is the lead's, every member moving as
+ * T_j = M_j T_lead (M_j the map of the re-tie: the held extrinsics, or for a capture of a sensor the sensor's map at the
+ * call's start, the home included, so that every E_s stays unchanged to rounding).  Listing several members of one rig
+ * resects it once and gives each of them the unit's outputs.  Outputs are in the caller's order and any of them may be NULL:
+ * status [num] RBA_RES_* bits, points [num] the unit's usable points over its members, cost [num] the unit's share of
+ * rba_compute_error at its final stored pose.  Evaluated in float64 for either Scalar; a written pose is rounded to Scalar.
+ * Only the cameras of the listed units are written; every other camera stays bit-identical.
+ * Free entries: the pose unless the unit has RBA_FIX_POSE; f, k1, k2 only with RBA_RESECT_INTRINSICS, for a single camera
+ * outside any intrinsics group of >= 2 cameras, each unless its own RBA_FIX_* bit is set.  A unit without a free entry is
+ * HELD and untouched.  A usable point is an observation in use (W != 0) of a camera with f != 0 whose distortion inverts
+ * (as for rba_triangulate_landmarks).  A unit with fewer than 3 usable points is FEW_POINTS and untouched, unless it carries
+ * a camera prior or a pair prior: then it is still refined.
+ * LINEAR (a unit with a free pose): the DLT of one member, the one with the most usable points (ties to the lowest index):
+ * p [12] = P row by row is the smallest eigenvector of M = sum_i G_i^T (I - v_i v_i^T) G_i with P X~_i = G_i p,
+ * X~_i = ((X_i - Xbar) / s, 1) (Xbar the mean and s the RMS distance of the usable points) and v_i = (m, 1) / |(m, 1)| the
+ * unit ray of the undistorted point m.  With P = [A | b] signed so that det A > 0, R is the polar factor of A, sigma the mean
+ * singular value of A and t = s b / sigma - R Xbar; the lead's pose is M_j^-1 T_j.  DEGENERATE (not written) with fewer
+ * than 6 usable points in that member, when the smallest principal standard deviation of the centred points is below 1e-3
+ * of the largest, or when |det A| <= 1e-10 |A|_F^3; BEHIND (not written) when more than half of the member's usable points
+ * lie at depth < eps_sqrt of the Scalar under the estimate.
+ * REFINE: Levenberg-Marquardt on the unit's share of the cost with the landmarks held: rho(|W r|^2)/2 of every observation
+ * in use by a member (its own loss or the handle's robust norm, use_valid_projections_only), the members' camera priors and
+ * every pair prior with an endpoint in the unit, counted once, each with its loss.  A pair endpoint outside the unit is read
+ * from the call's start, so a unit's result does not depend on which other cameras are listed.  The increment is the
+ * state's left increment R' = Exp(w) R, t' = Exp(w) t + v of the lead, restricted to the free entries, a member's Jacobian
+ * mapped through its adjoint A_j; IRLS-weighted normal equations, the damping, lambda schedule, acceptance (a strict cost
+ * decrease with no observation in use going from valid to invalid depth) and convergence rules of
+ * rba_triangulate_landmarks.  It starts from the pose LINEAR left (or the current one without LINEAR), and its result is
+ * written only when its cost, after rounding to Scalar, is below the cost at its start.
+ * The call is a state change: the state version is bumped, the error cache and the device-resident increment are
+ * discarded and rba_solve returns RBA_ERR_STATE until the next rba_linearize.  rba_backup is untouched, so rba_restore
+ * brings the previous cameras back.  Landmarks, rigs, sensors, groups, held flags and priors are read only.  Scratch device
+ * memory is allocated for the call and freed before it returns.
+ * RBA_ERR_INVALID_ARGUMENT before any device work, with nothing changed: o NULL, a mode with neither LINEAR nor REFINE,
+ * INTRINSICS without REFINE or an unknown bit, max_iterations < 0, function_tolerance negative or not finite, num < 0,
+ * cam_idx NULL with num != Nc, an index outside [0, Nc) or a repeated index.  RBA_ERR_UNSUPPORTED on a sharded handle
+ * (nranks > 1): a camera's observations span every shard. */
+int32_t rba_resect_cameras(rba_handle* h, const rba_resect_opts* o, int32_t num, const int32_t* cam_idx, uint8_t* status,
+                           int32_t* points, double* cost);
+
 /* ---- Marginal covariances (DESIGN.md section 16) ------------------------------------------ */
 
 /* Not in the reference.  DESIGN.md section 16.  The covariance of the Gauss-Newton step of the total objective (reprojection

@@ -54,6 +54,19 @@ TRI_BEHIND = 16
 TRI_REFINED = 32
 TRI_CONVERGED = 64
 
+# rba_resect_cameras: mode bits (RBA_RESECT_*) and status bits (RBA_RES_*)
+RESECT_LINEAR = 1
+RESECT_REFINE = 2
+RESECT_INTRINSICS = 4
+RESECT_MODES = {"linear": RESECT_LINEAR, "refine": RESECT_REFINE, "linear+refine": RESECT_LINEAR | RESECT_REFINE}
+RES_WRITTEN = 1
+RES_FEW_POINTS = 2
+RES_DEGENERATE = 4
+RES_BEHIND = 8
+RES_REFINED = 16
+RES_CONVERGED = 32
+RES_HELD = 64
+
 
 class RbaError(RuntimeError):
     def __init__(self, code: int, msg: str):
@@ -133,6 +146,11 @@ class TriangulateOpts(C.Structure):
                 ("function_tolerance", C.c_double), ("reserved", C.c_int32 * 2)]
 
 
+class ResectOpts(C.Structure):
+    _fields_ = [("mode", C.c_int32), ("max_iterations", C.c_int32), ("function_tolerance", C.c_double),
+                ("reserved", C.c_int32 * 2)]
+
+
 def struct_to_dict(s: C.Structure) -> dict:
     out = {}
     for name, _ in s._fields_:
@@ -183,6 +201,10 @@ def lib():
         _lib.rba_default_triangulate_opts.restype = None
         _lib.rba_triangulate_landmarks.argtypes = [C.c_void_p, C.POINTER(TriangulateOpts), C.c_int32, C.c_void_p, C.c_void_p,
                                                    C.c_void_p, C.c_void_p]
+        _lib.rba_default_resect_opts.argtypes = [C.POINTER(ResectOpts)]
+        _lib.rba_default_resect_opts.restype = None
+        _lib.rba_resect_cameras.argtypes = [C.c_void_p, C.POINTER(ResectOpts), C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                            C.c_void_p]
     return _lib
 
 

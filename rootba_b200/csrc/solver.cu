@@ -22,6 +22,7 @@
 #include "assembled.cuh"
 #include "rigs.cuh"
 #include "triangulate.cuh"
+#include "resect.cuh"
 #include "nccl_dyn.hpp"
 
 namespace rba {
@@ -31,6 +32,7 @@ thread_local std::string g_err;
 // the host builds the pair lists as IntPair (layout.hpp); the kernels read them as int2
 static_assert(sizeof(IntPair) == sizeof(int2), "IntPair must have the layout of int2");
 static_assert(sizeof(rba_triangulate_opts) == 32, "rba_triangulate_opts is 32 bytes without implicit padding");
+static_assert(sizeof(rba_resect_opts) == 24, "rba_resect_opts is 24 bytes without implicit padding");
 
 #define CU(call)                                                                                   \
   do {                                                                                             \
@@ -89,6 +91,8 @@ struct rba_handle {
   virtual int get_observation_residuals(void* residual, void* robust_weight, uint8_t* flags) = 0;
   virtual int triangulate(const rba_triangulate_opts* o, int32_t num, const int32_t* lm_idx, uint8_t* status, double* angle,
                           double* cost) = 0;
+  virtual int resect(const rba_resect_opts* o, int32_t num, const int32_t* cam_idx, uint8_t* status, int32_t* points,
+                     double* cost) = 0;
   virtual int compute_error(rba_residual_info* out) = 0;
   virtual int linearize() = 0;
   virtual int solve(double lambda, void* inc_out, rba_cg_summary* cg) = 0;
@@ -1712,6 +1716,120 @@ struct Solver : rba_handle {
     return RBA_OK;
   }
 
+  // Resection of the listed cameras' units from the current landmarks (DESIGN.md section 26): one k_resect launch, a CTA
+  // per unit, the units in decreasing observation count.  Every check runs before any device work.  A state change like
+  // triangulate: the error cache, the linearisation and the device-resident increment are discarded; the backup is not
+  // touched.
+  int resect(const rba_resect_opts* o, int32_t num, const int32_t* cam_idx, uint8_t* status, int32_t* points,
+             double* cost) override {
+    auto bad = [&](const std::string& what) { g_err = "rba_resect_cameras: " + what; return RBA_ERR_INVALID_ARGUMENT; };
+    if (!o) return bad("o is NULL");
+    const int md = o->mode;
+    if ((md & ~7) || !(md & 3) || ((md & RBA_RESECT_INTRINSICS) && !(md & RBA_RESECT_REFINE)))
+      return bad("mode must be LINEAR and / or REFINE, INTRINSICS only with REFINE (RBA_RESECT_* bits), got " + std::to_string(md));
+    if (o->max_iterations < 0) return bad("max_iterations must be >= 0, got " + std::to_string(o->max_iterations));
+    if (!std::isfinite(o->function_tolerance) || o->function_tolerance < 0) return bad("function_tolerance must be finite and >= 0");
+    if (num < 0) return bad("num must be >= 0, got " + std::to_string(num));
+    if (!cam_idx && num != nc)
+      return bad("cam_idx is NULL, so num must be the number of cameras " + std::to_string(nc) + ", got " + std::to_string(num));
+    std::vector<uint8_t> seen(cam_idx ? (size_t)nc : 0, 0);
+    for (int p = 0; p < num && cam_idx; ++p) {
+      const int c = cam_idx[p];
+      if (c < 0 || c >= nc) return bad("entry " + std::to_string(p) + " has a camera index outside [0, " + std::to_string(nc) + ")");
+      if (seen[c]) return bad("entry " + std::to_string(p) + " repeats camera " + std::to_string(c));
+      seen[c] = 1;
+    }
+    if (opt.nranks > 1) {
+      g_err = "rba_resect_cameras: a sharded handle is not supported (a camera's observations span every shard)";
+      return RBA_ERR_UNSUPPORTED;
+    }
+    // the units: a rig of >= 2 cameras is one unit led by its lead, its members ascending; any other camera is its own
+    auto lead_of = [&](int c) { return rig.n && rig.host_lead[c] >= 0 ? rig.host_lead[c] : c; };
+    std::vector<int> unit_of((size_t)nc, -1), unit_lead, caller_unit((size_t)num);
+    for (int p = 0; p < num; ++p) {
+      const int ld = lead_of(cam_idx ? cam_idx[p] : p);
+      if (unit_of[ld] < 0) { unit_of[ld] = (int)unit_lead.size(); unit_lead.push_back(ld); }
+      caller_unit[p] = unit_of[ld];
+    }
+    const size_t nu = unit_lead.size();
+    std::vector<std::vector<int>> members(nu);
+    for (int c = 0; c < nc; ++c)
+      if (unit_of[lead_of(c)] >= 0) members[unit_of[lead_of(c)]].push_back(c);
+    const auto& cp = L.csr_obs.cam_ptr;
+    std::vector<long long> nobs(nu, 0);
+    for (size_t u = 0; u < nu; ++u)
+      for (int c : members[u]) nobs[u] += cp[c + 1] - cp[c];
+    std::vector<int> order(nu);
+    for (size_t u = 0; u < nu; ++u) order[u] = (int)u;
+    std::sort(order.begin(), order.end(), [&](int a, int b) { return nobs[a] != nobs[b] ? nobs[a] > nobs[b] : unit_lead[a] < unit_lead[b]; });
+    std::vector<int> pos_of(nu);
+    std::vector<ResItem> items(nu);
+    std::vector<ResMember> mem;
+    for (size_t k = 0; k < nu; ++k) {
+      const int u = order[k], ld = unit_lead[u];
+      pos_of[u] = (int)k;
+      const unsigned fl = held.host.empty() ? 0u : held.host[ld];
+      unsigned fr = (fl & RBA_FIX_POSE) ? 0u : 0x3fu;
+      const bool single = members[u].size() == 1, grouped = grp.n && grp.host_lead[ld] >= 0;
+      if ((md & RBA_RESECT_INTRINSICS) && single && !grouped) fr |= ~fixed_entry_mask(fl | RBA_FIX_POSE) & 0x1c0u;
+      items[k] = {(int)mem.size(), (int)members[u].size(), ld, fr};
+      for (int c : members[u]) mem.push_back({c, cp[c], cp[c + 1]});
+    }
+    if (nu > 0) {
+      DeviceBuffer<char> scratch;  // per-call: the snapshot, the items, the members, their M_j and A_j, the outputs, the validity bytes
+      const size_t snap_b = (size_t)10 * nc * sizeof(S), item_b = nu * sizeof(ResItem), mem_b = mem.size() * sizeof(ResMember);
+      const size_t mx_b = mem.size() * RES_MX * sizeof(double), out_b = nu * (sizeof(double) + sizeof(int) + 1);
+      auto up8 = [](size_t b) { return (b + 15) & ~(size_t)15; };
+      TRY(alloc(scratch, up8(snap_b) + up8(item_b) + up8(mem_b) + up8(mx_b) + up8(out_b) + (size_t)L.nslots, false, false));
+      char* at = scratch.get();
+      S* d_snap = (S*)at; at += up8(snap_b);
+      ResItem* d_items = (ResItem*)at; at += up8(item_b);
+      ResMember* d_mem = (ResMember*)at; at += up8(mem_b);
+      double* d_mx = (double*)at; at += up8(mx_b);
+      double* d_cost = (double*)at;
+      int* d_points = (int*)(d_cost + nu);
+      uint8_t* d_status = (uint8_t*)(d_points + nu);
+      uint8_t* d_vb = (uint8_t*)(at + up8(out_b));
+      CU(cudaMemcpyAsync(d_snap, D.cams, snap_b, cudaMemcpyDeviceToDevice, stream));
+      CU(cudaMemcpyAsync(d_items, items.data(), item_b, cudaMemcpyHostToDevice, stream));
+      CU(cudaMemcpyAsync(d_mem, mem.data(), mem_b, cudaMemcpyHostToDevice, stream));
+      ResTerms<S> T{};
+      T.snap = d_snap;
+      T.slots = d_csr_obs_slots;
+      if (rig.n) T.R = rigs();
+      if (sen.n) T.Z = sensors();
+      if (cprior.on) { T.cp_mean = cprior.mean.get(); T.cp_L = cprior.L.get(); T.cp_loss = cprior.loss.on ? cprior.loss.rec.get() : nullptr; }
+      if (pprior.n > 0) {
+        T.pp_ij = pprior.ij.get(); T.pp_mean = pprior.mean.get(); T.pp_L = pprior.L.get();
+        T.pp_loss = pprior.loss.on ? pprior.loss.rec.get() : nullptr; T.pp_ptr = pprior.ptr.get(); T.pp_item = pprior.item.get();
+        T.pp_n = pprior.n;
+      }
+      const ResOpts ro{md, o->max_iterations, o->function_tolerance};
+      k_resect<S><<<(unsigned)nu, RES_THREADS, 0, stream>>>(D, ko, ro, T, d_items, d_mem, d_mx, d_vb, d_status, d_points, d_cost);
+      ++launches;
+      std::vector<uint8_t> st(nu);
+      std::vector<int> pt(nu);
+      std::vector<double> co(nu);
+      CU(cudaMemcpyAsync(st.data(), d_status, nu, cudaMemcpyDeviceToHost, stream));
+      CU(cudaMemcpyAsync(pt.data(), d_points, nu * sizeof(int), cudaMemcpyDeviceToHost, stream));
+      CU(cudaMemcpyAsync(co.data(), d_cost, nu * sizeof(double), cudaMemcpyDeviceToHost, stream));
+      CU(cudaStreamSynchronize(stream));
+      CU(cudaGetLastError());
+      for (int p = 0; p < num; ++p) {
+        const int k = pos_of[caller_unit[p]];
+        if (status) status[p] = st[k];
+        if (points) points[p] = pt[k];
+        if (cost) cost[p] = co[k];
+      }
+    }
+    ++state_version;
+    linearized = false;
+    damping_valid = false;
+    have_inc = false;
+    error_cache_valid = false;
+    return RBA_OK;
+  }
+
   // launch with optional programmatic dependent launch (the kernel may start before its predecessor in the stream has
   // finished and orders itself with griddepcontrol.wait) and optional thread-block-cluster dimension
   template <class... KArgs, class... Args>
@@ -3079,6 +3197,16 @@ void rba_default_triangulate_opts(rba_triangulate_opts* o) {
 int32_t rba_triangulate_landmarks(rba_handle* h, const rba_triangulate_opts* o, int32_t num, const int32_t* lm_idx,
                                   uint8_t* status, double* angle, double* cost) {
   return h->triangulate(o, num, lm_idx, status, angle, cost);
+}
+void rba_default_resect_opts(rba_resect_opts* o) {
+  *o = rba_resect_opts{};
+  o->mode = RBA_RESECT_LINEAR | RBA_RESECT_REFINE;
+  o->max_iterations = 20;
+  o->function_tolerance = 1e-10;
+}
+int32_t rba_resect_cameras(rba_handle* h, const rba_resect_opts* o, int32_t num, const int32_t* cam_idx, uint8_t* status,
+                           int32_t* points, double* cost) {
+  return h->resect(o, num, cam_idx, status, points, cost);
 }
 int32_t rba_get_observation_residuals(rba_handle* h, void* residual, void* robust_weight, uint8_t* flags) {
   return h->get_observation_residuals(residual, robust_weight, flags);

@@ -768,6 +768,29 @@ class LinearizorQR:
         self.download_state()
         return status, angle, cost
 
+    def resect(self, cameras=None, mode="linear+refine", intrinsics=False, max_iterations=20, function_tolerance=1e-10):
+        """Re-initialise and refine camera poses from the current landmarks, which are held (rba_resect_cameras, DESIGN.md
+        section 26).  cameras None (every camera) or camera indices; a camera of a rig stands for its whole rig.  mode
+        "linear", "refine" or "linear+refine" (or the RBA_RESECT_* bits); intrinsics also refines the free f, k1, k2 of
+        single cameras.  Returns (status uint8 RBA_RES_* bits, points int32 the unit's usable points, cost the unit's share
+        of compute_error at its final pose), in the order of `cameras`, and copies the new cameras into the BalProblem.
+        Needs a new linearize before the next solve."""
+        if isinstance(mode, str) and mode not in _lib.RESECT_MODES:
+            raise ValueError(f"mode must be one of {sorted(_lib.RESECT_MODES)}, got {mode!r}")
+        m = _lib.RESECT_MODES[mode] if isinstance(mode, str) else int(mode)
+        if intrinsics:
+            m |= _lib.RESECT_INTRINSICS
+        o = _lib.ResectOpts()
+        _lib.lib().rba_default_resect_opts(C.byref(o))
+        o.mode, o.max_iterations, o.function_tolerance = m, int(max_iterations), float(function_tolerance)
+        idx = None if cameras is None else np.ascontiguousarray(cameras, np.int32)
+        num = self.nc if idx is None else len(idx)
+        status, points, cost = np.zeros(num, np.uint8), np.zeros(num, np.int32), np.zeros(num)
+        check(_lib.lib().rba_resect_cameras(self.h, C.byref(o), int(num), None if idx is None else _p(idx), _p(status),
+                                            _p(points), _p(cost)))
+        self.download_state()
+        return status, points, cost
+
     def _backup(self):
         check(_lib.lib().rba_backup(self.h))
 
