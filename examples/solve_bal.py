@@ -47,6 +47,9 @@ def main():
     ap.add_argument("--max-num-iterations", type=int, default=20)
     ap.add_argument("--preconditioner-type", default="SCHUR_JACOBI", choices=["JACOBI", "SCHUR_JACOBI"])
     ap.add_argument("--operator-form", default="DENSE", choices=["DENSE", "IMPLICIT"])
+    ap.add_argument("--linear-solver-type", default="ITERATIVE_SCHUR", choices=["ITERATIVE_SCHUR", "DENSE_SCHUR"],
+                    help="the camera increment by truncated PCG, or exactly by a dense Cholesky factorisation of the reduced "
+                         "camera matrix (needs (9 cameras)^2 x 8 bytes of device memory)")
     ap.add_argument("--init-depth-threshold", type=float, default=0.0)
     ap.add_argument("--log-path", default="ba_log.json")
     ap.add_argument("--fix-intrinsics", action="store_true", help="hold f, k1, k2 of every camera constant")
@@ -212,7 +215,8 @@ def main():
             except ValueError as e:
                 ap.error(f"{flag}: {e}")
     options = rb.SolverOptions(max_num_iterations=args.max_num_iterations, preconditioner_type=args.preconditioner_type,
-                               operator_form=args.operator_form, use_double=not args.float)
+                               operator_form=args.operator_form, linear_solver_type=args.linear_solver_type,
+                               use_double=not args.float)
     if args.resect:
         lin_res = rb.LinearizorQR.create(problem, options)  # the new cameras go back into `problem`
         status, points, cost = lin_res.resect(mode=args.resect, intrinsics=args.resect_intrinsics)

@@ -93,7 +93,20 @@ typedef struct {
                                               solver/linearizor_power_sc.cpp: power-series solve, sc/linearization_power_sc.hpp:130-160;
                                               one GPU).  Types 1 and 2 store no Q2 panels; same entry points, same protocol. */
   int32_t power_order;                     /* :270 ; maximum number of terms of the power series (0 -> 20) */
-  int32_t reserved[2];
+  int32_t linear_solver_type;              /* SolverOptions::linear_solver_type (bal/solver_options.hpp:77-80, 225-230): how rba_solve
+                                              gets the camera increment.  0 = ITERATIVE_SCHUR (default): truncated PCG, or the power
+                                              series with solver_type = 2.  1 = DENSE_SCHUR: the exact increment -H_ff^-1 b_f of the
+                                              same reduced system, by a dense float64 Cholesky factorisation of the Jacobi-scaled,
+                                              damped reduced camera matrix on the device, re-linearised in float64 at the current
+                                              state for either Scalar (DESIGN.md section 27).  eta, min/max_linear_solver_iterations,
+                                              residual_reset_period and pcg_check_period are then ignored; the summary is
+                                              SUCCESS with reason 7, or FAILURE with reason 8 (a pivot <= 0 or not finite; the free
+                                              entries of the increment are then NaN), with 0 iterations and matvecs.  The dense
+                                              (9 nc rounded up to 64)^2 float64 matrix and the per-slot scratch are allocated by
+                                              rba_create_* (counted in device_bytes): RBA_ERR_UNSUPPORTED when they do not fit in
+                                              the free device memory.  Other values, or DENSE_SCHUR with solver_type = 2 ->
+                                              RBA_ERR_INVALID_ARGUMENT; DENSE_SCHUR with nranks > 1 -> RBA_ERR_UNSUPPORTED. */
+  int32_t reserved[1];
 } rba_solver_opts;
 
 /* ResidualInfo (bal/residual_info.hpp:59-89) */
@@ -113,7 +126,9 @@ typedef struct {
   int32_t termination_type; /* 0 NO_CONVERGENCE, 1 SUCCESS, 2 FAILURE */
   int32_t num_iterations;
   int32_t num_matvecs;
-  int32_t reason;           /* detail code for the message (see DESIGN.md) */
+  int32_t reason;           /* detail code for the message (see DESIGN.md); with linear_solver_type = DENSE_SCHUR:
+                               7 = the dense Cholesky solve succeeded (SUCCESS), 8 = a pivot of the scaled, damped reduced
+                               camera matrix was <= 0 or not finite (FAILURE, the free entries of the increment are NaN) */
 } rba_cg_summary;
 
 /* Device times (CUDA events on the solver stream) of the IterationSummary fields

@@ -87,7 +87,7 @@ class SolverOpts(C.Structure):
                 ("residual_reset_period", C.c_int32), ("device", C.c_int32), ("rank", C.c_int32),
                 ("nranks", C.c_int32), ("pcg_check_period", C.c_int32), ("use_cuda_graphs", C.c_int32),
                 ("operator_form", C.c_int32), ("stage2_form", C.c_int32), ("solver_type", C.c_int32), ("power_order", C.c_int32),
-                ("reserved", C.c_int32 * 2)]
+                ("linear_solver_type", C.c_int32), ("reserved", C.c_int32 * 1)]
 
 
 class ResidualInfo(C.Structure):

@@ -19,6 +19,7 @@
 #include "../host/bal_io_fast.hpp"
 #include "kernels.cuh"
 #include "covariance.cuh"
+#include "dense_solve.cuh"
 #include "assembled.cuh"
 #include "rigs.cuh"
 #include "triangulate.cuh"
@@ -319,6 +320,15 @@ struct Solver : rba_handle {
   int cov_nblk = 0;
   IntPair* d_cov_blk_cam = nullptr; int* d_cov_blk_ptr = nullptr; IntPair* d_cov_terms = nullptr;
   int* d_cov_lm_slot0 = nullptr; int* d_cov_lm_n = nullptr;
+  // linear_solver_type = DENSE_SCHUR (dense_solve.cuh, DESIGN.md section 27): the buffers of every solve, allocated by
+  // setup_dense.  A: the np x np matrix and its factor; W, Tt: the potrf scratch; d: the scaling; x, y: the right-hand side
+  // and the two substitutions; jp, kb: the per-slot rows; fail: the smallest failed pivot
+  struct DenseSolve {
+    double* A = nullptr; double* W = nullptr; double* Tt = nullptr; double* d = nullptr;
+    double* x = nullptr; double* y = nullptr; double* jp = nullptr; double* kb = nullptr;
+    int* fail = nullptr;
+    long long np = 0;
+  } dn;
   // assembled operator (setup_assembled, assembled.cuh): the terms as panel addresses in landmark-major order, the pair
   // list (term ranges, landmark-major position of every term), per pair its positions (lower, upper or -1) in the full
   // block-row CSR of S, the staging buffer of all terms, S_u per pair and S
@@ -426,6 +436,7 @@ struct Solver : rba_handle {
     TRY(deal_work());
     TRY(alloc_buffers());
     TRY(setup_assembled());
+    TRY(setup_dense());
     TRY(setup_kernels());
     CU(cudaStreamSynchronize(stream));
     return RBA_OK;
@@ -437,6 +448,9 @@ struct Solver : rba_handle {
     if (opt.operator_form != 0 && opt.operator_form != 1) { g_err = "operator_form must be 0 (dense) or 1 (implicit)"; return RBA_ERR_INVALID_ARGUMENT; }
     if (opt.solver_type < 0 || opt.solver_type > 2) { g_err = "solver_type must be 0 (SQUARE_ROOT), 1 (SCHUR_COMPLEMENT) or 2 (POWER_SCHUR_COMPLEMENT)"; return RBA_ERR_INVALID_ARGUMENT; }
     if (opt.solver_type == 2 && opt.nranks > 1) { g_err = "POWER_SCHUR_COMPLEMENT runs on one GPU (the power-series vector kernel has no peer exchange yet)"; return RBA_ERR_UNSUPPORTED; }
+    if (opt.linear_solver_type != 0 && opt.linear_solver_type != 1) { g_err = "linear_solver_type must be 0 (ITERATIVE_SCHUR) or 1 (DENSE_SCHUR)"; return RBA_ERR_INVALID_ARGUMENT; }
+    if (opt.linear_solver_type == 1 && opt.solver_type == 2) { g_err = "DENSE_SCHUR does not combine with POWER_SCHUR_COMPLEMENT: the power series is itself the linear solver"; return RBA_ERR_INVALID_ARGUMENT; }
+    if (opt.linear_solver_type == 1 && opt.nranks > 1) { g_err = "DENSE_SCHUR runs on one GPU: the dense reduced camera matrix would need a cross-rank sum"; return RBA_ERR_UNSUPPORTED; }
     if (opt.stage2_form != 0 && opt.stage2_form != 1) { g_err = "stage2_form must be 0 (Q2 panel, reference) or 1 (orthogonality identity)"; return RBA_ERR_INVALID_ARGUMENT; }
     if (opt.pcg_check_period <= 0) opt.pcg_check_period = 4;
     if (opt.residual_reset_period <= 0) opt.residual_reset_period = 10;
@@ -2268,6 +2282,7 @@ struct Solver : rba_handle {
       new_linearization_point = false;
       return RBA_OK;
     }
+    if (opt.linear_solver_type == 1) return dense_enqueue((double)lambda, inc_out);  // DENSE_SCHUR: no PCG (section 27)
     Handover h = handover();
     if (h == Handover::Counter) CU(cudaMemsetAsync(D.y, 0, (size_t)9 * nc * sizeof(S), stream));  // see handover()
     if (power) return power_enqueue(h, inc_out);
@@ -2712,6 +2727,124 @@ struct Solver : rba_handle {
     CU(cudaGetLastError());
     return RBA_OK;
   }
+  // + the camera and pair priors' blocks (k_cov_priors) on the lower triangle of the unscaled matrix A (ld)
+  void cov_priors(double* A, long long ld) {
+    const bool prior_loss = cprior.loss.on || pprior.loss.on;
+    if (cprior.on || pprior.n > 0)
+      (prior_loss ? k_cov_priors<S, true> : k_cov_priors<S>)<<<(nc + 127) / 128, 128, 0, stream>>>(
+          D.cams, nc, cprior.on ? cprior.mean.get() : nullptr, cprior.L.get(), pprior.ij.get(), pprior.mean.get(), pprior.L.get(),
+          pprior.n > 0 ? pprior.ptr.get() : nullptr, pprior.item.get(), pprior.nbr.get(), A, ld,
+          cprior.loss.on ? (const S*)cprior.loss.rec.get() : nullptr, pprior.loss.on ? (const S*)pprior.loss.rec.get() : nullptr, pprior.n);
+  }
+  // Cholesky of the lower triangle of the np x np matrix A (ld np) in place, right-looking by COV_TB tiles: factor the
+  // diagonal tile, panel <- panel L_kk^-T, trailing lower tiles -= panel panel^T.  A pivot <= tau (or NaN) leaves the smallest
+  // such index in *fail, on the device.  W [np][COV_TB] and Tt [COV_TB][COV_TB]: scratch.
+  int dense_potrf(double* A, long long np, double* W, double* Tt, double tau, int* fail) {
+    constexpr long long TB = COV_TB;
+    const int nt = (int)(np / TB);
+    for (int k = 0; k < nt; ++k) {
+      const long long k0 = k * TB, m = np - k0 - TB;
+      k_cov_tile_potrf<<<1, 256, 0, stream>>>(A, np, k0, tau, fail);
+      if (m == 0) break;
+      k_cov_tile_trtri<<<1, COV_TB, 0, stream>>>(A, np, k0, Tt, TB);
+      double* P = A + (k0 + TB) + k0 * np;
+      TRY(cov_copy(W, m, P, np, m, TB));
+      cov_gemm<false, true>(m, TB, TB, 1.0, W, m, Tt, TB, 0.0, P, np, 0, 0);
+      cov_gemm<false, true>(m, m, TB, -1.0, P, np, P, np, 1.0, P + TB * np, np, 1, 0);
+    }
+    return RBA_OK;
+  }
+
+  // ------------------------------------------------------------------------------------------
+  // linear_solver_type = DENSE_SCHUR (dense_solve.cuh, DESIGN.md section 27)
+  // the bytes setup_dense allocates: A, W, Tt, d, x, y, the per-slot rows and the pivot flag
+  void dense_bytes(long long& np, size_t& total) const {
+    np = (9LL * nc + COV_TB - 1) / COV_TB * COV_TB;
+    const size_t ns = (size_t)L.nslots;
+    total = (size_t)(np * np + np * COV_TB + COV_TB * COV_TB + 3 * np) * 8 + ns * (18 + 27) * 8 + 4;
+  }
+  // Everything a solve uses, allocated once and counted in device_bytes: the matrix, the potrf scratch, the vectors, the
+  // per-slot rows and the term lists of the covariances (build_pair_list).
+  int setup_dense() {
+    if (opt.linear_solver_type != 1) return RBA_OK;
+    long long np = 0;
+    size_t total = 0;
+    dense_bytes(np, total);
+    size_t free_b = 0, total_b = 0;
+    CU(cudaMemGetInfo(&free_b, &total_b));
+    if (total > free_b) {
+      g_err = "DENSE_SCHUR needs " + std::to_string(total) + " bytes of device memory (a dense " + std::to_string(np) + " x " +
+              std::to_string(np) + " float64 reduced camera matrix plus scratch); " + std::to_string(free_b) + " bytes are free";
+      return RBA_ERR_UNSUPPORTED;
+    }
+    TRY(cov_build_lists());
+    TRY(dalloc(&dn.A, (size_t)(np * np), false));
+    TRY(dalloc(&dn.W, (size_t)(np * COV_TB), false));
+    TRY(dalloc(&dn.Tt, (size_t)(COV_TB * COV_TB), false));
+    TRY(dalloc(&dn.d, (size_t)np, false));
+    TRY(dalloc(&dn.x, (size_t)np, false));
+    TRY(dalloc(&dn.y, (size_t)np, false));
+    TRY(dalloc(&dn.jp, (size_t)L.nslots * 18, false));
+    TRY(dalloc(&dn.kb, (size_t)L.nslots * 27, false));
+    TRY(dalloc(&dn.fail, 1, false));
+    dn.np = np;
+    return RBA_OK;
+  }
+  // The exact increment of the system PCG iterates on, after stage 2 and the preconditioner of this solve: no host
+  // synchronisation, the pivot flag is read on the device by k_dense_finish.
+  int dense_enqueue(double lambda, void* inc_out) {
+    TRY(start(ev_pcg));
+    constexpr long long TB = COV_TB;
+    const long long n = 9LL * nc, np = dn.np;
+    const int nl = L.nl_local, nt = (int)(np / TB);
+    const uint8_t* held = grp.n || rig.n ? tied_fixed() : D.cam_fixed;
+    double* A = dn.A;
+    CU(cudaMemsetAsync(A, 0, (size_t)(np * np) * 8, stream));
+    CU(cudaMemsetAsync(dn.fail, 0x7f, 4, stream));
+    CU(cudaMemsetAsync(d_state, 0, sizeof(PcgState), stream));
+    // 1.-2. the damped elimination, assembly, priors, ties, scaling, held parameters, lambda
+    k_dense_landmark<S><<<std::max(1, std::min((nl + 3) / 4, sm_count * 16)), 128, 0, stream>>>(
+        D, ko, d_cov_lm_slot0, d_cov_lm_n, nl, lambda, dn.jp, dn.kb, lprior.n > 0 ? lprior.of_lm.get() : nullptr);
+    k_cov_assemble<<<std::max(1, std::min((cov_nblk + 7) / 8, sm_count * 8)), 256, 0, stream>>>(
+        (const int2*)d_cov_blk_cam, d_cov_blk_ptr, (const int2*)d_cov_terms, cov_nblk, dn.jp, dn.kb, A, np);
+    launches += 2 + ((cprior.on || pprior.n > 0) ? 1 : 0);
+    cov_priors(A, np);
+    if (rig.n) { TRY(cov_rig_passes(A, np, n, 0)); launches += 3; }
+    if (grp.n) { TRY(cov_group_passes(A, np, n, 0)); launches += 3; }
+    const unsigned g1 = (unsigned)((np + 255) / 256);
+    k_dense_scaling<S><<<g1, 256, 0, stream>>>(D.scaling, n, np, dn.d);
+    if (rig.n) {
+      k_dense_tied_scaling<S><<<(rig.n + sen.n + 127) / 128, 128, 0, stream>>>(rigs(), sen.ds.get(), sen.ptr.get(), sen.mem.get(), sen.n, dn.d);
+      ++launches;
+    }
+    k_cov_equil<<<dim3((unsigned)(np / 32), (unsigned)(np / 8)), dim3(32, 8), 0, stream>>>(A, np, n, np, held, dn.d);
+    k_dense_gather<S><<<g1, 256, 0, stream>>>(A, np, n, np, held, lambda, D.b, dn.x, dn.fail);
+    launches += 3;
+    // 3. potrf: 4 kernels per tile but the last
+    TRY(dense_potrf(A, np, dn.W, dn.Tt, 0.0, dn.fail));
+    launches += 4LL * nt - 3;
+    // 4. L y = b, L^T x = y
+    for (int k = 0; k < nt; ++k) {
+      const long long k0 = k * TB, m = np - k0 - TB;
+      k_dense_trsv_fwd<<<(unsigned)std::max(1LL, (m + DENSE_TRSV_ROWS - 1) / DENSE_TRSV_ROWS), DENSE_TRSV_ROWS, 0, stream>>>(A, np, np, k0,
+                                                                                                                          dn.x, dn.y);
+    }
+    for (int k = nt - 1; k >= 0; --k) {
+      const long long k0 = k * TB;
+      k_dense_trsv_bwd<<<(unsigned)std::max(1LL, (k0 + DENSE_TRSV_COLS - 1) / DENSE_TRSV_COLS), 256, 0, stream>>>(A, np, k0, dn.y, dn.x);
+    }
+    // 5. the increment and the summary
+    k_dense_finish<S><<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(dn.x, n, np, held, dn.fail, D.inc, d_state);
+    launches += 2LL * nt + 1;
+    CU(cudaGetLastError());
+    TRY(tie_expand(D.inc));  // inc = P u for the back-substitution, the update and inc_out
+    CU(cudaMemcpyAsync(&h_state[0], d_state, sizeof(PcgState), cudaMemcpyDeviceToHost, stream));
+    if (inc_out) CU(cudaMemcpyAsync(inc_out, D.inc, (size_t)9 * nc * sizeof(S), cudaMemcpyDeviceToHost, stream));
+    TRY(stop(ev_pcg));
+    have_inc = true;
+    new_linearization_point = false;
+    return RBA_OK;
+  }
   // The dense inverse of one covariance call and what its extraction kernels read; the scratch is freed (after the kernels
   // have finished: cudaFree waits for them) when it goes out of scope.
   struct CovInverse {
@@ -2770,12 +2903,7 @@ struct Solver : rba_handle {
     k_cov_assemble<<<std::max(1, std::min((cov_nblk + 7) / 8, sm_count * 8)), 256, 0, stream>>>(
         (const int2*)d_cov_blk_cam, d_cov_blk_ptr, (const int2*)d_cov_terms, cov_nblk, jp, kb, A, np);
     // LOSS: the camera and pair priors' losses (section 22), their weights re-evaluated in double at the current state
-    const bool prior_loss = cprior.loss.on || pprior.loss.on;
-    if (cprior.on || pprior.n > 0)
-      (prior_loss ? k_cov_priors<S, true> : k_cov_priors<S>)<<<(nc + 127) / 128, 128, 0, stream>>>(
-          D.cams, nc, cprior.on ? cprior.mean.get() : nullptr, cprior.L.get(), pprior.ij.get(), pprior.mean.get(), pprior.L.get(),
-          pprior.n > 0 ? pprior.ptr.get() : nullptr, pprior.item.get(), pprior.nbr.get(), A, np,
-          cprior.loss.on ? (const S*)cprior.loss.rec.get() : nullptr, pprior.loss.on ? (const S*)pprior.loss.rec.get() : nullptr, pprior.n);
+    cov_priors(A, np);
     // intrinsics groups (DESIGN.md section 18): S_u = P^T S P, the members' entries 6..8 then held like the user's
     // (rigs, section 23: S_u = P^T S P through the adjoints, the members' pose entries then held)
     const uint8_t* held = D.cam_fixed;
@@ -2784,17 +2912,7 @@ struct Solver : rba_handle {
     if (grp.n || rig.n) held = tied_fixed();
     k_cov_diag<<<(unsigned)((np + 255) / 256), 256, 0, stream>>>(A, np, n, np, held, d);
     k_cov_equil<<<dim3((unsigned)(np / 32), (unsigned)(np / 8)), dim3(32, 8), 0, stream>>>(A, np, n, np, held, d);
-    // 3a. potrf, right-looking: factor the diagonal tile, panel <- panel L_kk^-T, trailing lower tiles -= panel panel^T
-    for (int k = 0; k < nt; ++k) {
-      const long long k0 = k * TB, m = np - k0 - TB;
-      k_cov_tile_potrf<<<1, 256, 0, stream>>>(A, np, k0, COV_PIVOT_TAU, fail);
-      if (m == 0) break;
-      k_cov_tile_trtri<<<1, COV_TB, 0, stream>>>(A, np, k0, Tt, TB);
-      double* P = A + (k0 + TB) + k0 * np;
-      TRY(cov_copy(W, m, P, np, m, TB));
-      cov_gemm<false, true>(m, TB, TB, 1.0, W, m, Tt, TB, 0.0, P, np, 0, 0);
-      cov_gemm<false, true>(m, m, TB, -1.0, P, np, P, np, 1.0, P + TB * np, np, 1, 0);
-    }
+    TRY(dense_potrf(A, np, W, Tt, COV_PIVOT_TAU, fail));
     int h_fail = 0;
     CU(cudaMemcpyAsync(&h_fail, fail, sizeof(int), cudaMemcpyDeviceToHost, stream));
     CU(cudaStreamSynchronize(stream));

@@ -143,6 +143,11 @@ int main(int argc, char** argv) {
     else if (a == "--operator-form") { const std::string v = next(); if (v != "dense" && v != "implicit") { std::cerr << "--operator-form dense|implicit\n"; return 2; } o.operator_form = v == "implicit"; }
     else if (a == "--solver-type") { const std::string v = next(); o.solver_type = v == "SCHUR_COMPLEMENT" ? SolverOptions::SolverType::SCHUR_COMPLEMENT : v == "POWER_SCHUR_COMPLEMENT" ? SolverOptions::SolverType::POWER_SCHUR_COMPLEMENT : SolverOptions::SolverType::SQUARE_ROOT; }
     else if (a == "--power-order") o.power_order = std::stoi(next());
+    else if (a == "--linear-solver-type") {
+      const std::string v = next();
+      if (v != "ITERATIVE_SCHUR" && v != "DENSE_SCHUR") { std::cerr << "--linear-solver-type ITERATIVE_SCHUR|DENSE_SCHUR\n"; return 2; }
+      o.linear_solver_type = v == "DENSE_SCHUR" ? SolverOptions::LinearSolverType::DENSE_SCHUR : SolverOptions::LinearSolverType::ITERATIVE_SCHUR;
+    }
     else if (a == "--log-path") log_path = next();
     else if (a == "--loader") { const std::string v = next(); if (v != "parallel" && v != "map") { std::cerr << "--loader parallel|map\n"; return 2; } parallel_loader = v == "parallel"; }
     else if (a == "--num-threads") num_threads = std::stoi(next());
@@ -157,6 +162,9 @@ int main(int argc, char** argv) {
     else if (a == "--selftest-log") return selftest_log(next());
     else if (a == "--help" || a == "-h") {
       std::cout << "usage: bal_qr --input <bal file> [--no-use-double] [--max-num-iterations N] [--preconditioner-type JACOBI|SCHUR_JACOBI] ...\n"
+                   "  --linear-solver-type ITERATIVE_SCHUR|DENSE_SCHUR\n"
+                   "                        the camera increment by truncated PCG (default) or exactly, by a dense Cholesky\n"
+                   "                        factorisation of the reduced camera matrix\n"
                    "  --fix-intrinsics      hold f, k1, k2 of every camera constant\n"
                    "  --shared-intrinsics   every camera shares one f, k1, k2 (camera 0's at the start)\n"
                    "  --fix-cameras I,J,... hold every parameter of the listed cameras constant; indices refer to the loaded problem\n"

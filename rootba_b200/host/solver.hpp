@@ -47,6 +47,8 @@ struct SolverOptions {
   enum class SolverType { SQUARE_ROOT = 0, SCHUR_COMPLEMENT = 1, POWER_SCHUR_COMPLEMENT = 2 };  // solver_options.hpp:63-76
   SolverType solver_type = SolverType::SQUARE_ROOT;
   int power_order = 20;   // :270
+  enum class LinearSolverType { ITERATIVE_SCHUR = 0, DENSE_SCHUR = 1 };  // solver_options.hpp:77-80, 225-230
+  LinearSolverType linear_solver_type = LinearSolverType::ITERATIVE_SCHUR;  // DENSE_SCHUR: exact steps (rba_solver_opts.linear_solver_type)
   int operator_form = 0;  // not in the reference: 0 = dense Q2 panels (reference algorithm), 1 = implicit (rba_solver_opts.operator_form)
   bool use_projection_validity_check() const { return optimized_cost != OptimizedCost::ERROR; }  // solver_options.cpp:41-51
 };
@@ -168,6 +170,7 @@ class LinearizorQR {
     so.operator_form = o.operator_form;
     so.solver_type = (int)o.solver_type;  // Linearizor::create (linearizor.cpp:48-65): same entry points for the three solvers
     so.power_order = o.power_order;
+    so.linear_solver_type = (int)o.linear_solver_type;
     bp.export_topology(lm_off_, obs_cam_, obs_xy_);
     rba_problem_view pv{bp.num_cameras(), bp.num_landmarks(), (int64_t)obs_cam_.size(), lm_off_.data(), obs_cam_.data(), obs_xy_.data()};
     check(Abi<Scalar>::create(&pv, &so, &h_));

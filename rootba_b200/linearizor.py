@@ -61,6 +61,7 @@ class SolverOptions:  # bal/solver_options.hpp (QR-relevant subset, reference de
     pcg_check_period: int = 4
     operator_form: str = "DENSE"                  # DENSE (reference: Q2 panels) | IMPLICIT (Jp^T Jp - Q1d^T Q1d from records)
     stage2_form: str = "PANEL"                    # PANEL (reference: b and SCHUR_JACOBI blocks from the Q2 panels) | IDENTITY
+    linear_solver_type: str = "ITERATIVE_SCHUR"   # ITERATIVE_SCHUR (PCG / power series) | DENSE_SCHUR (exact, dense Cholesky; :77-80, 225-230)
 
     def use_projection_validity_check(self) -> bool:  # solver_options.cpp:41-51
         return self.optimized_cost != "ERROR"
@@ -546,6 +547,7 @@ class LinearizorQR:
         o.stage2_form = {"PANEL": 0, "IDENTITY": 1}[options.stage2_form]
         o.solver_type = {"SQUARE_ROOT": 0, "SCHUR_COMPLEMENT": 1, "POWER_SCHUR_COMPLEMENT": 2}[options.solver_type]  # linearizor.cpp:48-65
         o.power_order = options.power_order
+        o.linear_solver_type = {"ITERATIVE_SCHUR": 0, "DENSE_SCHUR": 1}[options.linear_solver_type]
         self._opts = o
         pv = ProblemView(bal_problem.num_cameras(), bal_problem.num_landmarks(), bal_problem.num_observations(),
                          bal_problem.lm_off.ctypes.data, bal_problem.obs_cam.ctypes.data, bal_problem.obs_xy.ctypes.data)
