@@ -45,7 +45,11 @@ def main():
     ap.add_argument("input")
     ap.add_argument("--float", action="store_true", help="float32 instead of float64 (--no-use-double of the reference)")
     ap.add_argument("--max-num-iterations", type=int, default=20)
-    ap.add_argument("--preconditioner-type", default="SCHUR_JACOBI", choices=["JACOBI", "SCHUR_JACOBI"])
+    ap.add_argument("--preconditioner-type", default="SCHUR_JACOBI", choices=["JACOBI", "SCHUR_JACOBI", "CLUSTER_JACOBI"],
+                    help="CLUSTER_JACOBI: the block diagonal of the reduced camera matrix over clusters of co-visible cameras")
+    ap.add_argument("--cluster-size", type=int, default=None,
+                    help="with CLUSTER_JACOBI: cluster the cameras with at most K per cluster (1..16; default: the library's)")
+    ap.add_argument("--clusters", default=None, help="with CLUSTER_JACOBI: one int32 cluster id per camera (.npy)")
     ap.add_argument("--operator-form", default="DENSE", choices=["DENSE", "IMPLICIT"])
     ap.add_argument("--linear-solver-type", default="ITERATIVE_SCHUR", choices=["ITERATIVE_SCHUR", "DENSE_SCHUR"],
                     help="the camera increment by truncated PCG, or exactly by a dense Cholesky factorisation of the reduced "
@@ -239,12 +243,30 @@ def main():
             print("wrote", args.triangulation)
     if args.rig_extrinsics and problem.camera_rig is None:
         ap.error("--rig-extrinsics needs --camera-rigs")
-    lin_ba = rb.LinearizorQR.create(problem, options) if args.rig_extrinsics else None
+    if (args.cluster_size is not None or args.clusters) and args.preconditioner_type != "CLUSTER_JACOBI":
+        ap.error("--cluster-size and --clusters need --preconditioner-type CLUSTER_JACOBI")
+    if args.cluster_size is not None and args.clusters:
+        ap.error("give --cluster-size or --clusters, not both")
+    clusters = None
+    if args.cluster_size is not None:
+        try:
+            clusters = rb.cluster_cameras(problem, args.cluster_size)
+        except rb.RbaError as e:
+            ap.error(f"--cluster-size: {e}")
+    elif args.clusters:
+        clusters = np.load(args.clusters)
+    lin_ba = rb.LinearizorQR.create(problem, options) if args.rig_extrinsics or clusters is not None else None
+    if clusters is not None:
+        try:
+            lin_ba.set_camera_clusters(clusters)
+        except (ValueError, rb.RbaError) as e:
+            ap.error(f"--clusters: {e}")
     summary = rb.bundle_adjust_manual(problem, options, linearizor=lin_ba, verbose=True)
-    if lin_ba is not None:
+    if lin_ba is not None and args.rig_extrinsics:
         extrinsics = lin_ba.rig_extrinsics()
-        lin_ba.close()
         np.save(args.rig_extrinsics, extrinsics)
+    if lin_ba is not None:
+        lin_ba.close()
         print("wrote", args.rig_extrinsics)
         if problem.rig_sensor is not None:  # a later handle ties the sensors' captures to the refined extrinsics
             sensor = problem.rig_sensor

@@ -65,7 +65,13 @@ typedef struct {
   int32_t robust_norm;                     /* 0 NONE, 1 HUBER  (bal_residual_options.hpp:52) */
   double huber_parameter;                  /* bal_residual_options.hpp:58 */
   double jacobi_scaling_epsilon;           /* :208 ; 0 -> Sophus epsilonSqrt (linearizor_base.cpp:72-79) */
-  int32_t preconditioner_type;             /* 0 JACOBI, 1 SCHUR_JACOBI (:217) */
+  int32_t preconditioner_type;             /* 0 JACOBI, 1 SCHUR_JACOBI (:217), 2 CLUSTER_JACOBI (:73-75): the block diagonal
+                                              of the reduced camera matrix over clusters of co-visible cameras, each
+                                              (9k) x (9k) block with its cross blocks factorised in float64 once per solve
+                                              (DESIGN.md section 28; rba_cluster_cameras, rba_set_camera_clusters).  Other
+                                              values -> RBA_ERR_INVALID_ARGUMENT; CLUSTER_JACOBI with solver_type = 2 or
+                                              linear_solver_type = DENSE_SCHUR (no PCG) -> RBA_ERR_INVALID_ARGUMENT, with
+                                              nranks > 1 -> RBA_ERR_UNSUPPORTED. */
   int32_t min_linear_solver_iterations;    /* :180 */
   int32_t max_linear_solver_iterations;    /* :184 */
   double eta;                              /* :189 */
@@ -775,6 +781,33 @@ int32_t rba_get_rhs(rba_handle* h, void* b_out);
  * blocks it was built from (damping and the camera and pair priors' diagonal A^T A blocks already added; the blocks are written with SCHUR_JACOBI) [81*Nc].  For a camera with rba_set_camera_fixed flags the inverse is
  * that of the free sub-block, embedded in the 9x9 slot with zero fixed rows and columns; the blocks are not masked. */
 int32_t rba_get_preconditioner(rba_handle* h, void* inv_out, void* blocks_out);
+
+/* ---- CLUSTER_JACOBI (preconditioner_type = 2, DESIGN.md section 28) ------------------------- */
+
+#define RBA_CLUSTER_MAX_CAMERAS 16     /* 144 rows: a float64 cluster block fits in one CTA's shared memory */
+#define RBA_CLUSTER_DEFAULT_CAMERAS 4  /* the cluster size rba_create_* clusters a CLUSTER_JACOBI handle's cameras with: the least slow of 4, 8 and 16 measured (DESIGN.md section 28) */
+
+/* Deterministic single linkage with a size cap over the co-visibility graph; pure host code, no GPU.  The weight of an edge
+ * (i, j) is the number of landmarks both cameras observe; the edges are merged in the order (weight descending, i, j) with
+ * union-find, and a merge happens only when the joined size is at most max_cluster_size.  cluster_of_camera [Nc] receives
+ * dense ids numbered by their smallest camera; a camera without observations is a cluster of its own.
+ * RBA_ERR_INVALID_ARGUMENT: max_cluster_size outside [1, RBA_CLUSTER_MAX_CAMERAS], a camera index out of range, a NULL
+ * pointer or no camera. */
+int32_t rba_cluster_cameras(const rba_problem_view* problem, int32_t max_cluster_size, int32_t* cluster_of_camera);
+/* Replaces the clustering of a CLUSTER_JACOBI handle from the next rba_solve on; NULL restores the default one
+ * (rba_cluster_cameras with RBA_CLUSTER_DEFAULT_CAMERAS, made by rba_create_*).  Ids outside [0, Nc), ids that are not
+ * dense (an unused id below the largest) or a cluster of more than RBA_CLUSTER_MAX_CAMERAS cameras ->
+ * RBA_ERR_INVALID_ARGUMENT; another preconditioner_type -> RBA_ERR_STATE.  A rejected or failed call leaves the handle
+ * untouched.  On a CLUSTER_JACOBI handle rba_set_intrinsics_groups and rba_set_camera_rigs with a group or rig of >= 2
+ * cameras, and rba_set_rig_sensors with a sensor id, return RBA_ERR_UNSUPPORTED and change nothing. */
+int32_t rba_set_camera_clusters(rba_handle* h, const int32_t* cluster_of_camera);
+/* Reads back the clustering in use (cluster_of_camera [Nc]), the last solve's cluster blocks before their factorisation
+ * (blocks: per cluster in id order a full row-major (9k) x (9k) float64 block, its cameras ascending: the Jacobi-scaled,
+ * damped reduced camera matrix restricted to the cluster, the camera and pair priors included, the rows and columns of held
+ * entries set to the identity) and a status per cluster (0 factorised, 1 a pivot was <= 0 or not finite and the cluster
+ * fell back to its cameras' SCHUR_JACOBI blocks).  Any pointer may be NULL.  RBA_ERR_STATE: another preconditioner_type,
+ * or blocks / status asked for before a solve with the current clustering. */
+int32_t rba_get_cluster_preconditioner(rba_handle* h, int32_t* cluster_of_camera, double* blocks, int32_t* status);
 /* LinearizationQR::right_multiply (linearization_qr.hpp:823-825): y = (Q2^T Jp)^T (Q2^T Jp) x + lambda x (+ A^T A x of the
  * camera priors and the pair priors, off-diagonal blocks included: the operator PCG applies) with the damping of the last rba_solve.  A debug accessor of the full operator: it ignores rba_set_camera_fixed. */
 int32_t rba_right_multiply(rba_handle* h, const void* x, void* y);

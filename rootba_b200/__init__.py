@@ -4,6 +4,6 @@ The compute path is the CUDA library rootba_b200/librootba_b200.so (C ABI: inclu
 Python here is only the host-side mirror of the reference interface and the synthetic-data generator.
 """
 from .linearizor import (BalProblem, LinearizorQR, ResidualOptions, SolverOptions, bundle_adjust_manual,  # noqa: F401
-                         nccl_unique_id, partition_landmarks)
+                         cluster_cameras, nccl_unique_id, partition_landmarks)
 from ._lib import FIX_ALL, FIX_F, FIX_INTRINSICS, FIX_K1, FIX_K2, FIX_POSE, RbaError, build  # noqa: F401
 from .ba_log import make_ba_log, save_ba_log, summarize_problem  # noqa: F401

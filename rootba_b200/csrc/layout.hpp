@@ -326,7 +326,9 @@ struct PairList {
 };
 
 // Returns "" on success or an error message.
-inline std::string build_pair_list(const Layout& L, PairList& P) {
+// cluster_of (CLUSTER_JACOBI, DESIGN.md section 28): keep only the terms of two different cameras of one cluster
+// (cluster_of[ca] == cluster_of[cb], ca > cb); wpos then indexes the landmark-major enumeration of the kept terms.
+inline std::string build_pair_list(const Layout& L, PairList& P, const int* cluster_of = nullptr) {
   const int nl = L.nl_local, nc = L.nc;
   P = PairList();
   P.slot0.resize(nl); P.nn.resize(nl);
@@ -338,14 +340,19 @@ inline std::string build_pair_list(const Layout& L, PairList& P) {
     P.nn[lm] = T.n;
     nt += (long long)T.n * (T.n + 1) / 2;
   }
-  if (nt > std::numeric_limits<int>::max()) return "more than 2^31 camera-pair terms";
+  if (!cluster_of && nt > std::numeric_limits<int>::max()) return "more than 2^31 camera-pair terms";
   // landmark-major list, then two stable counting sorts of its positions (by cb, then by ca): ascending (ca, cb),
   // landmark order kept
   std::vector<IntPair> raw;
-  raw.reserve((size_t)nt);
+  if (!cluster_of) raw.reserve((size_t)nt);
   for (int lm = 0; lm < nl; ++lm)
     for (int a = 0; a < P.nn[lm]; ++a)
-      for (int b = 0; b <= a; ++b) raw.push_back({P.slot0[lm] + a, P.slot0[lm] + b});  // camera(a) >= camera(b)
+      for (int b = 0; b <= a; ++b) {  // camera(a) >= camera(b)
+        const IntPair t{P.slot0[lm] + a, P.slot0[lm] + b};
+        if (cluster_of && (b == a || cluster_of[L.slot_cam[t.x]] != cluster_of[L.slot_cam[t.y]])) continue;
+        raw.push_back(t);
+      }
+  if (raw.size() > (size_t)std::numeric_limits<int>::max()) return "more than 2^31 camera-pair terms";
   std::vector<int> idx(raw.size()), tmp(raw.size());
   std::iota(idx.begin(), idx.end(), 0);
   std::vector<long long> cnt((size_t)nc + 1);
@@ -502,6 +509,147 @@ inline void plan_assembled(const Layout& L, const PairList& P, int scalar_size, 
     deal_spmv(A.row_ptr, spmv_ctas, spmv_chunk_blocks(scalar_size), A.spmv);
     A.device_bytes += (long long)A.spmv.chunks.size() * (long long)sizeof(SpmvChunk) + (A.spmv.ctas + 1) * (long long)sizeof(int);
   }
+}
+
+// ------------------------------------------------------------------------------------------------
+// CLUSTER_JACOBI (DESIGN.md section 28): the preconditioner is the block diagonal of S over clusters of co-visible cameras.
+// ------------------------------------------------------------------------------------------------
+constexpr int CLUSTER_MAX_CAMERAS = 16;  // 144 rows: a float64 block fits in one CTA's shared memory
+
+// Single linkage with a size cap over the co-visibility graph (rba_cluster_cameras).  The weight of an edge (i, j) is the
+// number of landmarks both cameras observe; the edges are merged in the order (weight descending, i, j) with union-find,
+// and a merge happens only when the joined size is at most max_size.  Cluster ids are dense and numbered by their smallest
+// camera.  Returns "" on success or an error message.
+inline std::string cluster_cameras(int nc, int nl, const int64_t* lm_off, const int32_t* obs_cam, int max_size, int* cluster_of) {
+  if (max_size < 1 || max_size > CLUSTER_MAX_CAMERAS)
+    return "max_cluster_size " + std::to_string(max_size) + " is outside [1, " + std::to_string(CLUSTER_MAX_CAMERAS) + "]";
+  std::vector<long long> keys;  // i * nc + j, i < j, once per landmark that both observe
+  for (int l = 0; l < nl; ++l) {
+    if (lm_off[l + 1] < lm_off[l]) return "lm_obs_offset is not ascending";
+    for (int64_t a = lm_off[l]; a < lm_off[l + 1]; ++a) {
+      const int ca = obs_cam[a];
+      if (ca < 0 || ca >= nc) return "camera index out of range";
+      for (int64_t b = lm_off[l]; b < a; ++b) {
+        const int cb = obs_cam[b];
+        if (ca != cb) keys.push_back((long long)std::min(ca, cb) * nc + std::max(ca, cb));
+      }
+    }
+  }
+  std::sort(keys.begin(), keys.end());
+  struct Edge { long long w, key; };
+  std::vector<Edge> edges;
+  for (size_t k = 0; k < keys.size();) {
+    size_t e = k;
+    while (e < keys.size() && keys[e] == keys[k]) ++e;
+    edges.push_back({(long long)(e - k), keys[k]});
+    k = e;
+  }
+  std::stable_sort(edges.begin(), edges.end(), [](const Edge& a, const Edge& b) { return a.w > b.w; });  // key order kept
+  std::vector<int> parent(nc), size(nc, 1);
+  std::iota(parent.begin(), parent.end(), 0);
+  auto find = [&](int c) { while (parent[c] != c) c = parent[c] = parent[parent[c]]; return c; };
+  for (const Edge& e : edges) {
+    const int ri = find((int)(e.key / nc)), rj = find((int)(e.key % nc));
+    if (ri == rj || size[ri] + size[rj] > max_size) continue;
+    const int lo = std::min(ri, rj), hi = std::max(ri, rj);
+    parent[hi] = lo;
+    size[lo] += size[hi];
+  }
+  std::vector<int> id(nc, -1);
+  int next = 0;
+  for (int c = 0; c < nc; ++c) {
+    const int r = find(c);
+    if (id[r] < 0) id[r] = next++;
+    cluster_of[c] = id[r];
+  }
+  return "";
+}
+
+// "" when cluster_of holds dense ids 0..ncl-1 (every id used) and no cluster has more than CLUSTER_MAX_CAMERAS cameras
+inline std::string check_clusters(int nc, const int* cluster_of, int& ncl) {
+  ncl = 0;
+  std::vector<int> count(nc, 0);
+  for (int c = 0; c < nc; ++c) {
+    const int k = cluster_of[c];
+    if (k < 0 || k >= nc) return "camera " + std::to_string(c) + " has cluster id " + std::to_string(k) + ", outside [0, " + std::to_string(nc) + ")";
+    if (++count[k] > CLUSTER_MAX_CAMERAS) return "cluster " + std::to_string(k) + " has more than " + std::to_string(CLUSTER_MAX_CAMERAS) + " cameras";
+    ncl = std::max(ncl, k + 1);
+  }
+  for (int k = 0; k < ncl; ++k)
+    if (!count[k]) return "cluster ids are not dense: id " + std::to_string(k) + " is unused below " + std::to_string(ncl - 1);
+  return "";
+}
+
+// One cross block S[a, b] (a > b) of a cluster: its cameras' positions inside the cluster and its terms [t0, t1).
+struct ClusterBlock {
+  int la, lb, t0, t1;
+};
+
+// The device structure of a clustering.  Clusters in id order, their cameras ascending; per cluster the offsets of its
+// (9k)^2 block and of its packed lower factor (9k (9k + 1) / 2 entries, row-major); the cross blocks grouped by cluster,
+// ascending (ca, cb) inside one; the intra-cluster terms (build_pair_list with the cluster filter) as slot pairs and, for
+// the panel form, as panel addresses (pack_asm_term).
+struct ClusterPlan {
+  int ncl = 0, max_k = 0;
+  std::vector<int> ptr, cams;                    // [ncl + 1], [nc]
+  std::vector<long long> blk_off, fac_off;       // [ncl + 1]
+  std::vector<int> xb_ptr;                       // [ncl + 1] into xb
+  std::vector<ClusterBlock> xb;
+  std::vector<IntPair> slots;                    // [nt] (slot_a, slot_b)
+  std::vector<AsmTerm> panel_terms;              // [nt] when asked for
+  long long device_bytes = 0;                    // the structure's and the blocks', factors' and statuses' bytes
+};
+
+// Returns "" on success or an error message (from check_clusters).
+inline std::string plan_clusters(const Layout& L, const int* cluster_of, bool panel_terms, ClusterPlan& C) {
+  C = ClusterPlan();
+  const int nc = L.nc;
+  std::string msg = check_clusters(nc, cluster_of, C.ncl);
+  if (!msg.empty()) return msg;
+  const int ncl = C.ncl;
+  C.ptr.assign((size_t)ncl + 1, 0);
+  for (int c = 0; c < nc; ++c) ++C.ptr[cluster_of[c] + 1];
+  for (int k = 0; k < ncl; ++k) C.ptr[k + 1] += C.ptr[k];
+  C.cams.resize(nc);
+  std::vector<int> fill(C.ptr.begin(), C.ptr.end() - 1), local(nc);
+  for (int c = 0; c < nc; ++c) { local[c] = fill[cluster_of[c]] - C.ptr[cluster_of[c]]; C.cams[fill[cluster_of[c]]++] = c; }
+  C.blk_off.assign((size_t)ncl + 1, 0);
+  C.fac_off.assign((size_t)ncl + 1, 0);
+  for (int k = 0; k < ncl; ++k) {
+    const long long m = 9LL * (C.ptr[k + 1] - C.ptr[k]);
+    C.max_k = std::max(C.max_k, C.ptr[k + 1] - C.ptr[k]);
+    C.blk_off[k + 1] = C.blk_off[k] + m * m;
+    C.fac_off[k + 1] = C.fac_off[k] + m * (m + 1) / 2;
+  }
+  PairList P;
+  msg = build_pair_list(L, P, cluster_of);
+  if (!msg.empty()) return msg;
+  const size_t nb = P.blk_cam.size();
+  C.xb_ptr.assign((size_t)ncl + 1, 0);
+  for (const IntPair& b : P.blk_cam) ++C.xb_ptr[cluster_of[b.x] + 1];
+  for (int k = 0; k < ncl; ++k) C.xb_ptr[k + 1] += C.xb_ptr[k];
+  C.xb.resize(nb);
+  std::vector<int> xfill(C.xb_ptr.begin(), C.xb_ptr.end() - 1);
+  for (size_t b = 0; b < nb; ++b) {
+    const IntPair cc = P.blk_cam[b];
+    C.xb[xfill[cluster_of[cc.x]]++] = {local[cc.x], local[cc.y], P.blk_ptr[b], P.blk_ptr[b + 1]};
+  }
+  C.slots = P.terms;
+  if (panel_terms) {
+    C.panel_terms.reserve(P.terms.size());
+    for (const IntPair& t : P.terms) {
+      const int lm = L.slot_lm[t.x], sidx = L.sorted_of_lm[lm];
+      const TileInfo& T = L.tiles[L.tile_of_sorted[sidx]];
+      const int g = sidx - T.lm_base;
+      C.panel_terms.push_back(pack_asm_term(T.panel_off + 2LL * g * T.G, t.x - P.slot0[lm], t.y - P.slot0[lm], T.n, T.G, T.KP));
+    }
+  }
+  C.device_bytes = (long long)(C.ptr.size() + C.cams.size() + C.xb_ptr.size()) * (long long)sizeof(int) +
+                   (long long)(C.blk_off.size() + C.fac_off.size()) * (long long)sizeof(long long) +
+                   (long long)C.xb.size() * (long long)sizeof(ClusterBlock) + (long long)C.slots.size() * (long long)sizeof(IntPair) +
+                   (long long)C.panel_terms.size() * (long long)sizeof(AsmTerm) +
+                   (C.blk_off[ncl] + C.fac_off[ncl]) * 8 + (long long)ncl * (long long)sizeof(int);
+  return "";
 }
 
 }  // namespace rba

@@ -20,6 +20,7 @@
 #include "kernels.cuh"
 #include "covariance.cuh"
 #include "dense_solve.cuh"
+#include "cluster_precond.cuh"
 #include "assembled.cuh"
 #include "rigs.cuh"
 #include "triangulate.cuh"
@@ -32,6 +33,7 @@ thread_local std::string g_err;
 
 // the host builds the pair lists as IntPair (layout.hpp); the kernels read them as int2
 static_assert(sizeof(IntPair) == sizeof(int2), "IntPair must have the layout of int2");
+static_assert(RBA_CLUSTER_MAX_CAMERAS == CLUSTER_MAX_CAMERAS, "the header and the layout agree on the largest cluster");
 static_assert(sizeof(rba_triangulate_opts) == 32, "rba_triangulate_opts is 32 bytes without implicit padding");
 static_assert(sizeof(rba_resect_opts) == 24, "rba_resect_opts is 24 bytes without implicit padding");
 
@@ -105,6 +107,8 @@ struct rba_handle {
   virtual int get_scaling(void* scaling, void* diag2) = 0;
   virtual int get_rhs(void* b) = 0;
   virtual int get_precond(void* inv, void* blocks) = 0;
+  virtual int set_camera_clusters(const int32_t* cluster_of) = 0;
+  virtual int get_cluster_precond(int32_t* cluster_of, double* blocks, int32_t* status) = 0;
   virtual int right_multiply(const void* x, void* y) = 0;
   virtual int debug_get_block(int lm, void* out, int rows, int cols, void* jls) = 0;
   virtual int compute_covariance(double* cam_cov, double* lm_cov) = 0;
@@ -329,6 +333,28 @@ struct Solver : rba_handle {
     int* fail = nullptr;
     long long np = 0;
   } dn;
+  // preconditioner_type = CLUSTER_JACOBI (cluster_precond.cuh, DESIGN.md section 28).  The clustering's structure, blocks,
+  // factors and statuses are the term's own (rba_set_camera_clusters adopts new ones once they all exist); bh (L^-1 b),
+  // w (L^-T v), yh (L^-1 S w) and eye (the vector step's identity blocks) are allocated once by setup_clusters.
+  struct ClusterTerm {
+    bool on = false;
+    std::vector<int> host, dflt;   // [nc] the clustering in use, the default one (rba_cluster_cameras at create)
+    int ncl = 0, max_k = 0;
+    long long blk_n = 0, fac_n = 0;  // doubles of the blocks and of the factors
+    DeviceBuffer<int> ptr, cams, xb_ptr, status;
+    DeviceBuffer<long long> blk_off, fac_off;
+    DeviceBuffer<ClusterBlock> xb;
+    DeviceBuffer<IntPair> slots;
+    DeviceBuffer<AsmTerm> panel_terms;
+    DeviceBuffer<double> blocks, factor;
+    S* bh = nullptr; S* w = nullptr; S* yh = nullptr; S* eye = nullptr;
+    bool built = false;            // a solve has assembled the blocks of this clustering
+    void adopt(ClusterTerm& o) {
+      ptr.take(o.ptr); cams.take(o.cams); xb_ptr.take(o.xb_ptr); status.take(o.status); blk_off.take(o.blk_off);
+      fac_off.take(o.fac_off); xb.take(o.xb); slots.take(o.slots); panel_terms.take(o.panel_terms); blocks.take(o.blocks);
+      factor.take(o.factor);
+    }
+  } clu;
   // assembled operator (setup_assembled, assembled.cuh): the terms as panel addresses in landmark-major order, the pair
   // list (term ranges, landmark-major position of every term), per pair its positions (lower, upper or -1) in the full
   // block-row CSR of S, the staging buffer of all terms, S_u per pair and S
@@ -437,6 +463,7 @@ struct Solver : rba_handle {
     TRY(alloc_buffers());
     TRY(setup_assembled());
     TRY(setup_dense());
+    TRY(setup_clusters(pv));
     TRY(setup_kernels());
     CU(cudaStreamSynchronize(stream));
     return RBA_OK;
@@ -451,6 +478,10 @@ struct Solver : rba_handle {
     if (opt.linear_solver_type != 0 && opt.linear_solver_type != 1) { g_err = "linear_solver_type must be 0 (ITERATIVE_SCHUR) or 1 (DENSE_SCHUR)"; return RBA_ERR_INVALID_ARGUMENT; }
     if (opt.linear_solver_type == 1 && opt.solver_type == 2) { g_err = "DENSE_SCHUR does not combine with POWER_SCHUR_COMPLEMENT: the power series is itself the linear solver"; return RBA_ERR_INVALID_ARGUMENT; }
     if (opt.linear_solver_type == 1 && opt.nranks > 1) { g_err = "DENSE_SCHUR runs on one GPU: the dense reduced camera matrix would need a cross-rank sum"; return RBA_ERR_UNSUPPORTED; }
+    if (opt.preconditioner_type < 0 || opt.preconditioner_type > 2) { g_err = "preconditioner_type must be 0 (JACOBI), 1 (SCHUR_JACOBI) or 2 (CLUSTER_JACOBI)"; return RBA_ERR_INVALID_ARGUMENT; }
+    if (opt.preconditioner_type == 2 && opt.solver_type == 2) { g_err = "CLUSTER_JACOBI does not combine with POWER_SCHUR_COMPLEMENT: the power series has no PCG"; return RBA_ERR_INVALID_ARGUMENT; }
+    if (opt.preconditioner_type == 2 && opt.linear_solver_type == 1) { g_err = "CLUSTER_JACOBI does not combine with DENSE_SCHUR: the dense solve has no PCG"; return RBA_ERR_INVALID_ARGUMENT; }
+    if (opt.preconditioner_type == 2 && opt.nranks > 1) { g_err = "CLUSTER_JACOBI runs on one GPU: a cluster block would need a cross-rank sum"; return RBA_ERR_UNSUPPORTED; }
     if (opt.stage2_form != 0 && opt.stage2_form != 1) { g_err = "stage2_form must be 0 (Q2 panel, reference) or 1 (orthogonality identity)"; return RBA_ERR_INVALID_ARGUMENT; }
     if (opt.pcg_check_period <= 0) opt.pcg_check_period = 4;
     if (opt.residual_reset_period <= 0) opt.residual_reset_period = 10;
@@ -626,7 +657,7 @@ struct Solver : rba_handle {
     // the damping rows per slot: read by the SCHUR_JACOBI blocks of the panel form and by the assembly of S
     if (panel_form() || asm_candidate()) TRY(dalloc(&D.dmp, (size_t)28 * L.nslots));
     if (panel_form()) {
-      if (opt.preconditioner_type == 1) TRY(dalloc(&D.blk0, (size_t)48 * L.nslots));
+      if (opt.preconditioner_type >= 1) TRY(dalloc(&D.blk0, (size_t)48 * L.nslots));  // (CLUSTER_JACOBI: its diagonal blocks)
       TRY(dalloc(&D.blocks0, (size_t)81 * nc));
       TRY(dalloc(&D.b0, (size_t)9 * nc));
     }
@@ -887,6 +918,8 @@ struct Solver : rba_handle {
       if (lead[c] == c) gidx[c] = ng++;
     if (ng > 0 && opt.solver_type == 2)
       return fail(RBA_ERR_UNSUPPORTED, "POWER_SCHUR_COMPLEMENT does not support groups of >= 2 cameras (Hpp of the tied problem is not block-diagonal)");
+    if (ng > 0 && clu.on)
+      return fail(RBA_ERR_UNSUPPORTED, "CLUSTER_JACOBI does not support groups of >= 2 cameras (the tied system changes the unknowns of the cluster blocks)");
     const std::string why = group_flags_mismatch(lead, held.host);
     if (!why.empty()) return fail(RBA_ERR_INVALID_ARGUMENT, why);
     ptr.assign((size_t)ng + 1, 0);
@@ -1004,6 +1037,8 @@ struct Solver : rba_handle {
     for (int c = 0; c < nc; ++c) nr += lead[c] == c;
     if (nr > 0 && opt.solver_type == 2)
       return fail(RBA_ERR_UNSUPPORTED, "POWER_SCHUR_COMPLEMENT does not support rigs of >= 2 cameras (Hpp of the tied problem is not block-diagonal)");
+    if (nr > 0 && clu.on)
+      return fail(RBA_ERR_UNSUPPORTED, "CLUSTER_JACOBI does not support rigs of >= 2 cameras (the tied system changes the unknowns of the cluster blocks)");
     const std::string why = rig_flags_mismatch(lead, held.host);
     if (!why.empty()) return fail(RBA_ERR_INVALID_ARGUMENT, why);
     if (nr > 0) {
@@ -1105,6 +1140,10 @@ struct Solver : rba_handle {
     auto fail = [&](const std::string& what) { g_err = "rba_set_rig_sensors: " + what; return RBA_ERR_INVALID_ARGUMENT; };
     std::vector<int> home((size_t)nc, -1), lead = rig.host_first;
     int ns = 0;
+    if (sensor && clu.on && std::any_of(sensor, sensor + nc, [](int32_t v) { return v >= 0; })) {
+      g_err = "rba_set_rig_sensors: CLUSTER_JACOBI does not support sensors (the tied system changes the unknowns of the cluster blocks)";
+      return RBA_ERR_UNSUPPORTED;
+    }
     if (sensor) {
       std::vector<int> first((size_t)nc, -1), new_lead((size_t)nc, -1);
       std::vector<std::pair<int, int>> rig_sensor;  // (the rig's lowest-index camera, sensor id) of every sensor camera
@@ -2000,7 +2039,7 @@ struct Solver : rba_handle {
       // rows 3..2n-1 of the Q2 panels do not change with lambda: their part of the gradient (ipp:443-466) and of the
       // SCHUR_JACOBI blocks (ipp:520-552) is accumulated once per linearisation (this shard only; the sum over the
       // shards happens in solve() together with the damping-row part)
-      const int want_blocks = opt.preconditioner_type == 1 ? 1 : 0;
+      const int want_blocks = opt.preconditioner_type >= 1 ? 1 : 0;
       k_panel_grad_blocks<S><<<tile_grid(sm_count * 8), TILE_WARPS * 32, 0, stream>>>(D, want_blocks, order_kp);
       ++launches;
       rc = camera_reduce(d_csr_obs_slots, d_csr_obs_items, n_obs_items, d_csr_obs_item_ptr, D.b0, nullptr, false); if (rc) return rc;
@@ -2125,6 +2164,11 @@ struct Solver : rba_handle {
     if (grp.n || rig.n) {  // the contracted output, which holds the prior terms already (k_group_contract, k_rig_contract)
       Dv.y = tied_y(); Dv.prior_H = nullptr; Dv.pair_ov = nullptr;
     }
+    if (clu.on) {  // CLUSTER_JACOBI: L^-1 S L^-T (k_cluster_fwd wrote it whole into yh), L^-1 b, the masked identity blocks
+      Dv.y = clu.yh; Dv.b = clu.bh; Dv.inv = clu.eye; Dv.prior_H = nullptr; Dv.pair_ov = nullptr;
+      lambda = S(0);
+      from_partials = false;
+    }
     if (Dv.pair_ov && mode != 3) TRY(pair_ov(mode == 2 ? D.x : D.p, pdl));
     auto kern = Dv.pair_ov ? k_pcg_vec<S, true, true> : Dv.prior_H ? k_pcg_vec<S, true> : k_pcg_vec<S, false>;
     return launch_ex(kern, pcg_cluster, VEC_THREADS, 0, pdl, pcg_cluster, Dv, d_state, lambda, i, mode, (double)opt.eta,
@@ -2139,6 +2183,14 @@ struct Solver : rba_handle {
   // and rig.y; both: P~ v into rig.ve, P of it in place, the group contraction into grp.y and the rigs' in place there)
   int pcg_step(int i, int mode, int is_last, S lambda, Handover h) {
     const S* v = mode == 2 ? D.x : D.p;
+    if (clu.on) {  // CLUSTER_JACOBI (DESIGN.md section 28): S applied to w = L^-T v, then L^-1 of its output
+      cluster_back(v, clu.w, &d_state->done);
+      TRY(apply_operator(clu.w, h, true));
+      k_cluster_fwd<S><<<clu.ncl, CLUSTER_THREADS, cluster_factor_smem(clu.max_k), stream>>>(
+          cluster_view(), D, D.y, h == Handover::Partials ? op_item_ptr : nullptr, clu.w, lambda, clu.yh, &d_state->done);
+      ++launches;
+      return pcg_vec(i, mode, true, is_last, lambda);
+    }
     if (rig.n) {
       TRY(rig_expand(v, rig.ve.get(), true));
       v = rig.ve.get();
@@ -2231,7 +2283,8 @@ struct Solver : rba_handle {
     s_valid = su_new = false;  // S of the previous lambda; rebuilt if this solve runs long enough (solve_enqueue)
     rc = camera_reduce(d_csr_obs_slots, d_csr_obs_items, n_obs_items, d_csr_obs_item_ptr, D.b, panel_form() ? D.b0 : nullptr); if (rc) return rc;
     const bool power = opt.solver_type == 2;
-    const bool schur = opt.preconditioner_type == 1 && !power;  // Power-SC inverts Hpp = sum Jp^T Jp + lambda I instead
+    // (CLUSTER_JACOBI: the SCHUR_JACOBI blocks are its diagonal blocks)
+    const bool schur = opt.preconditioner_type >= 1 && !power;  // Power-SC inverts Hpp = sum Jp^T Jp + lambda I instead
     if (schur) { rc = panel_form() ? precond_blocks(2, D.blocks, D.blocks0, true) : precond_blocks(1, D.blocks, nullptr, true); if (rc) return rc; }
     rc = stop(ev_stage2); if (rc) return rc;
     rc = start(ev_precond); if (rc) return rc;
@@ -2265,6 +2318,7 @@ struct Solver : rba_handle {
                                                              D.prior_H ? (const S*)cprior.g.get() : nullptr);
       ++launches;
     }
+    if (clu.on && !held.all) TRY(cluster_build());  // the cluster blocks and their factors (CLUSTER_JACOBI, section 28)
     rc = stop(ev_precond); if (rc) return rc;
     last_lambda = lambda;
     damping_valid = true;
@@ -2337,6 +2391,7 @@ struct Solver : rba_handle {
         rc = enqueue_iteration(i); if (rc) return rc;
       }
     }
+    if (clu.on) cluster_back(D.inc, D.inc, nullptr);  // inc = -L^-T x^ (CLUSTER_JACOBI)
     TRY(tie_expand(D.inc));  // inc = P u for the back-substitution, the update and inc_out
     CU(cudaMemcpyAsync(&h_state[0], d_state, sizeof(PcgState), cudaMemcpyDeviceToHost, stream));
     if (inc_out) CU(cudaMemcpyAsync(inc_out, D.inc, (size_t)9 * nc * sizeof(S), cudaMemcpyDeviceToHost, stream));
@@ -2752,6 +2807,75 @@ struct Solver : rba_handle {
       cov_gemm<false, true>(m, TB, TB, 1.0, W, m, Tt, TB, 0.0, P, np, 0, 0);
       cov_gemm<false, true>(m, m, TB, -1.0, P, np, P, np, 1.0, P + TB * np, np, 1, 0);
     }
+    return RBA_OK;
+  }
+
+  // ------------------------------------------------------------------------------------------
+  // preconditioner_type = CLUSTER_JACOBI (cluster_precond.cuh, DESIGN.md section 28)
+  // The per-solve vectors and the default clustering (rba_cluster_cameras with RBA_CLUSTER_DEFAULT_CAMERAS).
+  int setup_clusters(const rba_problem_view* pv) {
+    if (opt.preconditioner_type != 2) return RBA_OK;
+    clu.dflt.resize((size_t)nc);
+    const std::string msg = cluster_cameras(nc, nl_total, pv->lm_obs_offset, pv->obs_cam_idx, RBA_CLUSTER_DEFAULT_CAMERAS, clu.dflt.data());
+    if (!msg.empty()) { g_err = msg; return RBA_ERR_INVALID_ARGUMENT; }
+    for (S** v : {&clu.bh, &clu.w, &clu.yh}) TRY(dalloc(v, (size_t)9 * nc));
+    TRY(dalloc(&clu.eye, (size_t)81 * nc));
+    clu.on = true;
+    return set_camera_clusters(nullptr);
+  }
+  // Every check runs before anything changes, and the new buffers are adopted once they all exist, so a rejected or failed
+  // call leaves the previous clustering.
+  int set_camera_clusters(const int32_t* cluster_of) override {
+    if (!clu.on) { g_err = "rba_set_camera_clusters: the handle's preconditioner_type is not CLUSTER_JACOBI"; return RBA_ERR_STATE; }
+    std::vector<int> host = cluster_of ? std::vector<int>(cluster_of, cluster_of + nc) : clu.dflt;
+    ClusterPlan P;
+    const std::string msg = plan_clusters(L, host.data(), panels, P);
+    if (!msg.empty()) { g_err = "rba_set_camera_clusters: " + msg; return RBA_ERR_INVALID_ARGUMENT; }
+    ClusterTerm next;
+    TRY(fit(next.ptr, {}, P.ptr.size(), &P.ptr)); TRY(fit(next.cams, {}, P.cams.size(), &P.cams));
+    TRY(fit(next.xb_ptr, {}, P.xb_ptr.size(), &P.xb_ptr)); TRY(fit(next.blk_off, {}, P.blk_off.size(), &P.blk_off));
+    TRY(fit(next.fac_off, {}, P.fac_off.size(), &P.fac_off)); TRY(fit(next.xb, {}, P.xb.size(), &P.xb));
+    TRY(fit(next.slots, {}, P.slots.size(), &P.slots)); TRY(fit(next.panel_terms, {}, P.panel_terms.size(), &P.panel_terms));
+    TRY(alloc(next.status, (size_t)P.ncl, true)); TRY(alloc(next.blocks, (size_t)P.blk_off[P.ncl], true));
+    TRY(alloc(next.factor, (size_t)P.fac_off[P.ncl], true));
+    const size_t smem = (size_t)81 * P.max_k * P.max_k * sizeof(double), fsmem = cluster_factor_smem(P.max_k);
+    CU(cudaFuncSetAttribute(k_cluster_build<S>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    CU(cudaFuncSetAttribute(k_cluster_fwd<S>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fsmem));
+    CU(cudaFuncSetAttribute(k_cluster_back<S>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fsmem));
+    CU(cudaStreamSynchronize(stream));
+    clu.adopt(next);
+    clu.host = std::move(host);
+    clu.ncl = P.ncl; clu.max_k = P.max_k; clu.blk_n = P.blk_off[P.ncl]; clu.fac_n = P.fac_off[P.ncl];
+    clu.built = false;
+    return RBA_OK;
+  }
+  static size_t cluster_factor_smem(int max_k) { return (size_t)(9 * max_k) * (9 * max_k + 1) / 2 * sizeof(double); }
+  ClusterView cluster_view() const {
+    return {clu.ncl, clu.ptr.get(), clu.cams.get(), clu.blk_off.get(), clu.fac_off.get(), clu.xb_ptr.get(), clu.xb.get(),
+            (const int2*)clu.slots.get(), panels ? clu.panel_terms.get() : nullptr, clu.blocks.get(), clu.factor.get(), clu.status.get()};
+  }
+  // the cluster blocks of this solve's lambda, their factors, the vector step's identity blocks and bh = L^-1 b (after
+  // k_precond_invert: the SCHUR_JACOBI blocks are written and b is final)
+  int cluster_build() {
+    const ClusterView cv = cluster_view();
+    k_cluster_build<S><<<clu.ncl, 256, (size_t)81 * clu.max_k * clu.max_k * sizeof(double), stream>>>(cv, D, clu.eye);
+    k_cluster_fwd<S><<<clu.ncl, CLUSTER_THREADS, cluster_factor_smem(clu.max_k), stream>>>(cv, D, D.b, nullptr, nullptr, S(0), clu.bh, nullptr);
+    launches += 2;
+    clu.built = true;
+    return RBA_OK;
+  }
+  // y = L^-T v (done: inside a solve, nothing once it has ended)
+  void cluster_back(const S* v, S* y, const int* done) {
+    k_cluster_back<S><<<clu.ncl, CLUSTER_THREADS, cluster_factor_smem(clu.max_k), stream>>>(cluster_view(), v, y, done);
+    ++launches;
+  }
+  int get_cluster_precond(int32_t* cluster_of, double* blocks, int32_t* status) override {
+    if (!clu.on) { g_err = "rba_get_cluster_preconditioner: the handle's preconditioner_type is not CLUSTER_JACOBI"; return RBA_ERR_STATE; }
+    if ((blocks || status) && !clu.built) { g_err = "rba_get_cluster_preconditioner: no solve has assembled the blocks of this clustering"; return RBA_ERR_STATE; }
+    if (cluster_of) std::copy(clu.host.begin(), clu.host.end(), cluster_of);
+    if (blocks) CU(cudaMemcpyAsync(blocks, clu.blocks.get(), (size_t)clu.blk_n * sizeof(double), cudaMemcpyDeviceToHost, stream));
+    if (status) CU(cudaMemcpyAsync(status, clu.status.get(), (size_t)clu.ncl * sizeof(int), cudaMemcpyDeviceToHost, stream));
+    CU(cudaStreamSynchronize(stream));
     return RBA_OK;
   }
 
@@ -3360,6 +3484,20 @@ int32_t rba_get_timings(const rba_handle* h, rba_stage_timings* out) { return h-
 int32_t rba_get_jacobian_scaling(rba_handle* h, void* s, void* d) { return h->get_scaling(s, d); }
 int32_t rba_get_rhs(rba_handle* h, void* b) { return h->get_rhs(b); }
 int32_t rba_get_preconditioner(rba_handle* h, void* inv, void* blocks) { return h->get_precond(inv, blocks); }
+int32_t rba_cluster_cameras(const rba_problem_view* p, int32_t max_cluster_size, int32_t* cluster_of_camera) {
+  if (!p || !cluster_of_camera || p->num_cameras <= 0 || p->num_landmarks < 0 || !p->lm_obs_offset || (p->num_landmarks > 0 && !p->obs_cam_idx)) {
+    rba::g_err = "rba_cluster_cameras: null or empty argument";
+    return RBA_ERR_INVALID_ARGUMENT;
+  }
+  const std::string msg = rba::cluster_cameras(p->num_cameras, p->num_landmarks, p->lm_obs_offset, p->obs_cam_idx, max_cluster_size,
+                                               cluster_of_camera);
+  if (!msg.empty()) { rba::g_err = "rba_cluster_cameras: " + msg; return RBA_ERR_INVALID_ARGUMENT; }
+  return RBA_OK;
+}
+int32_t rba_set_camera_clusters(rba_handle* h, const int32_t* cluster_of_camera) { return h->set_camera_clusters(cluster_of_camera); }
+int32_t rba_get_cluster_preconditioner(rba_handle* h, int32_t* cluster_of_camera, double* blocks, int32_t* status) {
+  return h->get_cluster_precond(cluster_of_camera, blocks, status);
+}
 int32_t rba_right_multiply(rba_handle* h, const void* x, void* y) { return h->right_multiply(x, y); }
 int32_t rba_debug_get_block(rba_handle* h, int32_t lm, void* out, int32_t rows, int32_t cols, void* jls) {
   return h->debug_get_block(lm, out, rows, cols, jls);

@@ -136,7 +136,13 @@ int main(int argc, char** argv) {
     else if (a == "--max-linear-solver-iterations") o.max_linear_solver_iterations = std::stoi(next());
     else if (a == "--eta") o.eta = std::stod(next());
     else if (a == "--function-tolerance") o.function_tolerance = std::stod(next());
-    else if (a == "--preconditioner-type") { const std::string v = next(); o.preconditioner_type = v == "JACOBI" ? SolverOptions::PreconditionerType::JACOBI : SolverOptions::PreconditionerType::SCHUR_JACOBI; }
+    else if (a == "--preconditioner-type") {
+      const std::string v = next();
+      if (v == "JACOBI") o.preconditioner_type = SolverOptions::PreconditionerType::JACOBI;
+      else if (v == "SCHUR_JACOBI") o.preconditioner_type = SolverOptions::PreconditionerType::SCHUR_JACOBI;
+      else if (v == "CLUSTER_JACOBI") o.preconditioner_type = SolverOptions::PreconditionerType::CLUSTER_JACOBI;
+      else { std::cerr << "--preconditioner-type JACOBI|SCHUR_JACOBI|CLUSTER_JACOBI\n"; return 2; }
+    }
     else if (a == "--residual-robust-norm") { const std::string v = next(); o.robust_norm = v == "HUBER" ? SolverOptions::RobustNorm::HUBER : SolverOptions::RobustNorm::NONE; }
     else if (a == "--residual-huber-parameter") o.huber_parameter = std::stod(next());
     else if (a == "--optimized-cost") { const std::string v = next(); o.optimized_cost = v == "ERROR" ? SolverOptions::OptimizedCost::ERROR : v == "ERROR_VALID" ? SolverOptions::OptimizedCost::ERROR_VALID : SolverOptions::OptimizedCost::ERROR_VALID_AVG; }
@@ -161,7 +167,7 @@ int main(int argc, char** argv) {
     }
     else if (a == "--selftest-log") return selftest_log(next());
     else if (a == "--help" || a == "-h") {
-      std::cout << "usage: bal_qr --input <bal file> [--no-use-double] [--max-num-iterations N] [--preconditioner-type JACOBI|SCHUR_JACOBI] ...\n"
+      std::cout << "usage: bal_qr --input <bal file> [--no-use-double] [--max-num-iterations N] [--preconditioner-type JACOBI|SCHUR_JACOBI|CLUSTER_JACOBI] ...\n"
                    "  --linear-solver-type ITERATIVE_SCHUR|DENSE_SCHUR\n"
                    "                        the camera increment by truncated PCG (default) or exactly, by a dense Cholesky\n"
                    "                        factorisation of the reduced camera matrix\n"

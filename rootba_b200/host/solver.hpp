@@ -22,7 +22,7 @@
 namespace rootba_b200 {
 
 struct SolverOptions {
-  enum class PreconditionerType { JACOBI = 0, SCHUR_JACOBI = 1 };
+  enum class PreconditionerType { JACOBI = 0, SCHUR_JACOBI = 1, CLUSTER_JACOBI = 2 };  // solver_options.hpp:73-75
   enum class OptimizedCost { ERROR = 0, ERROR_VALID = 1, ERROR_VALID_AVG = 2 };
   enum class RobustNorm { NONE = 0, HUBER = 1 };
   OptimizedCost optimized_cost = OptimizedCost::ERROR;

@@ -45,7 +45,7 @@ class SolverOptions:  # bal/solver_options.hpp (QR-relevant subset, reference de
     eta: float = 0.1
     residual_reset_period: int = 10              # ConjugateGradientsSolver::Options (cg/conjugate_gradient.hpp:87): r = b - H x every this many iterations
     jacobi_scaling_epsilon: float = 0.0
-    preconditioner_type: str = "SCHUR_JACOBI"     # JACOBI | SCHUR_JACOBI
+    preconditioner_type: str = "SCHUR_JACOBI"     # JACOBI | SCHUR_JACOBI | CLUSTER_JACOBI (:73-75; DESIGN.md section 28)
     function_tolerance: float = 1e-6
     use_double: bool = True
     use_householder_marginalization: bool = True
@@ -536,7 +536,7 @@ class LinearizorQR:
         o.robust_norm = {"NONE": 0, "HUBER": 1}[options.residual.robust_norm]
         o.huber_parameter = options.residual.huber_parameter
         o.jacobi_scaling_epsilon = options.jacobi_scaling_epsilon
-        o.preconditioner_type = {"JACOBI": 0, "SCHUR_JACOBI": 1}[options.preconditioner_type]
+        o.preconditioner_type = {"JACOBI": 0, "SCHUR_JACOBI": 1, "CLUSTER_JACOBI": 2}[options.preconditioner_type]
         o.min_linear_solver_iterations = options.min_linear_solver_iterations
         o.max_linear_solver_iterations = options.max_linear_solver_iterations
         o.eta = options.eta
@@ -911,6 +911,31 @@ class LinearizorQR:
         check(_lib.lib().rba_get_rhs(self.h, _p(b)))
         return b
 
+    def set_camera_clusters(self, cluster_of_camera):
+        """CLUSTER_JACOBI: the clusters of the preconditioner (rba_set_camera_clusters) from the next solve on: None (the
+        default clustering), or one int32 cluster id per camera (dense ids, at most RBA_CLUSTER_MAX_CAMERAS per cluster)."""
+        c = None if cluster_of_camera is None else np.ascontiguousarray(cluster_of_camera, dtype=np.int32)
+        if c is not None and c.shape != (self.nc,):
+            raise ValueError(f"cluster_of_camera must have shape ({self.nc},), not {c.shape}")
+        check(_lib.lib().rba_set_camera_clusters(self.h, None if c is None else _p(c)))
+
+    def cluster_preconditioner(self):
+        """CLUSTER_JACOBI read-back (rba_get_cluster_preconditioner): (cluster_of_camera [nc], blocks, status [ncl]); blocks
+        is a list of the last solve's unfactorised (9k, 9k) float64 cluster blocks in cluster order, cameras ascending."""
+        L = _lib.lib()
+        c = np.empty(self.nc, np.int32)
+        check(L.rba_get_cluster_preconditioner(self.h, _p(c), None, None))
+        sizes = np.bincount(c)
+        flat = np.empty(int(np.sum((9 * sizes) ** 2)), np.float64)
+        status = np.empty(len(sizes), np.int32)
+        check(L.rba_get_cluster_preconditioner(self.h, None, _p(flat), _p(status)))
+        blocks, off = [], 0
+        for k in sizes:
+            m = 9 * int(k)
+            blocks.append(flat[off:off + m * m].reshape(m, m))
+            off += m * m
+        return c, blocks, status
+
     def get_preconditioner(self):
         inv, blk = np.empty(81 * self.nc, self.dtype), np.empty(81 * self.nc, self.dtype)
         check(_lib.lib().rba_get_preconditioner(self.h, _p(inv), _p(blk)))
@@ -995,6 +1020,16 @@ def nccl_unique_id() -> bytes:
     buf = C.create_string_buffer(128)
     check(_lib.lib().rba_nccl_unique_id(buf))
     return buf.raw
+
+
+def cluster_cameras(bal_problem: BalProblem, max_size: int) -> np.ndarray:
+    """rba_cluster_cameras: the cameras clustered by single linkage over the co-visibility graph (edge weight = shared
+    landmarks), at most max_size cameras per cluster; dense int32 ids numbered by their smallest camera.  Host code only."""
+    out = np.empty(bal_problem.num_cameras(), np.int32)
+    pv = ProblemView(bal_problem.num_cameras(), bal_problem.num_landmarks(), bal_problem.num_observations(),
+                     bal_problem.lm_off.ctypes.data, bal_problem.obs_cam.ctypes.data, bal_problem.obs_xy.ctypes.data)
+    check(_lib.lib().rba_cluster_cameras(C.byref(pv), C.c_int32(max_size), _p(out)))
+    return out
 
 
 def partition_landmarks(lm_off: np.ndarray, nranks: int) -> np.ndarray:
